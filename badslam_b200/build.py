@@ -1,8 +1,8 @@
-"""Builds libbadba_b200.so (the product's CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libbadba_b200.so (the product's CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m badslam_b200.build [--force]
 
-The shared object is git-ignored but travels to the GPU box with the repo snapshot.
+The shared object and the objects under _obj/ are build products and are git-ignored.
 """
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libbadba_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "--expt-relaxed-constexpr"]
 # (source, extra flags).  kernels.cu is built with -use_fast_math like the reference
 # (applications/badslam/CMakeLists.txt:74-75); the fp64 pose solve and the host code are not.

@@ -1,7 +1,7 @@
 // badba.cu -- C ABI (include/badba.h) and host orchestration of libbadba_b200.
 //
 // Host-side structure mirrors the reference's DirectBA (direct_ba.{h,cc}, direct_ba_alternating.cc) but the
-// schedule is B200-first: per outer BA iteration the device runs
+// schedule is GPU-first: per outer BA iteration the device runs
 //     1 launch   activation + normals      (reference: 1 + K_active + 1 + K + 1 launches)
 //     1 launch   position + descriptors    (reference: 1 + K + 1 launches)
 //     <=30 x 2   pose accumulate + solve for ALL keyframes at once (reference: K x n_GN x {2 clears, kernel,
@@ -155,7 +155,7 @@ struct bba_context {
   float depth_K[4], color_K[4];
   float depth_a = 0.f;
   int cf_w = 0, cf_h = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   std::string error;
 
   float* surfels = nullptr;

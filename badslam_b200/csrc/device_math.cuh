@@ -1,4 +1,4 @@
-// device_math.cuh -- device-side surfel/keyframe maths of libbadba_b200 (sm_100a).
+// device_math.cuh -- device-side surfel/keyframe maths of libbadba_b200 (sm_90a).
 //
 // What is computed follows the reference's device headers (cited per function, paths relative to
 // /root/reference/applications/badslam/src/badslam/); how it is computed is our own: keyframe
@@ -72,43 +72,6 @@ __device__ __forceinline__ Vec3 Rotate(const float* __restrict__ T, const Vec3& 
 __device__ __forceinline__ Vec3 Transform(const float* __restrict__ T, const Vec3& p) {   // cuda_matrix.cuh:104-112
   return V3(T[0] * p.x + T[1] * p.y + T[2] * p.z + T[3], T[4] * p.x + T[5] * p.y + T[6] * p.z + T[7],
             T[8] * p.x + T[9] * p.y + T[10] * p.z + T[11]);
-}
-
-// ---- packed fp32x2 arithmetic (sm_100: FADD2 / FMUL2 / FFMA2) -----------------------------------------------------------------
-// A pair of floats in an aligned 64-bit register.  Every operation rounds each half exactly like the scalar instruction
-// (IEEE rn, flush-to-zero like the -use_fast_math scalar code); one issue slot does the work of two.  Splat() operands become
-// the instructions' scalar-broadcast form (Ra.F32), so a scalar x pair product costs no extra move.
-struct F2 {
-  unsigned long long v;
-};
-__device__ __forceinline__ F2 Pack(float lo, float hi) {
-  F2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ F2 Splat(float s) { return Pack(s, s); }
-__device__ __forceinline__ void Unpack(F2 a, float* lo, float* hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(*lo), "=f"(*hi) : "l"(a.v)); }
-__device__ __forceinline__ float Lo(F2 a) { float lo, hi; Unpack(a, &lo, &hi); return lo; }
-__device__ __forceinline__ float Hi(F2 a) { float lo, hi; Unpack(a, &lo, &hi); return hi; }
-__device__ __forceinline__ F2 operator+(F2 a, F2 b) {
-  F2 r;
-  asm("add.rn.ftz.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ F2 operator-(F2 a, F2 b) {
-  F2 r;
-  asm("sub.rn.ftz.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ F2 operator*(F2 a, F2 b) {
-  F2 r;
-  asm("mul.rn.ftz.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ F2 Fma(F2 a, F2 b, F2 c) {   // a * b + c, fused
-  F2 r;
-  asm("fma.rn.ftz.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-  return r;
 }
 
 // Sums acc[i] over the 32 lanes of the warp for all 32 i at once: after the call lane L holds the total of
@@ -391,105 +354,6 @@ __device__ __forceinline__ void DescPoseJacobian(const CameraParams& cam, const 
   J[3] = ((ls.y * ls.y + z_sq) * gy + xy * gx) * inv_z_sq;
   J[4] = -((ls.x * ls.x + z_sq) * gx + xy * gy) * inv_z_sq;
   J[5] = -(ls.x * gy - ls.y * gx) * inv_z;
-}
-
-// ---- packed (fp32x2) forms of the post-association maths -------------------------------------------------------------------
-// The association itself (ProjectIntoImage / Associate above) stays scalar and textually identical to the reference, so that
-// which pairs associate does not depend on how the compiler pairs instructions.  Everything after it -- tangent-point
-// projection, sample coordinates, residuals, Jacobians, the rank-1 updates -- is 2-wide: the (x, y) components of an image
-// point, columns (c, c+1) of a Jacobian row, or the two descriptor residuals of a pair.
-
-// frame_T_global with the first two rows interleaved: c_k = (T[k], T[4 + k]), so that (x, y) of Transform(T, q) is three FFMA2.
-struct KfPairs {
-  F2 c0, c1, c2, c3;
-};
-__device__ __forceinline__ KfPairs MakeKfPairs(const float* __restrict__ T) {
-  KfPairs P;
-  P.c0 = Pack(T[0], T[4]);
-  P.c1 = Pack(T[1], T[5]);
-  P.c2 = Pack(T[2], T[6]);
-  P.c3 = Pack(T[3], T[7]);
-  return P;
-}
-__device__ __forceinline__ F2 TransformXY(const KfPairs& P, const Vec3& q) {   // cuda_matrix.cuh:104-112, rows 0 and 1
-  return Fma(P.c0, Splat(q.x), Fma(P.c1, Splat(q.y), Fma(P.c2, Splat(q.z), P.c3)));
-}
-
-// cost_function.cuh:115-136 -> the two tangent points' pixel positions (x, y) in the colour image
-__device__ __forceinline__ void TangentProjections2(const CameraParams& cam, const KfPairs& P, const float* __restrict__ T,
-                                                    const Vec3& gp, const Vec3& n, float radius_sq, F2* t1_pxy, F2* t2_pxy) {
-  Vec3 t1 = Cross(n, (fabsf(n.x) > 0.9f) ? V3(0, 1, 0) : V3(1, 0, 0));
-  t1 = (kTangentScaling * sqrtf(radius_sq / fmaxf(1e-12f, Dot(t1, t1)))) * t1;
-  Vec3 t2 = Cross(n, t1);
-  t2 = (kTangentScaling * sqrtf(radius_sq / fmaxf(1e-12f, Dot(t2, t2)))) * t2;
-  const Vec3 q1 = gp + t1, q2 = gp + t2;
-  const float z1 = T[8] * q1.x + T[9] * q1.y + T[10] * q1.z + T[11];
-  const float z2 = T[8] * q2.x + T[9] * q2.y + T[10] * q2.z + T[11];
-  const F2 cf = Pack(cam.cfx, cam.cfy), cc = Pack(cam.ccx, cam.ccy);
-  *t1_pxy = Fma(cf, TransformXY(P, q1) * Splat(1.0f / z1), cc);
-  *t2_pxy = Fma(cf, TransformXY(P, q2) * Splat(1.0f / z2), cc);
-}
-
-// SamplePoint for an (x, y) pair: the coordinate arithmetic is packed, the gradient uses the gather's (x, y, z, w) quad as is.
-__device__ __forceinline__ void SamplePoint2(cudaTextureObject_t tex, F2 xy, float* intensity, float* dx, float* dy) {
-  float mx, my;
-  Unpack(xy - Splat(0.5f), &mx, &my);
-  mx = fmaxf(0.f, mx);
-  my = fmaxf(0.f, my);
-  const float fx = floorf(mx), fy = floorf(my);
-  const F2 f = Pack(fx, fy);
-  float tx, ty, gx, gy, x, y;
-  Unpack(Pack(mx, my) - f, &tx, &ty);
-  Unpack(f + Splat(1.0f), &gx, &gy);
-  Unpack(xy, &x, &y);
-  const float4 g = tex2Dgather<float4>(tex, gx, gy, 0);
-  *intensity = tex2D<float>(tex, x, y);
-  *dx = (g.y - g.x) * ty + (g.z - g.w) * (1 - ty);
-  *dy = (g.y - g.z) * tx + (g.x - g.w) * (1 - tx);
-}
-
-struct DescEval2 {
-  F2 r;        // (r1, r2) raw residuals (cost_function.cuh:140-156)
-  F2 g1, g2;   // (d r_i / d px, d r_i / d py) (cost_function.cuh:250-253)
-};
-__device__ __forceinline__ void EvalDescriptor2(cudaTextureObject_t tex, F2 c_pxy, F2 t1_pxy, F2 t2_pxy, float d1, float d2, DescEval2* e) {
-  float intensity, t1i, t2i, cdx, cdy, t1dx, t1dy, t2dx, t2dy;
-  SamplePoint2(tex, c_pxy, &intensity, &cdx, &cdy);
-  SamplePoint2(tex, t1_pxy, &t1i, &t1dx, &t1dy);
-  SamplePoint2(tex, t2_pxy, &t2i, &t2dx, &t2dy);
-  const F2 k = Splat(180.f);
-  e->r = k * (Pack(t1i, t2i) - Splat(intensity)) - Pack(d1, d2);
-  const F2 cd = Pack(cdx, cdy);
-  e->g1 = k * (Pack(t1dx, t1dy) - cd);
-  e->g2 = k * (Pack(t2dx, t2dy) - cd);
-}
-
-// kernel_opt_pose.cu:96-142 for both descriptor residuals of a pair: everything that depends on the surfel position only is
-// built once; each residual's six Jacobian entries then cost 1 + 3 + 3 packed instructions.
-struct DescJacShared {
-  F2 x_xy, y_a, nb_y, nxy_nx, iz2_iz;
-  float neg_iz, iz2;
-};
-__device__ __forceinline__ DescJacShared MakeDescJacShared(const Vec3& ls) {
-  DescJacShared s;
-  const float iz = 1.f / ls.z, z_sq = ls.z * ls.z, xy = ls.x * ls.y;
-  s.iz2 = iz * iz;
-  s.neg_iz = -iz;
-  s.x_xy = Pack(ls.x, xy);
-  s.y_a = Pack(ls.y, ls.y * ls.y + z_sq);
-  s.nb_y = Pack(-(ls.x * ls.x + z_sq), ls.y);
-  s.nxy_nx = Pack(-xy, -ls.x);
-  s.iz2_iz = Pack(s.iz2, iz);
-  return s;
-}
-// g = (gx, gy) of one residual -> (J0, J1), (J2, J3), (J4, J5)
-__device__ __forceinline__ void DescPoseJacobian2(const CameraParams& cam, const DescJacShared& s, F2 g, F2* J01, F2* J23, F2* J45) {
-  g = g * Pack(cam.cfx, cam.cfy);
-  float gx, gy;
-  Unpack(g, &gx, &gy);
-  *J01 = g * Splat(s.neg_iz);
-  *J23 = Fma(Splat(gx), s.x_xy, Splat(gy) * s.y_a) * Splat(s.iz2);
-  *J45 = Fma(Splat(gy), s.nxy_nx, Splat(gx) * s.nb_y) * s.iz2_iz;
 }
 
 }  // namespace bba

@@ -1,4 +1,4 @@
-// kernels.cu -- hand-written sm_100a kernels of the direct-BA hot path.
+// kernels.cu -- hand-written sm_90a kernels of the direct-BA hot path.
 //
 //  * PoseAccumulateKernel: ONE persistent launch evaluates the pose normal equations of a whole LIST of
 //    keyframes (the reference launches AccumulatePoseEstimationCoeffsCUDAKernel once per keyframe and
@@ -112,11 +112,6 @@ __device__ __forceinline__ void LoadKf(const KfDevice* __restrict__ kfs, int kf,
   r->activation = __ldg(reinterpret_cast<const int*>(p + 5));
 }
 
-#ifndef BBA_POSE_FFMA2
-#define BBA_POSE_FFMA2 1   // packed fp32x2 arithmetic (sm_100 FFMA2 / FMUL2) for the rank-1 updates of H and b
-#endif
-
-#if !BBA_POSE_FFMA2
 // H += w J^T J (upper triangle, row-major), b += w r J   (gauss_newton.cuh:59-92, per thread)
 __device__ __forceinline__ void AccumulateHb(float (&acc)[kPoseAccSize], const float (&J)[6], float raw, float w) {
   int idx = 0;
@@ -131,80 +126,6 @@ __device__ __forceinline__ void AccumulateHb(float (&acc)[kPoseAccSize], const f
   for (int i = 0; i < 6; ++i) acc[21 + i] += wr * J[i];
 }
 __device__ __forceinline__ int AccSlot(int lane) { return lane; }
-#else
-// The same update with packed fp32x2 instructions (fma.rn.f32x2 / mul.rn.f32x2 -> SASS FFMA2 / FMUL2): each instruction
-// updates two adjacent coefficients.  The per-lane accumulators are kept in a PAIR-ALIGNED order --
-//   0..5  H00 H01 H02 H03 H04 H05 | 6..9 H12 H13 H14 H15 | 10..13 H22 H23 H24 H25 | 14,15 H34 H35 | 16,17 H44 H45 |
-//   18..23 b0..b5 | 24 H11  25 H33  26 H55 | 27..31 statistics
-// -- so that every row of the upper triangle is a run of (even, odd) column pairs of J plus at most one leading diagonal
-// element; AccSlot() maps the order back to the row-major upper triangle + b the solver reads (gauss_newton.cuh:59-92).
-// 12 FFMA2 + 3 FMUL2 + 3 FFMA + 1 FMUL per residual instead of 27 FFMA + 7 FMUL; each product / sum is rounded exactly as in the
-// scalar form.
-typedef unsigned long long F32x2;
-__device__ __forceinline__ F32x2 Pack2(float lo, float hi) {
-  F32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void Unpack2(F32x2 v, float* lo, float* hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(*lo), "=f"(*hi) : "l"(v)); }
-__device__ __forceinline__ F32x2 Mul2(F32x2 a, F32x2 b) {
-  F32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ void Fma2(float* lo, float* hi, F32x2 a, F32x2 b) {   // (*lo, *hi) += a * b
-  F32x2 c = Pack2(*lo, *hi);
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(c) : "l"(a), "l"(b));
-  Unpack2(c, lo, hi);
-}
-__device__ __forceinline__ void AccumulateHbPacked(float (&acc)[kPoseAccSize], F32x2 J01, F32x2 J23, F32x2 J45, float raw, float w);
-__device__ __forceinline__ void AccumulateHb(float (&acc)[kPoseAccSize], const float (&J)[6], float raw, float w) {
-  AccumulateHbPacked(acc, Pack2(J[0], J[1]), Pack2(J[2], J[3]), Pack2(J[4], J[5]), raw, w);
-}
-__device__ __forceinline__ void AccumulateHbPacked(float (&acc)[kPoseAccSize], F32x2 J01, F32x2 J23, F32x2 J45, float raw, float w) {
-  float J[6];
-  Unpack2(J01, &J[0], &J[1]);
-  Unpack2(J23, &J[2], &J[3]);
-  Unpack2(J45, &J[4], &J[5]);
-  const F32x2 ww = Pack2(w, w);
-  float wj[6];
-  Unpack2(Mul2(ww, J01), &wj[0], &wj[1]);
-  Unpack2(Mul2(ww, J23), &wj[2], &wj[3]);
-  Unpack2(Mul2(ww, J45), &wj[4], &wj[5]);
-  const F32x2 d0 = Pack2(wj[0], wj[0]), d1 = Pack2(wj[1], wj[1]), d2 = Pack2(wj[2], wj[2]), d3 = Pack2(wj[3], wj[3]),
-              d4 = Pack2(wj[4], wj[4]);
-  Fma2(&acc[0], &acc[1], d0, J01);
-  Fma2(&acc[2], &acc[3], d0, J23);
-  Fma2(&acc[4], &acc[5], d0, J45);
-  acc[24] += wj[1] * J[1];
-  Fma2(&acc[6], &acc[7], d1, J23);
-  Fma2(&acc[8], &acc[9], d1, J45);
-  Fma2(&acc[10], &acc[11], d2, J23);
-  Fma2(&acc[12], &acc[13], d2, J45);
-  acc[25] += wj[3] * J[3];
-  Fma2(&acc[14], &acc[15], d3, J45);
-  Fma2(&acc[16], &acc[17], d4, J45);
-  acc[26] += wj[5] * J[5];
-  const float wr = w * raw;
-  const F32x2 dr = Pack2(wr, wr);
-  Fma2(&acc[18], &acc[19], dr, J01);
-  Fma2(&acc[20], &acc[21], dr, J23);
-  Fma2(&acc[22], &acc[23], dr, J45);
-}
-// accumulator index in the pair-aligned order -> index in the solver's order (21 upper-triangle coefficients row-major, 6 b, 5 stats)
-__device__ __forceinline__ int AccSlot(int lane) {
-  //            H00 H01 H02 H03 H04 H05 H12 H13 H14 H15 H22 H23 H24 H25 H34 H35 H44 H45 b0  b1  b2  b3  b4  b5 H11 H33 H55
-  constexpr unsigned long long lo = 0x0ull | (1ull << 5) | (2ull << 10) | (3ull << 15) | (4ull << 20) | (5ull << 25) | (7ull << 30) |
-                                    (8ull << 35) | (9ull << 40) | (10ull << 45) | (11ull << 50) | (12ull << 55);   // slots 0..11
-  constexpr unsigned long long mid = 13ull | (14ull << 5) | (16ull << 10) | (17ull << 15) | (18ull << 20) | (19ull << 25) | (21ull << 30) |
-                                     (22ull << 35) | (23ull << 40) | (24ull << 45) | (25ull << 50) | (26ull << 55);   // slots 12..23
-  constexpr unsigned long long hi = 6ull | (15ull << 5) | (20ull << 10);                                               // slots 24..26
-  if (lane < 12) return static_cast<int>((lo >> (5 * lane)) & 31u);
-  if (lane < 24) return static_cast<int>((mid >> (5 * (lane - 12))) & 31u);
-  if (lane < 27) return static_cast<int>((hi >> (5 * (lane - 24))) & 31u);
-  return lane;
-}
-#endif
 
 #ifndef BBA_POSE_UNROLL
 #define BBA_POSE_UNROLL 1
@@ -212,26 +133,13 @@ __device__ __forceinline__ int AccSlot(int lane) {
 #ifndef BBA_POSE_MIN_CTAS
 #define BBA_POSE_MIN_CTAS 2   // resident CTAs per SM the register allocation is tuned for
 #endif
-// 2-wide (fp32x2) post-association maths (device_math.cuh: tangent points, sample coordinates, Jacobians).  OFF: measured on
-// B200 it does not shorten the kernel (3.7145 vs 3.7148 ms per launch: the kernel is bound by dependent-issue latency at 4 warps
-// per scheduler, not by the instruction count), and it rounds the texture sample coordinates differently from the reference's
-// compiled expressions -- the texture unit quantises the filter fraction to 1/256 pixel, so a last-bit change of a coordinate
-// flips the filter weights of ~1 % of the samples (residual changes of up to ~0.5 of +-180).  In the geometry kernel that cost
-// the bit-exact agreement of the surfel positions with the reference (errors up to 9e-5 m on 0.07 % of the surfels).
-#ifndef BBA_POSE_PACKED
-#define BBA_POSE_PACKED 0
-#endif
-#ifndef BBA_GEO_PACKED
-#define BBA_GEO_PACKED 0
-#endif
 #ifndef BBA_POSE_CHUNK_SHIFT
 #define BBA_POSE_CHUNK_SHIFT 8
 #endif
 constexpr int kPoseChunkShift = BBA_POSE_CHUNK_SHIFT;   // log2 of the surfels one warp evaluates per (keyframe) sub-item
 // Sub-item size chosen per ITEM from the number of keyframes in its group (so that the last, short group of a work list and the
-// tail of a Gauss-Newton loop still offer every warp a sub-item) instead of per launch.  OFF: measured on B200 at cfg3 it is
-// 0.5 % slower (pose stage 20.26 vs 20.15 ms; the extra warp reductions of the smaller chunks cost more than the idle warps of
-// the few short groups), tools/r2_gpu14.sh.
+// tail of a Gauss-Newton loop still offer every warp a sub-item) instead of per launch.  OFF: the extra warp reductions of the
+// smaller chunks cost more than the idle warps of the few short groups save (not measured on the H100).
 #ifndef BBA_POSE_ITEM_CHUNKS
 #define BBA_POSE_ITEM_CHUNKS 0
 #endif
@@ -249,7 +157,7 @@ constexpr int kPoseGroup = 8;        // keyframes per work item
 
 // Work decomposition.  A work ITEM is (group of <= 8 keyframes from the work list) x (tile of TILE surfels); items are
 // handed out through a global counter in GROUP-MAJOR order, so at any moment all resident CTAs read the images of the
-// same 8-16 keyframes (~12-24 MB: stays in the 126 MB L2) while surfel tiles stream through shared memory via TMA.
+// same 8-16 keyframes (~12-24 MB: stays in the H100's 50 MB L2) while surfel tiles stream through shared memory via TMA.
 // Inside an item the 8 warps steal SUB-ITEMS (keyframe, 256- or 128-surfel chunk) from a shared-memory counter, which
 // evens out the very different cost of culled vs. associated chunks.
 // STATS: also produce the residual costs and the stage counters of the byte model (the reference computes its
@@ -399,9 +307,6 @@ __global__ void __launch_bounds__(kPoseThreads, BBA_POSE_MIN_CTAS) PoseAccumulat
       const int kf = LoadKfShared(&s_kf[s][kf_local], &K);
       K.tex = UniformTexture(K.tex);
 
-#if BBA_POSE_PACKED
-      const KfPairs KP = MakeKfPairs(K.T);
-#endif
       float acc[kPoseAccSize];
 #pragma unroll
       for (int i = 0; i < kPoseAccSize; ++i) acc[i] = 0.f;
@@ -413,11 +318,7 @@ __global__ void __launch_bounds__(kPoseThreads, BBA_POSE_MIN_CTAS) PoseAccumulat
         int st = 0;
         Assoc r;
         Vec3 gp, nrm;
-#if BBA_POSE_PACKED
-        DescEval2 e2;
-#else
         DescEval e;
-#endif
         bool photo = false;
         if (j < j1) {
           gp = V3(sx[j], sy[j], sz[j]);
@@ -428,15 +329,6 @@ __global__ void __launch_bounds__(kPoseThreads, BBA_POSE_MIN_CTAS) PoseAccumulat
             const PixelLoads l = LoadPixel(cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r);
             nrm = PRE ? V3(sf[j], sf[TILE + j], sf[2 * TILE + j]) : UnpackNormal(__float_as_uint(sn[j]));
             if (cam.use_desc) {
-#if BBA_POSE_PACKED
-              const F2 c_pxy = Fma(Pack(cam.d2c_fx, cam.d2c_fy), Pack(r.pxf, r.pyf), Pack(cam.d2c_cx, cam.d2c_cy));   // DepthToColor
-              float ccx, ccy;
-              Unpack(c_pxy, &ccx, &ccy);
-              photo = ccx >= 0 && ccy >= 0 && static_cast<int>(ccx) < cam.cw && static_cast<int>(ccy) < cam.ch;
-              F2 t1, t2;
-              TangentProjections2(cam, KP, K.T, gp, nrm, sr[j], &t1, &t2);
-              EvalDescriptor2(K.tex, c_pxy, t1, t2, sd1[j], sd2[j], &e2);
-#else
               float ccx, ccy;
               photo = DepthToColor(cam, r.pxf, r.pyf, &ccx, &ccy);
               float t1x, t1y, t2x, t2y;
@@ -447,7 +339,6 @@ __global__ void __launch_bounds__(kPoseThreads, BBA_POSE_MIN_CTAS) PoseAccumulat
                 TangentProjections(cam, K.T, gp, nrm, sr[j], &t1x, &t1y, &t2x, &t2y);
               }
               EvalDescriptor(K.tex, ccx, ccy, t1x, t1y, t2x, t2y, sd1[j], sd2[j], &e);
-#endif
             }
             st = Associate(cam, K.T, nrm, l, &r);
           }
@@ -467,13 +358,6 @@ __global__ void __launch_bounds__(kPoseThreads, BBA_POSE_MIN_CTAS) PoseAccumulat
             Vec3 up;
             const float raw = DepthResidual(cam, r, &inv_stddev, &up);
             // kernel_opt_pose.cu:88-93
-#if BBA_POSE_PACKED
-            const F2 inv2 = Splat(inv_stddev);
-            const F2 J01 = inv2 * Pack(r.ln.x, r.ln.y);
-            const F2 J23 = inv2 * Pack(r.ln.z, -r.ln.y * up.z + r.ln.z * up.y);
-            const F2 J45 = inv2 * Pack(r.ln.x * up.z - r.ln.z * up.x, -r.ln.x * up.y + r.ln.y * up.x);
-            AccumulateHbPacked(acc, J01.v, J23.v, J45.v, raw, DepthWeight(raw));
-#else
             float J[6];
             J[0] = inv_stddev * r.ln.x;
             J[1] = inv_stddev * r.ln.y;
@@ -482,25 +366,10 @@ __global__ void __launch_bounds__(kPoseThreads, BBA_POSE_MIN_CTAS) PoseAccumulat
             J[4] = inv_stddev * (r.ln.x * up.z - r.ln.z * up.x);
             J[5] = inv_stddev * (-r.ln.x * up.y + r.ln.y * up.x);
             AccumulateHb(acc, J, raw, DepthWeight(raw));
-#endif
             if (STATS) acc[29] += DepthCost(raw);
           }
           if (cam.use_desc && photo) {
             acc[28] += 1.f;
-#if BBA_POSE_PACKED
-            const DescJacShared js = MakeDescJacShared(r.lp);
-            float r1, r2;
-            Unpack(e2.r, &r1, &r2);
-            F2 J01, J23, J45;
-            DescPoseJacobian2(cam, js, e2.g1, &J01, &J23, &J45);
-            AccumulateHbPacked(acc, J01.v, J23.v, J45.v, r1, DescWeight(r1));
-            DescPoseJacobian2(cam, js, e2.g2, &J01, &J23, &J45);
-            AccumulateHbPacked(acc, J01.v, J23.v, J45.v, r2, DescWeight(r2));
-            if (STATS) {
-              acc[30] += DescCost(r1);
-              acc[31] += DescCost(r2);
-            }
-#else
             float J[6];
             DescPoseJacobian(cam, r.lp, e.gx1, e.gy1, J);
             AccumulateHb(acc, J, e.r1, DescWeight(e.r1));
@@ -510,7 +379,6 @@ __global__ void __launch_bounds__(kPoseThreads, BBA_POSE_MIN_CTAS) PoseAccumulat
               acc[30] += DescCost(e.r1);
               acc[31] += DescCost(e.r2);
             }
-#endif
           }
         }
       }
@@ -616,7 +484,7 @@ void LaunchSurfelFrames(const float* surfels, uint32_t pitch, uint32_t n, float*
 // Geometry step.  One thread owns one surfel and keeps its accumulators in registers while it walks over a GROUP of
 // keyframes; work items (keyframe group, 256-surfel tile) are handed out group-major through a global counter so that
 // all resident CTAs gather from the same <= 16 keyframes' images at a time (L2-resident) -- the surfel-major variant
-// that looped over all K keyframes per thread re-read the images from HBM ~40 times (profiles/r1_notes.md).
+// that looped over all K keyframes per thread re-read the images from HBM ~40 times.
 // Between groups the partial sums of a surfel are parked in the scratch rows 8..16 of the surfel buffer (the rows the
 // reference uses for exactly this purpose, kernels.cuh:78-86); a per-tile epoch word orders (group g, tile t) after
 // (group g-1, tile t).  With K <= 16 there is a single group and no scratch traffic at all.
@@ -703,9 +571,8 @@ __device__ __forceinline__ void StageGroupRecords(const KfDevice* __restrict__ k
 }
 
 // The records of ALL keyframes of the launch, copied once per CTA (persistent grid) when they fit the shared-memory budget,
-// instead of a coalesced copy + an L2 round trip per (group, tile) item.  OFF: measured on B200 (tools/r2_gpu14.sh) it does not
-// pay -- position + descriptor 4.76 vs 4.58 ms at cfg3 and 0.81 vs 0.77 ms on one rank's share of an 8-GPU job (cfg3_rank8),
-// activation + normals unchanged: the per-warp slices keep the records a warp reads next to each other, the 19 KB block does not.
+// instead of a coalesced copy + an L2 round trip per (group, tile) item.  OFF: it did not pay where it was measured (not on the
+// H100): the per-warp slices keep the records a warp reads next to each other, the 19 KB block does not.
 // With it on, GeometryArgs::group (keyframes per work item, BADBA_GEO_GROUP) becomes a runtime choice: 32 / 64 / 200 instead of
 // 16 moved the two kernels by -10 % / +2 % ... +0 % / +38 % at cfg3_rank8, i.e. no setting beats 16 for both.
 #ifndef BBA_GEO_STAGE_ALL
@@ -904,25 +771,11 @@ __global__ void __launch_bounds__(kGeoThreads, 3) PositionDescriptorKernel(const
         DescEval e;
         bool photo = false;
         if (USE_DESC) {
-#if BBA_GEO_PACKED
-          const F2 c_pxy = Fma(Pack(a.cam.d2c_fx, a.cam.d2c_fy), Pack(r.pxf, r.pyf), Pack(a.cam.d2c_cx, a.cam.d2c_cy));   // DepthToColor
-          float ccx, ccy;
-          Unpack(c_pxy, &ccx, &ccy);
-          photo = ccx >= 0 && ccy >= 0 && static_cast<int>(ccx) < a.cam.cw && static_cast<int>(ccy) < a.cam.ch;
-          F2 t1, t2;
-          TangentProjections2(a.cam, MakeKfPairs(K.T), K.T, gp, nrm, radius_sq, &t1, &t2);
-          DescEval2 e2;
-          EvalDescriptor2(K.tex, c_pxy, t1, t2, d1, d2, &e2);
-          Unpack(e2.r, &e.r1, &e.r2);
-          Unpack(e2.g1, &e.gx1, &e.gy1);
-          Unpack(e2.g2, &e.gx2, &e.gy2);
-#else
           float ccx, ccy;
           photo = DepthToColor(a.cam, r.pxf, r.pyf, &ccx, &ccy);
           float t1x, t1y, t2x, t2y;
           TangentProjections(a.cam, K.T, gp, nrm, radius_sq, &t1x, &t1y, &t2x, &t2y);
           EvalDescriptor(K.tex, ccx, ccy, t1x, t1y, t2x, t2y, d1, d2, &e);
-#endif
         }
         if (Associate(a.cam, K.T, nrm, l, &r) != 3) continue;
         if (USE_DEPTH) {

@@ -1,4 +1,4 @@
-// kernels.cuh -- launch interface between the host orchestration (badba.cu) and the sm_100a kernels.
+// kernels.cuh -- launch interface between the host orchestration (badba.cu) and the sm_90a kernels.
 #pragma once
 
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// odometry.cu -- image-pair odometry (frame-to-keyframe direct tracking) for sm_100a, SURVEY.md 8(f4).
+// odometry.cu -- image-pair odometry (frame-to-keyframe direct tracking) for sm_90a, SURVEY.md 8(f4).
 //
 // What is computed follows the reference (BadSlam::RunOdometry bad_slam.cc:829-950, TrackFramePairwise
 // pairwise_frame_tracking.cc:153-678, kernel_downsample.cu, cuda_image_processing.cu:103-206, kernel_opt_pose.cu:422-1340);

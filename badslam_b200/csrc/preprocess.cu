@@ -1,7 +1,7 @@
 // Fused keyframe preprocessing kernel (one launch per frame; the tile program lives in preprocess_tile.cuh).
 //
 // Grid: one CTA of 256 threads per 32x32 depth tile (300 CTAs at 640x480), followed by one CTA per 1024 colour pixels (300
-// more): a single wave on 148 SMs (39 registers, 8.4 KB of shared memory per CTA).  Algorithmic bytes per frame: 2 (raw
+// more): a single wave on the H100's 132 SMs (39 registers, 8.4 KB of shared memory per CTA: up to 8 resident CTAs per SM).  Algorithmic bytes per frame: 2 (raw
 // depth) + 3 (rgb) read, 2 + 2 + 2 (depth, normals, radius) + 4 (rgba) written per pixel = 15 B/pixel, 4.6 MB at 640x480 --
 // well under a microsecond of HBM time, so the kernel
 // is bound by launch latency and by the ~30 exp / rcp per pixel of the bilateral filter; what the fusion buys is one launch

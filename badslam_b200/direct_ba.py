@@ -148,7 +148,7 @@ class MotionModel:
 
 
 class DirectBA:
-    """Drop-in for vis::DirectBA (direct_ba.h:65-550) backed by the sm_100a library."""
+    """Drop-in for vis::DirectBA (direct_ba.h:65-550) backed by the sm_90a library."""
 
     def __init__(self, max_surfel_count: int, raw_to_float_depth: float, baseline_fx: float,
                  sparse_surfel_cell_size: int, surfel_merge_dist_factor: float = 0.8,

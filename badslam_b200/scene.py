@@ -228,7 +228,7 @@ def raw_to_calibrated_depth(a, cfactor, raw_to_float, raw):
 
 def tex_luma(luma_u8, x, y, weight_mode=3):
     """tex2D(..).w of a clamp / linear-filter / normalized-float u8 texture (keyframe.cc:67-73).
-    weight_mode 3 (default) reproduces the B200 texture unit bit-exactly, 1 rounds the two fractions to 1/256 and
+    weight_mode 3 (default) reproduces the hardware texture unit bit-exactly, 1 rounds the two fractions to 1/256 and
     interpolates in float, 0 uses exact float weights."""
     h, w = luma_u8.shape
     xb = np.asarray(x, dtype=np.float32) - np.float32(0.5)
@@ -236,7 +236,7 @@ def tex_luma(luma_u8, x, y, weight_mode=3):
     fi, fj = np.floor(xb), np.floor(yb)
     al, be = xb - fi, yb - fj
     if weight_mode == 3:
-        # The filter of the B200 texture unit as measured (tools/tex_probe*.cu, bit-exact): 1.8 fixed-point fractions,
+        # The filter of the hardware texture unit as measured (tools/tex_probe*.cu, bit-exact): 1.8 fixed-point fractions,
         # w11 = round(a*b/256), w10 = a - w11, w01 = b - w11, w00 = 256 - rest, unorm16 texels, one final rounding.
         a = np.floor(al * 256 + np.float32(0.5)).astype(np.int64)
         b = np.floor(be * 256 + np.float32(0.5)).astype(np.int64)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- throughput of one outer bundle-adjustment iteration of the direct-BA hot path.
 
-    python bench.py --gpus 1 --steps K --warmup W            # our sm_100a backend
+    python bench.py --gpus 1 --steps K --warmup W [--dump-outputs DIR]
     python bench.py --impl reference --gpus 1 --steps K ...  # the reference's own CUDA kernels (oracle/_ref)
 
 A "step" is ONE outer iteration of DirectBA::BundleAdjustment (surfel activation + geometry optimisation +
@@ -10,7 +10,9 @@ restarted from the same perturbed state every step (device-to-device restore ins
 every step does the same work.  Metric (BASELINE.json): surfel-keyframe residuals per second =
 (depth residuals + descriptor residuals at the pose step's starting state) / step time.
 
-Prints exactly one JSON line on rank 0.
+Prints exactly one JSON line on rank 0.  --dump-outputs DIR writes what the last timed step computed as DIR/<name>.npy
+(float32 / float64): keyframe poses and activations, the step's statistics, and a fixed seeded sample of the surfel rows
+and active flags.
 """
 from __future__ import annotations
 
@@ -34,17 +36,12 @@ METRIC = "surfel_keyframe_residuals_per_second_per_BA_iteration"
 UNIT = "residuals/s"
 
 
-def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+# H100 SXM data sheet (NVIDIA): 3.35 TB/s of HBM3 bandwidth
+HBM_PEAK_GBS = 3350.0
 
 
 class ClockSampler:
-    """SM clock + throttle reasons sampled WHILE the timed region runs (B200_PROFILING.md clocks line): NVML polled from a
+    """SM clock + throttle reasons sampled WHILE the timed region runs: NVML polled from a
     thread every millisecond (a timed region can be a few tens of ms), nvidia-smi -lms as the fallback."""
 
     _REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap"}
@@ -246,6 +243,8 @@ def run_ours(args, scene, rank, world):
     barrier()
     torch.cuda.synchronize()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ba, res)
     ms_total = ev0.elapsed_time(ev1)
     if world > 1:   # device time, max over ranks
         t = torch.tensor([ms_total], device=dev)
@@ -260,17 +259,12 @@ def run_ours(args, scene, rank, world):
     value = residuals / (ms_step * 1e-3)
 
     # roofline of the dominant kernel (PoseAccumulateKernel), measured live with cudaEvents around each launch
-    peak, peak_src = load_peaks()
+    peak = HBM_PEAK_GBS
     alg = algorithmic_bytes(prof, prof["kf_evals"])
     pose_s = prof["pose_ms"] * 1e-3
     achieved = alg / pose_s / 1e9 if pose_s > 0 else 0.0
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "pose_kernel_dram_bytes_per_launch.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            traffic = json.load(f).get(scene.cfg.name)
     roofline = {"bound": "hbm", "kernel": "PoseAccumulateKernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": "H100 SXM data sheet (3.35 TB/s)",
                 "algorithmic_bytes_per_launch": alg / max(prof["pose_launches"], 1),
                 "avg_launch_ms": prof["pose_ms"] / max(prof["pose_launches"], 1),
                 "launches_timed": prof["pose_launches"],
@@ -335,6 +329,25 @@ def run_ours(args, scene, rank, world):
                                         "balanced by measured work (1 all-reduce of K x 17 floats); NCCL over NVLink")
         dist.barrier(device_ids=[dev.index])
     return out
+
+
+def dump_outputs(out_dir, ba, res, sample=262_144):
+    """What the last timed step returned to its caller: keyframe poses and activations, the step's statistics, and the surfel
+    rows / active flags at a fixed seeded sample of surfel indices (the full rows of cfg3 are 96 MB).  step_statistics holds
+    converged, cost, depth_residual_count, descriptor_residual_count, iterations_done, pose_iterations_total, surfels_size."""
+    os.makedirs(out_dir, exist_ok=True)
+    poses, act = ba.GetKeyframeStates()
+    rows, flags = ba.GetSurfelsHost(), ba.GetActiveHost()
+    n = rows.shape[1]
+    idx = np.sort(np.random.default_rng(0).choice(n, sample, replace=False)) if n > sample else np.arange(n)
+    stats = {f: float(getattr(res, f)) for f in ("iterations_done", "converged", "depth_residual_count", "descriptor_residual_count",
+                                                "cost", "pose_iterations_total", "surfels_size")}
+    arrays = {"keyframe_poses": np.asarray(poses, np.float32), "keyframe_activations": np.asarray(act, np.float32),
+              "surfel_sample_index": idx.astype(np.float64), "surfel_rows_sample": np.ascontiguousarray(rows[:, idx], np.float32),
+              "active_flags_sample": flags[idx].astype(np.float32),
+              "step_statistics": np.array([stats[k] for k in sorted(stats)], np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def check_replicas(scene, ba, step, dev, rank, world):
@@ -543,8 +556,8 @@ def run_reference(args, scene):
             "reference_debug_count": count_ref, "reference_depth_count": count_depth,
             "ms_full_ba_10_iterations": ms_full, "full_ba_iterations": int(full.iterations_done),
             "cpu_baseline": {"value": value, "unit": UNIT, "cores": 1, "kind": "reference",
-                             "sample": "the reference's own unmodified CUDA kernels (oracle/_ref, built for sm_100 with its own flags) on "
-                                       "ONE B200, driven by one host thread through the restated DirectBA host loop; the reference has "
+                             "sample": "the reference's own unmodified CUDA kernels (oracle/_ref, built for sm_90a with its own flags) on "
+                                       "one GPU, driven by one host thread through the restated DirectBA host loop; the reference has "
                                        "no CPU implementation of this path"},
             "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "gpu_launches": int(launches), "clocks": clocks,
@@ -588,21 +601,24 @@ def main():
 def _main(saved_stdout):
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps (at least 1)")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--workload", default=os.environ.get("BADBA_WORKLOAD", "cfg3"))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e-all", action="store_true", help="skip the e2e variant that re-uploads every keyframe every step")
     ap.add_argument("--intrinsics", action="store_true",
                     help="optimise depth intrinsics + depth deformation and colour intrinsics inside the step (the cfg4 configuration)")
     ap.add_argument("--residuals-override", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32 / float64, < 64 MB in all)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
 
-    from badslam_b200.scene import config_by_name, make_scene
     if args.impl == "reference" and rank != 0:
         return 0
     scene = load_scene(args.workload, rank, world)

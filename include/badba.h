@@ -1,4 +1,4 @@
-/* include/badba.h -- C ABI of libbadba_b200.so, the Blackwell (sm_100a) direct
+/* include/badba.h -- C ABI of libbadba_b200.so, the Hopper (sm_90a) direct
  * bundle-adjustment backend that drops in behind ETH3D/badslam's DirectBA.
  *
  * The reference has no FFI layer: its seam is the C++ class `DirectBA`

@@ -1,6 +1,6 @@
 // include/badba_direct_ba.hpp -- header-only C++ adaptor that keeps the reference's own signatures on top of the
 // C ABI of include/badba.h, so that BadSlam::RunBundleAdjustment (applications/badslam/src/badslam/bad_slam.cc:485-540)
-// and the BA thread (bad_slam.cc:1196-1317) can call the sm_100a backend without source changes beyond the include.
+// and the BA thread (bad_slam.cc:1196-1317) can call the sm_90a backend without source changes beyond the include.
 //
 // It mirrors  class vis::DirectBA  (applications/badslam/src/badslam/direct_ba.h:65-550):
 //   ctor                      direct_ba.h:73-88

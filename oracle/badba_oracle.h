@@ -28,7 +28,7 @@ enum { ORC_KF_ACTIVE = 0, ORC_KF_COVIS_ACTIVE = 1, ORC_KF_INACTIVE = 2 };
 /* Texture-filter emulation of cudaFilterModeLinear on a normalized-float u8
  * texture (keyframe.cc:67-73): 0 = exact float weights, 1 = weights rounded to
  * nearest 1/256 (CUDA programming guide: 9-bit fixed point, 8 fractional bits),
- * 2 = weights truncated to 1/256, 3 (default) = the measured B200 behaviour (8-bit rounded per-texel product
+ * 2 = weights truncated to 1/256, 3 (default) = the measured hardware behaviour (8-bit rounded per-texel product
  * weights, unorm16 result; tools/tex_probe*.cu), 4 = same with the coordinate converted to fixed point first. */
 void orc_set_tex_mode(int mode);
 int  orc_get_tex_mode(void);

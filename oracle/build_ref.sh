@@ -1,15 +1,15 @@
 #!/usr/bin/env bash
-# Compiles the reference's OWN, UNMODIFIED BA CUDA kernels from where they lie
-# under /root/reference into oracle/_ref/ (git-ignored, travels via gpurun),
+# Compiles the reference's OWN, UNMODIFIED BA CUDA kernels from a checkout of the
+# reference ($BADSLAM_REFERENCE) into oracle/_ref/ (git-ignored),
 # then links them with oracle/ref_driver.cu (our Eigen-free restatement of the
 # thin host wrappers kernel_opt_*.cc) into oracle/_ref/libbadslam_ref.so.
 # Test / baseline infrastructure only -- never loaded by the product path.
 #
 # Flags follow applications/badslam/CMakeLists.txt:74-75 (-use_fast_math
-# --expt-relaxed-constexpr, C++14); arch = sm_100 for the B200 box.
+# --expt-relaxed-constexpr, C++14); arch = sm_90a (H100).
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
-REF="${BADSLAM_REFERENCE:-/root/reference}"
+REF="${BADSLAM_REFERENCE:?set BADSLAM_REFERENCE to a checkout of the reference}"
 OUT="$HERE/_ref"
 mkdir -p "$OUT/obj"
 if [ ! -d "$REF/applications/badslam/src/badslam" ]; then
@@ -18,7 +18,7 @@ if [ ! -d "$REF/applications/badslam/src/badslam" ]; then
 fi
 B="$REF/applications/badslam/src/badslam"
 NVCC="${NVCC:-nvcc}"
-FLAGS=(-std=c++14 -O3 -arch=sm_100 -use_fast_math --expt-relaxed-constexpr
+FLAGS=(-std=c++14 -O3 -gencode arch=compute_90a,code=sm_90a -use_fast_math --expt-relaxed-constexpr
        -Xcompiler -fPIC -w
        -I "$HERE/ref_shim" -I "$REF/applications/badslam/src" -I "$REF/libvis/src"
        -I "$REF/libvis/third_party/loguru")
@@ -34,7 +34,7 @@ for s in "${SRCS[@]}"; do
   if [ ! -f "$o" ] || [ "$s" -nt "$o" ]; then
     extra=()
     # AccumulateIntrinsicsCoefficientsCUDAKernel is launched with 1024-thread blocks (CUDA_AUTO_TUNE_1D_TEMPLATED default,
-    # kernel_opt_intrinsics.cu:239-242) but compiles to > 64 registers for sm_100: "too many resources requested for
+    # kernel_opt_intrinsics.cu:239-242) but compiles to > 64 registers: "too many resources requested for
     # launch".  Same for PCGInitCUDAKernel (1024 threads, kernel_pcg.cu:538-541).  Cap the registers for these translation
     # units only (a build flag, the sources stay untouched).
     [[ "$s" == *kernel_opt_intrinsics.cu || "$s" == *kernel_pcg.cu ]] && extra=(-maxrregcount=64)

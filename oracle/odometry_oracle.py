@@ -16,7 +16,7 @@ Follows, function by function:
   TrackFramePairwise                            pairwise_frame_tracking.cc:153-678
   IsScaleNPoseEstimationConverged               convergence_analysis.h:56-63
   PinholeCamera4f::Scaled                       libvis/src/libvis/camera.h:1086-1097,1696-1705
-The texture unit is the bit-exact model of badslam_b200.scene.tex_luma (measured on B200, tools/tex_probe*.cu).  Pinned by
+The texture unit is the bit-exact model of badslam_b200.scene.tex_luma (measured, tools/tex_probe.cu).  Pinned by
 tests/golden/tiny_odometry.npz (outputs of the reference's own kernels on a B200, tools/make_golden.py --odometry-only).
 """
 from __future__ import annotations

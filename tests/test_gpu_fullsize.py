@@ -1,5 +1,5 @@
-"""GPU parity at the sizes bench.py measures (BASELINE.json configs 2 and 3): the sm_100a path through the C ABI against the
-reference's own CUDA kernels (oracle/_ref) on the same seeded scene -- the tile sizes (TILE = 1024 at 3 M surfels), the
+"""GPU parity at the sizes bench.py measures (BASELINE.json configs 2 and 3): the sm_90a path through the C ABI against the
+reference's own CUDA kernels (recorded outputs, tests/golden/ref) on the same seeded scene -- the tile sizes (TILE = 1024 at 3 M surfels), the
 8-keyframe work groups of the pose kernel and the 13 keyframe groups of the geometry kernels only exist at these sizes.
 
 Tolerances (BASELINE.json north_star): 1e-4 relative on normal-equation coefficients / residual sums, 1e-5 m / 1e-5 rad on
@@ -23,9 +23,9 @@ def rel(a, b):
 def mods():
     from badslam_b200 import scene as S
     from badslam_b200.direct_ba import DirectBA
-    from oracle import cpu_oracle, ref_cuda
-    assert ref_cuda.available(), "oracle/_ref/libbadslam_ref.so missing (oracle/build_ref.sh)"
-    return S, DirectBA, cpu_oracle, ref_cuda
+    from oracle import cpu_oracle, ref_golden
+    assert ref_golden.available(), "recording needs oracle/_ref/libbadslam_ref.so (oracle/build_ref.sh)"
+    return S, DirectBA, cpu_oracle, ref_golden
 
 
 def check_pose_coefficients(S, ba, ref, sc, keyframes):
@@ -38,7 +38,7 @@ def check_pose_coefficients(S, ba, ref, sc, keyframes):
         assert abs(pc.cost_depth + pc.cost_desc1 - cost) < REL * cost, (k, pc.cost_depth + pc.cost_desc1, cost)
 
 
-def check_one_ba_iteration(S, ba, ref, ref2, sc):
+def check_one_ba_iteration(S, R, ba, ref, ref2, sc):
     """One outer iteration of the alternation (activation, normals, position / descriptor, pose of every keyframe) from the
     same state on both sides; ref2 = a second run of the reference = its own noise floor."""
     K = sc.cfg.num_keyframes
@@ -59,10 +59,10 @@ def check_one_ba_iteration(S, ba, ref, ref2, sc):
         dt, dr = S.pose_error(ba.keyframes()[k].global_T_frame(), ref.pose(k))
         worst = max(worst, dt, dr)
         assert dt < POSE_T + 2 * noise and dr < POSE_R + 2 * noise, (k, dt, dr, noise)
-    assert np.array_equal(ba.GetKeyframeStates()[1], ref.activation())
+    assert R.equal(ba.GetKeyframeStates()[1], ref.activation())
     # activation flags: identical; surfel rows after the geometry step: positions to 2e-6 m, packed normals identical,
     # descriptors to 2e-3 of their +-180 range (tests/test_gpu_parity.py::test_activation_and_geometry at small size)
-    assert np.array_equal(ba.GetActiveHost(), ref.active())
+    assert R.equal(ba.GetActiveHost(), ref.active())
     a, b_ = ba.GetSurfelsHost(), ref.surfels()
     d = np.abs(a[:3] - b_[:3])
     assert d.max() < 1e-5 and (d > 2e-6).mean() < 1e-5, (d.max(), (d > 2e-6).mean())   # (2e-6 on every one of the 30 k surfels of `small`)
@@ -77,7 +77,7 @@ def test_cfg2_every_keyframe_and_one_ba_iteration(mods):
     sc = S.make_scene(S.config_by_name("cfg2"))
     ba, ref, ref2 = DirectBA.from_scene(sc), R.RefDirectBA(sc), R.RefDirectBA(sc)
     check_pose_coefficients(S, ba, ref, sc, range(sc.cfg.num_keyframes))
-    check_one_ba_iteration(S, ba, ref, ref2, sc)
+    check_one_ba_iteration(S, R, ba, ref, ref2, sc)
 
 
 def test_cfg3_spread_keyframes_and_one_ba_iteration(mods):
@@ -88,13 +88,13 @@ def test_cfg3_spread_keyframes_and_one_ba_iteration(mods):
     ba, ref = DirectBA.from_scene(sc), R.RefDirectBA(sc)
     check_pose_coefficients(S, ba, ref, sc, (0, 7, 8, 63, 100, 129, 150, 191, 192, 199))
     ref2 = R.RefDirectBA(sc)
-    check_one_ba_iteration(S, ba, ref, ref2, sc)
+    check_one_ba_iteration(S, R, ba, ref, ref2, sc)
 
 
 # BASELINE.json configs 4 and 5 (500 keyframes / 4 M surfels with intrinsics + depth deformation; 1280x720, 400 keyframes /
-# 8 M surfels).  Scene generation alone takes minutes, so these two only run when BADBA_BIG_CONFIGS=1 (tools/r2_big_configs.sh;
-# the logs of the hardware runs are under profiles/bench/).  The spot check is the one of the benchmarked configuration:
-# association counts, H, b and cost of four keyframes from different work groups against the reference's own kernels.
+# 8 M surfels).  Scene generation alone takes minutes, so these two only run when BADBA_BIG_CONFIGS=1.  The spot check is the
+# one of the benchmarked configuration: association counts, H, b and cost of four keyframes from different work groups against
+# the reference's own kernels (their recorded outputs, tests/golden/ref).
 import os
 
 big = pytest.mark.skipif(not os.environ.get("BADBA_BIG_CONFIGS"), reason="set BADBA_BIG_CONFIGS=1 (minutes of scene generation)")
@@ -136,4 +136,4 @@ def test_big_config_spot_check(mods, name):
         print(f"cfg4 after 2 BA iterations with intrinsics: a {a:.5f} / reference {ra:.5f}, fx {di[0]:.4f} / {rdi[0]:.4f}, "
               f"worst pose difference {worst:.2e}")
     free, total = torch.cuda.mem_get_info()
-    print(f"{name}: device memory in use with product + reference resident {(total - free) / 2**30:.2f} GiB")
+    print(f"{name}: device memory in use {(total - free) / 2**30:.2f} GiB")

@@ -1,4 +1,4 @@
-"""GPU parity of the end-of-BA surfel maintenance (PerformBASchemeEndTasks, direct_ba.cc:566-653): the sm_100a path through the
+"""GPU parity of the end-of-BA surfel maintenance (PerformBASchemeEndTasks, direct_ba.cc:566-653): the sm_90a path through the
 C ABI against the reference's own kernels (oracle/_ref) and the CPU oracle.  Deletion decisions, the compaction
 permutation and the radii are integer / exact-value work: the bar is bit-exact."""
 import numpy as np
@@ -13,9 +13,9 @@ def mods():
     assert torch.cuda.is_available()
     from badslam_b200 import scene as S
     from badslam_b200.direct_ba import DirectBA
-    from oracle import cpu_oracle, ref_cuda
-    assert ref_cuda.available(), "oracle/_ref/libbadslam_ref.so missing (oracle/build_ref.sh)"
-    return S, DirectBA, cpu_oracle, ref_cuda
+    from oracle import cpu_oracle, ref_golden
+    assert ref_golden.available(), "recording needs oracle/_ref/libbadslam_ref.so (oracle/build_ref.sh)"
+    return S, DirectBA, cpu_oracle, ref_golden
 
 
 def perturb(sc):
@@ -34,7 +34,7 @@ def test_end_tasks_three_way(mods, name):
     assert d0 == d1 > 0 and n0 == ref.surfels_size() == n - d0 == ba.surfels_size()
     a, b = ba.GetSurfelsHost(), ref.surfels()
     assert a.shape == b.shape == (8, n0)
-    assert np.array_equal(a.view(np.uint32), b.view(np.uint32))          # same survivors, same slots, same radii
+    assert R.equal(a.view(np.uint32), b.view(np.uint32))          # same survivors, same slots, same radii
     assert not np.any(a[0].view(np.uint32) == 0x7fffffff)
     if name != "cfg2":
         orc = O.Oracle(sc)
@@ -61,7 +61,7 @@ def test_bundle_adjustment_end_task_schedule(mods):
     # same survivors in the same slots (the two BA iterations before differ by fp32 round-off: a packed normal or a radius
     # decision may flip for a handful of surfels)
     assert (a[3].view(np.uint32) != b[3].view(np.uint32)).mean() < 1e-3 and (a[4] != b[4]).mean() < 1e-3
-    assert np.array_equal(a[5].view(np.uint32), b[5].view(np.uint32))
+    assert R.equal(a[5].view(np.uint32), b[5].view(np.uint32))
     assert np.abs(a[:3] - b[:3]).mean() < 1e-6 and np.abs(a[:3] - b[:3]).max() < 1e-3   # (displaced surfels that survive are ill-constrained)
     # increase_ba_iteration_count = false: counters 1 != -1 -> end tasks first (nothing left to delete), then not again
     r2 = ba.BundleAdjustment(None, False, False, False, True, True, 1, 1, increase_ba_iteration_count=False)
@@ -106,11 +106,9 @@ def test_create_surfels_for_keyframe_three_way(mods, name, filt):
     n0 = sc.num_surfels
     ba, ref, orc = DirectBA.from_scene(sc), R.RefDirectBA(sc), O.Oracle(sc)
     # The reference's outcome for cell size > 1 depends on an atomicCAS race (kernel_create_surfels.cu:68): two more independent
-    # runs give its own spread.  Measured on B200 with five runs (profiles/r2/lifecycle_spread.log): the reference scatters by
-    # 0.1 - 1 % per keyframe, while a fixed tie-break rule is a DIFFERENT sample of the race, systematically: this backend's hashed
-    # order creates +0.1 ... +3.5 % (13 % for the last keyframe of the smallest scene) more surfels than the reference's mean --
-    # 4 to 13 of the reference's standard deviations.  So the reference's spread cannot be the bound; the bound is the measured
-    # offset with a margin, and the spread is printed next to it.
+    # runs give its own spread.  A fixed tie-break rule is a DIFFERENT sample of the race, systematically: this backend's hashed
+    # order creates more surfels than the reference's mean, by several of the reference's standard deviations.  So the
+    # reference's spread cannot be the bound; the bound is the offset with a margin, and the spread is printed next to it.
     more = [R.RefDirectBA(sc) for _ in range(2)] if sc.cfg.cell > 1 else []
     K = sc.cfg.num_keyframes
     for k in range(K):
@@ -141,7 +139,7 @@ def test_create_surfels_for_keyframe_three_way(mods, name, filt):
         b = ref.surfels()
         assert b.shape == a.shape
         assert np.abs(a[:3] - b[:3]).max() < 2e-6 and (a[3].view(np.uint32) != b[3].view(np.uint32)).mean() < 1e-3
-        assert np.array_equal(a[4], b[4]) and np.array_equal(a[5].view(np.uint32), b[5].view(np.uint32))
+        assert R.equal(a[4], b[4]) and R.equal(a[5].view(np.uint32), b[5].view(np.uint32))
         assert np.abs(a[6:8] - b[6:8]).mean() < 2e-3 and np.abs(a[6:8] - b[6:8]).max() < 1.0
     # every new surfel is associated with the keyframe that created it: creating again adds (almost) nothing
     again = sum(ba.CreateSurfelsForKeyframe(None, filt, k) for k in range(K))
@@ -174,8 +172,8 @@ def test_merge_surfels_three_way(mods, name):
         assert d0 == d2, (k, d0, d2)
         total = [total[0] + d0, total[1] + d1, total[2] + d2]
     print("merged (ours, reference, second reference run, oracle):", total[0], total[1], total_ref2, total[2], "of", sc2.num_surfels)
-    # measured with five reference runs (profiles/r2/lifecycle_spread.log): the reference scatters by 0.3 - 0.7 %, this backend's
-    # fixed order merges 0.9 % / 4.3 % fewer surfels than its mean (tiny / small)
+    # the reference's first-come order scatters from run to run; this backend's fixed order merges a few per cent fewer surfels
+    # than its mean
     assert abs(total[1] - total_ref2) <= max(10, 0.05 * total[1]), (total[1], total_ref2)
     assert total[0] > 0 and abs(total[0] - total[1]) <= max(5, 0.08 * total[1]), total
     a, c = ba.GetSurfelsHost(), orc.surfels[:8, :orc.n]

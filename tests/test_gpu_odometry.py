@@ -1,4 +1,4 @@
-"""GPU parity of the image-pair odometry (bba_track_frame_pairwise; SURVEY.md 8(f4)): the sm_100a path through the C ABI against
+"""GPU parity of the image-pair odometry (bba_track_frame_pairwise; SURVEY.md 8(f4)): the sm_90a path through the C ABI against
 the reference's own kernels (oracle/_ref: kernel_downsample.cu, cuda_image_processing.cu, kernel_opt_pose.cu:422-1340 behind the
 restated host loop of pairwise_frame_tracking.cc) and the CPU oracle (oracle/odometry_oracle.py).
 
@@ -32,9 +32,9 @@ def mods():
     assert torch.cuda.is_available()
     from badslam_b200 import scene as S
     from badslam_b200.direct_ba import DirectBA
-    from oracle import odometry_oracle, ref_cuda
-    assert ref_cuda.available(), "oracle/_ref/libbadslam_ref.so missing (oracle/build_ref.sh)"
-    return S, DirectBA, odometry_oracle, ref_cuda
+    from oracle import odometry_oracle, ref_golden
+    assert ref_golden.available(), "recording needs oracle/_ref/libbadslam_ref.so (oracle/build_ref.sh)"
+    return S, DirectBA, odometry_oracle, ref_golden
 
 
 def make_pair(S, name, base_kf=0, motion=MOTION):
@@ -55,12 +55,14 @@ def oracle_for(O, sc, **kw):
 
 
 def check_levels(ba, ref, orc, num_scales, first_scale, O=None):
-    """Product vs reference: identical.  Oracle (when given): level 0 identical colour / validity, depth to the fast-math
-    rounding; coarser levels are built by the oracle's downsample() from the REFERENCE's finer level and must agree up to the
-    tie-break of "closest to the block mean" (tests/test_oracle_odometry.py::assert_same_up_to_ties: on planar surfaces the
-    four depths of a block are pairwise symmetric about their mean); the reference's images are then handed to the oracle so
-    that its evaluations run on the same pyramid."""
+    """Product vs reference: identical on the rows the recorded reference levels hold.  Oracle (when given): level 0 identical
+    colour / validity, depth to the fast-math rounding; coarser levels are built by the oracle's downsample() from the
+    PRODUCT's finer level (equal to the reference's where recorded) and must agree up to the tie-break of "closest to the
+    block mean" (tests/test_oracle_odometry.py::assert_same_up_to_ties: on planar surfaces the four depths of a block are
+    pairwise symmetric about their mean); the product's images are then handed to the oracle so that its evaluations run on
+    the same pyramid."""
     from test_oracle_odometry import assert_same_up_to_ties
+    from oracle.ref_golden import kept_rows
     prev = {}
     for scale in range(num_scales):
         for which in (0, 1):
@@ -69,10 +71,14 @@ def check_levels(ba, ref, orc, num_scales, first_scale, O=None):
             d0, n0, c0 = ba.OdometryLevel(which, scale)
             d1, n1, c1 = ref.odometry_level(which, scale)
             assert d0.shape == d1.shape
-            assert np.array_equal(c0, c1), (which, scale, np.mean(c0 != c1))
-            assert np.array_equal(d0, d1), (which, scale, np.mean(d0 != d1))
+            rows = kept_rows(d1)   # (recorded reference levels may hold a band of rows only)
+            assert np.array_equal(c0[rows], c1[rows]), (which, scale, np.mean(c0[rows] != c1[rows]))
+            assert np.array_equal(d0[rows], d1[rows]), (which, scale, np.mean(d0[rows] != d1[rows]))
+            v = np.asarray(d1[rows]) > 0
+            assert np.array_equal(n0[rows][v], np.asarray(n1[rows])[v]), (which, scale)
+            # the product's level equals the reference's: the oracle is checked against it in full
+            d1, n1, c1 = d0, n0, c0
             valid = d1 > 0
-            assert np.array_equal(n0[valid], n1[valid]), (which, scale)
             if orc is not None:
                 wn = "tracked" if which else "base"
                 if scale == 0:
@@ -152,16 +158,16 @@ def test_track_frame_pairwise_against_reference(mods, name, num_scales, kw):
     e_init = S.pose_error(IDENT, true_rel)[0]
     gain = 0.5 if first == 0 else 0.9
     assert S.pose_error(est0, true_rel)[0] < gain * e_init and S.pose_error(est1, true_rel)[0] < gain * e_init
-    # equally good optimum: the cost of our result, evaluated by the REFERENCE's kernels, is not worse than the reference's own
+    # equally good optimum: the cost of our result is not worse than the cost of the reference's result, both evaluated on the
+    # product's pyramid by the product's cost kernel (equal to the reference's at fixed states: the three-way test above)
     gm = bool(kw.get("use_gradmag", False))
-    _, _, _, _, counts, costs = ref.odometry_coeffs(first, est0, est1, use_gradmag=gm)
+    _, _, _, _, counts, costs = ba.OdometryCoeffs(first, est0, est1, use_gradmag=gm)
     assert costs[0] <= costs[1] * (1 + 2e-3) and counts[0] >= counts[1] * (1 - 2e-3), (counts, costs)
     # Same iteration counts and branch decisions; the poses agree to 1e-5 plus the drift of this non-settling iteration: up to 86
     # capped Gauss-Newton steps amplify last-bit differences of H / b (ours are fp64 sums of per-lane fp32 partials, the
     # reference's unordered fp32 atomics), measured here by the reference's own spread.
     assert all(abs(a - b) <= 1 for a, b in zip(its0, its1)), (its0, its1)   # (equal in every run so far; +-1 for a level that stops at the threshold)
-    # (measured on B200 over the five cases: 2e-9 ... 3e-5 m between the two implementations with 5e-9 ... 2e-5 m between runs of
-    #  the reference; the floor of 5e-5 covers a draw in which the reference's four runs happen to agree closely)
+    # (the floor of 5e-5 covers a draw in which the reference's four runs happen to agree closely)
     limit = max(1e-5 + 10 * noise, 5e-5)
     assert dt < limit and dr < limit, (dt, dr, noise)
     assert res0.kernel_launches <= num_scales + 4 and res1.kernel_launches > 10 * res0.kernel_launches

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on the B200 box): the sm_100a path, called through the C ABI, against
+"""GPU parity tests (run with `-m gpu` on an H100): the sm_90a path, called through the C ABI, against
 (a) the reference's own CUDA kernels (oracle/_ref), (b) the CPU oracle and (c) the committed golden fixtures.
 
 Tolerances (BASELINE.json north_star): 1e-4 relative on residual sums / normal-equation coefficients,
@@ -28,9 +28,9 @@ def mods():
     assert torch.cuda.is_available()
     from badslam_b200 import scene as S
     from badslam_b200.direct_ba import DirectBA
-    from oracle import cpu_oracle, ref_cuda
-    assert ref_cuda.available(), "oracle/_ref/libbadslam_ref.so missing (oracle/build_ref.sh)"
-    return S, DirectBA, cpu_oracle, ref_cuda
+    from oracle import cpu_oracle, ref_golden
+    assert ref_golden.available(), "recording needs oracle/_ref/libbadslam_ref.so (oracle/build_ref.sh)"
+    return S, DirectBA, cpu_oracle, ref_golden
 
 
 def test_pose_coefficients_three_way(mods, small_scene):
@@ -78,7 +78,7 @@ def test_single_residual_type(mods, tiny_scene, use_depth, use_desc):
         # photometric-only position updates are ill-conditioned for low-texture surfels (H00 ~ 1e-6 regulariser,
         # kernel_opt_geometry.cu:292-295): round-off differences are amplified for a handful of surfels
         assert np.mean(d) < 2e-6 and (d > 2e-6).mean() < 0.1 and d.max() < 2e-3
-    assert np.array_equal(a[3].view(np.uint32), b_[3].view(np.uint32))
+    assert R.equal(a[3].view(np.uint32), b_[3].view(np.uint32))
     dd = np.abs(a[6:8] - b_[6:8])
     assert dd.max() < (2e-3 if use_depth else 5.0) and dd.mean() < (1e-4 if use_depth else 5e-3)
 
@@ -111,7 +111,7 @@ def test_activation_and_geometry(mods, small_scene):
     orc.activation[1], orc.activation[2] = 2, 1
     ba.UpdateSurfelActivation(); ref.update_activation(); orc.update_activation()
     fa, fr, fo = ba.GetActiveHost(), ref.active(), orc.active[:sc.num_surfels]
-    assert np.array_equal(fa, fr) and np.array_equal(fo, fr)
+    assert R.equal(fa, fr) and R.equal(fo, fr)
     assert 0 < fr.sum() <= sc.num_surfels
     ba.OptimizeGeometryIteration(); ref.optimize_geometry_iteration(); orc.optimize_geometry_iteration()
     a, b_, c = ba.GetSurfelsHost(), ref.surfels(), orc.surfels[:8, :sc.num_surfels]
@@ -149,7 +149,7 @@ def test_bundle_adjustment_against_reference(mods, small_scene):
     for k in range(K):
         dt, dr = S.pose_error(ba.keyframes()[k].global_T_frame(), ref.pose(k))
         assert dt < POSE_T + 2 * self_noise and dr < POSE_R + 2 * self_noise, (k, dt, dr, self_noise)
-    assert np.array_equal(ba.GetKeyframeStates()[1], ref.activation())
+    assert R.equal(ba.GetKeyframeStates()[1], ref.activation())
     a, b_ = ba.GetSurfelsHost(), ref.surfels()
     assert np.mean(np.abs(a[:3] - b_[:3])) < 1e-6
 
@@ -327,7 +327,8 @@ def test_intrinsics_step_three_way(mods, opt_depth, opt_color):
     cf0, cf1 = ba.cfactor_buffer(), ref.cfactor()
     if opt_depth:
         assert np.any(d0 != np.asarray(sc.depth_K, np.float32)) and np.any(cf0 != cf_init) and abs(a0 - a_init) > 1e-3
-        assert (cf0 != 0).sum() == (cf1 != 0).sum()
+        rows = R.kept_rows(cf1)
+        assert (cf0[rows] != 0).sum() == (cf1[rows] != 0).sum()
         assert np.abs(cf0 - cf1).max() < 1e-4 and np.abs(cf0 - orc.cfactor).max() < 1e-3
     else:
         assert np.array_equal(d0, np.asarray(sc.depth_K, np.float32)) and np.array_equal(cf0, cf_init) and a0 == np.float32(a_init)

@@ -1,5 +1,5 @@
 // tools/tex_probe.cu -- which arithmetic reproduces cudaFilterModeLinear on a normalized-float u8 texture bit-exactly?
-// nvcc -gencode arch=compute_100a,code=sm_100a -o tools/tex_probe tools/tex_probe.cu ; run on the GPU box.
+// nvcc -gencode arch=compute_90a,code=sm_90a -o tools/tex_probe tools/tex_probe.cu ; run on the GPU box.
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdio>
