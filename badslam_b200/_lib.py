@@ -12,6 +12,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 # BADBA_LIB: development override for A/B runs of kernel variants (tools/ab_bench.sh); the product is the in-tree library
 LIB_PATH = os.environ.get("BADBA_LIB") or os.path.join(HERE, "libbadba_b200.so")
 
+ABI_VERSION = 9   # BBA_ABI_VERSION of the include/badba.h this binding types
+
+# bba_pose_variant: the pose kernel's instantiations (surfel tile, precomputed per-surfel frames)
+POSE_VARIANT_AUTO, POSE_VARIANT_256_PRE, POSE_VARIANT_512_PRE, POSE_VARIANT_256, POSE_VARIANT_512, POSE_VARIANT_1024 = range(6)
+
 OK, ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_STATE, ERR_UNSUPPORTED, ERR_NO_DEVICE = range(6)
 STATUS_NAMES = {0: "BBA_OK", 1: "BBA_ERR_INVALID_ARGUMENT", 2: "BBA_ERR_CUDA", 3: "BBA_ERR_STATE",
                 4: "BBA_ERR_UNSUPPORTED", 5: "BBA_ERR_NO_DEVICE"}
@@ -139,6 +144,7 @@ SYMBOLS = {
     "bba_get_cfactor_host": (C.c_int, [_P, _P, _P]),
     "bba_cfactor_size": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "bba_accumulate_pose_coeffs": (C.c_int, [_P, C.c_int, _F7, C.POINTER(PoseCoeffs), _P]),
+    "bba_debug_pose_coeffs_batch": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "bba_estimate_frame_pose": (C.c_int, [_P, C.c_int, _F7, _F7, C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_estimate_frame_pose_for_frame": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _F7, _F7,
                                                     C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
@@ -194,8 +200,8 @@ def load():
         fn = getattr(lib, name)   # AttributeError if the symbol is not exported
         fn.restype = restype
         fn.argtypes = argtypes
-    if lib.bba_abi_version() != 8:
-        raise ImportError("libbadba_b200.so ABI version mismatch")
+    if lib.bba_abi_version() != ABI_VERSION:
+        raise ImportError(f"libbadba_b200.so ABI version {lib.bba_abi_version()}, this binding expects {ABI_VERSION}")
     _lib = lib
     return lib
 

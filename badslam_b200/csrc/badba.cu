@@ -442,6 +442,43 @@ void AssignKeyframes(bba_handle h, const std::vector<int>& ids, std::vector<int>
   BalanceWork(cost.data(), static_cast<int>(ids.size()), h->cfg.world_size, owner->data());
 }
 
+// Launch setup of the pose kernel, shared by the pose step and the entry points that evaluate it at a fixed state: arguments
+// over the handle's buffers (the caller sets work_list / work_count) and, for a PRE variant, the per-surfel frames computed on s.
+// The surfels do not move during a pose step: what the descriptor residual needs of a surfel alone (unpacked normal, the two
+// tangent points) is computed once here instead of once per (surfel, keyframe, Gauss-Newton iteration) pair.  Not worth a
+// launch + 9 rows of traffic for a handful of keyframes (frame tracking): the kernel then derives them per pair.
+// variant = kPoseVariantAuto: that choice, from the number of keyframes n_work; any other: forced (bba_debug_pose_coeffs_batch).
+bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStream_t s, bba::PoseAccumulateArgs* acc) {
+  acc->cam = MakeCamera(h);
+  acc->surfels = h->surfels;
+  acc->pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
+  acc->n = h->surfels_size;
+  acc->kfs = h->d_kfs;
+  acc->work_records = h->d_work_records;
+  acc->acc = h->d_acc;
+  acc->stage_counts = h->d_stage_counts;
+  acc->queue = h->d_queue;
+  acc->frames = nullptr;
+  acc->frames_pitch = 0;
+  static const bool precompute = BBA_POSE_PRECOMPUTE && !std::getenv("BADBA_POSE_NO_PRECOMPUTE");   // (development switch for A/B runs)
+  const bool pre = variant == bba::kPoseVariantAuto ? precompute && h->cfg.use_descriptor_residuals && n_work >= 4
+                                                    : bba::PoseVariantPre(variant);
+  if (pre && h->surfels_size > 0) {
+    const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
+    if (!h->d_frames || h->frames_pitch < pitch) {
+      cudaFree(h->d_frames);
+      h->d_frames = nullptr;
+      h->frames_pitch = pitch;
+      BBA_CUDA(h, cudaMalloc(&h->d_frames, sizeof(float) * 9 * static_cast<size_t>(pitch)));
+    }
+    bba::LaunchSurfelFrames(h->surfels, pitch, h->surfels_size, h->d_frames, h->frames_pitch, s);
+    ++h->launches;
+    acc->frames = h->d_frames;
+    acc->frames_pitch = h->frames_pitch;
+  }
+  return BBA_OK;
+}
+
 bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, int max_iterations, cudaStream_t s) {
   const int K = static_cast<int>(h->keyframes.size());
   const int n = static_cast<int>(ids.size());
@@ -483,34 +520,7 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
   if (bba_status st = MarkStaging(h, s)) return st;
 
   bba::PoseAccumulateArgs acc;
-  acc.cam = MakeCamera(h);
-  acc.surfels = h->surfels;
-  acc.pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
-  acc.n = h->surfels_size;
-  acc.kfs = h->d_kfs;
-  acc.work_records = h->d_work_records;
-  acc.acc = h->d_acc;
-  acc.stage_counts = h->d_stage_counts;
-  acc.queue = h->d_queue;
-  acc.frames = nullptr;
-  acc.frames_pitch = 0;
-  // The surfels do not move during a pose step: what the descriptor residual needs of a surfel alone (unpacked normal, the two
-  // tangent points) is computed once here instead of once per (surfel, keyframe, Gauss-Newton iteration) pair.  Not worth a
-  // launch + 9 rows of traffic for a handful of keyframes (frame tracking): the kernel then derives them per pair.
-  static const bool precompute = BBA_POSE_PRECOMPUTE && !std::getenv("BADBA_POSE_NO_PRECOMPUTE");   // (development switch for A/B runs)
-  if (precompute && h->cfg.use_descriptor_residuals && n_local >= 4 && h->surfels_size > 0) {
-    const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
-    if (!h->d_frames || h->frames_pitch < pitch) {
-      cudaFree(h->d_frames);
-      h->d_frames = nullptr;
-      h->frames_pitch = pitch;
-      BBA_CUDA(h, cudaMalloc(&h->d_frames, sizeof(float) * 9 * static_cast<size_t>(pitch)));
-    }
-    bba::LaunchSurfelFrames(h->surfels, pitch, h->surfels_size, h->d_frames, h->frames_pitch, s);
-    ++h->launches;
-    acc.frames = h->d_frames;
-    acc.frames_pitch = h->frames_pitch;
-  }
+  if (bba_status st = PreparePoseAccumulate(h, n_local, bba::kPoseVariantAuto, s, &acc)) return st;
   bba::PoseSolveArgs sol;
   sol.kfs = h->d_kfs;
   sol.pose_est = h->d_pose_est;
@@ -2106,17 +2116,7 @@ bba_status bba_accumulate_pose_coeffs(bba_handle h, int id, const float pose[7],
   BBA_CUDA(h, cudaMemsetAsync(h->d_acc + static_cast<size_t>(id) * bba::kPoseAccSize, 0, sizeof(double) * bba::kPoseAccSize, s));
   BBA_CUDA(h, cudaMemsetAsync(h->d_stage_counts + 2 * id, 0, sizeof(unsigned long long) * 2, s));
   bba::PoseAccumulateArgs acc;
-  acc.cam = MakeCamera(h);
-  acc.surfels = h->surfels;
-  acc.pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
-  acc.n = h->surfels_size;
-  acc.kfs = h->d_kfs;
-  acc.work_records = h->d_work_records;
-  acc.frames = nullptr;
-  acc.frames_pitch = 0;
-  acc.acc = h->d_acc;
-  acc.stage_counts = h->d_stage_counts;
-  acc.queue = h->d_queue;
+  if (bba_status st = PreparePoseAccumulate(h, 1, bba::kPoseVariantAuto, s, &acc)) return st;
   BBA_CUDA(h, cudaMemsetAsync(h->d_queue, 0, sizeof(unsigned int), s));
   acc.work_list = h->d_work[0];
   acc.work_count = h->d_count;
@@ -2145,6 +2145,68 @@ bba_status bba_accumulate_pose_coeffs(bba_handle h, int id, const float pose[7],
   out->cost_depth = h->h_acc[29];
   out->cost_desc1 = h->h_acc[30];
   out->cost_desc2 = h->h_acc[31];
+  return BBA_OK;
+}
+
+bba_status bba_debug_pose_coeffs_batch(bba_handle h, int count, const int* ids, const float* poses, int variant, int with_stats,
+                                       double* H, double* b, uint64_t* counts, double* costs, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (!ids || !poses || !H || !b || !counts || (with_stats && !costs))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_pose_coeffs_batch: null argument");
+  if (count < 1 || count > h->cfg.max_keyframes)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_pose_coeffs_batch: count out of range");
+  if (!bba::PoseVariantValid(variant)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_pose_coeffs_batch: unknown variant");
+  const int K = static_cast<int>(h->keyframes.size());
+  std::vector<char> listed(K, 0);
+  for (int i = 0; i < count; ++i) {
+    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_pose_coeffs_batch: bad keyframe id");
+    if (listed[ids[i]]) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_pose_coeffs_batch: keyframe listed twice");
+    listed[ids[i]] = 1;
+  }
+  if (bba_status st = CheckSurfels(h)) return st;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (bba_status st = WaitStaging(h)) return st;
+  for (int k = 0; k < K; ++k) FillKfDevice(h->keyframes[k], h->keyframes[k].pose, h->h_kfs + k);
+  for (int i = 0; i < count; ++i) {
+    FillKfDevice(h->keyframes[ids[i]], PoseFromArray(poses + 7 * i), h->h_kfs + ids[i]);
+    h->h_work[i] = ids[i];
+  }
+  h->h_work[h->cfg.max_keyframes] = count;
+  BBA_CUDA(h, cudaMemcpyAsync(h->d_kfs, h->h_kfs, sizeof(KfDevice) * K, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemcpyAsync(h->d_work[0], h->h_work, sizeof(int) * count, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemcpyAsync(h->d_count, h->h_work + h->cfg.max_keyframes, sizeof(int), cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->d_acc, 0, sizeof(double) * bba::kPoseAccSize * K, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->d_stage_counts, 0, sizeof(unsigned long long) * 2 * K, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->d_queue, 0, sizeof(unsigned int), s));
+  bba::PoseAccumulateArgs acc;
+  if (bba_status st = PreparePoseAccumulate(h, count, variant, s, &acc)) return st;
+  acc.work_list = h->d_work[0];
+  acc.work_count = h->d_count;
+  if (h->surfels_size > 0) {
+    bba::LaunchPoseAccumulate(acc, h->sm_count, with_stats != 0, count, s, variant);
+    h->launches += 2;   // record packing + the kernel
+  }
+  BBA_CUDA(h, cudaGetLastError());
+  // every keyframe's record, listed or not: a record written outside the work list shows up in the caller's rows
+  std::vector<double> rec(static_cast<size_t>(bba::kPoseAccSize) * K);
+  std::vector<unsigned long long> sc(2 * static_cast<size_t>(K));
+  BBA_CUDA(h, cudaMemcpyAsync(rec.data(), h->d_acc, sizeof(double) * rec.size(), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaMemcpyAsync(sc.data(), h->d_stage_counts, sizeof(unsigned long long) * sc.size(), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->d_acc, 0, sizeof(double) * rec.size(), s));
+  BBA_CUDA(h, cudaMemsetAsync(h->d_stage_counts, 0, sizeof(unsigned long long) * sc.size(), s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  h->staging_pending = false;
+  for (int k = 0; k < K; ++k) {
+    const double* r = rec.data() + static_cast<size_t>(k) * bba::kPoseAccSize;
+    std::memcpy(H + 21 * static_cast<size_t>(k), r, sizeof(double) * 21);
+    std::memcpy(b + 6 * static_cast<size_t>(k), r + 21, sizeof(double) * 6);
+    uint64_t* c = counts + 4 * static_cast<size_t>(k);
+    c[0] = sc[2 * k];
+    c[1] = sc[2 * k + 1];
+    c[2] = static_cast<uint64_t>(r[27] + 0.5);
+    c[3] = static_cast<uint64_t>(r[28] + 0.5);
+    if (with_stats) std::memcpy(costs + 3 * static_cast<size_t>(k), r + 29, sizeof(double) * 3);
+  }
   return BBA_OK;
 }
 

@@ -438,26 +438,29 @@ static void LaunchPoseAccumulateT(const PoseAccumulateArgs& args, int sm_count, 
 }
 
 template <bool STATS>
-static void LaunchPoseAccumulateS(const PoseAccumulateArgs& args, int sm_count, cudaStream_t stream) {
+static void LaunchPoseAccumulateS(const PoseAccumulateArgs& args, int sm_count, int variant, cudaStream_t stream) {
   // Tile size: as large as possible (one group of TMA transactions per item), but small enough that a keyframe group still
   // yields several items per resident CTA.  With the precomputed frames 14 rows are staged: 512 surfels x 2 stages = 56 KB per
   // CTA (two CTAs per SM), the same footprint as 1024 surfels of the 7-row variant.
-  const uint64_t slots = static_cast<uint64_t>(BBA_POSE_MIN_CTAS * sm_count) * 4;
-  if (args.frames != nullptr) {
-    if (args.n >= slots * 512) LaunchPoseAccumulateT<512, STATS, true>(args, sm_count, stream);
-    else LaunchPoseAccumulateT<256, STATS, true>(args, sm_count, stream);
-    return;
+  if (variant == kPoseVariantAuto) {
+    const uint64_t slots = static_cast<uint64_t>(BBA_POSE_MIN_CTAS * sm_count) * 4;
+    if (args.frames != nullptr) variant = args.n >= slots * 512 ? kPoseVariant512Pre : kPoseVariant256Pre;
+    else variant = args.n >= slots * 1024 ? kPoseVariant1024 : args.n >= slots * 512 ? kPoseVariant512 : kPoseVariant256;
   }
-  if (args.n >= slots * 1024) LaunchPoseAccumulateT<1024, STATS, false>(args, sm_count, stream);
-  else if (args.n >= slots * 512) LaunchPoseAccumulateT<512, STATS, false>(args, sm_count, stream);
-  else LaunchPoseAccumulateT<256, STATS, false>(args, sm_count, stream);
+  switch (variant) {
+    case kPoseVariant256Pre: LaunchPoseAccumulateT<256, STATS, true>(args, sm_count, stream); break;
+    case kPoseVariant512Pre: LaunchPoseAccumulateT<512, STATS, true>(args, sm_count, stream); break;
+    case kPoseVariant256: LaunchPoseAccumulateT<256, STATS, false>(args, sm_count, stream); break;
+    case kPoseVariant512: LaunchPoseAccumulateT<512, STATS, false>(args, sm_count, stream); break;
+    case kPoseVariant1024: LaunchPoseAccumulateT<1024, STATS, false>(args, sm_count, stream); break;
+  }
 }
 
-void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream) {
+void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream, int variant) {
   if (args.n == 0) return;
   PackWorkRecordsKernel<<<(max_work * 6 + 127) / 128, 128, 0, stream>>>(args.kfs, args.work_list, args.work_count, args.work_records);
-  if (with_stats) LaunchPoseAccumulateS<true>(args, sm_count, stream);
-  else LaunchPoseAccumulateS<false>(args, sm_count, stream);
+  if (with_stats) LaunchPoseAccumulateS<true>(args, sm_count, variant, stream);
+  else LaunchPoseAccumulateS<false>(args, sm_count, variant, stream);
 }
 
 __global__ void __launch_bounds__(256) SurfelFramesKernel(const float* __restrict__ surfels, uint32_t pitch, uint32_t n,

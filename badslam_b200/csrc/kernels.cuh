@@ -38,9 +38,17 @@ struct PoseAccumulateArgs {
 // keyframe poses are optimised): rows 0-2 unpacked + re-normalised normal (util_nvcc_only.cuh:83-95), rows 3-5 / 6-8 the tangent
 // points gp + t1 / gp + t2 (cost_function.cuh:115-133).  frames: [9][frames_pitch] floats.
 void LaunchSurfelFrames(const float* surfels, uint32_t pitch, uint32_t n, float* frames, uint32_t frames_pitch, cudaStream_t stream);
+// Instantiations of the pose kernel (surfel tile, PRE = stages the precomputed frames); the values are bba_pose_variant's.
+enum PoseVariant { kPoseVariantAuto = 0, kPoseVariant256Pre = 1, kPoseVariant512Pre = 2, kPoseVariant256 = 3, kPoseVariant512 = 4,
+                   kPoseVariant1024 = 5 };
+inline bool PoseVariantValid(int v) { return v >= kPoseVariantAuto && v <= kPoseVariant1024; }
+inline bool PoseVariantPre(int v) { return v == kPoseVariant256Pre || v == kPoseVariant512Pre; }
 // max_work: upper bound of *work_count known to the host (sizes the record-packing launch that precedes the kernel).
-// args.frames != null selects the variant that stages the precomputed frames instead of the packed normal / radius rows.
-void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream);
+// variant = kPoseVariantAuto: the tile follows from args.n and the SM count, and args.frames != null selects the variant that
+// stages the precomputed frames instead of the packed normal / radius rows.  Any other variant forces that instantiation; a PRE
+// variant needs args.frames, the others ignore it.
+void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
+                          int variant = kPoseVariantAuto);
 
 struct PoseSolveArgs {
   KfDevice* kfs;

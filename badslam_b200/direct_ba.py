@@ -445,6 +445,22 @@ class DirectBA:
                                                          C.byref(out), self._stream_ptr(stream)))
         return out
 
+    def PoseCoeffsBatch(self, keyframe_ids, global_T_frame_estimates, variant: int = _lib.POSE_VARIANT_AUTO, with_stats: bool = True,
+                        stream=None):
+        """Parity hook (bba_debug_pose_coeffs_batch): the pose kernel over a work list of keyframes, each at its own pose
+        ([count, 7]), in the instantiation the BA pose step runs (or a forced one, _lib.POSE_VARIANT_*).  Returns
+        (H [K, 21], b [K, 6], counts [K, 4] = in image / depth ok / associated / photometric, costs [K, 3]) indexed by keyframe
+        id over all K keyframes; rows of keyframes outside the list are what the launch left in their records (zeros)."""
+        ids = np.ascontiguousarray(keyframe_ids, np.int32)
+        poses = np.ascontiguousarray(global_T_frame_estimates, np.float32).reshape(len(ids), 7)
+        K = len(self._keyframes)
+        H, b, costs = np.zeros((K, 21)), np.zeros((K, 6)), np.zeros((K, 3))
+        counts = np.zeros((K, 4), np.uint64)
+        self._check(self._lib.bba_debug_pose_coeffs_batch(self._h, len(ids), ids.ctypes.data, poses.ctypes.data, int(variant),
+                                                          int(with_stats), H.ctypes.data, b.ctypes.data, counts.ctypes.data,
+                                                          costs.ctypes.data, self._stream_ptr(stream)))
+        return H, b, counts, costs
+
     def EstimateFramePose(self, stream, global_T_frame_initial_estimate, keyframe_id: int):
         """direct_ba.h:122-129; returns (global_T_frame_estimate, iterations, converged)."""
         p = np.ascontiguousarray(global_T_frame_initial_estimate, np.float32)

@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define BBA_ABI_VERSION 8
+#define BBA_ABI_VERSION 9
 
 typedef struct bba_context* bba_handle;
 
@@ -199,6 +199,27 @@ bba_status bba_cfactor_size(bba_handle h, int* cf_width, int* cf_height);
  * `keyframe_id` evaluated at global_T_frame_estimate.  Synchronises the stream. */
 bba_status bba_accumulate_pose_coeffs(bba_handle h, int keyframe_id, const float global_T_frame_estimate[7],
                                       bba_pose_coeffs* out, void* stream);
+/* Parity hook for the pose kernel as the BA pose step runs it: one launch over a work list of `count` distinct keyframes
+ * (ids [count], each evaluated at its own global_T_frame [count][7]), in groups of 8, with the record packing and -- for the
+ * PRE variants -- the per-surfel frames the pose step computes first.  variant = BBA_POSE_VARIANT_AUTO picks the instantiation
+ * the pose step would (PRE from 4 keyframes with descriptor residuals, the tile from the surfel count and the SM count);
+ * any other value forces that (surfel tile, PRE) instantiation.  with_stats = 0 runs the kernel without the residual costs
+ * and stage counters, as the pose step does after its first Gauss-Newton iteration.
+ * Outputs are indexed by KEYFRAME ID over all keyframe_count keyframes, listed or not (a keyframe outside the list reads back
+ * zeros unless the kernel wrote to its record): H [keyframe_count][21] (upper triangle, row-major), b [keyframe_count][6],
+ * counts [keyframe_count][4] = {in image, depth ok, associated, photometric} (the first two stay 0 without stats), costs
+ * [keyframe_count][3] = {depth, descriptor 1, descriptor 2} (written only with stats; may be NULL without).  Every
+ * keyframe's accumulator and counters are cleared before the launch and after the read-back.  Synchronises the stream. */
+typedef enum {
+  BBA_POSE_VARIANT_AUTO = 0,
+  BBA_POSE_VARIANT_256_PRE = 1,   /* 256-surfel tiles, precomputed per-surfel frames */
+  BBA_POSE_VARIANT_512_PRE = 2,
+  BBA_POSE_VARIANT_256 = 3,       /* 256-surfel tiles, tangent points derived per pair */
+  BBA_POSE_VARIANT_512 = 4,
+  BBA_POSE_VARIANT_1024 = 5
+} bba_pose_variant;
+bba_status bba_debug_pose_coeffs_batch(bba_handle h, int count, const int* keyframe_ids, const float* global_T_frame, int variant,
+                                       int with_stats, double* H, double* b, uint64_t* counts, double* costs, void* stream);
 /* DirectBA::EstimateFramePose (direct_ba.h:122-129, direct_ba_alternating.cc:42-283) against a stored keyframe's
  * images.  iterations/converged may be NULL. */
 bba_status bba_estimate_frame_pose(bba_handle h, int keyframe_id, const float global_T_frame_initial[7],

@@ -24,7 +24,12 @@ def test_header_declares_the_hot_path():
         assert required in names
 
 
-def test_library_exports_every_declared_symbol():
+def declared_abi_version():
+    src = open(os.path.join(ROOT, "include", "badba.h")).read()
+    return int(re.search(r"^#define BBA_ABI_VERSION (\d+)$", src, flags=re.M).group(1))
+
+
+def test_library_exports_every_declared_symbol_at_the_header_abi_version():
     from badslam_b200 import _lib
     assert os.path.exists(_lib.LIB_PATH), "build libbadba_b200.so first (python -m badslam_b200.build)"
     lib = ctypes.CDLL(_lib.LIB_PATH)
@@ -32,7 +37,8 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in include/badba.h but not exported"
     # and the python binding types every one of them
     assert set(declared_symbols()) == set(_lib.SYMBOLS.keys())
-    assert _lib.load().bba_abi_version() == 8
+    # library, header and binding are one version: v9 added bba_debug_pose_coeffs_batch
+    assert _lib.load().bba_abi_version() == declared_abi_version() == _lib.ABI_VERSION == 9
 
 
 def test_no_cpu_fallback_without_a_device():
