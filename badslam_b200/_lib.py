@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 # BADBA_LIB: development override for A/B runs of kernel variants (tools/ab_bench.sh); the product is the in-tree library
 LIB_PATH = os.environ.get("BADBA_LIB") or os.path.join(HERE, "libbadba_b200.so")
 
-ABI_VERSION = 9   # BBA_ABI_VERSION of the include/badba.h this binding types
+ABI_VERSION = 10   # BBA_ABI_VERSION of the include/badba.h this binding types
 
 # bba_pose_variant: the pose kernel's instantiations (surfel tile, precomputed per-surfel frames)
 POSE_VARIANT_AUTO, POSE_VARIANT_256_PRE, POSE_VARIANT_512_PRE, POSE_VARIANT_256, POSE_VARIANT_512, POSE_VARIANT_1024 = range(6)
@@ -44,6 +44,13 @@ class BAOptions(C.Structure):
                 ("increase_ba_iteration_count", C.c_int), ("time_limit_seconds", C.c_double),
                 ("pcg_max_inner_iterations", C.c_int), ("pcg_max_keyframes", C.c_int), ("pcg_gauge_keyframe", C.c_int),
                 ("progress_function", PROGRESS_FN), ("progress_user", C.c_void_p)]
+
+
+class PcgProbe(C.Structure):   # bba_pcg_probe
+    _fields_ = [("r", C.c_void_p), ("M", C.c_void_p), ("p", C.c_void_p), ("g", C.c_void_p), ("delta", C.c_void_p),
+                ("alpha_n", C.c_double), ("alpha_d", C.c_double),
+                ("r_step2", C.c_void_p), ("delta_step2", C.c_void_p), ("z", C.c_void_p), ("beta_n", C.c_double),
+                ("p_step3", C.c_void_p), ("g_step3", C.c_void_p), ("alpha_d_step3", C.c_double)]
 
 
 class BAResult(C.Structure):
@@ -165,7 +172,7 @@ SYMBOLS = {
     "bba_compact_surfels": (C.c_int, [_P, C.c_uint32, C.c_int, C.POINTER(C.c_uint32), _P]),
     "bba_preprocess_frame": (C.c_int, [_P, C.POINTER(PreprocessOptions), _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
                                        _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
-    "bba_pcg_debug": (C.c_int, [_P, C.POINTER(BAOptions), C.POINTER(C.c_uint32), _P, _P, _P, _P, _P, _P]),
+    "bba_pcg_debug": (C.c_int, [_P, C.POINTER(BAOptions), C.c_int, C.c_int, C.POINTER(C.c_uint32), C.POINTER(PcgProbe), _P]),
     "bba_bundle_adjust": (C.c_int, [_P, C.POINTER(BAOptions), C.POINTER(BAResult), _P]),
     "bba_peer_export": (C.c_int, [_P, _P]),
     "bba_peer_import": (C.c_int, [_P, _P, C.c_int]),

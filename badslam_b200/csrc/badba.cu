@@ -1199,6 +1199,119 @@ bba::PcgArgs MakePcgArgs(bba_handle h, const PcgLayout& L, int gauge) {
   return a;
 }
 
+// The PCG solver's phases, shared by BundleAdjustPCG and the parity hook bba_pcg_debug.  Vectors: d_pcg = {r, M, delta, g, p};
+// scalars = {alpha_n or beta_n (slot an), alpha_d (1), beta_n or alpha_n (slot bn), this rank's alpha_d (3, multi-GPU)}.
+// Init: r = -J^T W F and M = diag(J^T W J) over every keyframe (:312-361), then PCGInit2 (:363-373) into slot `an`.
+bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int an, cudaStream_t s) {
+  const uint32_t U = L.unknown_count;
+  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg[0], 0, sizeof(float) * U, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg[1], 0, sizeof(float) * U, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg_scalars, 0, sizeof(double) * 4, s));
+  bba::LaunchPcgAccumulate(a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
+  if (h->cfg.world_size > 1) {
+    h->collective(h->collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->d_pcg[0], U, s);
+    h->collective(h->collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->d_pcg[1], U, s);
+    h->replicated_pass_pending = false;
+  }
+  bba::LaunchPcgInit2(U, L.a_index, h->depth_a, a.kf_count, h->d_pcg[0], h->d_pcg[1], h->d_pcg[2], h->d_pcg[3], h->d_pcg[4],
+                      h->d_pcg_scalars, an, h->sm_count, s);
+  h->launches += 2;
+  return BBA_OK;
+}
+
+// Inner step, first half: g += J^T W J p and alpha_d += p^T J^T W J p over every keyframe (PCGStep1CUDA, :392-419).
+bba_status PcgStep1(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, cudaStream_t s) {
+  bba::LaunchPcgAccumulate(a, h->sm_count, false, s);
+  if (h->cfg.world_size > 1) {   // g and this rank's part of alpha_d: one all-reduce
+    float* g = h->d_pcg[3];
+    bba::LaunchPcgPackAlphaD(h->d_pcg_scalars, g + L.unknown_count, s);
+    h->collective(h->collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, g, static_cast<size_t>(L.unknown_count) + 2, s);
+    bba::LaunchPcgUnpackAlphaD(h->d_pcg_scalars, g + L.unknown_count, s);
+    h->launches += 2;
+  }
+  return BBA_OK;
+}
+
+// Inner step, second half: delta += alpha p, r -= alpha A p, z = M^-1 r (into g), beta_n = z^T r into slot `bn` (:421-437).
+bba_status PcgStep2(bba_handle h, const PcgLayout& L, int an, int bn, cudaStream_t s) {
+  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg_scalars + bn, 0, sizeof(double), s));
+  bba::LaunchPcgStep2(L.unknown_count, L.a_index, h->d_pcg[0], h->d_pcg[1], h->d_pcg[2], h->d_pcg[3], h->d_pcg[4], h->d_pcg_scalars,
+                      an, bn, h->sm_count, s);
+  h->launches += 2;
+  BBA_CUDA(h, cudaGetLastError());
+  return BBA_OK;
+}
+
+// Before the next inner step: p = z + beta p, g = 0, alpha_d re-armed with its lambda / prior term (:456-464).
+bba_status PcgStep3(bba_handle h, const PcgLayout& L, int an, int bn, cudaStream_t s) {
+  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg_scalars + 1, 0, sizeof(double), s));
+  bba::LaunchPcgStep3(L.unknown_count, L.a_index, static_cast<int>(h->keyframes.size()), h->d_pcg[3], h->d_pcg[4], h->d_pcg_scalars,
+                      an, bn, h->sm_count, s);
+  ++h->launches;
+  return BBA_OK;
+}
+
+// Applies pcg_delta (:552-638): surfels, cfactors, poses (all but the gauge keyframe), intrinsics.  *num_converged counts the
+// keyframes whose pose update is below the convergence threshold (the gauge keyframe included).
+bba_status PcgApplyDelta(bba_handle h, const PcgLayout& L, int gauge, cudaStream_t s, int* num_converged) {
+  const int K = static_cast<int>(h->keyframes.size());
+  const uint32_t N = h->surfels_size, P = static_cast<uint32_t>(h->cf_w) * h->cf_h;
+  const float* pcg_delta = h->d_pcg[2];
+  size_t n_host = 0;
+  const size_t pose_floats = L.opt_poses ? 6 * static_cast<size_t>(K - 1) : 0;
+  if (pose_floats) BBA_CUDA(h, cudaMemcpyAsync(h->h_pcg_delta, pcg_delta, sizeof(float) * pose_floats, cudaMemcpyDeviceToHost, s));
+  n_host = pose_floats;
+  float* h_di = h->h_pcg_delta + n_host;
+  if (L.opt_depth_intr) {
+    BBA_CUDA(h, cudaMemcpyAsync(h_di, pcg_delta + L.depth_start, sizeof(float) * 5, cudaMemcpyDeviceToHost, s));
+    n_host += 5;
+  }
+  float* h_ci = h->h_pcg_delta + n_host;
+  if (L.opt_color_intr) BBA_CUDA(h, cudaMemcpyAsync(h_ci, pcg_delta + L.color_start, sizeof(float) * 4, cudaMemcpyDeviceToHost, s));
+  if (L.opt_geometry && N > 0) {
+    bba::LaunchPcgUpdateSurfels(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N, L.use_desc, L.surfel_start,
+                                pcg_delta, s);
+    ++h->launches;
+    h->replicated_pass_pending = true;   // every rank rewrites its whole replica (PeerFence)
+  }
+  if (L.opt_depth_intr) {
+    bba::LaunchPcgUpdateCfactor(h->d_cfactor, P, pcg_delta + L.depth_start + 5, s);
+    ++h->launches;
+  }
+  BBA_CUDA(h, cudaGetLastError());
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  if (L.opt_poses) {
+    for (int k = 0; k < K; ++k) {
+      if (k == gauge) {
+        ++*num_converged;
+        continue;
+      }
+      const float* d6 = h->h_pcg_delta + 6 * static_cast<size_t>(k < gauge ? k : k - 1);
+      const Pose delta = bba::Exp(d6);
+      h->keyframes[k].pose = bba::Compose(h->keyframes[k].pose, delta);   // :569-570
+      float lg[6];
+      bba::Log(delta, lg);
+      if (bba::IsScale1PoseEstimationConverged(lg)) ++*num_converged;
+    }
+  }
+  if (L.opt_depth_intr) {   // :590-612
+    const double old_fx_inv = 1. / h->depth_K[0], old_fy_inv = 1. / h->depth_K[1];
+    const double old_cx_inv = -(h->depth_K[2] - 0.5) * old_fx_inv, old_cy_inv = -(h->depth_K[3] - 0.5) * old_fy_inv;
+    const double new_fx = 1. / (old_fx_inv + h_di[0]);
+    const double new_fy = 1. / (old_fy_inv + h_di[1]);
+    const double new_cx = -(new_fx * (old_cx_inv + h_di[2])) + 0.5;
+    const double new_cy = -(new_fy * (old_cy_inv + h_di[3])) + 0.5;
+    h->depth_K[0] = static_cast<float>(new_fx);
+    h->depth_K[1] = static_cast<float>(new_fy);
+    h->depth_K[2] = static_cast<float>(new_cx);
+    h->depth_K[3] = static_cast<float>(new_cy);
+    h->depth_a += h_di[4];
+  }
+  if (L.opt_color_intr)   // :623-638
+    for (int c = 0; c < 4; ++c) h->color_K[c] = static_cast<float>(h->color_K[c] + h_ci[c]);
+  return BBA_OK;
+}
+
 // DirectBA::BundleAdjustmentPCG (direct_ba_pcg.cc:43-819) without the surfel lifecycle branches.
 bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result* res, cudaStream_t s) {
   const int K = static_cast<int>(h->keyframes.size());
@@ -1217,9 +1330,7 @@ bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result*
   if (o->pcg_gauge_keyframe >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "pcg_gauge_keyframe out of range");
   PcgLayout L;
   if (bba_status st = MakePcgLayout(h, o, &L)) return st;
-  const bool opt_depth_intr = L.opt_depth_intr, opt_color_intr = L.opt_color_intr, opt_poses = L.opt_poses, opt_geometry = L.opt_geometry;
-  const bool use_desc = L.use_desc;
-  const uint32_t P = static_cast<uint32_t>(h->cf_w) * h->cf_h;
+  const bool opt_poses = L.opt_poses, opt_geometry = L.opt_geometry;
   const uint64_t launches_before = h->launches;
   const auto t_start = std::chrono::steady_clock::now();
   if (!o->increase_ba_iteration_count && h->ba_iteration_count != h->last_ba_iteration_count) {   // :157-161
@@ -1263,42 +1374,20 @@ bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result*
     BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
 
     if (bba_status st = MakePcgLayout(h, o, &L)) return st;   // unknown layout (:273-309)
-    const uint32_t surfel_start = L.surfel_start, depth_start = L.depth_start, a_index = L.a_index, color_start = L.color_start;
     const uint32_t unknown_count = L.unknown_count;
-    float *pcg_r = h->d_pcg[0], *pcg_M = h->d_pcg[1], *pcg_delta = h->d_pcg[2], *pcg_g = h->d_pcg[3], *pcg_p = h->d_pcg[4];
     const int gauge = o->pcg_gauge_keyframe >= 0 ? o->pcg_gauge_keyframe : (rand() % K);   // :324
 
     int num_converged = 0;
     if (unknown_count > 0) {
-      BBA_CUDA(h, cudaMemsetAsync(pcg_r, 0, sizeof(float) * unknown_count, s));   // :312-313
-      BBA_CUDA(h, cudaMemsetAsync(pcg_M, 0, sizeof(float) * unknown_count, s));
-      BBA_CUDA(h, cudaMemsetAsync(h->d_pcg_scalars, 0, sizeof(double) * 4, s));
       const bba::PcgArgs a = MakePcgArgs(h, L, gauge);
-      bba::LaunchPcgAccumulate(a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe, :336-361
-      if (world > 1) {
-        h->collective(h->collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, pcg_r, unknown_count, s);
-        h->collective(h->collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, pcg_M, unknown_count, s);
-        h->replicated_pass_pending = false;
-      }
       int an = 0, bn = 2;
-      bba::LaunchPcgInit2(unknown_count, a_index, h->depth_a, K, pcg_r, pcg_M, pcg_delta, pcg_g, pcg_p, h->d_pcg_scalars, an,
-                          h->sm_count, s);   // :363-373
-      h->launches += 2;
+      if (bba_status st = PcgInit(h, L, a, an, s)) return st;
       float prev_r_norm = std::numeric_limits<float>::infinity();
       int without_improvement = 0;
       for (int step = 0; step < max_inner; ++step) {
         if (step > 0) std::swap(an, bn);   // alpha_n <- beta_n (:386); g was cleared and alpha_d re-armed by PcgStep3Kernel
-        bba::LaunchPcgAccumulate(a, h->sm_count, false, s);   // PCGStep1CUDA for every keyframe, :392-419
-        if (world > 1) {   // g and this rank's part of alpha_d: one all-reduce
-          bba::LaunchPcgPackAlphaD(h->d_pcg_scalars, pcg_g + unknown_count, s);
-          h->collective(h->collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, pcg_g, static_cast<size_t>(unknown_count) + 2, s);
-          bba::LaunchPcgUnpackAlphaD(h->d_pcg_scalars, pcg_g + unknown_count, s);
-          h->launches += 2;
-        }
-        BBA_CUDA(h, cudaMemsetAsync(h->d_pcg_scalars + bn, 0, sizeof(double), s));
-        bba::LaunchPcgStep2(unknown_count, a_index, pcg_r, pcg_M, pcg_delta, pcg_g, pcg_p, h->d_pcg_scalars, an, bn, h->sm_count, s);
-        h->launches += 2;
-        BBA_CUDA(h, cudaGetLastError());
+        if (bba_status st = PcgStep1(h, L, a, s)) return st;
+        if (bba_status st = PcgStep2(h, L, an, bn, s)) return st;
         BBA_CUDA(h, cudaMemcpyAsync(h->h_pcg_scalars, h->d_pcg_scalars, sizeof(double) * 4, cudaMemcpyDeviceToHost, s));
         BBA_CUDA(h, cudaStreamSynchronize(s));   // :436-437
         ++res->pcg_inner_iterations_total;
@@ -1311,65 +1400,11 @@ bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result*
         }
         prev_r_norm = r_norm;
         if (step < max_inner - 1) {   // :456-464
-          BBA_CUDA(h, cudaMemsetAsync(h->d_pcg_scalars + 1, 0, sizeof(double), s));
-          bba::LaunchPcgStep3(unknown_count, a_index, K, pcg_g, pcg_p, h->d_pcg_scalars, an, bn, h->sm_count, s);
-          ++h->launches;
+          if (bba_status st = PcgStep3(h, L, an, bn, s)) return st;
         }
       }
       BBA_CUDA(h, cudaEventRecord(h->ev[2], s));
-
-      // --- apply pcg_delta (:552-638)
-      size_t n_host = 0;
-      const size_t pose_floats = opt_poses ? 6 * static_cast<size_t>(K - 1) : 0;
-      if (pose_floats) BBA_CUDA(h, cudaMemcpyAsync(h->h_pcg_delta, pcg_delta, sizeof(float) * pose_floats, cudaMemcpyDeviceToHost, s));
-      n_host = pose_floats;
-      float* h_di = h->h_pcg_delta + n_host;
-      if (opt_depth_intr) {
-        BBA_CUDA(h, cudaMemcpyAsync(h_di, pcg_delta + depth_start, sizeof(float) * 5, cudaMemcpyDeviceToHost, s));
-        n_host += 5;
-      }
-      float* h_ci = h->h_pcg_delta + n_host;
-      if (opt_color_intr) BBA_CUDA(h, cudaMemcpyAsync(h_ci, pcg_delta + color_start, sizeof(float) * 4, cudaMemcpyDeviceToHost, s));
-      if (opt_geometry && N > 0) {
-        bba::LaunchPcgUpdateSurfels(h->surfels, a.pitch, N, use_desc, surfel_start, pcg_delta, s);
-        ++h->launches;
-        h->replicated_pass_pending = true;   // every rank rewrites its whole replica (PeerFence)
-      }
-      if (opt_depth_intr) {
-        bba::LaunchPcgUpdateCfactor(h->d_cfactor, P, pcg_delta + depth_start + 5, s);
-        ++h->launches;
-      }
-      BBA_CUDA(h, cudaGetLastError());
-      BBA_CUDA(h, cudaStreamSynchronize(s));
-      if (opt_poses) {
-        for (int k = 0; k < K; ++k) {
-          if (k == gauge) {
-            ++num_converged;
-            continue;
-          }
-          const float* d6 = h->h_pcg_delta + 6 * static_cast<size_t>(k < gauge ? k : k - 1);
-          const Pose delta = bba::Exp(d6);
-          h->keyframes[k].pose = bba::Compose(h->keyframes[k].pose, delta);   // :569-570
-          float lg[6];
-          bba::Log(delta, lg);
-          if (bba::IsScale1PoseEstimationConverged(lg)) ++num_converged;
-        }
-      }
-      if (opt_depth_intr) {   // :590-612
-        const double old_fx_inv = 1. / h->depth_K[0], old_fy_inv = 1. / h->depth_K[1];
-        const double old_cx_inv = -(h->depth_K[2] - 0.5) * old_fx_inv, old_cy_inv = -(h->depth_K[3] - 0.5) * old_fy_inv;
-        const double new_fx = 1. / (old_fx_inv + h_di[0]);
-        const double new_fy = 1. / (old_fy_inv + h_di[1]);
-        const double new_cx = -(new_fx * (old_cx_inv + h_di[2])) + 0.5;
-        const double new_cy = -(new_fy * (old_cy_inv + h_di[3])) + 0.5;
-        h->depth_K[0] = static_cast<float>(new_fx);
-        h->depth_K[1] = static_cast<float>(new_fy);
-        h->depth_K[2] = static_cast<float>(new_cx);
-        h->depth_K[3] = static_cast<float>(new_cy);
-        h->depth_a += h_di[4];
-      }
-      if (opt_color_intr)   // :623-638
-        for (int c = 0; c < 4; ++c) h->color_K[c] = static_cast<float>(h->color_K[c] + h_ci[c]);
+      if (bba_status st = PcgApplyDelta(h, L, gauge, s, &num_converged)) return st;
       // surfel merge + compaction (:644-690) for the keyframes that received new surfels
       if (o->do_surfel_updates && !keyframes_with_new_surfels.empty()) {
         uint32_t merged = 0;
@@ -2788,38 +2823,58 @@ bba_status bba_compact_surfels(bba_handle h, uint32_t free_count, int with_activ
   return BBA_OK;
 }
 
-bba_status bba_pcg_debug(bba_handle h, const bba_ba_options* o, uint32_t* unknown_count, float* out_r, float* out_M, float* out_p,
-                         float* out_g, double out_scalars[2], void* stream) {
-  if (!h || !o || !unknown_count) return BBA_ERR_INVALID_ARGUMENT;
+bba_status bba_pcg_debug(bba_handle h, const bba_ba_options* o, int step, int apply, uint32_t* unknown_count, bba_pcg_probe* out,
+                         void* stream) {
+  if (!h || !o || !unknown_count || step < 0) return BBA_ERR_INVALID_ARGUMENT;
   if (bba_status st = CheckSurfels(h)) return st;
   const int K = static_cast<int>(h->keyframes.size());
   if (K == 0) return Fail(h, BBA_ERR_STATE, "no keyframes");
   if (o->pcg_gauge_keyframe < 0 || o->pcg_gauge_keyframe >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "pcg_gauge_keyframe out of range");
+  if (h->cfg.world_size > 1) return Fail(h, BBA_ERR_UNSUPPORTED, "bba_pcg_debug runs on one rank");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   PcgLayout L;
   if (bba_status st = MakePcgLayout(h, o, &L)) return st;
   *unknown_count = L.unknown_count;
-  if (!out_r || L.unknown_count == 0) return BBA_OK;
+  if (!out || L.unknown_count == 0) return BBA_OK;
   const uint32_t U = L.unknown_count;
+  auto copy = [&](float* dst, const float* src) -> bba_status {
+    if (dst) BBA_CUDA(h, cudaMemcpyAsync(dst, src, sizeof(float) * U, cudaMemcpyDeviceToHost, s));
+    return BBA_OK;
+  };
+  // the scalar slots of alpha_n / beta_n of step `step` (BundleAdjustPCG swaps them at every step after the first)
+  auto scalars = [&](int slot, double* dst) -> bba_status {
+    BBA_CUDA(h, cudaMemcpyAsync(h->h_pcg_scalars, h->d_pcg_scalars, sizeof(double) * 4, cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaStreamSynchronize(s));
+    *dst = h->h_pcg_scalars[slot];
+    return BBA_OK;
+  };
   if (bba_status st = UploadKeyframes(h, s)) return st;
-  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg[0], 0, sizeof(float) * U, s));
-  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg[1], 0, sizeof(float) * U, s));
-  BBA_CUDA(h, cudaMemsetAsync(h->d_pcg_scalars, 0, sizeof(double) * 4, s));
   const bba::PcgArgs a = MakePcgArgs(h, L, o->pcg_gauge_keyframe);
-  bba::LaunchPcgAccumulate(a, h->sm_count, true, s);
-  BBA_CUDA(h, cudaMemcpyAsync(out_r, h->d_pcg[0], sizeof(float) * U, cudaMemcpyDeviceToHost, s));
-  BBA_CUDA(h, cudaMemcpyAsync(out_M, h->d_pcg[1], sizeof(float) * U, cudaMemcpyDeviceToHost, s));
-  bba::LaunchPcgInit2(U, L.a_index, h->depth_a, K, h->d_pcg[0], h->d_pcg[1], h->d_pcg[2], h->d_pcg[3], h->d_pcg[4], h->d_pcg_scalars, 0,
-                      h->sm_count, s);
-  BBA_CUDA(h, cudaMemcpyAsync(out_p, h->d_pcg[4], sizeof(float) * U, cudaMemcpyDeviceToHost, s));
-  bba::LaunchPcgAccumulate(a, h->sm_count, false, s);
-  h->launches += 3;
+  int an = 0, bn = 2;
+  if (bba_status st = PcgInit(h, L, a, an, s)) return st;
+  for (int k = 0;; ++k) {
+    if (k > 0) std::swap(an, bn);
+    if (bba_status st = PcgStep1(h, L, a, s)) return st;
+    if (k == step) break;
+    if (bba_status st = PcgStep2(h, L, an, bn, s)) return st;
+    if (bba_status st = PcgStep3(h, L, an, bn, s)) return st;
+  }
   BBA_CUDA(h, cudaGetLastError());
-  BBA_CUDA(h, cudaMemcpyAsync(out_g, h->d_pcg[3], sizeof(float) * U, cudaMemcpyDeviceToHost, s));
-  BBA_CUDA(h, cudaMemcpyAsync(h->h_pcg_scalars, h->d_pcg_scalars, sizeof(double) * 4, cudaMemcpyDeviceToHost, s));
+  float *r = h->d_pcg[0], *M = h->d_pcg[1], *delta = h->d_pcg[2], *g = h->d_pcg[3], *p = h->d_pcg[4];
+  bba_status st = BBA_OK;
+  if ((st = copy(out->r, r)) || (st = copy(out->M, M)) || (st = copy(out->p, p)) || (st = copy(out->g, g)) || (st = copy(out->delta, delta)) ||
+      (st = scalars(an, &out->alpha_n)) || (st = scalars(1, &out->alpha_d)))
+    return st;
+  if ((st = PcgStep2(h, L, an, bn, s)) || (st = copy(out->r_step2, r)) || (st = copy(out->delta_step2, delta)) || (st = copy(out->z, g)) ||
+      (st = scalars(bn, &out->beta_n)))
+    return st;
+  if ((st = PcgStep3(h, L, an, bn, s)) || (st = copy(out->p_step3, p)) || (st = copy(out->g_step3, g)) || (st = scalars(1, &out->alpha_d_step3)))
+    return st;
+  if (apply) {
+    int num_converged = 0;
+    if ((st = PcgApplyDelta(h, L, o->pcg_gauge_keyframe, s, &num_converged))) return st;
+  }
   BBA_CUDA(h, cudaStreamSynchronize(s));
-  out_scalars[0] = h->h_pcg_scalars[0];
-  out_scalars[1] = h->h_pcg_scalars[1];
   return MarkStaging(h, s);
 }
 

@@ -611,17 +611,28 @@ class DirectBA:
 
     def PCGDebug(self, optimize_poses=True, optimize_geometry=True, optimize_depth_intrinsics=False,
                  optimize_color_intrinsics=False, gauge_keyframe=0, stream=None):
-        """Parity hook (bba_pcg_debug): r, M, p0, g = J^T W J p0 and (alpha_n, alpha_d) of the PCG solver's first step."""
+        """Parity hook (bba_pcg_debug at step 0): r, M, p0, g = J^T W J p0 and (alpha_n, alpha_d) of the PCG solver's first step."""
+        s = self.PCGProbe(0, False, optimize_poses, optimize_geometry, optimize_depth_intrinsics, optimize_color_intrinsics,
+                          gauge_keyframe, stream)
+        return s["r"], s["M"], s["p"], s["g"], np.array([s["alpha_n"], s["alpha_d"]])
+
+    def PCGProbe(self, step, apply=False, optimize_poses=True, optimize_geometry=True, optimize_depth_intrinsics=False,
+                 optimize_color_intrinsics=False, gauge_keyframe=0, stream=None) -> dict:
+        """bba_pcg_debug: the PCG solver's init pass, `step` complete inner steps, then inner step `step` observed before
+        PCGStep2 (r, M, p, g, delta, alpha_n, alpha_d), after it (r_step2, delta_step2, z, beta_n) and after PCGStep3 (p_step3,
+        g_step3, alpha_d_step3).  apply=True then applies delta to the surfels, cfactors, poses and intrinsics."""
         o = _lib.BAOptions(int(optimize_depth_intrinsics), int(optimize_color_intrinsics), 0, int(optimize_poses),
                            int(optimize_geometry), 1, 1, 1, 0, len(self._keyframes) - 1, 0, 0.0, 30, 2500, int(gauge_keyframe))
         n = C.c_uint32()
-        self._check(self._lib.bba_pcg_debug(self._h, C.byref(o), C.byref(n), None, None, None, None, None,
+        self._check(self._lib.bba_pcg_debug(self._h, C.byref(o), int(step), 0, C.byref(n), None, self._stream_ptr(stream)))
+        vectors = ("r", "M", "p", "g", "delta", "r_step2", "delta_step2", "z", "p_step3", "g_step3")
+        out = {k: np.zeros(n.value, np.float32) for k in vectors}
+        probe = _lib.PcgProbe(**{k: out[k].ctypes.data for k in vectors})
+        self._check(self._lib.bba_pcg_debug(self._h, C.byref(o), int(step), int(bool(apply)), C.byref(n), C.byref(probe),
                                             self._stream_ptr(stream)))
-        r, M, p, g = (np.zeros(n.value, np.float32) for _ in range(4))
-        sc = np.zeros(2, np.float64)
-        self._check(self._lib.bba_pcg_debug(self._h, C.byref(o), C.byref(n), r.ctypes.data, M.ctypes.data, p.ctypes.data,
-                                            g.ctypes.data, sc.ctypes.data, self._stream_ptr(stream)))
-        return r, M, p, g, sc
+        for k in ("alpha_n", "alpha_d", "beta_n", "alpha_d_step3"):
+            out[k] = getattr(probe, k)
+        return out
 
     def EnablePeerExchange(self, group=None) -> int:
         """Maps the surfel replicas of the other ranks into this process (CUDA IPC over NVLink, bba_peer_export /

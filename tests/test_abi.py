@@ -29,7 +29,7 @@ def declared_abi_version():
     return int(re.search(r"^#define BBA_ABI_VERSION (\d+)$", src, flags=re.M).group(1))
 
 
-def test_library_exports_every_declared_symbol_at_the_header_abi_version():
+def test_library_exports_every_declared_symbol_at_abi_version_10():
     from badslam_b200 import _lib
     assert os.path.exists(_lib.LIB_PATH), "build libbadba_b200.so first (python -m badslam_b200.build)"
     lib = ctypes.CDLL(_lib.LIB_PATH)
@@ -37,8 +37,8 @@ def test_library_exports_every_declared_symbol_at_the_header_abi_version():
         assert hasattr(lib, name), f"{name} declared in include/badba.h but not exported"
     # and the python binding types every one of them
     assert set(declared_symbols()) == set(_lib.SYMBOLS.keys())
-    # library, header and binding are one version: v9 added bba_debug_pose_coeffs_batch
-    assert _lib.load().bba_abi_version() == declared_abi_version() == _lib.ABI_VERSION == 9
+    # library, header and binding are one version: v10 made bba_pcg_debug stop at any inner step (bba_pcg_probe)
+    assert _lib.load().bba_abi_version() == declared_abi_version() == _lib.ABI_VERSION == 10
 
 
 def test_no_cpu_fallback_without_a_device():

@@ -23,7 +23,7 @@ def perturb(sc):
     return displace_surfels(sc)[0]
 
 
-@pytest.mark.parametrize("name", ["tiny", "small", "cfg2"])
+@pytest.mark.parametrize("name", ["tiny", "small", "many", "cfg2"])
 def test_end_tasks_three_way(mods, name):
     S, DirectBA, O, R = mods
     sc = perturb(S.make_scene(S.config_by_name(name)))
