@@ -70,6 +70,11 @@ class PreprocessOptions(C.Structure):
                 ("bilateral_filter_radius_factor", C.c_float), ("max_depth", C.c_float)]
 
 
+class RawFrameOptions(C.Structure):   # bba_raw_frame_options
+    _fields_ = [("base", PreprocessOptions), ("median_filter_and_densify_iterations", C.c_int),
+                ("pyramid_level_for_depth", C.c_int), ("pyramid_level_for_color", C.c_int)]
+
+
 class OdometryOptions(C.Structure):
     _fields_ = [("num_scales", C.c_int), ("use_pyramid_level_0", C.c_int), ("use_gradmag", C.c_int),
                 ("test_different_initial_estimates", C.c_int), ("max_iterations_per_scale", C.c_int)]
@@ -172,6 +177,9 @@ SYMBOLS = {
     "bba_compact_surfels": (C.c_int, [_P, C.c_uint32, C.c_int, C.POINTER(C.c_uint32), _P]),
     "bba_preprocess_frame": (C.c_int, [_P, C.POINTER(PreprocessOptions), _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
                                        _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
+    "bba_preprocess_raw_frame": (C.c_int, [_P, C.POINTER(RawFrameOptions), _P, C.c_size_t, C.c_int, C.c_int, _P, C.c_size_t, C.c_int,
+                                           C.c_int, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
+                                           C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "bba_pcg_debug": (C.c_int, [_P, C.POINTER(BAOptions), C.c_int, C.c_int, C.POINTER(C.c_uint32), C.POINTER(PcgProbe), _P]),
     "bba_bundle_adjust": (C.c_int, [_P, C.POINTER(BAOptions), C.POINTER(BAResult), _P]),
     "bba_peer_export": (C.c_int, [_P, _P]),

@@ -2475,29 +2475,38 @@ bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, c
   return BBA_OK;
 }
 
-bba_status bba_preprocess_frame(bba_handle h, const bba_preprocess_options* o,
-                                const uint16_t* device_raw_depth, size_t raw_depth_pitch,
-                                const uint8_t* device_rgb, size_t rgb_pitch,
-                                uint16_t* device_depth, size_t depth_pitch,
-                                uint16_t* device_normals, size_t normals_pitch,
-                                uint16_t* device_radius, size_t radius_pitch,
-                                uint8_t* device_color_rgba, size_t color_pitch,
-                                float* min_depth, float* max_depth, void* stream) {
-  if (!h || !o || !device_raw_depth || !device_depth || !device_normals || !device_radius) return h ? Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_frame: null argument") : BBA_ERR_INVALID_ARGUMENT;
+namespace {
+
+// Stage 0 of bba_preprocess_raw_frame (validated by the caller), or nullptr for bba_preprocess_frame.
+struct RawStage {
+  int median_iterations, depth_level, raw_w, raw_h, color_level;
+};
+
+// bba_preprocess_frame and bba_preprocess_raw_frame after their own checks; `fn` prefixes the error messages.
+bba_status PreprocessFrame(bba_handle h, const char* fn, const bba_preprocess_options* o,
+                           const uint16_t* device_raw_depth, size_t raw_depth_pitch,
+                           const uint8_t* device_rgb, size_t rgb_pitch,
+                           uint16_t* device_depth, size_t depth_pitch,
+                           uint16_t* device_normals, size_t normals_pitch,
+                           uint16_t* device_radius, size_t radius_pitch,
+                           uint8_t* device_color_rgba, size_t color_pitch,
+                           float* min_depth, float* max_depth, void* stream, const RawStage* raw_stage) {
+  const std::string name(fn);
+  if (!h || !o || !device_raw_depth || !device_depth || !device_normals || !device_radius) return h ? Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null argument") : BBA_ERR_INVALID_ARGUMENT;
   if ((device_rgb == nullptr) != (device_color_rgba == nullptr))
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_frame: rgb input and rgba output go together");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": rgb input and rgba output go together");
   if ((raw_depth_pitch | depth_pitch | normals_pitch | radius_pitch) & 1u)
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_frame: u16 image pitches must be even");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": u16 image pitches must be even");
   if (device_color_rgba && ((color_pitch & 3u) || (reinterpret_cast<uintptr_t>(device_color_rgba) & 3u)))
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_frame: the rgba image must be 4-byte aligned");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": the rgba image must be 4-byte aligned");
   if (device_depth == device_raw_depth)
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_frame: in-place filtering is not possible (tiles read their neighbours' raw depth)");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": in-place filtering is not possible (tiles read their neighbours' raw depth)");
   // BilateralFilteringAndDepthCutoffCUDA (cuda_depth_processing.cu:100-128)
   const int radius = static_cast<int>(o->bilateral_filter_radius_factor * o->bilateral_filter_sigma_xy + 0.5f);
   if (radius < 0 || radius > bba::pre::kMaxFilterRadius)
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_frame: bilateral filter radius outside [0, 16]");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": bilateral filter radius outside [0, 16]");
   if (!(o->bilateral_filter_sigma_xy > 0.f) || !(o->bilateral_filter_sigma_inv_depth > 0.f) || !(o->max_depth > 0.f))
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_frame: sigma_xy, sigma_inv_depth and max_depth must be positive");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": sigma_xy, sigma_inv_depth and max_depth must be positive");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!h->d_min_max) {
     BBA_CUDA(h, cudaMalloc(&h->d_min_max, 2 * sizeof(float)));
@@ -2525,7 +2534,15 @@ bba_status bba_preprocess_frame(bba_handle h, const bba_preprocess_options* o,
   f.rgba = device_color_rgba; f.rgba_pitch = static_cast<uint32_t>(color_pitch);
   f.tiles_x = (f.w + bba::pre::kTile - 1) / bba::pre::kTile;
   f.tiles_y = (f.h + bba::pre::kTile - 1) / bba::pre::kTile;
-  h->launches += bba::LaunchPreprocessFrame(f, s);
+  if (raw_stage) {
+    f.median_iterations = raw_stage->median_iterations;
+    f.depth_level = raw_stage->depth_level;
+    f.raw_w = raw_stage->raw_w; f.raw_h = raw_stage->raw_h;
+    f.color_level = raw_stage->color_level;
+    h->launches += bba::LaunchPreprocessRawFrame(f, s);
+  } else {
+    h->launches += bba::LaunchPreprocessFrame(f, s);
+  }
   BBA_CUDA(h, cudaGetLastError());
   if (min_depth || max_depth) {   // ComputeMinMaxDepthCUDA returns host values and synchronises (cuda_depth_processing.cu:452-463)
     BBA_CUDA(h, cudaMemcpyAsync(h->h_min_max, h->d_min_max, 2 * sizeof(float), cudaMemcpyDeviceToHost, s));
@@ -2534,6 +2551,61 @@ bba_status bba_preprocess_frame(bba_handle h, const bba_preprocess_options* o,
     if (max_depth) *max_depth = h->h_min_max[1];
   }
   return BBA_OK;
+}
+
+}  // namespace
+
+bba_status bba_preprocess_frame(bba_handle h, const bba_preprocess_options* o,
+                                const uint16_t* device_raw_depth, size_t raw_depth_pitch,
+                                const uint8_t* device_rgb, size_t rgb_pitch,
+                                uint16_t* device_depth, size_t depth_pitch,
+                                uint16_t* device_normals, size_t normals_pitch,
+                                uint16_t* device_radius, size_t radius_pitch,
+                                uint8_t* device_color_rgba, size_t color_pitch,
+                                float* min_depth, float* max_depth, void* stream) {
+  return PreprocessFrame(h, "bba_preprocess_frame", o, device_raw_depth, raw_depth_pitch, device_rgb, rgb_pitch, device_depth,
+                         depth_pitch, device_normals, normals_pitch, device_radius, radius_pitch, device_color_rgba, color_pitch,
+                         min_depth, max_depth, stream, nullptr);
+}
+
+bba_status bba_preprocess_raw_frame(bba_handle h, const bba_raw_frame_options* o,
+                                    const uint16_t* device_raw_depth, size_t raw_depth_pitch,
+                                    int raw_depth_width, int raw_depth_height,
+                                    const uint8_t* device_rgb, size_t rgb_pitch, int rgb_width, int rgb_height,
+                                    uint16_t* device_depth, size_t depth_pitch,
+                                    uint16_t* device_normals, size_t normals_pitch,
+                                    uint16_t* device_radius, size_t radius_pitch,
+                                    uint8_t* device_color_rgba, size_t color_pitch,
+                                    float* min_depth, float* max_depth, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (!o) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: null argument");
+  const int n = o->median_filter_and_densify_iterations, ld = o->pyramid_level_for_depth, lc = o->pyramid_level_for_color;
+  if (n < 0 || ld < 0 || lc < 0)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: iteration counts and pyramid levels must not be negative");
+  if (n > bba::pre::kMaxMedianIterations)
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: at most 8 median filter and densify iterations are supported");
+  if (ld > bba::pre::kMaxPyramidLevel || lc > bba::pre::kMaxPyramidLevel)
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: pyramid levels above 3 are not supported");
+  if (n > 0 && ld > 0)   // bad_slam.cc:671-673
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: Simultaneous downscaling and median filtering of depth maps is not implemented.");
+  const int w = h->cfg.depth_width, hh = h->cfg.depth_height, cw = h->cfg.color_width, ch = h->cfg.color_height;
+  // Camera::Scaled(2^-L) (camera.h:1696-1704): int(factor * W + 0.5)
+  const auto scaled = [](int size, int level) { return static_cast<int>(static_cast<double>(size) / (1 << level) + 0.5f); };
+  if (raw_depth_width <= 0 || raw_depth_height <= 0 || scaled(raw_depth_width, ld) != w || scaled(raw_depth_height, ld) != hh)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: the depth camera is " + std::to_string(w) + "x" +
+                std::to_string(hh) + ", not the raw depth's " + std::to_string(raw_depth_width) + "x" +
+                std::to_string(raw_depth_height) + " scaled to pyramid level " + std::to_string(ld));
+  if (raw_depth_width > (w << ld) || raw_depth_height > (hh << ld))
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: raw depth sizes above depth camera size x 2^level give boxes "
+                "of more than 2^level pixels per axis, which the median selection does not hold");
+  if (device_rgb && (rgb_width != (cw << lc) || rgb_height != (ch << lc)))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: the rgb image must be the colour camera's size x 2^" +
+                std::to_string(lc) + " (" + std::to_string(cw << lc) + "x" + std::to_string(ch << lc) + ", even at every level), not " +
+                std::to_string(rgb_width) + "x" + std::to_string(rgb_height));
+  const RawStage raw_stage{n, ld, raw_depth_width, raw_depth_height, lc};
+  return PreprocessFrame(h, "bba_preprocess_raw_frame", &o->base, device_raw_depth, raw_depth_pitch, device_rgb, rgb_pitch,
+                         device_depth, depth_pitch, device_normals, normals_pitch, device_radius, radius_pitch, device_color_rgba,
+                         color_pitch, min_depth, max_depth, stream, (n | ld | lc) ? &raw_stage : nullptr);
 }
 
 bba_status bba_update_surfel_activation(bba_handle h, void* stream) {

@@ -45,6 +45,26 @@ __global__ void __launch_bounds__(kThreads) PreprocessFrameKernel(FrameArgs f) {
   }
 }
 
+// The same program behind a stage 0 that builds the raw depth of each tile from a raw frame (median densify filter or median
+// downscaling, DESIGN.md 3.6b) and a colour pyramid level; one instantiation per stage 0 and depth level, the colour level is
+// a uniform branch.
+template <Stage0 kS0, int kLevel>
+__global__ void __launch_bounds__(kThreads) PreprocessRawFrameKernel(FrameArgs f) {
+  extern __shared__ uint16_t smem[];
+  const int depth_tiles = f.tiles_x * f.tiles_y;
+  const int b = static_cast<int>(blockIdx.x);
+  if (b < depth_tiles) {
+    DepthTile<BlockTeam, kS0, kLevel>(f, b % f.tiles_x, b / f.tiles_x, smem, BlockTeam());
+  } else {
+    switch (f.color_level) {
+      case 0: ColorChunk<BlockTeam, 0>(f, b - depth_tiles, BlockTeam()); break;
+      case 1: ColorChunk<BlockTeam, 1>(f, b - depth_tiles, BlockTeam()); break;
+      case 2: ColorChunk<BlockTeam, 2>(f, b - depth_tiles, BlockTeam()); break;
+      default: ColorChunk<BlockTeam, 3>(f, b - depth_tiles, BlockTeam()); break;
+    }
+  }
+}
+
 __global__ void InitMinMaxKernel(float* min_max) {
   min_max[0] = INFINITY;   // cuda_depth_processing.cc:41
   min_max[1] = 0.f;
@@ -58,6 +78,23 @@ int LaunchPreprocessFrame(const pre::FrameArgs& f, cudaStream_t stream) {
   const int blocks = f.tiles_x * f.tiles_y + ((f.rgb && f.rgba) ? pre::ColorChunks(f.cw, f.ch) : 0);
   const size_t smem = sizeof(uint16_t) * static_cast<size_t>(pre::SharedWords(f.radius));
   pre::PreprocessFrameKernel<<<blocks, pre::kThreads, smem, stream>>>(f);
+  return 2;
+}
+
+// The raw-frame variant (the host has validated f: at most one of median_iterations / a downscaled raw size, levels <= 3);
+// returns the number of launches (2).
+int LaunchPreprocessRawFrame(const pre::FrameArgs& f, cudaStream_t stream) {
+  using pre::Stage0;
+  pre::InitMinMaxKernel<<<1, 1, 0, stream>>>(f.min_max);
+  const int blocks = f.tiles_x * f.tiles_y + ((f.rgb && f.rgba) ? pre::ColorChunks(f.cw, f.ch) : 0);
+  const size_t smem = sizeof(uint16_t) * static_cast<size_t>(pre::SharedWordsRaw(f.radius, f.median_iterations));
+  switch (f.median_iterations > 0 ? -1 : f.depth_level) {
+    case -1: pre::PreprocessRawFrameKernel<Stage0::kMedian, 0><<<blocks, pre::kThreads, smem, stream>>>(f); break;
+    case 0: pre::PreprocessRawFrameKernel<Stage0::kCopy, 0><<<blocks, pre::kThreads, smem, stream>>>(f); break;
+    case 1: pre::PreprocessRawFrameKernel<Stage0::kDownscale, 1><<<blocks, pre::kThreads, smem, stream>>>(f); break;
+    case 2: pre::PreprocessRawFrameKernel<Stage0::kDownscale, 2><<<blocks, pre::kThreads, smem, stream>>>(f); break;
+    default: pre::PreprocessRawFrameKernel<Stage0::kDownscale, 3><<<blocks, pre::kThreads, smem, stream>>>(f); break;
+  }
   return 2;
 }
 

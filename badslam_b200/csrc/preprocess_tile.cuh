@@ -10,6 +10,9 @@
 // Here one CTA owns a 32x32 tile of the depth image, stages the raw depth of the tile plus its halo in shared memory once and
 // runs the depth stages back to back on it (A on tile+2, B on tile+1, radius / final depth / min-max on the tile); the raw
 // depth is read from HBM once and the intermediate images never exist in memory.
+// For a raw frame (bba_preprocess_raw_frame) a stage 0 in front of them builds that raw depth from the sensor's image: n
+// passes of the median densify filter on a halo grown by n pixels, or the median downscaling of the full-resolution depth; the
+// colour chunks then read the 2^L x 2^L block of each output pixel and halve it L times in registers (DESIGN.md 3.6b).
 //
 // This header holds the tile program itself, written against a small "team" interface (thread index, thread count, barrier,
 // min/max commit) so that the same code runs as a CUDA block (preprocess.cu) and, one thread at a time, on the host in the
@@ -25,6 +28,11 @@
 #define BBA_PRE_HD __host__ __device__ __forceinline__
 #else
 #define BBA_PRE_HD inline
+#endif
+#if defined(__CUDA_ARCH__)
+#define BBA_PRE_UNROLL _Pragma("unroll")   // register arrays: every index must be a constant
+#else
+#define BBA_PRE_UNROLL
 #endif
 
 namespace bba {
@@ -58,12 +66,29 @@ struct FrameArgs {
   const uint8_t* rgb; uint32_t rgb_pitch;      // uchar3
   uint8_t* rgba; uint32_t rgba_pitch;          // uchar4, .w = luma
   int tiles_x, tiles_y;                        // depth tiles; CTAs behind them convert colour rows
+  // stage 0 of a raw frame (bba_preprocess_raw_frame); all 0 for bba_preprocess_frame
+  int median_iterations;                       // MedianFilterAndDensifyDepthMap passes, 0..kMaxMedianIterations
+  int depth_level;                             // pyramid_level_for_depth: raw_depth (raw_w x raw_h) is downscaled to w x h
+  int raw_w, raw_h;
+  int color_level;                             // pyramid_level_for_color: rgb is (cw << color_level) x (ch << color_level)
 };
+
+// Stage 0: how the raw depth of a tile (the input of the bilateral filter) is produced.
+enum class Stage0 { kCopy, kMedian, kDownscale };
+constexpr int kMaxMedianIterations = 8;        // halo growth: 2 px of shared memory edge per iteration
+constexpr int kMaxPyramidLevel = 3;            // boxes of up to 8 x 8 raw pixels, median selected in registers
 
 BBA_PRE_HD int RawEdge(int radius) { return kTile + 2 * (kHaloA + radius); }
 BBA_PRE_HD int SharedWords(int radius) {   // u16 elements: raw | A | B
   const int e = RawEdge(radius);
   return e * e + (kTile + 4) * (kTile + 4) + (kTile + 2) * (kTile + 2);
+}
+// With n median iterations the raw depth is staged n pixels further out and filtered ping-pong between two buffers, each pass
+// on a region one pixel smaller: S0 (edge + 2n)^2 | S1 (edge + 2n - 2)^2 | A | B.  n = 8, radius 16: 32.5 KB.
+BBA_PRE_HD int SharedWordsRaw(int radius, int median_iterations) {
+  if (median_iterations <= 0) return SharedWords(radius);
+  const int e0 = RawEdge(radius) + 2 * median_iterations;
+  return e0 * e0 + (e0 - 2) * (e0 - 2) + (kTile + 4) * (kTile + 4) + (kTile + 2) * (kTile + 2);
 }
 
 template <typename T>
@@ -230,8 +255,95 @@ BBA_PRE_HD uint8_t Luma(uint8_t r, uint8_t g, uint8_t b) {
   return static_cast<uint8_t>((0.299f * r + 0.587f * g + 0.114f * b) + 0.5f);
 }
 
+// ---- stage 0 of a raw frame: median densify filter / median downscaling (the reference runs both on the host) ----
+
+// a / b rounded to nearest: -use_fast_math would otherwise turn the division into an approximate reciprocal product, and the
+// reference computes these means on the CPU.
+BBA_PRE_HD float DivRn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fdiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+
+constexpr uint32_t kExcluded = 0x10000u;   // a slot without a value: larger than every u16, so it sorts behind the valid ones
+
+// The median of the `count` valid entries of v (the others hold kExcluded) as the reference's sort-based code picks it
+// (preprocessing.cc:66-79, image.h:1036-1047): odd count -> the middle value; even count -> the lower middle value if it is
+// strictly closer to the mean (fp32 sum / count; the sums of at most 64 u16 values are exact) than the upper one, else the
+// upper one.  Counting selection: v[i] is the k-th smallest iff #{v < v[i]} <= k < #{v <= v[i]}; fully unrolled, so v stays
+// in registers.
+template <int N>
+BBA_PRE_HD uint16_t SortedMedian(const uint32_t (&v)[N], int count, float sum) {
+  const int k_lo = (count - 1) >> 1, k_hi = count >> 1;
+  uint32_t lo = 0, hi = 0;
+BBA_PRE_UNROLL
+  for (int i = 0; i < N; ++i) {
+    int less = 0, leq = 0;
+BBA_PRE_UNROLL
+    for (int j = 0; j < N; ++j) {
+      less += v[j] < v[i] ? 1 : 0;
+      leq += v[j] <= v[i] ? 1 : 0;
+    }
+    if (less <= k_lo && k_lo < leq) lo = v[i];
+    if (less <= k_hi && k_hi < leq) hi = v[i];
+  }
+  if (count & 1) return static_cast<uint16_t>(hi);
+  const float mean = DivRn(sum, static_cast<float>(count));
+  return static_cast<uint16_t>(fabsf(static_cast<float>(lo) - mean) < fabsf(static_cast<float>(hi) - mean) ? lo : hi);
+}
+
+// MedianFilterAndDensifyDepthMap (preprocessing.cc:40-85) for one pixel: `src` holds the previous pass with row length `es`,
+// (lx, ly) is the pixel there.  Pixels outside the image hold 0 in every pass, so skipping zeros reproduces the reference's
+// window clamped to the image.  Fewer than 2 non-zero values in the 3x3 window: the pixel keeps its value.
+BBA_PRE_HD uint16_t MedianDensifyPixel(const uint16_t* src, int es, int lx, int ly) {
+  uint32_t v[9];
+  int count = 0;
+  float sum = 0;
+BBA_PRE_UNROLL
+  for (int k = 0; k < 9; ++k) {
+    const uint16_t u = src[(ly + k / 3 - 1) * es + (lx + k % 3 - 1)];
+    v[k] = u ? u : kExcluded;
+    count += u ? 1 : 0;
+    sum += static_cast<float>(u);
+  }
+  if (count < 2) return src[ly * es + lx];
+  return SortedMedian(v, count, sum);
+}
+
+// Image::DownscaleUsingMedianWhileExcluding(0, w, h) (libvis image.h:1003-1053) for the output pixel (x, y): the median of
+// the non-zero raw pixels of its box [W x / w, W (x + 1) / w) x [H y / h, H (y + 1) / h) (u32 arithmetic like the reference),
+// 0 for a box without one.  The host checks W <= w 2^kLevel and H <= h 2^kLevel, so a box spans at most 2^kLevel pixels per axis.
+template <int kLevel>
+BBA_PRE_HD uint16_t DownscaledPixel(const FrameArgs& f, int x, int y) {
+  constexpr int S = 1 << kLevel;
+  const uint32_t W = static_cast<uint32_t>(f.raw_w), H = static_cast<uint32_t>(f.raw_h);
+  const uint32_t w = static_cast<uint32_t>(f.w), h = static_cast<uint32_t>(f.h);
+  const uint32_t sx0 = (W * static_cast<uint32_t>(x)) / w, sx1 = (W * static_cast<uint32_t>(x + 1)) / w;
+  const uint32_t sy0 = (H * static_cast<uint32_t>(y)) / h, sy1 = (H * static_cast<uint32_t>(y + 1)) / h;
+  uint32_t v[S * S];
+  int count = 0;
+  float sum = 0;
+BBA_PRE_UNROLL
+  for (int dy = 0; dy < S; ++dy) {
+    const bool row_in = sy0 + dy < sy1;
+    const uint16_t* row = RowPtr(f.raw_depth, f.raw_pitch, static_cast<int>(row_in ? sy0 + dy : sy0));
+BBA_PRE_UNROLL
+    for (int dx = 0; dx < S; ++dx) {
+      const uint16_t u = (row_in && sx0 + dx < sx1) ? row[sx0 + dx] : static_cast<uint16_t>(0);
+      v[dy * S + dx] = u ? u : kExcluded;
+      count += u ? 1 : 0;
+      sum += static_cast<float>(u);
+    }
+  }
+  if (count == 0) return 0;
+  return SortedMedian(v, count, sum);
+}
+
 // One depth tile.  `Team` provides: int tid(), int size(), void sync(), void commit_min_max(float mn, float mx, float* out).
-template <class Team>
+// kS0 selects stage 0 (kLevel: the depth pyramid level of kDownscale); everything after it is the same for all of them.
+template <class Team, Stage0 kS0 = Stage0::kCopy, int kLevel = 0>
 BBA_PRE_HD void DepthTile(const FrameArgs& f, int tile_x, int tile_y, uint16_t* smem, Team team) {
   const int halo = kHaloA + f.radius;
   const int edge = RawEdge(f.radius);
@@ -241,15 +353,50 @@ BBA_PRE_HD void DepthTile(const FrameArgs& f, int tile_x, int tile_y, uint16_t* 
   const int x0 = tile_x * kTile, y0 = tile_y * kTile;
   const int rx0 = x0 - halo, ry0 = y0 - halo;
 
-  // raw depth of the tile and its halo; 0 (= no measurement) outside the image
-  for (int i = team.tid(); i < edge * edge; i += team.size()) {
-    const int ly = i / edge, lx = i - ly * edge;
-    const int x = rx0 + lx, y = ry0 + ly;
-    uint16_t v = 0;
-    if (x >= 0 && y >= 0 && x < f.w && y < f.h) v = RowPtr(f.raw_depth, f.raw_pitch, y)[x];
-    raw[i] = v;
+  if constexpr (kS0 == Stage0::kMedian) {
+    // raw depth of the tile, its halo and n more pixels; then n passes, pass `it` on the region n - it pixels beyond the halo
+    const int n = f.median_iterations;
+    const int e0 = edge + 2 * n;
+    uint16_t* src = smem;
+    uint16_t* dst = smem + e0 * e0;
+    A = dst + (e0 - 2) * (e0 - 2);
+    B = A + (kTile + 4) * (kTile + 4);
+    for (int i = team.tid(); i < e0 * e0; i += team.size()) {
+      const int ly = i / e0, lx = i - ly * e0;
+      const int x = rx0 - n + lx, y = ry0 - n + ly;
+      uint16_t v = 0;
+      if (x >= 0 && y >= 0 && x < f.w && y < f.h) v = RowPtr(f.raw_depth, f.raw_pitch, y)[x];
+      src[i] = v;
+    }
+    team.sync();
+    for (int it = 1; it <= n; ++it) {
+      const int es = e0 - 2 * (it - 1), ed = es - 2, o = n - it;   // dst origin: (rx0 - o, ry0 - o)
+      for (int i = team.tid(); i < ed * ed; i += team.size()) {
+        const int ly = i / ed, lx = i - ly * ed;
+        const int x = rx0 - o + lx, y = ry0 - o + ly;
+        uint16_t v = 0;                                   // outside the image: stays "no measurement" in every pass
+        if (x >= 0 && y >= 0 && x < f.w && y < f.h) v = MedianDensifyPixel(src, es, lx + 1, ly + 1);
+        dst[i] = v;
+      }
+      team.sync();
+      uint16_t* t = src; src = dst; dst = t;
+    }
+    raw = src;                                           // edge x edge, origin (rx0, ry0)
+  } else {
+    // raw depth of the tile and its halo (downscaled: the box medians of the full-resolution image); 0 (= no measurement)
+    // outside the image
+    for (int i = team.tid(); i < edge * edge; i += team.size()) {
+      const int ly = i / edge, lx = i - ly * edge;
+      const int x = rx0 + lx, y = ry0 + ly;
+      uint16_t v = 0;
+      if (x >= 0 && y >= 0 && x < f.w && y < f.h) {
+        if constexpr (kS0 == Stage0::kDownscale) v = DownscaledPixel<kLevel>(f, x, y);
+        else v = RowPtr(f.raw_depth, f.raw_pitch, y)[x];
+      }
+      raw[i] = v;
+    }
+    team.sync();
   }
-  team.sync();
 
   // A: bilateral filter + depth cut-off on tile +- 2
   constexpr int ea = kTile + 4;
@@ -310,8 +457,27 @@ BBA_PRE_HD void DepthTile(const FrameArgs& f, int tile_x, int tile_y, uint16_t* 
   team.commit_min_max(mn, mx, f.min_max);
 }
 
-// One chunk of colour pixels (rows are split into chunks of kTile * kTile pixels).
-template <class Team>
+struct Rgb8 { uint8_t r, g, b; };
+
+// Pixel (x, y) of level kLevel of the colour pyramid of rgb: ImagePyramid (image_cache.h:205-231) applies
+// Image::DownscaleToHalfSize (libvis image.h:929-948) once per level, a / 4 + b / 4 + c / 4 + d / 4 per channel with
+// truncation -- level by level, which is not one average over the 2^kLevel x 2^kLevel block.
+template <int kLevel>
+BBA_PRE_HD Rgb8 PyramidColor(const FrameArgs& f, int x, int y) {
+  if constexpr (kLevel == 0) {
+    const uint8_t* s = RowPtr(f.rgb, f.rgb_pitch, y) + 3 * x;
+    return Rgb8{s[0], s[1], s[2]};
+  } else {
+    const Rgb8 a = PyramidColor<kLevel - 1>(f, 2 * x, 2 * y), b = PyramidColor<kLevel - 1>(f, 2 * x + 1, 2 * y);
+    const Rgb8 c = PyramidColor<kLevel - 1>(f, 2 * x, 2 * y + 1), d = PyramidColor<kLevel - 1>(f, 2 * x + 1, 2 * y + 1);
+    return Rgb8{static_cast<uint8_t>(a.r / 4 + b.r / 4 + c.r / 4 + d.r / 4),
+                static_cast<uint8_t>(a.g / 4 + b.g / 4 + c.g / 4 + d.g / 4),
+                static_cast<uint8_t>(a.b / 4 + b.b / 4 + c.b / 4 + d.b / 4)};
+  }
+}
+
+// One chunk of colour pixels (rows are split into chunks of kTile * kTile pixels); kLevel: pyramid level of the rgb input.
+template <class Team, int kLevel = 0>
 BBA_PRE_HD void ColorChunk(const FrameArgs& f, int chunk, Team team) {
   const long long total = static_cast<long long>(f.cw) * f.ch;
   const long long begin = static_cast<long long>(chunk) * (kTile * kTile);
@@ -319,8 +485,8 @@ BBA_PRE_HD void ColorChunk(const FrameArgs& f, int chunk, Team team) {
     const long long p = begin + i;
     if (p >= total) break;
     const int y = static_cast<int>(p / f.cw), x = static_cast<int>(p - static_cast<long long>(y) * f.cw);
-    const uint8_t* src = RowPtr(f.rgb, f.rgb_pitch, y) + 3 * x;
-    const uint8_t r = src[0], g = src[1], b = src[2];
+    const Rgb8 src = PyramidColor<kLevel>(f, x, y);
+    const uint8_t r = src.r, g = src.g, b = src.b;
     uint8_t* dst = RowPtr(f.rgba, f.rgba_pitch, y) + 4 * x;
 #if defined(__CUDA_ARCH__)
     *reinterpret_cast<uchar4*>(dst) = make_uchar4(r, g, b, Luma(r, g, b));
@@ -338,7 +504,8 @@ inline int ColorChunks(int cw, int ch) {
 }  // namespace pre
 
 #if defined(__CUDACC__)
-int LaunchPreprocessFrame(const pre::FrameArgs& f, cudaStream_t stream);   // preprocess.cu
+int LaunchPreprocessFrame(const pre::FrameArgs& f, cudaStream_t stream);      // preprocess.cu
+int LaunchPreprocessRawFrame(const pre::FrameArgs& f, cudaStream_t stream);   // preprocess.cu: stage 0 per f's raw-frame fields
 #endif
 
 }  // namespace bba

@@ -236,6 +236,27 @@ class DirectBA {
           "bba_preprocess_frame");
   }
 
+  // ... of the frame as the sensor delivers it, with the rest of BadSlam::PreprocessFrame (bad_slam.cc:649-689) in the same
+  // launch: BadSlamConfig::median_filter_and_densify_iterations, pyramid_level_for_depth (raw_depth is raw_width x raw_height,
+  // the depth camera Camera::Scaled(2^-level) of it) and pyramid_level_for_color (rgb is rgb_width x rgb_height, the colour
+  // camera x 2^level).  The outputs have the cameras' sizes.
+  void PreprocessFrame(cudaStream_t stream, float bilateral_filter_sigma_xy, float bilateral_filter_sigma_inv_depth,
+                       float bilateral_filter_radius_factor, float depth_cutoff, int median_filter_and_densify_iterations,
+                       int pyramid_level_for_depth, int pyramid_level_for_color,
+                       DeviceImage<uint16_t> raw_depth, int raw_width, int raw_height,
+                       DeviceImage<uint8_t> rgb, int rgb_width, int rgb_height,
+                       MutableDeviceImage<uint16_t> depth, MutableDeviceImage<uint16_t> normals,
+                       MutableDeviceImage<uint16_t> radius, MutableDeviceImage<uint8_t> color_rgba,
+                       float* min_depth, float* max_depth) {
+    const bba_raw_frame_options o{{bilateral_filter_sigma_xy, bilateral_filter_sigma_inv_depth, bilateral_filter_radius_factor, depth_cutoff},
+                                  median_filter_and_densify_iterations, pyramid_level_for_depth, pyramid_level_for_color};
+    Check(bba_preprocess_raw_frame(h_, &o, raw_depth.address, raw_depth.pitch_bytes, raw_width, raw_height, rgb.address,
+                                   rgb.pitch_bytes, rgb_width, rgb_height, depth.address, depth.pitch_bytes, normals.address,
+                                   normals.pitch_bytes, radius.address, radius.pitch_bytes, color_rgba.address,
+                                   color_rgba.pitch_bytes, min_depth, max_depth, stream),
+          "bba_preprocess_raw_frame");
+  }
+
   // direct_ba.cc:566-653 (runs inside BundleAdjustment on the reference's schedule; exposed like the reference does)
   void PerformBASchemeEndTasks(cudaStream_t stream, bool do_surfel_updates) {   // direct_ba.h:435-437
     Check(bba_perform_end_tasks(h_, do_surfel_updates ? 1 : 0, nullptr, nullptr, stream), "bba_perform_end_tasks");

@@ -1,4 +1,6 @@
-"""Times the fused keyframe preprocessing (bba_preprocess_frame) against the reference's five kernels on one GPU.
+"""Times the fused keyframe preprocessing (bba_preprocess_frame) against the reference's five kernels on one GPU, and the
+raw-frame stage 0 (bba_preprocess_raw_frame): 640x480 with 1 and 4 median densify iterations, 1280x960 -> 640x480 at depth and
+colour pyramid level 1.
 
     python tools/preprocess_time.py [--size 640x480] [--iters 200]
 
@@ -56,6 +58,28 @@ def main():
     bytes_alg = 15.0 * w * h
     print(f"fused preprocessing {w}x{h}: {us:.1f} us per frame (2 launches, output tensors allocated per call), "
           f"{bytes_alg / us * 1e-3:.1f} GB/s algorithmic")
+    # raw-frame stage 0, same event timing without flush (the same blank 640x480 camera; the 2x frame is the random surface at
+    # twice the resolution)
+    sc6 = S.blank_scene(640, 480)
+    ba6 = DirectBA.from_scene(sc6)
+    raw6, rgb6 = S.random_raw_frame(640, 480, seed=1, hole_fraction=0.3)
+    raw12, rgb12 = S.random_raw_frame(1280, 960, seed=2, hole_fraction=0.3)
+    cases = [("640x480, no stage 0 (bba_preprocess_frame)", raw6, rgb6, {}),
+             ("640x480, median_filter_and_densify_iterations 1", raw6, rgb6, dict(median_filter_and_densify_iterations=1)),
+             ("640x480, median_filter_and_densify_iterations 4", raw6, rgb6, dict(median_filter_and_densify_iterations=4)),
+             ("1280x960 -> 640x480, pyramid_level_for_depth 1 + pyramid_level_for_color 1", raw12, rgb12,
+              dict(pyramid_level_for_depth=1, pyramid_level_for_color=1))]
+    for name, r, c, opts in cases:
+        d_r, d_c = torch.from_numpy(r.view(np.int16)).cuda(), torch.from_numpy(c).cuda()
+        for _ in range(5):
+            ba6.PreprocessFrame(d_r, d_c, want_min_max=False, **opts)
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(a.iters):
+            ba6.PreprocessFrame(d_r, d_c, want_min_max=False, **opts)
+        e1.record()
+        torch.cuda.synchronize()
+        print(f"raw frame {name}: {e0.elapsed_time(e1) / a.iters:.4f} ms per frame")
     try:
         from oracle import ref_cuda as R
         if R.available():

@@ -6,8 +6,10 @@
 
 Every `--keyframe-interval`-th frame becomes a keyframe at its trajectory pose (the reference's odometry front-end is out of
 scope: poses come from the file, perturbed by --pose-noise to give BA something to do): raw depth + colour are uploaded,
-DirectBA.CreateKeyframeFromFrame preprocesses them on the device (bba_preprocess_frame) and adds the keyframe, surfels are
-created for it, and BundleAdjustment runs every --ba-interval keyframes.  Prints one JSON line.
+DirectBA.CreateKeyframeFromFrame preprocesses them on the device (bba_preprocess_frame, or bba_preprocess_raw_frame with
+--median-filter-iterations / --pyramid-level-for-depth / --pyramid-level-for-color: the full-resolution frames are uploaded and
+filtered or downscaled in the same launch, the cameras are the calibration's Scaled(0.5 ** level)) and adds the keyframe,
+surfels are created for it, and BundleAdjustment runs every --ba-interval keyframes.  Prints one JSON line.
 """
 import argparse
 import json
@@ -44,6 +46,10 @@ def main():
     ap.add_argument("--cell-size", type=int, default=4)
     ap.add_argument("--max-surfels", type=int, default=20_000_000)
     ap.add_argument("--pose-noise", type=float, default=0.002, help="metres / radians added to the trajectory poses")
+    ap.add_argument("--median-filter-iterations", type=int, default=0,        # bad_slam_config.h: median_filter_and_densify_iterations
+                    help="median densify filter passes over the raw depth (0..8)")
+    ap.add_argument("--pyramid-level-for-depth", type=int, default=0, help="downscale the depth by 2^level (0..3)")
+    ap.add_argument("--pyramid-level-for-color", type=int, default=0, help="downscale the colour by 2^level (0..3)")
     a = ap.parse_args()
     if a.make_synthetic:
         make_synthetic(a.make_synthetic)
@@ -55,8 +61,12 @@ def main():
     ds = D.TUMRGBDDataset(a.folder, a.trajectory)
     cam = PinholeCamera4f(ds.width, ds.height, ds.camera_parameters)
     idx = list(range(0, len(ds), a.keyframe_interval))[:a.max_keyframes]
-    ba = DirectBA(a.max_surfels, a.raw_to_float_depth, 40.0, a.cell_size, color_camera_initial_estimate=cam,
-                  depth_camera_initial_estimate=cam, max_keyframes=len(idx))
+    # main.cc:457-460: the cameras of the handle are the calibration scaled to the pyramid levels
+    depth_cam, color_cam = cam.Scaled(0.5 ** a.pyramid_level_for_depth), cam.Scaled(0.5 ** a.pyramid_level_for_color)
+    ba = DirectBA(a.max_surfels, a.raw_to_float_depth, 40.0, a.cell_size, color_camera_initial_estimate=color_cam,
+                  depth_camera_initial_estimate=depth_cam, max_keyframes=len(idx))
+    raw_options = dict(median_filter_and_densify_iterations=a.median_filter_iterations,
+                       pyramid_level_for_depth=a.pyramid_level_for_depth, pyramid_level_for_color=a.pyramid_level_for_color)
     surfels = torch.zeros((17, a.max_surfels), dtype=torch.float32, device="cuda")
     ba.SetSurfels(surfels, 0)
     rng = np.random.default_rng(0)
@@ -69,7 +79,7 @@ def main():
         rgb = torch.from_numpy(ds.load_color(i)).cuda()
         torch.cuda.synchronize()
         t = time.perf_counter()
-        kf = ba.CreateKeyframeFromFrame(i, raw, rgb, noisy, max_depth=a.max_depth)
+        kf = ba.CreateKeyframeFromFrame(i, raw, rgb, noisy, max_depth=a.max_depth, **raw_options)
         created += ba.CreateSurfelsForKeyframe(None, True, kf.id)
         torch.cuda.synchronize()
         t_pre += time.perf_counter() - t
@@ -82,7 +92,8 @@ def main():
     poses = ba.GetKeyframeStates()[0]
     rel = lambda P, k: S.se3_mul(S.se3_inverse(P[0]), P[k])
     err = [S.pose_error(rel(poses, k), rel(true_poses, k)) for k in range(1, len(idx))]
-    print(json.dumps({"frames": len(ds), "keyframes": len(idx), "image": [ds.width, ds.height], "surfels_created": created,
+    print(json.dumps({"frames": len(ds), "keyframes": len(idx), "image": [ds.width, ds.height],
+                      "depth_image": [depth_cam.width, depth_cam.height], "surfels_created": created,
                       "surfels": ba.surfels_size(), "ba_calls": results, "seconds_preprocess_and_creation": round(t_pre, 3),
                       "seconds_bundle_adjustment": round(t_ba, 3),
                       "max_relative_pose_error_m_rad": [max(e[0] for e in err), max(e[1] for e in err)] if err else None}))
