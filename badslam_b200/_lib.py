@@ -9,8 +9,7 @@ import ctypes as C
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-# BADBA_LIB: development override for A/B runs of kernel variants (tools/ab_bench.sh); the product is the in-tree library
-LIB_PATH = os.environ.get("BADBA_LIB") or os.path.join(HERE, "libbadba_b200.so")
+LIB_PATH = os.path.join(HERE, "libbadba_b200.so")
 
 ABI_VERSION = 10   # BBA_ABI_VERSION of the include/badba.h this binding types
 

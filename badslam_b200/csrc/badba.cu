@@ -26,10 +26,6 @@
 #include "odometry.cuh"
 #include "preprocess_tile.cuh"
 
-#ifndef BBA_POSE_PRECOMPUTE
-#define BBA_POSE_PRECOMPUTE 1   // per-surfel frames (normal, tangent points) computed once per pose step (kernels.cuh LaunchSurfelFrames)
-#endif
-
 namespace {
 
 using bba::KfDevice;
@@ -134,7 +130,6 @@ struct Keyframe {
   size_t depth_pitch = 0, normals_pitch = 0, radius_pitch = 0;
   cudaArray_t luma = nullptr;   // library-owned u8 CUDA array (the .w channel of the caller's uchar4 colour buffer)
   cudaTextureObject_t tex = 0;
-  bool tex_alias = false;       // development switch BADBA_ALIAS_LUMA (tools/ab_locality.py): tex belongs to keyframe 0
   void* owned[3] = {nullptr, nullptr, nullptr};   // depth / normals / radius copies made by bba_add_keyframe_host
   const uint8_t* rgba = nullptr;   // uchar4 colour image (caller-owned, or owned_rgba): surfel colours at creation
   size_t rgba_pitch = 0;
@@ -460,8 +455,7 @@ bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStre
   acc->queue = h->d_queue;
   acc->frames = nullptr;
   acc->frames_pitch = 0;
-  static const bool precompute = BBA_POSE_PRECOMPUTE && !std::getenv("BADBA_POSE_NO_PRECOMPUTE");   // (development switch for A/B runs)
-  const bool pre = variant == bba::kPoseVariantAuto ? precompute && h->cfg.use_descriptor_residuals && n_work >= 4
+  const bool pre = variant == bba::kPoseVariantAuto ? h->cfg.use_descriptor_residuals && n_work >= 4
                                                     : bba::PoseVariantPre(variant);
   if (pre && h->surfels_size > 0) {
     const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
@@ -731,11 +725,6 @@ bba_status BuildGeometryArgs(bba_handle h, bba::GeometryArgs* g, cudaStream_t s)
   g->kf_count = cnt;
   g->queue = h->d_geo_queue;
   g->tile_shift = 8;
-  // Keyframes per work item.  A group's images (1.5 MB per keyframe at 640x480) are what all resident warps gather from at one
-  // time; between groups a surfel's partial sums are parked in the scratch rows.  16 keeps a group's images in a fifth of the L2
-  // when millions of surfels stream past them; (development switch BADBA_GEO_GROUP for A/B runs)
-  static const int group_override = std::getenv("BADBA_GEO_GROUP") ? std::atoi(std::getenv("BADBA_GEO_GROUP")) : 0;
-  g->group = group_override;
   g->peers = (h->cfg.world_size > 1 && h->peers.count == h->cfg.world_size - 1) ? h->peers : bba::PeerSet{};
   if (!h->d_tile_epoch || h->tile_epoch_capacity < (h->surfels_size + 31u) / 32u) {
     cudaFree(h->d_tile_epoch);
@@ -1613,14 +1602,7 @@ bba::odom::LevelCamera MakeLevelCamera(bba_handle h, int scale, int level_w, int
 bba_status AddKeyframeCommon(bba_handle h, Keyframe&& kf, const uint8_t* device_rgba, size_t color_pitch, const float pose[7],
                              float min_depth, float max_depth, cudaStream_t s, int* out_id) {
   if (static_cast<int>(h->keyframes.size()) >= h->cfg.max_keyframes) return Fail(h, BBA_ERR_STATE, "max_keyframes exceeded");
-  // (development switch for the locality A/B of tools/ab_locality.py: every keyframe samples keyframe 0's luma array)
-  static const bool alias_luma = std::getenv("BADBA_ALIAS_LUMA") != nullptr;
-  if (alias_luma && !h->keyframes.empty()) {
-    kf.tex = h->keyframes[0].tex;
-    kf.tex_alias = true;
-  } else if (bba_status st = MakeLumaTexture(h, device_rgba, color_pitch, &kf.luma, &kf.tex, s)) {
-    return st;
-  }
+  if (bba_status st = MakeLumaTexture(h, device_rgba, color_pitch, &kf.luma, &kf.tex, s)) return st;
   kf.pose = PoseFromArray(pose);
   kf.activation = BBA_KF_ACTIVE;   // keyframe.cc:75
   kf.min_depth = min_depth;
@@ -1740,7 +1722,7 @@ void bba_destroy(bba_handle h) {
   if (!h) return;
   cudaDeviceSynchronize();
   for (Keyframe& kf : h->keyframes) {
-    if (kf.tex && !kf.tex_alias) cudaDestroyTextureObject(kf.tex);
+    if (kf.tex) cudaDestroyTextureObject(kf.tex);
     if (kf.luma) cudaFreeArray(kf.luma);
     for (void* p : kf.owned) cudaFree(p);
     cudaFree(kf.owned_rgba);

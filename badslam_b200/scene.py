@@ -66,7 +66,7 @@ def config_by_name(name: str) -> SceneConfig:
         return SceneConfig(1280, 720, 400, 8_000_000, cell=4, seed=5, name="cfg5")
     if name == "cfg3_rank8":
         # what ONE rank of an 8-GPU cfg3 job sees in the geometry step: every keyframe, an eighth of the surfels (development
-        # workload for tuning the geometry kernels at small shards on a single GPU, tools/ab_fast.py --workload cfg3_rank8)
+        # workload for tuning the geometry kernels at small shards on a single GPU, bench.py --workload cfg3_rank8)
         return SceneConfig(640, 480, 200, 375_000, cell=4, seed=3, name="cfg3_rank8")
     if name == "tiny":
         return SceneConfig(160, 120, 4, 6000, cell=2, seed=7, name="tiny")
