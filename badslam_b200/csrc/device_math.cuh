@@ -75,19 +75,22 @@ __device__ __forceinline__ Vec3 Transform(const float* __restrict__ T, const Vec
 }
 
 // Sums acc[i] over the 32 lanes of the warp for all 32 i at once: after the call lane L holds the total of
-// acc[L].  16+8+4+2+1 = 31 shuffles instead of 32 x 5.
-__device__ __forceinline__ float WarpTransposeReduce(float (&v)[32], int lane) {
+// acc[L].  16+8+4+2+1 = 31 shuffles instead of 32 x 5.  One template level per butterfly stage: written as a loop over the
+// stages, the outer loop is not unrolled and v lives in a 128-byte stack frame.
+template <int HALF>
+__device__ __forceinline__ void WarpTransposeStage(float (&v)[32], int lane) {
+  const bool upper = (lane & HALF) != 0;
 #pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-    const bool upper = (lane & half) != 0;
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float lo = v[i], hi = v[i + half];
-      const float send = upper ? lo : hi;
-      const float keep = upper ? hi : lo;
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-    }
+  for (int i = 0; i < HALF; ++i) {
+    const float lo = v[i], hi = v[i + HALF];
+    const float send = upper ? lo : hi;
+    const float keep = upper ? hi : lo;
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, HALF);
   }
+  if constexpr (HALF > 1) WarpTransposeStage<HALF / 2>(v, lane);
+}
+__device__ __forceinline__ float WarpTransposeReduce(float (&v)[32], int lane) {
+  WarpTransposeStage<16>(v, lane);
   return v[0];
 }
 
