@@ -20,6 +20,7 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler",
 # (applications/badslam/CMakeLists.txt:74-75); the fp64 pose solve and the host code are not.
 UNITS = [
     ("kernels.cu", ["-use_fast_math", "-Xptxas", "-v"]),
+    ("spatial_order.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("intrinsics.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("pcg.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("lifecycle.cu", ["-use_fast_math", "-Xptxas", "-v"]),

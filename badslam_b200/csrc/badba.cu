@@ -172,8 +172,16 @@ struct bba_context {
   // device state sized for cfg.max_keyframes
   KfDevice* d_kfs = nullptr;
   KfDevice* d_work_records = nullptr;   // [max_kf] the pose kernel's work list as contiguous records
-  float* d_frames = nullptr;            // [9][frames_pitch] per-surfel normal + tangent points, rebuilt at the start of a pose step
-  uint32_t frames_pitch = 0;
+  // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream).
+  // The order is rebuilt at the start of every BA call, after an in-loop change of the surfel set, and whenever the surfel count
+  // differs from the one it was built for; in between it may lag behind the positions, which costs culling, never correctness.
+  float* d_pose_stream = nullptr;       // [kPoseStreamRows][stream_pitch], rebuilt at the start of a pose step
+  float* d_chunk_boxes = nullptr;       // [order_capacity / kSpatialChunk][8]
+  uint32_t stream_pitch = 0;
+  bba::SpatialOrderBuffers order{};
+  uint32_t order_capacity = 0;
+  uint32_t order_n = 0;
+  bool order_stale = true;
   float* d_pose_est = nullptr;
   double* d_acc = nullptr;
   unsigned long long* d_stage_counts = nullptr;
@@ -437,11 +445,57 @@ void AssignKeyframes(bba_handle h, const std::vector<int>& ids, std::vector<int>
   BalanceWork(cost.data(), static_cast<int>(ids.size()), h->cfg.world_size, owner->data());
 }
 
+void FreeSpatialOrder(bba_handle h) {
+  cudaFree(h->d_pose_stream);
+  cudaFree(h->d_chunk_boxes);
+  cudaFree(h->order.keys_in);
+  cudaFree(h->order.temp);
+  h->d_pose_stream = nullptr;
+  h->d_chunk_boxes = nullptr;
+  h->order = bba::SpatialOrderBuffers{};
+  h->order_capacity = 0;
+  h->stream_pitch = 0;
+  h->order_stale = true;
+}
+
+// Sizes the pose stream for surfels_size surfels and, with sort, makes the spatial order of the surfels current (see
+// Handle::order_stale).
+bba_status EnsureSpatialOrder(bba_handle h, bool sort, cudaStream_t s) {
+  const uint32_t n = h->surfels_size;
+  if (n > h->order_capacity) {
+    FreeSpatialOrder(h);
+    const uint32_t cap = (n + 511u) / 512u * 512u;   // a multiple of the largest pose tile: 16-byte aligned stream rows
+    const size_t sort_bytes = bba::SpatialOrderTempBytes(cap);
+    uint32_t* words = nullptr;   // keys in / out, index, perm, 8 bound words
+    BBA_CUDA(h, cudaMalloc(&words, sizeof(uint32_t) * (4 * static_cast<size_t>(cap) + 8)));
+    h->order.keys_in = words;
+    h->order.keys_out = words + cap;
+    h->order.index_in = words + 2 * static_cast<size_t>(cap);
+    h->order.perm = words + 3 * static_cast<size_t>(cap);
+    h->order.bounds = words + 4 * static_cast<size_t>(cap);
+    BBA_CUDA(h, cudaMalloc(&h->order.temp, sort_bytes));
+    h->order.temp_bytes = sort_bytes;
+    BBA_CUDA(h, cudaMalloc(&h->d_pose_stream, sizeof(float) * bba::kPoseStreamRows * static_cast<size_t>(cap)));
+    BBA_CUDA(h, cudaMalloc(&h->d_chunk_boxes, sizeof(float) * 8 * static_cast<size_t>(cap / bba::kSpatialChunk)));
+    h->order_capacity = cap;
+    h->stream_pitch = cap;
+  }
+  if (sort && (h->order_stale || h->order_n != n)) {
+    bba::LaunchSpatialOrder(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), n, h->order, s);
+    BBA_CUDA(h, cudaGetLastError());
+    h->launches += 3;   // bounds, keys, the sort (counted as one)
+    h->order_n = n;
+    h->order_stale = false;
+  }
+  return BBA_OK;
+}
+
 // Launch setup of the pose kernel, shared by the pose step and the entry points that evaluate it at a fixed state: arguments
-// over the handle's buffers (the caller sets work_list / work_count) and, for a PRE variant, the per-surfel frames computed on s.
+// over the handle's buffers (the caller sets work_list / work_count) and, for a PRE variant, the pose stream built on s.
 // The surfels do not move during a pose step: what the descriptor residual needs of a surfel alone (unpacked normal, the two
-// tangent points) is computed once here instead of once per (surfel, keyframe, Gauss-Newton iteration) pair.  Not worth a
-// launch + 9 rows of traffic for a handful of keyframes (frame tracking): the kernel then derives them per pair.
+// tangent points) is computed once here instead of once per (surfel, keyframe, Gauss-Newton iteration) pair, and the surfels are
+// put into spatial order with a bounding box per chunk, so that the kernel skips whole chunks outside a keyframe's view.  Not
+// worth a launch + 14 rows of traffic for a handful of keyframes (frame tracking): the kernel then derives the frames per pair.
 // variant = kPoseVariantAuto: that choice, from the number of keyframes n_work; any other: forced (bba_debug_pose_coeffs_batch).
 bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStream_t s, bba::PoseAccumulateArgs* acc) {
   acc->cam = MakeCamera(h);
@@ -453,22 +507,26 @@ bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStre
   acc->acc = h->d_acc;
   acc->stage_counts = h->d_stage_counts;
   acc->queue = h->d_queue;
-  acc->frames = nullptr;
-  acc->frames_pitch = 0;
+  acc->stream = nullptr;
+  acc->stream_pitch = 0;
+  acc->boxes = nullptr;
   const bool pre = variant == bba::kPoseVariantAuto ? h->cfg.use_descriptor_residuals && n_work >= 4
                                                     : bba::PoseVariantPre(variant);
   if (pre && h->surfels_size > 0) {
-    const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
-    if (!h->d_frames || h->frames_pitch < pitch) {
-      cudaFree(h->d_frames);
-      h->d_frames = nullptr;
-      h->frames_pitch = pitch;
-      BBA_CUDA(h, cudaMalloc(&h->d_frames, sizeof(float) * 9 * static_cast<size_t>(pitch)));
-    }
-    bba::LaunchSurfelFrames(h->surfels, pitch, h->surfels_size, h->d_frames, h->frames_pitch, s);
+    // The rebuild (bounds, keys, radix sort) has a fixed cost of ~0.1 ms, most of it launch overhead at the start of a pose step
+    // whose stream has just drained: measured on cfg2 (20 keyframes x 200 k surfels) it cost more than the culling it buys, on
+    // cfg3_rank8 (200 x 375 k) it paid for itself many times over.  Below kSpatialOrderMinPairs (surfel, keyframe) pairs per
+    // launch the stream keeps the caller's order; its chunk boxes are culled all the same.  A forced variant always sorts.
+    constexpr uint64_t kSpatialOrderMinPairs = 16u << 20;
+    const bool sort = variant != bba::kPoseVariantAuto ||
+                      static_cast<uint64_t>(h->surfels_size) * static_cast<uint64_t>(n_work) >= kSpatialOrderMinPairs;
+    if (bba_status st = EnsureSpatialOrder(h, sort, s)) return st;
+    bba::LaunchPoseStream(h->surfels, acc->pitch, h->surfels_size, sort ? h->order.perm : nullptr, h->d_pose_stream,
+                          h->stream_pitch, h->d_chunk_boxes, s);
     ++h->launches;
-    acc->frames = h->d_frames;
-    acc->frames_pitch = h->frames_pitch;
+    acc->stream = h->d_pose_stream;
+    acc->stream_pitch = h->stream_pitch;
+    acc->boxes = h->d_chunk_boxes;
   }
   return BBA_OK;
 }
@@ -1735,7 +1793,7 @@ void bba_destroy(bba_handle h) {
   if (h->luma_staging_free) cudaEventDestroy(h->luma_staging_free);
   cudaFree(h->d_kfs);
   cudaFree(h->d_work_records);
-  cudaFree(h->d_frames);
+  FreeSpatialOrder(h);
   cudaFree(h->d_pose_est);
   cudaFree(h->d_acc);
   cudaFree(h->d_stage_counts);
@@ -1812,6 +1870,7 @@ bba_status bba_set_surfels(bba_handle h, float* device_surfels, size_t pitch_byt
   h->surfels = device_surfels;
   h->surfel_pitch_bytes = pitch_bytes;
   h->surfels_size = surfels_size;
+  h->order_stale = true;
   return BBA_OK;
 }
 
@@ -2647,6 +2706,8 @@ bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_resul
   const uint64_t launches_before = h->launches;
   const auto t_start = std::chrono::steady_clock::now();
 
+  // the caller may have moved the surfels since the last call (through the device view): sort them again at the first pose step
+  h->order_stale = true;
   const int fixed_ba_iteration_count = h->ba_iteration_count;
   if (!o->increase_ba_iteration_count && h->ba_iteration_count != h->last_ba_iteration_count) {   // :313-319
     h->last_ba_iteration_count = h->ba_iteration_count;
@@ -2690,6 +2751,7 @@ bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_resul
         if (bba_status st = CreateSurfelsForKeyframe(h, k, /*filter_new_surfels=*/true, s, &created)) return st;
         res->surfels_created += created;
       }
+      if (!keyframes_with_new_surfels.empty()) h->order_stale = true;
     }
 
     BBA_TRACE("creation done");
@@ -2742,6 +2804,7 @@ bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_resul
       }
       res->surfels_merged += merged;
       if (bba_status st = CompactSurfels(h, merged, /*with_active=*/true, s)) return st;
+      h->order_stale = true;
     }
 
     BBA_TRACE("before pose step");

@@ -290,7 +290,7 @@ __device__ __forceinline__ void TangentProjections(const CameraParams& cam, cons
 
 // The pose-independent half of ComputeTangentProjections (cost_function.cuh:115-133): the two tangent points gp + t1, gp + t2 of
 // a surfel.  Same expressions as TangentProjections above (the pose kernel reads them precomputed per surfel, see
-// SurfelFramesKernel; only Transform + projection depend on the keyframe).
+// PoseStreamKernel; only Transform + projection depend on the keyframe).
 __device__ __forceinline__ void TangentPoints(const Vec3& gp, const Vec3& n, float radius_sq, Vec3* q1, Vec3* q2) {
   Vec3 t1 = Cross(n, (fabsf(n.x) > 0.9f) ? V3(0, 1, 0) : V3(1, 0, 0));
   t1 = (kTangentScaling * sqrtf(radius_sq / fmaxf(1e-12f, Dot(t1, t1)))) * t1;

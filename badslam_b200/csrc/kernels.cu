@@ -131,7 +131,37 @@ constexpr int kPoseThreads = 256;
 constexpr int kPoseUnroll = 1;       // surfels of a chunk evaluated concurrently per lane
 constexpr int kPoseStagedRows = 7;   // x y z normal radius^2 d1 d2
 constexpr int kPoseStagedRowsPre = 14;   // x y z d1 d2 + the 9 frame rows (normal, tangent point 1, tangent point 2)
+static_assert(kPoseStagedRowsPre == kPoseStreamRows, "the PRE instantiations stage every row of the pose stream");
 constexpr int kPoseGroup = 8;        // keyframes per work item
+
+// Does the axis-aligned box {min x y z, -, max x y z, -} lie surely outside the view of the keyframe with frame_T_global T, i.e.
+// would ProjectIntoImage reject every position in it?  The box is culled when its 8 corners all lie beyond one plane: z = 0 or one
+// of the four image borders moved out by a pixel.  Each plane test is f(p) < -e A(p) with f linear in the camera-frame point
+// (e.g. fx x + (cx + 1) z for the left border) and A(p) the same sum over absolute terms (A >= the size of every intermediate in
+// fp32); f + e A is convex, so the test holding at the corners holds everywhere in the box.  With e = 1e-5, some 80 fp32 ulps,
+// it absorbs the rounding of this test and of the kernel's own transform, so that the kernel's fp32 z is <= 0 or its pixel
+// coordinate at least about a pixel beyond the border: culling drops no pair that the kernel would have found in the image.
+// Non-finite boxes compare false and are never culled.  Lane L evaluates corner L & 7; must be called by all 32 lanes.
+__device__ __forceinline__ bool BoxOutsideView(const CameraParams& cam, const float* __restrict__ T, const float* box, int lane) {
+  const int c = lane & 7;
+  const float px = box[(c & 1) ? 4 : 0], py = box[(c & 2) ? 5 : 1], pz = box[(c & 4) ? 6 : 2];
+  float v[3], a[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    v[r] = T[4 * r] * px + T[4 * r + 1] * py + T[4 * r + 2] * pz + T[4 * r + 3];
+    a[r] = fabsf(T[4 * r] * px) + fabsf(T[4 * r + 1] * py) + fabsf(T[4 * r + 2] * pz) + fabsf(T[4 * r + 3]);
+  }
+  constexpr float e = 1e-5f;
+  const float l_x = cam.cx + 1.f, r_x = cam.cx - static_cast<float>(cam.w) - 1.f;
+  const float l_y = cam.cy + 1.f, r_y = cam.cy - static_cast<float>(cam.h) - 1.f;
+  unsigned out = (v[2] < -e * a[2]) ? 1u : 0u;
+  out |= (cam.fx * v[0] + l_x * v[2] < -e * (cam.fx * a[0] + fabsf(l_x) * a[2])) ? 2u : 0u;
+  out |= (cam.fx * v[0] + r_x * v[2] > e * (cam.fx * a[0] + fabsf(r_x) * a[2])) ? 4u : 0u;
+  out |= (cam.fy * v[1] + l_y * v[2] < -e * (cam.fy * a[1] + fabsf(l_y) * a[2])) ? 8u : 0u;
+  out |= (cam.fy * v[1] + r_y * v[2] > e * (cam.fy * a[1] + fabsf(r_y) * a[2])) ? 16u : 0u;
+  if (!(cam.fx > 0.f && cam.fy > 0.f)) out &= 1u;   // the border planes assume a camera that does not mirror the image
+  return __reduce_and_sync(0xffffffffu, out) != 0u;
+}
 
 // Warp-specialised PRE instantiations: two producer warpgroups (association, no accumulators) and one consumer warpgroup (all the
 // per-pair maths after the association, the normal-equation sums and the reductions).  Consumer warp c serves producer warps c and
@@ -217,8 +247,9 @@ __device__ __forceinline__ void AccumulateRecord(const CameraParams& cam, const 
 // evens out the very different cost of culled vs. associated chunks.
 // STATS: also produce the residual costs and the stage counters of the byte model (the reference computes its
 // residual count / cost only in debug mode, kernel_opt_pose.cu:312-320,373-381).
-// PRE: the per-surfel frames (unpacked normal, tangent points) are staged instead of the packed normal and the radius, and the
-// CTA is warp-specialised: the producer warps run the item loop below up to the association and hand each associated pair to
+// PRE: the surfels are read from the pose stream in spatial order (LaunchPoseStream: positions, descriptors and the per-surfel
+// frames -- unpacked normal, tangent points -- instead of the packed normal and the radius), a sub-item whose chunk box lies outside
+// its keyframe's view (BoxOutsideView) is skipped without projecting a surfel, and the CTA is warp-specialised: the producer warps run the item loop below up to the association and hand each associated pair to
 // their consumer warp as a record.  Without PRE every warp accumulates its own pairs (26 of 32 lanes busy on average) and
 // holds the 32 sums in registers throughout.
 // A sub-item's records are packed densely in surfel order into 32-pair batches; lane L of the consumer sums pair L of every
@@ -232,6 +263,7 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
   float* stage_base = reinterpret_cast<float*>(smem_raw);   // [2][kRows][TILE]
   float* rings = stage_base + 2 * kRows * TILE;             // PRE: [producer][slot][kPoseBatchFloats]
   __shared__ __align__(16) KfDevice s_kf[2][kPoseGroup];   // the work group's keyframe records, staged with the tile
+  __shared__ __align__(16) float s_box[2][PRE ? TILE / kSpatialChunk : 1][8];   // PRE: the tile's chunk boxes, staged with it
   __shared__ __align__(8) uint64_t full_bar[2];
   __shared__ unsigned int s_item[2];
   __shared__ int s_sub[2];
@@ -263,17 +295,15 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
     const uint32_t cnt = min(static_cast<uint32_t>(TILE), args.n - base);
     const uint32_t bytes = ((cnt * 4u + 15u) / 16u) * 16u;
     const uint32_t kf_bytes = static_cast<uint32_t>(sizeof(KfDevice)) * min(kPoseGroup, n_work - static_cast<int>(group) * kPoseGroup);
-    MbarArriveExpectTx(&full_bar[s], bytes * kRows + kf_bytes);
+    // PRE: the boxes of the tile's chunks come with it (32 bytes each)
+    const uint32_t box_bytes = PRE ? (cnt + kSpatialChunk - 1) / kSpatialChunk * 8 * sizeof(float) : 0u;
+    MbarArriveExpectTx(&full_bar[s], bytes * kRows + kf_bytes + box_bytes);
     BulkCopyG2S(&s_kf[s][0], args.work_records + static_cast<size_t>(group) * kPoseGroup, kf_bytes, &full_bar[s]);
     if (PRE) {
-      constexpr int kPreRowIds[5] = {kRowX, kRowY, kRowZ, kRowD1, kRowD2};
+      BulkCopyG2S(&s_box[s][0][0], args.boxes + static_cast<size_t>(base / kSpatialChunk) * 8, box_bytes, &full_bar[s]);
 #pragma unroll
-      for (int r = 0; r < 5; ++r)
-        BulkCopyG2S(stage_base + (s * kRows + r) * TILE, args.surfels + static_cast<size_t>(kPreRowIds[r]) * args.pitch + base, bytes,
-                    &full_bar[s]);
-#pragma unroll
-      for (int r = 0; r < 9; ++r)
-        BulkCopyG2S(stage_base + (s * kRows + 5 + r) * TILE, args.frames + static_cast<size_t>(r) * args.frames_pitch + base, bytes,
+      for (int r = 0; r < kPoseStreamRows; ++r)
+        BulkCopyG2S(stage_base + (s * kRows + r) * TILE, args.stream + static_cast<size_t>(r) * args.stream_pitch + base, bytes,
                     &full_bar[s]);
     } else {
 #pragma unroll
@@ -406,6 +436,7 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
       const uint32_t j1 = min(cnt, j0 + chunk_len);
       KfRegs K;
       const int kf = LoadKfShared(&s_kf[s][kf_local], &K);
+      if (PRE && BoxOutsideView(cam, K.T, s_box[s][PRE ? j0 / kSpatialChunk : 0], lane)) continue;   // no pair in the image
       K.tex = UniformTexture(K.tex);
 
       float acc[kPoseAccSize];
@@ -548,7 +579,7 @@ static void LaunchPoseAccumulateS(const PoseAccumulateArgs& args, int sm_count, 
   // CTA (two CTAs per SM), the same footprint as 1024 surfels of the 7-row variant.
   if (variant == kPoseVariantAuto) {
     const uint64_t slots = static_cast<uint64_t>(kPoseMinCtas * sm_count) * 4;
-    if (args.frames != nullptr) variant = args.n >= slots * 512 ? kPoseVariant512Pre : kPoseVariant256Pre;
+    if (args.stream != nullptr) variant = args.n >= slots * 512 ? kPoseVariant512Pre : kPoseVariant256Pre;
     else variant = args.n >= slots * 1024 ? kPoseVariant1024 : args.n >= slots * 512 ? kPoseVariant512 : kPoseVariant256;
   }
   switch (variant) {
@@ -565,26 +596,6 @@ void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool wit
   PackWorkRecordsKernel<<<(max_work * 6 + 127) / 128, 128, 0, stream>>>(args.kfs, args.work_list, args.work_count, args.work_records);
   if (with_stats) LaunchPoseAccumulateS<true>(args, sm_count, variant, stream);
   else LaunchPoseAccumulateS<false>(args, sm_count, variant, stream);
-}
-
-__global__ void __launch_bounds__(256) SurfelFramesKernel(const float* __restrict__ surfels, uint32_t pitch, uint32_t n,
-                                                          float* __restrict__ frames, uint32_t fp) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const size_t P = pitch;
-  const Vec3 gp = V3(surfels[kRowX * P + i], surfels[kRowY * P + i], surfels[kRowZ * P + i]);
-  const Vec3 nrm = UnpackNormal(__float_as_uint(surfels[kRowNormal * P + i]));
-  Vec3 q1, q2;
-  TangentPoints(gp, nrm, surfels[kRowRadiusSq * P + i], &q1, &q2);
-  const size_t F = fp;
-  frames[0 * F + i] = nrm.x; frames[1 * F + i] = nrm.y; frames[2 * F + i] = nrm.z;
-  frames[3 * F + i] = q1.x;  frames[4 * F + i] = q1.y;  frames[5 * F + i] = q1.z;
-  frames[6 * F + i] = q2.x;  frames[7 * F + i] = q2.y;  frames[8 * F + i] = q2.z;
-}
-
-void LaunchSurfelFrames(const float* surfels, uint32_t pitch, uint32_t n, float* frames, uint32_t frames_pitch, cudaStream_t stream) {
-  if (n == 0) return;
-  SurfelFramesKernel<<<(n + 255) / 256, 256, 0, stream>>>(surfels, pitch, n, frames, frames_pitch);
 }
 
 // ------------------------------------------------------------------------------------------------

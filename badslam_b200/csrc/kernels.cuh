@@ -22,9 +22,10 @@ struct PoseAccumulateArgs {
   const KfDevice* kfs;
   const int* work_list;      // keyframe ids to evaluate
   const int* work_count;     // device scalar
-  const float* frames;       // 9 rows x frames_pitch: per-surfel unpacked normal, gp + t1, gp + t2 (SurfelFramesKernel); may be null
-  uint32_t frames_pitch;     // floats per row
-  KfDevice* work_records;    // [max_kf] scratch: the work list's KfDevice records in list order (pad = keyframe id), filled by
+  const float* stream;       // kPoseStreamRows rows x stream_pitch, in spatial order (LaunchPoseStream); may be null
+  uint32_t stream_pitch;     // floats per row
+  const float* boxes;        // [n / kSpatialChunk rounded up][8] bounding box of every stream chunk (LaunchPoseStream)
+  KfDevice* work_records;   // [max_kf] scratch: the work list's KfDevice records in list order (pad = keyframe id), filled by
                              // LaunchPoseAccumulate so that a work group's <= 8 records are ONE contiguous bulk copy
   double* acc;               // [max_kf][32]
   unsigned long long* stage_counts;  // [max_kf][2]
@@ -34,19 +35,39 @@ struct PoseAccumulateArgs {
 // Persistent, TMA-staged pose residual/Jacobian/Hessian kernel (AccumulatePoseEstimationCoeffsCUDAKernel,
 // kernel_opt_pose.cu:251-383, for a whole list of keyframes in one launch).
 // with_stats: also accumulate residual costs + the stage counters (iteration 0 of a pose step, profiling, debug API).
-// Per-surfel, pose-independent inputs of the descriptor residual, computed once per pose step (the surfels do not move while the
-// keyframe poses are optimised): rows 0-2 unpacked + re-normalised normal (util_nvcc_only.cuh:83-95), rows 3-5 / 6-8 the tangent
-// points gp + t1 / gp + t2 (cost_function.cuh:115-133).  frames: [9][frames_pitch] floats.
-void LaunchSurfelFrames(const float* surfels, uint32_t pitch, uint32_t n, float* frames, uint32_t frames_pitch, cudaStream_t stream);
-// Instantiations of the pose kernel (surfel tile, PRE = stages the precomputed frames); the values are bba_pose_variant's.
+// Spatial order of the surfels (spatial_order.cu).  The caller's surfels lie in creation order, raster order of the keyframe that
+// made them: 256 consecutive ones form a band across a whole image.  Sorted by the Morton code of their positions (10 bits per axis
+// inside the map's bounding box) they form compact chunks, most of which lie wholly outside a given keyframe's view.
+// perm[s] = caller index of the surfel at sorted position s.  A stable radix sort: the same positions give the same permutation.
+constexpr int kSpatialChunk = 256;   // surfels per bounding box of the pose stream
+struct SpatialOrderBuffers {
+  uint32_t* keys_in;     // [capacity]
+  uint32_t* keys_out;    // [capacity]
+  uint32_t* index_in;    // [capacity]
+  uint32_t* perm;        // [capacity]
+  unsigned int* bounds;  // [6] order-preserving encodings of the map's min / max
+  void* temp;            // CUB scratch of SpatialOrderTempBytes(capacity) bytes
+  size_t temp_bytes;
+};
+size_t SpatialOrderTempBytes(uint32_t capacity);
+void LaunchSpatialOrder(const float* surfels, uint32_t pitch, uint32_t n, const SpatialOrderBuffers& b, cudaStream_t stream);
+// The pose step's surfel stream, in spatial order: stream row r, column s holds, for surfel perm[s], x y z d1 d2 (rows 0-4), the
+// unpacked + re-normalised normal (rows 5-7, util_nvcc_only.cuh:83-95) and the tangent points gp + t1 / gp + t2 (rows 8-10 / 11-13,
+// cost_function.cuh:115-133).  What the descriptor residual needs of a surfel alone is computed once per pose step (the surfels do
+// not move while the keyframe poses are optimised) and the rows the kernel stages come from one buffer.  boxes[c] = min x y z, 0,
+// max x y z, 0 over the finite positions of stream columns [256 c, 256 c + 256).  perm = null: the caller's order.
+constexpr int kPoseStreamRows = 14;
+void LaunchPoseStream(const float* surfels, uint32_t pitch, uint32_t n, const uint32_t* perm, float* stream, uint32_t stream_pitch,
+                      float* boxes, cudaStream_t cuda_stream);
+// Instantiations of the pose kernel (surfel tile, PRE = stages the sorted stream); the values are bba_pose_variant's.
 enum PoseVariant { kPoseVariantAuto = 0, kPoseVariant256Pre = 1, kPoseVariant512Pre = 2, kPoseVariant256 = 3, kPoseVariant512 = 4,
                    kPoseVariant1024 = 5 };
 inline bool PoseVariantValid(int v) { return v >= kPoseVariantAuto && v <= kPoseVariant1024; }
 inline bool PoseVariantPre(int v) { return v == kPoseVariant256Pre || v == kPoseVariant512Pre; }
 // max_work: upper bound of *work_count known to the host (sizes the record-packing launch that precedes the kernel).
-// variant = kPoseVariantAuto: the tile follows from args.n and the SM count, and args.frames != null selects the variant that
-// stages the precomputed frames instead of the packed normal / radius rows.  Any other variant forces that instantiation; a PRE
-// variant needs args.frames, the others ignore it.
+// variant = kPoseVariantAuto: the tile follows from args.n and the SM count, and args.stream != null selects the variant that
+// stages the sorted stream (and skips the chunks whose box lies outside a keyframe's view) instead of the caller's rows.  Any other
+// variant forces that instantiation; a PRE variant needs args.stream and args.boxes, the others ignore them.
 void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
                           int variant = kPoseVariantAuto);
 

@@ -201,7 +201,8 @@ bba_status bba_accumulate_pose_coeffs(bba_handle h, int keyframe_id, const float
                                       bba_pose_coeffs* out, void* stream);
 /* Parity hook for the pose kernel as the BA pose step runs it: one launch over a work list of `count` distinct keyframes
  * (ids [count], each evaluated at its own global_T_frame [count][7]), in groups of 8, with the record packing and -- for the
- * PRE variants -- the per-surfel frames the pose step computes first.  variant = BBA_POSE_VARIANT_AUTO picks the instantiation
+ * PRE variants -- the surfel stream in spatial order with per-chunk boxes that the pose step builds first (the spatial order
+ * itself is rebuilt when the surfel count changed or new surfels were set since it was built).  variant = BBA_POSE_VARIANT_AUTO picks the instantiation
  * the pose step would (PRE from 4 keyframes with descriptor residuals, the tile from the surfel count and the SM count);
  * any other value forces that (surfel tile, PRE) instantiation.  with_stats = 0 runs the kernel without the residual costs
  * and stage counters, as the pose step does after its first Gauss-Newton iteration.
@@ -212,7 +213,7 @@ bba_status bba_accumulate_pose_coeffs(bba_handle h, int keyframe_id, const float
  * keyframe's accumulator and counters are cleared before the launch and after the read-back.  Synchronises the stream. */
 typedef enum {
   BBA_POSE_VARIANT_AUTO = 0,
-  BBA_POSE_VARIANT_256_PRE = 1,   /* 256-surfel tiles, precomputed per-surfel frames */
+  BBA_POSE_VARIANT_256_PRE = 1,   /* 256-surfel tiles, precomputed per-surfel frames in spatial order, culled chunks */
   BBA_POSE_VARIANT_512_PRE = 2,
   BBA_POSE_VARIANT_256 = 3,       /* 256-surfel tiles, tangent points derived per pair */
   BBA_POSE_VARIANT_512 = 4,
