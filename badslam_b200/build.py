@@ -28,8 +28,12 @@ UNITS = [
     ("odometry.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("pose_solve.cu", []),
     ("badba.cu", []),
+    ("pose_step.cu", []),
+    ("bundle_adjust.cu", []),
+    ("multi_gpu.cu", []),
+    ("frames.cu", []),
 ]
-HEADERS = ["device_math.cuh", "kernels.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", os.path.join("..", "..", "include", "badba.h")]
+HEADERS = ["device_math.cuh", "kernels.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", os.path.join("..", "..", "include", "badba.h")]
 
 
 def _newer(src, dst):

@@ -1,0 +1,1041 @@
+// bundle_adjust.cu -- bundle adjustment in libbadba_b200 (host side): the alternating scheme and the PCG scheme, the geometry and
+// intrinsics steps, the PCG phases, and the surfel lifecycle (creation, merging, compaction, end tasks) with their entry points.
+#include <chrono>
+#include <cmath>
+#include <cstring>
+#include <limits>
+
+#include "handle.hpp"
+
+namespace bba {
+namespace {
+
+// direct_ba.cc:549-564
+void DetermineCovisibleActiveKeyframes(bba_handle h) {
+  for (Keyframe& kf : h->keyframes) {
+    if (kf.activation != BBA_KF_ACTIVE) continue;
+    for (int o : kf.covis) {
+      Keyframe& other = h->keyframes[o];
+      if (other.activation == BBA_KF_INACTIVE) other.activation = BBA_KF_COVISIBLE_ACTIVE;
+    }
+  }
+}
+
+// The per-tile group epochs of the geometry kernels for surfels_size surfels, with room for max_surfel_count when they grow.
+bba_status ReserveTileEpochs(bba_handle h) {
+  const uint32_t need = (h->surfels_size + 31u) / 32u;
+  BBA_CUDA(h, h->geo.d_tile_epoch.Reserve(need, std::max<uint32_t>((h->cfg.max_surfel_count + 31u) / 32u, need) + 1));
+  return BBA_OK;
+}
+
+bba_status BuildGeometryArgs(bba_handle h, bba::GeometryArgs* g, cudaStream_t s) {
+  if (bba_status st = PeerFence(h, s)) return st;
+  const int K = static_cast<int>(h->keyframes.size());
+  int cnt = 0;
+  for (int k = 0; k < K; ++k)
+    if (h->keyframes[k].activation != BBA_KF_INACTIVE) h->geo.h_list[cnt++] = k;
+  if (cnt) BBA_CUDA(h, cudaMemcpyAsync(h->geo.d_list, h->geo.h_list, sizeof(int) * cnt, cudaMemcpyHostToDevice, s));
+  SetSurfelFields(h, g);
+  SetShardFields(h, g);
+  g->active = h->active;
+  g->kfs = h->d_kfs;
+  g->kf_list = h->geo.d_list;
+  g->kf_count = cnt;
+  g->queue = h->geo.d_queue;
+  g->tile_shift = 8;
+  g->peers = (h->cfg.world_size > 1 && h->xchg.peers.count == h->cfg.world_size - 1) ? h->xchg.peers : bba::PeerSet{};
+  if (bba_status st = ReserveTileEpochs(h)) return st;
+  g->tile_epoch = h->geo.d_tile_epoch;
+  return BBA_OK;
+}
+
+// OptimizeIntrinsicsCUDA (kernel_opt_intrinsics.cc:39-281): accumulate over EVERY keyframe, Schur-complement the
+// per-cell cfactors away, solve the 5x5 / 4x4 systems in fp64 on the host, update intrinsics, a and the cfactors.
+bba_status OptimizeIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cudaStream_t s) {
+  const int K = static_cast<int>(h->keyframes.size());
+  if (h->surfels_size == 0 || K == 0) return BBA_OK;   // :56-58
+  const uint32_t P = static_cast<uint32_t>(h->cf_w) * h->cf_h;
+  const size_t intr_floats = 64 + static_cast<size_t>(8) * P + 8;
+  BBA_CUDA(h, h->geo.d_intr.Reserve(intr_floats));
+  BBA_CUDA(h, h->geo.d_intr_sums.Reserve(bba::kIntrinsicsSums));
+  if (!h->geo.d_all_list) {   // (set only once it is filled)
+    DeviceBuffer<int> all;
+    BBA_CUDA(h, all.Reserve(h->cfg.max_keyframes));
+    std::vector<int> iota(h->cfg.max_keyframes);
+    for (int i = 0; i < h->cfg.max_keyframes; ++i) iota[i] = i;
+    BBA_CUDA(h, cudaMemcpy(all, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice));
+    h->geo.d_all_list = std::move(all);
+  }
+  BBA_CUDA(h, h->geo.h_intr_sums.Reserve(bba::kIntrinsicsSums));
+  BBA_CUDA(h, h->geo.h_intr_x1.Reserve(8));
+  if (bba_status st = UploadKeyframes(h, s)) return st;
+  BBA_CUDA(h, cudaMemsetAsync(h->geo.d_intr, 0, sizeof(float) * intr_floats, s));                      // :69-80
+  BBA_CUDA(h, cudaMemsetAsync(h->geo.d_intr_sums, 0, sizeof(double) * bba::kIntrinsicsSums, s));
+  float* cell_B = h->geo.d_intr + 64;
+  float* cell_D = cell_B + static_cast<size_t>(5) * P;
+  float* cell_b2 = cell_D + P;
+  float* cell_obs = cell_b2 + P;
+  float* d_x1 = cell_obs + P;
+
+  bba::IntrinsicsArgs a;
+  SetSurfelFields(h, &a);
+  SetShardFields(h, &a);
+  a.kfs = h->d_kfs;
+  a.kf_list = h->geo.d_all_list;
+  a.kf_count = K;
+  a.queue = h->geo.d_queue;
+  a.sums = h->geo.d_intr_sums;
+  a.cell_B = cell_B;
+  a.cell_D = cell_D;
+  a.cell_b2 = cell_b2;
+  a.cell_obs = cell_obs;
+  a.cell_count = P;
+  bba::LaunchIntrinsicsAccumulate(a, h->sm_count, opt_color, opt_depth, s);   // :84-108, one launch for all keyframes
+  ++h->launches;
+  if (h->cfg.world_size > 1) {
+    // every rank accumulated its surfel shard: one sum all-reduce over [34 global sums | B | D | b2 | obs]
+    bba::LaunchIntrinsicsConvertSums(h->geo.d_intr_sums, h->geo.d_intr, true, s);
+    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->geo.d_intr, 64 + static_cast<size_t>(8) * P, s);
+    bba::LaunchIntrinsicsConvertSums(h->geo.d_intr_sums, h->geo.d_intr, false, s);
+    h->launches += 2;
+  }
+  if (opt_depth) {
+    bba::LaunchIntrinsicsSchur(P, cell_B, cell_D, cell_b2, h->geo.d_intr_sums, s);   // :120-127
+    ++h->launches;
+  }
+  BBA_CUDA(h, cudaGetLastError());
+  BBA_CUDA(h, cudaMemcpyAsync(h->geo.h_intr_sums, h->geo.d_intr_sums, sizeof(double) * bba::kIntrinsicsSums, cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));   // :136
+
+  if (opt_depth) {
+    // the reference keeps A and b1 in fp32 buffers and solves in fp64 (:130-171)
+    double A[15], b1[5], x1[5];
+    for (int i = 0; i < 15; ++i) A[i] = static_cast<double>(static_cast<float>(h->geo.h_intr_sums[i]));
+    for (int i = 0; i < 5; ++i) b1[i] = static_cast<double>(static_cast<float>(h->geo.h_intr_sums[15 + i]));
+    constexpr float kAPriorWeight = 10;   // :153-155
+    A[14] = static_cast<double>(static_cast<float>(A[14]) + kAPriorWeight * kAPriorWeight);
+    b1[4] = static_cast<double>(static_cast<float>(b1[4]) + kAPriorWeight * kAPriorWeight * h->depth_a);
+    bba::SolveLDLT<5>(A, b1, x1);
+    float x1f[5];
+    for (int i = 0; i < 5; ++i) x1f[i] = static_cast<float>(x1[i]);
+    const bba::CameraParams& c = a.cam;   // :183-194
+    const float new_fx = 1.0f / (c.fx_inv - x1f[0]);
+    const float new_fy = 1.0f / (c.fy_inv - x1f[1]);
+    const float new_cx = -(new_fx * (c.cx_inv - x1f[2])) + 0.5f;
+    const float new_cy = -(new_fy * (c.cy_inv - x1f[3])) + 0.5f;
+    for (int i = 0; i < 5; ++i) h->geo.h_intr_x1[i] = x1f[i];
+    BBA_CUDA(h, cudaMemcpyAsync(d_x1, h->geo.h_intr_x1, sizeof(float) * 5, cudaMemcpyHostToDevice, s));   // :196
+    bba::LaunchIntrinsicsCellUpdate(P, cell_obs, cell_B, cell_D, d_x1, h->d_cfactor, s);             // :205-212
+    ++h->launches;
+    BBA_CUDA(h, cudaGetLastError());
+    BBA_CUDA(h, cudaStreamSynchronize(s));   // h_intr_x1 is reused by the next call
+    h->depth_K[0] = new_fx; h->depth_K[1] = new_fy; h->depth_K[2] = new_cx; h->depth_K[3] = new_cy;
+    h->depth_a -= x1f[4];
+  }
+  if (opt_color) {   // :256-280
+    double H[10], b[4], x[4];
+    for (int i = 0; i < 10; ++i) H[i] = static_cast<double>(static_cast<float>(h->geo.h_intr_sums[20 + i]));
+    for (int i = 0; i < 4; ++i) b[i] = static_cast<double>(static_cast<float>(h->geo.h_intr_sums[30 + i]));
+    bba::SolveLDLT<4>(H, b, x);
+    for (int i = 0; i < 4; ++i) h->color_K[i] -= static_cast<float>(x[i]);
+  }
+  return BBA_OK;
+}
+
+// ---- in-loop surfel lifecycle ---------------------------------------------------------------------------------------------
+// direct_ba.h:220-226
+int GetMinObservationCount(bba_handle h) {
+  const size_t K = h->keyframes.size();
+  return (K < 10) ? ((K < 5) ? h->cfg.min_observation_count_while_bootstrapping_1 : h->cfg.min_observation_count_while_bootstrapping_2)
+                  : h->cfg.min_observation_count;
+}
+
+uint32_t SurfelCapacity(bba_handle h) {
+  return std::min<uint32_t>(h->cfg.max_surfel_count, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)));
+}
+
+bba_status MakeLifecycleArgs(bba_handle h, int k, bba::LifecycleArgs* a, cudaStream_t s) {
+  const uint32_t cells = static_cast<uint32_t>(h->cf_w) * h->cf_h;
+  const uint32_t pixels = static_cast<uint32_t>(h->cfg.depth_width) * h->cfg.depth_height;
+  auto& l = h->life;
+  BBA_CUDA(h, l.d_sup.Reserve(3 * static_cast<size_t>(cells)));
+  BBA_CUDA(h, l.d_cell_bits.Reserve(cells));
+  BBA_CUDA(h, l.d_flags.Reserve(pixels));
+  BBA_CUDA(h, l.d_scan_out.Reserve(pixels));
+  BBA_CUDA(h, l.d_scan_sums.Reserve(bba::ScanScratchWords(pixels)));
+  BBA_CUDA(h, l.d_covis.Reserve(h->cfg.max_keyframes));
+  BBA_CUDA(h, l.h_covis.Reserve(h->cfg.max_keyframes));
+  BBA_CUDA(h, l.d_deleted_count.Reserve(1));
+  BBA_CUDA(h, l.h_deleted_count.Reserve(1));
+  const Keyframe& kf = h->keyframes[k];
+  a->cam = MakeCamera(h);
+  bba::ToMatrix3x4(bba::Inverse(kf.pose), a->T);
+  bba::ToMatrix3x4(kf.pose, a->G);
+  a->depth = kf.depth;
+  a->normals = kf.normals;
+  a->radius = kf.radius;
+  a->depth_pitch = static_cast<uint32_t>(kf.depth_pitch);
+  a->normals_pitch = static_cast<uint32_t>(kf.normals_pitch);
+  a->radius_pitch = static_cast<uint32_t>(kf.radius_pitch);
+  a->tex = kf.tex;
+  a->rgba = kf.rgba;
+  a->rgba_pitch = static_cast<uint32_t>(kf.rgba_pitch);
+  a->surfels = h->surfels;
+  a->pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
+  a->n = h->surfels_size;
+  a->sup = h->life.d_sup;
+  a->cell_bits = h->life.d_cell_bits;
+  a->cells = cells;
+  a->flags = h->life.d_flags;
+  a->covis = h->life.d_covis;
+  a->covis_count = 0;
+  a->min_observation_count = GetMinObservationCount(h);
+  const float c = static_cast<float>(h->cfg.sparse_surfel_cell_size);
+  a->cell_merge_dist_squared = c * c * h->cfg.surfel_merge_dist_factor * h->cfg.surfel_merge_dist_factor;   // kernel_supporting_surfels.cc:76-78
+  a->counter = h->life.d_deleted_count;
+  (void)s;
+  return BBA_OK;
+}
+
+// DirectBA::CreateSurfelsForKeyframe (direct_ba.cc:340-405)
+bba_status CreateSurfelsForKeyframe(bba_handle h, int k, bool filter, cudaStream_t s, uint32_t* new_count) {
+  *new_count = 0;
+  const Keyframe& kf = h->keyframes[k];
+  if (!kf.radius || !kf.rgba) return Fail(h, BBA_ERR_STATE, "surfel creation needs the keyframe's radius and colour buffers");
+  BBA_TRACE("create: enter");
+  h->xchg.replicated_pass_pending = true;
+  if (bba_status st = WaitStaging(h)) return st;
+  bba::LifecycleArgs a;
+  if (bba_status st = MakeLifecycleArgs(h, k, &a, s)) return st;
+  BBA_TRACE("create: args made");
+  if (filter) {   // covis_T_frame for every co-visible keyframe (direct_ba.cc:365-370)
+    int cnt = 0;
+    for (int c : kf.covis) {
+      const Keyframe& other = h->keyframes[c];
+      bba::CovisEntry& e = h->life.h_covis[cnt++];
+      bba::ToMatrix3x4(bba::Compose(bba::Inverse(other.pose), kf.pose), e.R);
+      e.depth = other.depth;
+      e.normals = other.normals;
+      e.depth_pitch = static_cast<uint32_t>(other.depth_pitch);
+      e.normals_pitch = static_cast<uint32_t>(other.normals_pitch);
+      e.pad[0] = e.pad[1] = 0;
+    }
+    a.covis_count = cnt;
+    if (cnt) BBA_CUDA(h, cudaMemcpyAsync(h->life.d_covis, h->life.h_covis, sizeof(bba::CovisEntry) * cnt, cudaMemcpyHostToDevice, s));
+  }
+  BBA_TRACE("create: covis uploaded");
+  const uint32_t pixels = static_cast<uint32_t>(h->cfg.depth_width) * h->cfg.depth_height;
+  bba::LaunchSupportSurfels(a, h->sm_count, s);     // DetermineSupportingSurfelsCUDA: is the cell supported at all
+  bba::LaunchSeedNewSurfels(a, filter, s);
+  bba::LaunchExclusiveScan(h->life.d_flags, pixels, h->life.d_scan_out, h->life.d_scan_sums, s);
+  h->launches += 6 + (filter ? 1 : 0);
+  BBA_CUDA(h, cudaGetLastError());
+  const uint32_t n_blocks = (pixels + 4095) / 4096;
+  BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_scan_sums + n_blocks, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_create_surfels.cu:466-474
+  h->staging.pending = false;
+  const uint32_t created = *h->life.h_deleted_count;
+  BBA_TRACE("create: counted");
+  if (created == 0) return BBA_OK;
+  if (h->surfels_size + static_cast<uint64_t>(created) > SurfelCapacity(h)) {
+    // the reference logs "Maximum surfel count exceeded" and creates nothing (kernel_create_surfels.cc:163-166)
+    h->error = "maximum surfel count exceeded: no surfels created for this keyframe";
+    return BBA_OK;
+  }
+  bba::LaunchCreateSurfels(a, h->life.d_scan_out, s);
+  ++h->launches;
+  BBA_CUDA(h, cudaGetLastError());
+  BBA_TRACE("create: appended");
+  h->surfels_size += created;
+  *new_count = created;
+  return MarkStaging(h, s);
+}
+
+// DetermineSupportingSurfelsAndMergeSurfelsCUDA (kernel_supporting_surfels.cc:40-118); deleted surfels are only marked
+bba_status MergeSurfelsForKeyframe(bba_handle h, int k, cudaStream_t s, uint32_t* deleted) {
+  *deleted = 0;
+  if (h->surfels_size == 0) return BBA_OK;
+  h->xchg.replicated_pass_pending = true;
+  bba::LifecycleArgs a;
+  if (bba_status st = MakeLifecycleArgs(h, k, &a, s)) return st;
+  BBA_CUDA(h, cudaMemsetAsync(h->life.d_deleted_count, 0, sizeof(unsigned int), s));
+  bba::LaunchMergeSurfels(a, h->sm_count, s);
+  h->launches += 5;
+  BBA_CUDA(h, cudaGetLastError());
+  BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_supporting_surfels.cc:93-96
+  *deleted = *h->life.h_deleted_count;
+  return BBA_OK;
+}
+
+bba_status CompactSurfels(bba_handle h, uint32_t free_count, bool with_active, cudaStream_t s) {
+  const uint32_t N = h->surfels_size;
+  if (free_count == 0 || N == 0) return BBA_OK;
+  h->xchg.replicated_pass_pending = true;
+  BBA_CUDA(h, h->life.d_compact_sums.Reserve(bba::CompactScratchWords(N),
+                                              bba::CompactScratchWords(std::max(h->cfg.max_surfel_count, N))));
+  bba::LaunchCompactSurfels(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N, free_count, h->life.d_compact_sums,
+                            with_active ? h->active : nullptr, s);
+  h->launches += 4;
+  BBA_CUDA(h, cudaGetLastError());
+  h->surfels_size = N - free_count;
+  return BBA_OK;
+}
+
+// DirectBA::PerformBASchemeEndTasks (direct_ba.cc:566-653) without the final merge (do_surfel_updates is not supported yet):
+// DeleteSurfelsAndUpdateRadiiCUDA over every keyframe, then CompactSurfelsCUDA.  Replicated on every rank of a multi-GPU
+// job (once per BA call, deterministic, identical inputs -> identical surfel buffers without an exchange).
+bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, bool do_surfel_updates = false) {
+  if (deleted_out) *deleted_out = 0;
+  const int K = static_cast<int>(h->keyframes.size());
+  const uint32_t N = h->surfels_size;
+  if (N == 0) return BBA_OK;   // kernel_delete_surfels.cc:52-54
+  h->xchg.replicated_pass_pending = true;
+  BBA_CUDA(h, h->life.d_kf_radius.Reserve(h->cfg.max_keyframes));
+  BBA_CUDA(h, h->life.h_kf_radius.Reserve(h->cfg.max_keyframes));
+  BBA_CUDA(h, h->life.d_deleted_count.Reserve(1));
+  BBA_CUDA(h, h->life.h_deleted_count.Reserve(1));
+  BBA_TRACE("end tasks");
+  // merge similar surfels using all keyframes which were active in this BA iteration block (direct_ba.cc:577-601)
+  uint32_t merged = 0;
+  if (do_surfel_updates) {
+    for (int k = 0; k < K; ++k) {
+      if (h->keyframes[k].last_active_in_ba_iteration != h->ba_iteration_count) continue;
+      uint32_t d = 0;
+      if (bba_status st = MergeSurfelsForKeyframe(h, k, s, &d)) return st;
+      merged += d;
+    }
+  }
+  if (bba_status st = UploadKeyframes(h, s)) return st;   // (waits for the previous use of the staging buffers)
+  for (int k = 0; k < K; ++k) {
+    if (!h->keyframes[k].radius) return Fail(h, BBA_ERR_STATE, "end tasks need the keyframes' radius buffers");
+    h->life.h_kf_radius[k].ptr = h->keyframes[k].radius;
+    h->life.h_kf_radius[k].pitch = static_cast<uint32_t>(h->keyframes[k].radius_pitch);
+    h->life.h_kf_radius[k].pad = 0;
+  }
+  if (K) BBA_CUDA(h, cudaMemcpyAsync(h->life.d_kf_radius, h->life.h_kf_radius, sizeof(bba::KfRadius) * K, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->life.d_deleted_count, 0, sizeof(unsigned int), s));
+  if (bba_status st = ReserveTileEpochs(h)) return st;
+  bba::SurfelStatsArgs a;
+  SetSurfelFields(h, &a);
+  a.kfs = h->d_kfs;
+  a.radius = h->life.d_kf_radius;
+  a.kf_count = K;
+  a.min_observation_count = GetMinObservationCount(h);
+  a.queue = h->geo.d_queue;
+  a.tile_epoch = h->geo.d_tile_epoch;
+  a.tile_shift = 8;
+  a.deleted_count = h->life.d_deleted_count;
+  // Multi-GPU: every rank evaluates the surfels of its granule shard (the launch is as expensive as a geometry pass over every
+  // keyframe); the two result rows reach the other replicas through peer stores or one all-gather, the deleted counts through a
+  // sum all-reduce (which is also the barrier behind the peer stores).  The compaction then runs replicated on identical replicas.
+  const int world = h->cfg.world_size, rank = h->cfg.rank;
+  const bool peers_mapped = world > 1 && h->xchg.peers.count == world - 1;
+  a.shard_rank = static_cast<uint32_t>(rank);
+  a.shard_world = static_cast<uint32_t>(world);
+  ShardSurfels(N, rank, world, &a.local_count, nullptr);
+  a.peers = peers_mapped ? h->xchg.peers : bba::PeerSet{};
+  if (world > 1) {
+    if (bba_status st = CheckCollective(h)) return st;
+    if (bba_status st = PeerFence(h, s)) return st;   // (e.g. the merges above rewrote whole replicas)
+  }
+  if (K > 0) {
+    bba::LaunchObservationStats(a, h->sm_count, s);
+    ++h->launches;
+    BBA_CUDA(h, cudaGetLastError());
+  }
+  // (with no keyframe at all the reference still runs MarkDeletedSurfels on zero counts; not reachable through this API,
+  // a BA call without keyframes has nothing to optimise)
+  uint32_t deleted_total = 0;
+  if (world > 1) {
+    if (!peers_mapped && K > 0) {
+      uint32_t shard_len;
+      ShardSurfels(N, rank, world, nullptr, &shard_len);
+      if (bba_status st = ReserveExchange(h, static_cast<size_t>(world) * 2 * shard_len)) return st;
+      const size_t slice_floats = static_cast<size_t>(2) * shard_len;
+      bba::LaunchPackStatsShard(h->surfels, a.pitch, N, rank, world, shard_len, h->xchg.d_exchange + slice_floats * rank, s);
+      h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLGATHER, h->xchg.d_exchange, slice_floats * sizeof(float), s);
+      bba::LaunchUnpackStatsShards(h->surfels, a.pitch, N, shard_len, world, rank, h->xchg.d_exchange, s);
+      h->launches += 2;
+    }
+    // deleted count of this shard as two exactly representable floats (low 12 bits, the rest), summed over the ranks
+    BBA_CUDA(h, h->xchg.d_count_xchg.Reserve(2));
+    BBA_CUDA(h, h->xchg.h_count_xchg.Reserve(2));
+    BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaStreamSynchronize(s));
+    h->xchg.h_count_xchg[0] = static_cast<float>(*h->life.h_deleted_count & 0xfffu);
+    h->xchg.h_count_xchg[1] = static_cast<float>(*h->life.h_deleted_count >> 12);
+    BBA_CUDA(h, cudaMemcpyAsync(h->xchg.d_count_xchg, h->xchg.h_count_xchg, sizeof(float) * 2, cudaMemcpyHostToDevice, s));
+    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->xchg.d_count_xchg, 2, s);
+    BBA_CUDA(h, cudaMemcpyAsync(h->xchg.h_count_xchg, h->xchg.d_count_xchg, sizeof(float) * 2, cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaStreamSynchronize(s));
+    deleted_total = static_cast<uint32_t>(h->xchg.h_count_xchg[0] + 0.5f) + (static_cast<uint32_t>(h->xchg.h_count_xchg[1] + 0.5f) << 12);
+    h->xchg.replicated_pass_pending = true;   // the compaction below rewrites every replica as a whole
+  } else {
+    BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_delete_surfels.cc:93-96
+    deleted_total = *h->life.h_deleted_count;
+  }
+  h->staging.pending = false;
+  BBA_TRACE("stats done");
+  const uint32_t deleted = deleted_total + merged;
+  if (deleted_out) *deleted_out = deleted;
+  // kernel_compact_surfels.cu:167-169; direct_ba.cc:618: no active flags
+  return CompactSurfels(h, deleted, /*with_active=*/false, s);
+}
+
+// Merges the new surfels of `keyframes` into the map and compacts it (direct_ba_alternating.cc:489-541, direct_ba_pcg.cc:644-690,
+// 775-815); *merged: the number of surfels the merges deleted.
+bba_status MergeAndCompact(bba_handle h, const std::vector<int>& keyframes, cudaStream_t s, uint32_t* merged) {
+  *merged = 0;
+  for (int k : keyframes) {
+    uint32_t d = 0;
+    if (bba_status st = MergeSurfelsForKeyframe(h, k, s, &d)) return st;
+    *merged += d;
+  }
+  return CompactSurfels(h, *merged, /*with_active=*/true, s);
+}
+
+// Start of a BA call (direct_ba_alternating.cc:313-319, direct_ba_pcg.cc:157-161): the end tasks that the previous call left
+// for this one when it did not advance the BA iteration count.
+bba_status BeginBundleAdjust(bba_handle h, const bba_ba_options* o, bba_ba_result* res, cudaStream_t s) {
+  if (!o->increase_ba_iteration_count && h->ba_iteration_count != h->last_ba_iteration_count) {
+    h->last_ba_iteration_count = h->ba_iteration_count;
+    uint32_t deleted = 0;
+    if (bba_status st = PerformEndTasks(h, s, &deleted, o->do_surfel_updates != 0)) return st;
+    res->surfels_deleted += deleted;
+  }
+  return BBA_OK;
+}
+
+// End of a BA call (direct_ba_alternating.cc:725-735, direct_ba_pcg.cc:771-776): the end tasks when the call advances the BA
+// iteration count, then the map size and the launches of the call in the result.
+bba_status EndBundleAdjust(bba_handle h, const bba_ba_options* o, uint64_t launches_before, bba_ba_result* res, cudaStream_t s) {
+  if (o->increase_ba_iteration_count) {
+    uint32_t deleted = 0;
+    if (bba_status st = PerformEndTasks(h, s, &deleted, o->do_surfel_updates != 0)) return st;
+    res->surfels_deleted += deleted;
+    ++h->ba_iteration_count;
+  }
+  res->surfels_size = h->surfels_size;
+  res->kernel_launches = h->launches - launches_before;
+  return BBA_OK;
+}
+
+// Unknown layout of the PCG solver (direct_ba_pcg.cc:273-309) + the vectors sized for it.
+struct PcgLayout {
+  bool opt_poses, opt_geometry, opt_depth_intr, opt_color_intr, use_desc;
+  uint32_t surfel_start, stride, depth_start, a_index, color_start, unknown_count;
+};
+
+bba_status MakePcgLayout(bba_handle h, const bba_ba_options* o, PcgLayout* L) {
+  constexpr uint32_t kInvalid = 0xffffffffu;
+  const int K = static_cast<int>(h->keyframes.size());
+  const uint32_t N = h->surfels_size, P = static_cast<uint32_t>(h->cf_w) * h->cf_h;
+  L->opt_depth_intr = o->optimize_depth_intrinsics && h->cfg.use_depth_residuals;   // direct_ba.cc:427-434
+  L->opt_color_intr = o->optimize_color_intrinsics && h->cfg.use_descriptor_residuals;
+  L->opt_poses = o->optimize_poses != 0;
+  L->opt_geometry = o->optimize_geometry != 0;
+  L->use_desc = h->cfg.use_descriptor_residuals != 0;
+  L->stride = L->use_desc ? 3u : 1u;
+  uint32_t cur = 0;
+  if (L->opt_poses) cur += 6u * static_cast<uint32_t>(K - 1);
+  L->surfel_start = L->depth_start = L->a_index = L->color_start = kInvalid;
+  if (L->opt_geometry) { L->surfel_start = cur; cur += L->stride * N; }
+  if (L->opt_depth_intr) { L->depth_start = cur; cur += 5u + P; L->a_index = L->depth_start + 4u; }
+  if (L->opt_color_intr) { L->color_start = cur; cur += 4u; }
+  L->unknown_count = cur;
+  if (!h->pcg.d_scalars) {   // scalars + the ordered-sum workspace, zeroed once (set only once it is zeroed)
+    DeviceBuffer<double> scalars;
+    BBA_CUDA(h, scalars.Reserve(bba::kPcgScalarDoubles));
+    BBA_CUDA(h, cudaMemset(scalars, 0, sizeof(double) * bba::kPcgScalarDoubles));
+    h->pcg.d_scalars = std::move(scalars);
+  }
+  BBA_CUDA(h, h->pcg.h_scalars.Reserve(4));
+  BBA_CUDA(h, h->pcg.h_delta.Reserve(6 * static_cast<size_t>(h->cfg.max_keyframes) + 16));
+  const size_t cap = std::max<size_t>(L->unknown_count, 6 * static_cast<size_t>(h->cfg.max_keyframes) +
+                                                            3 * static_cast<size_t>(std::max(h->cfg.max_surfel_count, N)) + 9 + P);
+  for (auto& v : h->pcg.d_vec)   // (+ 8: the alpha_d pair that travels with g, multi-GPU)
+    BBA_CUDA(h, v.Reserve(static_cast<size_t>(L->unknown_count) + 8, cap + 8));
+  return BBA_OK;
+}
+
+bba::PcgArgs MakePcgArgs(bba_handle h, const PcgLayout& L, int gauge) {
+  bba::PcgArgs a;
+  SetSurfelFields(h, &a);
+  SetShardFields(h, &a);   // this rank's surfels (all of them on one GPU)
+  a.alpha_d_slot = h->cfg.world_size > 1 ? 3 : 1;
+  a.kfs = h->d_kfs;
+  a.kf_count = static_cast<int>(h->keyframes.size());
+  a.gauge_kf = gauge;
+  a.opt_poses = L.opt_poses;
+  a.opt_geometry = L.opt_geometry;
+  a.opt_depth_intr = L.opt_depth_intr;
+  a.opt_color_intr = L.opt_color_intr;
+  a.surfel_start = L.surfel_start;
+  a.surfel_stride = L.stride;
+  a.depth_intr_start = L.depth_start;
+  a.color_intr_start = L.color_start;
+  a.r = h->pcg.d_vec[0];
+  a.M = h->pcg.d_vec[1];
+  a.p = h->pcg.d_vec[4];
+  a.g = h->pcg.d_vec[3];
+  a.scalars = h->pcg.d_scalars;
+  a.queue = h->geo.d_queue;
+  return a;
+}
+
+// The PCG solver's phases, shared by BundleAdjustPCG and the parity hook bba_pcg_debug.  Vectors: d_pcg = {r, M, delta, g, p};
+// scalars = {alpha_n or beta_n (slot an), alpha_d (1), beta_n or alpha_n (slot bn), this rank's alpha_d (3, multi-GPU)}.
+// Init: r = -J^T W F and M = diag(J^T W J) over every keyframe (:312-361), then PCGInit2 (:363-373) into slot `an`.
+bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int an, cudaStream_t s) {
+  const uint32_t U = L.unknown_count;
+  BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_vec[0], 0, sizeof(float) * U, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_vec[1], 0, sizeof(float) * U, s));
+  BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars, 0, sizeof(double) * 4, s));
+  bba::LaunchPcgAccumulate(a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
+  if (h->cfg.world_size > 1) {
+    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[0], U, s);
+    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[1], U, s);
+    h->xchg.replicated_pass_pending = false;
+  }
+  bba::LaunchPcgInit2(U, L.a_index, h->depth_a, a.kf_count, h->pcg.d_vec[0], h->pcg.d_vec[1], h->pcg.d_vec[2], h->pcg.d_vec[3], h->pcg.d_vec[4],
+                      h->pcg.d_scalars, an, h->sm_count, s);
+  h->launches += 2;
+  return BBA_OK;
+}
+
+// Inner step, first half: g += J^T W J p and alpha_d += p^T J^T W J p over every keyframe (PCGStep1CUDA, :392-419).
+bba_status PcgStep1(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, cudaStream_t s) {
+  bba::LaunchPcgAccumulate(a, h->sm_count, false, s);
+  if (h->cfg.world_size > 1) {   // g and this rank's part of alpha_d: one all-reduce
+    float* g = h->pcg.d_vec[3];
+    bba::LaunchPcgPackAlphaD(h->pcg.d_scalars, g + L.unknown_count, s);
+    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, g, static_cast<size_t>(L.unknown_count) + 2, s);
+    bba::LaunchPcgUnpackAlphaD(h->pcg.d_scalars, g + L.unknown_count, s);
+    h->launches += 2;
+  }
+  return BBA_OK;
+}
+
+// Inner step, second half: delta += alpha p, r -= alpha A p, z = M^-1 r (into g), beta_n = z^T r into slot `bn` (:421-437).
+bba_status PcgStep2(bba_handle h, const PcgLayout& L, int an, int bn, cudaStream_t s) {
+  BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars + bn, 0, sizeof(double), s));
+  bba::LaunchPcgStep2(L.unknown_count, L.a_index, h->pcg.d_vec[0], h->pcg.d_vec[1], h->pcg.d_vec[2], h->pcg.d_vec[3], h->pcg.d_vec[4], h->pcg.d_scalars,
+                      an, bn, h->sm_count, s);
+  h->launches += 2;
+  BBA_CUDA(h, cudaGetLastError());
+  return BBA_OK;
+}
+
+// Before the next inner step: p = z + beta p, g = 0, alpha_d re-armed with its lambda / prior term (:456-464).
+bba_status PcgStep3(bba_handle h, const PcgLayout& L, int an, int bn, cudaStream_t s) {
+  BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars + 1, 0, sizeof(double), s));
+  bba::LaunchPcgStep3(L.unknown_count, L.a_index, static_cast<int>(h->keyframes.size()), h->pcg.d_vec[3], h->pcg.d_vec[4], h->pcg.d_scalars,
+                      an, bn, h->sm_count, s);
+  ++h->launches;
+  return BBA_OK;
+}
+
+// Applies pcg_delta (:552-638): surfels, cfactors, poses (all but the gauge keyframe), intrinsics.  *num_converged counts the
+// keyframes whose pose update is below the convergence threshold (the gauge keyframe included).
+bba_status PcgApplyDelta(bba_handle h, const PcgLayout& L, int gauge, cudaStream_t s, int* num_converged) {
+  const int K = static_cast<int>(h->keyframes.size());
+  const uint32_t N = h->surfels_size, P = static_cast<uint32_t>(h->cf_w) * h->cf_h;
+  const float* pcg_delta = h->pcg.d_vec[2];
+  size_t n_host = 0;
+  const size_t pose_floats = L.opt_poses ? 6 * static_cast<size_t>(K - 1) : 0;
+  if (pose_floats) BBA_CUDA(h, cudaMemcpyAsync(h->pcg.h_delta, pcg_delta, sizeof(float) * pose_floats, cudaMemcpyDeviceToHost, s));
+  n_host = pose_floats;
+  float* h_di = h->pcg.h_delta + n_host;
+  if (L.opt_depth_intr) {
+    BBA_CUDA(h, cudaMemcpyAsync(h_di, pcg_delta + L.depth_start, sizeof(float) * 5, cudaMemcpyDeviceToHost, s));
+    n_host += 5;
+  }
+  float* h_ci = h->pcg.h_delta + n_host;
+  if (L.opt_color_intr) BBA_CUDA(h, cudaMemcpyAsync(h_ci, pcg_delta + L.color_start, sizeof(float) * 4, cudaMemcpyDeviceToHost, s));
+  if (L.opt_geometry && N > 0) {
+    bba::LaunchPcgUpdateSurfels(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N, L.use_desc, L.surfel_start,
+                                pcg_delta, s);
+    ++h->launches;
+    h->xchg.replicated_pass_pending = true;   // every rank rewrites its whole replica (PeerFence)
+  }
+  if (L.opt_depth_intr) {
+    bba::LaunchPcgUpdateCfactor(h->d_cfactor, P, pcg_delta + L.depth_start + 5, s);
+    ++h->launches;
+  }
+  BBA_CUDA(h, cudaGetLastError());
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  if (L.opt_poses) {
+    for (int k = 0; k < K; ++k) {
+      if (k == gauge) {
+        ++*num_converged;
+        continue;
+      }
+      const float* d6 = h->pcg.h_delta + 6 * static_cast<size_t>(k < gauge ? k : k - 1);
+      const Pose delta = bba::Exp(d6);
+      h->keyframes[k].pose = bba::Compose(h->keyframes[k].pose, delta);   // :569-570
+      float lg[6];
+      bba::Log(delta, lg);
+      if (bba::IsScale1PoseEstimationConverged(lg)) ++*num_converged;
+    }
+  }
+  if (L.opt_depth_intr) {   // :590-612
+    const double old_fx_inv = 1. / h->depth_K[0], old_fy_inv = 1. / h->depth_K[1];
+    const double old_cx_inv = -(h->depth_K[2] - 0.5) * old_fx_inv, old_cy_inv = -(h->depth_K[3] - 0.5) * old_fy_inv;
+    const double new_fx = 1. / (old_fx_inv + h_di[0]);
+    const double new_fy = 1. / (old_fy_inv + h_di[1]);
+    const double new_cx = -(new_fx * (old_cx_inv + h_di[2])) + 0.5;
+    const double new_cy = -(new_fy * (old_cy_inv + h_di[3])) + 0.5;
+    h->depth_K[0] = static_cast<float>(new_fx);
+    h->depth_K[1] = static_cast<float>(new_fy);
+    h->depth_K[2] = static_cast<float>(new_cx);
+    h->depth_K[3] = static_cast<float>(new_cy);
+    h->depth_a += h_di[4];
+  }
+  if (L.opt_color_intr)   // :623-638
+    for (int c = 0; c < 4; ++c) h->color_K[c] = static_cast<float>(h->color_K[c] + h_ci[c]);
+  return BBA_OK;
+}
+
+// DirectBA::BundleAdjustmentPCG (direct_ba_pcg.cc:43-819) without the surfel lifecycle branches.
+bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result* res, cudaStream_t s) {
+  const int K = static_cast<int>(h->keyframes.size());
+  // Multi-GPU: the matrix-free products J^T W F / diag(J^T W J) / J^T W J p are summed over THIS rank's surfels (granule
+  // sharding of the geometry step); one sum all-reduce of the vector per product makes every rank hold the full result (a
+  // surfel's entries are non-zero on its owner only, pose / intrinsics entries are true sums), and the vector kernels, the
+  // scalars and the updates then run replicated and bit-identically on every rank (fixed-order sums, pcg.cu GridOrderedAdd).
+  const int world = h->cfg.world_size;
+  if (bba_status st = CheckCollective(h)) return st;
+  if (world > 1 && o->pcg_gauge_keyframe < 0)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "use_pcg with more than one rank needs pcg_gauge_keyframe >= 0 (the reference draws rand() % K)");
+  if (K == 0) return Fail(h, BBA_ERR_STATE, "use_pcg: no keyframes");
+  const int max_inner = o->pcg_max_inner_iterations > 0 ? o->pcg_max_inner_iterations : 30;
+  const int max_keyframes = o->pcg_max_keyframes > 0 ? o->pcg_max_keyframes : 2500;
+  if (K > max_keyframes) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "use_pcg: more keyframes than pcg_max_keyframes");   // :232
+  if (o->pcg_gauge_keyframe >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "pcg_gauge_keyframe out of range");
+  PcgLayout L;
+  if (bba_status st = MakePcgLayout(h, o, &L)) return st;
+  const bool opt_poses = L.opt_poses, opt_geometry = L.opt_geometry;
+  const uint64_t launches_before = h->launches;
+  const auto t_start = std::chrono::steady_clock::now();
+  if (bba_status st = BeginBundleAdjust(h, o, res, s)) return st;
+  std::vector<int> keyframes_with_new_surfels;
+
+  for (int iteration = 0; iteration < o->max_iterations; ++iteration) {
+    if (o->progress_function && !o->progress_function(o->progress_user, iteration)) break;
+    ++res->iterations_done;
+    // surfel creation (:183-206)
+    keyframes_with_new_surfels.clear();
+    if (opt_geometry && o->do_surfel_updates) {
+      for (int k = 0; k < K; ++k) {
+        Keyframe& kf = h->keyframes[k];
+        if (kf.activation == BBA_KF_ACTIVE && kf.last_active_in_ba_iteration != h->ba_iteration_count) {
+          kf.last_active_in_ba_iteration = h->ba_iteration_count;
+          uint32_t created = 0;
+          if (bba_status st = CreateSurfelsForKeyframe(h, k, /*filter_new_surfels=*/true, s, &created)) return st;
+          res->surfels_created += created;
+          keyframes_with_new_surfels.push_back(k);
+        } else if (kf.activation == BBA_KF_COVISIBLE_ACTIVE && kf.last_covis_in_ba_iteration != h->ba_iteration_count) {
+          kf.last_covis_in_ba_iteration = h->ba_iteration_count;
+        }
+      }
+    }
+    const uint32_t N = h->surfels_size;
+    if (N > 0) BBA_CUDA(h, cudaMemsetAsync(h->active, bba::kSurfelActiveFlag, N, s));   // :209-212
+    if (bba_status st = UploadKeyframes(h, s)) return st;
+    BBA_CUDA(h, cudaEventRecord(h->ev[0], s));
+    if (opt_geometry && N > 0) {   // UpdateSurfelNormalsCUDA, :215-227
+      bba::GeometryArgs g;
+      if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
+      bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
+      ++h->launches;
+      if (bba_status st = ExchangeGeometry(h, s)) return st;   // multi-GPU: every replica gets the other shards' normals
+    }
+    BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
+
+    if (bba_status st = MakePcgLayout(h, o, &L)) return st;   // unknown layout (:273-309)
+    const uint32_t unknown_count = L.unknown_count;
+    const int gauge = o->pcg_gauge_keyframe >= 0 ? o->pcg_gauge_keyframe : (rand() % K);   // :324
+
+    int num_converged = 0;
+    if (unknown_count > 0) {
+      const bba::PcgArgs a = MakePcgArgs(h, L, gauge);
+      int an = 0, bn = 2;
+      if (bba_status st = PcgInit(h, L, a, an, s)) return st;
+      float prev_r_norm = std::numeric_limits<float>::infinity();
+      int without_improvement = 0;
+      for (int step = 0; step < max_inner; ++step) {
+        if (step > 0) std::swap(an, bn);   // alpha_n <- beta_n (:386); g was cleared and alpha_d re-armed by PcgStep3Kernel
+        if (bba_status st = PcgStep1(h, L, a, s)) return st;
+        if (bba_status st = PcgStep2(h, L, an, bn, s)) return st;
+        BBA_CUDA(h, cudaMemcpyAsync(h->pcg.h_scalars, h->pcg.d_scalars, sizeof(double) * 4, cudaMemcpyDeviceToHost, s));
+        BBA_CUDA(h, cudaStreamSynchronize(s));   // :436-437
+        ++res->pcg_inner_iterations_total;
+        const float r_norm = std::sqrt(static_cast<float>(h->pcg.h_scalars[bn]));
+        res->pcg_last_r_norm = r_norm;
+        if (static_cast<double>(r_norm) < static_cast<double>(prev_r_norm) - 1e-3) {   // :442-449
+          without_improvement = 0;
+        } else if (++without_improvement >= 3) {
+          break;
+        }
+        prev_r_norm = r_norm;
+        if (step < max_inner - 1) {   // :456-464
+          if (bba_status st = PcgStep3(h, L, an, bn, s)) return st;
+        }
+      }
+      BBA_CUDA(h, cudaEventRecord(h->ev[2], s));
+      if (bba_status st = PcgApplyDelta(h, L, gauge, s, &num_converged)) return st;
+      // surfel merge + compaction (:644-690) for the keyframes that received new surfels
+      if (o->do_surfel_updates && !keyframes_with_new_surfels.empty()) {
+        uint32_t merged = 0;
+        if (bba_status st = MergeAndCompact(h, keyframes_with_new_surfels, s, &merged)) return st;
+        res->surfels_merged += merged;
+      }
+    } else {
+      BBA_CUDA(h, cudaEventRecord(h->ev[2], s));
+      BBA_CUDA(h, cudaStreamSynchronize(s));
+      num_converged = opt_poses ? 1 : 0;
+    }
+    cudaEventElapsedTime(&res->ms_geometry_optimization, h->ev[0], h->ev[1]);   // "BA normals update", :722-727
+    cudaEventElapsedTime(&res->ms_pcg, h->ev[1], h->ev[2]);
+
+    if (iteration >= o->min_iterations - 1 && (num_converged == K || !opt_poses)) {   // :757-766
+      res->converged = 1;
+      break;
+    }
+    if (o->time_limit_seconds > 0) {
+      const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_start).count();
+      if (el > o->time_limit_seconds) break;
+    }
+  }
+  if (!o->increase_ba_iteration_count && o->do_surfel_updates && !keyframes_with_new_surfels.empty()) {
+    // :775-815: without the end tasks, the keyframes of the last iteration's creation step are merged (and the map compacted) once more
+    uint32_t merged = 0;
+    if (bba_status st = MergeAndCompact(h, keyframes_with_new_surfels, s, &merged)) return st;
+    res->surfels_merged += merged;
+  }
+  return EndBundleAdjust(h, o, launches_before, res, s);
+}
+
+}  // namespace
+}  // namespace bba
+
+using namespace bba;
+
+extern "C" {
+
+bba_status bba_update_surfel_activation(bba_handle h, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (bba_status st = CheckSurfels(h)) return st;
+  if (h->surfels_size == 0) return BBA_OK;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (bba_status st = UploadKeyframes(h, s)) return st;
+  bba::GeometryArgs g;
+  if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
+  if (bba_status st = CheckCollective(h)) return st;
+  bba::LaunchActivationAndNormals(g, h->sm_count, true, false, s);
+  ++h->launches;
+  BBA_CUDA(h, cudaGetLastError());
+  if (bba_status st = ExchangeGeometry(h, s)) return st;
+  return MarkStaging(h, s);
+}
+
+bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (bba_status st = CheckSurfels(h)) return st;
+  if (h->surfels_size == 0) return BBA_OK;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (bba_status st = UploadKeyframes(h, s)) return st;
+  bba::GeometryArgs g;
+  if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
+  if (bba_status st = CheckCollective(h)) return st;
+  bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
+  bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
+  h->launches += 2;
+  BBA_CUDA(h, cudaGetLastError());
+  if (bba_status st = ExchangeGeometry(h, s)) return st;
+  return MarkStaging(h, s);
+}
+
+bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth, int optimize_color, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (!optimize_depth && !optimize_color) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "nothing to optimise");   // kernel_opt_intrinsics.cc:54
+  if (bba_status st = CheckSurfels(h)) return st;
+  if (bba_status st = CheckCollective(h)) return st;
+  return OptimizeIntrinsics(h, optimize_depth != 0, optimize_color != 0, static_cast<cudaStream_t>(stream));
+}
+
+bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_result* res, void* stream) {
+  if (!h || !o || !res) return BBA_ERR_INVALID_ARGUMENT;
+  std::memset(res, 0, sizeof(*res));
+  if (bba_status st = CheckSurfels(h)) return st;
+  // (do_surfel_updates with more than one rank: creation / merging / compaction run REPLICATED -- they are deterministic and
+  // every rank holds the whole surfel buffer -- while the geometry and pose steps stay sharded; see PeerFence)
+  if (o->use_pcg) return BundleAdjustPCG(h, o, res, static_cast<cudaStream_t>(stream));   // direct_ba.cc:436-457
+  // direct_ba.cc:427-434
+  const bool opt_depth_intr = o->optimize_depth_intrinsics && h->cfg.use_depth_residuals;
+  const bool opt_color_intr = o->optimize_color_intrinsics && h->cfg.use_descriptor_residuals;
+  if (bba_status st = CheckCollective(h)) return st;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int K = static_cast<int>(h->keyframes.size());
+  const uint64_t launches_before = h->launches;
+  const auto t_start = std::chrono::steady_clock::now();
+
+  // the caller may have moved the surfels since the last call (through the device view): sort them again at the first pose step
+  h->pose.order_stale = true;
+  const int fixed_ba_iteration_count = h->ba_iteration_count;
+  if (bba_status st = BeginBundleAdjust(h, o, res, s)) return st;
+  std::vector<int> keyframes_with_new_surfels;
+
+  const bool fixed_window = o->active_keyframe_window_start > 0 || o->active_keyframe_window_end > 0;   // :330-331
+  const bool whole_window = !(o->active_keyframe_window_start != 0 || o->active_keyframe_window_end != K - 1);
+
+  BBA_CUDA(h, cudaMemsetAsync(h->active, 0, h->surfels_size, s));   // :338
+
+  for (int iteration = 0; iteration < o->max_iterations; ++iteration) {
+    if (o->progress_function && !o->progress_function(o->progress_user, iteration)) break;
+    ++res->iterations_done;
+    if (fixed_window) {   // :354-372
+      for (int k = 0; k < K; ++k)
+        h->keyframes[k].activation =
+            (k >= o->active_keyframe_window_start && k <= o->active_keyframe_window_end) ? BBA_KF_ACTIVE : BBA_KF_INACTIVE;
+      DetermineCovisibleActiveKeyframes(h);
+    }
+
+    BBA_TRACE("iteration start");
+    // --- surfel creation (:399-430): keyframes that became active for the first time within this BA iteration block
+    keyframes_with_new_surfels.clear();
+    const uint32_t old_surfels_size = h->surfels_size;
+    if (o->optimize_geometry && o->do_surfel_updates) {
+      for (int k = 0; k < K; ++k) {
+        Keyframe& kf = h->keyframes[k];
+        if (kf.activation == BBA_KF_ACTIVE && kf.last_active_in_ba_iteration != fixed_ba_iteration_count) {
+          kf.last_active_in_ba_iteration = fixed_ba_iteration_count;
+          keyframes_with_new_surfels.push_back(k);
+        } else if (kf.activation == BBA_KF_COVISIBLE_ACTIVE && kf.last_covis_in_ba_iteration != fixed_ba_iteration_count) {
+          kf.last_covis_in_ba_iteration = fixed_ba_iteration_count;
+        }
+      }
+      for (int k : keyframes_with_new_surfels) {
+        uint32_t created = 0;
+        if (bba_status st = CreateSurfelsForKeyframe(h, k, /*filter_new_surfels=*/true, s, &created)) return st;
+        res->surfels_created += created;
+      }
+      if (!keyframes_with_new_surfels.empty()) h->pose.order_stale = true;
+    }
+
+    BBA_TRACE("creation done");
+    if (bba_status st = UploadKeyframes(h, s)) return st;
+    BBA_TRACE("keyframes uploaded");
+    bba::GeometryArgs g;
+    if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
+
+    BBA_TRACE("after creation + upload");
+    // --- surfel activation (:432-456) fused with the normal update of the geometry step (:466-485)
+    BBA_CUDA(h, cudaEventRecord(h->ev[0], s));
+    const bool has_new = o->optimize_geometry && h->surfels_size > old_surfels_size;
+    if (has_new)   // new surfels are active (:435-441); only the old ones are re-evaluated below
+      BBA_CUDA(h, cudaMemsetAsync(h->active + old_surfels_size, bba::kSurfelActiveFlag, h->surfels_size - old_surfels_size, s));
+    if (!whole_window) BBA_CUDA(h, cudaMemsetAsync(h->active, bba::kSurfelActiveFlag, old_surfels_size, s));
+    if (h->surfels_size > 0) {
+      if (whole_window && has_new) {
+        bba::GeometryArgs g_old = g, g_new = g;   // (begin / end are LOCAL indices of this rank's shard)
+        g_old.end = LocalCountBelow(old_surfels_size, h->cfg.rank, h->cfg.world_size);
+        g_new.begin = g_old.end;
+        bba::LaunchActivationAndNormals(g_old, h->sm_count, true, true, s);
+        bba::LaunchActivationAndNormals(g_new, h->sm_count, false, true, s);
+        h->launches += 2;
+      } else if (whole_window) {
+        bba::LaunchActivationAndNormals(g, h->sm_count, true, o->optimize_geometry != 0, s);
+        ++h->launches;
+      } else if (o->optimize_geometry) {
+        bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
+        ++h->launches;
+      }
+    }
+    BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
+    if (o->optimize_geometry && h->surfels_size > 0) {
+      bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
+      ++h->launches;
+    }
+    BBA_CUDA(h, cudaGetLastError());
+    if (bba_status st = ExchangeGeometry(h, s)) return st;   // multi-GPU: all-gather of the updated surfel shards
+    BBA_CUDA(h, cudaEventRecord(h->ev[2], s));
+    if (bba_status st = MarkStaging(h, s)) return st;
+
+    BBA_TRACE("after geometry");
+    // --- surfel merge + compaction (:489-541) for the keyframes that received new surfels
+    if (o->do_surfel_updates && !keyframes_with_new_surfels.empty()) {
+      uint32_t merged = 0;
+      if (bba_status st = MergeAndCompact(h, keyframes_with_new_surfels, s, &merged)) return st;
+      res->surfels_merged += merged;
+      h->pose.order_stale = true;
+    }
+
+    BBA_TRACE("before pose step");
+    // --- pose optimisation (:543-577): all non-inactive keyframes at once
+    int num_converged = 0;
+    if (o->optimize_poses) {
+      std::vector<int> ids;
+      std::vector<Pose> init;
+      for (int k = 0; k < K; ++k) {
+        if (h->keyframes[k].activation == BBA_KF_INACTIVE) {
+          ++num_converged;
+          continue;
+        }
+        ids.push_back(k);
+        init.push_back(h->keyframes[k].pose);
+      }
+      if (bba_status st = RunPoseStep(h, ids, init, 30, s)) return st;
+      res->depth_residual_count = 0;
+      res->descriptor_residual_count = 0;
+      res->cost = 0;
+      for (int k : ids) {
+        Keyframe& kf = h->keyframes[k];
+        const Pose est = PoseFromArray(h->pose.h_pose_est + 7 * k);
+        float lg[6];
+        bba::Log(bba::Compose(bba::Inverse(kf.pose), est), lg);   // :562-563
+        const bool moved = !bba::IsScale1PoseEstimationConverged(lg);
+        kf.pose = est;
+        if (moved) {
+          kf.activation = BBA_KF_ACTIVE;
+        } else {
+          kf.activation = BBA_KF_INACTIVE;
+          ++num_converged;
+        }
+        res->pose_iterations_total += h->pose.h_iterations[k];
+        const double* fs = h->pose.h_first_stats + 8 * k;
+        res->depth_residual_count += static_cast<uint64_t>(fs[0] + 0.5);
+        res->descriptor_residual_count += 2 * static_cast<uint64_t>(fs[1] + 0.5);
+        res->cost += fs[2] + fs[3];
+      }
+    } else {
+      BBA_CUDA(h, cudaStreamSynchronize(s));
+    }
+    BBA_CUDA(h, cudaEventRecord(h->ev[3], s));
+    // --- intrinsics optimisation (:584-624)
+    if (opt_depth_intr || opt_color_intr) {
+      if (bba_status st = OptimizeIntrinsics(h, opt_depth_intr, opt_color_intr, s)) return st;
+      BBA_CUDA(h, cudaEventRecord(h->ev[4], s));
+      BBA_CUDA(h, cudaEventSynchronize(h->ev[4]));
+      cudaEventElapsedTime(&res->ms_intrinsics_optimization, h->ev[3], h->ev[4]);
+    }
+    BBA_CUDA(h, cudaEventSynchronize(h->ev[3]));
+    cudaEventElapsedTime(&res->ms_surfel_activation, h->ev[0], h->ev[1]);
+    cudaEventElapsedTime(&res->ms_geometry_optimization, h->ev[1], h->ev[2]);
+    cudaEventElapsedTime(&res->ms_pose_optimization, h->ev[2], h->ev[3]);
+    if (h->profiling) {
+      h->profile.activation_normals_ms += res->ms_surfel_activation;
+      h->profile.position_descriptor_ms += res->ms_geometry_optimization;
+      h->profile.geometry_launches += (o->optimize_geometry ? 2 : 1);
+    }
+
+    // --- convergence (:693-701)
+    if (iteration >= o->min_iterations - 1 && (num_converged == K || !o->optimize_poses)) {
+      res->converged = 1;
+      break;
+    }
+    if (o->time_limit_seconds > 0) {   // :704-709
+      const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_start).count();
+      if (el > o->time_limit_seconds) break;
+    }
+    DetermineCovisibleActiveKeyframes(h);   // :711-717
+  }
+  BBA_TRACE("iterations done");
+  return EndBundleAdjust(h, o, launches_before, res, s);
+}
+
+bba_status bba_perform_end_tasks(bba_handle h, int do_surfel_updates, uint32_t* deleted, uint32_t* surfels_size, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (bba_status st = CheckSurfels(h)) return st;
+  uint32_t d = 0;
+  if (bba_status st = PerformEndTasks(h, static_cast<cudaStream_t>(stream), &d, do_surfel_updates != 0)) return st;
+  if (deleted) *deleted = d;
+  if (surfels_size) *surfels_size = h->surfels_size;
+  return BBA_OK;
+}
+
+bba_status bba_create_surfels_for_keyframe(bba_handle h, int id, int filter_new_surfels, uint32_t* created, void* stream) {
+  CHECK_KF(h, id);
+  if (bba_status st = CheckSurfels(h)) return st;
+  uint32_t c = 0;
+  if (bba_status st = CreateSurfelsForKeyframe(h, id, filter_new_surfels != 0, static_cast<cudaStream_t>(stream), &c)) return st;
+  if (created) *created = c;
+  return BBA_OK;
+}
+
+bba_status bba_merge_surfels_for_keyframe(bba_handle h, int id, uint32_t* deleted, void* stream) {
+  CHECK_KF(h, id);
+  if (bba_status st = CheckSurfels(h)) return st;
+  uint32_t d = 0;
+  if (bba_status st = MergeSurfelsForKeyframe(h, id, static_cast<cudaStream_t>(stream), &d)) return st;
+  if (deleted) *deleted = d;
+  return BBA_OK;
+}
+
+bba_status bba_compact_surfels(bba_handle h, uint32_t free_count, int with_active_flags, uint32_t* surfels_size, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (bba_status st = CheckSurfels(h)) return st;
+  if (free_count > h->surfels_size) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "free_count exceeds surfels_size");
+  if (bba_status st = CompactSurfels(h, free_count, with_active_flags != 0, static_cast<cudaStream_t>(stream))) return st;
+  if (surfels_size) *surfels_size = h->surfels_size;
+  return BBA_OK;
+}
+
+bba_status bba_pcg_debug(bba_handle h, const bba_ba_options* o, int step, int apply, uint32_t* unknown_count, bba_pcg_probe* out,
+                         void* stream) {
+  if (!h || !o || !unknown_count || step < 0) return BBA_ERR_INVALID_ARGUMENT;
+  if (bba_status st = CheckSurfels(h)) return st;
+  const int K = static_cast<int>(h->keyframes.size());
+  if (K == 0) return Fail(h, BBA_ERR_STATE, "no keyframes");
+  if (o->pcg_gauge_keyframe < 0 || o->pcg_gauge_keyframe >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "pcg_gauge_keyframe out of range");
+  if (h->cfg.world_size > 1) return Fail(h, BBA_ERR_UNSUPPORTED, "bba_pcg_debug runs on one rank");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  PcgLayout L;
+  if (bba_status st = MakePcgLayout(h, o, &L)) return st;
+  *unknown_count = L.unknown_count;
+  if (!out || L.unknown_count == 0) return BBA_OK;
+  const uint32_t U = L.unknown_count;
+  auto copy = [&](float* dst, const float* src) -> bba_status {
+    if (dst) BBA_CUDA(h, cudaMemcpyAsync(dst, src, sizeof(float) * U, cudaMemcpyDeviceToHost, s));
+    return BBA_OK;
+  };
+  // the scalar slots of alpha_n / beta_n of step `step` (BundleAdjustPCG swaps them at every step after the first)
+  auto scalars = [&](int slot, double* dst) -> bba_status {
+    BBA_CUDA(h, cudaMemcpyAsync(h->pcg.h_scalars, h->pcg.d_scalars, sizeof(double) * 4, cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaStreamSynchronize(s));
+    *dst = h->pcg.h_scalars[slot];
+    return BBA_OK;
+  };
+  if (bba_status st = UploadKeyframes(h, s)) return st;
+  const bba::PcgArgs a = MakePcgArgs(h, L, o->pcg_gauge_keyframe);
+  int an = 0, bn = 2;
+  if (bba_status st = PcgInit(h, L, a, an, s)) return st;
+  for (int k = 0;; ++k) {
+    if (k > 0) std::swap(an, bn);
+    if (bba_status st = PcgStep1(h, L, a, s)) return st;
+    if (k == step) break;
+    if (bba_status st = PcgStep2(h, L, an, bn, s)) return st;
+    if (bba_status st = PcgStep3(h, L, an, bn, s)) return st;
+  }
+  BBA_CUDA(h, cudaGetLastError());
+  float *r = h->pcg.d_vec[0], *M = h->pcg.d_vec[1], *delta = h->pcg.d_vec[2], *g = h->pcg.d_vec[3], *p = h->pcg.d_vec[4];
+  bba_status st = BBA_OK;
+  if ((st = copy(out->r, r)) || (st = copy(out->M, M)) || (st = copy(out->p, p)) || (st = copy(out->g, g)) || (st = copy(out->delta, delta)) ||
+      (st = scalars(an, &out->alpha_n)) || (st = scalars(1, &out->alpha_d)))
+    return st;
+  if ((st = PcgStep2(h, L, an, bn, s)) || (st = copy(out->r_step2, r)) || (st = copy(out->delta_step2, delta)) || (st = copy(out->z, g)) ||
+      (st = scalars(bn, &out->beta_n)))
+    return st;
+  if ((st = PcgStep3(h, L, an, bn, s)) || (st = copy(out->p_step3, p)) || (st = copy(out->g_step3, g)) || (st = scalars(1, &out->alpha_d_step3)))
+    return st;
+  if (apply) {
+    int num_converged = 0;
+    if ((st = PcgApplyDelta(h, L, o->pcg_gauge_keyframe, s, &num_converged))) return st;
+  }
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  return MarkStaging(h, s);
+}
+
+}  // extern "C"

@@ -1,0 +1,404 @@
+// frames.cu -- the frame side of libbadba_b200 (host side): image-pair odometry (buffers, pyramids, the persistent tracking
+// kernel's launch and its entry points) and keyframe preprocessing (bba_preprocess_frame, bba_preprocess_raw_frame).
+#include <cmath>
+#include <cstring>
+
+#include "handle.hpp"
+#include "preprocess_tile.cuh"
+
+namespace bba {
+namespace {
+
+// ---- image-pair odometry (bba_track_frame_pairwise) --------------------------------------------------------------------
+// A u8 plane in pitched device memory as a texture with the sampler state of CUDABuffer::CreateTextureObject as the reference
+// calls it for the pyramid colour planes (pairwise_frame_tracking.cc:57-79).
+bba_status MakePitchedU8Texture(bba_handle h, const PitchedBuffer& plane, int w, int ht, Texture* out) {
+  cudaResourceDesc res;
+  std::memset(&res, 0, sizeof(res));
+  res.resType = cudaResourceTypePitch2D;
+  res.res.pitch2D.devPtr = plane.get();
+  res.res.pitch2D.desc = cudaCreateChannelDesc(8, 0, 0, 0, cudaChannelFormatKindUnsigned);
+  res.res.pitch2D.width = w;
+  res.res.pitch2D.height = ht;
+  res.res.pitch2D.pitchInBytes = plane.pitch();
+  const cudaTextureDesc tex = LinearTextureDesc();
+  BBA_CUDA(h, cudaCreateTextureObject(&out->tex.r, &res, &tex, nullptr));
+  return BBA_OK;
+}
+
+// PairwiseFrameTrackingBuffers + CreatePairwiseTrackingInputBuffersAndTextures (pairwise_frame_tracking.cc:39-151)
+bba_status EnsureOdometry(bba_handle h, int num_scales) {
+  auto& o = h->odo;
+  if (o.num_scales >= num_scales) return BBA_OK;
+  o = bba_context::Odometry{};   // frees the smaller pyramids first
+  const int cw = h->cfg.color_width, ch = h->cfg.color_height;
+  for (int f = 0; f < 2; ++f) {
+    BBA_CUDA(h, o.gradmag[f].Allocate(cw, ch));
+    if (bba_status st = MakePitchedU8Texture(h, o.gradmag[f], cw, ch, &o.gradmag_tex[f])) return st;
+  }
+  for (int s = 0; s < num_scales; ++s) {
+    // pairwise_frame_tracking.cc:51-53: int scale_width = depth_width / pow(2, scale)
+    o.w[s] = static_cast<int>(h->cfg.depth_width / std::pow(2, s));
+    o.h[s] = static_cast<int>(h->cfg.depth_height / std::pow(2, s));
+    if (o.w[s] < 1 || o.h[s] < 1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: too many pyramid levels for this image size");
+    for (int f = 0; f < 2; ++f) {
+      bba::odom::Image& im = o.image[f][s];
+      BBA_CUDA(h, o.depth[f][s].Allocate(sizeof(float) * o.w[s], o.h[s]));
+      im.depth = o.depth[f][s].get<float>();
+      im.depth_pitch = static_cast<uint32_t>(o.depth[f][s].pitch() / sizeof(float));
+      if (s >= 1) {   // level 0 uses the caller's normal images
+        BBA_CUDA(h, o.normals[f][s].Allocate(sizeof(uint16_t) * o.w[s], o.h[s]));
+        im.normals = o.normals[f][s].get<uint16_t>();
+        im.normals_pitch = static_cast<uint32_t>(o.normals[f][s].pitch());
+      }
+      BBA_CUDA(h, o.color[f][s].Allocate(o.w[s], o.h[s]));
+      im.color = o.color[f][s].get();
+      im.color_pitch = static_cast<uint32_t>(o.color[f][s].pitch());
+      if (bba_status st = MakePitchedU8Texture(h, o.color[f][s], o.w[s], o.h[s], &o.color_tex[f][s])) return st;
+      im.color_tex = o.color_tex[f][s].tex;
+    }
+  }
+  BBA_CUDA(h, o.d_acc.Reserve(96));
+  BBA_CUDA(h, o.d_barrier.Reserve(2));
+  BBA_CUDA(h, o.d_result.Reserve(1));
+  BBA_CUDA(h, o.h_result.Reserve(1));
+  o.num_scales = num_scales;
+  return BBA_OK;
+}
+
+// The camera model of one pyramid level: PinholeCamera4f::Scaled (libvis camera.h:1696-1705, 1086-1097: all four parameters
+// times the factor, width = factor * width + 0.5) through the builders of surfel_projection.h:42-124.
+bba::odom::LevelCamera MakeLevelCamera(bba_handle h, int scale, int level_w, int level_h) {
+  bba::odom::LevelCamera c;
+  const float scaling_factor = static_cast<float>(std::pow(2, scale));
+  const float df = static_cast<float>(1.f / scaling_factor);   // depth_camera.Scaled(1.f / scaling_factor)
+  const float cf = static_cast<float>((h->cfg.depth_width == h->cfg.color_width) ? (1.f / scaling_factor) : (2.f / scaling_factor));
+  const float dK[4] = {h->depth_K[0] * df, h->depth_K[1] * df, h->depth_K[2] * df, h->depth_K[3] * df};
+  const float cK[4] = {h->color_K[0] * cf, h->color_K[1] * cf, h->color_K[2] * cf, h->color_K[3] * cf};
+  c.w = level_w; c.h = level_h;
+  c.fx = dK[0]; c.fy = dK[1]; c.cx = dK[2]; c.cy = dK[3];
+  c.fx_inv = 1.0f / dK[0];
+  c.fy_inv = 1.0f / dK[1];
+  c.cx_inv = -(dK[2] - 0.5f) * c.fx_inv;
+  c.cy_inv = -(dK[3] - 0.5f) * c.fy_inv;
+  c.d2c_fx = cK[0] / dK[0];
+  c.d2c_cx = -1 * cK[0] * dK[2] / dK[0] + cK[2];
+  c.d2c_fy = cK[1] / dK[1];
+  c.d2c_cy = -1 * cK[1] * dK[3] / dK[1] + cK[3];
+  c.cw = static_cast<int>(static_cast<double>(cf) * h->cfg.color_width + 0.5f);
+  c.ch = static_cast<int>(static_cast<double>(cf) * h->cfg.color_height + 0.5f);
+  c.cfx = cK[0]; c.cfy = cK[1];
+  return c;
+}
+
+// Fills the pyramids of both frames for the given options (stages 1-3 of odometry.cuh) and the level descriptors in h->odo.level.
+bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, const Keyframe& base, const uint16_t* trk_depth, size_t trk_depth_pitch,
+                                 const uint16_t* trk_normals, size_t trk_normals_pitch, cudaStream_t s) {
+  namespace od = bba::odom;
+  auto& st = h->odo;
+  const int S = o.num_scales;
+  od::BrightnessArgs br{};
+  br.luma_tex[0] = base.tex; br.luma_tex[1] = h->staging.scratch.tex;
+  for (int f = 0; f < 2; ++f) { br.out[f] = st.gradmag[f].get(); br.out_pitch[f] = static_cast<uint32_t>(st.gradmag[f].pitch()); }
+  br.w = h->cfg.color_width; br.h = h->cfg.color_height;
+  br.use_gradmag = o.use_gradmag;
+  od::LaunchBrightness(br, s);
+  ++h->launches;
+
+  // level images as seen by the kernels: level 0 normals are the keyframe's / the frame's own buffers
+  od::Image img[2][od::kMaxScales];
+  for (int f = 0; f < 2; ++f)
+    for (int l = 0; l < S; ++l) img[f][l] = st.image[f][l];
+  img[0][0].normals = const_cast<uint16_t*>(base.normals); img[0][0].normals_pitch = static_cast<uint32_t>(base.normals_pitch);
+  img[1][0].normals = const_cast<uint16_t*>(trk_normals);  img[1][0].normals_pitch = static_cast<uint32_t>(trk_normals_pitch);
+
+  const bba::CameraParams cam = MakeCamera(h);
+  od::Level0Args l0{};
+  l0.raw_depth[0] = base.depth; l0.raw_depth_pitch[0] = static_cast<uint32_t>(base.depth_pitch);
+  l0.raw_depth[1] = trk_depth;  l0.raw_depth_pitch[1] = static_cast<uint32_t>(trk_depth_pitch);
+  l0.raw_normals = trk_normals; l0.raw_normals_pitch = static_cast<uint32_t>(trk_normals_pitch);
+  l0.gradmag_tex[0] = st.gradmag_tex[0].tex; l0.gradmag_tex[1] = st.gradmag_tex[1].tex;
+  l0.out[0] = img[0][0];
+  l0.skip_level0 = o.use_pyramid_level_0 ? 0 : 1;
+  l0.out[1] = l0.skip_level0 ? img[1][1] : img[1][0];
+  l0.w = st.w[0]; l0.h = st.h[0];
+  l0.out_w = l0.skip_level0 ? st.w[1] : st.w[0];
+  l0.out_h = l0.skip_level0 ? st.h[1] : st.h[0];
+  l0.d2c_fx = cam.d2c_fx; l0.d2c_fy = cam.d2c_fy; l0.d2c_cx = cam.d2c_cx; l0.d2c_cy = cam.d2c_cy;
+  l0.cw = cam.cw; l0.ch = cam.ch;
+  l0.a = cam.a; l0.raw_to_float = cam.raw_to_float; l0.cfactor = cam.cfactor; l0.cf_w = cam.cf_w; l0.cell = cam.cell;
+  l0.downsample_color = h->cfg.depth_width == h->cfg.color_width;
+  od::LaunchLevel0(l0, s);
+  ++h->launches;
+
+  for (int l = 1; l < S; ++l) {
+    // pairwise_frame_tracking.cc:325-347: the tracked image from level 2 on (level 1 too when level 0 is in use), the base always
+    od::DownsampleArgs d{};
+    d.in[0] = img[0][l - 1]; d.out[0] = img[0][l];
+    d.count = 1;
+    if (l >= 2 || o.use_pyramid_level_0) {
+      d.in[1] = img[1][l - 1]; d.out[1] = img[1][l];
+      d.count = 2;
+    }
+    d.w = st.w[l]; d.h = st.h[l];
+    d.in_w = st.w[l - 1]; d.in_h = st.h[l - 1];
+    od::LaunchDownsample(d, s);
+    ++h->launches;
+  }
+  for (int l = 0; l < S; ++l) {
+    st.level[l].cam = MakeLevelCamera(h, l, st.w[l], st.h[l]);
+    st.level[l].base = img[0][l];
+    st.level[l].tracked = img[1][l];
+  }
+  st.last_num_scales = S;
+  st.last_first_scale = o.use_pyramid_level_0 ? 0 : 1;
+  BBA_CUDA(h, cudaGetLastError());
+  return BBA_OK;
+}
+
+bba_status LaunchOdometryKernel(bba_handle h, int num_scales, int first_scale, int max_iterations, int use_gradmag, int test_different,
+                                int debug_scale, const float init1[7], const float init2[7], cudaStream_t s) {
+  namespace od = bba::odom;
+  auto& st = h->odo;
+  od::TrackArgs a{};
+  for (int l = 0; l < num_scales; ++l) a.level[l] = st.level[l];
+  a.num_scales = num_scales;
+  a.first_scale = first_scale;
+  a.max_iterations = max_iterations;
+  a.use_depth = h->cfg.use_depth_residuals;
+  a.use_desc = h->cfg.use_descriptor_residuals;
+  a.use_gradmag = use_gradmag;
+  a.test_different_initial_estimates = test_different;
+  a.debug_scale = debug_scale;
+  a.baseline_fx = h->cfg.baseline_fx;
+  std::memcpy(a.init1, init1, sizeof(float) * 7);
+  std::memcpy(a.init2, init2, sizeof(float) * 7);
+  a.acc = st.d_acc;
+  a.barrier = st.d_barrier;
+  a.result = st.d_result;
+  BBA_CUDA(h, cudaMemsetAsync(st.d_acc, 0, sizeof(double) * 96, s));
+  BBA_CUDA(h, cudaMemsetAsync(st.d_barrier, 0, sizeof(unsigned int) * 2, s));
+  BBA_CUDA(h, cudaMemsetAsync(st.d_result, 0, sizeof(od::TrackResult), s));
+  od::LaunchTrack(a, h->sm_count, s);
+  ++h->launches;
+  BBA_CUDA(h, cudaGetLastError());
+  BBA_CUDA(h, cudaMemcpyAsync(st.h_result, st.d_result, sizeof(od::TrackResult), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  if (st.h_result->barrier_timeout) return Fail(h, BBA_ERR_CUDA, "odometry kernel: grid barrier timed out");
+  return BBA_OK;
+}
+
+// Stage 0 of bba_preprocess_raw_frame (validated by the caller), or nullptr for bba_preprocess_frame.
+struct RawStage {
+  int median_iterations, depth_level, raw_w, raw_h, color_level;
+};
+
+// bba_preprocess_frame and bba_preprocess_raw_frame after their own checks; `fn` prefixes the error messages.
+bba_status PreprocessFrame(bba_handle h, const char* fn, const bba_preprocess_options* o,
+                           const uint16_t* device_raw_depth, size_t raw_depth_pitch,
+                           const uint8_t* device_rgb, size_t rgb_pitch,
+                           uint16_t* device_depth, size_t depth_pitch,
+                           uint16_t* device_normals, size_t normals_pitch,
+                           uint16_t* device_radius, size_t radius_pitch,
+                           uint8_t* device_color_rgba, size_t color_pitch,
+                           float* min_depth, float* max_depth, void* stream, const RawStage* raw_stage) {
+  const std::string name(fn);
+  if (!h || !o || !device_raw_depth || !device_depth || !device_normals || !device_radius) return h ? Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null argument") : BBA_ERR_INVALID_ARGUMENT;
+  if ((device_rgb == nullptr) != (device_color_rgba == nullptr))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": rgb input and rgba output go together");
+  if ((raw_depth_pitch | depth_pitch | normals_pitch | radius_pitch) & 1u)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": u16 image pitches must be even");
+  if (device_color_rgba && ((color_pitch & 3u) || (reinterpret_cast<uintptr_t>(device_color_rgba) & 3u)))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": the rgba image must be 4-byte aligned");
+  if (device_depth == device_raw_depth)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": in-place filtering is not possible (tiles read their neighbours' raw depth)");
+  // BilateralFilteringAndDepthCutoffCUDA (cuda_depth_processing.cu:100-128)
+  const int radius = static_cast<int>(o->bilateral_filter_radius_factor * o->bilateral_filter_sigma_xy + 0.5f);
+  if (radius < 0 || radius > bba::pre::kMaxFilterRadius)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": bilateral filter radius outside [0, 16]");
+  if (!(o->bilateral_filter_sigma_xy > 0.f) || !(o->bilateral_filter_sigma_inv_depth > 0.f) || !(o->max_depth > 0.f))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": sigma_xy, sigma_inv_depth and max_depth must be positive");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  BBA_CUDA(h, h->pre.d_min_max.Reserve(2));
+  BBA_CUDA(h, h->pre.h_min_max.Reserve(2));
+  const bba::CameraParams cam = MakeCamera(h);
+  bba::pre::FrameArgs f{};
+  f.w = cam.w; f.h = cam.h;
+  f.fx_inv = cam.fx_inv; f.fy_inv = cam.fy_inv; f.cx_inv = cam.cx_inv; f.cy_inv = cam.cy_inv;
+  f.raw_to_float = cam.raw_to_float; f.a = cam.a;
+  f.cell = cam.cell; f.cf_w = cam.cf_w; f.cfactor = cam.cfactor;
+  f.denom_xy = 2.0f * o->bilateral_filter_sigma_xy * o->bilateral_filter_sigma_xy;
+  f.denom_value = 2.0f * o->bilateral_filter_sigma_inv_depth * o->bilateral_filter_sigma_inv_depth;
+  f.radius = radius;
+  f.radius_squared = radius * radius;
+  const float max_raw = o->max_depth / cam.raw_to_float;   // bad_slam.cc:703 (float -> u16 at the call)
+  f.max_depth = max_raw >= 65535.f ? static_cast<uint16_t>(65535) : static_cast<uint16_t>(max_raw);
+  f.raw_depth = device_raw_depth; f.raw_pitch = static_cast<uint32_t>(raw_depth_pitch);
+  f.out_depth = device_depth; f.out_depth_pitch = static_cast<uint32_t>(depth_pitch);
+  f.out_normals = device_normals; f.out_normals_pitch = static_cast<uint32_t>(normals_pitch);
+  f.out_radius = device_radius; f.out_radius_pitch = static_cast<uint32_t>(radius_pitch);
+  f.min_max = h->pre.d_min_max;
+  f.cw = cam.cw; f.ch = cam.ch;
+  f.rgb = device_rgb; f.rgb_pitch = static_cast<uint32_t>(rgb_pitch);
+  f.rgba = device_color_rgba; f.rgba_pitch = static_cast<uint32_t>(color_pitch);
+  f.tiles_x = (f.w + bba::pre::kTile - 1) / bba::pre::kTile;
+  f.tiles_y = (f.h + bba::pre::kTile - 1) / bba::pre::kTile;
+  if (raw_stage) {
+    f.median_iterations = raw_stage->median_iterations;
+    f.depth_level = raw_stage->depth_level;
+    f.raw_w = raw_stage->raw_w; f.raw_h = raw_stage->raw_h;
+    f.color_level = raw_stage->color_level;
+    h->launches += bba::LaunchPreprocessRawFrame(f, s);
+  } else {
+    h->launches += bba::LaunchPreprocessFrame(f, s);
+  }
+  BBA_CUDA(h, cudaGetLastError());
+  if (min_depth || max_depth) {   // ComputeMinMaxDepthCUDA returns host values and synchronises (cuda_depth_processing.cu:452-463)
+    BBA_CUDA(h, cudaMemcpyAsync(h->pre.h_min_max, h->pre.d_min_max, 2 * sizeof(float), cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaStreamSynchronize(s));
+    if (min_depth) *min_depth = h->pre.h_min_max[0];
+    if (max_depth) *max_depth = h->pre.h_min_max[1];
+  }
+  return BBA_OK;
+}
+
+}  // namespace
+
+}  // namespace bba
+
+using namespace bba;
+
+extern "C" {
+
+bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* o, int base_keyframe_id,
+                                    const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals, size_t normals_pitch,
+                                    const uint8_t* device_color_rgba, size_t color_pitch, const float init1[7], const float init2[7],
+                                    float out[7], bba_odometry_result* result, void* stream) {
+  if (!h || !o || !device_depth || !device_normals || !device_color_rgba || !init1 || !out) return h ? Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: null argument") : BBA_ERR_INVALID_ARGUMENT;
+  if (base_keyframe_id < 0 || base_keyframe_id >= static_cast<int>(h->keyframes.size()))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: no such keyframe");
+  if (o->num_scales < 1 || o->num_scales > bba::odom::kMaxScales || (!o->use_pyramid_level_0 && o->num_scales < 2))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: num_scales must be 1..8 (>= 2 without pyramid level 0)");
+  if (!FramePitchesOk(h, depth_pitch, normals_pitch, color_pitch) || ((depth_pitch | normals_pitch) & 1u))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: bad frame buffer pitch");
+  // pairwise_frame_tracking.cc:300-306 (LOG(FATAL) in the reference)
+  if (!o->use_pyramid_level_0 && h->cfg.depth_width != h->cfg.color_width && h->cfg.depth_width != 2 * h->cfg.color_width)
+    return Fail(h, BBA_ERR_UNSUPPORTED, "The chosen depth / color pyramid level combination is not supported here.");
+  if (o->test_different_initial_estimates && !init2)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: test_different_initial_estimates needs the second estimate");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const uint64_t launches_before = h->launches;
+  if (bba_status st = EnsureOdometry(h, o->num_scales)) return st;
+  if (bba_status st = MakeLumaTexture(h, device_color_rgba, color_pitch, &h->staging.scratch, s)) return st;
+  const Keyframe& base = h->keyframes[base_keyframe_id];
+  if (bba_status st = BuildOdometryPyramids(h, *o, base, device_depth, depth_pitch, device_normals, normals_pitch, s)) return st;
+  const int max_it = o->max_iterations_per_scale > 0 ? o->max_iterations_per_scale : 30;
+  if (bba_status st = LaunchOdometryKernel(h, o->num_scales, o->use_pyramid_level_0 ? 0 : 1, max_it, o->use_gradmag ? 1 : 0,
+                                           o->test_different_initial_estimates ? 1 : 0, -1, init1, init2 ? init2 : init1, s))
+    return st;
+  const bba::odom::TrackResult& r = *h->odo.h_result;
+  std::memcpy(out, r.base_T_frame, sizeof(float) * 7);
+  if (result) {
+    for (int i = 0; i < 8; ++i) {
+      result->iterations[i] = r.iterations[i];
+      result->chose_initial[i] = i < o->num_scales ? r.chose_initial[i] : -1;
+    }
+    result->residual_count = r.residual_count;
+    result->residual_sum = r.residual_sum;
+    result->passes = r.passes;
+    result->kernel_launches = static_cast<uint32_t>(h->launches - launches_before);
+  }
+  return BBA_OK;
+}
+
+bba_status bba_odometry_get_level(bba_handle h, int which, int scale, float* host_depth, uint16_t* host_normals, uint8_t* host_color,
+                                  int* width, int* height, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  auto& st = h->odo;
+  if (which < 0 || which > 1 || scale < 0 || scale >= st.last_num_scales || (which == 1 && scale < st.last_first_scale))
+    return Fail(h, BBA_ERR_STATE, "bba_odometry_get_level: this level was not built by the last bba_track_frame_pairwise call");
+  const bba::odom::Image& im = which ? st.level[scale].tracked : st.level[scale].base;
+  const int w = st.w[scale], ht = st.h[scale];
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (host_depth) BBA_CUDA(h, cudaMemcpy2DAsync(host_depth, sizeof(float) * w, im.depth, sizeof(float) * im.depth_pitch, sizeof(float) * w, ht, cudaMemcpyDeviceToHost, s));
+  if (host_normals) BBA_CUDA(h, cudaMemcpy2DAsync(host_normals, sizeof(uint16_t) * w, im.normals, im.normals_pitch, sizeof(uint16_t) * w, ht, cudaMemcpyDeviceToHost, s));
+  if (host_color) BBA_CUDA(h, cudaMemcpy2DAsync(host_color, w, im.color, im.color_pitch, w, ht, cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  if (width) *width = w;
+  if (height) *height = ht;
+  return BBA_OK;
+}
+
+bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, const float pose_a[7], const float pose_b[7], float H[21],
+                                     float b[6], uint32_t* residual_count, float* residual_sum, uint32_t counts[2], float costs[2], void* stream) {
+  if (!h || !pose_a) return BBA_ERR_INVALID_ARGUMENT;
+  auto& st = h->odo;
+  if (scale < st.last_first_scale || scale >= st.last_num_scales)
+    return Fail(h, BBA_ERR_STATE, "bba_odometry_debug_coeffs: this level was not built by the last bba_track_frame_pairwise call");
+  if (bba_status s2 = LaunchOdometryKernel(h, st.last_num_scales, st.last_first_scale, 1, use_gradmag ? 1 : 0, 0, scale, pose_a,
+                                           pose_b ? pose_b : pose_a, static_cast<cudaStream_t>(stream)))
+    return s2;
+  const double* d = st.h_result->debug;
+  if (H) for (int i = 0; i < 21; ++i) H[i] = static_cast<float>(d[i]);
+  if (b) for (int i = 0; i < 6; ++i) b[i] = static_cast<float>(d[21 + i]);
+  if (residual_count) *residual_count = static_cast<uint32_t>(d[27] + 0.5);
+  if (residual_sum) *residual_sum = static_cast<float>(d[28]);
+  if (counts) { counts[0] = static_cast<uint32_t>(d[32] + 0.5); counts[1] = static_cast<uint32_t>(d[34] + 0.5); }
+  if (costs) { costs[0] = static_cast<float>(d[33]); costs[1] = static_cast<float>(d[35]); }
+  return BBA_OK;
+}
+
+bba_status bba_preprocess_frame(bba_handle h, const bba_preprocess_options* o,
+                                const uint16_t* device_raw_depth, size_t raw_depth_pitch,
+                                const uint8_t* device_rgb, size_t rgb_pitch,
+                                uint16_t* device_depth, size_t depth_pitch,
+                                uint16_t* device_normals, size_t normals_pitch,
+                                uint16_t* device_radius, size_t radius_pitch,
+                                uint8_t* device_color_rgba, size_t color_pitch,
+                                float* min_depth, float* max_depth, void* stream) {
+  return PreprocessFrame(h, "bba_preprocess_frame", o, device_raw_depth, raw_depth_pitch, device_rgb, rgb_pitch, device_depth,
+                         depth_pitch, device_normals, normals_pitch, device_radius, radius_pitch, device_color_rgba, color_pitch,
+                         min_depth, max_depth, stream, nullptr);
+}
+
+bba_status bba_preprocess_raw_frame(bba_handle h, const bba_raw_frame_options* o,
+                                    const uint16_t* device_raw_depth, size_t raw_depth_pitch,
+                                    int raw_depth_width, int raw_depth_height,
+                                    const uint8_t* device_rgb, size_t rgb_pitch, int rgb_width, int rgb_height,
+                                    uint16_t* device_depth, size_t depth_pitch,
+                                    uint16_t* device_normals, size_t normals_pitch,
+                                    uint16_t* device_radius, size_t radius_pitch,
+                                    uint8_t* device_color_rgba, size_t color_pitch,
+                                    float* min_depth, float* max_depth, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (!o) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: null argument");
+  const int n = o->median_filter_and_densify_iterations, ld = o->pyramid_level_for_depth, lc = o->pyramid_level_for_color;
+  if (n < 0 || ld < 0 || lc < 0)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: iteration counts and pyramid levels must not be negative");
+  if (n > bba::pre::kMaxMedianIterations)
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: at most 8 median filter and densify iterations are supported");
+  if (ld > bba::pre::kMaxPyramidLevel || lc > bba::pre::kMaxPyramidLevel)
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: pyramid levels above 3 are not supported");
+  if (n > 0 && ld > 0)   // bad_slam.cc:671-673
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: Simultaneous downscaling and median filtering of depth maps is not implemented.");
+  const int w = h->cfg.depth_width, hh = h->cfg.depth_height, cw = h->cfg.color_width, ch = h->cfg.color_height;
+  // Camera::Scaled(2^-L) (camera.h:1696-1704): int(factor * W + 0.5)
+  const auto scaled = [](int size, int level) { return static_cast<int>(static_cast<double>(size) / (1 << level) + 0.5f); };
+  if (raw_depth_width <= 0 || raw_depth_height <= 0 || scaled(raw_depth_width, ld) != w || scaled(raw_depth_height, ld) != hh)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: the depth camera is " + std::to_string(w) + "x" +
+                std::to_string(hh) + ", not the raw depth's " + std::to_string(raw_depth_width) + "x" +
+                std::to_string(raw_depth_height) + " scaled to pyramid level " + std::to_string(ld));
+  if (raw_depth_width > (w << ld) || raw_depth_height > (hh << ld))
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_preprocess_raw_frame: raw depth sizes above depth camera size x 2^level give boxes "
+                "of more than 2^level pixels per axis, which the median selection does not hold");
+  if (device_rgb && (rgb_width != (cw << lc) || rgb_height != (ch << lc)))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: the rgb image must be the colour camera's size x 2^" +
+                std::to_string(lc) + " (" + std::to_string(cw << lc) + "x" + std::to_string(ch << lc) + ", even at every level), not " +
+                std::to_string(rgb_width) + "x" + std::to_string(rgb_height));
+  const RawStage raw_stage{n, ld, raw_depth_width, raw_depth_height, lc};
+  return PreprocessFrame(h, "bba_preprocess_raw_frame", &o->base, device_raw_depth, raw_depth_pitch, device_rgb, rgb_pitch,
+                         device_depth, depth_pitch, device_normals, normals_pitch, device_radius, radius_pitch, device_color_rgba,
+                         color_pitch, min_depth, max_depth, stream, (n | ld | lc) ? &raw_stage : nullptr);
+}
+
+}  // extern "C"

@@ -1,0 +1,361 @@
+// handle.hpp -- the library handle (bba_context) and what the host units of libbadba_b200 share: the owners of device / pinned
+// memory, events and textures, the keyframe record, error reporting and the helpers that more than one unit calls.
+//
+// Host units: badba.cu (handle, setters / getters, keyframes, textures, bba_host_*), pose_step.cu (spatial order, pose step),
+// bundle_adjust.cu (BA schemes, intrinsics, PCG, surfel lifecycle), multi_gpu.cu (sharding, exchange, peer replicas),
+// frames.cu (odometry, preprocessing).  None of them contains a kernel.
+#pragma once
+
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdio>
+#include <cstdlib>
+#include <string>
+#include <vector>
+
+#include "../../include/badba.h"
+#include "host_math.hpp"
+#include "kernels.cuh"
+#include "odometry.cuh"
+
+namespace bba {
+
+// ---- owners ------------------------------------------------------------------------------------------------------------------
+// One CUDA resource (a pointer, event, array or texture object) that Free releases when its owner is destroyed or assigned to.
+template <class R, auto Free>
+struct Owned {
+  R r{};
+  Owned() = default;
+  Owned(Owned&& o) noexcept : r(o.r) { o.r = R{}; }
+  Owned& operator=(Owned&& o) noexcept {
+    Owned old(std::move(*this));
+    r = o.r;
+    o.r = R{};
+    return *this;
+  }
+  ~Owned() {
+    if (r) Free(r);
+  }
+  operator R() const { return r; }
+};
+
+// `count` elements of T from Alloc, released by Free.  Reserve(need, alloc) grows on demand: nothing happens when the buffer
+// exists and holds `need` elements; otherwise the old buffer is freed first and max(need, alloc) elements are allocated (alloc:
+// headroom for later growth).  Pointer and capacity change together, after the allocation succeeded; a failed call leaves no
+// buffer.
+template <class T, cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+class Buffer {
+ public:
+  cudaError_t Reserve(size_t need, size_t alloc = 0) {
+    if (p_.r && need <= count_) return cudaSuccess;
+    p_ = {};
+    count_ = 0;
+    void* p = nullptr;
+    if (cudaError_t e = Alloc(&p, sizeof(T) * std::max(need, alloc))) return e;
+    p_.r = static_cast<T*>(p);
+    count_ = std::max(need, alloc);
+    return cudaSuccess;
+  }
+  T* get() const { return p_.r; }
+  operator T*() const { return p_.r; }
+  T* operator->() const { return p_.r; }
+
+ private:
+  Owned<T*, Free> p_;
+  size_t count_ = 0;
+};
+
+inline cudaError_t MappedAlloc(void** p, size_t bytes) { return cudaHostAlloc(p, bytes, cudaHostAllocMapped); }
+template <class T> using DeviceBuffer = Buffer<T, cudaMalloc, cudaFree>;
+template <class T> using PinnedBuffer = Buffer<T, cudaMallocHost, cudaFreeHost>;
+template <class T> using MappedBuffer = Buffer<T, MappedAlloc, cudaFreeHost>;   // pinned host memory the device can address
+
+// A pitched 2-D device image; Allocate (re)allocates it, and a failed call leaves no image.
+class PitchedBuffer {
+ public:
+  cudaError_t Allocate(size_t width_bytes, size_t height) {
+    p_ = {};
+    pitch_ = 0;
+    void* p = nullptr;
+    size_t pitch = 0;
+    if (cudaError_t e = cudaMallocPitch(&p, &pitch, width_bytes, height)) return e;
+    p_.r = p;
+    pitch_ = pitch;
+    return cudaSuccess;
+  }
+  template <class T = uint8_t> T* get() const { return static_cast<T*>(p_.r); }
+  size_t pitch() const { return pitch_; }
+  explicit operator bool() const { return p_.r != nullptr; }
+
+ private:
+  Owned<void*, cudaFree> p_;
+  size_t pitch_ = 0;
+};
+
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+
+// A texture object and, when the texture reads a CUDA array, that array (released after the texture).
+struct Texture {
+  Owned<cudaArray_t, cudaFreeArray> array;
+  Owned<cudaTextureObject_t, cudaDestroyTextureObject> tex;
+};
+
+// ---- keyframes ---------------------------------------------------------------------------------------------------------------
+struct Keyframe {
+  // what the kernels read: the caller's buffers, or the owned copies below
+  const uint16_t* depth = nullptr;
+  const uint16_t* normals = nullptr;
+  const uint16_t* radius = nullptr;
+  size_t depth_pitch = 0, normals_pitch = 0, radius_pitch = 0;
+  cudaTextureObject_t tex = 0;     // luma.tex, or a texture the entry borrows
+  const uint8_t* rgba = nullptr;   // uchar4 colour image (caller-owned, or owned_rgba): surfel colours at creation
+  size_t rgba_pitch = 0;
+  PitchedBuffer owned[3];          // depth / normals / radius copies made by bba_add_keyframe_host
+  PitchedBuffer owned_rgba;
+  Texture luma;                    // library-owned u8 CUDA array (the .w channel of the colour image) + its texture
+  int last_active_in_ba_iteration = -1;   // keyframe.cc:47-48
+  int last_covis_in_ba_iteration = -1;
+  Pose pose;                 // global_T_frame
+  int activation = BBA_KF_ACTIVE;
+  float min_depth = 0.f, max_depth = 0.f;
+  Frustum frustum;
+  std::vector<int> covis;
+};
+
+}  // namespace bba
+
+struct bba_context {
+  bba_config cfg;
+  float depth_K[4], color_K[4];
+  float depth_a = 0.f;
+  int cf_w = 0, cf_h = 0;
+  int sm_count = 132;
+  std::string error;
+
+  float* surfels = nullptr;
+  size_t surfel_pitch_bytes = 0;
+  uint32_t surfels_size = 0;
+  uint8_t* active = nullptr;
+  bba::DeviceBuffer<float> owned_surfels;   // bba_set_surfels_host
+  size_t owned_surfel_pitch = 0;
+  bba::DeviceBuffer<uint8_t> owned_active;
+
+  bba::DeviceBuffer<float> d_cfactor;
+  std::vector<bba::Keyframe> keyframes;
+  bba::DeviceBuffer<bba::KfDevice> d_kfs;   // [max_kf] the keyframes' parameters as the kernels read them
+
+  // staging: pinned records and the shared planes of the keyframe / frame uploads
+  struct Staging {
+    bba::PinnedBuffer<bba::KfDevice> h_kfs;
+    bba::Event event;      // recorded after the last upload from the pinned staging buffers
+    bool pending = false;
+    bba::PitchedBuffer luma;    // u8 plane staging for the luma arrays
+    bba::Event luma_free;       // recorded after the staging plane was consumed; the next user (any stream) waits on it
+    bba::PitchedBuffer color;   // uchar4 staging image for bba_update_keyframe_host
+    bba::Texture scratch;       // luma array + texture of a frame that is not a keyframe (frame pose, odometry)
+  } staging;
+
+  // pose step (pose_step.cu) and the spatial order of the surfels
+  struct PoseStep {
+    bba::DeviceBuffer<bba::KfDevice> d_work_records;   // [max_kf] the pose kernel's work list as contiguous records
+    bba::DeviceBuffer<float> d_pose_est;
+    bba::DeviceBuffer<double> d_acc;
+    bba::DeviceBuffer<unsigned long long> d_stage_counts;
+    bba::DeviceBuffer<int> d_work[2];
+    bba::DeviceBuffer<int> d_count;   // 2 ints
+    bba::DeviceBuffer<int> d_iterations;
+    bba::DeviceBuffer<int> d_converged;
+    bba::DeviceBuffer<double> d_first_stats;
+    bba::DeviceBuffer<unsigned long long> d_totals;   // [8]
+    bba::DeviceBuffer<unsigned int> d_queue;          // work-item counter of the pose kernel
+    bba::MappedBuffer<int> flag;         // 4 ints
+    volatile int* h_flag = nullptr;      // flag: {iterations completed, work items left}
+    int* d_flag = nullptr;               // device alias of h_flag
+    bba::PinnedBuffer<float> h_pose_est;
+    bba::PinnedBuffer<int> h_work;   // max_kf + 2
+    bba::PinnedBuffer<int> h_iterations;
+    bba::PinnedBuffer<int> h_converged;
+    bba::PinnedBuffer<double> h_first_stats;
+    bba::PinnedBuffer<unsigned long long> h_totals;
+    // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream).
+    // The order is rebuilt at the start of every BA call, after an in-loop change of the surfel set, and whenever the surfel
+    // count differs from the one it was built for; in between it may lag behind the positions, which costs culling, never
+    // correctness.
+    struct Order {
+      bba::DeviceBuffer<uint32_t> words;       // keys in / out, index, perm, 8 bound words
+      bba::DeviceBuffer<unsigned char> temp;   // CUB scratch
+      bba::DeviceBuffer<float> stream;         // [kPoseStreamRows][capacity], rebuilt at the start of a pose step
+      bba::DeviceBuffer<float> boxes;          // [capacity / kSpatialChunk][8]
+      bba::SpatialOrderBuffers view{};
+      uint32_t capacity = 0;                   // also the stream's pitch
+    } order;
+    uint32_t order_n = 0;
+    bool order_stale = true;
+  } pose;
+
+  // geometry step and intrinsics step (bundle_adjust.cu)
+  struct Geometry {
+    bba::DeviceBuffer<int> d_list;
+    bba::PinnedBuffer<int> h_list;
+    bba::DeviceBuffer<unsigned int> d_queue;        // work-item counter of the geometry kernels
+    bba::DeviceBuffer<unsigned int> d_tile_epoch;   // per-tile group epochs of the geometry kernels
+    // intrinsics step: [head 64 | B 5P | D P | b2 P | obs P | x1 8] floats + 34 fp64 sums
+    bba::DeviceBuffer<float> d_intr;
+    bba::DeviceBuffer<double> d_intr_sums;
+    bba::DeviceBuffer<int> d_all_list;   // 0 .. max_kf-1
+    bba::PinnedBuffer<double> h_intr_sums;
+    bba::PinnedBuffer<float> h_intr_x1;   // 8 floats
+  } geo;
+
+  // in-loop surfel lifecycle (creation / merge / compaction) and the end tasks
+  struct Lifecycle {
+    bba::DeviceBuffer<unsigned int> d_sup;         // [3][cells]
+    bba::DeviceBuffer<unsigned int> d_cell_bits;   // [cells]
+    bba::DeviceBuffer<unsigned int> d_flags;       // [w * h]
+    bba::DeviceBuffer<unsigned int> d_scan_out;    // [w * h]
+    bba::DeviceBuffer<unsigned int> d_scan_sums;
+    bba::DeviceBuffer<bba::CovisEntry> d_covis;    // [max_keyframes]
+    bba::PinnedBuffer<bba::CovisEntry> h_covis;
+    bba::DeviceBuffer<bba::KfRadius> d_kf_radius;  // [max_keyframes]
+    bba::PinnedBuffer<bba::KfRadius> h_kf_radius;
+    bba::DeviceBuffer<unsigned int> d_deleted_count;
+    bba::PinnedBuffer<unsigned int> h_deleted_count;
+    bba::DeviceBuffer<unsigned int> d_compact_sums;
+  } life;
+  int last_ba_iteration_count = -1;   // direct_ba.cc:126
+
+  // PCG solver: r, M, delta, g, p
+  struct Pcg {
+    bba::DeviceBuffer<float> d_vec[5];
+    bba::DeviceBuffer<double> d_scalars;   // [0] / [2] alpha_n, beta_n (roles swap), [1] alpha_d
+    bba::PinnedBuffer<double> h_scalars;
+    bba::PinnedBuffer<float> h_delta;      // pose part (6 * max_keyframes) + 16
+  } pcg;
+
+  // multi-GPU exchange (multi_gpu.cu)
+  struct Exchange {
+    bba_collective_fn collective = nullptr;
+    void* collective_user = nullptr;
+    bba::DeviceBuffer<float> d_exchange;    // [world][kShardRows][shard_len] floats
+    bba::DeviceBuffer<float> d_pose_pack;   // [max_kf][kPoseSlot] floats
+    bba::PinnedBuffer<float> h_pose_pack;
+    bba::DeviceBuffer<int> d_local_ids;     // [max_kf]
+    bba::DeviceBuffer<float> d_count_xchg;  // [2] deleted count of this rank's shard for the sum all-reduce
+    bba::PinnedBuffer<float> h_count_xchg;
+    bba::DeviceBuffer<float> d_barrier;
+    // NVLink peer replicas (bba_peer_import)
+    bba::PeerSet peers{};                       // count == 0: not mapped
+    void* peer_bases[2 * bba::kMaxPeers] = {};  // what cudaIpcOpenMemHandle returned (closed on unmap)
+    int peer_base_count = 0;
+    // With mapped peers: set by every REPLICATED whole-buffer pass (surfel creation / merge / compaction / end tasks), cleared
+    // by the next collective.  The geometry kernels store into the other ranks' replicas; a rank must not start them while a
+    // slower rank is still reading or rewriting its whole replica in such a pass (PeerFence).
+    bool replicated_pass_pending = false;
+  } xchg;
+
+  // image-pair odometry (bba_track_frame_pairwise), lazily allocated: intensity / gradient-magnitude images of both frames
+  // (colour-sized), the depth / normal / colour pyramids of both frames, accumulators + barrier + result of the persistent kernel
+  struct Odometry {
+    int num_scales = 0;          // levels allocated
+    int last_num_scales = 0;     // levels filled by the last call (parity hooks)
+    int last_first_scale = 0;
+    bba::PitchedBuffer gradmag[2];
+    bba::Texture gradmag_tex[2];
+    bba::odom::Image image[2][bba::odom::kMaxScales] = {};   // [0 base | 1 tracked][scale]; views of the planes below
+    bba::PitchedBuffer depth[2][bba::odom::kMaxScales], normals[2][bba::odom::kMaxScales], color[2][bba::odom::kMaxScales];
+    bba::Texture color_tex[2][bba::odom::kMaxScales];
+    int w[bba::odom::kMaxScales] = {}, h[bba::odom::kMaxScales] = {};
+    bba::odom::Level level[bba::odom::kMaxScales] = {};      // as passed to the last launch
+    bba::DeviceBuffer<double> d_acc;             // [3][32]
+    bba::DeviceBuffer<unsigned int> d_barrier;   // [2]
+    bba::DeviceBuffer<bba::odom::TrackResult> d_result;
+    bba::PinnedBuffer<bba::odom::TrackResult> h_result;
+  } odo;
+
+  // keyframe preprocessing (bba_preprocess_frame)
+  struct Preprocess {
+    bba::DeviceBuffer<float> d_min_max;
+    bba::PinnedBuffer<float> h_min_max;
+  } pre;
+
+  uint64_t launches = 0;
+  int ba_iteration_count = 0;
+  // predicted cost of one pose step per keyframe (Gauss-Newton iterations x per-evaluation cost of the last step it took
+  // part in); 0 = unknown.  Identical on every rank; drives the keyframe -> rank assignment of the pose step.
+  std::vector<float> kf_cost;
+
+  // profiling (bba_set_profiling)
+  int profiling = 0;   // 0 off, 1 event timing, 2 event timing + byte-model counters in every iteration
+  bba_profile profile;
+  bba::Event prof_ev[64];
+  bba::Event ev[6];
+};
+
+namespace bba {
+
+bba_status Fail(bba_handle h, bba_status s, const std::string& msg);
+
+#define BBA_CUDA(h, expr)                                                                                  \
+  do {                                                                                                      \
+    cudaError_t e__ = (expr);                                                                               \
+    if (e__ != cudaSuccess)                                                                                 \
+      return Fail(h, BBA_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e__));                    \
+  } while (0)
+
+// BADBA_TRACE=1: stage markers on stderr (debugging aid for host-side faults)
+#define BBA_TRACE(msg)                                                                   \
+  do {                                                                                   \
+    static const bool on__ = std::getenv("BADBA_TRACE") != nullptr;                      \
+    if (on__) { std::fprintf(stderr, "[badba] %s:%d %s\n", __func__, __LINE__, msg); std::fflush(stderr); } \
+  } while (0)
+
+#define CHECK_KF(h, id)                                                                   \
+  if (!(h)) return BBA_ERR_INVALID_ARGUMENT;                                              \
+  if ((id) < 0 || (id) >= static_cast<int>((h)->keyframes.size())) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bad keyframe id")
+
+// badba.cu
+Pose PoseFromArray(const float p[7]);
+void PoseToArray(const Pose& r, float p[7]);
+CameraParams MakeCamera(bba_handle h);
+bba_status WaitStaging(bba_handle h);
+bba_status MarkStaging(bba_handle h, cudaStream_t s);
+void FillKfDevice(const Keyframe& kf, const Pose& global_T_frame, KfDevice* d);
+bba_status UploadKeyframes(bba_handle h, cudaStream_t s);
+bba_status CheckSurfels(bba_handle h);
+// Whether the depth / normal / colour pitches of a frame hold rows of the configured image sizes (and fit kernel arguments).
+bool FramePitchesOk(bba_handle h, size_t depth_pitch, size_t normals_pitch, size_t color_pitch);
+// Clamp addressing, linear filtering, normalised float reads and unnormalised coordinates (keyframe.cc:67-73, and
+// CUDABuffer::CreateTextureObject as pairwise_frame_tracking.cc:57-79 calls it).
+cudaTextureDesc LinearTextureDesc();
+// The camera, the surfel buffer, its pitch in floats and the surfel count in kernel arguments.
+template <class Args> void SetSurfelFields(bba_handle h, Args* a) {
+  a->cam = MakeCamera(h);
+  a->surfels = h->surfels;
+  a->pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
+  a->n = h->surfels_size;
+}
+bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t color_pitch, Texture* luma, cudaStream_t s);
+
+// pose_step.cu
+bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, int max_iterations, cudaStream_t s);
+
+// multi_gpu.cu
+void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t* shard_len);
+uint32_t LocalCountBelow(uint32_t global_end, int rank, int world);
+void AssignKeyframes(bba_handle h, const std::vector<int>& ids, std::vector<int>* owner);
+bba_status CheckCollective(bba_handle h);
+bba_status PeerFence(bba_handle h, cudaStream_t s);
+bba_status ExchangeGeometry(bba_handle h, cudaStream_t s);
+bba_status ReserveExchange(bba_handle h, size_t need);
+void UnmapPeers(bba_handle h);
+
+// The range of this rank's surfel shard (all surfels on one GPU) in kernel arguments.
+template <class Args> void SetShardFields(bba_handle h, Args* a) {
+  a->begin = 0;
+  a->shard_rank = static_cast<uint32_t>(h->cfg.rank);
+  a->shard_world = static_cast<uint32_t>(h->cfg.world_size);
+  ShardSurfels(h->surfels_size, h->cfg.rank, h->cfg.world_size, &a->end, nullptr);
+}
+
+}  // namespace bba

@@ -227,4 +227,97 @@ BBA_HD void SolveLDLT(const double* upper, const double* b, double* x) {
   for (int i = 0; i < N; ++i) x[perm[i]] = y[i];
 }
 
+// Camera frusta and their intersection test (co-visibility of keyframes), host only.
+struct Frustum {   // libvis/src/libvis/camera_frustum.h:43-250
+  float p[8][3];
+  float bmin[3], bmax[3];
+  float axes[6][3];
+  float plane_n[6][3];
+  float plane_d[6];
+};
+
+inline void Sub(const float a[3], const float b[3], float o[3]) { o[0] = a[0] - b[0]; o[1] = a[1] - b[1]; o[2] = a[2] - b[2]; }
+inline void CrossP(const float a[3], const float b[3], float o[3]) {
+  o[0] = a[1] * b[2] - a[2] * b[1];
+  o[1] = a[2] * b[0] - a[0] * b[2];
+  o[2] = a[0] * b[1] - a[1] * b[0];
+}
+inline float DotP(const float a[3], const float b[3]) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+
+inline void MakeFrustum(Frustum* f, const float K[4], int width, int height, float min_depth, float max_depth, const Pose& global_T_cam) {
+  float M[12];
+  ToMatrix3x4(global_T_cam, M);
+  for (int i = 0; i < 3; ++i) {
+    f->bmin[i] = INFINITY;
+    f->bmax[i] = -INFINITY;
+  }
+  // corner order of camera_frustum.h:155-177: top-left, top-right, bottom-left, bottom-right; min then max depth
+  const float cx[4] = {0.f, static_cast<float>(width), 0.f, static_cast<float>(width)};
+  const float cy[4] = {0.f, 0.f, static_cast<float>(height), static_cast<float>(height)};
+  for (int c = 0; c < 4; ++c) {
+    const float dx = (cx[c] - K[2]) / K[0], dy = (cy[c] - K[3]) / K[1];   // UnprojectFromPixelCornerConv
+    for (int d = 0; d < 2; ++d) {
+      const float depth = d ? max_depth : min_depth;
+      const float v[3] = {depth * dx, depth * dy, depth};
+      float* o = f->p[2 * c + d];
+      for (int r = 0; r < 3; ++r) {
+        o[r] = M[r * 4] * v[0] + M[r * 4 + 1] * v[1] + M[r * 4 + 2] * v[2] + M[r * 4 + 3];
+        f->bmin[r] = fminf(f->bmin[r], o[r]);
+        f->bmax[r] = fmaxf(f->bmax[r], o[r]);
+      }
+    }
+  }
+  // camera_frustum.h:180-218
+  Sub(f->p[7], f->p[6], f->axes[0]);
+  Sub(f->p[3], f->p[2], f->axes[1]);
+  Sub(f->p[5], f->p[4], f->axes[2]);
+  Sub(f->p[1], f->p[0], f->axes[3]);
+  Sub(f->p[2], f->p[6], f->axes[4]);
+  Sub(f->p[0], f->p[2], f->axes[5]);
+  float fwd[3];
+  CrossP(f->axes[5], f->axes[4], fwd);
+  for (int i = 0; i < 3; ++i) {
+    f->plane_n[0][i] = fwd[i];
+    f->plane_n[1][i] = -fwd[i];
+  }
+  f->plane_d[0] = -DotP(fwd, f->p[1]);
+  f->plane_d[1] = DotP(fwd, f->p[0]);
+  CrossP(f->axes[0], f->axes[4], f->plane_n[2]); f->plane_d[2] = -DotP(f->plane_n[2], f->p[6]);
+  CrossP(f->axes[1], f->axes[5], f->plane_n[3]); f->plane_d[3] = -DotP(f->plane_n[3], f->p[2]);
+  CrossP(f->axes[4], f->axes[2], f->plane_n[4]); f->plane_d[4] = -DotP(f->plane_n[4], f->p[4]);
+  CrossP(f->axes[5], f->axes[0], f->plane_n[5]); f->plane_d[5] = -DotP(f->plane_n[5], f->p[6]);
+}
+
+inline bool AllOutside(const Frustum& planes_of, const Frustum& points_of) {
+  for (int pl = 0; pl < 6; ++pl) {
+    int v = 0;
+    for (; v < 8; ++v)
+      if (DotP(planes_of.plane_n[pl], points_of.p[v]) + planes_of.plane_d[pl] < 0) break;
+    if (v == 8) return true;
+  }
+  return false;
+}
+
+inline bool FrustaIntersect(const Frustum& a, const Frustum& b) {   // camera_frustum.h:73-143
+  for (int i = 0; i < 3; ++i)
+    if (fmaxf(a.bmin[i], b.bmin[i]) > fminf(a.bmax[i], b.bmax[i])) return false;
+  if (AllOutside(a, b) || AllOutside(b, a)) return false;
+  // Separating-axis part.  The reference crosses two edge directions of the SAME frustum (camera_frustum.h:122
+  // uses axes_[this_edge] and axes_[other_edge], both members of `this`); kept as is for parity.
+  for (int e1 = 0; e1 < 6; ++e1)
+    for (int e2 = 0; e2 < 6; ++e2) {
+      float dir[3];
+      CrossP(a.axes[e1], a.axes[e2], dir);
+      if (DotP(dir, dir) < 1e-5f) continue;
+      float amin = INFINITY, amax = -INFINITY, bmin = INFINITY, bmax = -INFINITY;
+      for (int p = 0; p < 8; ++p) {
+        const float va = DotP(dir, a.p[p]), vb = DotP(dir, b.p[p]);
+        amin = fminf(amin, va); amax = fmaxf(amax, va);
+        bmin = fminf(bmin, vb); bmax = fmaxf(bmax, vb);
+      }
+      if (amax <= bmin || amin >= bmax) return false;
+    }
+  return true;
+}
+
 }  // namespace bba

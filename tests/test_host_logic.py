@@ -1,4 +1,4 @@
-"""CPU-only: the product's HOST arithmetic (badslam_b200/csrc/host_math.hpp and the frustum code of badba.cu, exported through the
+"""CPU-only: the product's HOST arithmetic (badslam_b200/csrc/host_math.hpp, including the frustum code, exported through the
 device-free bba_host_* entry points of include/badba.h) against the oracle's independent C versions, numpy and closed forms."""
 import ctypes as C
 

@@ -140,7 +140,7 @@ def test_keyframe_balancing_rule():
 
 
 def _worker_round2(rank, world, port, n, K, out_dir):
-    """The exchange patterns added in round 2 (badba.cu BundleAdjustPCG / PerformEndTasks with world_size > 1), with the same
+    """The exchange patterns added in round 2 (bundle_adjust.cu BundleAdjustPCG / PerformEndTasks with world_size > 1), with the same
     arithmetic on the host: (1) PCG products -- every rank sums over ITS surfels only, one fp32 sum all-reduce of the vector with the
     rank's fp64 part of alpha_d appended as a (high, low) float pair; (2) end tasks -- the two result rows of a rank's shard through
     the all-gather, the deleted count as two exactly representable floats through a sum all-reduce."""
