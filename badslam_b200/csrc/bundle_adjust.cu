@@ -28,15 +28,35 @@ bba_status ReserveTileEpochs(bba_handle h) {
   return BBA_OK;
 }
 
-bba_status BuildGeometryArgs(bba_handle h, bba::GeometryArgs* g, cudaStream_t s) {
-  if (bba_status st = PeerFence(h, s)) return st;
+// In which order the geometry launches visit the surfels.  kCaller: the caller's (the in-loop creation's two launches address the
+// old and the new surfels by caller index, the PCG scheme's shards are the caller's granules).  kByPairs: the spatial order from
+// kSpatialOrderMinPairs (surfel, keyframe) pairs per launch, the pose step's rule (the pose step then reuses the order).
+// kSpatial: always the spatial order (the standalone entry points, like the forced pose variants).
+enum class GeoOrder { kCaller, kByPairs, kSpatial };
+
+bba_status BuildGeometryArgs(bba_handle h, bba::GeometryArgs* g, cudaStream_t s, GeoOrder order) {
   const int K = static_cast<int>(h->keyframes.size());
   int cnt = 0;
   for (int k = 0; k < K; ++k)
     if (h->keyframes[k].activation != BBA_KF_INACTIVE) h->geo.h_list[cnt++] = k;
   if (cnt) BBA_CUDA(h, cudaMemcpyAsync(h->geo.d_list, h->geo.h_list, sizeof(int) * cnt, cudaMemcpyHostToDevice, s));
+  // With several ranks the order is rebuilt here from the replicated positions, so that every rank deals the same granules (the
+  // pose step sorts by its own share of the keyframes, so a current order need not be the same on every rank).  With mapped peers
+  // (stores into the other ranks' replicas) the launches keep the caller's order: in spatial order that mode left about 3 % of
+  // the surfels different from the one-GPU result in a two-rank run, for a reason not yet found, while the host-collective
+  // exchange in spatial order reproduces it bit for bit.
+  const bool peer_stores = h->cfg.world_size > 1 && h->xchg.peers.count == h->cfg.world_size - 1;
+  const bool sort = !peer_stores && (order == GeoOrder::kSpatial ||
+                                     (order == GeoOrder::kByPairs &&
+                                      static_cast<uint64_t>(h->surfels_size) * static_cast<uint64_t>(cnt) >= kSpatialOrderMinPairs));
+  if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/h->cfg.world_size > 1, s)) return st;
+  if (bba_status st = PeerFence(h, s)) return st;
   SetSurfelFields(h, g);
   SetShardFields(h, g);
+  g->perm = sort && h->surfels_size > 0 ? h->pose.order.view.perm : nullptr;
+  g->stream = h->pose.order.stream;
+  g->stream_pitch = h->pose.order.capacity;
+  h->geo.perm = g->perm;
   g->active = h->active;
   g->kfs = h->d_kfs;
   g->kf_list = h->geo.d_list;
@@ -647,9 +667,8 @@ bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result*
     BBA_CUDA(h, cudaEventRecord(h->ev[0], s));
     if (opt_geometry && N > 0) {   // UpdateSurfelNormalsCUDA, :215-227
       bba::GeometryArgs g;
-      if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
-      bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
-      ++h->launches;
+      if (bba_status st = BuildGeometryArgs(h, &g, s, GeoOrder::kCaller)) return st;
+      h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
       if (bba_status st = ExchangeGeometry(h, s)) return st;   // multi-GPU: every replica gets the other shards' normals
     }
     BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
@@ -732,10 +751,9 @@ bba_status bba_update_surfel_activation(bba_handle h, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (bba_status st = UploadKeyframes(h, s)) return st;
   bba::GeometryArgs g;
-  if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
+  if (bba_status st = BuildGeometryArgs(h, &g, s, GeoOrder::kSpatial)) return st;
   if (bba_status st = CheckCollective(h)) return st;
-  bba::LaunchActivationAndNormals(g, h->sm_count, true, false, s);
-  ++h->launches;
+  h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, true, false, s);
   BBA_CUDA(h, cudaGetLastError());
   if (bba_status st = ExchangeGeometry(h, s)) return st;
   return MarkStaging(h, s);
@@ -748,11 +766,10 @@ bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (bba_status st = UploadKeyframes(h, s)) return st;
   bba::GeometryArgs g;
-  if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
+  if (bba_status st = BuildGeometryArgs(h, &g, s, GeoOrder::kSpatial)) return st;
   if (bba_status st = CheckCollective(h)) return st;
-  bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
-  bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
-  h->launches += 2;
+  h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
+  h->launches += bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
   BBA_CUDA(h, cudaGetLastError());
   if (bba_status st = ExchangeGeometry(h, s)) return st;
   return MarkStaging(h, s);
@@ -828,13 +845,13 @@ bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_resul
     BBA_TRACE("creation done");
     if (bba_status st = UploadKeyframes(h, s)) return st;
     BBA_TRACE("keyframes uploaded");
+    const bool has_new = o->optimize_geometry && h->surfels_size > old_surfels_size;
     bba::GeometryArgs g;
-    if (bba_status st = BuildGeometryArgs(h, &g, s)) return st;
+    if (bba_status st = BuildGeometryArgs(h, &g, s, has_new ? GeoOrder::kCaller : GeoOrder::kByPairs)) return st;
 
     BBA_TRACE("after creation + upload");
     // --- surfel activation (:432-456) fused with the normal update of the geometry step (:466-485)
     BBA_CUDA(h, cudaEventRecord(h->ev[0], s));
-    const bool has_new = o->optimize_geometry && h->surfels_size > old_surfels_size;
     if (has_new)   // new surfels are active (:435-441); only the old ones are re-evaluated below
       BBA_CUDA(h, cudaMemsetAsync(h->active + old_surfels_size, bba::kSurfelActiveFlag, h->surfels_size - old_surfels_size, s));
     if (!whole_window) BBA_CUDA(h, cudaMemsetAsync(h->active, bba::kSurfelActiveFlag, old_surfels_size, s));
@@ -843,21 +860,17 @@ bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_resul
         bba::GeometryArgs g_old = g, g_new = g;   // (begin / end are LOCAL indices of this rank's shard)
         g_old.end = LocalCountBelow(old_surfels_size, h->cfg.rank, h->cfg.world_size);
         g_new.begin = g_old.end;
-        bba::LaunchActivationAndNormals(g_old, h->sm_count, true, true, s);
-        bba::LaunchActivationAndNormals(g_new, h->sm_count, false, true, s);
-        h->launches += 2;
+        h->launches += bba::LaunchActivationAndNormals(g_old, h->sm_count, true, true, s);
+        h->launches += bba::LaunchActivationAndNormals(g_new, h->sm_count, false, true, s);
       } else if (whole_window) {
-        bba::LaunchActivationAndNormals(g, h->sm_count, true, o->optimize_geometry != 0, s);
-        ++h->launches;
+        h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, true, o->optimize_geometry != 0, s);
       } else if (o->optimize_geometry) {
-        bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
-        ++h->launches;
+        h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
       }
     }
     BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
     if (o->optimize_geometry && h->surfels_size > 0) {
-      bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
-      ++h->launches;
+      h->launches += bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
     }
     BBA_CUDA(h, cudaGetLastError());
     if (bba_status st = ExchangeGeometry(h, s)) return st;   // multi-GPU: all-gather of the updated surfel shards

@@ -54,6 +54,15 @@ struct __align__(16) KfDevice {
 };
 static_assert(sizeof(KfDevice) == 96, "KfDevice layout");
 
+// Order-preserving map of a float onto an unsigned int (for integer min / max reductions), and back.
+__device__ __forceinline__ unsigned int OrderedBits(float f) {
+  const unsigned int u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float FromOrderedBits(unsigned int u) {
+  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+
 struct Vec3 {
   float x, y, z;
 };

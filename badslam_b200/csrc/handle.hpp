@@ -178,14 +178,15 @@ struct bba_context {
     bba::PinnedBuffer<int> h_converged;
     bba::PinnedBuffer<double> h_first_stats;
     bba::PinnedBuffer<unsigned long long> h_totals;
-    // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream).
+    // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream); the
+    // geometry step's stream (bba::LaunchGeometryStream) shares the buffer.
     // The order is rebuilt at the start of every BA call, after an in-loop change of the surfel set, and whenever the surfel
     // count differs from the one it was built for; in between it may lag behind the positions, which costs culling, never
     // correctness.
     struct Order {
       bba::DeviceBuffer<uint32_t> words;       // keys in / out, index, perm, 8 bound words
       bba::DeviceBuffer<unsigned char> temp;   // CUB scratch
-      bba::DeviceBuffer<float> stream;         // [kPoseStreamRows][capacity], rebuilt at the start of a pose step
+      bba::DeviceBuffer<float> stream;         // [kPoseStreamRows][capacity], rebuilt at the start of a pose step / geometry launch
       bba::DeviceBuffer<float> boxes;          // [capacity / kSpatialChunk][8]
       bba::SpatialOrderBuffers view{};
       uint32_t capacity = 0;                   // also the stream's pitch
@@ -200,6 +201,7 @@ struct bba_context {
     bba::PinnedBuffer<int> h_list;
     bba::DeviceBuffer<unsigned int> d_queue;        // work-item counter of the geometry kernels
     bba::DeviceBuffer<unsigned int> d_tile_epoch;   // per-tile group epochs of the geometry kernels
+    const uint32_t* perm = nullptr;   // the order of the last geometry launches (pose.order's perm or null), for ExchangeGeometry
     // intrinsics step: [head 64 | B 5P | D P | b2 P | obs P | x1 8] floats + 34 fp64 sums
     bba::DeviceBuffer<float> d_intr;
     bba::DeviceBuffer<double> d_intr_sums;
@@ -338,6 +340,10 @@ template <class Args> void SetSurfelFields(bba_handle h, Args* a) {
 bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t color_pitch, Texture* luma, cudaStream_t s);
 
 // pose_step.cu
+// The surfel count from which a launch over n keyframes puts the surfels into spatial order: sorting costs ~0.1 ms of launches
+// plus the sort itself, more than the culling it buys on small work (PreparePoseAccumulate).
+constexpr uint64_t kSpatialOrderMinPairs = 16u << 20;   // (surfel, keyframe) pairs per launch
+bba_status EnsureSpatialOrder(bba_handle h, bool sort, bool rebuild, cudaStream_t s);
 bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, int max_iterations, cudaStream_t s);
 
 // multi_gpu.cu

@@ -102,6 +102,10 @@ struct PeerSet {
   uint8_t* active[kMaxPeers];
 };
 
+// The geometry kernels visit the surfels in stream order: local index li -> stream position s = SurfelShardToGlobal(li) -> caller
+// index perm[s] (s when perm is null).  Each launch first gathers its surfels' inputs into the geometry stream (LaunchGeo), so
+// that a warp's 32 lanes read coalesced rows and hold a compact cluster of surfels; the partial sums parked between keyframe
+// groups live in the caller's scratch rows 8..16 at column s, the results go to column perm[s] of the caller's rows.
 struct GeometryArgs {
   CameraParams cam;
   float* surfels;
@@ -109,6 +113,9 @@ struct GeometryArgs {
   uint32_t n;
   uint32_t begin, end;         // range of this rank's LOCAL surfel indices (SurfelShardToGlobal maps them; 0 .. n on one GPU)
   uint32_t shard_rank, shard_world;
+  const uint32_t* perm;        // spatial order (SpatialOrderBuffers::perm), or null: the caller's order
+  float* stream;               // kGeoStreamRows x stream_pitch, filled by the launcher in stream order
+  uint32_t stream_pitch;       // floats per row, >= n
   uint8_t* active;
   const KfDevice* kfs;
   const int* kf_list;          // non-inactive keyframes (ascending ids)
@@ -118,11 +125,18 @@ struct GeometryArgs {
   int tile_shift;              // log2(surfels per tile), 5..8; chosen by the launcher
   PeerSet peers;
 };
+// The geometry stream: x y z, packed normal, radius^2, d1, d2 and the active flags (as u32 bits) of the launch's surfels at their
+// stream positions.  It shares the pose stream's buffer (the pose step rebuilds its own rows at its start).  desc_rows: also
+// gather radius^2, d1, d2 (what the position / descriptor kernel reads with descriptors; the other launches read rows 0-3 + flags).
+constexpr int kGeoStreamRows = 8;
+static_assert(kGeoStreamRows <= kPoseStreamRows, "the geometry stream lives in the pose stream's buffer");
+void LaunchGeometryStream(const GeometryArgs& args, bool desc_rows, cudaStream_t stream);
 // SetSurfelInactive + DetermineActiveSurfels (kernel_surfel_activation.cu:38-79) fused with the normal
 // accumulation + update (kernel_opt_geometry.cu:527-597).
-void LaunchActivationAndNormals(const GeometryArgs& args, int sm_count, bool determine_activation, bool update_normals, cudaStream_t stream);
+// Both return the number of kernels launched (the stream gather and the kernel, 0 when there is nothing to launch).
+int LaunchActivationAndNormals(const GeometryArgs& args, int sm_count, bool determine_activation, bool update_normals, cudaStream_t stream);
 // Position (+ descriptor) accumulation and per-surfel solve (kernel_opt_geometry.cu:118-231,273-361 or :417-507).
-void LaunchPositionAndDescriptor(const GeometryArgs& args, int sm_count, cudaStream_t stream);
+int LaunchPositionAndDescriptor(const GeometryArgs& args, int sm_count, cudaStream_t stream);
 
 // Multi-GPU surfel sharding: 256-surfel granules are dealt round-robin to the ranks (granule g belongs to rank g % world), so
 // that every rank sees the same mix of well- and poorly-observed surfels (surfels are stored in creation order, and the
@@ -131,12 +145,13 @@ constexpr uint32_t kShardGranuleShift = 8;
 __host__ __device__ inline uint32_t SurfelShardToGlobal(uint32_t local, uint32_t rank, uint32_t world) {
   return world <= 1 ? local : ((((local >> kShardGranuleShift) * world + rank) << kShardGranuleShift) | (local & ((1u << kShardGranuleShift) - 1u)));
 }
-// Exchange of the shards: 7 rows (x y z normal d1 d2 active-as-float) x shard_len floats per rank, in local index order.
+// Exchange of the shards: 7 rows (x y z normal d1 d2 active-as-float) x shard_len floats per rank, in local index order.  The
+// shards are the geometry step's: granules of stream positions, surfel perm[s] at position s (perm null: the caller's order).
 constexpr int kShardRows = 7;
-void LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, uint32_t rank, uint32_t world,
-                     uint32_t shard_len, float* slice, cudaStream_t stream);
-void LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, uint32_t shard_len, int world, int skip_rank,
-                        const float* buffer, cudaStream_t stream);
+void LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t rank,
+                     uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream);
+void LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t shard_len, int world,
+                        int skip_rank, const float* buffer, cudaStream_t stream);
 // Pose results of the locally owned keyframes -> [K][17] floats (zeros elsewhere) for the sum all-reduce.
 constexpr int kPoseSlot = 17;   // 7 pose, iterations, converged, 8 first-iteration statistics
 void LaunchPackPoseResults(const int* ids, int n, const float* pose_est, const int* iterations, const int* converged,

@@ -104,7 +104,8 @@ bba_status ReserveExchange(bba_handle h, size_t need) {
   return BBA_OK;
 }
 
-// After the geometry step every rank has updated only its own surfel shard: one all-gather makes the replicas equal.
+// After the geometry step every rank has updated only its own surfel shard (granules of the order the geometry launches used):
+// one all-gather makes the replicas equal.
 bba_status ExchangeGeometry(bba_handle h, cudaStream_t s) {
   if (h->cfg.world_size <= 1 || h->surfels_size == 0) return BBA_OK;
   auto& x = h->xchg;
@@ -116,9 +117,9 @@ bba_status ExchangeGeometry(bba_handle h, cudaStream_t s) {
   if (bba_status st = ReserveExchange(h, static_cast<size_t>(world) * kShardRows * shard_len)) return st;
   const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
   const size_t slice_floats = static_cast<size_t>(kShardRows) * shard_len;
-  LaunchPackShard(h->surfels, pitch, h->active, h->surfels_size, rank, world, shard_len, x.d_exchange + slice_floats * rank, s);
+  LaunchPackShard(h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, rank, world, shard_len, x.d_exchange + slice_floats * rank, s);
   x.collective(x.collective_user, BBA_COLLECTIVE_ALLGATHER, x.d_exchange, slice_floats * sizeof(float), s);
-  LaunchUnpackShards(h->surfels, pitch, h->active, h->surfels_size, shard_len, world, rank, x.d_exchange, s);
+  LaunchUnpackShards(h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, shard_len, world, rank, x.d_exchange, s);
   h->launches += 2;
   BBA_CUDA(h, cudaGetLastError());
   return BBA_OK;

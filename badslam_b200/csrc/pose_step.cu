@@ -6,11 +6,10 @@
 #include "handle.hpp"
 
 namespace bba {
-namespace {
 
 // Sizes the pose stream for surfels_size surfels and, with sort, makes the spatial order of the surfels current (see
-// PoseStep::order_stale).
-bba_status EnsureSpatialOrder(bba_handle h, bool sort, cudaStream_t s) {
+// PoseStep::order_stale); with rebuild it is sorted again even when it is current.
+bba_status EnsureSpatialOrder(bba_handle h, bool sort, bool rebuild, cudaStream_t s) {
   auto& p = h->pose;
   const uint32_t n = h->surfels_size;
   if (n > p.order.capacity) {
@@ -32,7 +31,7 @@ bba_status EnsureSpatialOrder(bba_handle h, bool sort, cudaStream_t s) {
     p.order.view.temp_bytes = sort_bytes;
     p.order.capacity = cap;
   }
-  if (sort && (p.order_stale || p.order_n != n)) {
+  if (sort && (rebuild || p.order_stale || p.order_n != n)) {
     LaunchSpatialOrder(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), n, p.order.view, s);
     BBA_CUDA(h, cudaGetLastError());
     h->launches += 3;   // bounds, keys, the sort (counted as one)
@@ -41,6 +40,8 @@ bba_status EnsureSpatialOrder(bba_handle h, bool sort, cudaStream_t s) {
   }
   return BBA_OK;
 }
+
+namespace {
 
 // Launch setup of the pose kernel, shared by the pose step and the entry points that evaluate it at a fixed state: arguments
 // over the handle's buffers (the caller sets work_list / work_count) and, for a PRE variant, the pose stream built on s.
@@ -65,11 +66,11 @@ bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStre
     // The rebuild (bounds, keys, radix sort) has a fixed cost of ~0.1 ms, most of it launch overhead at the start of a pose step
     // whose stream has just drained: measured on cfg2 (20 keyframes x 200 k surfels) it cost more than the culling it buys, on
     // cfg3_rank8 (200 x 375 k) it paid for itself many times over.  Below kSpatialOrderMinPairs (surfel, keyframe) pairs per
-    // launch the stream keeps the caller's order; its chunk boxes are culled all the same.  A forced variant always sorts.
-    constexpr uint64_t kSpatialOrderMinPairs = 16u << 20;
+    // launch the stream keeps the caller's order; its chunk boxes are culled all the same.  A forced variant always sorts.  (In a
+    // BA iteration the geometry step has usually made the order current already.)
     const bool sort = variant != kPoseVariantAuto ||
                       static_cast<uint64_t>(h->surfels_size) * static_cast<uint64_t>(n_work) >= kSpatialOrderMinPairs;
-    if (bba_status st = EnsureSpatialOrder(h, sort, s)) return st;
+    if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/false, s)) return st;
     LaunchPoseStream(h->surfels, acc->pitch, h->surfels_size, sort ? p.order.view.perm : nullptr, p.order.stream,
                      p.order.capacity, p.order.boxes, s);
     ++h->launches;

@@ -1,4 +1,4 @@
-// spatial_order.cu -- the surfels' spatial (Morton) order and the pose step's surfel stream in that order.
+// spatial_order.cu -- the surfels' spatial (Morton) order and the pose and geometry steps' surfel streams in that order.
 //
 // The pose kernel evaluates (keyframe, 256-surfel chunk) sub-items.  In the caller's order (creation order: raster order inside the
 // keyframe that created them) a chunk is a band across a whole source image, partly inside and partly outside any other keyframe's
@@ -17,15 +17,6 @@ namespace bba {
 namespace {
 
 constexpr int kMortonBits = 10;   // per axis: 30-bit keys
-
-// Order-preserving map of a float onto an unsigned int (for atomicMin / atomicMax), and back.
-__device__ __forceinline__ unsigned int OrderedBits(float f) {
-  const unsigned int u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float FromOrderedBits(unsigned int u) {
-  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
 
 // Spreads the low 10 bits of v to every third bit.
 __device__ __forceinline__ uint32_t Spread3(uint32_t v) {
@@ -144,7 +135,30 @@ __global__ void __launch_bounds__(kSpatialChunk) PoseStreamKernel(const float* _
   }
 }
 
+// One thread per local index of the launch: gather surfel perm[s] into geometry-stream column s (GeometryArgs).  Without desc_rows
+// the rows radius^2, d1, d2 are left alone: only the position / descriptor kernel with descriptors reads them.
+__global__ void __launch_bounds__(256) GeometryStreamKernel(const __grid_constant__ GeometryArgs a, bool desc_rows) {
+  const uint32_t li = a.begin + blockIdx.x * blockDim.x + threadIdx.x;
+  if (li >= a.end) return;
+  const uint32_t s = SurfelShardToGlobal(li, a.shard_rank, a.shard_world);
+  if (s >= a.n) return;
+  const size_t P = a.pitch, F = a.stream_pitch, i = a.perm ? __ldg(a.perm + s) : s;
+  constexpr int kRows[kGeoStreamRows - 1] = {kRowX, kRowY, kRowZ, kRowNormal, kRowRadiusSq, kRowD1, kRowD2};
+#pragma unroll
+  for (int r = 0; r < 4; ++r) a.stream[r * F + s] = a.surfels[kRows[r] * P + i];
+  if (desc_rows) {
+#pragma unroll
+    for (int r = 4; r < kGeoStreamRows - 1; ++r) a.stream[r * F + s] = a.surfels[kRows[r] * P + i];
+  }
+  a.stream[(kGeoStreamRows - 1) * F + s] = __uint_as_float(a.active[i]);
+}
+
 }  // namespace
+
+void LaunchGeometryStream(const GeometryArgs& a, bool desc_rows, cudaStream_t stream) {
+  if (a.end <= a.begin) return;
+  GeometryStreamKernel<<<(a.end - a.begin + 255) / 256, 256, 0, stream>>>(a, desc_rows);
+}
 
 size_t SpatialOrderTempBytes(uint32_t capacity) {
   size_t bytes = 0;

@@ -73,8 +73,9 @@ def config_by_name(name: str) -> SceneConfig:
     if name == "small":
         return SceneConfig(320, 240, 6, 30_000, cell=2, seed=8, name="small")
     if name == "many":
-        # many small keyframes: 37 = 4 full 8-keyframe work groups of the pose kernel + 5, and 16 + 16 + 5 for the PCG,
-        # intrinsics and geometry kernels' 16-keyframe groups, at a size the CPU oracle evaluates in well under a second
+        # many small keyframes: 37 = 4 full 8-keyframe work groups of the pose kernel + 5, 16 + 16 + 5 for the PCG and
+        # intrinsics kernels' 16-keyframe groups and 32 + 5 for the geometry kernels' 32-keyframe groups, at a size the CPU
+        # oracle evaluates in well under a second
         return SceneConfig(160, 120, 37, 24_000, cell=2, seed=11, name="many")
     raise KeyError(name)
 
