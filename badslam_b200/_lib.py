@@ -161,6 +161,9 @@ SYMBOLS = {
                                                     C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_track_frame_pairwise": (C.c_int, [_P, C.POINTER(OdometryOptions), C.c_int, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
                                            _F7, _F7, _F7, C.POINTER(OdometryResult), _P]),
+    "bba_track_frame_pairwise_to_frame": (C.c_int, [_P, C.POINTER(OdometryOptions), _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
+                                                    _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _F7, _F7, _F7,
+                                                    C.POINTER(OdometryResult), _P]),
     "bba_odometry_get_level": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_odometry_debug_coeffs": (C.c_int, [_P, C.c_int, C.c_int, _F7, _F7, _P, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_float),
                                             _P, _P, _P]),

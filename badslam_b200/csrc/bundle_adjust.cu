@@ -159,7 +159,7 @@ bba_status OptimizeIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cuda
     bba::SolveLDLT<4>(H, b, x);
     for (int i = 0; i < 4; ++i) h->color_K[i] -= static_cast<float>(x[i]);
   }
-  return BBA_OK;
+  return Publish(h, s, opt_depth);   // cameras, a and (depth) the cfactor together
 }
 
 // ---- in-loop surfel lifecycle ---------------------------------------------------------------------------------------------
@@ -259,7 +259,7 @@ bba_status CreateSurfelsForKeyframe(bba_handle h, int k, bool filter, cudaStream
   if (created == 0) return BBA_OK;
   if (h->surfels_size + static_cast<uint64_t>(created) > SurfelCapacity(h)) {
     // the reference logs "Maximum surfel count exceeded" and creates nothing (kernel_create_surfels.cc:163-166)
-    h->error = "maximum surfel count exceeded: no surfels created for this keyframe";
+    SetError(h, "maximum surfel count exceeded: no surfels created for this keyframe");
     return BBA_OK;
   }
   bba::LaunchCreateSurfels(a, h->life.d_scan_out, s);
@@ -615,7 +615,7 @@ bba_status PcgApplyDelta(bba_handle h, const PcgLayout& L, int gauge, cudaStream
   }
   if (L.opt_color_intr)   // :623-638
     for (int c = 0; c < 4; ++c) h->color_K[c] = static_cast<float>(h->color_K[c] + h_ci[c]);
-  return BBA_OK;
+  return Publish(h, s, L.opt_depth_intr);   // poses, cameras, a and (depth) the cfactor together
 }
 
 // DirectBA::BundleAdjustmentPCG (direct_ba_pcg.cc:43-819) without the surfel lifecycle branches.
@@ -783,8 +783,13 @@ bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth, int optimiz
   return OptimizeIntrinsics(h, optimize_depth != 0, optimize_color != 0, static_cast<cudaStream_t>(stream));
 }
 
-bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_result* res, void* stream) {
-  if (!h || !o || !res) return BBA_ERR_INVALID_ARGUMENT;
+}  // extern "C"
+
+namespace bba {
+namespace {
+
+// bba_bundle_adjust
+bba_status BundleAdjust(bba_handle h, const bba_ba_options* o, bba_ba_result* res, void* stream) {
   std::memset(res, 0, sizeof(*res));
   if (bba_status st = CheckSurfels(h)) return st;
   // (do_surfel_updates with more than one rank: creation / merging / compaction run REPLICATED -- they are deterministic and
@@ -926,6 +931,7 @@ bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_resul
     } else {
       BBA_CUDA(h, cudaStreamSynchronize(s));
     }
+    if (bba_status st = Publish(h, s, false)) return st;   // every pose of this step at once
     BBA_CUDA(h, cudaEventRecord(h->ev[3], s));
     // --- intrinsics optimisation (:584-624)
     if (opt_depth_intr || opt_color_intr) {
@@ -954,10 +960,25 @@ bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_resul
       if (el > o->time_limit_seconds) break;
     }
     DetermineCovisibleActiveKeyframes(h);   // :711-717
+    if (bba_status st = Publish(h, s, false)) return st;
   }
   BBA_TRACE("iterations done");
   return EndBundleAdjust(h, o, launches_before, res, s);
 }
+
+}  // namespace
+}  // namespace bba
+
+extern "C" bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* o, bba_ba_result* res, void* stream) {
+  if (!h || !o || !res) return BBA_ERR_INVALID_ARGUMENT;
+  const bba_status st = bba::BundleAdjust(h, o, res, static_cast<cudaStream_t>(stream));
+  // whatever the call changed of the published state, also on an early return (poses and cameras are published where they
+  // change; this covers the activations and the keyframe state of a failed call)
+  bba::Publish(h, static_cast<cudaStream_t>(stream), false);
+  return st;
+}
+
+extern "C" {
 
 bba_status bba_perform_end_tasks(bba_handle h, int do_surfel_updates, uint32_t* deleted, uint32_t* surfels_size, void* stream) {
   if (!h) return BBA_ERR_INVALID_ARGUMENT;

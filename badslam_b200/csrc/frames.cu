@@ -1,5 +1,6 @@
 // frames.cu -- the frame side of libbadba_b200 (host side): image-pair odometry (buffers, pyramids, the persistent tracking
-// kernel's launch and its entry points) and keyframe preprocessing (bba_preprocess_frame, bba_preprocess_raw_frame).
+// kernel's launch and its entry points) and keyframe preprocessing (bba_preprocess_frame, bba_preprocess_raw_frame).  These are
+// the front-end calls of include/badba.h: they read the published view of the handle (FrontEndCall), never its live state.
 #include <cmath>
 #include <cstring>
 
@@ -68,13 +69,13 @@ bba_status EnsureOdometry(bba_handle h, int num_scales) {
 
 // The camera model of one pyramid level: PinholeCamera4f::Scaled (libvis camera.h:1696-1705, 1086-1097: all four parameters
 // times the factor, width = factor * width + 0.5) through the builders of surfel_projection.h:42-124.
-bba::odom::LevelCamera MakeLevelCamera(bba_handle h, int scale, int level_w, int level_h) {
+bba::odom::LevelCamera MakeLevelCamera(bba_handle h, const CameraView& v, int scale, int level_w, int level_h) {
   bba::odom::LevelCamera c;
   const float scaling_factor = static_cast<float>(std::pow(2, scale));
   const float df = static_cast<float>(1.f / scaling_factor);   // depth_camera.Scaled(1.f / scaling_factor)
   const float cf = static_cast<float>((h->cfg.depth_width == h->cfg.color_width) ? (1.f / scaling_factor) : (2.f / scaling_factor));
-  const float dK[4] = {h->depth_K[0] * df, h->depth_K[1] * df, h->depth_K[2] * df, h->depth_K[3] * df};
-  const float cK[4] = {h->color_K[0] * cf, h->color_K[1] * cf, h->color_K[2] * cf, h->color_K[3] * cf};
+  const float dK[4] = {v.depth_K[0] * df, v.depth_K[1] * df, v.depth_K[2] * df, v.depth_K[3] * df};
+  const float cK[4] = {v.color_K[0] * cf, v.color_K[1] * cf, v.color_K[2] * cf, v.color_K[3] * cf};
   c.w = level_w; c.h = level_h;
   c.fx = dK[0]; c.fy = dK[1]; c.cx = dK[2]; c.cy = dK[3];
   c.fx_inv = 1.0f / dK[0];
@@ -91,19 +92,21 @@ bba::odom::LevelCamera MakeLevelCamera(bba_handle h, int scale, int level_w, int
   return c;
 }
 
-// Fills the pyramids of both frames for the given options (stages 1-3 of odometry.cuh) and the level descriptors in h->odo.level.
-bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, const Keyframe& base, const uint16_t* trk_depth, size_t trk_depth_pitch,
-                                 const uint16_t* trk_normals, size_t trk_normals_pitch, cudaStream_t s) {
+// Fills the pyramids of both frames for the given options (stages 1-3 of odometry.cuh) and the level descriptors in h->odo.level,
+// with the cameras and the cfactor of the call's snapshot.  The tracked frame's luma is in h->fe.frame.
+bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, const FrontEndCall& view, const KeyframeView& base,
+                                 const uint16_t* trk_depth, size_t trk_depth_pitch, const uint16_t* trk_normals, size_t trk_normals_pitch,
+                                 cudaStream_t s) {
   namespace od = bba::odom;
   auto& st = h->odo;
   const int S = o.num_scales;
   od::BrightnessArgs br{};
-  br.luma_tex[0] = base.tex; br.luma_tex[1] = h->staging.scratch.tex;
+  br.luma_tex[0] = base.tex; br.luma_tex[1] = h->fe.frame.tex;
   for (int f = 0; f < 2; ++f) { br.out[f] = st.gradmag[f].get(); br.out_pitch[f] = static_cast<uint32_t>(st.gradmag[f].pitch()); }
   br.w = h->cfg.color_width; br.h = h->cfg.color_height;
   br.use_gradmag = o.use_gradmag;
   od::LaunchBrightness(br, s);
-  ++h->launches;
+  ++h->front_end_launches;
 
   // level images as seen by the kernels: level 0 normals are the keyframe's / the frame's own buffers
   od::Image img[2][od::kMaxScales];
@@ -112,7 +115,7 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
   img[0][0].normals = const_cast<uint16_t*>(base.normals); img[0][0].normals_pitch = static_cast<uint32_t>(base.normals_pitch);
   img[1][0].normals = const_cast<uint16_t*>(trk_normals);  img[1][0].normals_pitch = static_cast<uint32_t>(trk_normals_pitch);
 
-  const bba::CameraParams cam = MakeCamera(h);
+  const bba::CameraParams cam = MakeCamera(h, view.cams, view.cfactor);
   od::Level0Args l0{};
   l0.raw_depth[0] = base.depth; l0.raw_depth_pitch[0] = static_cast<uint32_t>(base.depth_pitch);
   l0.raw_depth[1] = trk_depth;  l0.raw_depth_pitch[1] = static_cast<uint32_t>(trk_depth_pitch);
@@ -129,7 +132,7 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
   l0.a = cam.a; l0.raw_to_float = cam.raw_to_float; l0.cfactor = cam.cfactor; l0.cf_w = cam.cf_w; l0.cell = cam.cell;
   l0.downsample_color = h->cfg.depth_width == h->cfg.color_width;
   od::LaunchLevel0(l0, s);
-  ++h->launches;
+  ++h->front_end_launches;
 
   for (int l = 1; l < S; ++l) {
     // pairwise_frame_tracking.cc:325-347: the tracked image from level 2 on (level 1 too when level 0 is in use), the base always
@@ -143,10 +146,10 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
     d.w = st.w[l]; d.h = st.h[l];
     d.in_w = st.w[l - 1]; d.in_h = st.h[l - 1];
     od::LaunchDownsample(d, s);
-    ++h->launches;
+    ++h->front_end_launches;
   }
   for (int l = 0; l < S; ++l) {
-    st.level[l].cam = MakeLevelCamera(h, l, st.w[l], st.h[l]);
+    st.level[l].cam = MakeLevelCamera(h, view.cams, l, st.w[l], st.h[l]);
     st.level[l].base = img[0][l];
     st.level[l].tracked = img[1][l];
   }
@@ -156,8 +159,8 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
   return BBA_OK;
 }
 
-bba_status LaunchOdometryKernel(bba_handle h, int num_scales, int first_scale, int max_iterations, int use_gradmag, int test_different,
-                                int debug_scale, const float init1[7], const float init2[7], cudaStream_t s) {
+bba_status LaunchOdometryKernel(bba_handle h, const CameraView& cams, int num_scales, int first_scale, int max_iterations, int use_gradmag,
+                                int test_different, int debug_scale, const float init1[7], const float init2[7], cudaStream_t s) {
   namespace od = bba::odom;
   auto& st = h->odo;
   od::TrackArgs a{};
@@ -165,8 +168,8 @@ bba_status LaunchOdometryKernel(bba_handle h, int num_scales, int first_scale, i
   a.num_scales = num_scales;
   a.first_scale = first_scale;
   a.max_iterations = max_iterations;
-  a.use_depth = h->cfg.use_depth_residuals;
-  a.use_desc = h->cfg.use_descriptor_residuals;
+  a.use_depth = cams.use_depth;
+  a.use_desc = cams.use_desc;
   a.use_gradmag = use_gradmag;
   a.test_different_initial_estimates = test_different;
   a.debug_scale = debug_scale;
@@ -180,7 +183,7 @@ bba_status LaunchOdometryKernel(bba_handle h, int num_scales, int first_scale, i
   BBA_CUDA(h, cudaMemsetAsync(st.d_barrier, 0, sizeof(unsigned int) * 2, s));
   BBA_CUDA(h, cudaMemsetAsync(st.d_result, 0, sizeof(od::TrackResult), s));
   od::LaunchTrack(a, h->sm_count, s);
-  ++h->launches;
+  ++h->front_end_launches;
   BBA_CUDA(h, cudaGetLastError());
   BBA_CUDA(h, cudaMemcpyAsync(st.h_result, st.d_result, sizeof(od::TrackResult), cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));
@@ -219,9 +222,12 @@ bba_status PreprocessFrame(bba_handle h, const char* fn, const bba_preprocess_op
   if (!(o->bilateral_filter_sigma_xy > 0.f) || !(o->bilateral_filter_sigma_inv_depth > 0.f) || !(o->max_depth > 0.f))
     return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": sigma_xy, sigma_inv_depth and max_depth must be positive");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::lock_guard<std::mutex> call(h->fe.call);
   BBA_CUDA(h, h->pre.d_min_max.Reserve(2));
   BBA_CUDA(h, h->pre.h_min_max.Reserve(2));
-  const bba::CameraParams cam = MakeCamera(h);
+  FrontEndCall view(h);
+  if (bba_status st = view.Snapshot(s, -1, fn)) return st;
+  const bba::CameraParams cam = MakeCamera(h, view.cams, view.cfactor);
   bba::pre::FrameArgs f{};
   f.w = cam.w; f.h = cam.h;
   f.fx_inv = cam.fx_inv; f.fy_inv = cam.fy_inv; f.cx_inv = cam.cx_inv; f.cy_inv = cam.cy_inv;
@@ -248,11 +254,12 @@ bba_status PreprocessFrame(bba_handle h, const char* fn, const bba_preprocess_op
     f.depth_level = raw_stage->depth_level;
     f.raw_w = raw_stage->raw_w; f.raw_h = raw_stage->raw_h;
     f.color_level = raw_stage->color_level;
-    h->launches += bba::LaunchPreprocessRawFrame(f, s);
+    h->front_end_launches += bba::LaunchPreprocessRawFrame(f, s);
   } else {
-    h->launches += bba::LaunchPreprocessFrame(f, s);
+    h->front_end_launches += bba::LaunchPreprocessFrame(f, s);
   }
   BBA_CUDA(h, cudaGetLastError());
+  if (bba_status st = view.ReleaseSlot()) return st;
   if (min_depth || max_depth) {   // ComputeMinMaxDepthCUDA returns host values and synchronises (cuda_depth_processing.cu:452-463)
     BBA_CUDA(h, cudaMemcpyAsync(h->pre.h_min_max, h->pre.d_min_max, 2 * sizeof(float), cudaMemcpyDeviceToHost, s));
     BBA_CUDA(h, cudaStreamSynchronize(s));
@@ -262,38 +269,58 @@ bba_status PreprocessFrame(bba_handle h, const char* fn, const bba_preprocess_op
   return BBA_OK;
 }
 
-}  // namespace
+// The base frame of bba_track_frame_pairwise_to_frame.
+struct BaseBuffers {
+  const uint16_t* depth;
+  size_t depth_pitch;
+  const uint16_t* normals;
+  size_t normals_pitch;
+  const uint8_t* rgba;
+  size_t rgba_pitch;
+};
 
-}  // namespace bba
-
-using namespace bba;
-
-extern "C" {
-
-bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* o, int base_keyframe_id,
-                                    const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals, size_t normals_pitch,
-                                    const uint8_t* device_color_rgba, size_t color_pitch, const float init1[7], const float init2[7],
-                                    float out[7], bba_odometry_result* result, void* stream) {
-  if (!h || !o || !device_depth || !device_normals || !device_color_rgba || !init1 || !out) return h ? Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: null argument") : BBA_ERR_INVALID_ARGUMENT;
-  if (base_keyframe_id < 0 || base_keyframe_id >= static_cast<int>(h->keyframes.size()))
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: no such keyframe");
+// bba_track_frame_pairwise (base = keyframe base_keyframe_id) and bba_track_frame_pairwise_to_frame (base = *base_buffers).
+bba_status TrackFramePairwise(bba_handle h, const char* fn, const bba_odometry_options* o, int base_keyframe_id, const BaseBuffers* base_buffers,
+                              const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals, size_t normals_pitch,
+                              const uint8_t* device_color_rgba, size_t color_pitch, const float init1[7], const float init2[7],
+                              float out[7], bba_odometry_result* result, void* stream) {
+  const std::string name(fn);
+  if (!h || !o || !device_depth || !device_normals || !device_color_rgba || !init1 || !out) return h ? Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null argument") : BBA_ERR_INVALID_ARGUMENT;
+  if (base_keyframe_id < 0 && !base_buffers) return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": no such keyframe");
   if (o->num_scales < 1 || o->num_scales > bba::odom::kMaxScales || (!o->use_pyramid_level_0 && o->num_scales < 2))
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: num_scales must be 1..8 (>= 2 without pyramid level 0)");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": num_scales must be 1..8 (>= 2 without pyramid level 0)");
   if (!FramePitchesOk(h, depth_pitch, normals_pitch, color_pitch) || ((depth_pitch | normals_pitch) & 1u))
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: bad frame buffer pitch");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": bad frame buffer pitch");
+  if (base_buffers) {
+    const BaseBuffers& b = *base_buffers;
+    if (!b.depth || !b.normals || !b.rgba) return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null argument");
+    if (!FramePitchesOk(h, b.depth_pitch, b.normals_pitch, b.rgba_pitch) || ((b.depth_pitch | b.normals_pitch) & 1u))
+      return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": bad base buffer pitch");
+  }
   // pairwise_frame_tracking.cc:300-306 (LOG(FATAL) in the reference)
   if (!o->use_pyramid_level_0 && h->cfg.depth_width != h->cfg.color_width && h->cfg.depth_width != 2 * h->cfg.color_width)
     return Fail(h, BBA_ERR_UNSUPPORTED, "The chosen depth / color pyramid level combination is not supported here.");
   if (o->test_different_initial_estimates && !init2)
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: test_different_initial_estimates needs the second estimate");
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": test_different_initial_estimates needs the second estimate");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const uint64_t launches_before = h->launches;
+  std::lock_guard<std::mutex> call(h->fe.call);
+  const uint64_t launches_before = h->front_end_launches;
+  FrontEndCall view(h);
+  if (bba_status st = view.Snapshot(s, base_buffers ? -1 : base_keyframe_id, fn)) return st;
   if (bba_status st = EnsureOdometry(h, o->num_scales)) return st;
-  if (bba_status st = MakeLumaTexture(h, device_color_rgba, color_pitch, &h->staging.scratch, s)) return st;
-  const Keyframe& base = h->keyframes[base_keyframe_id];
-  if (bba_status st = BuildOdometryPyramids(h, *o, base, device_depth, depth_pitch, device_normals, normals_pitch, s)) return st;
+  if (bba_status st = MakeLumaTexture(h, device_color_rgba, color_pitch, &h->fe.frame, s, /*front_end=*/true)) return st;
+  KeyframeView base = view.base;
+  if (base_buffers) {   // the luma the keyframe would get from bba_add_keyframe, in the front end's base texture
+    const BaseBuffers& b = *base_buffers;
+    if (bba_status st = MakeLumaTexture(h, b.rgba, b.rgba_pitch, &h->fe.base, s, /*front_end=*/true)) return st;
+    base.depth = b.depth; base.depth_pitch = b.depth_pitch;
+    base.normals = b.normals; base.normals_pitch = b.normals_pitch;
+    base.tex = h->fe.base.tex;
+  }
+  if (bba_status st = BuildOdometryPyramids(h, *o, view, base, device_depth, depth_pitch, device_normals, normals_pitch, s)) return st;
+  if (bba_status st = view.ReleaseSlot()) return st;   // (level 0 was the last reader of the cfactor)
   const int max_it = o->max_iterations_per_scale > 0 ? o->max_iterations_per_scale : 30;
-  if (bba_status st = LaunchOdometryKernel(h, o->num_scales, o->use_pyramid_level_0 ? 0 : 1, max_it, o->use_gradmag ? 1 : 0,
+  if (bba_status st = LaunchOdometryKernel(h, view.cams, o->num_scales, o->use_pyramid_level_0 ? 0 : 1, max_it, o->use_gradmag ? 1 : 0,
                                            o->test_different_initial_estimates ? 1 : 0, -1, init1, init2 ? init2 : init1, s))
     return st;
   const bba::odom::TrackResult& r = *h->odo.h_result;
@@ -306,14 +333,43 @@ bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* o,
     result->residual_count = r.residual_count;
     result->residual_sum = r.residual_sum;
     result->passes = r.passes;
-    result->kernel_launches = static_cast<uint32_t>(h->launches - launches_before);
+    result->kernel_launches = static_cast<uint32_t>(h->front_end_launches - launches_before);
   }
   return BBA_OK;
+}
+
+}  // namespace
+}  // namespace bba
+
+using namespace bba;
+
+extern "C" {
+
+bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* o, int base_keyframe_id,
+                                    const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals, size_t normals_pitch,
+                                    const uint8_t* device_color_rgba, size_t color_pitch, const float init1[7], const float init2[7],
+                                    float out[7], bba_odometry_result* result, void* stream) {
+  return TrackFramePairwise(h, "bba_track_frame_pairwise", o, base_keyframe_id, nullptr, device_depth, depth_pitch, device_normals,
+                            normals_pitch, device_color_rgba, color_pitch, init1, init2, out, result, stream);
+}
+
+bba_status bba_track_frame_pairwise_to_frame(bba_handle h, const bba_odometry_options* o,
+                                             const uint16_t* base_depth, size_t base_depth_pitch,
+                                             const uint16_t* base_normals, size_t base_normals_pitch,
+                                             const uint8_t* base_color_rgba, size_t base_color_pitch,
+                                             const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals,
+                                             size_t normals_pitch, const uint8_t* device_color_rgba, size_t color_pitch,
+                                             const float init1[7], const float init2[7], float out[7], bba_odometry_result* result,
+                                             void* stream) {
+  const BaseBuffers base{base_depth, base_depth_pitch, base_normals, base_normals_pitch, base_color_rgba, base_color_pitch};
+  return TrackFramePairwise(h, "bba_track_frame_pairwise_to_frame", o, -1, &base, device_depth, depth_pitch, device_normals,
+                            normals_pitch, device_color_rgba, color_pitch, init1, init2, out, result, stream);
 }
 
 bba_status bba_odometry_get_level(bba_handle h, int which, int scale, float* host_depth, uint16_t* host_normals, uint8_t* host_color,
                                   int* width, int* height, void* stream) {
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> call(h->fe.call);
   auto& st = h->odo;
   if (which < 0 || which > 1 || scale < 0 || scale >= st.last_num_scales || (which == 1 && scale < st.last_first_scale))
     return Fail(h, BBA_ERR_STATE, "bba_odometry_get_level: this level was not built by the last bba_track_frame_pairwise call");
@@ -332,11 +388,16 @@ bba_status bba_odometry_get_level(bba_handle h, int which, int scale, float* hos
 bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, const float pose_a[7], const float pose_b[7], float H[21],
                                      float b[6], uint32_t* residual_count, float* residual_sum, uint32_t counts[2], float costs[2], void* stream) {
   if (!h || !pose_a) return BBA_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> call(h->fe.call);
   auto& st = h->odo;
   if (scale < st.last_first_scale || scale >= st.last_num_scales)
     return Fail(h, BBA_ERR_STATE, "bba_odometry_debug_coeffs: this level was not built by the last bba_track_frame_pairwise call");
-  if (bba_status s2 = LaunchOdometryKernel(h, st.last_num_scales, st.last_first_scale, 1, use_gradmag ? 1 : 0, 0, scale, pose_a,
-                                           pose_b ? pose_b : pose_a, static_cast<cudaStream_t>(stream)))
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  FrontEndCall view(h);   // (the residual types; the pyramids hold the cameras of the tracking call)
+  if (bba_status s2 = view.Snapshot(s, -1, "bba_odometry_debug_coeffs")) return s2;
+  if (bba_status s2 = view.ReleaseSlot(/*record=*/false)) return s2;   // (the cfactor is not read)
+  if (bba_status s2 = LaunchOdometryKernel(h, view.cams, st.last_num_scales, st.last_first_scale, 1, use_gradmag ? 1 : 0, 0, scale, pose_a,
+                                           pose_b ? pose_b : pose_a, s))
     return s2;
   const double* d = st.h_result->debug;
   if (H) for (int i = 0; i < 21; ++i) H[i] = static_cast<float>(d[i]);

@@ -9,9 +9,14 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
+#include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
+#include <map>
+#include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../../include/badba.h"
@@ -123,6 +128,32 @@ struct Keyframe {
   std::vector<int> covis;
 };
 
+// ---- the front end's view (badba.h "Conventions"; DESIGN.md "Front end beside a running BA") -----------------------------------
+// What front-end calls read of a keyframe: copied from its Keyframe record whenever the BA side publishes.
+struct KeyframeView {
+  const uint16_t* depth = nullptr;
+  const uint16_t* normals = nullptr;
+  size_t depth_pitch = 0, normals_pitch = 0;
+  cudaTextureObject_t tex = 0;
+  Pose pose;
+  float min_depth = 0.f, max_depth = 0.f;
+  int activation = BBA_KF_ACTIVE;
+};
+
+// The cameras, the depth deformation parameter a and the residual types as the BA side published them last.
+struct CameraView {
+  float depth_K[4] = {}, color_K[4] = {};
+  float depth_a = 0.f;
+  int use_depth = 1, use_desc = 1;
+};
+
+// A u8 plane that luma extraction writes before the copy into a CUDA array, and the event after which the next user may
+// overwrite it.
+struct LumaStaging {
+  PitchedBuffer plane;
+  Event free;
+};
+
 }  // namespace bba
 
 struct bba_context {
@@ -131,7 +162,9 @@ struct bba_context {
   float depth_a = 0.f;
   int cf_w = 0, cf_h = 0;
   int sm_count = 132;
-  std::string error;
+  // bba_last_error: the message of the last failed call per calling thread
+  std::mutex error_mu;
+  std::map<std::thread::id, std::string> errors;
 
   float* surfels = nullptr;
   size_t surfel_pitch_bytes = 0;
@@ -150,8 +183,7 @@ struct bba_context {
     bba::PinnedBuffer<bba::KfDevice> h_kfs;
     bba::Event event;      // recorded after the last upload from the pinned staging buffers
     bool pending = false;
-    bba::PitchedBuffer luma;    // u8 plane staging for the luma arrays
-    bba::Event luma_free;       // recorded after the staging plane was consumed; the next user (any stream) waits on it
+    bba::LumaStaging luma;      // u8 plane staging for the luma arrays of the BA side; the next user (any stream) waits on .free
     bba::PitchedBuffer color;   // uchar4 staging image for bba_update_keyframe_host
     bba::Texture scratch;       // luma array + texture of a frame that is not a keyframe (frame pose, odometry)
   } staging;
@@ -281,7 +313,31 @@ struct bba_context {
     bba::PinnedBuffer<float> h_min_max;
   } pre;
 
-  uint64_t launches = 0;
+  // The state front-end calls read (Publish writes it; FrontEndCall takes a snapshot), and the buffers only they use.  Front-end
+  // calls never touch the live state above, which the BA side changes while it runs.
+  struct FrontEnd {
+    std::mutex mu;                       // guards the published fields below; never held across a launch or a synchronise
+    std::condition_variable slot_free;   // a cfactor slot lost its last reader
+    bba::CameraView cams;
+    std::vector<bba::KeyframeView> kfs;
+    // Two device copies of the cfactor.  Publish copies d_cfactor into the slot that is not current, on the BA side's stream,
+    // after that slot's readers are done, records `published` and makes the slot current; a front-end call claims the
+    // current slot, makes its stream wait on `published` and records `readers_done` after its last read.
+    bba::DeviceBuffer<float> cfactor[2];
+    bba::Event published[2];
+    bba::Event readers_done[2];
+    int current = 0;
+    int readers[2] = {0, 0};   // claims between FrontEndCall::Snapshot and ReleaseSlot
+    std::mutex call;           // serialises the front-end calls that use the buffers below and odo / pre
+    bba::LumaStaging luma;
+    bba::Texture frame;        // luma of the tracked frame
+    bba::Texture base;         // luma of a base frame given as buffers (bba_track_frame_pairwise_to_frame)
+  } fe;
+
+  // kernels launched by BA-side calls and by front-end calls (bba_kernel_launch_count: the sum); two counters so that the
+  // launches a BA call reports are its own while the front end runs beside it
+  std::atomic<uint64_t> launches{0};
+  std::atomic<uint64_t> front_end_launches{0};
   int ba_iteration_count = 0;
   // predicted cost of one pose step per keyframe (Gauss-Newton iterations x per-evaluation cost of the last step it took
   // part in); 0 = unknown.  Identical on every rank; drives the keyframe -> rank assignment of the pose step.
@@ -297,6 +353,8 @@ struct bba_context {
 namespace bba {
 
 bba_status Fail(bba_handle h, bba_status s, const std::string& msg);
+// Sets the calling thread's bba_last_error message.
+void SetError(bba_handle h, const std::string& msg);
 
 #define BBA_CUDA(h, expr)                                                                                  \
   do {                                                                                                      \
@@ -319,7 +377,35 @@ bba_status Fail(bba_handle h, bba_status s, const std::string& msg);
 // badba.cu
 Pose PoseFromArray(const float p[7]);
 void PoseToArray(const Pose& r, float p[7]);
+// The camera of the BA side's live state, or of a published view with the cfactor slot it claimed.
 CameraParams MakeCamera(bba_handle h);
+CameraParams MakeCamera(bba_handle h, const CameraView& v, const float* cfactor);
+// Publishes the cameras, residual types and keyframe records for the front end and, with `cfactor`, a copy of d_cfactor
+// enqueued on s (BA side only; after every change of that state).
+bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor);
+
+// The snapshot a front-end call reads instead of the live state.  Snapshot copies the published cameras (and the record of
+// keyframe `kf_id` when >= 0) under fe.mu and claims the current cfactor slot: s waits for its publication.  ReleaseSlot
+// drops the claim after the call's last read of the slot: with `record`, s first waits for the slot's previous readers and
+// then records "readers done" (without, the caller has synchronised s).  The destructor releases a claim still held.
+class FrontEndCall {
+ public:
+  explicit FrontEndCall(bba_handle h) : h_(h) {}
+  ~FrontEndCall() { ReleaseSlot(); }
+  FrontEndCall(const FrontEndCall&) = delete;
+  FrontEndCall& operator=(const FrontEndCall&) = delete;
+  bba_status Snapshot(cudaStream_t s, int kf_id, const char* fn);
+  bba_status ReleaseSlot(bool record = true);
+  CameraView cams;
+  KeyframeView base;
+  const float* cfactor = nullptr;
+
+ private:
+  bba_handle h_;
+  cudaStream_t s_ = nullptr;
+  int slot_ = -1;
+};
+
 bba_status WaitStaging(bba_handle h);
 bba_status MarkStaging(bba_handle h, cudaStream_t s);
 void FillKfDevice(const Keyframe& kf, const Pose& global_T_frame, KfDevice* d);
@@ -337,7 +423,9 @@ template <class Args> void SetSurfelFields(bba_handle h, Args* a) {
   a->pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
   a->n = h->surfels_size;
 }
-bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t color_pitch, Texture* luma, cudaStream_t s);
+// front_end: through the front end's staging plane, counted as a front-end launch.
+bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t color_pitch, Texture* luma, cudaStream_t s,
+                           bool front_end = false);
 
 // pose_step.cu
 // The surfel count from which a launch over n keyframes puts the surfels into spatial order: sorting costs ~0.1 ms of launches

@@ -527,6 +527,30 @@ class DirectBA:
             out.ctypes.data_as(F), C.byref(res), self._stream_ptr(stream)))
         return out, res
 
+    def TrackFramePairwiseToFrame(self, stream, base_depth_buffer: torch.Tensor, base_normals_buffer: torch.Tensor,
+                                  base_color_buffer: torch.Tensor, depth_buffer: torch.Tensor, normals_buffer: torch.Tensor,
+                                  color_buffer: torch.Tensor, base_T_frame_initial_estimate_1, base_T_frame_initial_estimate_2=None,
+                                  num_scales: int = 5, use_pyramid_level_0: bool = True, use_gradmag: bool = False,
+                                  test_different_initial_estimates: bool = True, max_iterations_per_scale: int = 30):
+        """TrackFramePairwise against a base frame that is not a keyframe (yet), given by the buffers AddKeyframe would take
+        (depth / normals [h, w] u16, colour [ch, cw, 4] u8): what the odometry thread does with the keyframe the BA thread has not
+        added yet.  Same result as TrackFramePairwise against those buffers as a keyframe.  Returns (base_T_frame_estimate,
+        OdometryResult)."""
+        p1 = np.ascontiguousarray(base_T_frame_initial_estimate_1, np.float32)
+        p2 = p1 if base_T_frame_initial_estimate_2 is None else np.ascontiguousarray(base_T_frame_initial_estimate_2, np.float32)
+        out = np.zeros(7, np.float32)
+        o = _lib.OdometryOptions(int(num_scales), int(use_pyramid_level_0), int(use_gradmag), int(test_different_initial_estimates),
+                                 int(max_iterations_per_scale))
+        res = _lib.OdometryResult()
+        F = C.POINTER(C.c_float)
+        self._check(self._lib.bba_track_frame_pairwise_to_frame(
+            self._h, C.byref(o), base_depth_buffer.data_ptr(), base_depth_buffer.stride(0) * 2, base_normals_buffer.data_ptr(),
+            base_normals_buffer.stride(0) * 2, base_color_buffer.data_ptr(), base_color_buffer.stride(0),
+            depth_buffer.data_ptr(), depth_buffer.stride(0) * 2, normals_buffer.data_ptr(), normals_buffer.stride(0) * 2,
+            color_buffer.data_ptr(), color_buffer.stride(0), p1.ctypes.data_as(F), p2.ctypes.data_as(F), out.ctypes.data_as(F),
+            C.byref(res), self._stream_ptr(stream)))
+        return out, res
+
     def OdometryLevel(self, which: int, scale: int, stream=None):
         """Parity hook: (depth f32, normals u16, colour u8) of one pyramid level of the last TrackFramePairwise call
         (which: 0 = base keyframe, 1 = tracked frame)."""

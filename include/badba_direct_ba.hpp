@@ -158,6 +158,32 @@ class DirectBA {
     std::memcpy(out_base_T_frame_estimate->data(), out, sizeof(out));
   }
 
+  // The same against a base frame that is not a keyframe yet, given by the buffers AddKeyframe takes: the keyframe that still
+  // waits in the BA thread's queue while the odometry thread tracks against it (parallel BA, INTEGRATION.md section 2).
+  void TrackFramePairwise(cudaStream_t stream, DeviceImage<uint16_t> base_depth_buffer, DeviceImage<uint16_t> base_normals_buffer,
+                          DeviceImage<uint8_t> base_color_buffer_rgba, bool use_pyramid_level_0, bool use_gradmag,
+                          DeviceImage<uint16_t> tracked_depth_buffer, DeviceImage<uint16_t> tracked_normals_buffer,
+                          DeviceImage<uint8_t> tracked_color_buffer_rgba, bool test_different_initial_estimates,
+                          const SE3f& base_T_frame_initial_estimate_1, const SE3f& base_T_frame_initial_estimate_2,
+                          SE3f* out_base_T_frame_estimate, int num_scales = 5, bba_odometry_result* result = nullptr) {
+    bba_odometry_options o{};
+    o.num_scales = num_scales;
+    o.use_pyramid_level_0 = use_pyramid_level_0;
+    o.use_gradmag = use_gradmag;
+    o.test_different_initial_estimates = test_different_initial_estimates;
+    o.max_iterations_per_scale = 30;
+    float out[7];
+    Check(bba_track_frame_pairwise_to_frame(h_, &o, base_depth_buffer.address, base_depth_buffer.pitch_bytes, base_normals_buffer.address,
+                                            base_normals_buffer.pitch_bytes, base_color_buffer_rgba.address,
+                                            base_color_buffer_rgba.pitch_bytes, tracked_depth_buffer.address,
+                                            tracked_depth_buffer.pitch_bytes, tracked_normals_buffer.address,
+                                            tracked_normals_buffer.pitch_bytes, tracked_color_buffer_rgba.address,
+                                            tracked_color_buffer_rgba.pitch_bytes, base_T_frame_initial_estimate_1.data(),
+                                            base_T_frame_initial_estimate_2.data(), out, result, stream),
+          "bba_track_frame_pairwise_to_frame");
+    std::memcpy(out_base_T_frame_estimate->data(), out, sizeof(out));
+  }
+
   // direct_ba.h:143-162, same argument order and defaults (Timer* is any type with GetTimeSinceStart()).
   template <typename TimerT = NoTimer>
   void BundleAdjustment(cudaStream_t stream, bool optimize_depth_intrinsics, bool optimize_color_intrinsics, bool do_surfel_updates,
