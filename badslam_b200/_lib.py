@@ -149,6 +149,7 @@ SYMBOLS = {
     "bba_host_motion_model_predict": (C.c_int, [C.POINTER(MotionModelRecord), C.c_int, _P, _P]),
     "bba_host_motion_model_push": (None, [C.POINTER(MotionModelRecord), _P]),
     "bba_host_motion_model_rebase": (None, [C.POINTER(MotionModelRecord)]),
+    "bba_host_deform_trajectory": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, _P]),
     "bba_set_residual_types": (C.c_int, [_P, C.c_int, C.c_int]),
     "bba_get_residual_types": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "bba_set_cfactor_host": (C.c_int, [_P, _P, _P]),

@@ -618,6 +618,45 @@ void bba_host_motion_model_rebase(bba_motion_model* m) {   // bad_slam.cc:1057-1
   CopyPose(kIdentityPose, m->frame_tr_base_kf[m->count - 1]);
 }
 
+// Trajectory deformation after a BA call.  Statement by statement trajectory_deformation.cc:45-130 on arrays: keyframes are never
+// null here (no deletion), so the reference's skipping of null entries has nothing to skip.  A frame's frame_T_global is the
+// inverse of its global_T_frame, as ImageFrame::SetGlobalTFrame stores it (libvis image_frame.h:84-88).
+int bba_host_deform_trajectory(int keyframe_count, const int* keyframe_frame_index, const float* original_keyframe_T_global,
+                               const float* keyframe_global_T_frame, int start_frame, int end_frame, float* frame_global_T_frame) {
+  if (keyframe_count < 1 || !keyframe_frame_index || !original_keyframe_T_global || !keyframe_global_T_frame ||
+      !frame_global_T_frame || start_frame < 0 || start_frame > end_frame || keyframe_frame_index[0] < 0)
+    return BBA_ERR_INVALID_ARGUMENT;
+  for (int k = 1; k < keyframe_count; ++k)
+    if (keyframe_frame_index[k] <= keyframe_frame_index[k - 1]) return BBA_ERR_INVALID_ARGUMENT;
+  const int K = keyframe_count;
+  const int* kf_frame = keyframe_frame_index;
+  auto original = [&](int k) { return PoseFromArray(original_keyframe_T_global + 7 * k); };
+  auto kf_global_T_frame = [&](int k) { return PoseFromArray(keyframe_global_T_frame + 7 * k); };
+  int prev = 0, next = 0;
+  for (int frame = start_frame; frame <= end_frame; ++frame) {
+    while (next < K && kf_frame[next] <= frame) prev = next++;
+    if (kf_frame[prev] == frame) continue;   // a keyframe
+    float* pose = frame_global_T_frame + 7 * static_cast<size_t>(frame);
+    const Pose global_T_other = PoseFromArray(pose);
+    Pose new_global_T_other;
+    if (next >= K || kf_frame[prev] > frame) {   // extrapolate at the end / at the start
+      new_global_T_other = bba::Compose(kf_global_T_frame(prev), bba::Compose(original(prev), global_T_other));
+    } else {   // interpolate
+      const Pose other_T_global = bba::Inverse(global_T_other);
+      const Pose from_prev = bba::Compose(other_T_global, bba::Compose(kf_global_T_frame(prev), bba::Compose(original(prev), global_T_other)));
+      const Pose from_next = bba::Compose(other_T_global, bba::Compose(kf_global_T_frame(next), bba::Compose(original(next), global_T_other)));
+      const float factor = static_cast<float>(frame - kf_frame[prev]) * 1.0f / static_cast<float>(kf_frame[next] - kf_frame[prev]);
+      Pose interpolated;
+      for (int i = 0; i < 3; ++i) interpolated.t[i] = (1 - factor) * from_prev.t[i] + factor * from_next.t[i];
+      bba::QuatSlerp(from_prev.q, factor, from_next.q, interpolated.q);
+      bba::QuatNormalize(interpolated.q);
+      new_global_T_other = bba::Compose(global_T_other, interpolated);
+    }
+    PoseToArray(new_global_T_other, pose);
+  }
+  return BBA_OK;
+}
+
 // The readers below are front-end calls: they read the published state (identical to the live state between BA-side calls).
 int bba_keyframe_count(bba_handle h) {
   if (!h) return 0;

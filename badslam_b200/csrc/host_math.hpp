@@ -82,6 +82,33 @@ BBA_HD Pose Compose(const Pose& a, const Pose& b) {   // se3.hpp:203-207, so3.hp
   return r;
 }
 
+// Quaternion interpolation of the trajectory deformation, host only.  Eigen's 4-float dot product and squared norm reduce as its
+// SSE packet code does, (x + z) + (y + w); sin / acos are the fp32 library functions std::sin / std::acos call for float.
+inline float QuatDot(const float a[4], const float b[4]) { return (a[0] * b[0] + a[2] * b[2]) + (a[1] * b[1] + a[3] * b[3]); }
+
+inline void QuatSlerp(const float q0[4], float t, const float q1[4], float out[4]) {   // Eigen QuaternionBase::slerp
+  const float one = 1.0f - 1.1920928955078125e-7f;   // 1 - NumTraits<float>::epsilon()
+  const float d = QuatDot(q0, q1);
+  const float abs_d = fabsf(d);
+  float scale0, scale1;
+  if (abs_d >= one) {
+    scale0 = 1.0f - t;
+    scale1 = t;
+  } else {
+    const float theta = acosf(abs_d);
+    const float sin_theta = sinf(theta);
+    scale0 = sinf((1.0f - t) * theta) / sin_theta;
+    scale1 = sinf(t * theta) / sin_theta;
+  }
+  if (d < 0.0f) scale1 = -scale1;
+  for (int i = 0; i < 4; ++i) out[i] = scale0 * q0[i] + scale1 * q1[i];
+}
+
+inline void QuatNormalize(float q[4]) {   // so3.hpp:159-168 (SO3::normalize, behind setQuaternion)
+  const float length = sqrtf(QuatDot(q, q));
+  for (int i = 0; i < 4; ++i) q[i] /= length;
+}
+
 // Row-major 3x4 [R|t].
 BBA_HD void ToMatrix3x4(const Pose& p, float M[12]) {
   float R[9];

@@ -155,6 +155,27 @@ class MotionModel:
         return np.array([list(self._m.frame_tr_base_kf[i]) for i in range(self._m.count)], np.float32).reshape(-1, 7)
 
 
+def deform_trajectory(start_frame: int, end_frame: int, keyframe_frame_indices, original_keyframe_T_global,
+                      keyframe_global_T_frame, frame_poses):
+    """ExtrapolateAndInterpolateKeyframePoseChanges (trajectory_deformation.cc:45-130) on explicit keyframe poses
+    (bba_host_deform_trajectory): the non-keyframe frames in [start_frame, min(end_frame, len(frame_poses) - 1)] of
+    frame_poses ([N, 7] global_T_frame) follow the change from original_keyframe_T_global ([K, 7] frame_T_global before the BA
+    call) to keyframe_global_T_frame ([K, 7] after it).  frame_poses is updated in place and returned."""
+    idx = np.ascontiguousarray(keyframe_frame_indices, np.int32)
+    original = np.ascontiguousarray(original_keyframe_T_global, np.float32).reshape(-1, 7)
+    current = np.ascontiguousarray(keyframe_global_T_frame, np.float32).reshape(-1, 7)
+    if not (len(idx) == len(original) == len(current)):
+        raise BadBAError(_lib.ERR_INVALID_ARGUMENT, "one frame index, original and current pose per keyframe")
+    if frame_poses.dtype != np.float32 or frame_poses.ndim != 2 or frame_poses.shape[1] != 7 or not frame_poses.flags.c_contiguous:
+        raise BadBAError(_lib.ERR_INVALID_ARGUMENT, "frame_poses must be a C-contiguous float32 [N, 7] array (updated in place)")
+    end_frame = min(int(end_frame), frame_poses.shape[0] - 1)   # trajectory_deformation.cc:51
+    st = _lib.load().bba_host_deform_trajectory(len(idx), idx.ctypes.data, original.ctypes.data, current.ctypes.data,
+                                                int(start_frame), end_frame, frame_poses.ctypes.data)
+    if st != _lib.OK:
+        raise BadBAError(st, "bba_host_deform_trajectory: invalid arguments")
+    return frame_poses
+
+
 class DirectBA:
     """Drop-in for vis::DirectBA (direct_ba.h:65-550) backed by the sm_90a library."""
 
@@ -435,6 +456,30 @@ class DirectBA:
         a = np.zeros(K, np.int32)
         self._check(self._lib.bba_get_keyframe_states(self._h, K, p.ctypes.data, a.ctypes.data))
         return p, a
+
+    # -- trajectory deformation around a BA call (trajectory_deformation.h:43-58) ----------------------------------------
+    def RememberKeyframePoses(self) -> np.ndarray:
+        """RememberKeyframePoses (trajectory_deformation.cc:33-42): frame_T_global of every keyframe, [K, 7], all from one
+        publication of the poses (bba_get_keyframe_states), so the front-end thread may call it while a BA call runs."""
+        K = self._lib.bba_keyframe_count(self._h)
+        p = np.zeros((K, 7), np.float32)
+        self._check(self._lib.bba_get_keyframe_states(self._h, K, p.ctypes.data, None))
+        out = np.empty_like(p)
+        for k in range(K):
+            self._lib.bba_host_se3_inverse(p[k].ctypes.data, out[k].ctypes.data)
+        return out
+
+    def ExtrapolateAndInterpolateKeyframePoseChanges(self, start_frame: int, end_frame: int, original_keyframe_T_global,
+                                                     keyframe_frame_indices, frame_poses: np.ndarray) -> np.ndarray:
+        """ExtrapolateAndInterpolateKeyframePoseChanges (trajectory_deformation.cc:45-130): moves the frames that are not
+        keyframes with the keyframes' pose change since RememberKeyframePoses.  original_keyframe_T_global: what
+        RememberKeyframePoses returned ([K, 7]); keyframe_frame_indices: the frame index of each of those K keyframes
+        (Keyframe.frame_index); frame_poses: global_T_frame of every frame, a C-contiguous float32 [N, 7] array, updated in place
+        and returned.  The keyframes' own rows are not touched."""
+        K = len(original_keyframe_T_global)
+        current = np.zeros((K, 7), np.float32)
+        self._check(self._lib.bba_get_keyframe_states(self._h, K, current.ctypes.data, None))
+        return deform_trajectory(start_frame, end_frame, keyframe_frame_indices, original_keyframe_T_global, current, frame_poses)
 
     def SurfelsDeviceView(self) -> torch.Tensor:
         """The 17-row surfel buffer as a torch tensor, whoever owns it (zero-copy)."""

@@ -540,6 +540,22 @@ void bba_host_motion_model_push(bba_motion_model* m, const float base_T_frame_es
 /* A keyframe was created from the frame tracked last: re-express the older estimates relative to it; the last becomes identity. */
 void bba_host_motion_model_rebase(bba_motion_model* m);
 
+/* ExtrapolateAndInterpolateKeyframePoseChanges (trajectory_deformation.cc:45-130) on caller arrays: after a bundle adjustment
+ * moved the keyframes, every frame in [start_frame, end_frame] that is not a keyframe is moved with them.  A frame before the
+ * first or after the last keyframe gets the change of the nearest keyframe; a frame between two keyframes gets the two
+ * keyframes' "old frame to new frame" corrections interpolated by its frame index (translation linearly, rotation by Eigen's
+ * Quaternion::slerp, renormalised like Sophus' setQuaternion).  SE3 arithmetic in fp32, like Sophus::SE3f.
+ *   keyframe_frame_index        [K]: frame index of each keyframe, >= 0 and strictly increasing
+ *   original_keyframe_T_global  [K][7]: each keyframe's frame_T_global before the BA call (RememberKeyframePoses)
+ *   keyframe_global_T_frame     [K][7]: each keyframe's global_T_frame after it
+ *   frame_global_T_frame        [end_frame + 1][7]: global_T_frame of every frame, updated in place for the non-keyframes in
+ *                               [start_frame, end_frame]; nothing else is read or written.  The caller clamps end_frame to its
+ *                               frame count - 1 (trajectory_deformation.cc:51).
+ * Returns BBA_OK, or BBA_ERR_INVALID_ARGUMENT without writing anything if keyframe_count < 1, an array is NULL, the keyframe
+ * frame indices are negative or not strictly increasing, start_frame < 0 or start_frame > end_frame. */
+int  bba_host_deform_trajectory(int keyframe_count, const int* keyframe_frame_index, const float* original_keyframe_T_global,
+                                const float* keyframe_global_T_frame, int start_frame, int end_frame, float* frame_global_T_frame);
+
 /* ---- instrumentation ---- */
 uint64_t   bba_kernel_launch_count(bba_handle h);   /* kernels launched through this handle so far */
 

@@ -15,6 +15,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <cstddef>
 #include <cstring>
@@ -105,13 +106,25 @@ class DirectBA {
   // DirectBA::AddKeyframe(const shared_ptr<Keyframe>&): pass keyframe->depth_buffer().ToCUDA() etc.
   int AddKeyframe(cudaStream_t stream, DeviceImage<uint16_t> depth, DeviceImage<uint16_t> normals, DeviceImage<uint16_t> radius,
                   DeviceImage<uint8_t> color_rgba, const SE3f& global_T_frame, float min_depth, float max_depth) {
+    return AddKeyframe(stream, -1, depth, normals, radius, color_rgba, global_T_frame, min_depth, max_depth);
+  }
+
+  // ... recording the keyframe's frame index in the video (Keyframe::frame_index(), keyframe.h:95), which
+  // ExtrapolateAndInterpolateKeyframePoseChanges needs.  The index stays in the adaptor; the library does not use it.
+  int AddKeyframe(cudaStream_t stream, int frame_index, DeviceImage<uint16_t> depth, DeviceImage<uint16_t> normals,
+                  DeviceImage<uint16_t> radius, DeviceImage<uint8_t> color_rgba, const SE3f& global_T_frame, float min_depth,
+                  float max_depth) {
     int id = -1;
     Check(bba_add_keyframe(h_, depth.address, depth.pitch_bytes, normals.address, normals.pitch_bytes, radius.address,
                            radius.pitch_bytes, color_rgba.address, color_rgba.pitch_bytes, global_T_frame.data(), min_depth,
                            max_depth, stream, &id),
           "bba_add_keyframe");
+    if (static_cast<size_t>(id) >= keyframe_frame_index_.size()) keyframe_frame_index_.resize(id + 1, -1);
+    keyframe_frame_index_[id] = frame_index;
     return id;
   }
+  // The frame index given to AddKeyframe (-1: added without one).
+  int keyframe_frame_index(int keyframe_id) const { return keyframe_frame_index_.at(keyframe_id); }
 
   // direct_ba.h:122-129 (frame = an already added keyframe)
   void EstimateFramePose(cudaStream_t stream, const SE3f& global_T_frame_initial_estimate, int keyframe_id,
@@ -333,6 +346,7 @@ class DirectBA {
   }
   bba_handle h_ = nullptr;
   bba_ba_result last_result_{};
+  std::vector<int> keyframe_frame_index_;   // by keyframe id; written by AddKeyframe (BA side)
   int pcg_gauge_keyframe_ = -1;
   int min_observation_counts_[3] = {1, 2, 3};
   mutable std::mutex mutex_;
@@ -410,5 +424,75 @@ class MotionModel {
   bba_motion_model m_{};
   bool use_motion_model_;
 };
+
+// The trajectory deformation around a BA call (trajectory_deformation.h:43-58), under the reference's names so that
+// BadSlam::RunBundleAdjustment and BAThreadMain (bad_slam.cc:505-533, 1267-1301) keep their shape:
+//   std::vector<SE3f> original_keyframe_T_global;
+//   RememberKeyframePoses(*direct_ba_, &original_keyframe_T_global);
+//   direct_ba_->BundleAdjustment(...);
+//   ExtrapolateAndInterpolateKeyframePoseChanges(start_frame, last_frame_index, *direct_ba_, original_keyframe_T_global, rgbd_video);
+
+// frame_T_global of every keyframe, all from one publication of the poses (bba_get_keyframe_states): a front-end call, so the
+// odometry thread may make it while a BA call runs.
+template <typename SE3f, typename PinholeCamera4f>
+void RememberKeyframePoses(const DirectBA<SE3f, PinholeCamera4f>& dense_ba, std::vector<SE3f>* original_keyframe_T_global) {
+  const int K = bba_keyframe_count(dense_ba.handle());
+  std::vector<float> poses(7 * static_cast<size_t>(K));
+  if (bba_get_keyframe_states(dense_ba.handle(), K, poses.data(), nullptr) != BBA_OK)
+    throw Error(BBA_ERR_INVALID_ARGUMENT, "RememberKeyframePoses: bba_get_keyframe_states failed");
+  original_keyframe_T_global->resize(K);
+  for (int k = 0; k < K; ++k) bba_host_se3_inverse(poses.data() + 7 * k, (*original_keyframe_T_global)[k].data());
+}
+
+// The deformation on explicit keyframe data: keyframe_frame_index[k], original_keyframe_T_global[k] (before the BA call) and
+// keyframe_global_T_frame[k] (after it) for the same K keyframes.  RGBDVideo is any type with frame_count() and
+// depth_frame_mutable(i) / color_frame_mutable(i) pointing to frames with global_T_frame() and SetGlobalTFrame() (libvis
+// RGBDVideo<Vec3u8, u16>).  Only frames in [start_frame, end_frame] that are not keyframes are set, depth and colour frame alike.
+template <typename SE3f, typename RGBDVideo>
+void ExtrapolateAndInterpolateKeyframePoseChanges(uint32_t start_frame, uint32_t end_frame, const std::vector<int>& keyframe_frame_index,
+                                                  const std::vector<SE3f>& original_keyframe_T_global,
+                                                  const std::vector<SE3f>& keyframe_global_T_frame, RGBDVideo* rgbd_video) {
+  const int K = static_cast<int>(keyframe_frame_index.size());
+  if (original_keyframe_T_global.size() != keyframe_frame_index.size() || keyframe_global_T_frame.size() != keyframe_frame_index.size())
+    throw Error(BBA_ERR_INVALID_ARGUMENT, "ExtrapolateAndInterpolateKeyframePoseChanges: one frame index and two poses per keyframe");
+  const int64_t last = std::min<int64_t>(end_frame, static_cast<int64_t>(rgbd_video->frame_count()) - 1);   // trajectory_deformation.cc:51
+  if (last < static_cast<int64_t>(start_frame)) return;
+  const int first = static_cast<int>(start_frame), end = static_cast<int>(last);
+  std::vector<float> original(7 * static_cast<size_t>(K)), current(7 * static_cast<size_t>(K));
+  for (int k = 0; k < K; ++k) {
+    std::memcpy(&original[7 * k], original_keyframe_T_global[k].data(), 7 * sizeof(float));
+    std::memcpy(&current[7 * k], keyframe_global_T_frame[k].data(), 7 * sizeof(float));
+  }
+  std::vector<float> frames(7 * (static_cast<size_t>(end) + 1));
+  for (int i = first; i <= end; ++i) std::memcpy(&frames[7 * i], rgbd_video->depth_frame_mutable(i)->global_T_frame().data(), 7 * sizeof(float));
+  if (bba_host_deform_trajectory(K, keyframe_frame_index.data(), original.data(), current.data(), first, end, frames.data()) != BBA_OK)
+    throw Error(BBA_ERR_INVALID_ARGUMENT, "ExtrapolateAndInterpolateKeyframePoseChanges: no keyframe, or frame indices not increasing");
+  for (int i = first; i <= end; ++i) {
+    if (std::binary_search(keyframe_frame_index.begin(), keyframe_frame_index.end(), i)) continue;
+    SE3f new_global_T_frame;
+    std::memcpy(new_global_T_frame.data(), &frames[7 * i], 7 * sizeof(float));
+    rgbd_video->depth_frame_mutable(i)->SetGlobalTFrame(new_global_T_frame);
+    rgbd_video->color_frame_mutable(i)->SetGlobalTFrame(new_global_T_frame);
+  }
+}
+
+// ... with the keyframes of `dense_ba`: the first original_keyframe_T_global.size() keyframes, their current (published) poses
+// and the frame indices given to AddKeyframe.  Called where BadSlam calls it, with the BA side idle (under DirectBA::Lock()).
+template <typename SE3f, typename PinholeCamera4f, typename RGBDVideo>
+void ExtrapolateAndInterpolateKeyframePoseChanges(uint32_t start_frame, uint32_t end_frame, const DirectBA<SE3f, PinholeCamera4f>& dense_ba,
+                                                  const std::vector<SE3f>& original_keyframe_T_global, RGBDVideo* rgbd_video) {
+  const int K = static_cast<int>(original_keyframe_T_global.size());
+  std::vector<int> frame_index(K);
+  for (int k = 0; k < K; ++k) {
+    frame_index[k] = dense_ba.keyframe_frame_index(k);
+    if (frame_index[k] < 0) throw Error(BBA_ERR_STATE, "ExtrapolateAndInterpolateKeyframePoseChanges: keyframe added without a frame index");
+  }
+  std::vector<float> poses(7 * static_cast<size_t>(K));
+  if (bba_get_keyframe_states(dense_ba.handle(), K, poses.data(), nullptr) != BBA_OK)
+    throw Error(BBA_ERR_INVALID_ARGUMENT, "ExtrapolateAndInterpolateKeyframePoseChanges: bba_get_keyframe_states failed");
+  std::vector<SE3f> current(K);
+  for (int k = 0; k < K; ++k) std::memcpy(current[k].data(), poses.data() + 7 * k, 7 * sizeof(float));
+  ExtrapolateAndInterpolateKeyframePoseChanges(start_frame, end_frame, frame_index, original_keyframe_T_global, current, rgbd_video);
+}
 
 }  // namespace badba

@@ -4,12 +4,24 @@
     python tools/run_dataset.py /tmp/synth --trajectory groundtruth.txt --keyframe-interval 1 --raw-to-float-depth 0.001
     python tools/run_dataset.py /path/to/eth3d/sequence --trajectory groundtruth.txt        # 5000 raw units per metre (default)
 
-Every `--keyframe-interval`-th frame becomes a keyframe at its trajectory pose (the reference's odometry front-end is out of
-scope: poses come from the file, perturbed by --pose-noise to give BA something to do): raw depth + colour are uploaded,
-DirectBA.CreateKeyframeFromFrame preprocesses them on the device (bba_preprocess_frame, or bba_preprocess_raw_frame with
---median-filter-iterations / --pyramid-level-for-depth / --pyramid-level-for-color: the full-resolution frames are uploaded and
-filtered or downscaled in the same launch, the cameras are the calibration's Scaled(0.5 ** level)) and adds the keyframe,
-surfels are created for it, and BundleAdjustment runs every --ba-interval keyframes.  Prints one JSON line.
+Every `--keyframe-interval`-th frame becomes a keyframe at its trajectory pose, perturbed by --pose-noise to give BA something to
+do: raw depth + colour are uploaded, DirectBA.CreateKeyframeFromFrame preprocesses them on the device (bba_preprocess_frame, or
+bba_preprocess_raw_frame with --median-filter-iterations / --pyramid-level-for-depth / --pyramid-level-for-color: the
+full-resolution frames are uploaded and filtered or downscaled in the same launch, the cameras are the calibration's
+Scaled(0.5 ** level)) and adds the keyframe, surfels are created for it, and BundleAdjustment runs every --ba-interval keyframes.
+Prints one JSON line.
+
+With --export-poses PATH every frame gets a pose, as BadSlam computes one: each frame after the first keyframe is preprocessed
+and tracked against the last keyframe with the image-pair odometry (bba_track_frame_pairwise), seeded by the motion model
+(direct_ba.MotionModel: predict, track, push; rebased when the frame becomes a keyframe), like BadSlam::RunOdometry.  Keyframes
+keep their trajectory pose (+ noise).  Every BundleAdjustment call is wrapped in RememberKeyframePoses /
+ExtrapolateAndInterpolateKeyframePoseChanges, so the tracked frames move with their keyframes, and the trajectory of all frames
+is written in the TUM format of rgbd_dataset.save_poses:
+
+    python tools/run_dataset.py /tmp/synth --keyframe-interval 2 --raw-to-float-depth 0.001 --export-poses /tmp/synth/poses.txt
+
+The views of --make-synthetic lie metres apart (a BA test scene, not a video), so odometry between them fails and only the
+keyframe poses of that sequence are meaningful; on a recorded sequence every frame is tracked from its neighbour.
 """
 import argparse
 import json
@@ -50,6 +62,8 @@ def main():
                     help="median densify filter passes over the raw depth (0..8)")
     ap.add_argument("--pyramid-level-for-depth", type=int, default=0, help="downscale the depth by 2^level (0..3)")
     ap.add_argument("--pyramid-level-for-color", type=int, default=0, help="downscale the colour by 2^level (0..3)")
+    ap.add_argument("--export-poses", metavar="PATH", default=None,
+                    help="track every frame, deform the tracked poses with each BA call and write all frames' poses (TUM format)")
     a = ap.parse_args()
     if a.make_synthetic:
         make_synthetic(a.make_synthetic)
@@ -57,7 +71,7 @@ def main():
     import torch
     from badslam_b200 import rgbd_dataset as D
     from badslam_b200 import scene as S
-    from badslam_b200.direct_ba import DirectBA, PinholeCamera4f
+    from badslam_b200.direct_ba import DirectBA, MotionModel, PinholeCamera4f
     ds = D.TUMRGBDDataset(a.folder, a.trajectory)
     cam = PinholeCamera4f(ds.width, ds.height, ds.camera_parameters)
     idx = list(range(0, len(ds), a.keyframe_interval))[:a.max_keyframes]
@@ -71,7 +85,29 @@ def main():
     ba.SetSurfels(surfels, 0)
     rng = np.random.default_rng(0)
     true_poses, t_pre, t_ba, created, results = [], 0.0, 0.0, 0, []
-    for n, i in enumerate(idx):
+    export = a.export_poses is not None
+    keyframe_frames = set(idx)
+    frame_poses = np.zeros((len(ds), 7), np.float32)   # global_T_frame of every frame (--export-poses)
+    motion_model, base_kf, tracked, t_odometry = MotionModel(), None, 0, 0.0
+    n = -1   # keyframes added so far - 1
+    for i in (range(len(ds)) if export else idx):
+        if export and base_kf is not None:
+            # BadSlam::RunOdometry: the frame against the last keyframe, seeded by the motion model
+            raw = torch.from_numpy(ds.load_depth(i).view(np.int16)).cuda()
+            rgb = torch.from_numpy(ds.load_color(i)).cuda()
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            depth, normals, _, rgba, _, _ = ba.PreprocessFrame(raw, rgb, max_depth=a.max_depth, want_min_max=False, **raw_options)
+            e1, e2 = motion_model.PredictFramePose()
+            base_T_frame, _ = ba.TrackFramePairwise(None, base_kf.id, depth, normals, rgba, e1, e2)
+            motion_model.Push(base_T_frame)
+            ba._lib.bba_host_se3_compose(base_kf.global_T_frame().ctypes.data, base_T_frame.ctypes.data, frame_poses[i].ctypes.data)
+            torch.cuda.synchronize()
+            t_odometry += time.perf_counter() - t
+            tracked += 1
+        if i not in keyframe_frames:
+            continue
+        n += 1
         pose = ds.frames[i].depth_global_T_frame
         true_poses.append(pose)
         noisy = S.se3_mul(pose, S.se3_exp(np.concatenate([rng.normal(0, a.pose_noise, 3), rng.normal(0, a.pose_noise, 3)])))
@@ -83,20 +119,38 @@ def main():
         created += ba.CreateSurfelsForKeyframe(None, True, kf.id)
         torch.cuda.synchronize()
         t_pre += time.perf_counter() - t
+        if export:
+            frame_poses[i] = noisy
+            if base_kf is not None:
+                motion_model.Rebase()   # bad_slam.cc:1057-1068: the frame tracked last became a keyframe
+            base_kf = kf
         if (n + 1) % a.ba_interval == 0 or n + 1 == len(idx):
+            original = ba.RememberKeyframePoses() if export else None
             t = time.perf_counter()
             r = ba.BundleAdjustment(None, False, False, True, True, True, 1, a.ba_iterations)
             torch.cuda.synchronize()
             t_ba += time.perf_counter() - t
             results.append((r.iterations_done, int(r.depth_residual_count + r.descriptor_residual_count), r.surfels_size))
+            if export:   # bad_slam.cc:1267-1301
+                ba.ExtrapolateAndInterpolateKeyframePoseChanges(0, i, original, [k.frame_index for k in ba.keyframes()], frame_poses)
     poses = ba.GetKeyframeStates()[0]
     rel = lambda P, k: S.se3_mul(S.se3_inverse(P[0]), P[k])
     err = [S.pose_error(rel(poses, k), rel(true_poses, k)) for k in range(1, len(idx))]
-    print(json.dumps({"frames": len(ds), "keyframes": len(idx), "image": [ds.width, ds.height],
-                      "depth_image": [depth_cam.width, depth_cam.height], "surfels_created": created,
-                      "surfels": ba.surfels_size(), "ba_calls": results, "seconds_preprocess_and_creation": round(t_pre, 3),
-                      "seconds_bundle_adjustment": round(t_ba, 3),
-                      "max_relative_pose_error_m_rad": [max(e[0] for e in err), max(e[1] for e in err)] if err else None}))
+    line = {"frames": len(ds), "keyframes": len(idx), "image": [ds.width, ds.height],
+            "depth_image": [depth_cam.width, depth_cam.height], "surfels_created": created,
+            "surfels": ba.surfels_size(), "ba_calls": results, "seconds_preprocess_and_creation": round(t_pre, 3),
+            "seconds_bundle_adjustment": round(t_ba, 3),
+            "max_relative_pose_error_m_rad": [max(e[0] for e in err), max(e[1] for e in err)] if err else None}
+    if export:
+        frame_poses[idx] = poses
+        all_true = [f.depth_global_T_frame for f in ds.frames]
+        frame_err = [S.pose_error(rel(frame_poses, k), rel(all_true, k)) for k in range(1, len(ds))]
+        if not D.save_poses(a.export_poses, [f.depth_time_string for f in ds.frames], frame_poses):
+            print(f"cannot write {a.export_poses}", file=sys.stderr)
+            return 1
+        line.update({"frames_tracked": tracked, "seconds_odometry": round(t_odometry, 3), "poses_exported": len(ds),
+                     "max_relative_frame_pose_error_m_rad": [max(e[0] for e in frame_err), max(e[1] for e in frame_err)] if frame_err else None})
+    print(json.dumps(line))
     return 0
 
 
