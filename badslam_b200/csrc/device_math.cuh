@@ -83,26 +83,6 @@ __device__ __forceinline__ Vec3 Transform(const float* __restrict__ T, const Vec
             T[8] * p.x + T[9] * p.y + T[10] * p.z + T[11]);
 }
 
-// Sums acc[i] over the 32 lanes of the warp for all 32 i at once: after the call lane L holds the total of
-// acc[L].  16+8+4+2+1 = 31 shuffles instead of 32 x 5.  One template level per butterfly stage: written as a loop over the
-// stages, the outer loop is not unrolled and v lives in a 128-byte stack frame.
-template <int HALF>
-__device__ __forceinline__ void WarpTransposeStage(float (&v)[32], int lane) {
-  const bool upper = (lane & HALF) != 0;
-#pragma unroll
-  for (int i = 0; i < HALF; ++i) {
-    const float lo = v[i], hi = v[i + HALF];
-    const float send = upper ? lo : hi;
-    const float keep = upper ? hi : lo;
-    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, HALF);
-  }
-  if constexpr (HALF > 1) WarpTransposeStage<HALF / 2>(v, lane);
-}
-__device__ __forceinline__ float WarpTransposeReduce(float (&v)[32], int lane) {
-  WarpTransposeStage<16>(v, lane);
-  return v[0];
-}
-
 // robust_weighting.cuh:39-86
 __device__ __forceinline__ float TukeyResidual(float r, float p) {
   if (fabsf(r) < p) {
@@ -213,6 +193,13 @@ __device__ __forceinline__ bool ProjectIntoImage(const CameraParams& cam, const 
   return (r->pxf >= 0.f) && (r->pyf >= 0.f) && r->px < cam.w && r->py < cam.h;
 }
 
+// The sparse cell (cfactor entry) of pixel (px, py): exact integer division by multiplication with a precomputed reciprocal.
+__device__ __forceinline__ unsigned int SparseCell(const CameraParams& cam, int px, int py) {
+  const unsigned int cx = (cam.cell == 1) ? static_cast<unsigned int>(px) : __umulhi(static_cast<unsigned int>(px), cam.cell_magic);
+  const unsigned int cy = (cam.cell == 1) ? static_cast<unsigned int>(py) : __umulhi(static_cast<unsigned int>(py), cam.cell_magic);
+  return cy * cam.cf_w + cx;
+}
+
 // Step B: the three independent gathers of the pixel the surfel projects to.  The keyframe normal is fetched together
 // with the depth (the reference reads it only after the depth and facing tests passed; ~99 % of in-image pairs do).
 struct PixelLoads {
@@ -225,7 +212,8 @@ __device__ __forceinline__ PixelLoads LoadPixel(const CameraParams& cam, const u
   PixelLoads l;
   l.measured = LoadU16Now(reinterpret_cast<const uint16_t*>(reinterpret_cast<const char*>(depth) + static_cast<size_t>(r.py) * depth_pitch) + r.px);
   l.kf_normal = LoadU16Now(reinterpret_cast<const uint16_t*>(reinterpret_cast<const char*>(normals) + static_cast<size_t>(r.py) * normals_pitch) + r.px);
-  // sparse cell of the pixel: exact integer division by multiplication with a precomputed reciprocal
+  // SparseCell spelled out: the address adds row and column to the pointer one at a time.  Through SparseCell's 32-bit index
+  // ptxas schedules the pose and geometry pair loops differently.
   const unsigned int cell_x = (cam.cell == 1) ? static_cast<unsigned int>(r.px) : __umulhi(static_cast<unsigned int>(r.px), cam.cell_magic);
   const unsigned int cell_y = (cam.cell == 1) ? static_cast<unsigned int>(r.py) : __umulhi(static_cast<unsigned int>(r.py), cam.cell_magic);
   l.cf = LoadF32Now(cam.cfactor + cell_y * cam.cf_w + cell_x);
@@ -278,6 +266,29 @@ __device__ __forceinline__ float DepthResidual(const CameraParams& cam, const As
   *inv_stddev = cam.baseline_fx / (kDepthUncertaintyFactor * fabsf(r.ln.x * r.nx + r.ln.y * r.ny + r.ln.z) * (r.d * r.d));
   *unproj = V3(r.d * r.nx, r.d * r.ny, r.d);
   return *inv_stddev * Dot(r.ln, *unproj - r.lp);
+}
+// kernel_opt_pose.cu:88-93: Jacobian of the depth residual wrt the pose, from DepthResidual's inv_stddev and unprojected point.
+__device__ __forceinline__ void DepthPoseJacobian(const Assoc& r, float inv_stddev, const Vec3& up, float (&J)[6]) {
+  J[0] = inv_stddev * r.ln.x;
+  J[1] = inv_stddev * r.ln.y;
+  J[2] = inv_stddev * r.ln.z;
+  J[3] = inv_stddev * (-r.ln.y * up.z + r.ln.z * up.y);
+  J[4] = inv_stddev * (r.ln.x * up.z - r.ln.z * up.x);
+  J[5] = inv_stddev * (-r.ln.x * up.y + r.ln.y * up.x);
+}
+
+// H += w J^T J (upper triangle, row-major), b += w r J   (gauss_newton.cuh:59-92, per thread)
+__device__ __forceinline__ void AccumulateHb(float (&acc)[32], const float (&J)[6], float raw, float w) {
+  int idx = 0;
+#pragma unroll
+  for (int r = 0; r < 6; ++r) {
+    const float wj = w * J[r];
+#pragma unroll
+    for (int c = r; c < 6; ++c) acc[idx++] += wj * J[c];
+  }
+  const float wr = w * raw;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) acc[21 + i] += wr * J[i];
 }
 
 // cost_function.cuh:115-136
@@ -366,6 +377,13 @@ __device__ __forceinline__ void DescPoseJacobian(const CameraParams& cam, const 
   J[3] = ((ls.y * ls.y + z_sq) * gy + xy * gx) * inv_z_sq;
   J[4] = -((ls.x * ls.x + z_sq) * gx + xy * gy) * inv_z_sq;
   J[5] = -(ls.x * gy - ls.y * gx) * inv_z;
+}
+
+// kernel_opt_intrinsics.cu:139-160 / kernel_pcg.cu:453-503: Jacobians of the two descriptor residuals wrt the colour camera's
+// (fx, fy, cx, cy), from the un-scaled gradients.
+__device__ __forceinline__ void ColorIntrinsicsJacobians(const Assoc& r, const DescEval& e, float (&J1)[4], float (&J2)[4]) {
+  J1[0] = e.gx1 * r.nx; J1[1] = e.gy1 * r.ny; J1[2] = e.gx1; J1[3] = e.gy1;
+  J2[0] = e.gx2 * r.nx; J2[1] = e.gy2 * r.ny; J2[2] = e.gx2; J2[3] = e.gy2;
 }
 
 }  // namespace bba

@@ -12,9 +12,7 @@
 // The 5x5 / 4x4 solves stay on the host in fp64 like the reference (kernel_opt_intrinsics.cc:171,272).
 #include <cuda.h>
 
-#include <algorithm>
-
-#include "kernels.cuh"
+#include "persistent.cuh"
 
 namespace bba {
 
@@ -23,47 +21,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kGroup = 16;
 constexpr int kTile = 256;
-
-__device__ __forceinline__ float WarpSum(float v) {
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// same butterfly as in kernels.cu (kept local: different translation unit)
-__device__ __forceinline__ float TransposeReduce32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-    const bool upper = (lane & half) != 0;
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float lo = v[i], hi = v[i + half];
-      const float send = upper ? lo : hi;
-      const float keep = upper ? hi : lo;
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-    }
-  }
-  return v[0];
-}
-
-struct KfLite {
-  float T[12];
-  const uint16_t* depth;
-  const uint16_t* normals;
-  cudaTextureObject_t tex;
-  uint32_t depth_pitch, normals_pitch;
-};
-
-__device__ __forceinline__ void LoadKfLite(const KfDevice* __restrict__ kfs, int kf, KfLite* r) {
-  const KfDevice& k = kfs[kf];
-#pragma unroll
-  for (int i = 0; i < 12; ++i) r->T[i] = __ldg(&k.T[i]);
-  r->depth = k.depth;
-  r->normals = k.normals;
-  r->tex = k.tex;
-  r->depth_pitch = k.depth_pitch;
-  r->normals_pitch = k.normals_pitch;
-}
 
 }  // namespace
 
@@ -76,12 +33,8 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
   const size_t P = a.pitch;
   const int lane = threadIdx.x & 31;
   const CameraParams& cam = a.cam;
-  for (;;) {
-    unsigned int item = 0;
-    if (lane == 0) item = atomicAdd(a.queue, 1u);
-    item = __shfl_sync(0xffffffffu, item, 0);
-    if (item >= n_items) break;
-    const uint32_t group = item / n_tiles, tile = item - group * n_tiles;
+  uint32_t group, tile;
+  while (ClaimItem(a.queue, n_tiles, n_items, nullptr, &group, &tile)) {
     const int j_begin = group * kGroup, j_end = min(a.kf_count, static_cast<int>(group + 1) * kGroup);
     float acc[32];
 #pragma unroll
@@ -100,8 +53,8 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
         d2 = a.surfels[kRowD2 * P + i];
       }
       for (int j = j_begin; j < j_end; ++j) {
-        KfLite K;
-        LoadKfLite(a.kfs, __ldg(a.kf_list + j), &K);
+        KfRegs K;
+        LoadKfGlobal(a.kfs, __ldg(a.kf_list + j), &K);
         Assoc r;
         if (!ProjectIntoImage(cam, K.T, gp, &r)) continue;
         const PixelLoads l = LoadPixel(cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r);
@@ -117,8 +70,6 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
         if (Associate(cam, K.T, nrm, l, &r) != 3) continue;
         if (OPT_DEPTH) {
           // kernel_opt_intrinsics.cu:84-121
-          const unsigned int spx = (cam.cell == 1) ? static_cast<unsigned int>(r.px) : __umulhi(static_cast<unsigned int>(r.px), cam.cell_magic);
-          const unsigned int spy = (cam.cell == 1) ? static_cast<unsigned int>(r.py) : __umulhi(static_cast<unsigned int>(r.py), cam.cell_magic);
           const float raw_inv_depth = 1.0f / (cam.raw_to_float * l.measured);
           const float exp_inv_depth = expf(-cam.a * raw_inv_depth);
           const float corrected_inv_depth = l.cf * exp_inv_depth + raw_inv_depth;
@@ -148,7 +99,7 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
 #pragma unroll
             for (int rr = 0; rr < 5; ++rr) acc[15 + rr] += wr * J[rr];
             // per-cell terms (kernel_opt_intrinsics.cu:173-190)
-            const unsigned int sp = spx + spy * cam.cf_w;
+            const unsigned int sp = SparseCell(cam, r.px, r.py);
 #pragma unroll
             for (int rr = 0; rr < 5; ++rr) atomicAdd(a.cell_B + static_cast<size_t>(rr) * a.cell_count + sp, w * J[rr] * J[5]);
             atomicAdd(a.cell_D + sp, w * J[5] * J[5]);
@@ -158,8 +109,8 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
         }
         if (OPT_COLOR && photo) {
           // kernel_opt_intrinsics.cu:139-160,193-211: residuals that are exactly 0 are skipped
-          const float J1[4] = {e.gx1 * r.nx, e.gy1 * r.ny, e.gx1, e.gy1};
-          const float J2[4] = {e.gx2 * r.nx, e.gy2 * r.ny, e.gx2, e.gy2};
+          float J1[4], J2[4];
+          ColorIntrinsicsJacobians(r, e, J1, J2);
           const float w1 = (e.r1 != 0) ? DescWeight(e.r1) : 0.f;
           const float w2 = (e.r2 != 0) ? DescWeight(e.r2) : 0.f;
           int idx = 20;
@@ -176,7 +127,7 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
       }
     }
     __syncwarp();
-    const float total = TransposeReduce32(acc, lane);
+    const float total = WarpTransposeReduce(acc, lane);
     if (total != 0.f) atomicAdd(a.sums + lane, static_cast<double>(total));
     if (OPT_COLOR) {
       extra0 = WarpSum(extra0);
@@ -263,9 +214,7 @@ void LaunchIntrinsicsAccumulate(const IntrinsicsArgs& a, int sm_count, bool opti
   auto launch = [&](auto kernel) {
     int per_sm = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, 0);
-    if (per_sm < 1) per_sm = 1;
-    const uint64_t ctas = std::min<uint64_t>((n_items + 7) / 8, static_cast<uint64_t>(per_sm) * sm_count);
-    kernel<<<static_cast<uint32_t>(ctas), kThreads, 0, stream>>>(a);
+    kernel<<<ItemGrid(per_sm, sm_count, n_items), kThreads, 0, stream>>>(a);
   };
   if (optimize_color && optimize_depth) launch(IntrinsicsAccumulateKernel<true, true>);
   else if (optimize_color) launch(IntrinsicsAccumulateKernel<true, false>);

@@ -13,7 +13,7 @@
 
 #include <algorithm>
 
-#include "kernels.cuh"
+#include "persistent.cuh"
 
 namespace bba {
 
@@ -22,15 +22,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kGroup = 16;
 constexpr uint32_t kDeletedPattern = 0x7fffffffu;   // CUDART_NAN_F
-
-__device__ __forceinline__ unsigned int LoadAcquire(const unsigned int* p) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void StoreRelease(unsigned int* p, unsigned int v) {
-  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 
 }  // namespace
 
@@ -42,27 +33,8 @@ __global__ void __launch_bounds__(kThreads) ObservationStatsKernel(const __grid_
   const size_t P = a.pitch;
   const int lane = threadIdx.x & 31;
   const CameraParams& cam = a.cam;
-  // result rows of this rank's surfels go to the local replica and -- with mapped peers -- to every other rank's (NVLink)
-  auto store_row = [&](int row, uint32_t i, float v) {
-    const size_t o = static_cast<size_t>(row) * P + i;
-    a.surfels[o] = v;
-#pragma unroll
-    for (int p = 0; p < kMaxPeers; ++p)
-      if (p < a.peers.count) a.peers.surfels[p][o] = v;
-  };
-  for (;;) {
-    // warp-owned item (group, tile); (g, t) runs after (g - 1, t) has been retired
-    unsigned int item = 0;
-    if (lane == 0) {
-      item = atomicAdd(a.queue, 1u);
-      if (item < n_items) {
-        const uint32_t g = item / n_tiles, t = item - g * n_tiles;
-        while (LoadAcquire(a.tile_epoch + t) < g) __nanosleep(64);
-      }
-    }
-    item = __shfl_sync(0xffffffffu, item, 0);
-    if (item >= n_items) break;
-    const uint32_t group = item / n_tiles, tile = item - group * n_tiles;
+  uint32_t group, tile;
+  while (ClaimItem(a.queue, n_tiles, n_items, a.tile_epoch, &group, &tile)) {
     const bool first = group == 0, last = group + 1 == n_groups;
     const int j_begin = group * kGroup, j_end = min(a.kf_count, static_cast<int>(group + 1) * kGroup);
     unsigned int deleted_here = 0;
@@ -115,22 +87,18 @@ __global__ void __launch_bounds__(kThreads) ObservationStatsKernel(const __grid_
           // MarkDeletedSurfelsCUDAKernel (kernel_delete_surfels.cu:129-164)
           if (obs < static_cast<float>(a.min_observation_count) || viol > obs) {
             if (__float_as_uint(x) != kDeletedPattern) {
-              store_row(kRowX, i, __uint_as_float(kDeletedPattern));
+              StoreReplicas(a.surfels, a.peers.surfels, a.peers.count, kRowX * P + i, __uint_as_float(kDeletedPattern));
               deleted = true;
             }
           } else {
-            store_row(kRowRadiusSq, i, min_r2);
+            StoreReplicas(a.surfels, a.peers.surfels, a.peers.count, kRowRadiusSq * P + i, min_r2);
           }
         }
       }
       deleted_here += __popc(__ballot_sync(0xffffffffu, deleted));
     }
-    __syncwarp();
-    if (lane == 0) {
-      if (deleted_here) atomicAdd(a.deleted_count, deleted_here);
-      __threadfence();
-      StoreRelease(a.tile_epoch + tile, group + 1);
-    }
+    if (lane == 0 && deleted_here) atomicAdd(a.deleted_count, deleted_here);
+    RetireItem(a.tile_epoch, group, tile);
   }
 }
 
@@ -324,12 +292,6 @@ __device__ __forceinline__ float SampleRgbaChannel(const LifecycleArgs& a, float
   return __fdiv_rn(static_cast<float>((sum + 128) >> 8), 65535.f);   // IEEE division: the texture unit's value, also under -use_fast_math
 }
 
-__device__ __forceinline__ unsigned int CellOf(const CameraParams& cam, int px, int py) {
-  const unsigned int cx = (cam.cell == 1) ? static_cast<unsigned int>(px) : __umulhi(static_cast<unsigned int>(px), cam.cell_magic);
-  const unsigned int cy = (cam.cell == 1) ? static_cast<unsigned int>(py) : __umulhi(static_cast<unsigned int>(py), cam.cell_magic);
-  return cy * cam.cf_w + cx;
-}
-
 }  // namespace
 
 // pass 0: the cell every surfel is associated with (cached) + smallest surfel index per cell
@@ -342,7 +304,7 @@ __global__ void __launch_bounds__(256) SupportLevel0Kernel(const __grid_constant
     Assoc r;
     unsigned int cell = kInvalidIndex;
     if (ProjectAssociate(a.cam, a.T, a.depth, a.depth_pitch, a.normals, a.normals_pitch, gp, nrm, &r) == 3) {
-      cell = CellOf(a.cam, r.px, r.py);
+      cell = SparseCell(a.cam, r.px, r.py);
       atomicMin(a.sup + cell, SurfelArrivalKey(i));   // (0xffffffff is the key of one index < 2^32 only in theory: n < 2^31)
     }
     cache[i] = cell;
@@ -446,7 +408,7 @@ __global__ void __launch_bounds__(128) FilterSeedsKernel(const __grid_constant__
     // IsAssociatedWithPixel<true> for a pixel-defined surfel (surfel_projection_nvcc_only.cuh:130-236)
     const uint16_t measured = LoadPixelU16(ce.depth, ce.depth_pitch, r.px, r.py);
     if (measured & kInvalidDepthBit) continue;
-    const float pd = RawToCalibratedDepth(cam.a, __ldg(cam.cfactor + CellOf(cam, r.px, r.py)), cam.raw_to_float, measured);
+    const float pd = RawToCalibratedDepth(cam.a, __ldg(cam.cfactor + SparseCell(cam, r.px, r.py)), cam.raw_to_float, measured);
     const Vec3 ln = Rotate(ce.R, n_in);
     const float nx = cam.fx_inv * r.px + cam.cx_inv, ny = cam.fy_inv * r.py + cam.cy_inv;
     const float thr = kDepthTukey * ((kDepthUncertaintyFactor * fabsf(ln.x * nx + ln.y * ny + ln.z) * (pd * pd)) / cam.baseline_fx);
@@ -471,7 +433,7 @@ __global__ void __launch_bounds__(256) CreateSurfelsKernel(const __grid_constant
   const int y = s / cam.w, x = s - y * cam.w;
   const uint32_t out = a.n + index[s];
   const size_t P = a.pitch;
-  const float d = RawToCalibratedDepth(cam.a, __ldg(cam.cfactor + CellOf(cam, x, y)), cam.raw_to_float, LoadPixelU16(a.depth, a.depth_pitch, x, y));
+  const float d = RawToCalibratedDepth(cam.a, __ldg(cam.cfactor + SparseCell(cam, x, y)), cam.raw_to_float, LoadPixelU16(a.depth, a.depth_pitch, x, y));
   const Vec3 gp = Transform(a.G, V3(d * (cam.fx_inv * x + cam.cx_inv), d * (cam.fy_inv * y + cam.cy_inv), d));
   const Vec3 gn = Rotate(a.G, U16ToImageSpaceNormal(LoadPixelU16(a.normals, a.normals_pitch, x, y)));
   const float r2 = __half2float(__ushort_as_half(LoadPixelU16(a.radius, a.radius_pitch, x, y)));
@@ -650,17 +612,11 @@ void LaunchObservationStats(SurfelStatsArgs a, int sm_count, cudaStream_t stream
   if (a.local_count == 0 || a.kf_count <= 0) return;
   int per_sm = 0;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ObservationStatsKernel, kThreads, 0);
-  if (per_sm < 1) per_sm = 1;
-  const uint64_t resident_warps = static_cast<uint64_t>(per_sm) * sm_count * (kThreads / 32);
-  int shift = 8;
-  while (shift > 5 && 2 * static_cast<uint64_t>((a.local_count + (1u << shift) - 1) >> shift) < 3 * resident_warps) --shift;
-  a.tile_shift = shift;
-  const uint32_t n_tiles = (a.local_count + (1u << shift) - 1) >> shift;
-  const uint64_t n_items = static_cast<uint64_t>(n_tiles) * ((a.kf_count + kGroup - 1) / kGroup);
+  const uint32_t ctas = EpochOrderedGrid(per_sm, sm_count, kThreads, a.local_count, (a.kf_count + kGroup - 1) / kGroup, &a.tile_shift);
+  const uint32_t n_tiles = (a.local_count + (1u << a.tile_shift) - 1) >> a.tile_shift;
   cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream);
   cudaMemsetAsync(a.tile_epoch, 0, sizeof(unsigned int) * n_tiles, stream);
-  const uint64_t ctas = std::min<uint64_t>((n_items + kThreads / 32 - 1) / (kThreads / 32), static_cast<uint64_t>(per_sm) * sm_count);
-  ObservationStatsKernel<<<static_cast<uint32_t>(ctas), kThreads, 0, stream>>>(a);
+  ObservationStatsKernel<<<ctas, kThreads, 0, stream>>>(a);
 }
 
 uint32_t CompactScratchWords(uint32_t n) { return (n + kScanBlock - 1) / kScanBlock + 2; }

@@ -18,8 +18,8 @@
 
 #include <math_constants.h>
 
-#include "device_math.cuh"
 #include "host_math.hpp"
+#include "persistent.cuh"
 
 namespace bba {
 namespace odom {
@@ -355,33 +355,13 @@ __device__ __forceinline__ float DepthCostScaled(float r, float s) { return Tuke
 __device__ __forceinline__ float DescWeightScaled(float r, float s) { return s * kDescWeight * HuberWeight(r, kDescHuber); }
 __device__ __forceinline__ float DescCostScaled(float r, float s) { return s * kDescWeight * HuberResidual(r, kDescHuber); }
 
-// H += w J^T J (upper triangle, row-major), b += w r J   (gauss_newton.cuh:59-92, per thread)
-__device__ __forceinline__ void AccumulateHb(float (&acc)[32], const float (&J)[6], float raw, float w) {
-  int idx = 0;
-#pragma unroll
-  for (int r = 0; r < 6; ++r) {
-    const float wj = w * J[r];
-#pragma unroll
-    for (int c = r; c < 6; ++c) acc[idx++] += wj * J[c];
-  }
-  const float wr = w * raw;
-#pragma unroll
-  for (int i = 0; i < 6; ++i) acc[21 + i] += wr * J[i];
-}
-
-__device__ __forceinline__ unsigned int LoadAcquireU32(const unsigned int* p) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-
 // Grid-wide barrier of a persistent kernel whose CTAs are all resident (one per SM).  bar[0] = arrival count, bar[1] = generation.
 // A CTA that waits longer than ~2^22 polls (seconds; a pass takes microseconds) gives up and raises *timeout: the launch is
 // cooperative, so this can only happen after a device fault elsewhere -- the kernel must still terminate.
 __device__ __forceinline__ void GridBarrier(unsigned int* bar, unsigned int* timeout) {
   __syncthreads();
   if (threadIdx.x == 0) {
-    const unsigned int gen = LoadAcquireU32(bar + 1);
+    const unsigned int gen = LoadAcquire(bar + 1);
     __threadfence();
     if (atomicAdd(bar, 1u) == gridDim.x - 1) {
       bar[0] = 0u;
@@ -389,7 +369,7 @@ __device__ __forceinline__ void GridBarrier(unsigned int* bar, unsigned int* tim
       atomicAdd(bar + 1, 1u);
     } else {
       unsigned int polls = 0;
-      while (LoadAcquireU32(bar + 1) == gen) {
+      while (LoadAcquire(bar + 1) == gen) {
         __nanosleep(64);
         if (++polls > (1u << 22)) {
           *timeout = 1u;
