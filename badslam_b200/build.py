@@ -33,7 +33,7 @@ UNITS = [
     ("multi_gpu.cu", []),
     ("frames.cu", []),
 ]
-HEADERS = ["device_math.cuh", "kernels.cuh", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", os.path.join("..", "..", "include", "badba.h")]
+HEADERS = ["device_math.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", os.path.join("..", "..", "include", "badba.h")]
 
 
 def _newer(src, dst):

@@ -223,9 +223,8 @@ bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t colo
     const cudaChannelFormatDesc desc = cudaCreateChannelDesc(8, 0, 0, 0, cudaChannelFormatKindUnsigned);
     BBA_CUDA(h, cudaMallocArray(&luma->array.r, &desc, cw, ch, cudaArrayTextureGather));
   }
-  LaunchExtractLuma(device_rgba, color_pitch, plane.get(), plane.pitch(), cw, ch, s);
-  ++(front_end ? h->front_end_launches : h->launches);
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, front_end ? h->front_end_launches : h->launches, LaunchExtractLuma, device_rgba, color_pitch, plane.get(), plane.pitch(),
+             cw, ch, s);
   BBA_CUDA(h, cudaMemcpy2DToArrayAsync(luma->array, 0, 0, plane.get(), plane.pitch(), cw, ch, cudaMemcpyDeviceToDevice, s));
   BBA_CUDA(h, cudaEventRecord(staging.free, s));
   if (!luma->tex) {
@@ -315,6 +314,7 @@ bba_status bba_create(const bba_config* cfg, bba_handle* out) {
   cudaDeviceProp prop;
   CREATE_TRY(cudaGetDeviceProperties(&prop, cfg->device));
   h->sm_count = prop.multiProcessorCount;
+  CREATE_TRY(bba::SetPoseAccumulateSmemLimits());
   const size_t K = static_cast<size_t>(cfg->max_keyframes);
   auto& p = h->pose;
   CREATE_TRY(h->d_cfactor.Reserve(static_cast<size_t>(h->cf_w) * h->cf_h));

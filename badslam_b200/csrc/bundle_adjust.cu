@@ -110,20 +110,14 @@ bba_status OptimizeIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cuda
   a.cell_b2 = cell_b2;
   a.cell_obs = cell_obs;
   a.cell_count = P;
-  bba::LaunchIntrinsicsAccumulate(a, h->sm_count, opt_color, opt_depth, s);   // :84-108, one launch for all keyframes
-  ++h->launches;
+  BBA_LAUNCH(h, h->launches, LaunchIntrinsicsAccumulate, a, h->sm_count, opt_color, opt_depth, s);   // :84-108, one launch for all keyframes
   if (h->cfg.world_size > 1) {
     // every rank accumulated its surfel shard: one sum all-reduce over [34 global sums | B | D | b2 | obs]
-    bba::LaunchIntrinsicsConvertSums(h->geo.d_intr_sums, h->geo.d_intr, true, s);
+    BBA_LAUNCH(h, h->launches, LaunchIntrinsicsConvertSums, h->geo.d_intr_sums, h->geo.d_intr, true, s);
     h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->geo.d_intr, 64 + static_cast<size_t>(8) * P, s);
-    bba::LaunchIntrinsicsConvertSums(h->geo.d_intr_sums, h->geo.d_intr, false, s);
-    h->launches += 2;
+    BBA_LAUNCH(h, h->launches, LaunchIntrinsicsConvertSums, h->geo.d_intr_sums, h->geo.d_intr, false, s);
   }
-  if (opt_depth) {
-    bba::LaunchIntrinsicsSchur(P, cell_B, cell_D, cell_b2, h->geo.d_intr_sums, s);   // :120-127
-    ++h->launches;
-  }
-  BBA_CUDA(h, cudaGetLastError());
+  if (opt_depth) BBA_LAUNCH(h, h->launches, LaunchIntrinsicsSchur, P, cell_B, cell_D, cell_b2, h->geo.d_intr_sums, s);   // :120-127
   BBA_CUDA(h, cudaMemcpyAsync(h->geo.h_intr_sums, h->geo.d_intr_sums, sizeof(double) * bba::kIntrinsicsSums, cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));   // :136
 
@@ -145,9 +139,7 @@ bba_status OptimizeIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cuda
     const float new_cy = -(new_fy * (c.cy_inv - x1f[3])) + 0.5f;
     for (int i = 0; i < 5; ++i) h->geo.h_intr_x1[i] = x1f[i];
     BBA_CUDA(h, cudaMemcpyAsync(d_x1, h->geo.h_intr_x1, sizeof(float) * 5, cudaMemcpyHostToDevice, s));   // :196
-    bba::LaunchIntrinsicsCellUpdate(P, cell_obs, cell_B, cell_D, d_x1, h->d_cfactor, s);             // :205-212
-    ++h->launches;
-    BBA_CUDA(h, cudaGetLastError());
+    BBA_LAUNCH(h, h->launches, LaunchIntrinsicsCellUpdate, P, cell_obs, cell_B, cell_D, d_x1, h->d_cfactor, s);   // :205-212
     BBA_CUDA(h, cudaStreamSynchronize(s));   // h_intr_x1 is reused by the next call
     h->depth_K[0] = new_fx; h->depth_K[1] = new_fy; h->depth_K[2] = new_cx; h->depth_K[3] = new_cy;
     h->depth_a -= x1f[4];
@@ -245,11 +237,9 @@ bba_status CreateSurfelsForKeyframe(bba_handle h, int k, bool filter, cudaStream
   }
   BBA_TRACE("create: covis uploaded");
   const uint32_t pixels = static_cast<uint32_t>(h->cfg.depth_width) * h->cfg.depth_height;
-  bba::LaunchSupportSurfels(a, h->sm_count, s);     // DetermineSupportingSurfelsCUDA: is the cell supported at all
-  bba::LaunchSeedNewSurfels(a, filter, s);
-  bba::LaunchExclusiveScan(h->life.d_flags, pixels, h->life.d_scan_out, h->life.d_scan_sums, s);
-  h->launches += 6 + (filter ? 1 : 0);
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchSupportSurfels, a, h->sm_count, s);   // DetermineSupportingSurfelsCUDA: is the cell supported at all
+  BBA_LAUNCH(h, h->launches, LaunchSeedNewSurfels, a, filter, s);
+  BBA_LAUNCH(h, h->launches, LaunchExclusiveScan, h->life.d_flags, pixels, h->life.d_scan_out, h->life.d_scan_sums, s);
   const uint32_t n_blocks = (pixels + 4095) / 4096;
   BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_scan_sums + n_blocks, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_create_surfels.cu:466-474
@@ -262,9 +252,7 @@ bba_status CreateSurfelsForKeyframe(bba_handle h, int k, bool filter, cudaStream
     SetError(h, "maximum surfel count exceeded: no surfels created for this keyframe");
     return BBA_OK;
   }
-  bba::LaunchCreateSurfels(a, h->life.d_scan_out, s);
-  ++h->launches;
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchCreateSurfels, a, h->life.d_scan_out, s);
   BBA_TRACE("create: appended");
   h->surfels_size += created;
   *new_count = created;
@@ -279,9 +267,7 @@ bba_status MergeSurfelsForKeyframe(bba_handle h, int k, cudaStream_t s, uint32_t
   bba::LifecycleArgs a;
   if (bba_status st = MakeLifecycleArgs(h, k, &a, s)) return st;
   BBA_CUDA(h, cudaMemsetAsync(h->life.d_deleted_count, 0, sizeof(unsigned int), s));
-  bba::LaunchMergeSurfels(a, h->sm_count, s);
-  h->launches += 5;
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchMergeSurfels, a, h->sm_count, s);
   BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_supporting_surfels.cc:93-96
   *deleted = *h->life.h_deleted_count;
@@ -294,10 +280,8 @@ bba_status CompactSurfels(bba_handle h, uint32_t free_count, bool with_active, c
   h->xchg.replicated_pass_pending = true;
   BBA_CUDA(h, h->life.d_compact_sums.Reserve(bba::CompactScratchWords(N),
                                               bba::CompactScratchWords(std::max(h->cfg.max_surfel_count, N))));
-  bba::LaunchCompactSurfels(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N, free_count, h->life.d_compact_sums,
-                            with_active ? h->active : nullptr, s);
-  h->launches += 4;
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchCompactSurfels, h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N, free_count,
+             h->life.d_compact_sums, with_active ? h->active : nullptr, s);
   h->surfels_size = N - free_count;
   return BBA_OK;
 }
@@ -359,11 +343,7 @@ bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, 
     if (bba_status st = CheckCollective(h)) return st;
     if (bba_status st = PeerFence(h, s)) return st;   // (e.g. the merges above rewrote whole replicas)
   }
-  if (K > 0) {
-    bba::LaunchObservationStats(a, h->sm_count, s);
-    ++h->launches;
-    BBA_CUDA(h, cudaGetLastError());
-  }
+  if (K > 0) BBA_LAUNCH(h, h->launches, LaunchObservationStats, a, h->sm_count, s);
   // (with no keyframe at all the reference still runs MarkDeletedSurfels on zero counts; not reachable through this API,
   // a BA call without keyframes has nothing to optimise)
   uint32_t deleted_total = 0;
@@ -373,10 +353,10 @@ bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, 
       ShardSurfels(N, rank, world, nullptr, &shard_len);
       if (bba_status st = ReserveExchange(h, static_cast<size_t>(world) * 2 * shard_len)) return st;
       const size_t slice_floats = static_cast<size_t>(2) * shard_len;
-      bba::LaunchPackStatsShard(h->surfels, a.pitch, N, rank, world, shard_len, h->xchg.d_exchange + slice_floats * rank, s);
+      BBA_LAUNCH(h, h->launches, LaunchPackStatsShard, h->surfels, a.pitch, N, rank, world, shard_len,
+                 h->xchg.d_exchange + slice_floats * rank, s);
       h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLGATHER, h->xchg.d_exchange, slice_floats * sizeof(float), s);
-      bba::LaunchUnpackStatsShards(h->surfels, a.pitch, N, shard_len, world, rank, h->xchg.d_exchange, s);
-      h->launches += 2;
+      BBA_LAUNCH(h, h->launches, LaunchUnpackStatsShards, h->surfels, a.pitch, N, shard_len, world, rank, h->xchg.d_exchange, s);
     }
     // deleted count of this shard as two exactly representable floats (low 12 bits, the rest), summed over the ranks
     BBA_CUDA(h, h->xchg.d_count_xchg.Reserve(2));
@@ -513,27 +493,25 @@ bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int 
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_vec[0], 0, sizeof(float) * U, s));
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_vec[1], 0, sizeof(float) * U, s));
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars, 0, sizeof(double) * 4, s));
-  bba::LaunchPcgAccumulate(a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
+  BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
   if (h->cfg.world_size > 1) {
     h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[0], U, s);
     h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[1], U, s);
     h->xchg.replicated_pass_pending = false;
   }
-  bba::LaunchPcgInit2(U, L.a_index, h->depth_a, a.kf_count, h->pcg.d_vec[0], h->pcg.d_vec[1], h->pcg.d_vec[2], h->pcg.d_vec[3], h->pcg.d_vec[4],
-                      h->pcg.d_scalars, an, h->sm_count, s);
-  h->launches += 2;
+  BBA_LAUNCH(h, h->launches, LaunchPcgInit2, U, L.a_index, h->depth_a, a.kf_count, h->pcg.d_vec[0], h->pcg.d_vec[1], h->pcg.d_vec[2],
+             h->pcg.d_vec[3], h->pcg.d_vec[4], h->pcg.d_scalars, an, h->sm_count, s);
   return BBA_OK;
 }
 
 // Inner step, first half: g += J^T W J p and alpha_d += p^T J^T W J p over every keyframe (PCGStep1CUDA, :392-419).
 bba_status PcgStep1(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, cudaStream_t s) {
-  bba::LaunchPcgAccumulate(a, h->sm_count, false, s);
+  BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, false, s);
   if (h->cfg.world_size > 1) {   // g and this rank's part of alpha_d: one all-reduce
     float* g = h->pcg.d_vec[3];
-    bba::LaunchPcgPackAlphaD(h->pcg.d_scalars, g + L.unknown_count, s);
+    BBA_LAUNCH(h, h->launches, LaunchPcgPackAlphaD, h->pcg.d_scalars, g + L.unknown_count, s);
     h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, g, static_cast<size_t>(L.unknown_count) + 2, s);
-    bba::LaunchPcgUnpackAlphaD(h->pcg.d_scalars, g + L.unknown_count, s);
-    h->launches += 2;
+    BBA_LAUNCH(h, h->launches, LaunchPcgUnpackAlphaD, h->pcg.d_scalars, g + L.unknown_count, s);
   }
   return BBA_OK;
 }
@@ -541,19 +519,16 @@ bba_status PcgStep1(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, cud
 // Inner step, second half: delta += alpha p, r -= alpha A p, z = M^-1 r (into g), beta_n = z^T r into slot `bn` (:421-437).
 bba_status PcgStep2(bba_handle h, const PcgLayout& L, int an, int bn, cudaStream_t s) {
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars + bn, 0, sizeof(double), s));
-  bba::LaunchPcgStep2(L.unknown_count, L.a_index, h->pcg.d_vec[0], h->pcg.d_vec[1], h->pcg.d_vec[2], h->pcg.d_vec[3], h->pcg.d_vec[4], h->pcg.d_scalars,
-                      an, bn, h->sm_count, s);
-  h->launches += 2;
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchPcgStep2, L.unknown_count, L.a_index, h->pcg.d_vec[0], h->pcg.d_vec[1], h->pcg.d_vec[2], h->pcg.d_vec[3],
+             h->pcg.d_vec[4], h->pcg.d_scalars, an, bn, h->sm_count, s);
   return BBA_OK;
 }
 
 // Before the next inner step: p = z + beta p, g = 0, alpha_d re-armed with its lambda / prior term (:456-464).
 bba_status PcgStep3(bba_handle h, const PcgLayout& L, int an, int bn, cudaStream_t s) {
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars + 1, 0, sizeof(double), s));
-  bba::LaunchPcgStep3(L.unknown_count, L.a_index, static_cast<int>(h->keyframes.size()), h->pcg.d_vec[3], h->pcg.d_vec[4], h->pcg.d_scalars,
-                      an, bn, h->sm_count, s);
-  ++h->launches;
+  BBA_LAUNCH(h, h->launches, LaunchPcgStep3, L.unknown_count, L.a_index, static_cast<int>(h->keyframes.size()), h->pcg.d_vec[3],
+             h->pcg.d_vec[4], h->pcg.d_scalars, an, bn, h->sm_count, s);
   return BBA_OK;
 }
 
@@ -575,16 +550,11 @@ bba_status PcgApplyDelta(bba_handle h, const PcgLayout& L, int gauge, cudaStream
   float* h_ci = h->pcg.h_delta + n_host;
   if (L.opt_color_intr) BBA_CUDA(h, cudaMemcpyAsync(h_ci, pcg_delta + L.color_start, sizeof(float) * 4, cudaMemcpyDeviceToHost, s));
   if (L.opt_geometry && N > 0) {
-    bba::LaunchPcgUpdateSurfels(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N, L.use_desc, L.surfel_start,
-                                pcg_delta, s);
-    ++h->launches;
+    BBA_LAUNCH(h, h->launches, LaunchPcgUpdateSurfels, h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N,
+               L.use_desc, L.surfel_start, pcg_delta, s);
     h->xchg.replicated_pass_pending = true;   // every rank rewrites its whole replica (PeerFence)
   }
-  if (L.opt_depth_intr) {
-    bba::LaunchPcgUpdateCfactor(h->d_cfactor, P, pcg_delta + L.depth_start + 5, s);
-    ++h->launches;
-  }
-  BBA_CUDA(h, cudaGetLastError());
+  if (L.opt_depth_intr) BBA_LAUNCH(h, h->launches, LaunchPcgUpdateCfactor, h->d_cfactor, P, pcg_delta + L.depth_start + 5, s);
   BBA_CUDA(h, cudaStreamSynchronize(s));
   if (L.opt_poses) {
     for (int k = 0; k < K; ++k) {
@@ -668,7 +638,7 @@ bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result*
     if (opt_geometry && N > 0) {   // UpdateSurfelNormalsCUDA, :215-227
       bba::GeometryArgs g;
       if (bba_status st = BuildGeometryArgs(h, &g, s, GeoOrder::kCaller)) return st;
-      h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
+      BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g, h->sm_count, false, true, s);
       if (bba_status st = ExchangeGeometry(h, s)) return st;   // multi-GPU: every replica gets the other shards' normals
     }
     BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
@@ -753,8 +723,7 @@ bba_status bba_update_surfel_activation(bba_handle h, void* stream) {
   bba::GeometryArgs g;
   if (bba_status st = BuildGeometryArgs(h, &g, s, GeoOrder::kSpatial)) return st;
   if (bba_status st = CheckCollective(h)) return st;
-  h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, true, false, s);
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g, h->sm_count, true, false, s);
   if (bba_status st = ExchangeGeometry(h, s)) return st;
   return MarkStaging(h, s);
 }
@@ -768,9 +737,8 @@ bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream) {
   bba::GeometryArgs g;
   if (bba_status st = BuildGeometryArgs(h, &g, s, GeoOrder::kSpatial)) return st;
   if (bba_status st = CheckCollective(h)) return st;
-  h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
-  h->launches += bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g, h->sm_count, false, true, s);
+  BBA_LAUNCH(h, h->launches, LaunchPositionAndDescriptor, g, h->sm_count, s);
   if (bba_status st = ExchangeGeometry(h, s)) return st;
   return MarkStaging(h, s);
 }
@@ -865,19 +833,16 @@ bba_status BundleAdjust(bba_handle h, const bba_ba_options* o, bba_ba_result* re
         bba::GeometryArgs g_old = g, g_new = g;   // (begin / end are LOCAL indices of this rank's shard)
         g_old.end = LocalCountBelow(old_surfels_size, h->cfg.rank, h->cfg.world_size);
         g_new.begin = g_old.end;
-        h->launches += bba::LaunchActivationAndNormals(g_old, h->sm_count, true, true, s);
-        h->launches += bba::LaunchActivationAndNormals(g_new, h->sm_count, false, true, s);
+        BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g_old, h->sm_count, true, true, s);
+        BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g_new, h->sm_count, false, true, s);
       } else if (whole_window) {
-        h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, true, o->optimize_geometry != 0, s);
+        BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g, h->sm_count, true, o->optimize_geometry != 0, s);
       } else if (o->optimize_geometry) {
-        h->launches += bba::LaunchActivationAndNormals(g, h->sm_count, false, true, s);
+        BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g, h->sm_count, false, true, s);
       }
     }
     BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
-    if (o->optimize_geometry && h->surfels_size > 0) {
-      h->launches += bba::LaunchPositionAndDescriptor(g, h->sm_count, s);
-    }
-    BBA_CUDA(h, cudaGetLastError());
+    if (o->optimize_geometry && h->surfels_size > 0) BBA_LAUNCH(h, h->launches, LaunchPositionAndDescriptor, g, h->sm_count, s);
     if (bba_status st = ExchangeGeometry(h, s)) return st;   // multi-GPU: all-gather of the updated surfel shards
     BBA_CUDA(h, cudaEventRecord(h->ev[2], s));
     if (bba_status st = MarkStaging(h, s)) return st;
@@ -1053,7 +1018,6 @@ bba_status bba_pcg_debug(bba_handle h, const bba_ba_options* o, int step, int ap
     if (bba_status st = PcgStep2(h, L, an, bn, s)) return st;
     if (bba_status st = PcgStep3(h, L, an, bn, s)) return st;
   }
-  BBA_CUDA(h, cudaGetLastError());
   float *r = h->pcg.d_vec[0], *M = h->pcg.d_vec[1], *delta = h->pcg.d_vec[2], *g = h->pcg.d_vec[3], *p = h->pcg.d_vec[4];
   bba_status st = BBA_OK;
   if ((st = copy(out->r, r)) || (st = copy(out->M, M)) || (st = copy(out->p, p)) || (st = copy(out->g, g)) || (st = copy(out->delta, delta)) ||

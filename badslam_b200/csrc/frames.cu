@@ -105,8 +105,7 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
   for (int f = 0; f < 2; ++f) { br.out[f] = st.gradmag[f].get(); br.out_pitch[f] = static_cast<uint32_t>(st.gradmag[f].pitch()); }
   br.w = h->cfg.color_width; br.h = h->cfg.color_height;
   br.use_gradmag = o.use_gradmag;
-  od::LaunchBrightness(br, s);
-  ++h->front_end_launches;
+  BBA_LAUNCH(h, h->front_end_launches, od::LaunchBrightness, br, s);
 
   // level images as seen by the kernels: level 0 normals are the keyframe's / the frame's own buffers
   od::Image img[2][od::kMaxScales];
@@ -131,8 +130,7 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
   l0.cw = cam.cw; l0.ch = cam.ch;
   l0.a = cam.a; l0.raw_to_float = cam.raw_to_float; l0.cfactor = cam.cfactor; l0.cf_w = cam.cf_w; l0.cell = cam.cell;
   l0.downsample_color = h->cfg.depth_width == h->cfg.color_width;
-  od::LaunchLevel0(l0, s);
-  ++h->front_end_launches;
+  BBA_LAUNCH(h, h->front_end_launches, od::LaunchLevel0, l0, s);
 
   for (int l = 1; l < S; ++l) {
     // pairwise_frame_tracking.cc:325-347: the tracked image from level 2 on (level 1 too when level 0 is in use), the base always
@@ -145,8 +143,7 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
     }
     d.w = st.w[l]; d.h = st.h[l];
     d.in_w = st.w[l - 1]; d.in_h = st.h[l - 1];
-    od::LaunchDownsample(d, s);
-    ++h->front_end_launches;
+    BBA_LAUNCH(h, h->front_end_launches, od::LaunchDownsample, d, s);
   }
   for (int l = 0; l < S; ++l) {
     st.level[l].cam = MakeLevelCamera(h, view.cams, l, st.w[l], st.h[l]);
@@ -155,7 +152,6 @@ bba_status BuildOdometryPyramids(bba_handle h, const bba_odometry_options& o, co
   }
   st.last_num_scales = S;
   st.last_first_scale = o.use_pyramid_level_0 ? 0 : 1;
-  BBA_CUDA(h, cudaGetLastError());
   return BBA_OK;
 }
 
@@ -182,9 +178,7 @@ bba_status LaunchOdometryKernel(bba_handle h, const CameraView& cams, int num_sc
   BBA_CUDA(h, cudaMemsetAsync(st.d_acc, 0, sizeof(double) * 96, s));
   BBA_CUDA(h, cudaMemsetAsync(st.d_barrier, 0, sizeof(unsigned int) * 2, s));
   BBA_CUDA(h, cudaMemsetAsync(st.d_result, 0, sizeof(od::TrackResult), s));
-  od::LaunchTrack(a, h->sm_count, s);
-  ++h->front_end_launches;
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->front_end_launches, od::LaunchTrack, a, h->sm_count, s);
   BBA_CUDA(h, cudaMemcpyAsync(st.h_result, st.d_result, sizeof(od::TrackResult), cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));
   if (st.h_result->barrier_timeout) return Fail(h, BBA_ERR_CUDA, "odometry kernel: grid barrier timed out");
@@ -254,11 +248,10 @@ bba_status PreprocessFrame(bba_handle h, const char* fn, const bba_preprocess_op
     f.depth_level = raw_stage->depth_level;
     f.raw_w = raw_stage->raw_w; f.raw_h = raw_stage->raw_h;
     f.color_level = raw_stage->color_level;
-    h->front_end_launches += bba::LaunchPreprocessRawFrame(f, s);
+    BBA_LAUNCH(h, h->front_end_launches, LaunchPreprocessRawFrame, f, s);
   } else {
-    h->front_end_launches += bba::LaunchPreprocessFrame(f, s);
+    BBA_LAUNCH(h, h->front_end_launches, LaunchPreprocessFrame, f, s);
   }
-  BBA_CUDA(h, cudaGetLastError());
   if (bba_status st = view.ReleaseSlot()) return st;
   if (min_depth || max_depth) {   // ComputeMinMaxDepthCUDA returns host values and synchronises (cuda_depth_processing.cu:452-463)
     BBA_CUDA(h, cudaMemcpyAsync(h->pre.h_min_max, h->pre.d_min_max, 2 * sizeof(float), cudaMemcpyDeviceToHost, s));

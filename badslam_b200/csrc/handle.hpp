@@ -363,6 +363,17 @@ void SetError(bba_handle h, const std::string& msg);
       return Fail(h, BBA_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e__));                    \
   } while (0)
 
+// Calls launcher(...), adds the kernels it enqueued to `counter` (h->launches or h->front_end_launches) and fails when the
+// launcher or the runtime's last error reports an error.  Never synchronises: a fault while a kernel runs surfaces later.
+#define BBA_LAUNCH(h, counter, launcher, ...)                                                                \
+  do {                                                                                                      \
+    const ::bba::LaunchResult r__ = launcher(__VA_ARGS__);                                                  \
+    (counter) += r__.kernels;                                                                               \
+    const cudaError_t last__ = cudaGetLastError();                                                          \
+    const cudaError_t e__ = r__.error != cudaSuccess ? r__.error : last__;                                  \
+    if (e__ != cudaSuccess) return Fail(h, BBA_ERR_CUDA, std::string(#launcher) + ": " + cudaGetErrorString(e__)); \
+  } while (0)
+
 // BADBA_TRACE=1: stage markers on stderr (debugging aid for host-side faults)
 #define BBA_TRACE(msg)                                                                   \
   do {                                                                                   \

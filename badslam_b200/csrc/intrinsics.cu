@@ -205,20 +205,23 @@ __global__ void __launch_bounds__(256) IntrinsicsCellUpdateKernel(uint32_t cell_
   cfactor[p] = cf;
 }
 
-void LaunchIntrinsicsAccumulate(const IntrinsicsArgs& a, int sm_count, bool optimize_color, bool optimize_depth, cudaStream_t stream) {
-  if (a.end <= a.begin || a.kf_count <= 0) return;
-  cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream);
+LaunchResult LaunchIntrinsicsAccumulate(const IntrinsicsArgs& a, int sm_count, bool optimize_color, bool optimize_depth,
+                                        cudaStream_t stream) {
+  if (a.end <= a.begin || a.kf_count <= 0) return {};
+  LaunchResult r{0, cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream)};
   const uint32_t n_tiles = (a.end - a.begin + kTile - 1) / kTile;
   const uint32_t n_groups = (a.kf_count + kGroup - 1) / kGroup;
   const uint64_t n_items = static_cast<uint64_t>(n_tiles) * n_groups;
   auto launch = [&](auto kernel) {
     int per_sm = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, 0);
+    r += cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, 0);
     kernel<<<ItemGrid(per_sm, sm_count, n_items), kThreads, 0, stream>>>(a);
+    r.kernels = 1;
   };
   if (optimize_color && optimize_depth) launch(IntrinsicsAccumulateKernel<true, true>);
   else if (optimize_color) launch(IntrinsicsAccumulateKernel<true, false>);
   else if (optimize_depth) launch(IntrinsicsAccumulateKernel<false, true>);
+  return r;
 }
 
 __global__ void IntrinsicsConvertSumsKernel(double* sums, float* head, int to_float) {
@@ -227,17 +230,20 @@ __global__ void IntrinsicsConvertSumsKernel(double* sums, float* head, int to_fl
   if (to_float) head[i] = static_cast<float>(sums[i]);
   else sums[i] = static_cast<double>(head[i]);
 }
-void LaunchIntrinsicsConvertSums(double* sums, float* head, bool to_float, cudaStream_t stream) {
+LaunchResult LaunchIntrinsicsConvertSums(double* sums, float* head, bool to_float, cudaStream_t stream) {
   IntrinsicsConvertSumsKernel<<<1, 64, 0, stream>>>(sums, head, to_float ? 1 : 0);
+  return {1};
 }
 
-void LaunchIntrinsicsSchur(uint32_t cell_count, float* B, float* D, const float* b2, double* sums, cudaStream_t stream) {
+LaunchResult LaunchIntrinsicsSchur(uint32_t cell_count, float* B, float* D, const float* b2, double* sums, cudaStream_t stream) {
   IntrinsicsSchurKernel<<<1, 1024, 0, stream>>>(cell_count, B, D, b2, sums);
+  return {1};
 }
 
-void LaunchIntrinsicsCellUpdate(uint32_t cell_count, const float* obs, const float* B, const float* D, const float* x1,
-                                float* cfactor, cudaStream_t stream) {
+LaunchResult LaunchIntrinsicsCellUpdate(uint32_t cell_count, const float* obs, const float* B, const float* D, const float* x1,
+                                        float* cfactor, cudaStream_t stream) {
   IntrinsicsCellUpdateKernel<<<(cell_count + 255) / 256, 256, 0, stream>>>(cell_count, obs, B, D, x1, cfactor);
+  return {1};
 }
 
 }  // namespace bba

@@ -517,14 +517,27 @@ __global__ void __launch_bounds__(128) PackWorkRecordsKernel(const KfDevice* __r
   }
 }
 
+static constexpr size_t PoseSmemBytes(int tile, bool pre) {
+  return static_cast<size_t>(2) * (pre ? kPoseStagedRowsPre : kPoseStagedRows) * tile * sizeof(float) + (pre ? kPoseRingBytes : 0);
+}
+
+template <int TILE, bool PRE>
+static cudaError_t SetPoseSmemLimit() {
+  const int smem = static_cast<int>(PoseSmemBytes(TILE, PRE));
+  const cudaError_t e = cudaFuncSetAttribute(PoseAccumulateKernel<TILE, false, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  return e != cudaSuccess ? e : cudaFuncSetAttribute(PoseAccumulateKernel<TILE, true, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+}
+
+cudaError_t SetPoseAccumulateSmemLimits() {
+  for (cudaError_t e : {SetPoseSmemLimit<256, true>(), SetPoseSmemLimit<512, true>(), SetPoseSmemLimit<256, false>(),
+                        SetPoseSmemLimit<512, false>(), SetPoseSmemLimit<1024, false>()})
+    if (e != cudaSuccess) return e;
+  return cudaSuccess;
+}
+
 template <int TILE, bool STATS, bool PRE>
 static void LaunchPoseAccumulateT(const PoseAccumulateArgs& args, int sm_count, cudaStream_t stream) {
-  const size_t smem = static_cast<size_t>(2) * (PRE ? kPoseStagedRowsPre : kPoseStagedRows) * TILE * sizeof(float) + (PRE ? kPoseRingBytes : 0);
-  static bool configured = false;
-  if (!configured) {
-    cudaFuncSetAttribute(PoseAccumulateKernel<TILE, STATS, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    configured = true;
-  }
+  constexpr size_t smem = PoseSmemBytes(TILE, PRE);
   PoseAccumulateKernel<TILE, STATS, PRE><<<kPoseMinCtas * sm_count, PRE ? kPoseWsThreads : kPoseThreads, smem, stream>>>(args);   // persistent
 }
 
@@ -547,11 +560,13 @@ static void LaunchPoseAccumulateS(const PoseAccumulateArgs& args, int sm_count, 
   }
 }
 
-void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream, int variant) {
-  if (args.n == 0) return;
+LaunchResult LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
+                                  int variant) {
+  if (args.n == 0) return {};
   PackWorkRecordsKernel<<<(max_work * 6 + 127) / 128, 128, 0, stream>>>(args.kfs, args.work_list, args.work_count, args.work_records);
   if (with_stats) LaunchPoseAccumulateS<true>(args, sm_count, variant, stream);
   else LaunchPoseAccumulateS<false>(args, sm_count, variant, stream);
+  return {2};
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -879,33 +894,34 @@ __global__ void __launch_bounds__(kGeoThreads, 3) PositionDescriptorKernel(const
 constexpr size_t kGeoSmemBytes = sizeof(KfDevice) * (kGeoThreads / 32) * kGeoGroup;   // the per-warp record slices
 
 template <typename Kernel>
-static int LaunchGeo(Kernel kernel, GeometryArgs a, int sm_count, bool desc_rows, cudaStream_t stream) {
+static LaunchResult LaunchGeo(Kernel kernel, GeometryArgs a, int sm_count, bool desc_rows, cudaStream_t stream) {
   int per_sm = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGeoThreads, kGeoSmemBytes);
+  LaunchResult r{1, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGeoThreads, kGeoSmemBytes)};
   const uint32_t grid =
       EpochOrderedGrid(per_sm, sm_count, kGeoThreads, a.end - a.begin, (a.kf_count + kGeoGroup - 1) / kGeoGroup, &a.tile_shift);
   const uint32_t n_tiles = (a.end - a.begin + (1u << a.tile_shift) - 1) >> a.tile_shift;
-  cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream);
-  cudaMemsetAsync(a.tile_epoch, 0, sizeof(unsigned int) * n_tiles, stream);
-  LaunchGeometryStream(a, desc_rows, stream);
+  r += cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream);
+  r += cudaMemsetAsync(a.tile_epoch, 0, sizeof(unsigned int) * n_tiles, stream);
+  r += LaunchGeometryStream(a, desc_rows, stream);
   kernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
-  return 2;
+  return r;
 }
 
-int LaunchActivationAndNormals(const GeometryArgs& a, int sm_count, bool determine_activation, bool update_normals, cudaStream_t stream) {
-  if (a.end <= a.begin || (!determine_activation && !update_normals)) return 0;
+LaunchResult LaunchActivationAndNormals(const GeometryArgs& a, int sm_count, bool determine_activation, bool update_normals,
+                                        cudaStream_t stream) {
+  if (a.end <= a.begin || (!determine_activation && !update_normals)) return {};
   if (a.kf_count <= 0) {
     // no keyframe to look at: activation clears every flag, normals keep their value
-    if (determine_activation) cudaMemsetAsync(a.active, 0, a.n, stream);   // (every rank clears its whole replica)
-    return 0;
+    if (determine_activation) return {0, cudaMemsetAsync(a.active, 0, a.n, stream)};   // (every rank clears its whole replica)
+    return {};
   }
   if (determine_activation && update_normals) return LaunchGeo(ActivationNormalsKernel<true, true>, a, sm_count, false, stream);
   if (determine_activation) return LaunchGeo(ActivationNormalsKernel<true, false>, a, sm_count, false, stream);
   return LaunchGeo(ActivationNormalsKernel<false, true>, a, sm_count, false, stream);
 }
 
-int LaunchPositionAndDescriptor(const GeometryArgs& a, int sm_count, cudaStream_t stream) {
-  if (a.end <= a.begin || a.kf_count <= 0) return 0;
+LaunchResult LaunchPositionAndDescriptor(const GeometryArgs& a, int sm_count, cudaStream_t stream) {
+  if (a.end <= a.begin || a.kf_count <= 0) return {};
   if (a.cam.use_desc) {
     if (a.cam.use_depth) return LaunchGeo(PositionDescriptorKernel<true, true>, a, sm_count, true, stream);
     return LaunchGeo(PositionDescriptorKernel<false, true>, a, sm_count, true, stream);
@@ -949,17 +965,19 @@ __global__ void __launch_bounds__(256) UnpackShardsKernel(float* __restrict__ su
   active[i] = static_cast<uint8_t>(slice[static_cast<size_t>(kShardRows - 1) * shard_len + c]);
 }
 
-void LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t rank,
-                     uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream) {
-  if (shard_len == 0) return;
+LaunchResult LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t rank,
+                             uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream) {
+  if (shard_len == 0) return {};
   PackShardKernel<<<(shard_len + 255) / 256, 256, 0, stream>>>(surfels, pitch, active, n, perm, rank, world, shard_len, slice);
+  return {1};
 }
 
-void LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t shard_len, int world,
-                        int skip_rank, const float* buffer, cudaStream_t stream) {
-  if (n == 0) return;
+LaunchResult LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t shard_len,
+                                int world, int skip_rank, const float* buffer, cudaStream_t stream) {
+  if (n == 0) return {};
   UnpackShardsKernel<<<(n + 255) / 256, 256, 0, stream>>>(surfels, pitch, active, n, perm, shard_len, static_cast<uint32_t>(world),
                                                           skip_rank, buffer);
+  return {1};
 }
 
 __global__ void PackPoseResultsKernel(const int* __restrict__ ids, int n, const float* __restrict__ pose_est,
@@ -975,10 +993,11 @@ __global__ void PackPoseResultsKernel(const int* __restrict__ ids, int n, const 
   for (int j = 0; j < 8; ++j) o[9 + j] = static_cast<float>(first_stats[kf * 8 + j]);
 }
 
-void LaunchPackPoseResults(const int* ids, int n, const float* pose_est, const int* iterations, const int* converged,
-                           const double* first_stats, float* out, cudaStream_t stream) {
-  if (n <= 0) return;
+LaunchResult LaunchPackPoseResults(const int* ids, int n, const float* pose_est, const int* iterations, const int* converged,
+                                   const double* first_stats, float* out, cudaStream_t stream) {
+  if (n <= 0) return {};
   PackPoseResultsKernel<<<(n + 127) / 128, 128, 0, stream>>>(ids, n, pose_est, iterations, converged, first_stats, out);
+  return {1};
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1000,10 +1019,11 @@ __global__ void __launch_bounds__(256) ExtractLumaKernel(const uint8_t* __restri
   }
 }
 
-void LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream) {
+LaunchResult LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream) {
   dim3 block(256);
   dim3 grid((w / 4 + 255) / 256 + 1, h);
   ExtractLumaKernel<<<grid, block, 0, stream>>>(rgba, rgba_pitch, luma, luma_pitch, w, h);
+  return {1};
 }
 
 }  // namespace bba

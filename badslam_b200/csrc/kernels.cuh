@@ -1,10 +1,12 @@
 // kernels.cuh -- launch interface between the host orchestration (handle.hpp and its host units) and the sm_90a kernels.
+// Every Launch* function returns the kernels it enqueued and the first error of its runtime calls (launch.hpp).
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "device_math.cuh"
+#include "launch.hpp"
 
 namespace bba {
 
@@ -50,26 +52,29 @@ struct SpatialOrderBuffers {
   size_t temp_bytes;
 };
 size_t SpatialOrderTempBytes(uint32_t capacity);
-void LaunchSpatialOrder(const float* surfels, uint32_t pitch, uint32_t n, const SpatialOrderBuffers& b, cudaStream_t stream);
+// Three launches: bounds, keys and the CUB radix sort, whose kernels count as one launch.
+LaunchResult LaunchSpatialOrder(const float* surfels, uint32_t pitch, uint32_t n, const SpatialOrderBuffers& b, cudaStream_t stream);
 // The pose step's surfel stream, in spatial order: stream row r, column s holds, for surfel perm[s], x y z d1 d2 (rows 0-4), the
 // unpacked + re-normalised normal (rows 5-7, util_nvcc_only.cuh:83-95) and the tangent points gp + t1 / gp + t2 (rows 8-10 / 11-13,
 // cost_function.cuh:115-133).  What the descriptor residual needs of a surfel alone is computed once per pose step (the surfels do
 // not move while the keyframe poses are optimised) and the rows the kernel stages come from one buffer.  boxes[c] = min x y z, 0,
 // max x y z, 0 over the finite positions of stream columns [256 c, 256 c + 256).  perm = null: the caller's order.
 constexpr int kPoseStreamRows = 14;
-void LaunchPoseStream(const float* surfels, uint32_t pitch, uint32_t n, const uint32_t* perm, float* stream, uint32_t stream_pitch,
-                      float* boxes, cudaStream_t cuda_stream);
+LaunchResult LaunchPoseStream(const float* surfels, uint32_t pitch, uint32_t n, const uint32_t* perm, float* stream, uint32_t stream_pitch,
+                              float* boxes, cudaStream_t cuda_stream);
 // Instantiations of the pose kernel (surfel tile, PRE = stages the sorted stream); the values are bba_pose_variant's.
 enum PoseVariant { kPoseVariantAuto = 0, kPoseVariant256Pre = 1, kPoseVariant512Pre = 2, kPoseVariant256 = 3, kPoseVariant512 = 4,
                    kPoseVariant1024 = 5 };
 inline bool PoseVariantValid(int v) { return v >= kPoseVariantAuto && v <= kPoseVariant1024; }
 inline bool PoseVariantPre(int v) { return v == kPoseVariant256Pre || v == kPoseVariant512Pre; }
-// max_work: upper bound of *work_count known to the host (sizes the record-packing launch that precedes the kernel).
+// max_work: upper bound of *work_count known to the host (sizes the record-packing launch that precedes the kernel; both count).
 // variant = kPoseVariantAuto: the tile follows from args.n and the SM count, and args.stream != null selects the variant that
 // stages the sorted stream (and skips the chunks whose box lies outside a keyframe's view) instead of the caller's rows.  Any other
 // variant forces that instantiation; a PRE variant needs args.stream and args.boxes, the others ignore them.
-void LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
-                          int variant = kPoseVariantAuto);
+LaunchResult LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
+                                  int variant = kPoseVariantAuto);
+// Sets the dynamic shared-memory limit of every instantiation of the pose kernel on the current device (once per handle).
+cudaError_t SetPoseAccumulateSmemLimits();
 
 struct PoseSolveArgs {
   KfDevice* kfs;
@@ -90,7 +95,7 @@ struct PoseSolveArgs {
   int max_iterations;
 };
 // Device-side Gauss-Newton step for every keyframe in the list (direct_ba_alternating.cc:173-233).
-void LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
+LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
 
 // Replicas of the surfel buffer / active flags on the OTHER ranks of a one-process-per-GPU job, mapped into this process
 // (CUDA IPC) and written directly over NVLink by the geometry kernels: the owner of a surfel stores its updated rows into
@@ -130,13 +135,14 @@ struct GeometryArgs {
 // gather radius^2, d1, d2 (what the position / descriptor kernel reads with descriptors; the other launches read rows 0-3 + flags).
 constexpr int kGeoStreamRows = 8;
 static_assert(kGeoStreamRows <= kPoseStreamRows, "the geometry stream lives in the pose stream's buffer");
-void LaunchGeometryStream(const GeometryArgs& args, bool desc_rows, cudaStream_t stream);
+LaunchResult LaunchGeometryStream(const GeometryArgs& args, bool desc_rows, cudaStream_t stream);
 // SetSurfelInactive + DetermineActiveSurfels (kernel_surfel_activation.cu:38-79) fused with the normal
 // accumulation + update (kernel_opt_geometry.cu:527-597).
-// Both return the number of kernels launched (the stream gather and the kernel, 0 when there is nothing to launch).
-int LaunchActivationAndNormals(const GeometryArgs& args, int sm_count, bool determine_activation, bool update_normals, cudaStream_t stream);
+// Both launch the stream gather and the kernel, or nothing when there is nothing to do.
+LaunchResult LaunchActivationAndNormals(const GeometryArgs& args, int sm_count, bool determine_activation, bool update_normals,
+                                        cudaStream_t stream);
 // Position (+ descriptor) accumulation and per-surfel solve (kernel_opt_geometry.cu:118-231,273-361 or :417-507).
-int LaunchPositionAndDescriptor(const GeometryArgs& args, int sm_count, cudaStream_t stream);
+LaunchResult LaunchPositionAndDescriptor(const GeometryArgs& args, int sm_count, cudaStream_t stream);
 
 // Multi-GPU surfel sharding: 256-surfel granules are dealt round-robin to the ranks (granule g belongs to rank g % world), so
 // that every rank sees the same mix of well- and poorly-observed surfels (surfels are stored in creation order, and the
@@ -148,14 +154,14 @@ __host__ __device__ inline uint32_t SurfelShardToGlobal(uint32_t local, uint32_t
 // Exchange of the shards: 7 rows (x y z normal d1 d2 active-as-float) x shard_len floats per rank, in local index order.  The
 // shards are the geometry step's: granules of stream positions, surfel perm[s] at position s (perm null: the caller's order).
 constexpr int kShardRows = 7;
-void LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t rank,
-                     uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream);
-void LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t shard_len, int world,
-                        int skip_rank, const float* buffer, cudaStream_t stream);
+LaunchResult LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t rank,
+                             uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream);
+LaunchResult LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t shard_len, int world,
+                                int skip_rank, const float* buffer, cudaStream_t stream);
 // Pose results of the locally owned keyframes -> [K][17] floats (zeros elsewhere) for the sum all-reduce.
 constexpr int kPoseSlot = 17;   // 7 pose, iterations, converged, 8 first-iteration statistics
-void LaunchPackPoseResults(const int* ids, int n, const float* pose_est, const int* iterations, const int* converged,
-                           const double* first_stats, float* out, cudaStream_t stream);
+LaunchResult LaunchPackPoseResults(const int* ids, int n, const float* pose_est, const int* iterations, const int* converged,
+                                   const double* first_stats, float* out, cudaStream_t stream);
 
 // Intrinsics + depth-deformation step (intrinsics.cu; OptimizeIntrinsicsCUDA, kernel_opt_intrinsics.cc:39-281).
 constexpr int kIntrinsicsSums = 34;   // A (15) b1 (5) colour H (10) colour b (4), fp64
@@ -177,11 +183,11 @@ struct IntrinsicsArgs {
   float* cell_obs;             // [cell_count] observation count (fp32 so that one sum all-reduce covers everything)
   uint32_t cell_count;
 };
-void LaunchIntrinsicsAccumulate(const IntrinsicsArgs& a, int sm_count, bool optimize_color, bool optimize_depth, cudaStream_t stream);
-void LaunchIntrinsicsSchur(uint32_t cell_count, float* B, float* D, const float* b2, double* sums, cudaStream_t stream);
-void LaunchIntrinsicsConvertSums(double* sums, float* head, bool to_float, cudaStream_t stream);
-void LaunchIntrinsicsCellUpdate(uint32_t cell_count, const float* obs, const float* B, const float* D, const float* x1,
-                                float* cfactor, cudaStream_t stream);
+LaunchResult LaunchIntrinsicsAccumulate(const IntrinsicsArgs& a, int sm_count, bool optimize_color, bool optimize_depth, cudaStream_t stream);
+LaunchResult LaunchIntrinsicsSchur(uint32_t cell_count, float* B, float* D, const float* b2, double* sums, cudaStream_t stream);
+LaunchResult LaunchIntrinsicsConvertSums(double* sums, float* head, bool to_float, cudaStream_t stream);
+LaunchResult LaunchIntrinsicsCellUpdate(uint32_t cell_count, const float* obs, const float* B, const float* D, const float* x1,
+                                        float* cfactor, cudaStream_t stream);
 
 // PCG Gauss-Newton step over all unknowns (pcg.cu; BundleAdjustmentPCG, direct_ba_pcg.cc:43-819).
 struct PcgArgs {
@@ -208,18 +214,18 @@ struct PcgArgs {
 // Layout of the fp64 scalar block: [0] / [2] alpha_n, beta_n (swapping roles), [1] alpha_d, [3] this rank's part of alpha_d
 // (multi-GPU), then the workspace of the fixed-order grid sums of the vector kernels.
 constexpr int kPcgPartialsA = 8, kPcgPartialsB = 8 + 2048, kPcgCounters = 8 + 4096, kPcgScalarDoubles = 8 + 4096 + 2;
-void LaunchPcgAccumulate(const PcgArgs& a, int sm_count, bool init, cudaStream_t stream);
-void LaunchPcgPackAlphaD(const double* scalars, float* tail, cudaStream_t stream);
-void LaunchPcgUnpackAlphaD(double* scalars, const float* tail, cudaStream_t stream);
-void LaunchPcgInit2(uint32_t n, uint32_t a_index, float a, int kf_count, const float* r, const float* M, float* delta, float* g, float* p,
-                    double* scalars, int slot_alpha_n, int sm_count, cudaStream_t stream);
-void LaunchPcgStep2(uint32_t n, uint32_t a_index, float* r, const float* M, float* delta, float* g, const float* p, double* scalars,
-                    int slot_alpha_n, int slot_beta_n, int sm_count, cudaStream_t stream);
-void LaunchPcgStep3(uint32_t n, uint32_t a_index, int kf_count, float* g, float* p, double* scalars, int slot_alpha_n, int slot_beta_n,
-                    int sm_count, cudaStream_t stream);
-void LaunchPcgUpdateSurfels(float* surfels, uint32_t pitch, uint32_t n, bool use_desc, uint32_t surfel_start, const float* delta,
-                            cudaStream_t stream);
-void LaunchPcgUpdateCfactor(float* cfactor, uint32_t cells, const float* delta, cudaStream_t stream);
+LaunchResult LaunchPcgAccumulate(const PcgArgs& a, int sm_count, bool init, cudaStream_t stream);
+LaunchResult LaunchPcgPackAlphaD(const double* scalars, float* tail, cudaStream_t stream);
+LaunchResult LaunchPcgUnpackAlphaD(double* scalars, const float* tail, cudaStream_t stream);
+LaunchResult LaunchPcgInit2(uint32_t n, uint32_t a_index, float a, int kf_count, const float* r, const float* M, float* delta, float* g, float* p,
+                            double* scalars, int slot_alpha_n, int sm_count, cudaStream_t stream);
+LaunchResult LaunchPcgStep2(uint32_t n, uint32_t a_index, float* r, const float* M, float* delta, float* g, const float* p, double* scalars,
+                            int slot_alpha_n, int slot_beta_n, int sm_count, cudaStream_t stream);
+LaunchResult LaunchPcgStep3(uint32_t n, uint32_t a_index, int kf_count, float* g, float* p, double* scalars, int slot_alpha_n, int slot_beta_n,
+                            int sm_count, cudaStream_t stream);
+LaunchResult LaunchPcgUpdateSurfels(float* surfels, uint32_t pitch, uint32_t n, bool use_desc, uint32_t surfel_start, const float* delta,
+                                    cudaStream_t stream);
+LaunchResult LaunchPcgUpdateCfactor(float* cfactor, uint32_t cells, const float* delta, cudaStream_t stream);
 
 // End-of-BA surfel maintenance (lifecycle.cu; PerformBASchemeEndTasks, direct_ba.cc:566-653).
 struct KfRadius {
@@ -245,17 +251,17 @@ struct SurfelStatsArgs {
   uint32_t local_count, shard_rank, shard_world;
   PeerSet peers;
 };
-void LaunchObservationStats(SurfelStatsArgs a, int sm_count, cudaStream_t stream);
+LaunchResult LaunchObservationStats(SurfelStatsArgs a, int sm_count, cudaStream_t stream);
 // Exchange of the end tasks' two result rows through the host collective (no mapped peers): slice = [2][shard_len] floats.
-void LaunchPackStatsShard(const float* surfels, uint32_t pitch, uint32_t n, uint32_t rank, uint32_t world, uint32_t shard_len, float* slice,
-                          cudaStream_t stream);
-void LaunchUnpackStatsShards(float* surfels, uint32_t pitch, uint32_t n, uint32_t shard_len, int world, int skip_rank, const float* buffer,
-                             cudaStream_t stream);
+LaunchResult LaunchPackStatsShard(const float* surfels, uint32_t pitch, uint32_t n, uint32_t rank, uint32_t world, uint32_t shard_len, float* slice,
+                                  cudaStream_t stream);
+LaunchResult LaunchUnpackStatsShards(float* surfels, uint32_t pitch, uint32_t n, uint32_t shard_len, int world, int skip_rank, const float* buffer,
+                                     cudaStream_t stream);
 uint32_t CompactScratchWords(uint32_t n);   // size of block_sums for LaunchCompactSurfels
 // Moves surviving surfels from the tail into the free spots; afterwards the first n - free_count slots are the surfels.
 // active != nullptr: the active flags move with them (CompactSurfelsCUDA's adapt_active_surfels).
-void LaunchCompactSurfels(float* surfels, uint32_t pitch, uint32_t n, uint32_t free_count, unsigned int* block_sums, uint8_t* active,
-                          cudaStream_t stream);
+LaunchResult LaunchCompactSurfels(float* surfels, uint32_t pitch, uint32_t n, uint32_t free_count, unsigned int* block_sums, uint8_t* active,
+                                  cudaStream_t stream);
 
 // In-loop surfel lifecycle for ONE keyframe (CreateSurfelsForKeyframe / DetermineSupportingSurfelsAndMergeSurfels).
 struct CovisEntry {              // one co-visible keyframe of the keyframe new surfels are created for
@@ -288,14 +294,14 @@ struct LifecycleArgs {
   float cell_merge_dist_squared;
   unsigned int* counter;         // device scalar (deleted surfels)
 };
-void LaunchSupportSurfels(const LifecycleArgs& a, int sm_count, cudaStream_t stream);   // sup[0] only (occupancy for the creation)
-void LaunchMergeSurfels(const LifecycleArgs& a, int sm_count, cudaStream_t stream);     // supports + merge, += *counter
-void LaunchSeedNewSurfels(const LifecycleArgs& a, bool filter, cudaStream_t stream);    // a.flags after LaunchSupportSurfels
+LaunchResult LaunchSupportSurfels(const LifecycleArgs& a, int sm_count, cudaStream_t stream);   // sup[0] only (occupancy for the creation)
+LaunchResult LaunchMergeSurfels(const LifecycleArgs& a, int sm_count, cudaStream_t stream);     // supports + merge, += *counter
+LaunchResult LaunchSeedNewSurfels(const LifecycleArgs& a, bool filter, cudaStream_t stream);    // a.flags after LaunchSupportSurfels
 uint32_t ScanScratchWords(uint32_t n);
-void LaunchExclusiveScan(const unsigned int* in, uint32_t n, unsigned int* out, unsigned int* block_sums, cudaStream_t stream);
-void LaunchCreateSurfels(const LifecycleArgs& a, const unsigned int* index, cudaStream_t stream);
+LaunchResult LaunchExclusiveScan(const unsigned int* in, uint32_t n, unsigned int* out, unsigned int* block_sums, cudaStream_t stream);
+LaunchResult LaunchCreateSurfels(const LifecycleArgs& a, const unsigned int* index, cudaStream_t stream);
 
 // uchar4 (.w = luma) -> u8 plane.
-void LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream);
+LaunchResult LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream);
 
 }  // namespace bba

@@ -117,11 +117,11 @@ bba_status ExchangeGeometry(bba_handle h, cudaStream_t s) {
   if (bba_status st = ReserveExchange(h, static_cast<size_t>(world) * kShardRows * shard_len)) return st;
   const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
   const size_t slice_floats = static_cast<size_t>(kShardRows) * shard_len;
-  LaunchPackShard(h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, rank, world, shard_len, x.d_exchange + slice_floats * rank, s);
+  BBA_LAUNCH(h, h->launches, LaunchPackShard, h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, rank, world, shard_len,
+             x.d_exchange + slice_floats * rank, s);
   x.collective(x.collective_user, BBA_COLLECTIVE_ALLGATHER, x.d_exchange, slice_floats * sizeof(float), s);
-  LaunchUnpackShards(h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, shard_len, world, rank, x.d_exchange, s);
-  h->launches += 2;
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchUnpackShards, h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, shard_len, world, rank,
+             x.d_exchange, s);
   return BBA_OK;
 }
 

@@ -53,9 +53,10 @@ __global__ void __launch_bounds__(256) BrightnessKernel(const __grid_constant__ 
   a.out[f][static_cast<size_t>(y) * a.out_pitch[f] + x] = v;
 }
 
-void LaunchBrightness(const BrightnessArgs& a, cudaStream_t stream) {
+LaunchResult LaunchBrightness(const BrightnessArgs& a, cudaStream_t stream) {
   dim3 grid((a.w + 31) / 32, (a.h + 7) / 8, 2);
   BrightnessKernel<<<grid, 256, 0, stream>>>(a);
+  return {1};
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -140,9 +141,10 @@ __global__ void __launch_bounds__(256) Level0Kernel(const __grid_constant__ Leve
   }
 }
 
-void LaunchLevel0(const Level0Args& a, cudaStream_t stream) {
+LaunchResult LaunchLevel0(const Level0Args& a, cudaStream_t stream) {
   dim3 grid((a.w + 31) / 32, (a.h + 7) / 8, 2);
   Level0Kernel<<<grid, 256, 0, stream>>>(a);
+  return {1};
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -184,10 +186,11 @@ __global__ void __launch_bounds__(256) DownsampleKernel(const __grid_constant__ 
   o.color[static_cast<size_t>(y) * o.color_pitch + x] = static_cast<uint8_t>(255.f * color + 0.5f);
 }
 
-void LaunchDownsample(const DownsampleArgs& a, cudaStream_t stream) {
-  if (a.count <= 0) return;
+LaunchResult LaunchDownsample(const DownsampleArgs& a, cudaStream_t stream) {
+  if (a.count <= 0) return {};
   dim3 grid((a.w + 31) / 32, (a.h + 7) / 8, a.count);
   DownsampleKernel<<<grid, 256, 0, stream>>>(a);
+  return {1};
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -568,15 +571,15 @@ __global__ void __launch_bounds__(kTrackThreads, 1) OdomTrackKernel(const __grid
   }
 }
 
-void LaunchTrack(const TrackArgs& a, int sm_count, cudaStream_t stream) {
+LaunchResult LaunchTrack(const TrackArgs& a, int sm_count, cudaStream_t stream) {
   // one CTA per SM (all co-resident: the grid barrier needs it), never more CTAs than the finest level has tiles
   const Level& L0 = a.level[a.first_scale];
   const int tiles = ((L0.cam.w + 31) / 32) * ((L0.cam.h + 7) / 8);
   const int grid = tiles < sm_count ? (tiles > 0 ? tiles : 1) : sm_count;
   // cooperative launch: the runtime guarantees that all CTAs are resident at the same time (or refuses the launch)
   void* params[] = {const_cast<TrackArgs*>(&a)};
-  if (a.use_gradmag) cudaLaunchCooperativeKernel(reinterpret_cast<void*>(OdomTrackKernel<true>), dim3(grid), dim3(kTrackThreads), params, 0, stream);
-  else cudaLaunchCooperativeKernel(reinterpret_cast<void*>(OdomTrackKernel<false>), dim3(grid), dim3(kTrackThreads), params, 0, stream);
+  void* kernel = a.use_gradmag ? reinterpret_cast<void*>(OdomTrackKernel<true>) : reinterpret_cast<void*>(OdomTrackKernel<false>);
+  return {1, cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kTrackThreads), params, 0, stream)};
 }
 
 }  // namespace odom

@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "launch.hpp"
+
 namespace bba {
 namespace odom {
 
@@ -50,7 +52,7 @@ struct BrightnessArgs {
   int w, h;
   int use_gradmag;
 };
-void LaunchBrightness(const BrightnessArgs& a, cudaStream_t stream);
+LaunchResult LaunchBrightness(const BrightnessArgs& a, cudaStream_t stream);
 
 // Stage 2 (depth-sized, level 0): base = CalibrateDepthAndTransformColorToDepthCUDAKernel (kernel_downsample.cu:345-372);
 // tracked = CalibrateDepthCUDAKernel (:404-426) + CUDABuffer::SetToReadModeNormalized (cuda_buffer.cu:82-102), or -- without
@@ -72,7 +74,7 @@ struct Level0Args {
   int skip_level0;                // !use_pyramid_level_0
   int downsample_color;           // depth width == colour width (pairwise_frame_tracking.cc:309)
 };
-void LaunchLevel0(const Level0Args& a, cudaStream_t stream);
+LaunchResult LaunchLevel0(const Level0Args& a, cudaStream_t stream);
 
 // Stage 3: DownsampleImagesCUDAKernel (kernel_downsample.cu:107-156), level s-1 -> s, for up to two images in one launch.
 struct DownsampleArgs {
@@ -81,7 +83,7 @@ struct DownsampleArgs {
   int w, h;       // output size
   int in_w, in_h; // input size (>= 2 w, 2 h; one more when the finer level is odd-sized)
 };
-void LaunchDownsample(const DownsampleArgs& a, cudaStream_t stream);
+LaunchResult LaunchDownsample(const DownsampleArgs& a, cudaStream_t stream);
 
 // Stage 4: the whole coarse-to-fine Gauss-Newton of TrackFramePairwise in ONE persistent launch (grid-wide barriers between
 // passes, the 6x6 solve + SE3 update replicated in every CTA).
@@ -109,7 +111,7 @@ struct TrackArgs {
   unsigned int* barrier;       // [2] {arrival count, generation}, zero at launch
   TrackResult* result;
 };
-void LaunchTrack(const TrackArgs& a, int sm_count, cudaStream_t stream);
+LaunchResult LaunchTrack(const TrackArgs& a, int sm_count, cudaStream_t stream);
 
 }  // namespace odom
 }  // namespace bba

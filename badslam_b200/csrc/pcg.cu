@@ -458,21 +458,28 @@ __global__ void PcgUnpackAlphaDKernel(double* __restrict__ scalars, const float*
   scalars[1] += static_cast<double>(tail[0]) + static_cast<double>(tail[1]);
   scalars[3] = 0.0;
 }
-void LaunchPcgPackAlphaD(const double* scalars, float* tail, cudaStream_t stream) { PcgPackAlphaDKernel<<<1, 1, 0, stream>>>(scalars, tail); }
-void LaunchPcgUnpackAlphaD(double* scalars, const float* tail, cudaStream_t stream) { PcgUnpackAlphaDKernel<<<1, 1, 0, stream>>>(scalars, tail); }
+LaunchResult LaunchPcgPackAlphaD(const double* scalars, float* tail, cudaStream_t stream) {
+  PcgPackAlphaDKernel<<<1, 1, 0, stream>>>(scalars, tail);
+  return {1};
+}
+LaunchResult LaunchPcgUnpackAlphaD(double* scalars, const float* tail, cudaStream_t stream) {
+  PcgUnpackAlphaDKernel<<<1, 1, 0, stream>>>(scalars, tail);
+  return {1};
+}
 
-void LaunchPcgAccumulate(const PcgArgs& a, int sm_count, bool init, cudaStream_t stream) {
-  if (a.end <= a.begin || a.kf_count <= 0) return;
-  cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream);
+LaunchResult LaunchPcgAccumulate(const PcgArgs& a, int sm_count, bool init, cudaStream_t stream) {
+  if (a.end <= a.begin || a.kf_count <= 0) return {};
+  LaunchResult r{1, cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream)};
   const uint64_t n_tiles = (a.end - a.begin + 31u) / 32u;
   const uint64_t n_items = n_tiles * ((a.kf_count + kGroup - 1) / kGroup);
   auto launch = [&](auto kernel) {
     int per_sm = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, 0);
+    r += cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, 0);
     kernel<<<ItemGrid(per_sm, sm_count, n_items), kThreads, 0, stream>>>(a);
   };
   if (init) launch(PcgAccumulateKernel<true>);
   else launch(PcgAccumulateKernel<false>);
+  return r;
 }
 
 static uint32_t VectorGrid(uint32_t n, int sm_count) {
@@ -480,25 +487,30 @@ static uint32_t VectorGrid(uint32_t n, int sm_count) {
   return static_cast<uint32_t>(std::min<uint64_t>(std::min<uint64_t>((static_cast<uint64_t>(n) + 255) / 256, static_cast<uint64_t>(sm_count) * 8), 2048));
 }
 
-void LaunchPcgInit2(uint32_t n, uint32_t a_index, float a, int kf_count, const float* r, const float* M, float* delta, float* g, float* p,
-                    double* scalars, int slot_alpha_n, int sm_count, cudaStream_t stream) {
+LaunchResult LaunchPcgInit2(uint32_t n, uint32_t a_index, float a, int kf_count, const float* r, const float* M, float* delta, float* g,
+                            float* p, double* scalars, int slot_alpha_n, int sm_count, cudaStream_t stream) {
   PcgInit2Kernel<<<VectorGrid(n, sm_count), 256, 0, stream>>>(n, a_index, a, kf_count, r, M, delta, g, p, scalars, slot_alpha_n);
+  return {1};
 }
-void LaunchPcgStep2(uint32_t n, uint32_t a_index, float* r, const float* M, float* delta, float* g, const float* p, double* scalars,
-                    int slot_alpha_n, int slot_beta_n, int sm_count, cudaStream_t stream) {
+LaunchResult LaunchPcgStep2(uint32_t n, uint32_t a_index, float* r, const float* M, float* delta, float* g, const float* p, double* scalars,
+                            int slot_alpha_n, int slot_beta_n, int sm_count, cudaStream_t stream) {
   PcgStep2Kernel<<<VectorGrid(n, sm_count), 256, 0, stream>>>(n, a_index, r, M, delta, g, p, scalars, slot_alpha_n, slot_beta_n);
+  return {1};
 }
-void LaunchPcgStep3(uint32_t n, uint32_t a_index, int kf_count, float* g, float* p, double* scalars, int slot_alpha_n, int slot_beta_n,
-                    int sm_count, cudaStream_t stream) {
+LaunchResult LaunchPcgStep3(uint32_t n, uint32_t a_index, int kf_count, float* g, float* p, double* scalars, int slot_alpha_n,
+                            int slot_beta_n, int sm_count, cudaStream_t stream) {
   PcgStep3Kernel<<<VectorGrid(n, sm_count), 256, 0, stream>>>(n, a_index, kf_count, g, p, scalars, slot_alpha_n, slot_beta_n);
+  return {1};
 }
-void LaunchPcgUpdateSurfels(float* surfels, uint32_t pitch, uint32_t n, bool use_desc, uint32_t surfel_start, const float* delta,
-                            cudaStream_t stream) {
-  if (n == 0) return;
+LaunchResult LaunchPcgUpdateSurfels(float* surfels, uint32_t pitch, uint32_t n, bool use_desc, uint32_t surfel_start, const float* delta,
+                                    cudaStream_t stream) {
+  if (n == 0) return {};
   PcgUpdateSurfelsKernel<<<(n + 255) / 256, 256, 0, stream>>>(surfels, pitch, n, use_desc ? 1 : 0, surfel_start, delta);
+  return {1};
 }
-void LaunchPcgUpdateCfactor(float* cfactor, uint32_t cells, const float* delta, cudaStream_t stream) {
+LaunchResult LaunchPcgUpdateCfactor(float* cfactor, uint32_t cells, const float* delta, cudaStream_t stream) {
   PcgUpdateCfactorKernel<<<(cells + 255) / 256, 256, 0, stream>>>(cfactor, cells, delta);
+  return {1};
 }
 
 }  // namespace bba

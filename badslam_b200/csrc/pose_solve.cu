@@ -81,6 +81,9 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
   }
 }
 
-void LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream) { PoseSolveKernel<<<1, 256, 0, stream>>>(args); }
+LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream) {
+  PoseSolveKernel<<<1, 256, 0, stream>>>(args);
+  return {1};
+}
 
 }  // namespace bba

@@ -32,9 +32,8 @@ bba_status EnsureSpatialOrder(bba_handle h, bool sort, bool rebuild, cudaStream_
     p.order.capacity = cap;
   }
   if (sort && (rebuild || p.order_stale || p.order_n != n)) {
-    LaunchSpatialOrder(h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), n, p.order.view, s);
-    BBA_CUDA(h, cudaGetLastError());
-    h->launches += 3;   // bounds, keys, the sort (counted as one)
+    BBA_LAUNCH(h, h->launches, LaunchSpatialOrder, h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), n,
+               p.order.view, s);
     p.order_n = n;
     p.order_stale = false;
   }
@@ -71,9 +70,8 @@ bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStre
     const bool sort = variant != kPoseVariantAuto ||
                       static_cast<uint64_t>(h->surfels_size) * static_cast<uint64_t>(n_work) >= kSpatialOrderMinPairs;
     if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/false, s)) return st;
-    LaunchPoseStream(h->surfels, acc->pitch, h->surfels_size, sort ? p.order.view.perm : nullptr, p.order.stream,
-                     p.order.capacity, p.order.boxes, s);
-    ++h->launches;
+    BBA_LAUNCH(h, h->launches, LaunchPoseStream, h->surfels, acc->pitch, h->surfels_size, sort ? p.order.view.perm : nullptr, p.order.stream,
+               p.order.capacity, p.order.boxes, s);
     acc->stream = p.order.stream;
     acc->stream_pitch = p.order.capacity;
     acc->boxes = p.order.boxes;
@@ -119,11 +117,7 @@ bba_status PoseCoeffsBatch(bba_handle h, const std::vector<int>& ids, const std:
   if (bba_status st = PreparePoseAccumulate(h, count, variant, s, &acc)) return st;
   acc.work_list = p.d_work[0];
   acc.work_count = p.d_count;
-  if (h->surfels_size > 0) {
-    LaunchPoseAccumulate(acc, h->sm_count, with_stats, count, s, variant);
-    h->launches += 2;   // record packing + the kernel
-  }
-  BBA_CUDA(h, cudaGetLastError());
+  BBA_LAUNCH(h, h->launches, LaunchPoseAccumulate, acc, h->sm_count, with_stats, count, s, variant);
   rec->resize(static_cast<size_t>(kPoseAccSize) * K);
   sc->resize(2 * static_cast<size_t>(K));
   BBA_CUDA(h, cudaMemcpyAsync(rec->data(), p.d_acc, sizeof(double) * rec->size(), cudaMemcpyDeviceToHost, s));
@@ -192,17 +186,15 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
     acc.work_count = p.d_count + cur;
     if (h->surfels_size > 0) {
       if (h->profiling && it < 32) BBA_CUDA(h, cudaEventRecord(h->prof_ev[2 * it], s));
-      LaunchPoseAccumulate(acc, h->sm_count, /*with_stats=*/it == 0 || h->profiling >= 2, n_local, s);
+      BBA_LAUNCH(h, h->launches, LaunchPoseAccumulate, acc, h->sm_count, /*with_stats=*/it == 0 || h->profiling >= 2, n_local, s);
       if (h->profiling && it < 32) BBA_CUDA(h, cudaEventRecord(h->prof_ev[2 * it + 1], s));
-      h->launches += 2;   // record packing + the kernel
     }
     sol.work_in = p.d_work[cur];
     sol.count_in = p.d_count + cur;
     sol.work_out = p.d_work[cur ^ 1];
     sol.count_out = p.d_count + (cur ^ 1);
     sol.iteration = it;
-    LaunchPoseSolve(sol, s);
-    ++h->launches;
+    BBA_LAUNCH(h, h->launches, LaunchPoseSolve, sol, s);
     ++enqueued;
     // Keep kDepth iterations queued ahead of the one executing: wait (host poll on zero-copy memory, the stream is never
     // blocked) until iteration it-kDepth has finished, and stop as soon as an iteration left no unconverged keyframe.  (An
@@ -221,12 +213,11 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
     }
     if (it >= 1 && p.h_flag[0] >= 1 && p.h_flag[1] == 0) break;   // (h_flag[1] belongs to the last finished iteration)
   }
-  BBA_CUDA(h, cudaGetLastError());
   if (world > 1) {
     // ONE all-reduce per pose step: every rank contributes the slots of its keyframes, all others are zero.
     BBA_CUDA(h, cudaMemsetAsync(x.d_pose_pack, 0, sizeof(float) * kPoseSlot * K, s));
-    LaunchPackPoseResults(x.d_local_ids, n_local, p.d_pose_est, p.d_iterations, p.d_converged, p.d_first_stats, x.d_pose_pack, s);
-    ++h->launches;
+    BBA_LAUNCH(h, h->launches, LaunchPackPoseResults, x.d_local_ids, n_local, p.d_pose_est, p.d_iterations, p.d_converged, p.d_first_stats,
+               x.d_pose_pack, s);
     x.collective(x.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, x.d_pose_pack, static_cast<size_t>(kPoseSlot) * K, s);
     x.replicated_pass_pending = false;   // (every rank's earlier work on this stream precedes its contribution)
     BBA_CUDA(h, cudaMemcpyAsync(x.h_pose_pack, x.d_pose_pack, sizeof(float) * kPoseSlot * K, cudaMemcpyDeviceToHost, s));

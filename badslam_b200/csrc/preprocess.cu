@@ -72,18 +72,18 @@ __global__ void InitMinMaxKernel(float* min_max) {
 
 }  // namespace pre
 
-// Enqueues the initialisation of min_max and the fused kernel; returns the number of launches (2).
-int LaunchPreprocessFrame(const pre::FrameArgs& f, cudaStream_t stream) {
+// Enqueues the initialisation of min_max and the fused kernel (2 launches).
+LaunchResult LaunchPreprocessFrame(const pre::FrameArgs& f, cudaStream_t stream) {
   pre::InitMinMaxKernel<<<1, 1, 0, stream>>>(f.min_max);
   const int blocks = f.tiles_x * f.tiles_y + ((f.rgb && f.rgba) ? pre::ColorChunks(f.cw, f.ch) : 0);
   const size_t smem = sizeof(uint16_t) * static_cast<size_t>(pre::SharedWords(f.radius));
   pre::PreprocessFrameKernel<<<blocks, pre::kThreads, smem, stream>>>(f);
-  return 2;
+  return {2};
 }
 
 // The raw-frame variant (the host has validated f: at most one of median_iterations / a downscaled raw size, levels <= 3);
-// returns the number of launches (2).
-int LaunchPreprocessRawFrame(const pre::FrameArgs& f, cudaStream_t stream) {
+// 2 launches.
+LaunchResult LaunchPreprocessRawFrame(const pre::FrameArgs& f, cudaStream_t stream) {
   using pre::Stage0;
   pre::InitMinMaxKernel<<<1, 1, 0, stream>>>(f.min_max);
   const int blocks = f.tiles_x * f.tiles_y + ((f.rgb && f.rgba) ? pre::ColorChunks(f.cw, f.ch) : 0);
@@ -95,7 +95,7 @@ int LaunchPreprocessRawFrame(const pre::FrameArgs& f, cudaStream_t stream) {
     case 2: pre::PreprocessRawFrameKernel<Stage0::kDownscale, 2><<<blocks, pre::kThreads, smem, stream>>>(f); break;
     default: pre::PreprocessRawFrameKernel<Stage0::kDownscale, 3><<<blocks, pre::kThreads, smem, stream>>>(f); break;
   }
-  return 2;
+  return {2};
 }
 
 }  // namespace bba

@@ -25,6 +25,8 @@
 
 #if defined(__CUDACC__)
 #include <cuda_fp16.h>
+
+#include "launch.hpp"
 #define BBA_PRE_HD __host__ __device__ __forceinline__
 #else
 #define BBA_PRE_HD inline
@@ -504,8 +506,8 @@ inline int ColorChunks(int cw, int ch) {
 }  // namespace pre
 
 #if defined(__CUDACC__)
-int LaunchPreprocessFrame(const pre::FrameArgs& f, cudaStream_t stream);      // preprocess.cu
-int LaunchPreprocessRawFrame(const pre::FrameArgs& f, cudaStream_t stream);   // preprocess.cu: stage 0 per f's raw-frame fields
+LaunchResult LaunchPreprocessFrame(const pre::FrameArgs& f, cudaStream_t stream);      // preprocess.cu
+LaunchResult LaunchPreprocessRawFrame(const pre::FrameArgs& f, cudaStream_t stream);   // preprocess.cu: stage 0 per f's raw-frame fields
 #endif
 
 }  // namespace bba

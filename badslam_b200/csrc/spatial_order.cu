@@ -155,9 +155,10 @@ __global__ void __launch_bounds__(256) GeometryStreamKernel(const __grid_constan
 
 }  // namespace
 
-void LaunchGeometryStream(const GeometryArgs& a, bool desc_rows, cudaStream_t stream) {
-  if (a.end <= a.begin) return;
+LaunchResult LaunchGeometryStream(const GeometryArgs& a, bool desc_rows, cudaStream_t stream) {
+  if (a.end <= a.begin) return {};
   GeometryStreamKernel<<<(a.end - a.begin + 255) / 256, 256, 0, stream>>>(a, desc_rows);
+  return {1};
 }
 
 size_t SpatialOrderTempBytes(uint32_t capacity) {
@@ -168,23 +169,27 @@ size_t SpatialOrderTempBytes(uint32_t capacity) {
   return bytes;
 }
 
-void LaunchSpatialOrder(const float* surfels, uint32_t pitch, uint32_t n, const SpatialOrderBuffers& b, cudaStream_t stream) {
-  if (n == 0) return;
-  cudaMemsetAsync(b.bounds, 0xff, 3 * sizeof(unsigned int), stream);
-  cudaMemsetAsync(b.bounds + 3, 0, 3 * sizeof(unsigned int), stream);
+// The sort reports some errors (a temp buffer that is too small) only through its return value, never through the last error.
+LaunchResult LaunchSpatialOrder(const float* surfels, uint32_t pitch, uint32_t n, const SpatialOrderBuffers& b, cudaStream_t stream) {
+  if (n == 0) return {};
+  LaunchResult r{3};   // bounds, keys, the sort
+  r += cudaMemsetAsync(b.bounds, 0xff, 3 * sizeof(unsigned int), stream);
+  r += cudaMemsetAsync(b.bounds + 3, 0, 3 * sizeof(unsigned int), stream);
   const uint32_t blocks = min((n + 255u) / 256u, 1024u);
   SurfelBoundsKernel<<<blocks, 256, 0, stream>>>(surfels, pitch, n, b.bounds);
   MortonKeysKernel<<<(n + 255) / 256, 256, 0, stream>>>(surfels, pitch, n, b.bounds, b.keys_in, b.index_in);
   size_t temp_bytes = b.temp_bytes;
-  cub::DeviceRadixSort::SortPairs(b.temp, temp_bytes, b.keys_in, b.keys_out, b.index_in, b.perm, static_cast<int>(n), 0,
-                                  3 * kMortonBits, stream);
+  r += cub::DeviceRadixSort::SortPairs(b.temp, temp_bytes, b.keys_in, b.keys_out, b.index_in, b.perm, static_cast<int>(n), 0,
+                                       3 * kMortonBits, stream);
+  return r;
 }
 
-void LaunchPoseStream(const float* surfels, uint32_t pitch, uint32_t n, const uint32_t* perm, float* stream, uint32_t stream_pitch,
-                      float* boxes, cudaStream_t cuda_stream) {
-  if (n == 0) return;
+LaunchResult LaunchPoseStream(const float* surfels, uint32_t pitch, uint32_t n, const uint32_t* perm, float* stream, uint32_t stream_pitch,
+                              float* boxes, cudaStream_t cuda_stream) {
+  if (n == 0) return {};
   PoseStreamKernel<<<(n + kSpatialChunk - 1) / kSpatialChunk, kSpatialChunk, 0, cuda_stream>>>(surfels, pitch, n, perm, stream,
                                                                                              stream_pitch, boxes);
+  return {1};
 }
 
 }  // namespace bba

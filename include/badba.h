@@ -127,7 +127,8 @@ typedef struct {
   float ms_geometry_optimization;
   float ms_pose_optimization;
   float ms_intrinsics_optimization;
-  uint64_t kernel_launches;            /* kernels this call launched */
+  uint64_t kernel_launches;            /* kernels this call launched, as the launchers report them: the CUB radix sort of the
+                                        * spatial order counts as one, memsets and copies are not counted */
   /* use_pcg: inner PCG steps summed over the outer iterations, last residual norm sqrt(beta_n), device time of the
    * last iteration's PCG solve ("BA PCG step", direct_ba_pcg.cc:733-737) */
   int pcg_inner_iterations_total;
@@ -469,7 +470,7 @@ typedef struct {
   uint32_t residual_count;  /* the reference's debug counters at the last accumulation (kernel_opt_pose.cu:619-657) */
   float residual_sum;
   uint32_t passes;          /* image passes (grid-wide barriers) of the persistent kernel */
-  uint32_t kernel_launches; /* launches of the whole call */
+  uint32_t kernel_launches; /* kernels the whole call launched (memsets and copies are not counted) */
 } bba_odometry_result;
 bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* options, int base_keyframe_id,
                                     const uint16_t* device_depth, size_t depth_pitch,
