@@ -166,6 +166,11 @@ uint32_t SurfelCapacity(bba_handle h) {
   return std::min<uint32_t>(h->cfg.max_surfel_count, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)));
 }
 
+// size of life.d_scan_sums: the surfel creation scans the pixels, the compaction the surfels
+size_t ScanSumsAlloc(bba_handle h) {
+  return bba::ScanScratchWords(std::max(static_cast<uint32_t>(h->cfg.depth_width) * h->cfg.depth_height, SurfelCapacity(h)));
+}
+
 bba_status MakeLifecycleArgs(bba_handle h, int k, bba::LifecycleArgs* a, cudaStream_t s) {
   const uint32_t cells = static_cast<uint32_t>(h->cf_w) * h->cf_h;
   const uint32_t pixels = static_cast<uint32_t>(h->cfg.depth_width) * h->cfg.depth_height;
@@ -174,11 +179,11 @@ bba_status MakeLifecycleArgs(bba_handle h, int k, bba::LifecycleArgs* a, cudaStr
   BBA_CUDA(h, l.d_cell_bits.Reserve(cells));
   BBA_CUDA(h, l.d_flags.Reserve(pixels));
   BBA_CUDA(h, l.d_scan_out.Reserve(pixels));
-  BBA_CUDA(h, l.d_scan_sums.Reserve(bba::ScanScratchWords(pixels)));
+  BBA_CUDA(h, l.d_scan_sums.Reserve(bba::ScanScratchWords(pixels), ScanSumsAlloc(h)));
   BBA_CUDA(h, l.d_covis.Reserve(h->cfg.max_keyframes));
   BBA_CUDA(h, l.h_covis.Reserve(h->cfg.max_keyframes));
   BBA_CUDA(h, l.d_deleted_count.Reserve(1));
-  BBA_CUDA(h, l.h_deleted_count.Reserve(1));
+  BBA_CUDA(h, l.h_count.Reserve(1));
   const Keyframe& kf = h->keyframes[k];
   a->cam = MakeCamera(h);
   bba::ToMatrix3x4(bba::Inverse(kf.pose), a->T);
@@ -240,11 +245,10 @@ bba_status CreateSurfelsForKeyframe(bba_handle h, int k, bool filter, cudaStream
   BBA_LAUNCH(h, h->launches, LaunchSupportSurfels, a, h->sm_count, s);   // DetermineSupportingSurfelsCUDA: is the cell supported at all
   BBA_LAUNCH(h, h->launches, LaunchSeedNewSurfels, a, filter, s);
   BBA_LAUNCH(h, h->launches, LaunchExclusiveScan, h->life.d_flags, pixels, h->life.d_scan_out, h->life.d_scan_sums, s);
-  const uint32_t n_blocks = (pixels + 4095) / 4096;
-  BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_scan_sums + n_blocks, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaMemcpyAsync(h->life.h_count, h->life.d_scan_sums + bba::ScanTotalIndex(pixels), sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_create_surfels.cu:466-474
   h->staging.pending = false;
-  const uint32_t created = *h->life.h_deleted_count;
+  const uint32_t created = *h->life.h_count;
   BBA_TRACE("create: counted");
   if (created == 0) return BBA_OK;
   if (h->surfels_size + static_cast<uint64_t>(created) > SurfelCapacity(h)) {
@@ -268,9 +272,9 @@ bba_status MergeSurfelsForKeyframe(bba_handle h, int k, cudaStream_t s, uint32_t
   if (bba_status st = MakeLifecycleArgs(h, k, &a, s)) return st;
   BBA_CUDA(h, cudaMemsetAsync(h->life.d_deleted_count, 0, sizeof(unsigned int), s));
   BBA_LAUNCH(h, h->launches, LaunchMergeSurfels, a, h->sm_count, s);
-  BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaMemcpyAsync(h->life.h_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_supporting_surfels.cc:93-96
-  *deleted = *h->life.h_deleted_count;
+  *deleted = *h->life.h_count;
   return BBA_OK;
 }
 
@@ -278,10 +282,9 @@ bba_status CompactSurfels(bba_handle h, uint32_t free_count, bool with_active, c
   const uint32_t N = h->surfels_size;
   if (free_count == 0 || N == 0) return BBA_OK;
   h->xchg.replicated_pass_pending = true;
-  BBA_CUDA(h, h->life.d_compact_sums.Reserve(bba::CompactScratchWords(N),
-                                              bba::CompactScratchWords(std::max(h->cfg.max_surfel_count, N))));
+  BBA_CUDA(h, h->life.d_scan_sums.Reserve(bba::ScanScratchWords(N), ScanSumsAlloc(h)));
   BBA_LAUNCH(h, h->launches, LaunchCompactSurfels, h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), N, free_count,
-             h->life.d_compact_sums, with_active ? h->active : nullptr, s);
+             h->life.d_scan_sums, with_active ? h->active : nullptr, s);
   h->surfels_size = N - free_count;
   return BBA_OK;
 }
@@ -298,7 +301,7 @@ bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, 
   BBA_CUDA(h, h->life.d_kf_radius.Reserve(h->cfg.max_keyframes));
   BBA_CUDA(h, h->life.h_kf_radius.Reserve(h->cfg.max_keyframes));
   BBA_CUDA(h, h->life.d_deleted_count.Reserve(1));
-  BBA_CUDA(h, h->life.h_deleted_count.Reserve(1));
+  BBA_CUDA(h, h->life.h_count.Reserve(1));
   BBA_TRACE("end tasks");
   // merge similar surfels using all keyframes which were active in this BA iteration block (direct_ba.cc:577-601)
   uint32_t merged = 0;
@@ -361,10 +364,10 @@ bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, 
     // deleted count of this shard as two exactly representable floats (low 12 bits, the rest), summed over the ranks
     BBA_CUDA(h, h->xchg.d_count_xchg.Reserve(2));
     BBA_CUDA(h, h->xchg.h_count_xchg.Reserve(2));
-    BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaMemcpyAsync(h->life.h_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
     BBA_CUDA(h, cudaStreamSynchronize(s));
-    h->xchg.h_count_xchg[0] = static_cast<float>(*h->life.h_deleted_count & 0xfffu);
-    h->xchg.h_count_xchg[1] = static_cast<float>(*h->life.h_deleted_count >> 12);
+    h->xchg.h_count_xchg[0] = static_cast<float>(*h->life.h_count & 0xfffu);
+    h->xchg.h_count_xchg[1] = static_cast<float>(*h->life.h_count >> 12);
     BBA_CUDA(h, cudaMemcpyAsync(h->xchg.d_count_xchg, h->xchg.h_count_xchg, sizeof(float) * 2, cudaMemcpyHostToDevice, s));
     h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->xchg.d_count_xchg, 2, s);
     BBA_CUDA(h, cudaMemcpyAsync(h->xchg.h_count_xchg, h->xchg.d_count_xchg, sizeof(float) * 2, cudaMemcpyDeviceToHost, s));
@@ -372,9 +375,9 @@ bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, 
     deleted_total = static_cast<uint32_t>(h->xchg.h_count_xchg[0] + 0.5f) + (static_cast<uint32_t>(h->xchg.h_count_xchg[1] + 0.5f) << 12);
     h->xchg.replicated_pass_pending = true;   // the compaction below rewrites every replica as a whole
   } else {
-    BBA_CUDA(h, cudaMemcpyAsync(h->life.h_deleted_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaMemcpyAsync(h->life.h_count, h->life.d_deleted_count, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
     BBA_CUDA(h, cudaStreamSynchronize(s));   // kernel_delete_surfels.cc:93-96
-    deleted_total = *h->life.h_deleted_count;
+    deleted_total = *h->life.h_count;
   }
   h->staging.pending = false;
   BBA_TRACE("stats done");

@@ -248,14 +248,13 @@ struct bba_context {
     bba::DeviceBuffer<unsigned int> d_cell_bits;   // [cells]
     bba::DeviceBuffer<unsigned int> d_flags;       // [w * h]
     bba::DeviceBuffer<unsigned int> d_scan_out;    // [w * h]
-    bba::DeviceBuffer<unsigned int> d_scan_sums;
+    bba::DeviceBuffer<unsigned int> d_scan_sums;   // block sums of the creation's and the compaction's scan
     bba::DeviceBuffer<bba::CovisEntry> d_covis;    // [max_keyframes]
     bba::PinnedBuffer<bba::CovisEntry> h_covis;
     bba::DeviceBuffer<bba::KfRadius> d_kf_radius;  // [max_keyframes]
     bba::PinnedBuffer<bba::KfRadius> h_kf_radius;
     bba::DeviceBuffer<unsigned int> d_deleted_count;
-    bba::PinnedBuffer<unsigned int> h_deleted_count;
-    bba::DeviceBuffer<unsigned int> d_compact_sums;
+    bba::PinnedBuffer<unsigned int> h_count;       // a created or deleted count on its way to the host
   } life;
   int last_ba_iteration_count = -1;   // direct_ba.cc:126
 

@@ -257,7 +257,10 @@ LaunchResult LaunchPackStatsShard(const float* surfels, uint32_t pitch, uint32_t
                                   cudaStream_t stream);
 LaunchResult LaunchUnpackStatsShards(float* surfels, uint32_t pitch, uint32_t n, uint32_t shard_len, int world, int skip_rank, const float* buffer,
                                      cudaStream_t stream);
-uint32_t CompactScratchWords(uint32_t n);   // size of block_sums for LaunchCompactSurfels
+// Exclusive scan of n u32 counts, shared by the compaction and the surfel creation: block_sums needs ScanScratchWords(n) words,
+// and block_sums[ScanTotalIndex(n)] receives the sum of all counts.
+uint32_t ScanScratchWords(uint32_t n);
+uint32_t ScanTotalIndex(uint32_t n);
 // Moves surviving surfels from the tail into the free spots; afterwards the first n - free_count slots are the surfels.
 // active != nullptr: the active flags move with them (CompactSurfelsCUDA's adapt_active_surfels).
 LaunchResult LaunchCompactSurfels(float* surfels, uint32_t pitch, uint32_t n, uint32_t free_count, unsigned int* block_sums, uint8_t* active,
@@ -297,7 +300,6 @@ struct LifecycleArgs {
 LaunchResult LaunchSupportSurfels(const LifecycleArgs& a, int sm_count, cudaStream_t stream);   // sup[0] only (occupancy for the creation)
 LaunchResult LaunchMergeSurfels(const LifecycleArgs& a, int sm_count, cudaStream_t stream);     // supports + merge, += *counter
 LaunchResult LaunchSeedNewSurfels(const LifecycleArgs& a, bool filter, cudaStream_t stream);    // a.flags after LaunchSupportSurfels
-uint32_t ScanScratchWords(uint32_t n);
 LaunchResult LaunchExclusiveScan(const unsigned int* in, uint32_t n, unsigned int* out, unsigned int* block_sums, cudaStream_t stream);
 LaunchResult LaunchCreateSurfels(const LifecycleArgs& a, const unsigned int* index, cudaStream_t stream);
 

@@ -31,29 +31,19 @@ constexpr float kAPriorWeight = 10.f;   // kernel_pcg.cu:48
 // alpha / beta (and with them identical step lengths and identical inner-loop decisions), and single-GPU runs are reproducible.
 // partials: >= gridDim.x doubles; counter: zero before the launch, zero again after it.
 __device__ __forceinline__ void GridOrderedAdd(double* dst, double v, double* partials, unsigned int* counter) {
-  __shared__ double partial[32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if (lane == 0) partial[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    double s = (lane < static_cast<int>(blockDim.x >> 5)) ? partial[lane] : 0.0;
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) {
-      partials[blockIdx.x] = s;
+  v = BlockSum(v);
+  if (threadIdx.x == 0) {
+    partials[blockIdx.x] = v;
+    __threadfence();
+    if (atomicAdd(counter, 1u) == gridDim.x - 1) {
       __threadfence();
-      if (atomicAdd(counter, 1u) == gridDim.x - 1) {
-        __threadfence();
-        double total = 0.0;
-        for (unsigned int b = 0; b < gridDim.x; ++b) total += __ldcg(partials + b);
-        *dst += total;
-        *counter = 0u;
-      }
+      double total = 0.0;
+      for (unsigned int b = 0; b < gridDim.x; ++b) total += __ldcg(partials + b);
+      *dst += total;
+      *counter = 0u;
     }
   }
-  __syncthreads();
+  __syncthreads();   // (BlockSum's partials are reused by the next call)
 }
 
 __device__ __forceinline__ float DiagExtra(uint32_t i, uint32_t a_index) {   // lambda (+ the prior on `a`) on the diagonal

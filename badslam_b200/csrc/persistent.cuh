@@ -1,5 +1,6 @@
-// persistent.cuh -- the machinery the persistent kernels share: warp reductions, the (keyframe group x surfel tile) work-item
-// loop with its per-tile epochs, the stores into the surfel replicas, the keyframe record loaders and the launch sizing.
+// persistent.cuh -- the machinery the persistent kernels share: warp and block reductions and the block scan, the (keyframe
+// group x surfel tile) work-item loop with its per-tile epochs, the stores into the surfel replicas, the keyframe record loaders
+// and the launch sizing.
 #pragma once
 
 #include <algorithm>
@@ -18,10 +19,56 @@ __device__ __forceinline__ void StoreRelease(unsigned int* p, unsigned int v) {
   asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-__device__ __forceinline__ float WarpSum(float v) {
+template <typename T>
+__device__ __forceinline__ T WarpSum(T v) {
 #pragma unroll
   for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// Sum of v over the block: a butterfly within each warp, one partial per warp in shared memory, then a butterfly over the
+// partials in warp 0.  The total is valid in warp 0 only.  A second call in the same kernel needs a __syncthreads() in between:
+// warp 0 may still be reading the partials.
+template <typename T>
+__device__ __forceinline__ T BlockSum(T v) {
+  __shared__ T partial[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  v = WarpSum(v);
+  if (lane == 0) partial[warp] = v;
+  __syncthreads();
+  if (warp == 0) v = WarpSum(lane < static_cast<int>(blockDim.x >> 5) ? partial[lane] : T(0));
+  return v;
+}
+
+// Exclusive scan of one count per thread over a block of 1024 threads: a shuffle-up scan within each warp, then warp 0 scans the
+// 32 warp totals.  Returns the thread's exclusive offset; *total receives the block total.  A second call in the same kernel
+// needs a __syncthreads() in between: slow threads may still be reading the warp offsets.
+__device__ __forceinline__ unsigned int BlockExclusiveScan(unsigned int v, unsigned int* total) {
+  __shared__ unsigned int warp_offset[32];
+  __shared__ unsigned int block_total;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  if (lane == 31) warp_offset[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    const unsigned int w = warp_offset[lane];
+    unsigned int winc = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned int t = __shfl_up_sync(0xffffffffu, winc, o);
+      if (lane >= o) winc += t;
+    }
+    warp_offset[lane] = winc - w;
+    if (lane == 31) block_total = winc;
+  }
+  __syncthreads();
+  *total = block_total;
+  return warp_offset[warp] + inc - v;
 }
 
 // Sums v[i] over the warp for all N i at once (N = 8, 16, 32): afterwards lane L holds the total of v[L % N].  For N = 32 that
