@@ -198,6 +198,10 @@ SYMBOLS = {
     "bba_balance_keyframes": (None, [_P, C.c_int, C.c_int, _P]),
     "bba_kernel_launch_count": (C.c_uint64, [_P]),
     "bba_update_keyframe_host": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P]),
+    "bba_set_deterministic": (C.c_int, [_P, C.c_int]),
+    "bba_get_deterministic": (C.c_int, [_P, C.POINTER(C.c_int)]),
+    "bba_debug_exact_sum": (C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_double), _P]),
+    "bba_host_exact_sum": (None, [_P, C.c_size_t, C.POINTER(C.c_double)]),
     "bba_set_profiling": (C.c_int, [_P, C.c_int]),
     "bba_get_profile": (C.c_int, [_P, C.POINTER(Profile), C.c_int]),
 }

@@ -17,7 +17,7 @@ LIB = os.path.join(HERE, "libbadba_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "--expt-relaxed-constexpr"]
 # (source, extra flags).  kernels.cu is built with -use_fast_math like the reference
-# (applications/badslam/CMakeLists.txt:74-75); the fp64 pose solve and the host code are not.
+# (applications/badslam/CMakeLists.txt:74-75); the fp64 pose solve, the exact sum's debug kernels and the host code are not.
 UNITS = [
     ("kernels.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("spatial_order.cu", ["-use_fast_math", "-Xptxas", "-v"]),
@@ -27,13 +27,14 @@ UNITS = [
     ("preprocess.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("odometry.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("pose_solve.cu", []),
+    ("exact_sum.cu", ["-Xptxas", "-v"]),
     ("badba.cu", []),
     ("pose_step.cu", []),
     ("bundle_adjust.cu", []),
     ("multi_gpu.cu", []),
     ("frames.cu", []),
 ]
-HEADERS = ["device_math.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", os.path.join("..", "..", "include", "badba.h")]
+HEADERS = ["device_math.cuh", "exact_sum.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", os.path.join("..", "..", "include", "badba.h")]
 
 
 def _newer(src, dst):

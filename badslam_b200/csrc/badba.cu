@@ -43,6 +43,7 @@ CameraView LiveCameraView(bba_handle h) {
   v.depth_a = h->depth_a;
   v.use_depth = h->cfg.use_depth_residuals;
   v.use_desc = h->cfg.use_descriptor_residuals;
+  v.deterministic = h->deterministic ? 1 : 0;
   return v;
 }
 }  // namespace
@@ -657,6 +658,27 @@ int bba_host_deform_trajectory(int keyframe_count, const int* keyframe_frame_ind
   return BBA_OK;
 }
 
+void bba_host_exact_sum(const float* values, size_t n, double* out) {
+  if (!out) return;
+  long long w[kExactWords] = {};
+  ExactSum sum{};
+  for (size_t i = 0; i < n; ++i) {
+    int word;
+    long long lo, hi;
+    unsigned long long flag;
+    if (bba::ExactSplit(values[i], &word, &lo, &hi, &flag)) {
+      w[word] += lo;
+      w[word + 1] += hi;
+    } else {
+      sum.flags |= flag;
+    }
+    // (the words stay exact for any n: carried before any of them could reach 2^62)
+    if ((i & 0x3fffffffull) == 0x3fffffffull) bba::ExactCarry(w);
+  }
+  for (int i = 0; i < kExactWords; ++i) sum.w[i] = static_cast<unsigned long long>(w[i]);
+  *out = bba::ExactFinalize(sum);
+}
+
 // The readers below are front-end calls: they read the published state (identical to the live state between BA-side calls).
 int bba_keyframe_count(bba_handle h) {
   if (!h) return 0;
@@ -795,6 +817,47 @@ bba_status bba_set_ba_iteration_counts(bba_handle h, int ba_iteration_count, int
 }
 
 uint64_t bba_kernel_launch_count(bba_handle h) { return h ? h->launches + h->front_end_launches : 0; }
+
+bba_status bba_set_deterministic(bba_handle h, int on) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (on && h->cfg.world_size > 1)
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_set_deterministic: the deterministic mode runs on one rank (world_size 1)");
+  if (on && !h->deterministic) {
+    // the exact sums of the pose kernel and of the intrinsics step, zero from here on (every user clears what it consumed)
+    const uint32_t P = static_cast<uint32_t>(h->cf_w) * h->cf_h;
+    const size_t pose = static_cast<size_t>(kPoseAccSize) * h->cfg.max_keyframes;
+    const size_t intr = static_cast<size_t>(7) * P + kIntrinsicsSums;
+    BBA_CUDA(h, h->pose.d_exact.Reserve(pose));
+    BBA_CUDA(h, h->geo.d_intr_exact.Reserve(intr));
+    BBA_CUDA(h, cudaMemset(h->pose.d_exact, 0, sizeof(ExactSum) * pose));
+    BBA_CUDA(h, cudaMemset(h->geo.d_intr_exact, 0, sizeof(ExactSum) * intr));
+  }
+  h->deterministic = on != 0;
+  return Publish(h, nullptr, false);
+}
+
+bba_status bba_get_deterministic(bba_handle h, int* on) {
+  if (!h || !on) return BBA_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lock(h->fe.mu);
+  *on = h->fe.cams.deterministic;
+  return BBA_OK;
+}
+
+bba_status bba_debug_exact_sum(bba_handle h, const float* device_values, uint64_t n, double* out, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (!out || (n && !device_values)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_exact_sum: null argument");
+  if (n >= (1ull << 31)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_exact_sum: an exact sum holds fewer than 2^31 values");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  DeviceBuffer<ExactSum> sum;
+  DeviceBuffer<double> d_out;
+  BBA_CUDA(h, sum.Reserve(1));
+  BBA_CUDA(h, d_out.Reserve(1));
+  BBA_CUDA(h, cudaMemsetAsync(sum, 0, sizeof(ExactSum), s));
+  BBA_LAUNCH(h, h->launches, LaunchExactSumDebug, device_values, n, sum, d_out, h->sm_count, s);
+  BBA_CUDA(h, cudaMemcpyAsync(out, d_out, sizeof(double), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  return BBA_OK;
+}
 
 bba_status bba_set_profiling(bba_handle h, int enable) {
   if (!h) return BBA_ERR_INVALID_ARGUMENT;

@@ -91,6 +91,8 @@ bba_status OptimizeIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cuda
   if (bba_status st = UploadKeyframes(h, s)) return st;
   BBA_CUDA(h, cudaMemsetAsync(h->geo.d_intr, 0, sizeof(float) * intr_floats, s));                      // :69-80
   BBA_CUDA(h, cudaMemsetAsync(h->geo.d_intr_sums, 0, sizeof(double) * bba::kIntrinsicsSums, s));
+  const size_t exact_count = static_cast<size_t>(7) * P + bba::kIntrinsicsSums;
+  if (h->deterministic) BBA_CUDA(h, cudaMemsetAsync(h->geo.d_intr_exact, 0, sizeof(bba::ExactSum) * exact_count, s));
   float* cell_B = h->geo.d_intr + 64;
   float* cell_D = cell_B + static_cast<size_t>(5) * P;
   float* cell_b2 = cell_D + P;
@@ -110,7 +112,10 @@ bba_status OptimizeIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cuda
   a.cell_b2 = cell_b2;
   a.cell_obs = cell_obs;
   a.cell_count = P;
+  a.exact_cells = h->deterministic ? h->geo.d_intr_exact.get() : nullptr;
+  a.exact_sums = h->deterministic ? a.exact_cells + static_cast<size_t>(7) * P : nullptr;
   BBA_LAUNCH(h, h->launches, LaunchIntrinsicsAccumulate, a, h->sm_count, opt_color, opt_depth, s);   // :84-108, one launch for all keyframes
+  if (h->deterministic) BBA_LAUNCH(h, h->launches, LaunchIntrinsicsFinalize, P, a.exact_cells, cell_B, a.exact_sums, h->geo.d_intr_sums, s);
   if (h->cfg.world_size > 1) {
     // every rank accumulated its surfel shard: one sum all-reduce over [34 global sums | B | D | b2 | obs]
     BBA_LAUNCH(h, h->launches, LaunchIntrinsicsConvertSums, h->geo.d_intr_sums, h->geo.d_intr, true, s);
@@ -765,6 +770,8 @@ bba_status BundleAdjust(bba_handle h, const bba_ba_options* o, bba_ba_result* re
   if (bba_status st = CheckSurfels(h)) return st;
   // (do_surfel_updates with more than one rank: creation / merging / compaction run REPLICATED -- they are deterministic and
   // every rank holds the whole surfel buffer -- while the geometry and pose steps stay sharded; see PeerFence)
+  if (o->use_pcg && h->deterministic)
+    return Fail(h, BBA_ERR_UNSUPPORTED, "bba_bundle_adjust: use_pcg is not available in the deterministic mode (bba_set_deterministic)");
   if (o->use_pcg) return BundleAdjustPCG(h, o, res, static_cast<cudaStream_t>(stream));   // direct_ba.cc:436-457
   // direct_ba.cc:427-434
   const bool opt_depth_intr = o->optimize_depth_intrinsics && h->cfg.use_depth_residuals;
@@ -993,6 +1000,7 @@ bba_status bba_pcg_debug(bba_handle h, const bba_ba_options* o, int step, int ap
   if (K == 0) return Fail(h, BBA_ERR_STATE, "no keyframes");
   if (o->pcg_gauge_keyframe < 0 || o->pcg_gauge_keyframe >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "pcg_gauge_keyframe out of range");
   if (h->cfg.world_size > 1) return Fail(h, BBA_ERR_UNSUPPORTED, "bba_pcg_debug runs on one rank");
+  if (h->deterministic) return Fail(h, BBA_ERR_UNSUPPORTED, "bba_pcg_debug: the PCG solver is not available in the deterministic mode");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   PcgLayout L;
   if (bba_status st = MakePcgLayout(h, o, &L)) return st;

@@ -173,6 +173,11 @@ bba_status LaunchOdometryKernel(bba_handle h, const CameraView& cams, int num_sc
   std::memcpy(a.init1, init1, sizeof(float) * 7);
   std::memcpy(a.init2, init2, sizeof(float) * 7);
   a.acc = st.d_acc;
+  a.partials = nullptr;
+  if (cams.deterministic) {   // the snapshot's mode: fixed-order sums of per-CTA partials
+    BBA_CUDA(h, st.d_partials.Reserve(static_cast<size_t>(3) * 32 * od::TrackGrid(a, h->sm_count)));
+    a.partials = st.d_partials;
+  }
   a.barrier = st.d_barrier;
   a.result = st.d_result;
   BBA_CUDA(h, cudaMemsetAsync(st.d_acc, 0, sizeof(double) * 96, s));

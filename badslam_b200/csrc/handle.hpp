@@ -140,11 +140,12 @@ struct KeyframeView {
   int activation = BBA_KF_ACTIVE;
 };
 
-// The cameras, the depth deformation parameter a and the residual types as the BA side published them last.
+// The cameras, the depth deformation parameter a, the residual types and the deterministic mode as the BA side published them last.
 struct CameraView {
   float depth_K[4] = {}, color_K[4] = {};
   float depth_a = 0.f;
   int use_depth = 1, use_desc = 1;
+  int deterministic = 0;
 };
 
 // A u8 plane that luma extraction writes before the copy into a CUDA array, and the event after which the next user may
@@ -193,6 +194,7 @@ struct bba_context {
     bba::DeviceBuffer<bba::KfDevice> d_work_records;   // [max_kf] the pose kernel's work list as contiguous records
     bba::DeviceBuffer<float> d_pose_est;
     bba::DeviceBuffer<double> d_acc;
+    bba::DeviceBuffer<bba::ExactSum> d_exact;   // deterministic mode: [max_kf][32], the pose kernel's sums instead of d_acc
     bba::DeviceBuffer<unsigned long long> d_stage_counts;
     bba::DeviceBuffer<int> d_work[2];
     bba::DeviceBuffer<int> d_count;   // 2 ints
@@ -237,6 +239,7 @@ struct bba_context {
     // intrinsics step: [head 64 | B 5P | D P | b2 P | obs P | x1 8] floats + 34 fp64 sums
     bba::DeviceBuffer<float> d_intr;
     bba::DeviceBuffer<double> d_intr_sums;
+    bba::DeviceBuffer<bba::ExactSum> d_intr_exact;   // deterministic mode: [7 P] per-cell sums (B rows, D, b2) + kIntrinsicsSums
     bba::DeviceBuffer<int> d_all_list;   // 0 .. max_kf-1
     bba::PinnedBuffer<double> h_intr_sums;
     bba::PinnedBuffer<float> h_intr_x1;   // 8 floats
@@ -301,6 +304,7 @@ struct bba_context {
     int w[bba::odom::kMaxScales] = {}, h[bba::odom::kMaxScales] = {};
     bba::odom::Level level[bba::odom::kMaxScales] = {};      // as passed to the last launch
     bba::DeviceBuffer<double> d_acc;             // [3][32]
+    bba::DeviceBuffer<double> d_partials;        // deterministic mode: [3][grid][32] per-CTA totals (TrackArgs::partials)
     bba::DeviceBuffer<unsigned int> d_barrier;   // [2]
     bba::DeviceBuffer<bba::odom::TrackResult> d_result;
     bba::PinnedBuffer<bba::odom::TrackResult> h_result;
@@ -341,6 +345,9 @@ struct bba_context {
   // predicted cost of one pose step per keyframe (Gauss-Newton iterations x per-evaluation cost of the last step it took
   // part in); 0 = unknown.  Identical on every rank; drives the keyframe -> rank assignment of the pose step.
   std::vector<float> kf_cost;
+
+  // deterministic mode (bba_set_deterministic): exact or fixed-order sums on the pose, intrinsics and odometry paths
+  bool deterministic = false;
 
   // profiling (bba_set_profiling)
   int profiling = 0;   // 0 off, 1 event timing, 2 event timing + byte-model counters in every iteration

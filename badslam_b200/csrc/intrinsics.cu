@@ -25,7 +25,11 @@ constexpr int kTile = 256;
 }  // namespace
 
 // sums layout: [0..14] A upper triangle (5x5), [15..19] b1, [20..29] colour H upper triangle (4x4), [30..33] colour b
-template <bool OPT_COLOR, bool OPT_DEPTH>
+// DET (the deterministic mode): every fp32 atomic below except the observation count (an integer below 2^24, exact in any order)
+// becomes a deposit into an exact sum.  A cell's sums receive one deposit per associated pair that falls into it, a few per keyframe
+// and cell size squared (tens of thousands at cfg3), a global sum one per work item, at most ceil(n / 256) x ceil(K / 16): both far
+// below the 2^31 deposits an ExactSum holds.
+template <bool OPT_COLOR, bool OPT_DEPTH, bool DET>
 __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __grid_constant__ IntrinsicsArgs a) {
   const uint32_t n_tiles = (a.end - a.begin + kTile - 1) / kTile;
   const uint32_t n_groups = (a.kf_count + kGroup - 1) / kGroup;
@@ -100,10 +104,17 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
             for (int rr = 0; rr < 5; ++rr) acc[15 + rr] += wr * J[rr];
             // per-cell terms (kernel_opt_intrinsics.cu:173-190)
             const unsigned int sp = SparseCell(cam, r.px, r.py);
+            if constexpr (DET) {
 #pragma unroll
-            for (int rr = 0; rr < 5; ++rr) atomicAdd(a.cell_B + static_cast<size_t>(rr) * a.cell_count + sp, w * J[rr] * J[5]);
-            atomicAdd(a.cell_D + sp, w * J[5] * J[5]);
-            atomicAdd(a.cell_b2 + sp, w * raw * J[5]);
+              for (int rr = 0; rr < 5; ++rr) ExactDeposit(a.exact_cells + static_cast<size_t>(rr) * a.cell_count + sp, w * J[rr] * J[5]);
+              ExactDeposit(a.exact_cells + static_cast<size_t>(5) * a.cell_count + sp, w * J[5] * J[5]);
+              ExactDeposit(a.exact_cells + static_cast<size_t>(6) * a.cell_count + sp, w * raw * J[5]);
+            } else {
+#pragma unroll
+              for (int rr = 0; rr < 5; ++rr) atomicAdd(a.cell_B + static_cast<size_t>(rr) * a.cell_count + sp, w * J[rr] * J[5]);
+              atomicAdd(a.cell_D + sp, w * J[5] * J[5]);
+              atomicAdd(a.cell_b2 + sp, w * raw * J[5]);
+            }
             atomicAdd(a.cell_obs + sp, 1.0f);   // fp32 count: exact to 2^24, only tested against 0
           }
         }
@@ -128,13 +139,17 @@ __global__ void __launch_bounds__(kThreads) IntrinsicsAccumulateKernel(const __g
     }
     __syncwarp();
     const float total = WarpTransposeReduce(acc, lane);
-    if (total != 0.f) atomicAdd(a.sums + lane, static_cast<double>(total));
+    auto store = [&](int slot, float v) {
+      if constexpr (DET) ExactDeposit(a.exact_sums + slot, v);
+      else atomicAdd(a.sums + slot, static_cast<double>(v));
+    };
+    if (total != 0.f) store(lane, total);
     if (OPT_COLOR) {
       extra0 = WarpSum(extra0);
       extra1 = WarpSum(extra1);
       if (lane == 0 && (extra0 != 0.f || extra1 != 0.f)) {
-        atomicAdd(a.sums + 32, static_cast<double>(extra0));
-        atomicAdd(a.sums + 33, static_cast<double>(extra1));
+        store(32, extra0);
+        store(33, extra1);
       }
     }
   }
@@ -218,10 +233,28 @@ LaunchResult LaunchIntrinsicsAccumulate(const IntrinsicsArgs& a, int sm_count, b
     kernel<<<ItemGrid(per_sm, sm_count, n_items), kThreads, 0, stream>>>(a);
     r.kernels = 1;
   };
-  if (optimize_color && optimize_depth) launch(IntrinsicsAccumulateKernel<true, true>);
-  else if (optimize_color) launch(IntrinsicsAccumulateKernel<true, false>);
-  else if (optimize_depth) launch(IntrinsicsAccumulateKernel<false, true>);
+  const bool det = a.exact_cells != nullptr;
+  if (optimize_color && optimize_depth) det ? launch(IntrinsicsAccumulateKernel<true, true, true>) : launch(IntrinsicsAccumulateKernel<true, true, false>);
+  else if (optimize_color) det ? launch(IntrinsicsAccumulateKernel<true, false, true>) : launch(IntrinsicsAccumulateKernel<true, false, false>);
+  else if (optimize_depth) det ? launch(IntrinsicsAccumulateKernel<false, true, true>) : launch(IntrinsicsAccumulateKernel<false, true, false>);
   return r;
+}
+
+// One thread per value: the 7 cell rows (cell_B's 5, then cell_D and cell_b2, which follow it in memory) as fp32 of the rounded
+// exact sum, then the kIntrinsicsSums global sums in fp64.
+__global__ void __launch_bounds__(256) IntrinsicsFinalizeKernel(uint32_t cell_count, const ExactSum* __restrict__ exact_cells,
+                                                                float* __restrict__ cells, const ExactSum* __restrict__ exact_sums,
+                                                                double* __restrict__ sums) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const size_t n_cells = static_cast<size_t>(7) * cell_count;
+  if (i < n_cells) cells[i] = static_cast<float>(ExactFinalize(exact_cells[i]));
+  else if (i < n_cells + kIntrinsicsSums) sums[i - n_cells] = ExactFinalize(exact_sums[i - n_cells]);
+}
+LaunchResult LaunchIntrinsicsFinalize(uint32_t cell_count, const ExactSum* exact_cells, float* cell_B, const ExactSum* exact_sums, double* sums,
+                                      cudaStream_t stream) {
+  const size_t n = static_cast<size_t>(7) * cell_count + kIntrinsicsSums;
+  IntrinsicsFinalizeKernel<<<static_cast<unsigned int>((n + 255) / 256), 256, 0, stream>>>(cell_count, exact_cells, cell_B, exact_sums, sums);
+  return {1};
 }
 
 __global__ void IntrinsicsConvertSumsKernel(double* sums, float* head, int to_float) {

@@ -196,6 +196,16 @@ __device__ __forceinline__ void AccumulateRecord(const CameraParams& cam, const 
   AccumulatePair<STATS>(cam, r, e, rec[15 * 32] != 0.f, acc);
 }
 
+// Where a sub-item's warp total of slot `lane` goes: one fp64 atomic into acc, or (DET, the deterministic mode) a deposit into the
+// slot's exact sum, whose value does not depend on the order in which the sub-items finish.  A keyframe's slot receives one deposit
+// per sub-item, at most chunks per tile x tiles = ceil(n / 128) <= 2^25 for any surfel count below 2^32: far below the 2^31 deposits
+// an ExactSum holds.
+template <bool DET>
+__device__ __forceinline__ void StorePoseTotal(const PoseAccumulateArgs& args, int kf, int lane, float total) {
+  if constexpr (DET) ExactDeposit(args.exact + static_cast<size_t>(kf) * kPoseAccSize + lane, total);
+  else atomicAdd(args.acc + static_cast<size_t>(kf) * kPoseAccSize + lane, static_cast<double>(total));
+}
+
 // Work decomposition.  A work ITEM is (group of <= 8 keyframes from the work list) x (tile of TILE surfels); items are
 // handed out through a global counter in GROUP-MAJOR order, so at any moment all resident CTAs read the images of the
 // same 8-16 keyframes (~12-24 MB: stays in the H100's 50 MB L2) while surfel tiles stream through shared memory via TMA.
@@ -211,7 +221,9 @@ __device__ __forceinline__ void AccumulateRecord(const CameraParams& cam, const 
 // A sub-item's records are packed densely in surfel order into 32-pair batches; lane L of the consumer sums pair L of every
 // batch of the sub-item, with fresh sums, and reduces once at its last batch.  The fp32 partials therefore depend on the
 // sub-item alone, never on timing, and are the same with and without STATS.
-template <int TILE, bool STATS, bool PRE>
+// DET: the warp totals go to exact sums (StorePoseTotal); with the partials fixed by the sub-item, the result is then the same bits
+// in every run.
+template <int TILE, bool STATS, bool PRE, bool DET>
 __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinCtas)
     PoseAccumulateKernel(const __grid_constant__ PoseAccumulateArgs args) {
   constexpr int kRows = PRE ? kPoseStagedRowsPre : kPoseStagedRows;
@@ -326,8 +338,7 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
         MbarArrive(&batch_empty[p][b]);
         ++seq;
         if (h.y) {
-          const float total = WarpTransposeReduce(acc, lane);
-          atomicAdd(args.acc + static_cast<size_t>(h.z) * kPoseAccSize + lane, static_cast<double>(total));
+          StorePoseTotal<DET>(args, h.z, lane, WarpTransposeReduce(acc, lane));
 #pragma unroll
           for (int i = 0; i < kPoseAccSize; ++i) acc[i] = 0.f;
         }
@@ -476,8 +487,7 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
         batch_owned = false;
         batch_fill = 0;
       } else if (touched) {
-        const float total = WarpTransposeReduce(acc, lane);
-        atomicAdd(args.acc + static_cast<size_t>(kf) * kPoseAccSize + lane, static_cast<double>(total));
+        StorePoseTotal<DET>(args, kf, lane, WarpTransposeReduce(acc, lane));
       }
       if (STATS) {
         n_inimg = __reduce_add_sync(0xffffffffu, n_inimg);
@@ -524,8 +534,12 @@ static constexpr size_t PoseSmemBytes(int tile, bool pre) {
 template <int TILE, bool PRE>
 static cudaError_t SetPoseSmemLimit() {
   const int smem = static_cast<int>(PoseSmemBytes(TILE, PRE));
-  const cudaError_t e = cudaFuncSetAttribute(PoseAccumulateKernel<TILE, false, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  return e != cudaSuccess ? e : cudaFuncSetAttribute(PoseAccumulateKernel<TILE, true, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  for (const void* k : {reinterpret_cast<const void*>(PoseAccumulateKernel<TILE, false, PRE, false>),
+                        reinterpret_cast<const void*>(PoseAccumulateKernel<TILE, true, PRE, false>),
+                        reinterpret_cast<const void*>(PoseAccumulateKernel<TILE, false, PRE, true>),
+                        reinterpret_cast<const void*>(PoseAccumulateKernel<TILE, true, PRE, true>)})
+    if (const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) return e;
+  return cudaSuccess;
 }
 
 cudaError_t SetPoseAccumulateSmemLimits() {
@@ -538,7 +552,9 @@ cudaError_t SetPoseAccumulateSmemLimits() {
 template <int TILE, bool STATS, bool PRE>
 static void LaunchPoseAccumulateT(const PoseAccumulateArgs& args, int sm_count, cudaStream_t stream) {
   constexpr size_t smem = PoseSmemBytes(TILE, PRE);
-  PoseAccumulateKernel<TILE, STATS, PRE><<<kPoseMinCtas * sm_count, PRE ? kPoseWsThreads : kPoseThreads, smem, stream>>>(args);   // persistent
+  const dim3 grid(kPoseMinCtas * sm_count), block(PRE ? kPoseWsThreads : kPoseThreads);   // persistent
+  if (args.exact) PoseAccumulateKernel<TILE, STATS, PRE, true><<<grid, block, smem, stream>>>(args);
+  else PoseAccumulateKernel<TILE, STATS, PRE, false><<<grid, block, smem, stream>>>(args);
 }
 
 template <bool STATS>

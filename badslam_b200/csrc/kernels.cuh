@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include "device_math.cuh"
+#include "exact_sum.cuh"
 #include "launch.hpp"
 
 namespace bba {
@@ -30,6 +31,7 @@ struct PoseAccumulateArgs {
   KfDevice* work_records;   // [max_kf] scratch: the work list's KfDevice records in list order (pad = keyframe id), filled by
                              // LaunchPoseAccumulate so that a work group's <= 8 records are ONE contiguous bulk copy
   double* acc;               // [max_kf][32]
+  ExactSum* exact;           // deterministic mode: [max_kf][32] exact sums that take the warp totals instead of acc; else null
   unsigned long long* stage_counts;  // [max_kf][2]
   unsigned int* queue;       // global work-item counter, must be 0 at launch
 };
@@ -70,7 +72,8 @@ inline bool PoseVariantPre(int v) { return v == kPoseVariant256Pre || v == kPose
 // max_work: upper bound of *work_count known to the host (sizes the record-packing launch that precedes the kernel; both count).
 // variant = kPoseVariantAuto: the tile follows from args.n and the SM count, and args.stream != null selects the variant that
 // stages the sorted stream (and skips the chunks whose box lies outside a keyframe's view) instead of the caller's rows.  Any other
-// variant forces that instantiation; a PRE variant needs args.stream and args.boxes, the others ignore them.
+// variant forces that instantiation; a PRE variant needs args.stream and args.boxes, the others ignore them.  args.exact != null
+// selects the deterministic instantiation of the same variant.
 LaunchResult LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
                                   int variant = kPoseVariantAuto);
 // Sets the dynamic shared-memory limit of every instantiation of the pose kernel on the current device (once per handle).
@@ -80,6 +83,7 @@ struct PoseSolveArgs {
   KfDevice* kfs;
   float* pose_est;             // [max_kf][7] global_T_frame estimates, updated in place
   double* acc;                 // consumed and re-zeroed
+  ExactSum* exact;             // deterministic mode: consumed (rounded to fp64) and re-zeroed instead of acc; else null
   unsigned long long* stage_counts;
   const int* work_in;          // list consumed by this iteration
   const int* count_in;
@@ -182,8 +186,16 @@ struct IntrinsicsArgs {
   float* cell_b2;              // [cell_count]
   float* cell_obs;             // [cell_count] observation count (fp32 so that one sum all-reduce covers everything)
   uint32_t cell_count;
+  // deterministic mode: exact sums that take the per-cell terms ([7][cell_count]: B rows 0-4, D, b2) and the global sums
+  // ([kIntrinsicsSums]) instead of cell_B / cell_D / cell_b2 and sums (LaunchIntrinsicsFinalize rounds them); else null
+  ExactSum* exact_cells;
+  ExactSum* exact_sums;
 };
 LaunchResult LaunchIntrinsicsAccumulate(const IntrinsicsArgs& a, int sm_count, bool optimize_color, bool optimize_depth, cudaStream_t stream);
+// Deterministic mode: cell_B / cell_D / cell_b2 (contiguous, [7][cell_count]) <- fp32 of the exact cell sums and sums <- the exact
+// global sums, ahead of LaunchIntrinsicsSchur.
+LaunchResult LaunchIntrinsicsFinalize(uint32_t cell_count, const ExactSum* exact_cells, float* cell_B, const ExactSum* exact_sums, double* sums,
+                                      cudaStream_t stream);
 LaunchResult LaunchIntrinsicsSchur(uint32_t cell_count, float* B, float* D, const float* b2, double* sums, cudaStream_t stream);
 LaunchResult LaunchIntrinsicsConvertSums(double* sums, float* head, bool to_float, cudaStream_t stream);
 LaunchResult LaunchIntrinsicsCellUpdate(uint32_t cell_count, const float* obs, const float* B, const float* D, const float* x1,
@@ -302,6 +314,10 @@ LaunchResult LaunchMergeSurfels(const LifecycleArgs& a, int sm_count, cudaStream
 LaunchResult LaunchSeedNewSurfels(const LifecycleArgs& a, bool filter, cudaStream_t stream);    // a.flags after LaunchSupportSurfels
 LaunchResult LaunchExclusiveScan(const unsigned int* in, uint32_t n, unsigned int* out, unsigned int* block_sums, cudaStream_t stream);
 LaunchResult LaunchCreateSurfels(const LifecycleArgs& a, const unsigned int* index, cudaStream_t stream);
+
+// bba_debug_exact_sum: deposits the n values into *sum (zero at launch) from many CTAs, each visiting the values in a scrambled
+// order, and rounds the result into *out.
+LaunchResult LaunchExactSumDebug(const float* values, uint64_t n, ExactSum* sum, double* out, int sm_count, cudaStream_t stream);
 
 // uchar4 (.w = luma) -> u8 plane.
 LaunchResult LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream);

@@ -390,9 +390,12 @@ constexpr int kTrackThreads = 256;
 // One pass over the base image of a level: MODE 0 accumulates H, b, residual count and cost at pose T; MODE 1 evaluates residual
 // count and cost at the two poses TA and TB (ComputeCostAndResidualCountFromImagesCUDA twice, pairwise_frame_tracking.cc:433-475).
 // Slots: MODE 0: 0..20 H, 21..26 b, 27 count, 28 cost.  MODE 1: 0 count A, 1 cost A, 2 count B, 3 cost B.
-template <bool GRADMAG, int MODE>
+// DET (the deterministic mode): g_acc is the pass's [grid][32] partials buffer; every CTA stores its 32 totals, its warps' totals
+// summed in warp order, into its own row (SumPartials adds the rows in CTA order).  The tile partition is static, so every sum then
+// runs in the same order in every run.  s_warp: DET only, [8][32].
+template <bool GRADMAG, int MODE, bool DET>
 __device__ __forceinline__ void LevelPass(const TrackArgs& a, const Level& L, const float* TA, const float* TB, float threshold_factor,
-                                          double* s_acc, double* g_acc) {
+                                          double* s_acc, double* g_acc, double (*s_warp)[32]) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   float acc[32];
 #pragma unroll
@@ -434,6 +437,18 @@ __device__ __forceinline__ void LevelPass(const TrackArgs& a, const Level& L, co
       }
     }
   }
+  if constexpr (DET) {
+    const float total = __any_sync(0xffffffffu, any) ? WarpTransposeReduce(acc, lane) : 0.f;
+    __syncthreads();   // the previous pass's readers of s_warp are done
+    s_warp[warp][lane] = static_cast<double>(total);
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      double s = 0.0;
+      for (int w = 0; w < kTrackThreads / 32; ++w) s += s_warp[w][threadIdx.x];
+      __stcg(g_acc + blockIdx.x * 32 + threadIdx.x, s);
+    }
+    return;
+  }
   // warp -> CTA -> grid
   if (threadIdx.x < 32) s_acc[threadIdx.x] = 0.0;
   __syncthreads();
@@ -445,9 +460,27 @@ __device__ __forceinline__ void LevelPass(const TrackArgs& a, const Level& L, co
   if (threadIdx.x < 32 && s_acc[threadIdx.x] != 0.0) atomicAdd(g_acc + threadIdx.x, s_acc[threadIdx.x]);
 }
 
-template <bool GRADMAG>
+// DET: after a grid barrier, s_sum[j] = slot j of the pass's partials summed over the CTAs in CTA order (threads 0-31).
+__device__ __forceinline__ void SumPartials(const double* part, double* s_sum) {
+  if (threadIdx.x < 32) {
+    double s = 0.0;
+    for (unsigned int c = 0; c < gridDim.x; ++c) s += __ldcg(part + c * 32 + threadIdx.x);
+    s_sum[threadIdx.x] = s;
+  }
+  __syncthreads();
+}
+
+template <bool GRADMAG, bool DET>
 __global__ void __launch_bounds__(kTrackThreads, 1) OdomTrackKernel(const __grid_constant__ TrackArgs a) {
   __shared__ double s_acc[32];
+  __shared__ double s_warp[DET ? kTrackThreads / 32 : 1][32];
+  // The pass's accumulator buffer and the reads of its sums after the grid barrier: acc (fp64 atomics), or with DET the pass's
+  // partials and their ordered sums in s_acc.
+  auto pass_buffer = [&](unsigned int p) { return DET ? a.partials + (p % 3) * gridDim.x * 32 : a.acc + (p % 3) * 32; };
+  auto read_sums = [&](const double* g) {
+    if constexpr (DET) SumPartials(g, s_acc);
+  };
+  auto sum = [&](const double* g, int j) { return DET ? s_acc[j] : __ldcg(g + j); };
   __shared__ float s_T[2][12];   // frame_T_base of the current estimate (and of the second arm of a cost comparison)
   __shared__ int s_flag;
   // replicated per-CTA state, touched by thread 0 only
@@ -481,10 +514,19 @@ __global__ void __launch_bounds__(kTrackThreads, 1) OdomTrackKernel(const __grid
       set_matrix(1, load_pose(a.init2));
     }
     __syncthreads();
-    LevelPass<GRADMAG, 0>(a, L, s_T[0], s_T[0], threshold_factor, s_acc, a.acc);
-    LevelPass<GRADMAG, 1>(a, L, s_T[0], s_T[1], threshold_factor, s_acc, a.acc + 32);
+    LevelPass<GRADMAG, 0, DET>(a, L, s_T[0], s_T[0], threshold_factor, s_acc, pass_buffer(0), s_warp);
+    LevelPass<GRADMAG, 1, DET>(a, L, s_T[0], s_T[1], threshold_factor, s_acc, DET ? pass_buffer(1) : a.acc + 32, s_warp);
     GridBarrier(a.barrier, &a.result->barrier_timeout);
-    if (blockIdx.x == 0 && threadIdx.x < 36) a.result->debug[threadIdx.x] = __ldcg(a.acc + threadIdx.x);
+    if constexpr (DET) {
+      if (blockIdx.x != 0) return;
+      SumPartials(pass_buffer(0), s_acc);
+      if (threadIdx.x < 32) a.result->debug[threadIdx.x] = s_acc[threadIdx.x];
+      __syncthreads();
+      SumPartials(pass_buffer(1), s_acc);
+      if (threadIdx.x < 4) a.result->debug[32 + threadIdx.x] = s_acc[threadIdx.x];
+    } else if (blockIdx.x == 0 && threadIdx.x < 36) {
+      a.result->debug[threadIdx.x] = __ldcg(a.acc + threadIdx.x);
+    }
     return;
   }
 
@@ -504,13 +546,14 @@ __global__ void __launch_bounds__(kTrackThreads, 1) OdomTrackKernel(const __grid
         set_matrix(1, arm_b);
       }
       __syncthreads();
-      double* g = a.acc + (pass % 3) * 32;
-      LevelPass<GRADMAG, 1>(a, L, s_T[0], s_T[1], threshold_factor, s_acc, g);
+      double* g = pass_buffer(pass);
+      LevelPass<GRADMAG, 1, DET>(a, L, s_T[0], s_T[1], threshold_factor, s_acc, g, s_warp);
       next_buffer_clear();
       GridBarrier(a.barrier, &a.result->barrier_timeout);
+      read_sums(g);
       if (threadIdx.x == 0) {
-        const unsigned int count_a = static_cast<unsigned int>(__ldcg(g + 0) + 0.5), count_b = static_cast<unsigned int>(__ldcg(g + 2) + 0.5);
-        const float cost_a = static_cast<float>(__ldcg(g + 1)), cost_b = static_cast<float>(__ldcg(g + 3));
+        const unsigned int count_a = static_cast<unsigned int>(sum(g, 0) + 0.5), count_b = static_cast<unsigned int>(sum(g, 2) + 0.5);
+        const float cost_a = static_cast<float>(sum(g, 1)), cost_b = static_cast<float>(sum(g, 3));
         bool take_a;
         if (count_a > 2 * count_b) take_a = true;
         else if (count_b > 2 * count_a) take_a = false;
@@ -528,15 +571,16 @@ __global__ void __launch_bounds__(kTrackThreads, 1) OdomTrackKernel(const __grid
     for (; iteration < a.max_iterations;) {
       if (threadIdx.x == 0) set_matrix(0, est);
       __syncthreads();
-      double* g = a.acc + (pass % 3) * 32;
-      LevelPass<GRADMAG, 0>(a, L, s_T[0], s_T[0], threshold_factor, s_acc, g);
+      double* g = pass_buffer(pass);
+      LevelPass<GRADMAG, 0, DET>(a, L, s_T[0], s_T[0], threshold_factor, s_acc, g, s_warp);
       next_buffer_clear();
       GridBarrier(a.barrier, &a.result->barrier_timeout);
+      read_sums(g);
       if (threadIdx.x == 0) {
         // the reference's buffers are fp32 and are cast to double for the solve (pairwise_frame_tracking.cc:557-566)
         double H[21], b[6], xd[6];
-        for (int j = 0; j < 21; ++j) H[j] = static_cast<double>(static_cast<float>(__ldcg(g + j)));
-        for (int j = 0; j < 6; ++j) b[j] = static_cast<double>(static_cast<float>(__ldcg(g + 21 + j)));
+        for (int j = 0; j < 21; ++j) H[j] = static_cast<double>(static_cast<float>(sum(g, j)));
+        for (int j = 0; j < 6; ++j) b[j] = static_cast<double>(static_cast<float>(sum(g, 21 + j)));
         SolveLDLT<6>(H, b, xd);
         float x[6], step[6];
         // damping, pairwise_frame_tracking.cc:581-590
@@ -552,8 +596,8 @@ __global__ void __launch_bounds__(kTrackThreads, 1) OdomTrackKernel(const __grid
         const float sq = x[0] * x[0] + x[1] * x[1] + x[2] * x[2] + x[3] * x[3] + x[4] * x[4] + x[5] * x[5];
         s_flag = (sq < scaling_factor * scaling_factor * 1e-08f) ? 1 : 0;
         if (blockIdx.x == 0) {
-          a.result->residual_count = static_cast<unsigned int>(__ldcg(g + 27) + 0.5);
-          a.result->residual_sum = static_cast<float>(__ldcg(g + 28));
+          a.result->residual_count = static_cast<unsigned int>(sum(g, 27) + 0.5);
+          a.result->residual_sum = static_cast<float>(sum(g, 28));
         }
       }
       ++pass;
@@ -571,14 +615,19 @@ __global__ void __launch_bounds__(kTrackThreads, 1) OdomTrackKernel(const __grid
   }
 }
 
-LaunchResult LaunchTrack(const TrackArgs& a, int sm_count, cudaStream_t stream) {
-  // one CTA per SM (all co-resident: the grid barrier needs it), never more CTAs than the finest level has tiles
+int TrackGrid(const TrackArgs& a, int sm_count) {
   const Level& L0 = a.level[a.first_scale];
   const int tiles = ((L0.cam.w + 31) / 32) * ((L0.cam.h + 7) / 8);
-  const int grid = tiles < sm_count ? (tiles > 0 ? tiles : 1) : sm_count;
+  return tiles < sm_count ? (tiles > 0 ? tiles : 1) : sm_count;
+}
+
+LaunchResult LaunchTrack(const TrackArgs& a, int sm_count, cudaStream_t stream) {
+  // one CTA per SM (all co-resident: the grid barrier needs it), never more CTAs than the finest level has tiles
+  const int grid = TrackGrid(a, sm_count);
   // cooperative launch: the runtime guarantees that all CTAs are resident at the same time (or refuses the launch)
   void* params[] = {const_cast<TrackArgs*>(&a)};
-  void* kernel = a.use_gradmag ? reinterpret_cast<void*>(OdomTrackKernel<true>) : reinterpret_cast<void*>(OdomTrackKernel<false>);
+  void* kernel = a.partials ? (a.use_gradmag ? reinterpret_cast<void*>(OdomTrackKernel<true, true>) : reinterpret_cast<void*>(OdomTrackKernel<false, true>))
+                            : (a.use_gradmag ? reinterpret_cast<void*>(OdomTrackKernel<true, false>) : reinterpret_cast<void*>(OdomTrackKernel<false, false>));
   return {1, cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kTrackThreads), params, 0, stream)};
 }
 

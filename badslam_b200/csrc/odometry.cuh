@@ -108,9 +108,12 @@ struct TrackArgs {
   float baseline_fx;
   float init1[7], init2[7];    // base_T_frame initial estimates
   double* acc;                 // [3][32] rotating accumulators, zero at launch
+  double* partials;            // deterministic mode: [3][grid][32] per-CTA totals, summed in CTA order instead of acc; else null
   unsigned int* barrier;       // [2] {arrival count, generation}, zero at launch
   TrackResult* result;
 };
+// The grid: one CTA per SM, never more than the finest level has tiles (TrackArgs::partials holds 3 x 32 doubles per CTA).
+int TrackGrid(const TrackArgs& a, int sm_count);
 LaunchResult LaunchTrack(const TrackArgs& a, int sm_count, cudaStream_t stream);
 
 }  // namespace odom

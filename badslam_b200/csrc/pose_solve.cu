@@ -12,6 +12,8 @@
 
 namespace bba {
 
+// DET (the deterministic mode): the accumulator record is read from the keyframe's exact sums, rounded to fp64, instead of acc.
+template <bool DET>
 __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
   __shared__ int next_count;
   __shared__ unsigned long long tot[5];
@@ -22,6 +24,15 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
   for (int i = threadIdx.x; i < count; i += blockDim.x) {
     const int kf = a.work_in[i];
     double* acc = a.acc + static_cast<size_t>(kf) * kPoseAccSize;
+    double rounded[DET ? kPoseAccSize : 1];
+    if constexpr (DET) {
+      ExactSum* e = a.exact + static_cast<size_t>(kf) * kPoseAccSize;
+      for (int j = 0; j < kPoseAccSize; ++j) {
+        rounded[j] = ExactFinalize(e[j]);
+        e[j] = ExactSum{};
+      }
+      acc = rounded;
+    }
     // The reference's buffers are fp32 (PoseEstimationHelperBuffers, kernels.h:47-58); it casts to double for the
     // solve (direct_ba_alternating.cc:206).  Round to fp32 first to stay on its numerical path.
     double H[21], b[6], x[6];
@@ -82,7 +93,8 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
 }
 
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream) {
-  PoseSolveKernel<<<1, 256, 0, stream>>>(args);
+  if (args.exact) PoseSolveKernel<true><<<1, 256, 0, stream>>>(args);
+  else PoseSolveKernel<false><<<1, 256, 0, stream>>>(args);
   return {1};
 }
 

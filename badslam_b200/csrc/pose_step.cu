@@ -55,6 +55,7 @@ bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStre
   acc->kfs = h->d_kfs;
   acc->work_records = p.d_work_records;
   acc->acc = p.d_acc;
+  acc->exact = h->deterministic ? p.d_exact.get() : nullptr;
   acc->stage_counts = p.d_stage_counts;
   acc->queue = p.d_queue;
   acc->stream = nullptr;
@@ -99,6 +100,7 @@ bba_status StagePoseWork(bba_handle h, const std::vector<int>& ids, const std::v
   if (n) BBA_CUDA(h, cudaMemcpyAsync(p.d_work[0], p.h_work, sizeof(int) * n, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemcpyAsync(p.d_count, p.h_work + M, sizeof(int) * 2, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemsetAsync(p.d_acc, 0, sizeof(double) * kPoseAccSize * K, s));
+  if (h->deterministic) BBA_CUDA(h, cudaMemsetAsync(p.d_exact, 0, sizeof(ExactSum) * kPoseAccSize * K, s));
   BBA_CUDA(h, cudaMemsetAsync(p.d_stage_counts, 0, sizeof(unsigned long long) * 2 * K, s));
   BBA_CUDA(h, cudaMemsetAsync(p.d_queue, 0, sizeof(unsigned int), s));
   *n_work = n;
@@ -106,7 +108,8 @@ bba_status StagePoseWork(bba_handle h, const std::vector<int>& ids, const std::v
 }
 
 // One launch of the pose kernel for keyframes ids at poses; on return (stream synchronised) rec / sc hold every keyframe's
-// accumulator record and its two stage counts, and the device records are zero again.
+// accumulator record (in the deterministic mode its exact sums rounded to fp64) and its two stage counts, and the device records
+// are zero again.
 bba_status PoseCoeffsBatch(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& poses, int variant, bool with_stats,
                            cudaStream_t s, std::vector<double>* rec, std::vector<unsigned long long>* sc) {
   auto& p = h->pose;
@@ -120,12 +123,19 @@ bba_status PoseCoeffsBatch(bba_handle h, const std::vector<int>& ids, const std:
   BBA_LAUNCH(h, h->launches, LaunchPoseAccumulate, acc, h->sm_count, with_stats, count, s, variant);
   rec->resize(static_cast<size_t>(kPoseAccSize) * K);
   sc->resize(2 * static_cast<size_t>(K));
-  BBA_CUDA(h, cudaMemcpyAsync(rec->data(), p.d_acc, sizeof(double) * rec->size(), cudaMemcpyDeviceToHost, s));
+  std::vector<ExactSum> exact(h->deterministic ? rec->size() : 0);
+  if (h->deterministic) {
+    BBA_CUDA(h, cudaMemcpyAsync(exact.data(), p.d_exact, sizeof(ExactSum) * exact.size(), cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaMemsetAsync(p.d_exact, 0, sizeof(ExactSum) * exact.size(), s));
+  } else {
+    BBA_CUDA(h, cudaMemcpyAsync(rec->data(), p.d_acc, sizeof(double) * rec->size(), cudaMemcpyDeviceToHost, s));
+  }
   BBA_CUDA(h, cudaMemcpyAsync(sc->data(), p.d_stage_counts, sizeof(unsigned long long) * sc->size(), cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaMemsetAsync(p.d_acc, 0, sizeof(double) * rec->size(), s));
   BBA_CUDA(h, cudaMemsetAsync(p.d_stage_counts, 0, sizeof(unsigned long long) * sc->size(), s));
   BBA_CUDA(h, cudaStreamSynchronize(s));
   h->staging.pending = false;
+  for (size_t i = 0; i < exact.size(); ++i) (*rec)[i] = ExactFinalize(exact[i]);
   return BBA_OK;
 }
 
@@ -168,6 +178,7 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
   sol.kfs = h->d_kfs;
   sol.pose_est = p.d_pose_est;
   sol.acc = p.d_acc;
+  sol.exact = acc.exact;
   sol.stage_counts = p.d_stage_counts;
   sol.iterations = p.d_iterations;
   sol.converged = p.d_converged;

@@ -176,6 +176,15 @@ def deform_trajectory(start_frame: int, end_frame: int, keyframe_frame_indices, 
     return frame_poses
 
 
+
+def exact_sum(values) -> float:
+    """The exact sum of fp32 values rounded once to fp64 (bba_host_exact_sum, the accumulator of the deterministic mode): the
+    result does not depend on the order of the values."""
+    v = np.ascontiguousarray(values, np.float32).ravel()
+    out = C.c_double()
+    _lib.load().bba_host_exact_sum(v.ctypes.data, v.size, C.byref(out))
+    return out.value
+
 class DirectBA:
     """Drop-in for vis::DirectBA (direct_ba.h:65-550) backed by the sm_90a library."""
 
@@ -421,6 +430,25 @@ class DirectBA:
 
     def SetUseDescriptorResiduals(self, use_descriptor_residuals: bool):
         self._check(self._lib.bba_set_residual_types(self._h, int(self.use_depth_residuals()), int(use_descriptor_residuals)))
+
+    def deterministic(self) -> bool:
+        """Whether the deterministic mode is on (the published mode, bba_get_deterministic)."""
+        on = C.c_int()
+        self._check(self._lib.bba_get_deterministic(self._h, C.byref(on)))
+        return bool(on.value)
+
+    def SetDeterministic(self, on: bool):
+        """The deterministic mode (bba_set_deterministic): bitwise reproducible bundle adjustment, frame pose estimation and
+        odometry on one GPU, from the next call on.  Off by default."""
+        self._check(self._lib.bba_set_deterministic(self._h, int(on)))
+
+    def DebugExactSum(self, values: torch.Tensor, stream=None) -> float:
+        """Parity hook (bba_debug_exact_sum): the exact sum of a contiguous fp32 device tensor, deposited by many CTAs in a scrambled
+        order and rounded to fp64."""
+        assert values.dtype == torch.float32 and values.is_cuda and values.is_contiguous()
+        out = C.c_double()
+        self._check(self._lib.bba_debug_exact_sum(self._h, values.data_ptr(), values.numel(), C.byref(out), self._stream_ptr(stream)))
+        return out.value
 
     def SetA(self, a: float):
         d, c, _ = self._intrinsics()

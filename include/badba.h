@@ -502,6 +502,27 @@ bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, c
                                      float H[21], float b[6], uint32_t* residual_count, float* residual_sum,
                                      uint32_t counts[2], float costs[2], void* stream);
 
+/* ---- deterministic mode ----
+ * Off by default.  When on, every floating-point sum whose order depends on the scheduling of the GPU goes through an exact,
+ * order-independent accumulator (or, in the odometry kernel, a fixed-order sum of per-CTA totals), so that the same inputs on the
+ * same GPU model give the same results bit for bit in every run, whatever else runs beside them on other streams.  Covered:
+ * bba_bundle_adjust (pose, geometry and intrinsics steps, surfel lifecycle), bba_estimate_frame_pose (both forms),
+ * bba_accumulate_pose_coeffs, bba_debug_pose_coeffs_batch, bba_optimize_intrinsics, bba_track_frame_pairwise(_to_frame),
+ * bba_odometry_debug_coeffs and the preprocessing.  The results differ from those of the default mode only by the rounding of
+ * those sums.  Not covered: the PCG solver -- bba_bundle_adjust with use_pcg and bba_pcg_debug return BBA_ERR_UNSUPPORTED while
+ * the mode is on -- and more than one rank (the setter returns BBA_ERR_UNSUPPORTED for world_size > 1).  A call with
+ * time_limit_seconds > 0, or whose progress_function looks at the wall clock, is reproducible only up to the number of iterations
+ * it ran; the ms_* timings are measurements, not results.
+ * bba_set_deterministic is a BA-side call that takes effect from the next call and publishes; front-end calls use the mode of their
+ * snapshot.  Switching it on for the first time allocates the exact sums: 80 bytes per value, max_keyframes x 32 values for the
+ * pose kernel and 7 per sparse cell for the intrinsics step (about 11 MB at 640x480 with cell size 4).  bba_get_deterministic is a
+ * front-end call (the published mode). */
+bba_status bba_set_deterministic(bba_handle h, int on);
+bba_status bba_get_deterministic(bba_handle h, int* on);
+/* Parity hook for the exact accumulator: deposits the n (< 2^31) device values through the device path, from many CTAs in a
+ * scrambled order, and returns the sum rounded to fp64 (bba_host_exact_sum's result).  Synchronises the stream. */
+bba_status bba_debug_exact_sum(bba_handle h, const float* device_values, uint64_t n, double* out, void* stream);
+
 /* ---- host-side building blocks (no handle, no device) ----
  * The host arithmetic the backend runs between kernels, exported so that it can be checked without a GPU: Sophus'
  * SE3 exp / log / product / inverse on {qx,qy,qz,qw,tx,ty,tz} (se3.hpp:127-130,203-207,293-313,435-468), the convergence test of
@@ -517,6 +538,10 @@ int  bba_host_solve_ldlt(int n, const double* upper, const double* b, double* x)
 int  bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height,
                                const float global_T_frame_a[7], float min_depth_a, float max_depth_a,
                                const float global_T_frame_b[7], float min_depth_b, float max_depth_b);
+/* The exact accumulator of the deterministic mode on the host: the sum of n fp32 values, computed exactly and rounded once to
+ * fp64 (to nearest, ties to even), so the result does not depend on the order of the values.  An exact zero gives +0.0.  Non-finite
+ * values follow IEEE addition: NaN if there is a NaN or both infinities, else the infinity there is. */
+void bba_host_exact_sum(const float* values, size_t n, double* out);
 
 /* The constant-motion model in front of the image-pair odometry (BadSlam::PredictFramePose / RunOdometry / ClearMotionModel /
  * the rebase in BadSlam::ProcessFrame when a keyframe is created: bad_slam.cc:542-565, 767-827, 949-954, 1057-1068).  Host

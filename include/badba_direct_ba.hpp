@@ -337,6 +337,9 @@ class DirectBA {
   bool use_descriptor_residuals() const { int d = 0, c = 0; bba_get_residual_types(h_, &d, &c); return c != 0; }
   void SetUseDepthResiduals(bool v) { Check(bba_set_residual_types(h_, v, use_descriptor_residuals()), "bba_set_residual_types"); }
   void SetUseDescriptorResiduals(bool v) { Check(bba_set_residual_types(h_, use_depth_residuals(), v), "bba_set_residual_types"); }
+  // The deterministic mode (bba_set_deterministic): bitwise reproducible BA, frame pose estimation and odometry on one GPU.
+  void SetDeterministic(bool on) { Check(bba_set_deterministic(h_, on ? 1 : 0), "bba_set_deterministic"); }
+  bool deterministic() const { int on = 0; bba_get_deterministic(h_, &on); return on != 0; }
   const bba_ba_result& last_result() const { return last_result_; }
   bba_handle handle() const { return h_; }
 
