@@ -100,6 +100,11 @@ class PoseCoeffs(C.Structure):
                 ("cost_depth", C.c_double), ("cost_desc1", C.c_double), ("cost_desc2", C.c_double)]
 
 
+class FrameBuffers(C.Structure):   # bba_frame_buffers
+    _fields_ = [("depth", C.c_void_p), ("depth_pitch", C.c_size_t), ("normals", C.c_void_p), ("normals_pitch", C.c_size_t),
+                ("color_rgba", C.c_void_p), ("color_pitch", C.c_size_t)]
+
+
 class Profile(C.Structure):
     _fields_ = [("pose_launches", C.c_uint64), ("pose_ms", C.c_double), ("kf_evals", C.c_uint64),
                 ("n_pair", C.c_uint64), ("n_inimg", C.c_uint64), ("n_depthok", C.c_uint64),
@@ -160,6 +165,8 @@ SYMBOLS = {
     "bba_estimate_frame_pose": (C.c_int, [_P, C.c_int, _F7, _F7, C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_estimate_frame_pose_for_frame": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _F7, _F7,
                                                     C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
+    "bba_estimate_frame_poses_for_frames": (C.c_int, [_P, C.c_int, C.POINTER(FrameBuffers), C.c_int, _P, _P, _P, _P, _P,
+                                                      C.POINTER(PoseCoeffs), _P]),
     "bba_track_frame_pairwise": (C.c_int, [_P, C.POINTER(OdometryOptions), C.c_int, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
                                            _F7, _F7, _F7, C.POINTER(OdometryResult), _P]),
     "bba_track_frame_pairwise_to_frame": (C.c_int, [_P, C.POINTER(OdometryOptions), _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,

@@ -209,6 +209,23 @@ bba_status AcquireLumaStaging(bba_handle h, LumaStaging& staging, cudaStream_t s
   return BBA_OK;
 }
 
+// Creates the u8 array of *luma (colour-image sized, gather-enabled) and its texture where they do not exist yet.
+bba_status AllocateLumaTexture(bba_handle h, Texture* luma) {
+  if (!luma->array) {
+    const cudaChannelFormatDesc desc = cudaCreateChannelDesc(8, 0, 0, 0, cudaChannelFormatKindUnsigned);
+    BBA_CUDA(h, cudaMallocArray(&luma->array.r, &desc, h->cfg.color_width, h->cfg.color_height, cudaArrayTextureGather));
+  }
+  if (!luma->tex) {
+    cudaResourceDesc res;
+    std::memset(&res, 0, sizeof(res));
+    res.resType = cudaResourceTypeArray;
+    res.res.array.array = luma->array;
+    const cudaTextureDesc tex = LinearTextureDesc();
+    BBA_CUDA(h, cudaCreateTextureObject(&luma->tex.r, &res, &tex, nullptr));
+  }
+  return BBA_OK;
+}
+
 }  // namespace
 
 // The luma plane (the .w channel of a uchar4 image) as a gather-enabled CUDA array (block-linear: 2-D locality for the sample
@@ -220,22 +237,42 @@ bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t colo
   PitchedBuffer& plane = staging.plane;
   if (!plane) BBA_CUDA(h, plane.Allocate(cw, ch));
   if (bba_status st = AcquireLumaStaging(h, staging, s)) return st;
-  if (!luma->array) {
-    const cudaChannelFormatDesc desc = cudaCreateChannelDesc(8, 0, 0, 0, cudaChannelFormatKindUnsigned);
-    BBA_CUDA(h, cudaMallocArray(&luma->array.r, &desc, cw, ch, cudaArrayTextureGather));
-  }
+  if (bba_status st = AllocateLumaTexture(h, luma)) return st;
   BBA_LAUNCH(h, front_end ? h->front_end_launches : h->launches, LaunchExtractLuma, device_rgba, color_pitch, plane.get(), plane.pitch(),
              cw, ch, s);
   BBA_CUDA(h, cudaMemcpy2DToArrayAsync(luma->array, 0, 0, plane.get(), plane.pitch(), cw, ch, cudaMemcpyDeviceToDevice, s));
   BBA_CUDA(h, cudaEventRecord(staging.free, s));
-  if (!luma->tex) {
-    cudaResourceDesc res;
-    std::memset(&res, 0, sizeof(res));
-    res.resType = cudaResourceTypeArray;
-    res.res.array.array = luma->array;
-    const cudaTextureDesc tex = LinearTextureDesc();
-    BBA_CUDA(h, cudaCreateTextureObject(&luma->tex.r, &res, &tex, nullptr));
+  return BBA_OK;
+}
+
+bba_status MakeFrameLumaTextures(bba_handle h, int n, const uint8_t* const* rgba, const size_t* pitch, cudaStream_t s) {
+  const int cw = h->cfg.color_width, ch = h->cfg.color_height;
+  auto& f = h->frame_luma;
+  // the source table and the planes are rewritten below: the previous user's table upload, launch and copies must have run
+  if (f.stack.free) BBA_CUDA(h, cudaEventSynchronize(f.stack.free));
+  else BBA_CUDA(h, cudaEventCreateWithFlags(&f.stack.free.r, cudaEventDisableTiming));
+  if (f.stack_planes < n) {
+    f.stack_planes = 0;
+    BBA_CUDA(h, f.stack.plane.Allocate(cw, static_cast<size_t>(ch) * n));
+    f.stack_planes = n;
   }
+  BBA_CUDA(h, f.d_sources.Reserve(n));
+  BBA_CUDA(h, f.h_sources.Reserve(n));
+  while (static_cast<int>(f.pool.size()) < n) {
+    f.pool.emplace_back();
+    if (bba_status st = AllocateLumaTexture(h, &f.pool.back())) {
+      f.pool.pop_back();
+      return st;
+    }
+  }
+  for (int i = 0; i < n; ++i) f.h_sources[i] = LumaSource{rgba[i], pitch[i]};
+  BBA_CUDA(h, cudaMemcpyAsync(f.d_sources, f.h_sources, sizeof(LumaSource) * n, cudaMemcpyHostToDevice, s));
+  const size_t plane_pitch = f.stack.plane.pitch();
+  BBA_LAUNCH(h, h->launches, LaunchExtractLumaStack, f.d_sources, n, f.stack.plane.get(), plane_pitch, cw, ch, s);
+  for (int i = 0; i < n; ++i)
+    BBA_CUDA(h, cudaMemcpy2DToArrayAsync(f.pool[i].array, 0, 0, f.stack.plane.get() + static_cast<size_t>(i) * ch * plane_pitch,
+                                         plane_pitch, cw, ch, cudaMemcpyDeviceToDevice, s));
+  BBA_CUDA(h, cudaEventRecord(f.stack.free, s));
   return BBA_OK;
 }
 

@@ -186,8 +186,18 @@ struct bba_context {
     bool pending = false;
     bba::LumaStaging luma;      // u8 plane staging for the luma arrays of the BA side; the next user (any stream) waits on .free
     bba::PitchedBuffer color;   // uchar4 staging image for bba_update_keyframe_host
-    bba::Texture scratch;       // luma array + texture of a frame that is not a keyframe (frame pose, odometry)
   } staging;
+
+  // Luma of the frames that are not keyframes (bba_estimate_frame_poses_for_frames, pose_step.cu): one array + texture per
+  // distinct frame of a chunk, allocated on first use and trimmed to the free keyframe slots at the start of a call; the u8
+  // planes of a chunk's frames stacked in one image and the source table of the stacked extraction (MakeFrameLumaTextures).
+  struct FrameLuma {
+    std::vector<bba::Texture> pool;
+    bba::LumaStaging stack;   // .free: recorded after the last copy out of the planes (the source table is read before it)
+    int stack_planes = 0;     // planes the stack holds
+    bba::DeviceBuffer<bba::LumaSource> d_sources;
+    bba::PinnedBuffer<bba::LumaSource> h_sources;
+  } frame_luma;
 
   // pose step (pose_step.cu) and the spatial order of the surfels
   struct PoseStep {
@@ -443,6 +453,9 @@ template <class Args> void SetSurfelFields(bba_handle h, Args* a) {
 // front_end: through the front end's staging plane, counted as a front-end launch.
 bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t color_pitch, Texture* luma, cudaStream_t s,
                            bool front_end = false);
+// The luma textures of n colour images (rgba[i] with pitch[i]) in h->frame_luma.pool[0, n): one stacked extraction launch and one
+// copy per image into its array.  Grows the pool to n entries (never beyond what the caller asks for).
+bba_status MakeFrameLumaTextures(bba_handle h, int n, const uint8_t* const* rgba, const size_t* pitch, cudaStream_t s);
 
 // pose_step.cu
 // The surfel count from which a launch over n keyframes puts the surfels into spatial order: sorting costs ~0.1 ms of launches

@@ -1018,12 +1018,22 @@ LaunchResult LaunchPackPoseResults(const int* ids, int n, const float* pose_est,
 
 // ------------------------------------------------------------------------------------------------
 // uchar4 (.w = luma, cuda_image_processing.cu:165-176) -> dense u8 luma plane.  128-bit loads: 4 pixels per thread.
+// kStack: grid.z = frame; frame z reads stack[z] and writes rows [z * h, (z + 1) * h) of the luma planes (rgba / rgba_pitch are
+// unused).  Without it the kernel is the one-image case, and `stack` is an unused trailing argument that leaves its code alone.
 
+template <bool kStack>
 __global__ void __launch_bounds__(256) ExtractLumaKernel(const uint8_t* __restrict__ rgba, size_t rgba_pitch,
-                                                         uint8_t* __restrict__ luma, size_t luma_pitch, int w, int h) {
+                                                         uint8_t* __restrict__ luma, size_t luma_pitch, int w, int h,
+                                                         const LumaSource* __restrict__ stack) {
   const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   const int y = blockIdx.y;
   if (x4 >= w || y >= h) return;
+  if (kStack) {
+    const LumaSource f = stack[blockIdx.z];
+    rgba = f.rgba;
+    rgba_pitch = f.pitch;
+    luma += static_cast<size_t>(blockIdx.z) * h * luma_pitch;
+  }
   const uint8_t* src = rgba + static_cast<size_t>(y) * rgba_pitch + static_cast<size_t>(x4) * 4;
   uint8_t* dst = luma + static_cast<size_t>(y) * luma_pitch + x4;
   if (x4 + 3 < w && (reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
@@ -1038,7 +1048,17 @@ __global__ void __launch_bounds__(256) ExtractLumaKernel(const uint8_t* __restri
 LaunchResult LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream) {
   dim3 block(256);
   dim3 grid((w / 4 + 255) / 256 + 1, h);
-  ExtractLumaKernel<<<grid, block, 0, stream>>>(rgba, rgba_pitch, luma, luma_pitch, w, h);
+  ExtractLumaKernel<false><<<grid, block, 0, stream>>>(rgba, rgba_pitch, luma, luma_pitch, w, h, nullptr);
+  return {1};
+}
+
+LaunchResult LaunchExtractLumaStack(const LumaSource* sources, int frames, uint8_t* luma, size_t luma_pitch, int w, int h,
+                                    cudaStream_t stream) {
+  if (frames <= 0) return {};
+  if (frames > 65535) return {0, cudaErrorInvalidValue};   // grid.z
+  dim3 block(256);
+  dim3 grid((w / 4 + 255) / 256 + 1, h, frames);
+  ExtractLumaKernel<true><<<grid, block, 0, stream>>>(nullptr, 0, luma, luma_pitch, w, h, sources);
   return {1};
 }
 

@@ -321,5 +321,12 @@ LaunchResult LaunchExactSumDebug(const float* values, uint64_t n, ExactSum* sum,
 
 // uchar4 (.w = luma) -> u8 plane.
 LaunchResult LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream);
+// The same for `frames` images in one launch: image f (sources[f], device memory) -> rows [f * h, (f + 1) * h) of luma.
+struct LumaSource {
+  const uint8_t* rgba;
+  size_t pitch;
+};
+LaunchResult LaunchExtractLumaStack(const LumaSource* sources, int frames, uint8_t* luma, size_t luma_pitch, int w, int h,
+                                    cudaStream_t stream);
 
 }  // namespace bba

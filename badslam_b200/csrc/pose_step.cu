@@ -49,7 +49,10 @@ namespace {
 // put into spatial order with a bounding box per chunk, so that the kernel skips whole chunks outside a keyframe's view.  Not
 // worth a launch + 14 rows of traffic for a handful of keyframes (frame tracking): the kernel then derives the frames per pair.
 // variant = kPoseVariantAuto: that choice, from the number of keyframes n_work; any other: forced (bba_debug_pose_coeffs_batch).
-bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStream_t s, PoseAccumulateArgs* acc) {
+// stream_current: the last pose step built the stream for the same surfels and the same choice, and nothing has changed the
+// surfels since; it is used as it is.
+bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStream_t s, PoseAccumulateArgs* acc,
+                                 bool stream_current = false) {
   auto& p = h->pose;
   SetSurfelFields(h, acc);
   acc->kfs = h->d_kfs;
@@ -62,7 +65,11 @@ bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStre
   acc->stream_pitch = 0;
   acc->boxes = nullptr;
   const bool pre = variant == kPoseVariantAuto ? h->cfg.use_descriptor_residuals && n_work >= 4 : PoseVariantPre(variant);
-  if (pre && h->surfels_size > 0) {
+  if (pre && h->surfels_size > 0 && stream_current) {
+    acc->stream = p.order.stream;
+    acc->stream_pitch = p.order.capacity;
+    acc->boxes = p.order.boxes;
+  } else if (pre && h->surfels_size > 0) {
     // The rebuild (bounds, keys, radix sort) has a fixed cost of ~0.1 ms, most of it launch overhead at the start of a pose step
     // whose stream has just drained: measured on cfg2 (20 keyframes x 200 k surfels) it cost more than the culling it buys, on
     // cfg3_rank8 (200 x 375 k) it paid for itself many times over.  Below kSpatialOrderMinPairs (surfel, keyframe) pairs per
@@ -109,15 +116,15 @@ bba_status StagePoseWork(bba_handle h, const std::vector<int>& ids, const std::v
 
 // One launch of the pose kernel for keyframes ids at poses; on return (stream synchronised) rec / sc hold every keyframe's
 // accumulator record (in the deterministic mode its exact sums rounded to fp64) and its two stage counts, and the device records
-// are zero again.
+// are zero again.  stream_current: see PreparePoseAccumulate.
 bba_status PoseCoeffsBatch(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& poses, int variant, bool with_stats,
-                           cudaStream_t s, std::vector<double>* rec, std::vector<unsigned long long>* sc) {
+                           cudaStream_t s, std::vector<double>* rec, std::vector<unsigned long long>* sc, bool stream_current = false) {
   auto& p = h->pose;
   const int K = static_cast<int>(h->keyframes.size());
   int count = 0;
   if (bba_status st = StagePoseWork(h, ids, poses, nullptr, s, &count)) return st;
   PoseAccumulateArgs acc;
-  if (bba_status st = PreparePoseAccumulate(h, count, variant, s, &acc)) return st;
+  if (bba_status st = PreparePoseAccumulate(h, count, variant, s, &acc, stream_current)) return st;
   acc.work_list = p.d_work[0];
   acc.work_count = p.d_count;
   BBA_LAUNCH(h, h->launches, LaunchPoseAccumulate, acc, h->sm_count, with_stats, count, s, variant);
@@ -144,6 +151,97 @@ void FramePoseResult(bba_handle h, int id, float out[7], int* iterations, int* c
   std::memcpy(out, h->pose.h_pose_est + 7 * id, sizeof(float) * 7);
   if (iterations) *iterations = h->pose.h_iterations[id];
   if (converged) *converged = h->pose.h_converged[id];
+}
+
+// Keyframe slot id's coefficients out of what PoseCoeffsBatch read back (with stats).
+void FillPoseCoeffs(bba_handle h, const std::vector<double>& rec, const std::vector<unsigned long long>& sc, int id, bba_pose_coeffs* out) {
+  const double* r = rec.data() + static_cast<size_t>(id) * kPoseAccSize;
+  for (int i = 0; i < 21; ++i) out->H[i] = static_cast<float>(r[i]);
+  for (int i = 0; i < 6; ++i) out->b[i] = static_cast<float>(r[21 + i]);
+  out->n_pair = h->surfels_size;
+  out->n_inimg = sc[2 * id];
+  out->n_depthok = sc[2 * id + 1];
+  out->n_assoc = static_cast<uint64_t>(r[27] + 0.5);
+  out->n_photo = static_cast<uint64_t>(r[28] + 0.5);
+  out->cost_depth = r[29];
+  out->cost_desc1 = r[30];
+  out->cost_desc2 = r[31];
+}
+
+// Frame-to-model pose estimation (EstimateFramePose) of `count` entries, entry i = frame frame_of_entry[i] (i without the map)
+// from init[i]; the arguments are valid.  The entries ride through the pose step as temporary entries behind the keyframes, in
+// chunks of as many entries as there are free keyframe slots, in entry order: each chunk's distinct frames get a luma texture of
+// the pool (one stacked extraction launch), then one pose step runs every entry's Gauss-Newton loop and, with at_estimate, one more
+// pose-kernel launch with stats evaluates every entry at its result.  The temporary entries take part in nothing else (no
+// co-visibility, no activation state), own nothing and are removed before the next chunk; their slots' cost statistics are reset.
+// Serves both entry points: bba_estimate_frame_pose_for_frame is the one-entry, one-frame case.
+bba_status EstimateFramePoses(bba_handle h, int frame_count, const bba_frame_buffers* frames, int count, const int* frame_of_entry,
+                              const float* init, float* out, int* iterations, int* converged, bba_pose_coeffs* at_estimate,
+                              cudaStream_t s, const char* fn) {
+  const int K = static_cast<int>(h->keyframes.size());
+  const int free_slots = h->cfg.max_keyframes - K;
+  if (free_slots < 1) return Fail(h, BBA_ERR_STATE, std::string(fn) + " needs one free keyframe slot (max_keyframes reached)");
+  auto& luma = h->frame_luma;
+  if (static_cast<int>(luma.pool.size()) > free_slots) luma.pool.resize(free_slots);
+  if (luma.stack_planes > free_slots) {
+    luma.stack.plane = PitchedBuffer();
+    luma.stack_planes = 0;
+  }
+  std::vector<int> pool_entry(frame_count, -1);   // a frame's luma texture in the current chunk
+  std::vector<int> chunk_frames;
+  std::vector<const uint8_t*> rgba;
+  std::vector<size_t> pitch;
+  std::vector<int> ids;
+  std::vector<Pose> poses;
+  std::vector<double> rec;
+  std::vector<unsigned long long> sc;
+  for (int begin = 0; begin < count; begin += free_slots) {
+    const int n = std::min(free_slots, count - begin);
+    chunk_frames.clear();
+    rgba.clear();
+    pitch.clear();
+    for (int i = 0; i < n; ++i) {
+      const int f = frame_of_entry ? frame_of_entry[begin + i] : begin + i;
+      if (pool_entry[f] >= 0) continue;
+      pool_entry[f] = static_cast<int>(chunk_frames.size());
+      chunk_frames.push_back(f);
+      rgba.push_back(frames[f].color_rgba);
+      pitch.push_back(frames[f].color_pitch);
+    }
+    bba_status st = MakeFrameLumaTextures(h, static_cast<int>(chunk_frames.size()), rgba.data(), pitch.data(), s);
+    ids.resize(n);
+    poses.resize(n);
+    for (int i = 0; st == BBA_OK && i < n; ++i) {
+      const int f = frame_of_entry ? frame_of_entry[begin + i] : begin + i;
+      Keyframe entry{};
+      entry.depth = frames[f].depth; entry.depth_pitch = frames[f].depth_pitch;
+      entry.normals = frames[f].normals; entry.normals_pitch = frames[f].normals_pitch;
+      entry.tex = luma.pool[pool_entry[f]].tex;
+      entry.pose = PoseFromArray(init + 7 * static_cast<size_t>(begin + i));
+      entry.activation = BBA_KF_ACTIVE;
+      ids[i] = K + i;
+      poses[i] = entry.pose;
+      h->keyframes.push_back(std::move(entry));
+    }
+    if (st == BBA_OK) st = RunPoseStep(h, ids, poses, 30, s);
+    if (st == BBA_OK) {
+      for (int i = 0; i < n; ++i) {
+        const size_t e = static_cast<size_t>(begin + i);
+        FramePoseResult(h, K + i, out + 7 * e, iterations ? iterations + e : nullptr, converged ? converged + e : nullptr);
+        poses[i] = PoseFromArray(out + 7 * e);
+      }
+      // the pose step's surfel stream is still current: same surfels, same entry count and so the same variant
+      if (at_estimate) st = PoseCoeffsBatch(h, ids, poses, kPoseVariantAuto, /*with_stats=*/true, s, &rec, &sc, /*stream_current=*/true);
+    }
+    h->keyframes.erase(h->keyframes.begin() + K, h->keyframes.end());
+    for (int i = 0; i < n; ++i)   // the slots' cost statistics belong to future keyframes
+      if (K + i < static_cast<int>(h->kf_cost.size())) h->kf_cost[K + i] = 0.f;
+    for (int f : chunk_frames) pool_entry[f] = -1;
+    if (st) return st;
+    if (at_estimate)
+      for (int i = 0; i < n; ++i) FillPoseCoeffs(h, rec, sc, K + i, at_estimate + begin + i);
+  }
+  return BBA_OK;
 }
 
 }  // namespace
@@ -289,17 +387,7 @@ bba_status bba_accumulate_pose_coeffs(bba_handle h, int id, const float pose[7],
   if (bba_status st = PoseCoeffsBatch(h, std::vector<int>(1, id), std::vector<Pose>(1, PoseFromArray(pose)), kPoseVariantAuto,
                                       /*with_stats=*/true, static_cast<cudaStream_t>(stream), &rec, &sc))
     return st;
-  const double* r = rec.data() + static_cast<size_t>(id) * kPoseAccSize;
-  for (int i = 0; i < 21; ++i) out->H[i] = static_cast<float>(r[i]);
-  for (int i = 0; i < 6; ++i) out->b[i] = static_cast<float>(r[21 + i]);
-  out->n_pair = h->surfels_size;
-  out->n_inimg = sc[2 * id];
-  out->n_depthok = sc[2 * id + 1];
-  out->n_assoc = static_cast<uint64_t>(r[27] + 0.5);
-  out->n_photo = static_cast<uint64_t>(r[28] + 0.5);
-  out->cost_depth = r[29];
-  out->cost_desc1 = r[30];
-  out->cost_desc2 = r[31];
+  FillPoseCoeffs(h, rec, sc, id, out);
   return BBA_OK;
 }
 
@@ -360,28 +448,33 @@ bba_status bba_estimate_frame_pose_for_frame(bba_handle h, const uint16_t* devic
   if (!h || !device_depth || !device_normals || !device_color_rgba || !init || !out) return BBA_ERR_INVALID_ARGUMENT;
   if (!FramePitchesOk(h, depth_pitch, normals_pitch, color_pitch)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "frame buffer pitch too small");
   if (bba_status st = CheckSurfels(h)) return st;
-  const int id = static_cast<int>(h->keyframes.size());
-  if (id >= h->cfg.max_keyframes)
-    return Fail(h, BBA_ERR_STATE, "bba_estimate_frame_pose_for_frame needs one free keyframe slot (max_keyframes reached)");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (bba_status st = MakeLumaTexture(h, device_color_rgba, color_pitch, &h->staging.scratch, s)) return st;
-  // The frame rides through the pose step as a temporary entry behind the keyframes: it takes part in nothing else
-  // (no co-visibility, no activation state), borrows the scratch texture, owns nothing and is removed again before the call returns.
-  Keyframe frame{};
-  frame.depth = device_depth; frame.depth_pitch = depth_pitch;
-  frame.normals = device_normals; frame.normals_pitch = normals_pitch;
-  frame.tex = h->staging.scratch.tex;
-  frame.pose = PoseFromArray(init);
-  frame.activation = BBA_KF_ACTIVE;
-  h->keyframes.push_back(std::move(frame));
-  std::vector<int> ids(1, id);
-  std::vector<Pose> poses(1, PoseFromArray(init));
-  const bba_status st = RunPoseStep(h, ids, poses, 30, s);
-  h->keyframes.pop_back();
-  if (id < static_cast<int>(h->kf_cost.size())) h->kf_cost[id] = 0.f;   // the slot's cost statistics belong to a future keyframe
-  if (st) return st;
-  FramePoseResult(h, id, out, iterations, converged);
-  return BBA_OK;
+  const bba_frame_buffers frame{device_depth, depth_pitch, device_normals, normals_pitch, device_color_rgba, color_pitch};
+  return EstimateFramePoses(h, 1, &frame, 1, nullptr, init, out, iterations, converged, nullptr, static_cast<cudaStream_t>(stream),
+                            "bba_estimate_frame_pose_for_frame");
+}
+
+bba_status bba_estimate_frame_poses_for_frames(bba_handle h, int frame_count, const bba_frame_buffers* frames, int count,
+                                               const int* frame_of_entry, const float* global_T_frame_initial,
+                                               float* global_T_frame_estimate, int* iterations, int* converged,
+                                               bba_pose_coeffs* at_estimate, void* stream) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_estimate_frame_poses_for_frames: ";
+  if (!frames || !global_T_frame_initial || !global_T_frame_estimate) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  if (count < 1 || frame_count < 1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count and frame_count must be at least 1");
+  if (!frame_of_entry && count > frame_count)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "without frame_of_entry entry i uses frame i: count > frame_count");
+  for (int f = 0; f < frame_count; ++f) {
+    const bba_frame_buffers& b = frames[f];
+    if (!b.depth || !b.normals || !b.color_rgba) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null frame buffer");
+    if (!FramePitchesOk(h, b.depth_pitch, b.normals_pitch, b.color_pitch))
+      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "frame buffer pitch too small");
+  }
+  for (int i = 0; frame_of_entry && i < count; ++i)
+    if (frame_of_entry[i] < 0 || frame_of_entry[i] >= frame_count) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "frame index out of range");
+  if (h->cfg.world_size > 1) return Fail(h, BBA_ERR_UNSUPPORTED, fn + "runs on one rank only (world_size > 1)");
+  if (bba_status st = CheckSurfels(h)) return st;
+  return EstimateFramePoses(h, frame_count, frames, count, frame_of_entry, global_T_frame_initial, global_T_frame_estimate, iterations,
+                            converged, at_estimate, static_cast<cudaStream_t>(stream), "bba_estimate_frame_poses_for_frames");
 }
 
 }  // extern "C"

@@ -580,6 +580,31 @@ class DirectBA:
             out.ctypes.data_as(C.POINTER(C.c_float)), C.byref(it), C.byref(conv), self._stream_ptr(stream)))
         return out, it.value, bool(conv.value)
 
+    def EstimateFramePosesFromBuffers(self, stream, frames, initial_poses, frame_of_entry=None, with_coeffs: bool = False):
+        """EstimateFramePoseFromBuffers for many entries in one call (bba_estimate_frame_poses_for_frames).  frames: a sequence of
+        (depth, normals, colour) device tensors as EstimateFramePoseFromBuffers takes them; initial_poses: [count, 7]
+        global_T_frame starts, entry i tracking frames[frame_of_entry[i]] (frames[i] without frame_of_entry).  Returns
+        (global_T_frame_estimates [count, 7], iterations [count], converged [count] bool) and, with with_coeffs, a list of the
+        count PoseCoeffs at the returned poses as a fourth element.  The entries run in chunks of as many as there are free
+        keyframe slots."""
+        bufs = (_lib.FrameBuffers * len(frames))()
+        for b, (depth, normals, color) in zip(bufs, frames):
+            b.depth, b.depth_pitch = depth.data_ptr(), depth.stride(0) * 2
+            b.normals, b.normals_pitch = normals.data_ptr(), normals.stride(0) * 2
+            b.color_rgba, b.color_pitch = color.data_ptr(), color.stride(0)
+        init = np.ascontiguousarray(initial_poses, np.float32).reshape(-1, 7)
+        count = len(init)
+        fmap = None if frame_of_entry is None else np.ascontiguousarray(frame_of_entry, np.int32)
+        out = np.zeros((count, 7), np.float32)
+        it, conv = np.zeros(count, np.int32), np.zeros(count, np.int32)
+        coeffs = (_lib.PoseCoeffs * count)() if with_coeffs else None
+        self._check(self._lib.bba_estimate_frame_poses_for_frames(
+            self._h, len(frames), bufs, count, None if fmap is None else fmap.ctypes.data, init.ctypes.data, out.ctypes.data,
+            it.ctypes.data, conv.ctypes.data, coeffs, self._stream_ptr(stream)))
+        if with_coeffs:
+            return out, it, conv.astype(bool), list(coeffs)
+        return out, it, conv.astype(bool)
+
     def TrackFramePairwise(self, stream, base_keyframe_id: int, depth_buffer: torch.Tensor, normals_buffer: torch.Tensor,
                            color_buffer: torch.Tensor, base_T_frame_initial_estimate_1, base_T_frame_initial_estimate_2=None,
                            num_scales: int = 5, use_pyramid_level_0: bool = True, use_gradmag: bool = False,

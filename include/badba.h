@@ -258,6 +258,33 @@ bba_status bba_estimate_frame_pose_for_frame(bba_handle h, const uint16_t* devic
                                              const uint8_t* device_color_rgba, size_t color_pitch,
                                              const float global_T_frame_initial[7], float global_T_frame_estimate[7],
                                              int* iterations, int* converged, void* stream);
+/* The device buffers of a frame that is not a keyframe, as bba_estimate_frame_pose_for_frame takes them. */
+typedef struct {
+  const uint16_t* depth;      size_t depth_pitch;
+  const uint16_t* normals;    size_t normals_pitch;
+  const uint8_t*  color_rgba; size_t color_pitch;   /* uchar4, .w = luma */
+} bba_frame_buffers;
+/* bba_estimate_frame_pose_for_frame for many entries in one call.  An entry is one (frame, initial pose) pair: entry i tracks
+ * frames[frame_of_entry[i]] (frames[i] when frame_of_entry is NULL) from global_T_frame_initial[i] ([count][7]) against the
+ * current surfels, with the Gauss-Newton loop, iteration limit (30) and convergence test of the single-frame call, and writes
+ * global_T_frame_estimate[i] ([count][7]), iterations[i] and converged[i] (either array may be NULL).  A frame may appear in
+ * several entries: several initial poses for one frame (relocalisation hypotheses), or one pose per frame of a trajectory.
+ * With at_estimate ([count], may be NULL) entry i also gets what bba_accumulate_pose_coeffs returns at its returned pose -- H, b,
+ * the stage counts and the costs -- to rank hypotheses by association count or cost; that costs one more pose-kernel launch per
+ * chunk.
+ * The entries ride through the pose step as temporary entries behind the keyframes, in chunks of at most
+ * max_keyframes - keyframe_count entries, in entry order: one chunk runs one luma extraction launch for its distinct frames and
+ * one pose step for all its entries.  With no free keyframe slot the call returns BBA_ERR_STATE; nothing is reallocated on the
+ * pose path.  The frames' luma textures come from a library-owned pool, allocated on first use and never larger than the number
+ * of free slots.  When the call returns the handle is as it was (keyframes, poses, activations, co-visibility, surfels); only the
+ * spatial order of the surfels may have been rebuilt.  BBA_ERR_INVALID_ARGUMENT: a NULL array, count or frame_count < 1, a frame
+ * index out of range (or count > frame_count without frame_of_entry), a NULL frame buffer or a pitch too small; BBA_ERR_UNSUPPORTED:
+ * world_size > 1.  Arguments are checked before anything is enqueued, and a failed check leaves the handle unchanged.  A BA-side
+ * call; synchronises the stream. */
+bba_status bba_estimate_frame_poses_for_frames(bba_handle h, int frame_count, const bba_frame_buffers* frames, int count,
+                                               const int* frame_of_entry, const float* global_T_frame_initial,
+                                               float* global_T_frame_estimate, int* iterations, int* converged,
+                                               bba_pose_coeffs* at_estimate, void* stream);
 /* UpdateSurfelActivationCUDA (kernels.h:262-269, kernel_surfel_activation.cc:39-67) */
 bba_status bba_update_surfel_activation(bba_handle h, void* stream);
 /* OptimizeGeometryIterationCUDA (kernels.h:234-244, kernel_opt_geometry.cc:80-201) */
@@ -507,7 +534,7 @@ bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, c
  * order-independent accumulator (or, in the odometry kernel, a fixed-order sum of per-CTA totals), so that the same inputs on the
  * same GPU model give the same results bit for bit in every run, whatever else runs beside them on other streams.  Covered:
  * bba_bundle_adjust (pose, geometry and intrinsics steps, surfel lifecycle), bba_estimate_frame_pose (both forms),
- * bba_accumulate_pose_coeffs, bba_debug_pose_coeffs_batch, bba_optimize_intrinsics, bba_track_frame_pairwise(_to_frame),
+ * bba_estimate_frame_poses_for_frames, bba_accumulate_pose_coeffs, bba_debug_pose_coeffs_batch, bba_optimize_intrinsics, bba_track_frame_pairwise(_to_frame),
  * bba_odometry_debug_coeffs and the preprocessing.  The results differ from those of the default mode only by the rounding of
  * those sums.  Not covered: the PCG solver -- bba_bundle_adjust with use_pcg and bba_pcg_debug return BBA_ERR_UNSUPPORTED while
  * the mode is on -- and more than one rank (the setter returns BBA_ERR_UNSUPPORTED for world_size > 1).  A call with

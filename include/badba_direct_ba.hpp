@@ -44,6 +44,13 @@ struct DeviceImage {
   size_t pitch_bytes;
 };
 
+// The buffers of a frame that is not a keyframe, as EstimateFramePose takes them.
+struct FrameImages {
+  DeviceImage<uint16_t> depth;
+  DeviceImage<uint16_t> normals;
+  DeviceImage<uint8_t> color_rgba;
+};
+
 template <typename T>
 struct MutableDeviceImage {
   T* address;
@@ -146,6 +153,28 @@ class DirectBA {
                                             global_T_frame_initial_estimate.data(), out, nullptr, nullptr, stream),
           "bba_estimate_frame_pose_for_frame");
     std::memcpy(out_global_T_frame_estimate->data(), out, sizeof(out));
+  }
+
+  // The same for many entries in one call (bba_estimate_frame_poses_for_frames): entry i tracks frames[frame_of_entry[i]]
+  // (frames[i] when frame_of_entry is empty) from global_T_frame_initial_estimates[i]; *out_global_T_frame_estimates gets one
+  // estimate per entry and, when given, *at_estimate the pose-kernel coefficients at each estimate.
+  void EstimateFramePoses(cudaStream_t stream, const std::vector<FrameImages>& frames,
+                          const std::vector<SE3f>& global_T_frame_initial_estimates, std::vector<SE3f>* out_global_T_frame_estimates,
+                          const std::vector<int>& frame_of_entry = {}, std::vector<bba_pose_coeffs>* at_estimate = nullptr) {
+    const size_t count = global_T_frame_initial_estimates.size();
+    std::vector<bba_frame_buffers> buffers(frames.size());
+    for (size_t f = 0; f < frames.size(); ++f)
+      buffers[f] = {frames[f].depth.address, frames[f].depth.pitch_bytes, frames[f].normals.address, frames[f].normals.pitch_bytes,
+                    frames[f].color_rgba.address, frames[f].color_rgba.pitch_bytes};
+    std::vector<float> init(7 * count), out(7 * count);
+    for (size_t i = 0; i < count; ++i) std::memcpy(init.data() + 7 * i, global_T_frame_initial_estimates[i].data(), sizeof(float) * 7);
+    if (at_estimate) at_estimate->resize(count);
+    Check(bba_estimate_frame_poses_for_frames(h_, static_cast<int>(frames.size()), buffers.data(), static_cast<int>(count),
+                                              frame_of_entry.empty() ? nullptr : frame_of_entry.data(), init.data(), out.data(), nullptr,
+                                              nullptr, at_estimate ? at_estimate->data() : nullptr, stream),
+          "bba_estimate_frame_poses_for_frames");
+    out_global_T_frame_estimates->resize(count);
+    for (size_t i = 0; i < count; ++i) std::memcpy((*out_global_T_frame_estimates)[i].data(), out.data() + 7 * i, sizeof(float) * 7);
   }
 
   // TrackFramePairwise (pairwise_frame_tracking.h:71-108) as BadSlam::RunOdometry calls it (bad_slam.cc:911-938): the frame's

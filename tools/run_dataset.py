@@ -20,6 +20,12 @@ is written in the TUM format of rgbd_dataset.save_poses:
 
     python tools/run_dataset.py /tmp/synth --keyframe-interval 2 --raw-to-float-depth 0.001 --export-poses /tmp/synth/poses.txt
 
+With --refine-frames (needs --export-poses) the handle gets --refine-headroom free keyframe slots, the preprocessed buffers of every
+tracked frame are kept on the device, and after the last BA every frame that is not a keyframe is tracked against the final
+surfel map in one call (DirectBA.EstimateFramePosesFromBuffers, bba_estimate_frame_poses_for_frames, which runs in chunks of the
+free slots), starting from its deformed pose; the JSON line then also gives the refined frame-pose error and the seconds the
+refinement took.  That keeps every frame's buffers resident: about 2.5 MB per 640x480 frame.
+
 The views of --make-synthetic lie metres apart (a BA test scene, not a video), so odometry between them fails and only the
 keyframe poses of that sequence are meaningful; on a recorded sequence every frame is tracked from its neighbour.
 """
@@ -64,7 +70,12 @@ def main():
     ap.add_argument("--pyramid-level-for-color", type=int, default=0, help="downscale the colour by 2^level (0..3)")
     ap.add_argument("--export-poses", metavar="PATH", default=None,
                     help="track every frame, deform the tracked poses with each BA call and write all frames' poses (TUM format)")
+    ap.add_argument("--refine-frames", action="store_true",
+                    help="after the last BA, refine every non-keyframe pose against the final map in one call (needs --export-poses)")
+    ap.add_argument("--refine-headroom", type=int, default=64, help="free keyframe slots the handle keeps for --refine-frames")
     a = ap.parse_args()
+    if a.refine_frames and a.export_poses is None:
+        ap.error("--refine-frames needs --export-poses")
     if a.make_synthetic:
         make_synthetic(a.make_synthetic)
         return 0
@@ -78,7 +89,8 @@ def main():
     # main.cc:457-460: the cameras of the handle are the calibration scaled to the pyramid levels
     depth_cam, color_cam = cam.Scaled(0.5 ** a.pyramid_level_for_depth), cam.Scaled(0.5 ** a.pyramid_level_for_color)
     ba = DirectBA(a.max_surfels, a.raw_to_float_depth, 40.0, a.cell_size, color_camera_initial_estimate=color_cam,
-                  depth_camera_initial_estimate=depth_cam, max_keyframes=len(idx))
+                  depth_camera_initial_estimate=depth_cam,
+                  max_keyframes=len(idx) + (a.refine_headroom if a.refine_frames else 0))
     raw_options = dict(median_filter_and_densify_iterations=a.median_filter_iterations,
                        pyramid_level_for_depth=a.pyramid_level_for_depth, pyramid_level_for_color=a.pyramid_level_for_color)
     surfels = torch.zeros((17, a.max_surfels), dtype=torch.float32, device="cuda")
@@ -89,6 +101,7 @@ def main():
     keyframe_frames = set(idx)
     frame_poses = np.zeros((len(ds), 7), np.float32)   # global_T_frame of every frame (--export-poses)
     motion_model, base_kf, tracked, t_odometry = MotionModel(), None, 0, 0.0
+    kept = {}   # --refine-frames: frame index -> its preprocessed (depth, normals, rgba)
     n = -1   # keyframes added so far - 1
     for i in (range(len(ds)) if export else idx):
         if export and base_kf is not None:
@@ -105,6 +118,8 @@ def main():
             torch.cuda.synchronize()
             t_odometry += time.perf_counter() - t
             tracked += 1
+            if a.refine_frames and i not in keyframe_frames:
+                kept[i] = (depth, normals, rgba)
         if i not in keyframe_frames:
             continue
         n += 1
@@ -144,12 +159,23 @@ def main():
     if export:
         frame_poses[idx] = poses
         all_true = [f.depth_global_T_frame for f in ds.frames]
-        frame_err = [S.pose_error(rel(frame_poses, k), rel(all_true, k)) for k in range(1, len(ds))]
+        max_err = lambda P: ([max(e[0] for e in err), max(e[1] for e in err)]
+                             if (err := [S.pose_error(rel(P, k), rel(all_true, k)) for k in range(1, len(ds))]) else None)
+        line.update({"frames_tracked": tracked, "seconds_odometry": round(t_odometry, 3), "poses_exported": len(ds),
+                     "max_relative_frame_pose_error_m_rad": max_err(frame_poses)})
+        if a.refine_frames and kept:
+            # every tracked frame against the final map, from its deformed pose, in one call
+            order = sorted(kept)
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            refined = ba.EstimateFramePosesFromBuffers(None, [kept[i] for i in order], frame_poses[order])[0]
+            torch.cuda.synchronize()
+            frame_poses[order] = refined
+            line.update({"frames_refined": len(order), "seconds_refinement": round(time.perf_counter() - t, 3),
+                         "max_relative_frame_pose_error_refined_m_rad": max_err(frame_poses)})
         if not D.save_poses(a.export_poses, [f.depth_time_string for f in ds.frames], frame_poses):
             print(f"cannot write {a.export_poses}", file=sys.stderr)
             return 1
-        line.update({"frames_tracked": tracked, "seconds_odometry": round(t_odometry, 3), "poses_exported": len(ds),
-                     "max_relative_frame_pose_error_m_rad": [max(e[0] for e in frame_err), max(e[1] for e in frame_err)] if frame_err else None})
     print(json.dumps(line))
     return 0
 
