@@ -306,11 +306,15 @@ bba_status TrackFramePairwise(bba_handle h, const char* fn, const bba_odometry_o
   FrontEndCall view(h);
   if (bba_status st = view.Snapshot(s, base_buffers ? -1 : base_keyframe_id, fn)) return st;
   if (bba_status st = EnsureOdometry(h, o->num_scales)) return st;
-  if (bba_status st = MakeLumaTexture(h, device_color_rgba, color_pitch, &h->fe.frame, s, /*front_end=*/true)) return st;
+  const LumaSource frame_source{device_color_rgba, color_pitch};
+  Texture* const frame_luma = &h->fe.frame;
+  if (bba_status st = MakeLumaTextures(h, /*front_end=*/true, 1, &frame_source, &frame_luma, s)) return st;
   KeyframeView base = view.base;
   if (base_buffers) {   // the luma the keyframe would get from bba_add_keyframe, in the front end's base texture
     const BaseBuffers& b = *base_buffers;
-    if (bba_status st = MakeLumaTexture(h, b.rgba, b.rgba_pitch, &h->fe.base, s, /*front_end=*/true)) return st;
+    const LumaSource base_source{b.rgba, b.rgba_pitch};
+    Texture* const base_luma = &h->fe.base;
+    if (bba_status st = MakeLumaTextures(h, /*front_end=*/true, 1, &base_source, &base_luma, s)) return st;
     base.depth = b.depth; base.depth_pitch = b.depth_pitch;
     base.normals = b.normals; base.normals_pitch = b.normals_pitch;
     base.tex = h->fe.base.tex;

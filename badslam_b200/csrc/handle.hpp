@@ -148,10 +148,14 @@ struct CameraView {
   int deterministic = 0;
 };
 
-// A u8 plane that luma extraction writes before the copy into a CUDA array, and the event after which the next user may
-// overwrite it.
+// The u8 planes that luma extraction writes before the copies into CUDA arrays (stacked, `planes` colour images high), the
+// source table of the images after the first (pinned upload copy + device table) and the event after which the next user may
+// overwrite them (MakeLumaTextures).
 struct LumaStaging {
   PitchedBuffer plane;
+  int planes = 0;
+  PinnedBuffer<LumaSource> table_upload;
+  DeviceBuffer<LumaSource> table;
   Event free;
 };
 
@@ -184,20 +188,13 @@ struct bba_context {
     bba::PinnedBuffer<bba::KfDevice> h_kfs;
     bba::Event event;      // recorded after the last upload from the pinned staging buffers
     bool pending = false;
-    bba::LumaStaging luma;      // u8 plane staging for the luma arrays of the BA side; the next user (any stream) waits on .free
+    bba::LumaStaging luma;      // luma staging of the BA side: keyframes and bba_estimate_frame_poses_for_frames
     bba::PitchedBuffer color;   // uchar4 staging image for bba_update_keyframe_host
   } staging;
 
   // Luma of the frames that are not keyframes (bba_estimate_frame_poses_for_frames, pose_step.cu): one array + texture per
-  // distinct frame of a chunk, allocated on first use and trimmed to the free keyframe slots at the start of a call; the u8
-  // planes of a chunk's frames stacked in one image and the source table of the stacked extraction (MakeFrameLumaTextures).
-  struct FrameLuma {
-    std::vector<bba::Texture> pool;
-    bba::LumaStaging stack;   // .free: recorded after the last copy out of the planes (the source table is read before it)
-    int stack_planes = 0;     // planes the stack holds
-    bba::DeviceBuffer<bba::LumaSource> d_sources;
-    bba::PinnedBuffer<bba::LumaSource> h_sources;
-  } frame_luma;
+  // distinct frame of a chunk, created on first use; the pool is trimmed to the free keyframe slots at the start of a call.
+  std::vector<bba::Texture> frame_luma;
 
   // pose step (pose_step.cu) and the spatial order of the surfels
   struct PoseStep {
@@ -450,12 +447,9 @@ template <class Args> void SetSurfelFields(bba_handle h, Args* a) {
   a->pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
   a->n = h->surfels_size;
 }
-// front_end: through the front end's staging plane, counted as a front-end launch.
-bba_status MakeLumaTexture(bba_handle h, const uint8_t* device_rgba, size_t color_pitch, Texture* luma, cudaStream_t s,
-                           bool front_end = false);
-// The luma textures of n colour images (rgba[i] with pitch[i]) in h->frame_luma.pool[0, n): one stacked extraction launch and one
-// copy per image into its array.  Grows the pool to n entries (never beyond what the caller asks for).
-bba_status MakeFrameLumaTextures(bba_handle h, int n, const uint8_t* const* rgba, const size_t* pitch, cudaStream_t s);
+// The luma textures of n >= 1 colour images in device memory (sources[i] -> *out[i]): one extraction launch and one copy per
+// image into its array.  front_end: through fe.luma, counted as front-end launches; otherwise through staging.luma.
+bba_status MakeLumaTextures(bba_handle h, bool front_end, int n, const LumaSource* sources, Texture* const* out, cudaStream_t s);
 
 // pose_step.cu
 // The surfel count from which a launch over n keyframes puts the surfels into spatial order: sorting costs ~0.1 ms of launches

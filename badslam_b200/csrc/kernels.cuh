@@ -319,14 +319,13 @@ LaunchResult LaunchCreateSurfels(const LifecycleArgs& a, const unsigned int* ind
 // order, and rounds the result into *out.
 LaunchResult LaunchExactSumDebug(const float* values, uint64_t n, ExactSum* sum, double* out, int sm_count, cudaStream_t stream);
 
-// uchar4 (.w = luma) -> u8 plane.
-LaunchResult LaunchExtractLuma(const uint8_t* rgba, size_t rgba_pitch, uint8_t* luma, size_t luma_pitch, int w, int h, cudaStream_t stream);
-// The same for `frames` images in one launch: image f (sources[f], device memory) -> rows [f * h, (f + 1) * h) of luma.
+// uchar4 (.w = luma) -> u8 planes, `images` images in one launch: image i (first, or rest[i - 1] in device memory) -> rows
+// [i * h, (i + 1) * h) of luma.  One image reads no table (rest may be null).
 struct LumaSource {
   const uint8_t* rgba;
   size_t pitch;
 };
-LaunchResult LaunchExtractLumaStack(const LumaSource* sources, int frames, uint8_t* luma, size_t luma_pitch, int w, int h,
-                                    cudaStream_t stream);
+LaunchResult LaunchExtractLuma(LumaSource first, const LumaSource* rest, int images, uint8_t* luma, size_t luma_pitch, int w, int h,
+                               cudaStream_t stream);
 
 }  // namespace bba

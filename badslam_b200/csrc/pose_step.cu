@@ -171,7 +171,7 @@ void FillPoseCoeffs(bba_handle h, const std::vector<double>& rec, const std::vec
 // Frame-to-model pose estimation (EstimateFramePose) of `count` entries, entry i = frame frame_of_entry[i] (i without the map)
 // from init[i]; the arguments are valid.  The entries ride through the pose step as temporary entries behind the keyframes, in
 // chunks of as many entries as there are free keyframe slots, in entry order: each chunk's distinct frames get a luma texture of
-// the pool (one stacked extraction launch), then one pose step runs every entry's Gauss-Newton loop and, with at_estimate, one more
+// the pool (one extraction launch), then one pose step runs every entry's Gauss-Newton loop and, with at_estimate, one more
 // pose-kernel launch with stats evaluates every entry at its result.  The temporary entries take part in nothing else (no
 // co-visibility, no activation state), own nothing and are removed before the next chunk; their slots' cost statistics are reset.
 // Serves both entry points: bba_estimate_frame_pose_for_frame is the one-entry, one-frame case.
@@ -181,16 +181,19 @@ bba_status EstimateFramePoses(bba_handle h, int frame_count, const bba_frame_buf
   const int K = static_cast<int>(h->keyframes.size());
   const int free_slots = h->cfg.max_keyframes - K;
   if (free_slots < 1) return Fail(h, BBA_ERR_STATE, std::string(fn) + " needs one free keyframe slot (max_keyframes reached)");
-  auto& luma = h->frame_luma;
-  if (static_cast<int>(luma.pool.size()) > free_slots) luma.pool.resize(free_slots);
-  if (luma.stack_planes > free_slots) {
-    luma.stack.plane = PitchedBuffer();
-    luma.stack_planes = 0;
+  // the frames' luma memory stays bounded by the free slots: the pool (entries without an array hold no memory) and the BA
+  // side's staging planes (released when they hold more; the next user allocates as many as it needs)
+  auto& pool = h->frame_luma;
+  pool.resize(free_slots);
+  LumaStaging& staging = h->staging.luma;
+  if (staging.planes > free_slots) {
+    staging.plane = PitchedBuffer();
+    staging.planes = 0;
   }
   std::vector<int> pool_entry(frame_count, -1);   // a frame's luma texture in the current chunk
   std::vector<int> chunk_frames;
-  std::vector<const uint8_t*> rgba;
-  std::vector<size_t> pitch;
+  std::vector<LumaSource> sources;
+  std::vector<Texture*> textures;
   std::vector<int> ids;
   std::vector<Pose> poses;
   std::vector<double> rec;
@@ -198,17 +201,17 @@ bba_status EstimateFramePoses(bba_handle h, int frame_count, const bba_frame_buf
   for (int begin = 0; begin < count; begin += free_slots) {
     const int n = std::min(free_slots, count - begin);
     chunk_frames.clear();
-    rgba.clear();
-    pitch.clear();
+    sources.clear();
+    textures.clear();
     for (int i = 0; i < n; ++i) {
       const int f = frame_of_entry ? frame_of_entry[begin + i] : begin + i;
       if (pool_entry[f] >= 0) continue;
       pool_entry[f] = static_cast<int>(chunk_frames.size());
       chunk_frames.push_back(f);
-      rgba.push_back(frames[f].color_rgba);
-      pitch.push_back(frames[f].color_pitch);
+      sources.push_back(LumaSource{frames[f].color_rgba, frames[f].color_pitch});
+      textures.push_back(&pool[pool_entry[f]]);
     }
-    bba_status st = MakeFrameLumaTextures(h, static_cast<int>(chunk_frames.size()), rgba.data(), pitch.data(), s);
+    bba_status st = MakeLumaTextures(h, /*front_end=*/false, static_cast<int>(chunk_frames.size()), sources.data(), textures.data(), s);
     ids.resize(n);
     poses.resize(n);
     for (int i = 0; st == BBA_OK && i < n; ++i) {
@@ -216,7 +219,7 @@ bba_status EstimateFramePoses(bba_handle h, int frame_count, const bba_frame_buf
       Keyframe entry{};
       entry.depth = frames[f].depth; entry.depth_pitch = frames[f].depth_pitch;
       entry.normals = frames[f].normals; entry.normals_pitch = frames[f].normals_pitch;
-      entry.tex = luma.pool[pool_entry[f]].tex;
+      entry.tex = pool[pool_entry[f]].tex;
       entry.pose = PoseFromArray(init + 7 * static_cast<size_t>(begin + i));
       entry.activation = BBA_KF_ACTIVE;
       ids[i] = K + i;
