@@ -313,10 +313,12 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
     // iteration whose list turned out empty costs three immediately-returning launches, ~10 us; the depth rides out a host
     // thread that is descheduled for a moment -- on a box whose cores were oversubscribed, 2 CPUs for 4 ranks, a depth of one
     // left the GPU idle between iterations.)
-    constexpr int kDepth = 3;
-    if (it >= kDepth) {
+    // In the deterministic mode nothing is queued ahead: how many iterations the host had enqueued when the last one finished
+    // depends on its timing, and with it the number of launches the call reports (bba_ba_result::kernel_launches).
+    const int depth = h->deterministic ? 0 : 3;
+    if (it >= depth) {
       unsigned int polls = 0;
-      while (p.h_flag[0] < it - kDepth + 1) {
+      while (p.h_flag[0] < it - depth + 1) {
         // cudaSuccess: everything drained; any other result than "not ready" is a (sticky) device fault that would
         // otherwise leave this loop spinning for ever -- the BBA_CUDA check below reports it
         if (cudaStreamQuery(s) != cudaErrorNotReady) break;

@@ -685,6 +685,17 @@ class DirectBA:
         self._check(self._lib.bba_optimize_intrinsics(self._h, int(optimize_depth_intrinsics),
                                                       int(optimize_color_intrinsics), self._stream_ptr(stream)))
 
+    def IntrinsicsCoeffs(self, optimize_depth_intrinsics: bool, optimize_color_intrinsics: bool, stream=None):
+        """Parity hook (bba_debug_intrinsics_coeffs): the normal equations of the intrinsics step before the Schur complement.
+        Returns (sums [34] fp64: A upper triangle, b1, colour H upper triangle, colour b; cells [8, cf_h * cf_w] fp32: the five
+        rows of B, D, b2 and the observation count per sparse cell).  The handle's state does not change."""
+        w, h = C.c_int(), C.c_int()
+        self._check(self._lib.bba_cfactor_size(self._h, C.byref(w), C.byref(h)))
+        sums, cells = np.zeros(34), np.zeros((8, w.value * h.value), np.float32)
+        self._check(self._lib.bba_debug_intrinsics_coeffs(self._h, int(optimize_depth_intrinsics), int(optimize_color_intrinsics),
+                                                          sums.ctypes.data, cells.ctypes.data, self._stream_ptr(stream)))
+        return sums, cells
+
     def BundleAdjustment(self, stream, optimize_depth_intrinsics: bool, optimize_color_intrinsics: bool,
                          do_surfel_updates: bool, optimize_poses: bool, optimize_geometry: bool,
                          min_iterations: int, max_iterations: int, use_pcg: bool = False,

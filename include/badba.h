@@ -350,6 +350,14 @@ bba_status bba_pcg_debug(bba_handle h, const bba_ba_options* o, int step, int ap
 
 /* OptimizeIntrinsicsCUDA (kernels.h:246-260, kernel_opt_intrinsics.cc:39-281) */
 bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth_intrinsics, int optimize_color_intrinsics, void* stream);
+/* Parity hook for the intrinsics step: the normal equations bba_optimize_intrinsics accumulates, read back before the Schur
+ * complement touches them (in the deterministic mode: the rounded exact sums).  The first half of the step itself runs, nothing
+ * of the handle's state changes.  sums [34] (host, fp64): [0..14] upper triangle of the 5x5 A over (fx^-1, fy^-1, cx^-1, cy^-1, a),
+ * [15..19] b1, [20..29] upper triangle of the colour camera's 4x4 H, [30..33] its b.  cells [8][cf_width * cf_height] (host,
+ * fp32): rows 0..4 = B, 5 = D, 6 = b2, 7 = the observation count of each sparse cell.  Without surfels or keyframes everything
+ * reads back zero.  Synchronises the stream. */
+bba_status bba_debug_intrinsics_coeffs(bba_handle h, int optimize_depth_intrinsics, int optimize_color_intrinsics, double* sums,
+                                       float* cells, void* stream);
 /* DirectBA::BundleAdjustment (direct_ba.h:143-162, direct_ba.cc:407-453 -> direct_ba_alternating.cc:285-738) */
 bba_status bba_bundle_adjust(bba_handle h, const bba_ba_options* options, bba_ba_result* result, void* stream);
 

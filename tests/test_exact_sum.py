@@ -22,8 +22,14 @@ def arrays():
     big = np.full(1000, FLT_MAX, np.float32)
     big_mixed = np.concatenate([big, -big[:999], np.float32([FLT_TRUE_MIN])])
     million = (rng.standard_normal(10 ** 6) * 10.0 ** rng.uniform(-20, 20, 10 ** 6)).astype(np.float32)
+    # sums at or above 2^139 in magnitude reach the tenth 32-bit digit of the rounding (ExactFinalize, k == 9)
+    top = np.full(4096, FLT_MAX, np.float32)                                             # ~2^140
+    top_carry = np.concatenate([top, -top[:4095], np.float32([FLT_TRUE_MIN])])           # from the top digit down to bit 0
+    top_edge = np.full(4096, 2.0 ** 127, np.float32)                                     # exactly 2^139: the digit boundary
+    neg_tiny = np.full(1 << 20, -FLT_TRUE_MIN, np.float32)                               # a borrow through every word
     return dict(wide=wide, cancel=cancel, subnormal=sub, flt_max=big, flt_max_mixed=big_mixed, million=million,
-                three=np.float32([1e30, 1, -1e30]))
+                three=np.float32([1e30, 1, -1e30]), top_digit=top, top_digit_negative=-top, top_digit_carry=top_carry,
+                top_digit_edge=top_edge, negative_tiny=neg_tiny)
 
 
 def bits(x):

@@ -66,7 +66,9 @@ def test_pose_coeffs_batch_every_variant(mods):
             assert c0[:, 2].sum() > 0, tag
             for k in ids:
                 if c0[k, 2]:
-                    assert rel(H1[k], H0[k]) < 5e-7 and rel(b1[k], b0[k]) < 5e-7, (tag, k, rel(H1[k], H0[k]), rel(b1[k], b0[k]))
+                    # (H: 1.5e-8 measured on an H100 in the instantiations without the precomputed frames, bit-equal with them;
+                    #  tests/test_gpu_deterministic_values.py holds every slot to its own scale)
+                    assert rel(H1[k], H0[k]) < 1e-7 and rel(b1[k], b0[k]) < 5e-7, (tag, k, rel(H1[k], H0[k]), rel(b1[k], b0[k]))
 
 
 BA_KW = dict(optimize_depth_intrinsics=True, optimize_color_intrinsics=True, do_surfel_updates=True, optimize_poses=True,
