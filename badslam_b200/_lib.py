@@ -105,6 +105,14 @@ class FrameBuffers(C.Structure):   # bba_frame_buffers
                 ("color_rgba", C.c_void_p), ("color_pitch", C.c_size_t)]
 
 
+class OdometryEntry(C.Structure):   # bba_odometry_entry
+    _fields_ = [("base_keyframe_id", C.c_int), ("base_frame", C.c_int), ("tracked_frame", C.c_int),
+                ("base_T_frame_initial_1", C.c_float * 7), ("base_T_frame_initial_2", C.c_float * 7)]
+
+
+ODOMETRY_CHUNK_ENTRIES = 64   # BBA_ODOMETRY_CHUNK_ENTRIES
+
+
 class Profile(C.Structure):
     _fields_ = [("pose_launches", C.c_uint64), ("pose_ms", C.c_double), ("kf_evals", C.c_uint64),
                 ("n_pair", C.c_uint64), ("n_inimg", C.c_uint64), ("n_depthok", C.c_uint64),
@@ -169,6 +177,8 @@ SYMBOLS = {
                                                       C.POINTER(PoseCoeffs), _P]),
     "bba_track_frame_pairwise": (C.c_int, [_P, C.POINTER(OdometryOptions), C.c_int, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
                                            _F7, _F7, _F7, C.POINTER(OdometryResult), _P]),
+    "bba_track_frames_pairwise": (C.c_int, [_P, C.POINTER(OdometryOptions), C.c_int, C.POINTER(FrameBuffers), C.c_int,
+                                            C.POINTER(OdometryEntry), _P, C.POINTER(OdometryResult), C.POINTER(C.c_uint32), _P]),
     "bba_track_frame_pairwise_to_frame": (C.c_int, [_P, C.POINTER(OdometryOptions), _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
                                                     _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _F7, _F7, _F7,
                                                     C.POINTER(OdometryResult), _P]),

@@ -109,12 +109,13 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
   return BBA_OK;
 }
 
-bba_status FrontEndCall::Snapshot(cudaStream_t s, int kf_id, const char* fn) {
+bba_status FrontEndCall::Snapshot(cudaStream_t s, int kf_id, const char* fn, int max_kf_id, std::vector<KeyframeView>* all_kfs) {
   auto& f = h_->fe;
   {
     std::lock_guard<std::mutex> lock(f.mu);
-    if (kf_id >= static_cast<int>(f.kfs.size())) return Fail(h_, BBA_ERR_INVALID_ARGUMENT, std::string(fn) + ": no such keyframe");
+    if (std::max(kf_id, max_kf_id) >= static_cast<int>(f.kfs.size())) return Fail(h_, BBA_ERR_INVALID_ARGUMENT, std::string(fn) + ": no such keyframe");
     if (kf_id >= 0) base = f.kfs[kf_id];
+    if (all_kfs) *all_kfs = f.kfs;
     cams = f.cams;
     slot_ = f.current;
     ++f.readers[slot_];

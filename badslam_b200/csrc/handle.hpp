@@ -14,6 +14,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -297,23 +298,34 @@ struct bba_context {
     bool replicated_pass_pending = false;
   } xchg;
 
-  // image-pair odometry (bba_track_frame_pairwise), lazily allocated: intensity / gradient-magnitude images of both frames
-  // (colour-sized), the depth / normal / colour pyramids of both frames, accumulators + barrier + result of the persistent kernel
+  // image-pair odometry (bba_track_frame_pairwise, bba_track_frames_pairwise), lazily allocated: a pool of pyramids, one per
+  // distinct image and role of a chunk (the intensity / gradient-magnitude plane, colour-sized, and the depth / normal / colour
+  // levels), the chunk's image and entry tables, accumulators + barriers + results of the persistent kernel
+  struct Pyramid {
+    bba::PitchedBuffer gradmag;
+    bba::Texture gradmag_tex;
+    bba::PitchedBuffer depth[bba::odom::kMaxScales], normals[bba::odom::kMaxScales], color[bba::odom::kMaxScales];
+    bba::Texture color_tex[bba::odom::kMaxScales];
+    bba::odom::Image image[bba::odom::kMaxScales] = {};   // views of the planes above
+  };
   struct Odometry {
-    int num_scales = 0;          // levels allocated
+    int num_scales = 0;          // levels allocated in every pyramid of the pool
     int last_num_scales = 0;     // levels filled by the last call (parity hooks)
     int last_first_scale = 0;
-    bba::PitchedBuffer gradmag[2];
-    bba::Texture gradmag_tex[2];
-    bba::odom::Image image[2][bba::odom::kMaxScales] = {};   // [0 base | 1 tracked][scale]; views of the planes below
-    bba::PitchedBuffer depth[2][bba::odom::kMaxScales], normals[2][bba::odom::kMaxScales], color[2][bba::odom::kMaxScales];
-    bba::Texture color_tex[2][bba::odom::kMaxScales];
+    std::vector<std::unique_ptr<Pyramid>> pool;
     int w[bba::odom::kMaxScales] = {}, h[bba::odom::kMaxScales] = {};
-    bba::odom::Level level[bba::odom::kMaxScales] = {};      // as passed to the last launch
-    bba::DeviceBuffer<double> d_acc;             // [3][32]
-    bba::DeviceBuffer<double> d_partials;        // deterministic mode: [3][grid][32] per-CTA totals (TrackArgs::partials)
-    bba::DeviceBuffer<unsigned int> d_barrier;   // [2]
-    bba::DeviceBuffer<bba::odom::TrackResult> d_result;
+    // The last chunk's tables as the kernels read them; the parity hooks work on its last entry.
+    bba::odom::LevelCamera cam[bba::odom::kMaxScales] = {};
+    bba::odom::Image last_level[2][bba::odom::kMaxScales] = {};   // [0 base | 1 tracked][scale] of the last entry
+    bba::odom::TrackEntry last_entry{};
+    bba::PinnedBuffer<bba::odom::PyramidImage> h_images;
+    bba::DeviceBuffer<bba::odom::PyramidImage> d_images;
+    bba::PinnedBuffer<bba::odom::TrackEntry> h_entries;
+    bba::DeviceBuffer<bba::odom::TrackEntry> d_entries;
+    bba::DeviceBuffer<double> d_acc;             // [groups][3][32]
+    bba::DeviceBuffer<double> d_partials;        // deterministic mode: [groups][3][virtual grid][32] (TrackArgs::partials)
+    bba::DeviceBuffer<unsigned int> d_control;   // TrackArgs::control
+    bba::DeviceBuffer<bba::odom::TrackResult> d_result;   // [entries of a chunk]
     bba::PinnedBuffer<bba::odom::TrackResult> h_result;
   } odo;
 
@@ -342,6 +354,7 @@ struct bba_context {
     bba::LumaStaging luma;
     bba::Texture frame;        // luma of the tracked frame
     bba::Texture base;         // luma of a base frame given as buffers (bba_track_frame_pairwise_to_frame)
+    std::vector<bba::Texture> frames;   // luma of the distinct frames of a bba_track_frames_pairwise chunk, grown on demand
   } fe;
 
   // kernels launched by BA-side calls and by front-end calls (bba_kernel_launch_count: the sum); two counters so that the
@@ -418,7 +431,8 @@ class FrontEndCall {
   ~FrontEndCall() { ReleaseSlot(); }
   FrontEndCall(const FrontEndCall&) = delete;
   FrontEndCall& operator=(const FrontEndCall&) = delete;
-  bba_status Snapshot(cudaStream_t s, int kf_id, const char* fn);
+  // (max_kf_id: fails unless every keyframe id up to it is published; all_kfs: receives every published keyframe record)
+  bba_status Snapshot(cudaStream_t s, int kf_id, const char* fn, int max_kf_id = -1, std::vector<KeyframeView>* all_kfs = nullptr);
   bba_status ReleaseSlot(bool record = true);
   CameraView cams;
   KeyframeView base;

@@ -649,6 +649,35 @@ class DirectBA:
             C.byref(res), self._stream_ptr(stream)))
         return out, res
 
+    def TrackFramesPairwise(self, stream, frames, entries, num_scales: int = 5, use_pyramid_level_0: bool = True,
+                            use_gradmag: bool = False, test_different_initial_estimates: bool = True, max_iterations_per_scale: int = 30):
+        """TrackFramePairwise / TrackFramePairwiseToFrame for many independent pairs in one call (bba_track_frames_pairwise), all
+        with the same options.  frames: a sequence of (depth, normals, colour) device tensors as TrackFramePairwise takes them;
+        entries: a sequence of (base_keyframe_id, base_frame, tracked_frame, base_T_frame_initial_1[, base_T_frame_initial_2]),
+        base_keyframe_id -1 meaning frames[base_frame] is the base.  Returns (base_T_frame_estimates [count, 7], a list of the count
+        OdometryResult, the kernel launches of the whole call).  The entries run in chunks of _lib.ODOMETRY_CHUNK_ENTRIES."""
+        bufs = (_lib.FrameBuffers * len(frames))()
+        for b, (depth, normals, color) in zip(bufs, frames):
+            b.depth, b.depth_pitch = depth.data_ptr(), depth.stride(0) * 2
+            b.normals, b.normals_pitch = normals.data_ptr(), normals.stride(0) * 2
+            b.color_rgba, b.color_pitch = color.data_ptr(), color.stride(0)
+        ents = (_lib.OdometryEntry * len(entries))()
+        for e, spec in zip(ents, entries):
+            e.base_keyframe_id, e.base_frame, e.tracked_frame = int(spec[0]), int(spec[1]), int(spec[2])
+            p1 = np.ascontiguousarray(spec[3], np.float32).reshape(7)
+            p2 = p1 if len(spec) < 5 or spec[4] is None else np.ascontiguousarray(spec[4], np.float32).reshape(7)
+            e.base_T_frame_initial_1[:] = p1.tolist()
+            e.base_T_frame_initial_2[:] = p2.tolist()
+        count = len(entries)
+        out = np.zeros((count, 7), np.float32)
+        results = (_lib.OdometryResult * count)()
+        launches = C.c_uint32()
+        o = _lib.OdometryOptions(int(num_scales), int(use_pyramid_level_0), int(use_gradmag), int(test_different_initial_estimates),
+                                 int(max_iterations_per_scale))
+        self._check(self._lib.bba_track_frames_pairwise(self._h, C.byref(o), len(frames), bufs, count, ents, out.ctypes.data, results,
+                                                        C.byref(launches), self._stream_ptr(stream)))
+        return out, list(results), launches.value
+
     def OdometryLevel(self, which: int, scale: int, stream=None):
         """Parity hook: (depth f32, normals u16, colour u8) of one pyramid level of the last TrackFramePairwise call
         (which: 0 = base keyframe, 1 = tracked frame)."""

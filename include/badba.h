@@ -24,7 +24,8 @@
  *      front-end side: one further thread may make one call at a time, on its own stream, while a
  *        BA-side call is in flight -- also from inside progress_function.  The front-end calls are
  *        bba_preprocess_frame, bba_preprocess_raw_frame, bba_track_frame_pairwise,
- *        bba_track_frame_pairwise_to_frame, bba_odometry_get_level, bba_odometry_debug_coeffs, the
+ *        bba_track_frame_pairwise_to_frame, bba_track_frames_pairwise, bba_odometry_get_level,
+ *        bba_odometry_debug_coeffs, the
  *        bba_host_* functions (no handle) and the readers bba_keyframe_count, bba_get_keyframe_pose,
  *        bba_get_keyframe_states, bba_get_keyframe_activation, bba_get_intrinsics,
  *        bba_get_cfactor_host, bba_cfactor_size and bba_get_residual_types.
@@ -490,7 +491,7 @@ bba_status bba_preprocess_raw_frame(bba_handle h, const bba_raw_frame_options* o
  * launch with no host round trip (the reference synchronises the stream once per iteration).
  * The tracked frame is given like in bba_estimate_frame_pose_for_frame (preprocessed depth, normals, uchar4 colour with
  * .w = luma); poses are base_T_frame as {qx,qy,qz,qw,tx,ty,tz}.  Uses the handle's cameras, depth deformation and residual types.
- * Front-end calls (bba_track_frame_pairwise, bba_track_frame_pairwise_to_frame and the two parity hooks): the published cameras,
+ * Front-end calls (bba_track_frame_pairwise, bba_track_frame_pairwise_to_frame, bba_track_frames_pairwise and the two parity hooks): the published cameras,
  * a, cfactor, residual types and base keyframe record; their own luma staging plane and textures. */
 typedef struct {
   int num_scales;                        /* BadSlamConfig::num_scales, default 5 (bad_slam_config.h:167); 1..8 */
@@ -526,7 +527,43 @@ bba_status bba_track_frame_pairwise_to_frame(bba_handle h, const bba_odometry_op
                                              const uint8_t* device_color_rgba, size_t color_pitch,
                                              const float base_T_frame_initial_1[7], const float base_T_frame_initial_2[7],
                                              float base_T_frame_estimate[7], bba_odometry_result* result, void* stream);
-/* Parity hooks (the pyramids and normal equations of the LAST bba_track_frame_pairwise call of this handle, device-resident):
+/* bba_track_frame_pairwise / bba_track_frame_pairwise_to_frame for many independent (base, tracked frame) pairs in one call, all
+ * with the same options: re-tracking every frame against its base keyframe from its deformed pose after the final BA,
+ * verifying a frame against several keyframes, or trying more starting poses for one pair.  Entry i tracks
+ * frames[entries[i].tracked_frame] against keyframe entries[i].base_keyframe_id (>= 0) or, with -1, against the frame
+ * frames[entries[i].base_frame] given as buffers, from base_T_frame_initial_1 (and _2 with test_different_initial_estimates),
+ * and writes base_T_frame_estimate[i] ([count][7]) and results[i] ([count], may be NULL).  A frame or keyframe may appear in
+ * any number of entries.
+ * The entries run in chunks of at most BBA_ODOMETRY_CHUNK_ENTRIES, in entry order.  A chunk runs one luma launch for its distinct
+ * frames, one intensity launch, one level-0 launch and one launch per coarser level for all its pyramids, and one tracking
+ * launch in which groups of CTAs take the entries in order: 4 + (num_scales - 1) launches per chunk whatever its entry count;
+ * results[i].kernel_launches counts the launches of entry i's chunk, *kernel_launches (may be NULL) those of the whole call.
+ * The pyramids come from a library-owned pool, allocated on first use and grown to the largest chunk: one pyramid per
+ * distinct image and role of a chunk (a base keyframe tracked by ten entries has one base pyramid), at most
+ * 2 x BBA_ODOMETRY_CHUNK_ENTRIES.  One pyramid holds the colour-sized intensity plane and, per level, float depth, u16 normals
+ * (from level 1 on) and u8 intensity: 2.56 MB at 640x480 with 5 levels from the level sizes, plus the row padding of the
+ * pitched allocations.
+ * Each entry's result equals that of its own single-pair call up to the order of the sums; in the deterministic mode it equals
+ * it bit for bit, whatever else the call holds and in whatever order.  A front-end call like the single-pair calls: every
+ * keyframe an entry names must be in the published snapshot.  BBA_ERR_INVALID_ARGUMENT: a NULL array, count or frame_count < 1,
+ * a frame index or keyframe id out of range, a NULL frame buffer, a bad pitch, bad num_scales; BBA_ERR_UNSUPPORTED: the depth /
+ * colour pyramid combination the single-pair call rejects.  Arguments are checked before anything is enqueued, and a failed
+ * check leaves the handle and the launch counter unchanged.  Afterwards the parity hooks below describe the call's last entry.
+ * Synchronises the stream once per chunk. */
+#define BBA_ODOMETRY_CHUNK_ENTRIES 64
+typedef struct {
+  int base_keyframe_id;                 /* >= 0: that keyframe is the base; -1: frames[base_frame] is */
+  int base_frame;                       /* read only when base_keyframe_id < 0 */
+  int tracked_frame;                    /* index into frames */
+  float base_T_frame_initial_1[7];
+  float base_T_frame_initial_2[7];      /* read only with options->test_different_initial_estimates */
+} bba_odometry_entry;
+bba_status bba_track_frames_pairwise(bba_handle h, const bba_odometry_options* options, int frame_count, const bba_frame_buffers* frames,
+                                     int count, const bba_odometry_entry* entries, float* base_T_frame_estimate /* [count][7] */,
+                                     bba_odometry_result* results /* [count], may be NULL */, uint32_t* kernel_launches /* may be NULL */,
+                                     void* stream);
+/* Parity hooks (the pyramids and normal equations of the LAST bba_track_frame_pairwise call of this handle, device-resident;
+ * after bba_track_frames_pairwise, of its last entry):
  *  bba_odometry_get_level: one pyramid level of the base (which = 0) or tracked (1) image into dense host arrays
  *    [height][width] (any may be NULL); *width / *height return the level's size.
  *  bba_odometry_debug_coeffs: AccumulatePoseEstimationCoeffsFromImagesCUDA (kernels.h:181-203) at base_T_frame_a -> H[21], b[6],
@@ -543,6 +580,7 @@ bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, c
  * same GPU model give the same results bit for bit in every run, whatever else runs beside them on other streams.  Covered:
  * bba_bundle_adjust (pose, geometry and intrinsics steps, surfel lifecycle), bba_estimate_frame_pose (both forms),
  * bba_estimate_frame_poses_for_frames, bba_accumulate_pose_coeffs, bba_debug_pose_coeffs_batch, bba_optimize_intrinsics, bba_track_frame_pairwise(_to_frame),
+ * bba_track_frames_pairwise,
  * bba_odometry_debug_coeffs and the preprocessing.  The results differ from those of the default mode only by the rounding of
  * those sums.  Not covered: the PCG solver -- bba_bundle_adjust with use_pcg and bba_pcg_debug return BBA_ERR_UNSUPPORTED while
  * the mode is on -- and more than one rank (the setter returns BBA_ERR_UNSUPPORTED for world_size > 1).  A call with

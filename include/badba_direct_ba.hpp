@@ -226,6 +226,33 @@ class DirectBA {
     std::memcpy(out_base_T_frame_estimate->data(), out, sizeof(out));
   }
 
+  // Both forms above for many independent pairs in one call (bba_track_frames_pairwise), all with the same options: entry i
+  // tracks frames[entries[i].tracked_frame] against keyframe entries[i].base_keyframe_id, or with -1 against
+  // frames[entries[i].base_frame].  *out_base_T_frame_estimates gets one estimate per entry and, when given, *results one result.
+  void TrackFramesPairwise(cudaStream_t stream, const std::vector<FrameImages>& frames, const std::vector<bba_odometry_entry>& entries,
+                           bool use_pyramid_level_0, bool use_gradmag, bool test_different_initial_estimates,
+                           std::vector<SE3f>* out_base_T_frame_estimates, int num_scales = 5,
+                           std::vector<bba_odometry_result>* results = nullptr) {
+    bba_odometry_options o{};
+    o.num_scales = num_scales;
+    o.use_pyramid_level_0 = use_pyramid_level_0;
+    o.use_gradmag = use_gradmag;
+    o.test_different_initial_estimates = test_different_initial_estimates;
+    o.max_iterations_per_scale = 30;
+    std::vector<bba_frame_buffers> buffers(frames.size());
+    for (size_t f = 0; f < frames.size(); ++f)
+      buffers[f] = {frames[f].depth.address, frames[f].depth.pitch_bytes, frames[f].normals.address, frames[f].normals.pitch_bytes,
+                    frames[f].color_rgba.address, frames[f].color_rgba.pitch_bytes};
+    const size_t count = entries.size();
+    std::vector<float> out(7 * count);
+    if (results) results->resize(count);
+    Check(bba_track_frames_pairwise(h_, &o, static_cast<int>(frames.size()), buffers.data(), static_cast<int>(count), entries.data(),
+                                    out.data(), results ? results->data() : nullptr, nullptr, stream),
+          "bba_track_frames_pairwise");
+    out_base_T_frame_estimates->resize(count);
+    for (size_t i = 0; i < count; ++i) std::memcpy((*out_base_T_frame_estimates)[i].data(), out.data() + 7 * i, sizeof(float) * 7);
+  }
+
   // direct_ba.h:143-162, same argument order and defaults (Timer* is any type with GetTimeSinceStart()).
   template <typename TimerT = NoTimer>
   void BundleAdjustment(cudaStream_t stream, bool optimize_depth_intrinsics, bool optimize_color_intrinsics, bool do_surfel_updates,
