@@ -247,6 +247,21 @@ bba_status MakeLumaTextures(bba_handle h, bool front_end, int n, const LumaSourc
   return BBA_OK;
 }
 
+bba_status MakeFrameLumaTextures(bba_handle h, bool front_end, const bba_frame_buffers* frames, const std::vector<int>& uses,
+                                 std::vector<Texture>* pool, cudaTextureObject_t* luma, cudaStream_t s) {
+  std::map<int, int> slot_of_frame;
+  std::vector<LumaSource> sources;
+  for (int f : uses)
+    if (slot_of_frame.emplace(f, static_cast<int>(sources.size())).second) sources.push_back(LumaSource{frames[f].color_rgba, frames[f].color_pitch});
+  const int n = static_cast<int>(sources.size());
+  if (static_cast<int>(pool->size()) < n) pool->resize(n);
+  std::vector<Texture*> textures(n);
+  for (int i = 0; i < n; ++i) textures[i] = &(*pool)[i];
+  if (bba_status st = MakeLumaTextures(h, front_end, n, sources.data(), textures.data(), s)) return st;
+  for (const auto& [f, slot] : slot_of_frame) luma[f] = (*pool)[slot].tex;
+  return BBA_OK;
+}
+
 namespace {
 
 bba_status AddKeyframeCommon(bba_handle h, Keyframe&& kf, const uint8_t* device_rgba, size_t color_pitch, const float pose[7],

@@ -43,16 +43,13 @@ bool OdometryLevelSizes(bba_handle h, int num_scales, int* w, int* ht) {
 
 // PairwiseFrameTrackingBuffers + CreatePairwiseTrackingInputBuffersAndTextures (pairwise_frame_tracking.cc:39-151), once per
 // pyramid of the pool: at least `images` pyramids of at least num_scales levels.  More levels than allocated free the pool first.
+// (CheckOdometryCall has checked that every level of num_scales is non-empty.)
 bba_status EnsureOdometry(bba_handle h, int num_scales, int images) {
   auto& o = h->odo;
   if (o.num_scales < num_scales) {
-    int w[bba::odom::kMaxScales], ht[bba::odom::kMaxScales];
-    if (!OdometryLevelSizes(h, num_scales, w, ht))
-      return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: too many pyramid levels for this image size");
     o.pool.clear();
     o.num_scales = num_scales;
-    std::copy(w, w + num_scales, o.w);
-    std::copy(ht, ht + num_scales, o.h);
+    OdometryLevelSizes(h, num_scales, o.w, o.h);
   }
   const int cw = h->cfg.color_width, ch = h->cfg.color_height;
   while (static_cast<int>(o.pool.size()) < images) {
@@ -237,13 +234,34 @@ bba_status LaunchOdometryKernel(bba_handle h, const CameraView& cams, int num_sc
   return BBA_OK;
 }
 
-// The checks every odometry call shares: the options and the depth / colour pyramid combination.
-bba_status CheckOdometryOptions(bba_handle h, const std::string& name, const bba_odometry_options& o) {
-  if (o.num_scales < 1 || o.num_scales > bba::odom::kMaxScales || (!o.use_pyramid_level_0 && o.num_scales < 2))
+// The argument checks of every odometry call (h is not null; fn prefixes the messages): the arrays, the frame buffers, the
+// entries' frame indices, the options, the depth / colour pyramid combination and the level sizes.  The keyframe ids are checked
+// against the published keyframes in the snapshot, so that a failed check enqueues nothing.
+bba_status CheckOdometryCall(bba_handle h, const char* fn, const bba_odometry_options* o, int frame_count, const bba_frame_buffers* frames,
+                             int count, const bba_odometry_entry* entries, const float* out) {
+  const std::string name(fn);
+  if (!o || !frames || !entries || !out) return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null argument");
+  if (count < 1 || frame_count < 1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": count and frame_count must be at least 1");
+  for (int f = 0; f < frame_count; ++f) {
+    const bba_frame_buffers& b = frames[f];
+    if (!b.depth || !b.normals || !b.color_rgba) return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null frame buffer");
+    if (!FramePitchesOk(h, b.depth_pitch, b.normals_pitch, b.color_pitch) || ((b.depth_pitch | b.normals_pitch) & 1u))
+      return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": bad frame buffer pitch");
+  }
+  for (int i = 0; i < count; ++i) {
+    const bba_odometry_entry& e = entries[i];
+    if (e.tracked_frame < 0 || e.tracked_frame >= frame_count || e.base_keyframe_id < -1 ||
+        (e.base_keyframe_id < 0 && (e.base_frame < 0 || e.base_frame >= frame_count)))
+      return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": frame index out of range in entry " + std::to_string(i));
+  }
+  if (o->num_scales < 1 || o->num_scales > bba::odom::kMaxScales || (!o->use_pyramid_level_0 && o->num_scales < 2))
     return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": num_scales must be 1..8 (>= 2 without pyramid level 0)");
   // pairwise_frame_tracking.cc:300-306 (LOG(FATAL) in the reference)
-  if (!o.use_pyramid_level_0 && h->cfg.depth_width != h->cfg.color_width && h->cfg.depth_width != 2 * h->cfg.color_width)
+  if (!o->use_pyramid_level_0 && h->cfg.depth_width != h->cfg.color_width && h->cfg.depth_width != 2 * h->cfg.color_width)
     return Fail(h, BBA_ERR_UNSUPPORTED, "The chosen depth / color pyramid level combination is not supported here.");
+  int w[bba::odom::kMaxScales], ht[bba::odom::kMaxScales];
+  if (!OdometryLevelSizes(h, o->num_scales, w, ht))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": too many pyramid levels for this image size");
   return BBA_OK;
 }
 
@@ -335,72 +353,9 @@ bba_status PreprocessFrame(bba_handle h, const char* fn, const bba_preprocess_op
   return BBA_OK;
 }
 
-// The base frame of bba_track_frame_pairwise_to_frame.
-struct BaseBuffers {
-  const uint16_t* depth;
-  size_t depth_pitch;
-  const uint16_t* normals;
-  size_t normals_pitch;
-  const uint8_t* rgba;
-  size_t rgba_pitch;
-};
-
-// bba_track_frame_pairwise (base = keyframe base_keyframe_id) and bba_track_frame_pairwise_to_frame (base = *base_buffers): the
-// one-entry case of TrackFramesPairwise, with the luma of the tracked frame and of a base frame in launches of their own.
-bba_status TrackFramePairwise(bba_handle h, const char* fn, const bba_odometry_options* o, int base_keyframe_id, const BaseBuffers* base_buffers,
-                              const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals, size_t normals_pitch,
-                              const uint8_t* device_color_rgba, size_t color_pitch, const float init1[7], const float init2[7],
-                              float out[7], bba_odometry_result* result, void* stream) {
-  const std::string name(fn);
-  if (!h || !o || !device_depth || !device_normals || !device_color_rgba || !init1 || !out) return h ? Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null argument") : BBA_ERR_INVALID_ARGUMENT;
-  if (base_keyframe_id < 0 && !base_buffers) return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": no such keyframe");
-  if (!FramePitchesOk(h, depth_pitch, normals_pitch, color_pitch) || ((depth_pitch | normals_pitch) & 1u))
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": bad frame buffer pitch");
-  if (base_buffers) {
-    const BaseBuffers& b = *base_buffers;
-    if (!b.depth || !b.normals || !b.rgba) return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": null argument");
-    if (!FramePitchesOk(h, b.depth_pitch, b.normals_pitch, b.rgba_pitch) || ((b.depth_pitch | b.normals_pitch) & 1u))
-      return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": bad base buffer pitch");
-  }
-  if (bba_status st = CheckOdometryOptions(h, name, *o)) return st;
-  if (o->test_different_initial_estimates && !init2)
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, name + ": test_different_initial_estimates needs the second estimate");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  std::lock_guard<std::mutex> call(h->fe.call);
-  const uint64_t launches_before = h->front_end_launches;
-  FrontEndCall view(h);
-  if (bba_status st = view.Snapshot(s, base_buffers ? -1 : base_keyframe_id, fn)) return st;
-  const LumaSource frame_source{device_color_rgba, color_pitch};
-  Texture* const frame_luma = &h->fe.frame;
-  if (bba_status st = MakeLumaTextures(h, /*front_end=*/true, 1, &frame_source, &frame_luma, s)) return st;
-  ChunkImage base{view.base.depth, view.base.depth_pitch, view.base.normals, view.base.normals_pitch, view.base.tex};
-  if (base_buffers) {   // the luma the keyframe would get from bba_add_keyframe, in the front end's base texture
-    const BaseBuffers& b = *base_buffers;
-    const LumaSource base_source{b.rgba, b.rgba_pitch};
-    Texture* const base_luma = &h->fe.base;
-    if (bba_status st = MakeLumaTextures(h, /*front_end=*/true, 1, &base_source, &base_luma, s)) return st;
-    base = ChunkImage{b.depth, b.depth_pitch, b.normals, b.normals_pitch, h->fe.base.tex};
-  }
-  const std::vector<ChunkImage> images{base, ChunkImage{device_depth, depth_pitch, device_normals, normals_pitch, h->fe.frame.tex}};
-  if (bba_status st = BuildOdometryPyramids(h, *o, view, images, 1, s)) return st;
-  if (bba_status st = view.ReleaseSlot()) return st;   // (level 0 was the last reader of the cfactor)
-  bba::odom::TrackEntry entry{};
-  std::memcpy(entry.init1, init1, sizeof(float) * 7);
-  std::memcpy(entry.init2, init2 ? init2 : init1, sizeof(float) * 7);
-  entry.base = 0;
-  entry.tracked = 1;
-  const int max_it = o->max_iterations_per_scale > 0 ? o->max_iterations_per_scale : 30;
-  if (bba_status st = LaunchOdometryKernel(h, view.cams, o->num_scales, o->use_pyramid_level_0 ? 0 : 1, max_it, o->use_gradmag ? 1 : 0,
-                                           o->test_different_initial_estimates ? 1 : 0, -1, {entry}, s))
-    return st;
-  const bba::odom::TrackResult& r = h->odo.h_result[0];
-  std::memcpy(out, r.base_T_frame, sizeof(float) * 7);
-  if (result) CopyOdometryResult(r, o->num_scales, static_cast<uint32_t>(h->front_end_launches - launches_before), result);
-  return BBA_OK;
-}
-
-// bba_track_frames_pairwise after its checks: chunks of at most BBA_ODOMETRY_CHUNK_ENTRIES entries, each with one luma launch for
-// its distinct frames, one pyramid per distinct (image, role) and one tracking launch.
+// The odometry of bba_track_frames_pairwise and of its one-entry forms after CheckOdometryCall: chunks of at most
+// BBA_ODOMETRY_CHUNK_ENTRIES entries, each with one luma launch for its distinct frames, one pyramid per distinct (image, role)
+// and one tracking launch.
 bba_status TrackFramesPairwise(bba_handle h, const char* fn, const bba_odometry_options& o, int frame_count, const bba_frame_buffers* frames,
                                int count, const bba_odometry_entry* entries, float* out, bba_odometry_result* results,
                                uint32_t* kernel_launches, cudaStream_t s) {
@@ -413,16 +368,13 @@ bba_status TrackFramesPairwise(bba_handle h, const char* fn, const bba_odometry_
   std::vector<KeyframeView> kfs;
   if (bba_status st = view.Snapshot(s, -1, fn, max_kf, &kfs)) return st;
   const int max_it = o.max_iterations_per_scale > 0 ? o.max_iterations_per_scale : 30;
+  std::vector<cudaTextureObject_t> luma(frame_count);   // the luma textures of the current chunk's frames
   for (int begin = 0; begin < count; begin += BBA_ODOMETRY_CHUNK_ENTRIES) {
     const int n = std::min(BBA_ODOMETRY_CHUNK_ENTRIES, count - begin);
     const uint64_t chunk_before = h->front_end_launches;
-    // the chunk's distinct frames (one luma texture each) and distinct images: bases (keyframe or frame), then tracked frames
-    std::map<int, int> luma_of_frame, base_of_kf, base_of_frame, tracked_of_frame;
-    std::vector<int> chunk_frames;
-    auto frame_luma = [&](int f) {
-      auto it = luma_of_frame.emplace(f, static_cast<int>(chunk_frames.size()));
-      if (it.second) chunk_frames.push_back(f);
-    };
+    // the chunk's distinct images: bases (keyframe or frame), then tracked frames; and the frames among them, which need luma
+    std::map<int, int> base_of_kf, base_of_frame, tracked_of_frame;
+    std::vector<int> luma_frames;
     std::vector<od::TrackEntry> track(n);
     std::vector<std::pair<int, int>> base_images;   // (keyframe id, -1) or (-1, frame)
     for (int i = 0; i < n; ++i) {
@@ -431,7 +383,7 @@ bba_status TrackFramesPairwise(bba_handle h, const char* fn, const bba_odometry_
       const int key = e.base_keyframe_id >= 0 ? e.base_keyframe_id : e.base_frame;
       auto it = of.emplace(key, static_cast<int>(base_images.size()));
       if (it.second) base_images.emplace_back(e.base_keyframe_id >= 0 ? key : -1, e.base_keyframe_id >= 0 ? -1 : key);
-      if (e.base_keyframe_id < 0) frame_luma(e.base_frame);
+      if (e.base_keyframe_id < 0) luma_frames.push_back(e.base_frame);
       track[i].base = it.first->second;
     }
     const int n_base = static_cast<int>(base_images.size());
@@ -440,21 +392,12 @@ bba_status TrackFramesPairwise(bba_handle h, const char* fn, const bba_odometry_
       const bba_odometry_entry& e = entries[begin + i];
       auto it = tracked_of_frame.emplace(e.tracked_frame, n_base + static_cast<int>(tracked_images.size()));
       if (it.second) tracked_images.push_back(e.tracked_frame);
-      frame_luma(e.tracked_frame);
+      luma_frames.push_back(e.tracked_frame);
       track[i].tracked = it.first->second;
       std::memcpy(track[i].init1, e.base_T_frame_initial_1, sizeof(float) * 7);
       std::memcpy(track[i].init2, o.test_different_initial_estimates ? e.base_T_frame_initial_2 : e.base_T_frame_initial_1, sizeof(float) * 7);
     }
-    // one luma launch for the chunk's frames
-    const int nf = static_cast<int>(chunk_frames.size());
-    if (static_cast<int>(h->fe.frames.size()) < nf) h->fe.frames.resize(nf);
-    std::vector<LumaSource> sources(nf);
-    std::vector<Texture*> textures(nf);
-    for (int j = 0; j < nf; ++j) {
-      sources[j] = LumaSource{frames[chunk_frames[j]].color_rgba, frames[chunk_frames[j]].color_pitch};
-      textures[j] = &h->fe.frames[j];
-    }
-    if (bba_status st = MakeLumaTextures(h, /*front_end=*/true, nf, sources.data(), textures.data(), s)) return st;
+    if (bba_status st = MakeFrameLumaTextures(h, /*front_end=*/true, frames, luma_frames, &h->fe.frames, luma.data(), s)) return st;
     std::vector<ChunkImage> images;
     for (const auto& b : base_images) {
       if (b.first >= 0) {
@@ -462,12 +405,12 @@ bba_status TrackFramesPairwise(bba_handle h, const char* fn, const bba_odometry_
         images.push_back(ChunkImage{k.depth, k.depth_pitch, k.normals, k.normals_pitch, k.tex});
       } else {
         const bba_frame_buffers& f = frames[b.second];
-        images.push_back(ChunkImage{f.depth, f.depth_pitch, f.normals, f.normals_pitch, h->fe.frames[luma_of_frame[b.second]].tex});
+        images.push_back(ChunkImage{f.depth, f.depth_pitch, f.normals, f.normals_pitch, luma[b.second]});
       }
     }
     for (int t : tracked_images) {
       const bba_frame_buffers& f = frames[t];
-      images.push_back(ChunkImage{f.depth, f.depth_pitch, f.normals, f.normals_pitch, h->fe.frames[luma_of_frame[t]].tex});
+      images.push_back(ChunkImage{f.depth, f.depth_pitch, f.normals, f.normals_pitch, luma[t]});
     }
     if (bba_status st = BuildOdometryPyramids(h, o, view, images, n_base, s)) return st;
     if (begin + n >= count)
@@ -486,6 +429,25 @@ bba_status TrackFramesPairwise(bba_handle h, const char* fn, const bba_odometry_
   return BBA_OK;
 }
 
+// bba_track_frame_pairwise and bba_track_frame_pairwise_to_frame (h is not null): the one-entry call on `frames`, the tracked frame
+// last, against keyframe base_keyframe_id or, with -1, against frames[0].  Beside the entry's checks it refuses what an entry
+// cannot express: a null init1, and a null init2 with test_different_initial_estimates.
+bba_status TrackFramePair(bba_handle h, const char* fn, const bba_odometry_options* o, int base_keyframe_id, int frame_count,
+                          const bba_frame_buffers* frames, const float* init1, const float* init2, float* out, bba_odometry_result* result,
+                          void* stream) {
+  if (!init1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, std::string(fn) + ": null argument");
+  bba_odometry_entry entry{};
+  entry.base_keyframe_id = base_keyframe_id;
+  entry.base_frame = 0;
+  entry.tracked_frame = frame_count - 1;
+  std::memcpy(entry.base_T_frame_initial_1, init1, sizeof(float) * 7);
+  std::memcpy(entry.base_T_frame_initial_2, init2 ? init2 : init1, sizeof(float) * 7);
+  if (bba_status st = CheckOdometryCall(h, fn, o, frame_count, frames, 1, &entry, out)) return st;
+  if (o->test_different_initial_estimates && !init2)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, std::string(fn) + ": test_different_initial_estimates needs the second estimate");
+  return TrackFramesPairwise(h, fn, *o, frame_count, frames, 1, &entry, out, result, nullptr, static_cast<cudaStream_t>(stream));
+}
+
 }  // namespace
 }  // namespace bba
 
@@ -497,8 +459,11 @@ bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* o,
                                     const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals, size_t normals_pitch,
                                     const uint8_t* device_color_rgba, size_t color_pitch, const float init1[7], const float init2[7],
                                     float out[7], bba_odometry_result* result, void* stream) {
-  return TrackFramePairwise(h, "bba_track_frame_pairwise", o, base_keyframe_id, nullptr, device_depth, depth_pitch, device_normals,
-                            normals_pitch, device_color_rgba, color_pitch, init1, init2, out, result, stream);
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  // (-1 would mean a frame base in an entry)
+  if (base_keyframe_id < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: no such keyframe");
+  const bba_frame_buffers frame{device_depth, depth_pitch, device_normals, normals_pitch, device_color_rgba, color_pitch};
+  return TrackFramePair(h, "bba_track_frame_pairwise", o, base_keyframe_id, 1, &frame, init1, init2, out, result, stream);
 }
 
 bba_status bba_track_frame_pairwise_to_frame(bba_handle h, const bba_odometry_options* o,
@@ -509,36 +474,20 @@ bba_status bba_track_frame_pairwise_to_frame(bba_handle h, const bba_odometry_op
                                              size_t normals_pitch, const uint8_t* device_color_rgba, size_t color_pitch,
                                              const float init1[7], const float init2[7], float out[7], bba_odometry_result* result,
                                              void* stream) {
-  const BaseBuffers base{base_depth, base_depth_pitch, base_normals, base_normals_pitch, base_color_rgba, base_color_pitch};
-  return TrackFramePairwise(h, "bba_track_frame_pairwise_to_frame", o, -1, &base, device_depth, depth_pitch, device_normals,
-                            normals_pitch, device_color_rgba, color_pitch, init1, init2, out, result, stream);
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const bba_frame_buffers frames[2] = {{base_depth, base_depth_pitch, base_normals, base_normals_pitch, base_color_rgba, base_color_pitch},
+                                       {device_depth, depth_pitch, device_normals, normals_pitch, device_color_rgba, color_pitch}};
+  return TrackFramePair(h, "bba_track_frame_pairwise_to_frame", o, -1, 2, frames, init1, init2, out, result, stream);
 }
 
 bba_status bba_track_frames_pairwise(bba_handle h, const bba_odometry_options* o, int frame_count, const bba_frame_buffers* frames,
                                      int count, const bba_odometry_entry* entries, float* base_T_frame_estimate,
                                      bba_odometry_result* results, uint32_t* kernel_launches, void* stream) {
-  const std::string fn = "bba_track_frames_pairwise: ";
+  const char* fn = "bba_track_frames_pairwise";
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  if (!o || !frames || !entries || !base_T_frame_estimate) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  if (count < 1 || frame_count < 1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count and frame_count must be at least 1");
-  for (int f = 0; f < frame_count; ++f) {
-    const bba_frame_buffers& b = frames[f];
-    if (!b.depth || !b.normals || !b.color_rgba) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null frame buffer");
-    if (!FramePitchesOk(h, b.depth_pitch, b.normals_pitch, b.color_pitch) || ((b.depth_pitch | b.normals_pitch) & 1u))
-      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad frame buffer pitch");
-  }
-  for (int i = 0; i < count; ++i) {
-    const bba_odometry_entry& e = entries[i];
-    if (e.tracked_frame < 0 || e.tracked_frame >= frame_count || e.base_keyframe_id < -1 ||
-        (e.base_keyframe_id < 0 && (e.base_frame < 0 || e.base_frame >= frame_count)))
-      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "frame index out of range in entry " + std::to_string(i));
-  }
-  if (bba_status st = CheckOdometryOptions(h, "bba_track_frames_pairwise", *o)) return st;
-  int w[bba::odom::kMaxScales], ht[bba::odom::kMaxScales];
-  if (!OdometryLevelSizes(h, o->num_scales, w, ht)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "too many pyramid levels for this image size");
-  // (keyframe ids are checked against the published keyframes in the snapshot, before anything is enqueued)
-  return TrackFramesPairwise(h, "bba_track_frames_pairwise", *o, frame_count, frames, count, entries, base_T_frame_estimate, results,
-                             kernel_launches, static_cast<cudaStream_t>(stream));
+  if (bba_status st = CheckOdometryCall(h, fn, o, frame_count, frames, count, entries, base_T_frame_estimate)) return st;
+  return TrackFramesPairwise(h, fn, *o, frame_count, frames, count, entries, base_T_frame_estimate, results, kernel_launches,
+                             static_cast<cudaStream_t>(stream));
 }
 
 bba_status bba_odometry_get_level(bba_handle h, int which, int scale, float* host_depth, uint16_t* host_normals, uint8_t* host_color,

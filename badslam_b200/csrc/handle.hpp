@@ -352,9 +352,7 @@ struct bba_context {
     int readers[2] = {0, 0};   // claims between FrontEndCall::Snapshot and ReleaseSlot
     std::mutex call;           // serialises the front-end calls that use the buffers below and odo / pre
     bba::LumaStaging luma;
-    bba::Texture frame;        // luma of the tracked frame
-    bba::Texture base;         // luma of a base frame given as buffers (bba_track_frame_pairwise_to_frame)
-    std::vector<bba::Texture> frames;   // luma of the distinct frames of a bba_track_frames_pairwise chunk, grown on demand
+    std::vector<bba::Texture> frames;   // luma of the distinct frames of an odometry chunk, grown on demand
   } fe;
 
   // kernels launched by BA-side calls and by front-end calls (bba_kernel_launch_count: the sum); two counters so that the
@@ -464,6 +462,11 @@ template <class Args> void SetSurfelFields(bba_handle h, Args* a) {
 // The luma textures of n >= 1 colour images in device memory (sources[i] -> *out[i]): one extraction launch and one copy per
 // image into its array.  front_end: through fe.luma, counted as front-end launches; otherwise through staging.luma.
 bba_status MakeLumaTextures(bba_handle h, bool front_end, int n, const LumaSource* sources, Texture* const* out, cudaStream_t s);
+// The luma textures of the frames `uses` names (indices into frames, repeats allowed) in one MakeLumaTextures call: the distinct
+// frames in first-use order get (*pool)[0], (*pool)[1], ..., and luma[f] becomes frame f's texture.  The pool grows when it holds
+// fewer textures than there are distinct frames.
+bba_status MakeFrameLumaTextures(bba_handle h, bool front_end, const bba_frame_buffers* frames, const std::vector<int>& uses,
+                                 std::vector<Texture>* pool, cudaTextureObject_t* luma, cudaStream_t s);
 
 // pose_step.cu
 // The surfel count from which a launch over n keyframes puts the surfels into spatial order: sorting costs ~0.1 ms of launches

@@ -190,36 +190,25 @@ bba_status EstimateFramePoses(bba_handle h, int frame_count, const bba_frame_buf
     staging.plane = PitchedBuffer();
     staging.planes = 0;
   }
-  std::vector<int> pool_entry(frame_count, -1);   // a frame's luma texture in the current chunk
-  std::vector<int> chunk_frames;
-  std::vector<LumaSource> sources;
-  std::vector<Texture*> textures;
+  std::vector<cudaTextureObject_t> luma(frame_count);   // the luma textures of the current chunk's frames
+  std::vector<int> frame_of_chunk_entry;
   std::vector<int> ids;
   std::vector<Pose> poses;
   std::vector<double> rec;
   std::vector<unsigned long long> sc;
   for (int begin = 0; begin < count; begin += free_slots) {
     const int n = std::min(free_slots, count - begin);
-    chunk_frames.clear();
-    sources.clear();
-    textures.clear();
-    for (int i = 0; i < n; ++i) {
-      const int f = frame_of_entry ? frame_of_entry[begin + i] : begin + i;
-      if (pool_entry[f] >= 0) continue;
-      pool_entry[f] = static_cast<int>(chunk_frames.size());
-      chunk_frames.push_back(f);
-      sources.push_back(LumaSource{frames[f].color_rgba, frames[f].color_pitch});
-      textures.push_back(&pool[pool_entry[f]]);
-    }
-    bba_status st = MakeLumaTextures(h, /*front_end=*/false, static_cast<int>(chunk_frames.size()), sources.data(), textures.data(), s);
+    frame_of_chunk_entry.resize(n);
+    for (int i = 0; i < n; ++i) frame_of_chunk_entry[i] = frame_of_entry ? frame_of_entry[begin + i] : begin + i;
+    bba_status st = MakeFrameLumaTextures(h, /*front_end=*/false, frames, frame_of_chunk_entry, &pool, luma.data(), s);
     ids.resize(n);
     poses.resize(n);
     for (int i = 0; st == BBA_OK && i < n; ++i) {
-      const int f = frame_of_entry ? frame_of_entry[begin + i] : begin + i;
+      const int f = frame_of_chunk_entry[i];
       Keyframe entry{};
       entry.depth = frames[f].depth; entry.depth_pitch = frames[f].depth_pitch;
       entry.normals = frames[f].normals; entry.normals_pitch = frames[f].normals_pitch;
-      entry.tex = pool[pool_entry[f]].tex;
+      entry.tex = luma[f];
       entry.pose = PoseFromArray(init + 7 * static_cast<size_t>(begin + i));
       entry.activation = BBA_KF_ACTIVE;
       ids[i] = K + i;
@@ -239,7 +228,6 @@ bba_status EstimateFramePoses(bba_handle h, int frame_count, const bba_frame_buf
     h->keyframes.erase(h->keyframes.begin() + K, h->keyframes.end());
     for (int i = 0; i < n; ++i)   // the slots' cost statistics belong to future keyframes
       if (K + i < static_cast<int>(h->kf_cost.size())) h->kf_cost[K + i] = 0.f;
-    for (int f : chunk_frames) pool_entry[f] = -1;
     if (st) return st;
     if (at_estimate)
       for (int i = 0; i < n; ++i) FillPoseCoeffs(h, rec, sc, K + i, at_estimate + begin + i);

@@ -42,6 +42,21 @@ def _as_u16(t: torch.Tensor) -> torch.Tensor:
     return t
 
 
+def _frame_buffers(frames):
+    """The bba_frame_buffers table of a sequence of (depth, normals, colour) device tensors."""
+    bufs = (_lib.FrameBuffers * len(frames))()
+    for b, (depth, normals, color) in zip(bufs, frames):
+        b.depth, b.depth_pitch = depth.data_ptr(), depth.stride(0) * 2
+        b.normals, b.normals_pitch = normals.data_ptr(), normals.stride(0) * 2
+        b.color_rgba, b.color_pitch = color.data_ptr(), color.stride(0)
+    return bufs
+
+
+def _odometry_options(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates, max_iterations_per_scale):
+    return _lib.OdometryOptions(int(num_scales), int(use_pyramid_level_0), int(use_gradmag), int(test_different_initial_estimates),
+                                int(max_iterations_per_scale))
+
+
 class Keyframe:
     """Mirror of vis::Keyframe's buffer-taking constructor (keyframe.cc:41-79): owns the device buffers."""
 
@@ -587,11 +602,7 @@ class DirectBA:
         (global_T_frame_estimates [count, 7], iterations [count], converged [count] bool) and, with with_coeffs, a list of the
         count PoseCoeffs at the returned poses as a fourth element.  The entries run in chunks of as many as there are free
         keyframe slots."""
-        bufs = (_lib.FrameBuffers * len(frames))()
-        for b, (depth, normals, color) in zip(bufs, frames):
-            b.depth, b.depth_pitch = depth.data_ptr(), depth.stride(0) * 2
-            b.normals, b.normals_pitch = normals.data_ptr(), normals.stride(0) * 2
-            b.color_rgba, b.color_pitch = color.data_ptr(), color.stride(0)
+        bufs = _frame_buffers(frames)
         init = np.ascontiguousarray(initial_poses, np.float32).reshape(-1, 7)
         count = len(init)
         fmap = None if frame_of_entry is None else np.ascontiguousarray(frame_of_entry, np.int32)
@@ -615,8 +626,7 @@ class DirectBA:
         p1 = np.ascontiguousarray(base_T_frame_initial_estimate_1, np.float32)
         p2 = p1 if base_T_frame_initial_estimate_2 is None else np.ascontiguousarray(base_T_frame_initial_estimate_2, np.float32)
         out = np.zeros(7, np.float32)
-        o = _lib.OdometryOptions(int(num_scales), int(use_pyramid_level_0), int(use_gradmag), int(test_different_initial_estimates),
-                                 int(max_iterations_per_scale))
+        o = _odometry_options(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates, max_iterations_per_scale)
         res = _lib.OdometryResult()
         F = C.POINTER(C.c_float)
         self._check(self._lib.bba_track_frame_pairwise(
@@ -637,8 +647,7 @@ class DirectBA:
         p1 = np.ascontiguousarray(base_T_frame_initial_estimate_1, np.float32)
         p2 = p1 if base_T_frame_initial_estimate_2 is None else np.ascontiguousarray(base_T_frame_initial_estimate_2, np.float32)
         out = np.zeros(7, np.float32)
-        o = _lib.OdometryOptions(int(num_scales), int(use_pyramid_level_0), int(use_gradmag), int(test_different_initial_estimates),
-                                 int(max_iterations_per_scale))
+        o = _odometry_options(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates, max_iterations_per_scale)
         res = _lib.OdometryResult()
         F = C.POINTER(C.c_float)
         self._check(self._lib.bba_track_frame_pairwise_to_frame(
@@ -656,11 +665,7 @@ class DirectBA:
         entries: a sequence of (base_keyframe_id, base_frame, tracked_frame, base_T_frame_initial_1[, base_T_frame_initial_2]),
         base_keyframe_id -1 meaning frames[base_frame] is the base.  Returns (base_T_frame_estimates [count, 7], a list of the count
         OdometryResult, the kernel launches of the whole call).  The entries run in chunks of _lib.ODOMETRY_CHUNK_ENTRIES."""
-        bufs = (_lib.FrameBuffers * len(frames))()
-        for b, (depth, normals, color) in zip(bufs, frames):
-            b.depth, b.depth_pitch = depth.data_ptr(), depth.stride(0) * 2
-            b.normals, b.normals_pitch = normals.data_ptr(), normals.stride(0) * 2
-            b.color_rgba, b.color_pitch = color.data_ptr(), color.stride(0)
+        bufs = _frame_buffers(frames)
         ents = (_lib.OdometryEntry * len(entries))()
         for e, spec in zip(ents, entries):
             e.base_keyframe_id, e.base_frame, e.tracked_frame = int(spec[0]), int(spec[1]), int(spec[2])
@@ -672,8 +677,7 @@ class DirectBA:
         out = np.zeros((count, 7), np.float32)
         results = (_lib.OdometryResult * count)()
         launches = C.c_uint32()
-        o = _lib.OdometryOptions(int(num_scales), int(use_pyramid_level_0), int(use_gradmag), int(test_different_initial_estimates),
-                                 int(max_iterations_per_scale))
+        o = _odometry_options(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates, max_iterations_per_scale)
         self._check(self._lib.bba_track_frames_pairwise(self._h, C.byref(o), len(frames), bufs, count, ents, out.ctypes.data, results,
                                                         C.byref(launches), self._stream_ptr(stream)))
         return out, list(results), launches.value

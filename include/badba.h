@@ -492,7 +492,7 @@ bba_status bba_preprocess_raw_frame(bba_handle h, const bba_raw_frame_options* o
  * The tracked frame is given like in bba_estimate_frame_pose_for_frame (preprocessed depth, normals, uchar4 colour with
  * .w = luma); poses are base_T_frame as {qx,qy,qz,qw,tx,ty,tz}.  Uses the handle's cameras, depth deformation and residual types.
  * Front-end calls (bba_track_frame_pairwise, bba_track_frame_pairwise_to_frame, bba_track_frames_pairwise and the two parity hooks): the published cameras,
- * a, cfactor, residual types and base keyframe record; their own luma staging plane and textures. */
+ * a, cfactor, residual types and base keyframe records; a luma staging plane and a pool of frame luma textures of the front end. */
 typedef struct {
   int num_scales;                        /* BadSlamConfig::num_scales, default 5 (bad_slam_config.h:167); 1..8 */
   int use_pyramid_level_0;               /* RunOdometry passes true (bad_slam.cc:923) */
@@ -517,7 +517,9 @@ bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* op
 /* The same against a base frame that is not a keyframe (yet): its preprocessed depth, normals and uchar4 colour buffers, what
  * bba_add_keyframe takes -- the keyframe BadSlam's odometry tracks against while it still waits in the BA thread's queue
  * (bad_slam.cc:831-950).  The result equals that of bba_track_frame_pairwise against the same buffers registered as a
- * keyframe, bit for bit; kernel_launches counts one more launch (the base frame's luma).  Nothing of the base is kept. */
+ * keyframe, bit for bit, with the same kernel_launches (one luma launch serves both frames).  Nothing of the base is kept.
+ * Both single-pair calls are the one-entry case of bba_track_frames_pairwise below, with its checks: a failed check enqueues
+ * nothing. */
 bba_status bba_track_frame_pairwise_to_frame(bba_handle h, const bba_odometry_options* options,
                                              const uint16_t* base_depth, size_t base_depth_pitch,
                                              const uint16_t* base_normals, size_t base_normals_pitch,

@@ -162,10 +162,7 @@ class DirectBA {
                           const std::vector<SE3f>& global_T_frame_initial_estimates, std::vector<SE3f>* out_global_T_frame_estimates,
                           const std::vector<int>& frame_of_entry = {}, std::vector<bba_pose_coeffs>* at_estimate = nullptr) {
     const size_t count = global_T_frame_initial_estimates.size();
-    std::vector<bba_frame_buffers> buffers(frames.size());
-    for (size_t f = 0; f < frames.size(); ++f)
-      buffers[f] = {frames[f].depth.address, frames[f].depth.pitch_bytes, frames[f].normals.address, frames[f].normals.pitch_bytes,
-                    frames[f].color_rgba.address, frames[f].color_rgba.pitch_bytes};
+    const std::vector<bba_frame_buffers> buffers = MakeFrameBuffers(frames);
     std::vector<float> init(7 * count), out(7 * count);
     for (size_t i = 0; i < count; ++i) std::memcpy(init.data() + 7 * i, global_T_frame_initial_estimates[i].data(), sizeof(float) * 7);
     if (at_estimate) at_estimate->resize(count);
@@ -185,12 +182,7 @@ class DirectBA {
                           DeviceImage<uint8_t> tracked_color_buffer_rgba, bool test_different_initial_estimates,
                           const SE3f& base_T_frame_initial_estimate_1, const SE3f& base_T_frame_initial_estimate_2,
                           SE3f* out_base_T_frame_estimate, int num_scales = 5, bba_odometry_result* result = nullptr) {
-    bba_odometry_options o{};
-    o.num_scales = num_scales;
-    o.use_pyramid_level_0 = use_pyramid_level_0;
-    o.use_gradmag = use_gradmag;
-    o.test_different_initial_estimates = test_different_initial_estimates;
-    o.max_iterations_per_scale = 30;
+    const bba_odometry_options o = MakeOdometryOptions(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates);
     float out[7];
     Check(bba_track_frame_pairwise(h_, &o, base_keyframe_id, tracked_depth_buffer.address, tracked_depth_buffer.pitch_bytes,
                                    tracked_normals_buffer.address, tracked_normals_buffer.pitch_bytes, tracked_color_buffer_rgba.address,
@@ -208,12 +200,7 @@ class DirectBA {
                           DeviceImage<uint8_t> tracked_color_buffer_rgba, bool test_different_initial_estimates,
                           const SE3f& base_T_frame_initial_estimate_1, const SE3f& base_T_frame_initial_estimate_2,
                           SE3f* out_base_T_frame_estimate, int num_scales = 5, bba_odometry_result* result = nullptr) {
-    bba_odometry_options o{};
-    o.num_scales = num_scales;
-    o.use_pyramid_level_0 = use_pyramid_level_0;
-    o.use_gradmag = use_gradmag;
-    o.test_different_initial_estimates = test_different_initial_estimates;
-    o.max_iterations_per_scale = 30;
+    const bba_odometry_options o = MakeOdometryOptions(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates);
     float out[7];
     Check(bba_track_frame_pairwise_to_frame(h_, &o, base_depth_buffer.address, base_depth_buffer.pitch_bytes, base_normals_buffer.address,
                                             base_normals_buffer.pitch_bytes, base_color_buffer_rgba.address,
@@ -233,16 +220,8 @@ class DirectBA {
                            bool use_pyramid_level_0, bool use_gradmag, bool test_different_initial_estimates,
                            std::vector<SE3f>* out_base_T_frame_estimates, int num_scales = 5,
                            std::vector<bba_odometry_result>* results = nullptr) {
-    bba_odometry_options o{};
-    o.num_scales = num_scales;
-    o.use_pyramid_level_0 = use_pyramid_level_0;
-    o.use_gradmag = use_gradmag;
-    o.test_different_initial_estimates = test_different_initial_estimates;
-    o.max_iterations_per_scale = 30;
-    std::vector<bba_frame_buffers> buffers(frames.size());
-    for (size_t f = 0; f < frames.size(); ++f)
-      buffers[f] = {frames[f].depth.address, frames[f].depth.pitch_bytes, frames[f].normals.address, frames[f].normals.pitch_bytes,
-                    frames[f].color_rgba.address, frames[f].color_rgba.pitch_bytes};
+    const bba_odometry_options o = MakeOdometryOptions(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates);
+    const std::vector<bba_frame_buffers> buffers = MakeFrameBuffers(frames);
     const size_t count = entries.size();
     std::vector<float> out(7 * count);
     if (results) results->resize(count);
@@ -402,6 +381,24 @@ class DirectBA {
  private:
   void Check(bba_status s, const char* where) const {
     if (s != BBA_OK) throw Error(s, std::string(where) + ": " + (h_ ? bba_last_error(h_) : "no handle"));
+  }
+  // The odometry options of the TrackFramePairwise forms: the reference's 30 iterations per scale.
+  static bba_odometry_options MakeOdometryOptions(int num_scales, bool use_pyramid_level_0, bool use_gradmag,
+                                                  bool test_different_initial_estimates) {
+    bba_odometry_options o{};
+    o.num_scales = num_scales;
+    o.use_pyramid_level_0 = use_pyramid_level_0;
+    o.use_gradmag = use_gradmag;
+    o.test_different_initial_estimates = test_different_initial_estimates;
+    o.max_iterations_per_scale = 30;
+    return o;
+  }
+  static std::vector<bba_frame_buffers> MakeFrameBuffers(const std::vector<FrameImages>& frames) {
+    std::vector<bba_frame_buffers> buffers(frames.size());
+    for (size_t f = 0; f < frames.size(); ++f)
+      buffers[f] = {frames[f].depth.address, frames[f].depth.pitch_bytes, frames[f].normals.address, frames[f].normals.pitch_bytes,
+                    frames[f].color_rgba.address, frames[f].color_rgba.pitch_bytes};
+    return buffers;
   }
   bba_handle h_ = nullptr;
   bba_ba_result last_result_{};

@@ -8,8 +8,9 @@ What is demanded:
     or two initial estimates, 1, 3 and 5 pyramid levels;
   * default mode: iteration counts within one of the single calls', poses within the tolerance tests/test_gpu_odometry.py
     applies against the reference (1e-5 m / rad plus ten times the run-to-run drift of the single calls);
-  * 4 + (num_scales - 1) launches per chunk, whatever the entry count;
-  * every bad argument is refused before anything is enqueued: launch counter and keyframe states unchanged;
+  * 4 + (num_scales - 1) launches per chunk, whatever the entry count, and so per single-pair call of either form;
+  * every bad argument is refused before anything is enqueued, by the batch and by both single-pair forms: launch counter and
+    keyframe states unchanged;
   * the parity hooks describe the batch's last entry, bit for bit as after a single call on that pair;
   * a batch issued while a bundle adjustment holds at an iteration boundary equals the same batch run alone.
 """
@@ -179,7 +180,7 @@ def test_default_mode_against_single_calls(mods):
     print(f"default mode, {n} entries: largest pose difference to the single calls {worst:.2e}")
 
 
-def test_launches_per_chunk(mods):
+def test_launches_per_chunk_and_per_single_pair_call(mods):
     S, DirectBA, _lib = mods
     sc, ba, pairs = make(S, DirectBA, "tiny", deterministic=False)
     chunk = _lib.ODOMETRY_CHUNK_ENTRIES
@@ -192,10 +193,10 @@ def test_launches_per_chunk(mods):
             assert launches == chunks * per_chunk, (num_scales, count, launches)
             assert ba.kernel_launch_count() - before == launches
             assert all(r.kernel_launches == per_chunk for r in res)
-    # the single-pair calls are unchanged: the keyframe form and the buffer form (one more luma launch)
+    # the single-pair calls are one-entry chunks: the keyframe form and the buffer form (one luma launch for both frames)
     e = pairs.entries(2)
     assert single(ba, pairs, e[0], num_scales=3)[1].kernel_launches == 6
-    assert single(ba, pairs, e[1], num_scales=3)[1].kernel_launches == 7
+    assert single(ba, pairs, e[1], num_scales=3)[1].kernel_launches == 6
 
 
 def test_bad_arguments_change_nothing(mods):
@@ -249,6 +250,35 @@ def test_bad_arguments_change_nothing(mods):
     assert lib.bba_track_frames_pairwise(h, C.byref(o), nf, None, 1, ents, out.ctypes.data, None, None, None) == _lib.ERR_INVALID_ARGUMENT
     assert lib.bba_track_frames_pairwise(h, C.byref(o), nf, bufs, 1, None, out.ctypes.data, None, None, None) == _lib.ERR_INVALID_ARGUMENT
     assert lib.bba_track_frames_pairwise(h, C.byref(o), nf, bufs, 1, ents, None, None, None, None) == _lib.ERR_INVALID_ARGUMENT
+
+    # the single-pair forms refuse the same arguments before anything is enqueued, and what an entry cannot express
+    def refused_single(status, kf, frame, base=None, **kw):
+        with pytest.raises(_lib.BadBAError) as err:
+            if base is None:
+                ba.TrackFramePairwise(None, kf, *frame, e[3], e[4], **kw)
+            else:
+                ba.TrackFramePairwiseToFrame(None, *base, *frame, e[3], e[4], **kw)
+        assert err.value.status == status, (err.value, kf, base is None, kw)
+
+    frame = pairs.frames[0]
+    for base in (None, pairs.frames[1]):
+        refused_single(_lib.ERR_INVALID_ARGUMENT, 0, frame, base, num_scales=8)     # 160x120 has no level 7
+        refused_single(_lib.ERR_INVALID_ARGUMENT, 0, frame, base, num_scales=0)
+        refused_single(_lib.ERR_INVALID_ARGUMENT, 0, frame, base, num_scales=9)
+        refused_single(_lib.ERR_INVALID_ARGUMENT, 0, frame, base, num_scales=1, use_pyramid_level_0=False)
+        refused_single(_lib.ERR_INVALID_ARGUMENT, 0, narrow, base, num_scales=3)
+    refused_single(_lib.ERR_INVALID_ARGUMENT, 0, frame, narrow, num_scales=3)      # a base frame's pitch
+    refused_single(_lib.ERR_INVALID_ARGUMENT, K, frame, num_scales=3)              # no such keyframe
+    refused_single(_lib.ERR_INVALID_ARGUMENT, -1, frame, num_scales=3)
+    fb = bufs[0]
+    p1 = np.ascontiguousarray(e[3], np.float32)
+    F = C.POINTER(C.c_float)
+    for init1, init2, est in ((None, p1, out), (p1, None, out), (p1, p1, None)):   # test_different_initial_estimates needs init2
+        args = (None if init1 is None else init1.ctypes.data_as(F), None if init2 is None else init2.ctypes.data_as(F),
+                None if est is None else est.ctypes.data_as(F), None, None)
+        frame_args = (fb.depth, fb.depth_pitch, fb.normals, fb.normals_pitch, fb.color_rgba, fb.color_pitch)
+        assert lib.bba_track_frame_pairwise(h, C.byref(o), 0, *frame_args, *args) == _lib.ERR_INVALID_ARGUMENT
+        assert lib.bba_track_frame_pairwise_to_frame(h, C.byref(o), *frame_args, *frame_args, *args) == _lib.ERR_INVALID_ARGUMENT
     torch.cuda.synchronize()
     assert ba.kernel_launch_count() == launches
     assert all(np.asarray(a).tobytes() == np.asarray(b).tobytes() for a, b in zip(ba.GetKeyframeStates(), states))
@@ -260,9 +290,12 @@ def test_bad_arguments_change_nothing(mods):
     frame = (torch.zeros((120, 160), dtype=torch.int16, device="cuda"), torch.zeros((120, 160), dtype=torch.int16, device="cuda"),
              torch.zeros((76, 100, 4), dtype=torch.uint8, device="cuda"))
     before = ba2.kernel_launch_count()
-    with pytest.raises(_lib.BadBAError) as err:
-        ba2.TrackFramesPairwise(None, [frame], [(-1, 0, 0, IDENT, IDENT)], num_scales=3, use_pyramid_level_0=False)
-    assert err.value.status == _lib.ERR_UNSUPPORTED
+    for call in (lambda: ba2.TrackFramesPairwise(None, [frame], [(-1, 0, 0, IDENT, IDENT)], num_scales=3, use_pyramid_level_0=False),
+                 lambda: ba2.TrackFramePairwise(None, 0, *frame, IDENT, IDENT, num_scales=3, use_pyramid_level_0=False),
+                 lambda: ba2.TrackFramePairwiseToFrame(None, *frame, *frame, IDENT, IDENT, num_scales=3, use_pyramid_level_0=False)):
+        with pytest.raises(_lib.BadBAError) as err:
+            call()
+        assert err.value.status == _lib.ERR_UNSUPPORTED
     assert ba2.kernel_launch_count() == before
 
 
