@@ -376,14 +376,7 @@ bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, 
   uint32_t deleted_total = 0;
   if (world > 1) {
     if (!peers_mapped && K > 0) {
-      uint32_t shard_len;
-      ShardSurfels(N, rank, world, nullptr, &shard_len);
-      if (bba_status st = ReserveExchange(h, static_cast<size_t>(world) * 2 * shard_len)) return st;
-      const size_t slice_floats = static_cast<size_t>(2) * shard_len;
-      BBA_LAUNCH(h, h->launches, LaunchPackStatsShard, h->surfels, a.pitch, N, rank, world, shard_len,
-                 h->xchg.d_exchange + slice_floats * rank, s);
-      h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLGATHER, h->xchg.d_exchange, slice_floats * sizeof(float), s);
-      BBA_LAUNCH(h, h->launches, LaunchUnpackStatsShards, h->surfels, a.pitch, N, shard_len, world, rank, h->xchg.d_exchange, s);
+      if (bba_status st = ExchangeShards(h, bba::ShardRows{{bba::kRowX, bba::kRowRadiusSq}, 2, 0}, nullptr, s)) return st;
     }
     // deleted count of this shard as two exactly representable floats (low 12 bits, the rest), summed over the ranks
     BBA_CUDA(h, h->xchg.d_count_xchg.Reserve(2));

@@ -281,7 +281,7 @@ struct bba_context {
   struct Exchange {
     bba_collective_fn collective = nullptr;
     void* collective_user = nullptr;
-    bba::DeviceBuffer<float> d_exchange;    // [world][kShardRows][shard_len] floats
+    bba::DeviceBuffer<float> d_exchange;    // [world][rows][shard_len] floats, rows <= kShardRows (ExchangeShards)
     bba::DeviceBuffer<float> d_pose_pack;   // [max_kf][kPoseSlot] floats
     bba::PinnedBuffer<float> h_pose_pack;
     bba::DeviceBuffer<int> d_local_ids;     // [max_kf]
@@ -481,8 +481,8 @@ uint32_t LocalCountBelow(uint32_t global_end, int rank, int world);
 void AssignKeyframes(bba_handle h, const std::vector<int>& ids, std::vector<int>* owner);
 bba_status CheckCollective(bba_handle h);
 bba_status PeerFence(bba_handle h, cudaStream_t s);
+bba_status ExchangeShards(bba_handle h, const ShardRows& rows, const uint32_t* perm, cudaStream_t s);
 bba_status ExchangeGeometry(bba_handle h, cudaStream_t s);
-bba_status ReserveExchange(bba_handle h, size_t need);
 void UnmapPeers(bba_handle h);
 
 // The range of this rank's surfel shard (all surfels on one GPU) in kernel arguments.

@@ -948,25 +948,30 @@ LaunchResult LaunchPositionAndDescriptor(const GeometryArgs& a, int sm_count, cu
 // ------------------------------------------------------------------------------------------------
 // Multi-GPU exchange helpers (the collectives themselves run in the host's NCCL communicator).
 
-__constant__ int kShardRowIds[kShardRows - 1] = {kRowX, kRowY, kRowZ, kRowNormal, kRowD1, kRowD2};
-
+// Both kernels loop over kShardRows - 1 constant slots, so that rows.ids[r] is read straight from the kernel arguments, and load
+// every row before the first store, so that the loads are in flight together.
 __global__ void __launch_bounds__(256) PackShardKernel(const float* __restrict__ surfels, uint32_t pitch,
-                                                       const uint8_t* __restrict__ active, uint32_t n, const uint32_t* __restrict__ perm,
-                                                       uint32_t rank, uint32_t world, uint32_t shard_len, float* __restrict__ slice) {
+                                                       const uint8_t* __restrict__ active, uint32_t n, ShardRows rows,
+                                                       const uint32_t* __restrict__ perm, uint32_t rank, uint32_t world, uint32_t shard_len,
+                                                       float* __restrict__ slice) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;   // local index
   if (c >= shard_len) return;
   const uint32_t s = SurfelShardToGlobal(c, rank, world);   // stream position
   const bool in = s < n;
   const uint32_t i = in && perm ? __ldg(perm + s) : s;
+  float v[kShardRows];
+#pragma unroll
+  for (int r = 0; r < kShardRows - 1; ++r) v[r] = in && r < rows.count ? surfels[static_cast<size_t>(rows.ids[r]) * pitch + i] : 0.f;
+  v[kShardRows - 1] = in && rows.active ? static_cast<float>(active[i]) : 0.f;
 #pragma unroll
   for (int r = 0; r < kShardRows - 1; ++r)
-    slice[static_cast<size_t>(r) * shard_len + c] = in ? surfels[static_cast<size_t>(kShardRowIds[r]) * pitch + i] : 0.f;
-  slice[static_cast<size_t>(kShardRows - 1) * shard_len + c] = in ? static_cast<float>(active[i]) : 0.f;
+    if (r < rows.count) slice[static_cast<size_t>(r) * shard_len + c] = v[r];
+  if (rows.active) slice[static_cast<size_t>(rows.count) * shard_len + c] = v[kShardRows - 1];
 }
 
 __global__ void __launch_bounds__(256) UnpackShardsKernel(float* __restrict__ surfels, uint32_t pitch, uint8_t* __restrict__ active,
-                                                          uint32_t n, const uint32_t* __restrict__ perm, uint32_t shard_len, uint32_t world,
-                                                          int skip_rank, const float* __restrict__ buffer) {
+                                                          uint32_t n, ShardRows rows, const uint32_t* __restrict__ perm, uint32_t shard_len,
+                                                          uint32_t world, int skip_rank, const float* __restrict__ buffer) {
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;   // stream position
   if (s >= n) return;
   const uint32_t granule = s >> kShardGranuleShift;
@@ -974,24 +979,28 @@ __global__ void __launch_bounds__(256) UnpackShardsKernel(float* __restrict__ su
   if (static_cast<int>(rank) == skip_rank) return;
   const uint32_t c = ((granule / world) << kShardGranuleShift) | (s & ((1u << kShardGranuleShift) - 1u));
   const uint32_t i = perm ? __ldg(perm + s) : s;
-  const float* slice = buffer + static_cast<size_t>(rank) * kShardRows * shard_len;
+  const float* slice = buffer + static_cast<size_t>(rank) * (rows.count + rows.active) * shard_len;
+  float v[kShardRows];
+#pragma unroll
+  for (int r = 0; r < kShardRows - 1; ++r) v[r] = r < rows.count ? slice[static_cast<size_t>(r) * shard_len + c] : 0.f;
+  v[kShardRows - 1] = rows.active ? slice[static_cast<size_t>(rows.count) * shard_len + c] : 0.f;
 #pragma unroll
   for (int r = 0; r < kShardRows - 1; ++r)
-    surfels[static_cast<size_t>(kShardRowIds[r]) * pitch + i] = slice[static_cast<size_t>(r) * shard_len + c];
-  active[i] = static_cast<uint8_t>(slice[static_cast<size_t>(kShardRows - 1) * shard_len + c]);
+    if (r < rows.count) surfels[static_cast<size_t>(rows.ids[r]) * pitch + i] = v[r];
+  if (rows.active) active[i] = static_cast<uint8_t>(v[kShardRows - 1]);
 }
 
-LaunchResult LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t rank,
-                             uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream) {
+LaunchResult LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, ShardRows rows, const uint32_t* perm,
+                             uint32_t rank, uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream) {
   if (shard_len == 0) return {};
-  PackShardKernel<<<(shard_len + 255) / 256, 256, 0, stream>>>(surfels, pitch, active, n, perm, rank, world, shard_len, slice);
+  PackShardKernel<<<(shard_len + 255) / 256, 256, 0, stream>>>(surfels, pitch, active, n, rows, perm, rank, world, shard_len, slice);
   return {1};
 }
 
-LaunchResult LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t shard_len,
-                                int world, int skip_rank, const float* buffer, cudaStream_t stream) {
+LaunchResult LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, ShardRows rows, const uint32_t* perm,
+                                uint32_t shard_len, int world, int skip_rank, const float* buffer, cudaStream_t stream) {
   if (n == 0) return {};
-  UnpackShardsKernel<<<(n + 255) / 256, 256, 0, stream>>>(surfels, pitch, active, n, perm, shard_len, static_cast<uint32_t>(world),
+  UnpackShardsKernel<<<(n + 255) / 256, 256, 0, stream>>>(surfels, pitch, active, n, rows, perm, shard_len, static_cast<uint32_t>(world),
                                                           skip_rank, buffer);
   return {1};
 }

@@ -155,13 +155,18 @@ constexpr uint32_t kShardGranuleShift = 8;
 __host__ __device__ inline uint32_t SurfelShardToGlobal(uint32_t local, uint32_t rank, uint32_t world) {
   return world <= 1 ? local : ((((local >> kShardGranuleShift) * world + rank) << kShardGranuleShift) | (local & ((1u << kShardGranuleShift) - 1u)));
 }
-// Exchange of the shards: 7 rows (x y z normal d1 d2 active-as-float) x shard_len floats per rank, in local index order.  The
-// shards are the geometry step's: granules of stream positions, surfel perm[s] at position s (perm null: the caller's order).
-constexpr int kShardRows = 7;
-LaunchResult LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t rank,
-                             uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream);
-LaunchResult LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, const uint32_t* perm, uint32_t shard_len, int world,
-                                int skip_rank, const float* buffer, cudaStream_t stream);
+// Exchange of the shards: rows.count surfel rows, then the active flags as floats when rows.active, x shard_len floats per rank,
+// in local index order.  The shards are granules of stream positions, surfel perm[s] at position s (perm null: the caller's order).
+constexpr int kShardRows = 7;   // at most: x y z normal d1 d2 + active (the geometry step's)
+struct ShardRows {
+  int ids[kShardRows - 1];      // SurfelRow of each slice row
+  int count;                    // of ids
+  int active;                   // 1: one more slice row with the active flags
+};
+LaunchResult LaunchPackShard(const float* surfels, uint32_t pitch, const uint8_t* active, uint32_t n, ShardRows rows, const uint32_t* perm,
+                             uint32_t rank, uint32_t world, uint32_t shard_len, float* slice, cudaStream_t stream);
+LaunchResult LaunchUnpackShards(float* surfels, uint32_t pitch, uint8_t* active, uint32_t n, ShardRows rows, const uint32_t* perm,
+                                uint32_t shard_len, int world, int skip_rank, const float* buffer, cudaStream_t stream);
 // Pose results of the locally owned keyframes -> [K][17] floats (zeros elsewhere) for the sum all-reduce.
 constexpr int kPoseSlot = 17;   // 7 pose, iterations, converged, 8 first-iteration statistics
 LaunchResult LaunchPackPoseResults(const int* ids, int n, const float* pose_est, const int* iterations, const int* converged,
@@ -264,11 +269,6 @@ struct SurfelStatsArgs {
   PeerSet peers;
 };
 LaunchResult LaunchObservationStats(SurfelStatsArgs a, int sm_count, cudaStream_t stream);
-// Exchange of the end tasks' two result rows through the host collective (no mapped peers): slice = [2][shard_len] floats.
-LaunchResult LaunchPackStatsShard(const float* surfels, uint32_t pitch, uint32_t n, uint32_t rank, uint32_t world, uint32_t shard_len, float* slice,
-                                  cudaStream_t stream);
-LaunchResult LaunchUnpackStatsShards(float* surfels, uint32_t pitch, uint32_t n, uint32_t shard_len, int world, int skip_rank, const float* buffer,
-                                     cudaStream_t stream);
 // Exclusive scan of n u32 counts, shared by the compaction and the surfel creation: block_sums needs ScanScratchWords(n) words,
 // and block_sums[ScanTotalIndex(n)] receives the sum of all counts.
 uint32_t ScanScratchWords(uint32_t n);

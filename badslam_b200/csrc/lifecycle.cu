@@ -484,41 +484,6 @@ LaunchResult LaunchCreateSurfels(const LifecycleArgs& a, const unsigned int* ind
   return {1};
 }
 
-// rows x (deletion marker) and radius^2 of this rank's shard, in local index order
-__global__ void __launch_bounds__(256) PackStatsShardKernel(const float* __restrict__ surfels, uint32_t pitch, uint32_t n, uint32_t rank,
-                                                            uint32_t world, uint32_t shard_len, float* __restrict__ slice) {
-  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= shard_len) return;
-  const uint32_t i = SurfelShardToGlobal(c, rank, world);
-  const bool in = i < n;
-  slice[c] = in ? surfels[static_cast<size_t>(kRowX) * pitch + i] : 0.f;
-  slice[static_cast<size_t>(shard_len) + c] = in ? surfels[static_cast<size_t>(kRowRadiusSq) * pitch + i] : 0.f;
-}
-__global__ void __launch_bounds__(256) UnpackStatsShardsKernel(float* __restrict__ surfels, uint32_t pitch, uint32_t n, uint32_t shard_len,
-                                                               uint32_t world, int skip_rank, const float* __restrict__ buffer) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t granule = i >> kShardGranuleShift;
-  const uint32_t rank = granule % world;
-  if (static_cast<int>(rank) == skip_rank) return;
-  const uint32_t c = ((granule / world) << kShardGranuleShift) | (i & ((1u << kShardGranuleShift) - 1u));
-  const float* slice = buffer + static_cast<size_t>(rank) * 2 * shard_len;
-  surfels[static_cast<size_t>(kRowX) * pitch + i] = slice[c];
-  surfels[static_cast<size_t>(kRowRadiusSq) * pitch + i] = slice[static_cast<size_t>(shard_len) + c];
-}
-LaunchResult LaunchPackStatsShard(const float* surfels, uint32_t pitch, uint32_t n, uint32_t rank, uint32_t world, uint32_t shard_len,
-                                  float* slice, cudaStream_t stream) {
-  if (shard_len == 0) return {};
-  PackStatsShardKernel<<<(shard_len + 255) / 256, 256, 0, stream>>>(surfels, pitch, n, rank, world, shard_len, slice);
-  return {1};
-}
-LaunchResult LaunchUnpackStatsShards(float* surfels, uint32_t pitch, uint32_t n, uint32_t shard_len, int world, int skip_rank,
-                                     const float* buffer, cudaStream_t stream) {
-  if (n == 0) return {};
-  UnpackStatsShardsKernel<<<(n + 255) / 256, 256, 0, stream>>>(surfels, pitch, n, shard_len, static_cast<uint32_t>(world), skip_rank, buffer);
-  return {1};
-}
-
 LaunchResult LaunchObservationStats(SurfelStatsArgs a, int sm_count, cudaStream_t stream) {
   if (a.local_count == 0 || a.kf_count <= 0) return {};
   int per_sm = 0;

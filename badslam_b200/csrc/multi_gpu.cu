@@ -95,34 +95,32 @@ bba_status CheckCollective(bba_handle h) {
   return BBA_OK;
 }
 
-// The exchange buffer with room for `need` floats, sized for max_surfel_count surfels (or more) when it grows.
-bba_status ReserveExchange(bba_handle h, size_t need) {
-  const int world = h->cfg.world_size;
-  uint32_t max_len;
+// Every rank has updated `rows` of its own surfel shard only (granules of stream positions, surfel perm[s] at position s; perm
+// null: the caller's order): each rank packs them into its slice of the exchange buffer, one all-gather, and every rank unpacks
+// the other ranks' slices.  The buffer grows to room for kShardRows rows of max_surfel_count surfels (or more).
+bba_status ExchangeShards(bba_handle h, const ShardRows& rows, const uint32_t* perm, cudaStream_t s) {
+  auto& x = h->xchg;
+  const int world = h->cfg.world_size, rank = h->cfg.rank;
+  uint32_t shard_len, max_len;
+  ShardSurfels(h->surfels_size, rank, world, nullptr, &shard_len);
   ShardSurfels(std::max(h->cfg.max_surfel_count, h->surfels_size), 0, world, nullptr, &max_len);
-  BBA_CUDA(h, h->xchg.d_exchange.Reserve(need, static_cast<size_t>(world) * kShardRows * max_len));
+  const size_t slice_floats = static_cast<size_t>(rows.count + rows.active) * shard_len;
+  BBA_CUDA(h, x.d_exchange.Reserve(world * slice_floats, static_cast<size_t>(world) * kShardRows * max_len));
+  const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
+  BBA_LAUNCH(h, h->launches, LaunchPackShard, h->surfels, pitch, h->active, h->surfels_size, rows, perm, rank, world, shard_len,
+             x.d_exchange + slice_floats * rank, s);
+  x.collective(x.collective_user, BBA_COLLECTIVE_ALLGATHER, x.d_exchange, slice_floats * sizeof(float), s);
+  BBA_LAUNCH(h, h->launches, LaunchUnpackShards, h->surfels, pitch, h->active, h->surfels_size, rows, perm, shard_len, world, rank,
+             x.d_exchange, s);
   return BBA_OK;
 }
 
-// After the geometry step every rank has updated only its own surfel shard (granules of the order the geometry launches used):
-// one all-gather makes the replicas equal.
+// After the geometry step every rank has updated only its own surfel shard (granules of the order the geometry launches used).
 bba_status ExchangeGeometry(bba_handle h, cudaStream_t s) {
   if (h->cfg.world_size <= 1 || h->surfels_size == 0) return BBA_OK;
-  auto& x = h->xchg;
-  const int world = h->cfg.world_size, rank = h->cfg.rank;
   // the geometry kernels already stored the updated rows into every replica over NVLink: only a barrier is left
-  if (x.peers.count == world - 1) return Barrier(h, s);
-  uint32_t shard_len;
-  ShardSurfels(h->surfels_size, rank, world, nullptr, &shard_len);
-  if (bba_status st = ReserveExchange(h, static_cast<size_t>(world) * kShardRows * shard_len)) return st;
-  const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
-  const size_t slice_floats = static_cast<size_t>(kShardRows) * shard_len;
-  BBA_LAUNCH(h, h->launches, LaunchPackShard, h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, rank, world, shard_len,
-             x.d_exchange + slice_floats * rank, s);
-  x.collective(x.collective_user, BBA_COLLECTIVE_ALLGATHER, x.d_exchange, slice_floats * sizeof(float), s);
-  BBA_LAUNCH(h, h->launches, LaunchUnpackShards, h->surfels, pitch, h->active, h->surfels_size, h->geo.perm, shard_len, world, rank,
-             x.d_exchange, s);
-  return BBA_OK;
+  if (h->xchg.peers.count == h->cfg.world_size - 1) return Barrier(h, s);
+  return ExchangeShards(h, ShardRows{{kRowX, kRowY, kRowZ, kRowNormal, kRowD1, kRowD2}, 6, 1}, h->geo.perm, s);
 }
 
 // A barrier across the ranks in front of kernels that write into the peers' replicas, needed only when a replicated pass ran
