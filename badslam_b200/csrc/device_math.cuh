@@ -54,6 +54,16 @@ struct __align__(16) KfDevice {
 };
 static_assert(sizeof(KfDevice) == 96, "KfDevice layout");
 
+// A keyframe record as a kernel holds it in registers (LoadKfShared / LoadKfGlobal, persistent.cuh).
+struct KfRegs {
+  float T[12];
+  const uint16_t* depth;
+  const uint16_t* normals;
+  cudaTextureObject_t tex;
+  uint32_t depth_pitch, normals_pitch;
+  int activation;
+};
+
 // Order-preserving map of a float onto an unsigned int (for integer min / max reductions), and back.
 __device__ __forceinline__ unsigned int OrderedBits(float f) {
   const unsigned int u = __float_as_uint(f);
@@ -220,6 +230,17 @@ __device__ __forceinline__ PixelLoads LoadPixel(const CameraParams& cam, const u
   return l;
 }
 
+// The pair's calibrated depth, rotated normal and pixel ray (into *r), and the standard deviation of its depth: the depth
+// threshold, the largest |lp.z - d| of an associated pair, is kDepthTukey times that.
+__device__ __forceinline__ float PixelDepthStddev(const CameraParams& cam, const float* __restrict__ T, const Vec3& n,
+                                                  const PixelLoads& l, Assoc* r) {
+  r->d = RawToCalibratedDepth(cam.a, l.cf, cam.raw_to_float, l.measured);
+  r->ln = Rotate(T, n);
+  r->nx = cam.fx_inv * r->px + cam.cx_inv;
+  r->ny = cam.fy_inv * r->py + cam.cy_inv;
+  return (kDepthUncertaintyFactor * fabsf(r->ln.x * r->nx + r->ln.y * r->ny + r->ln.z) * (r->d * r->d)) / cam.baseline_fx;
+}
+
 // Step C: the association tests.  Returns the stage reached: 1 in image only, 2 passed valid-depth + depth-threshold +
 // facing tests, 3 associated.
 __device__ __forceinline__ int Associate(const CameraParams& cam, const float* __restrict__ T, const Vec3& n, const PixelLoads& l,
@@ -229,12 +250,7 @@ __device__ __forceinline__ int Associate(const CameraParams& cam, const float* _
   // test (three serial L2 round trips per pair); ~99 % of the in-image pairs pass every test anyway.  The predicates are the
   // reference's, including how they treat NaN (a comparison with NaN is false = "test passed", as in its `if (...) return`).
   const bool invalid = (l.measured & kInvalidDepthBit) != 0;
-  r->d = RawToCalibratedDepth(cam.a, l.cf, cam.raw_to_float, l.measured);
-  r->ln = Rotate(T, n);
-  r->nx = cam.fx_inv * r->px + cam.cx_inv;
-  r->ny = cam.fy_inv * r->py + cam.cy_inv;
-  const float stddev =
-      (kDepthUncertaintyFactor * fabsf(r->ln.x * r->nx + r->ln.y * r->ny + r->ln.z) * (r->d * r->d)) / cam.baseline_fx;
+  const float stddev = PixelDepthStddev(cam, T, n, l, r);
   const bool too_far = fabsf(r->lp.z - r->d) > kDepthTukey * stddev;
   // The reference tests (1 / |lp|) * dot(lp, ln) > 0 (surfel_projection_nvcc_only.cuh:104-108); for the finite,
   // positive |lp| of a point in front of the camera that is the sign of the dot product alone.
@@ -242,6 +258,22 @@ __device__ __forceinline__ int Associate(const CameraParams& cam, const float* _
   r->kf_normal = l.kf_normal;
   const bool incompatible = Dot(r->ln, U16ToImageSpaceNormal(l.kf_normal)) < kCosNormalCompat;
   return (invalid | too_far | back_facing) ? 1 : (incompatible ? 2 : 3);
+}
+
+// The association test that also reports free-space violations (IsAssociatedWithPixel<true>, surfel_projection_nvcc_only.cuh:
+// 48-236): the pixel's surface lies behind the surfel by more than the depth threshold.  The reference's early-outs in its order,
+// with its NaN behaviour (a comparison with NaN counts as "test passed").
+enum FreeSpaceTest { kFreeSpaceNeither = 0, kFreeSpaceAssociated, kFreeSpaceViolation };
+__device__ __forceinline__ FreeSpaceTest AssociateFreeSpace(const CameraParams& cam, const float* __restrict__ T, const Vec3& n,
+                                                            const PixelLoads& l, Assoc* r) {
+  if (l.measured & kInvalidDepthBit) return kFreeSpaceNeither;
+  const float thr = kDepthTukey * PixelDepthStddev(cam, T, n, l, r);
+  const float diff = r->d - r->lp.z;
+  if (diff > thr) return kFreeSpaceViolation;
+  if (diff < -thr) return kFreeSpaceNeither;
+  if (Dot(r->lp, r->ln) > 0) return kFreeSpaceNeither;
+  if (Dot(r->ln, U16ToImageSpaceNormal(l.kf_normal)) < kCosNormalCompat) return kFreeSpaceNeither;
+  return kFreeSpaceAssociated;
 }
 
 // All three steps.  Returns 0 culled / outside, else the stage of Associate().
@@ -366,6 +398,23 @@ __device__ __forceinline__ void EvalDescriptor(cudaTextureObject_t tex, float cx
   e->gy2 = 180.f * (t2dy - cdy);
 }
 
+// A pair that ProjectIntoImage put into the image (*r): LoadPixel, with `desc` the descriptor residual, then Associate's stage.
+// Fills *l, and with `desc` *e and *photo.  The in-image test stays with the caller: folded in as stage 0, it cost a spill.
+// Every gather is in flight before the first test: depth / normal / cfactor and -- speculatively, ~99 % of in-image pairs end
+// up associated -- the six texture fetches.  The tests then wait for the slowest load once.
+__device__ __forceinline__ int EvalPair(const CameraParams& cam, const KfRegs& K, const Vec3& gp, const Vec3& n, float radius_sq,
+                                        float d1, float d2, bool desc, Assoc* r, PixelLoads* l, DescEval* e, bool* photo) {
+  *l = LoadPixel(cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, *r);
+  if (desc) {
+    float ccx, ccy;
+    *photo = DepthToColor(cam, r->pxf, r->pyf, &ccx, &ccy);
+    float t1x, t1y, t2x, t2y;
+    TangentProjections(cam, K.T, gp, n, radius_sq, &t1x, &t1y, &t2x, &t2y);
+    EvalDescriptor(K.tex, ccx, ccy, t1x, t1y, t2x, t2y, d1, d2, e);
+  }
+  return Associate(cam, K.T, n, *l, r);
+}
+
 // kernel_opt_pose.cu:96-142: Jacobian of a descriptor residual wrt the pose (global_T_frame * exp(hat(delta))).
 __device__ __forceinline__ void DescPoseJacobian(const CameraParams& cam, const Vec3& ls, float gx, float gy, float (&J)[6]) {
   gx *= cam.cfx;
@@ -384,6 +433,27 @@ __device__ __forceinline__ void DescPoseJacobian(const CameraParams& cam, const 
 __device__ __forceinline__ void ColorIntrinsicsJacobians(const Assoc& r, const DescEval& e, float (&J1)[4], float (&J2)[4]) {
   J1[0] = e.gx1 * r.nx; J1[1] = e.gy1 * r.ny; J1[2] = e.gx1; J1[3] = e.gy1;
   J2[0] = e.gx2 * r.nx; J2[1] = e.gy2 * r.ny; J2[2] = e.gx2; J2[3] = e.gy2;
+}
+
+// kernel_opt_intrinsics.cu:84-121 / kernel_pcg.cu:266-300,728-760: Jacobian of the depth residual wrt the depth camera's
+// (fx^-1, fy^-1, cx^-1, cy^-1, a) in J[0..4] and wrt the pixel's cfactor in J[5].  Returns the corrected inverse depth, whose
+// magnitude each caller tests against 1e-4 the way its reference kernel does.
+__device__ __forceinline__ float DepthIntrinsicsJacobian(const CameraParams& cam, const Assoc& r, const PixelLoads& l, float (&J)[6]) {
+  float inv_stddev;
+  Vec3 up;
+  DepthResidual(cam, r, &inv_stddev, &up);   // for inv_stddev only
+  const float raw_inv_depth = 1.0f / (cam.raw_to_float * l.measured);
+  const float exp_inv_depth = expf(-cam.a * raw_inv_depth);
+  const float corrected_inv_depth = l.cf * exp_inv_depth + raw_inv_depth;
+  const float dot = r.nx * r.ln.x + r.ny * r.ln.y + r.ln.z;
+  const float jac_base = inv_stddev * dot * exp_inv_depth / (corrected_inv_depth * corrected_inv_depth);
+  J[2] = inv_stddev * r.d * r.ln.x;   // n_global . row0(frame_T_global) = rotated normal x
+  J[3] = inv_stddev * r.d * r.ln.y;
+  J[0] = r.px * J[2];
+  J[1] = r.py * J[3];
+  J[4] = l.cf * raw_inv_depth * jac_base;
+  J[5] = -jac_base;
+  return corrected_inv_depth;
 }
 
 }  // namespace bba

@@ -54,27 +54,14 @@ __global__ void __launch_bounds__(kThreads) ObservationStatsKernel(const __grid_
         const Vec3 gp = V3(x, a.surfels[kRowY * P + i], a.surfels[kRowZ * P + i]);
         const Vec3 nrm = UnpackNormal(__float_as_uint(a.surfels[kRowNormal * P + i]));
         for (int kf = j_begin; kf < j_end; ++kf) {
-          const KfDevice& K = a.kfs[kf];
-          float T[12];
-#pragma unroll
-          for (int c = 0; c < 12; ++c) T[c] = __ldg(&K.T[c]);
+          KfRegs K;
+          LoadKfGlobal(a.kfs, kf, &K);
           Assoc r;
-          if (!ProjectIntoImage(cam, T, gp, &r)) continue;
+          if (!ProjectIntoImage(cam, K.T, gp, &r)) continue;
           const PixelLoads l = LoadPixel(cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r);
-          // IsAssociatedWithPixel<return_free_space_violations = true> (surfel_projection_nvcc_only.cuh:48-127)
-          if (l.measured & kInvalidDepthBit) continue;
-          const float d = RawToCalibratedDepth(cam.a, l.cf, cam.raw_to_float, l.measured);
-          const Vec3 ln = Rotate(T, nrm);
-          const float nx = cam.fx_inv * r.px + cam.cx_inv, ny = cam.fy_inv * r.py + cam.cy_inv;
-          const float thr = kDepthTukey * ((kDepthUncertaintyFactor * fabsf(ln.x * nx + ln.y * ny + ln.z) * (d * d)) / cam.baseline_fx);
-          const float diff = d - r.lp.z;
-          if (diff > thr) {
-            viol += 1.f;
-            continue;
-          }
-          if (diff < -thr) continue;
-          if (Dot(r.lp, ln) > 0) continue;
-          if (Dot(ln, U16ToImageSpaceNormal(l.kf_normal)) < kCosNormalCompat) continue;
+          const FreeSpaceTest t = AssociateFreeSpace(cam, K.T, nrm, l, &r);
+          if (t == kFreeSpaceViolation) viol += 1.f;
+          if (t != kFreeSpaceAssociated) continue;
           obs += 1.f;
           const KfRadius& R = a.radius[kf];
           const uint16_t h = __ldg(reinterpret_cast<const uint16_t*>(reinterpret_cast<const char*>(R.ptr) + static_cast<size_t>(r.py) * R.pitch) + r.px);
@@ -380,20 +367,11 @@ __global__ void __launch_bounds__(128) FilterSeedsKernel(const __grid_constant__
     Assoc r;
     if (!ProjectIntoImage(cam, ce.R, p_in, &r)) continue;
     // IsAssociatedWithPixel<true> for a pixel-defined surfel (surfel_projection_nvcc_only.cuh:130-236)
-    const uint16_t measured = LoadPixelU16(ce.depth, ce.depth_pitch, r.px, r.py);
-    if (measured & kInvalidDepthBit) continue;
-    const float pd = RawToCalibratedDepth(cam.a, __ldg(cam.cfactor + SparseCell(cam, r.px, r.py)), cam.raw_to_float, measured);
-    const Vec3 ln = Rotate(ce.R, n_in);
-    const float nx = cam.fx_inv * r.px + cam.cx_inv, ny = cam.fy_inv * r.py + cam.cy_inv;
-    const float thr = kDepthTukey * ((kDepthUncertaintyFactor * fabsf(ln.x * nx + ln.y * ny + ln.z) * (pd * pd)) / cam.baseline_fx);
-    const float diff = pd - r.lp.z;
-    if (diff > thr) {
-      ++viol;
-      continue;
-    }
-    if (diff < -thr) continue;
-    if (Dot(r.lp, ln) > 0) continue;
-    if (Dot(ln, U16ToImageSpaceNormal(LoadPixelU16(ce.normals, ce.normals_pitch, r.px, r.py))) < kCosNormalCompat) continue;
+    const PixelLoads l{LoadPixelU16(ce.depth, ce.depth_pitch, r.px, r.py), LoadPixelU16(ce.normals, ce.normals_pitch, r.px, r.py),
+                       __ldg(cam.cfactor + SparseCell(cam, r.px, r.py))};
+    const FreeSpaceTest t = AssociateFreeSpace(cam, ce.R, n_in, l, &r);
+    if (t == kFreeSpaceViolation) ++viol;
+    if (t != kFreeSpaceAssociated) continue;
     ++obs;
   }
   if (obs < static_cast<unsigned int>(a.min_observation_count) || viol > obs) a.flags[static_cast<size_t>(sy) * cam.w + sx] = 0u;

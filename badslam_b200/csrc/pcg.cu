@@ -123,17 +123,7 @@ __global__ void __launch_bounds__(kThreads) PcgAccumulateKernel(const __grid_con
       PixelLoads l;
       DescEval e;
       bool photo = false;
-      if (valid && ProjectIntoImage(cam, K.T, gp, &r)) {
-        l = LoadPixel(cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r);
-        if (use_desc) {
-          float ccx, ccy;
-          photo = DepthToColor(cam, r.pxf, r.pyf, &ccx, &ccy);
-          float t1x, t1y, t2x, t2y;
-          TangentProjections(cam, K.T, gp, nrm, radius_sq, &t1x, &t1y, &t2x, &t2y);
-          EvalDescriptor(K.tex, ccx, ccy, t1x, t1y, t2x, t2y, d1, d2, &e);
-        }
-        st = Associate(cam, K.T, nrm, l, &r);
-      }
+      if (valid && ProjectIntoImage(cam, K.T, gp, &r)) st = EvalPair(cam, K, gp, nrm, radius_sq, d1, d2, use_desc, &r, &l, &e, &photo);
       bool visible = st == 3;
       if (__ballot_sync(0xffffffffu, visible) == 0) continue;
 
@@ -159,21 +149,10 @@ __global__ void __launch_bounds__(kThreads) PcgAccumulateKernel(const __grid_con
           float J[6];
           DepthPoseJacobian(r, inv_stddev, up, J);
           bool di_valid = false;
-          float Jd[5] = {0, 0, 0, 0, 0}, jcf = 0.f;
+          float Jd[6] = {0, 0, 0, 0, 0, 0};   // Jd[5]: wrt the pixel's cfactor
           uint32_t cf_u = 0;
           if (a.opt_depth_intr) {
-            const float raw_inv_depth = 1.0f / (cam.raw_to_float * l.measured);
-            const float exp_inv_depth = expf(-cam.a * raw_inv_depth);
-            const float corrected_inv_depth = l.cf * exp_inv_depth + raw_inv_depth;
-            di_valid = !(fabsf(corrected_inv_depth) < 1e-4f);
-            const float dot = r.nx * r.ln.x + r.ny * r.ln.y + r.ln.z;
-            const float jac_base = inv_stddev * dot * exp_inv_depth / (corrected_inv_depth * corrected_inv_depth);
-            Jd[2] = inv_stddev * r.d * r.ln.x;   // n_global . row0(frame_T_global) = rotated normal x
-            Jd[3] = inv_stddev * r.d * r.ln.y;
-            Jd[0] = r.px * Jd[2];
-            Jd[1] = r.py * Jd[3];
-            Jd[4] = l.cf * raw_inv_depth * jac_base;
-            jcf = -jac_base;
+            di_valid = !(fabsf(DepthIntrinsicsJacobian(cam, r, l, Jd)) < 1e-4f);
             cf_u = a.depth_intr_start + 5u + SparseCell(cam, r.px, r.py);
           }
           if constexpr (INIT) {
@@ -199,8 +178,8 @@ __global__ void __launch_bounds__(kThreads) PcgAccumulateKernel(const __grid_con
                   is[c] -= Jd[c] * wr;
                   is[5 + c] += Jd[c] * w * Jd[c];
                 }
-                atomicAdd(a.r + cf_u, -jcf * wr);
-                atomicAdd(a.M + cf_u, jcf * w * jcf);
+                atomicAdd(a.r + cf_u, -Jd[5] * wr);
+                atomicAdd(a.M + cf_u, Jd[5] * w * Jd[5]);
               }
             }
           } else {
@@ -213,7 +192,7 @@ __global__ void __launch_bounds__(kThreads) PcgAccumulateKernel(const __grid_con
             if (a.opt_depth_intr && di_valid) {
 #pragma unroll
               for (int c = 0; c < 5; ++c) sum += Jd[c] * pdi[c];
-              sum += jcf * __ldg(a.p + cf_u);
+              sum += Jd[5] * __ldg(a.p + cf_u);
             }
             is[9] += sum * w * sum;
             sum *= w;
@@ -225,7 +204,7 @@ __global__ void __launch_bounds__(kThreads) PcgAccumulateKernel(const __grid_con
             if (a.opt_depth_intr && di_valid) {
 #pragma unroll
               for (int c = 0; c < 5; ++c) is[c] += Jd[c] * sum;
-              atomicAdd(a.g + cf_u, jcf * sum);
+              atomicAdd(a.g + cf_u, Jd[5] * sum);
             }
           }
         }
@@ -235,6 +214,7 @@ __global__ void __launch_bounds__(kThreads) PcgAccumulateKernel(const __grid_con
           const float w1 = DescWeight(e.r1), w2 = DescWeight(e.r2);
           float jg1 = 0.f, jg2 = 0.f;
           if (a.opt_geometry) {
+            // PositionDescriptorKernel's copy applies cfx / cfy inside term1 / term2 instead; the two orders round differently
             const float term1 = -(r.ln.x * r.lp.z - r.ln.z * r.lp.x);
             const float term2 = -(r.ln.y * r.lp.z - r.ln.z * r.lp.y);
             const float term3 = 1.f / (r.lp.z * r.lp.z);

@@ -137,15 +137,6 @@ __device__ __forceinline__ void StoreReplicas(T* local, T* const (&peers)[kMaxPe
     if (p < peer_count) peers[p][o] = v;
 }
 
-struct KfRegs {
-  float T[12];
-  const uint16_t* depth;
-  const uint16_t* normals;
-  cudaTextureObject_t tex;
-  uint32_t depth_pitch, normals_pitch;
-  int activation;
-};
-
 // A keyframe record from shared memory (staged by the TMA engine together with the surfel tile).  Returns the keyframe id (pad).
 __device__ __forceinline__ int LoadKfShared(const KfDevice* rec, KfRegs* r) {
   const float4* p = reinterpret_cast<const float4*>(rec);
