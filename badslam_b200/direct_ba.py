@@ -940,7 +940,7 @@ class DirectBA:
         kw_host_owned = host_owned
         cfg = scene.cfg
         cam_d = PinholeCamera4f(cfg.width, cfg.height, scene.depth_K)
-        cam_c = PinholeCamera4f(cfg.width, cfg.height, scene.color_K)
+        cam_c = PinholeCamera4f(scene.color.shape[2], scene.color.shape[1], scene.color_K)
         device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         ba = cls(max_surfel_count=scene.pitch, raw_to_float_depth=cfg.raw_to_float_depth, baseline_fx=cfg.baseline_fx,
                  sparse_surfel_cell_size=cfg.cell, color_camera_initial_estimate=cam_c,

@@ -123,7 +123,8 @@ class Oracle:
         self.surfels = np.ascontiguousarray(scene.surfels, np.float32).copy()
         self.active = np.zeros(max(self.surfels.shape[1], 1), np.uint8)   # capacity (surfel creation grows n)
         m = Model()
-        m.depth_w, m.depth_h, m.color_w, m.color_h = cfg.width, cfg.height, cfg.width, cfg.height
+        m.depth_w, m.depth_h = cfg.width, cfg.height
+        m.color_h, m.color_w = scene.color.shape[1:3]
         m.depth_K[:] = [float(v) for v in scene.depth_K]
         m.color_K[:] = [float(v) for v in scene.color_K]
         m.raw_to_float_depth = cfg.raw_to_float_depth

@@ -136,7 +136,8 @@ class RefDirectBA:
         self.l = lib()
         cfg = scene.cfg
         c = Config()
-        c.depth_w, c.depth_h, c.color_w, c.color_h = cfg.width, cfg.height, cfg.width, cfg.height
+        c.depth_w, c.depth_h = cfg.width, cfg.height
+        c.color_h, c.color_w = scene.color.shape[1:3]
         c.depth_K[:] = [float(v) for v in scene.depth_K]
         c.color_K[:] = [float(v) for v in scene.color_K]
         c.raw_to_float_depth, c.baseline_fx, c.cell = cfg.raw_to_float_depth, cfg.baseline_fx, cfg.cell

@@ -111,8 +111,19 @@ def test_batch_of_one_is_the_single_frame_call(mods, name):
 
 @pytest.mark.parametrize("name", ["tiny", "small", "many"])
 def test_entries_agree_with_single_calls(mods, name):
+    check_entries_agree_with_single_calls(mods, scene(mods[0], name))
+
+
+def check_entries_agree_with_single_calls(mods, sc, reference=None):
+    """37 entries (the keyframes' buffers and rendered frames) in calls of 1 .. 37 entries against the single-frame calls, the
+    keyframe form, the oracle and the coefficients at the estimate.  With `reference` (a RefDirectBA of the scene), the keyframe
+    entries of the 37-entry call are also held to the reference's EstimateFramePose from the same start, and the reference's own
+    run-to-run spread there (a second run) widens the 1e-6 bar to the keyframe form, which sums in another order from 4 entries
+    on.  The oracle then has to match only where it took the reference's number of Gauss-Newton iterations: the convergence
+    test (|x|^2 < 1e-6 in scaled units, direct_ba_alternating.cc) lets a last step of up to ~1e-3 decide, and the oracle's IEEE
+    arithmetic puts that step on the other side of the threshold now and then."""
     S, DirectBA, L, O = mods
-    sc = scene(S, name)
+    name = sc.cfg.name
     K = sc.cfg.num_keyframes
     ba = DirectBA.from_scene(sc, max_keyframes=K + 37)
     frames, truth, kf_of_frame = frames_of(S, sc)
@@ -128,10 +139,20 @@ def test_entries_agree_with_single_calls(mods, name):
             assert bool(convs[i]) == want[i][2], tag
             k = kf_of_frame[frame_of_entry[i]]
             if k >= 0:
-                kf_pose, _, _ = ba.EstimateFramePose(None, init[i], k)
-                assert_pose_close(S, poses[i], kf_pose, 1e-6, ("keyframe form",) + tag)
+                kf_pose, kf_its, _ = ba.EstimateFramePose(None, init[i], k)
+                spread = 0.0
+                if reference is not None and count == 37:
+                    rp, rits, _ = reference.estimate_frame_pose(k, init[i])
+                    spread = max(S.pose_error(rp, reference.estimate_frame_pose(k, init[i])[0]))
+                    assert int(its[i]) == kf_its == rits, ("iterations",) + tag + (int(its[i]), kf_its, rits)
+                    assert_pose_close(S, poses[i], rp, POSE_TOL + 2 * spread, ("reference",) + tag)
+                assert_pose_close(S, poses[i], kf_pose, 1e-6 + 2 * spread, ("keyframe form",) + tag)
                 if count == 37:
-                    assert_pose_close(S, poses[i], orc.estimate_frame_pose(k, init[i])[0], POSE_TOL, ("oracle",) + tag)
+                    po, oits, _ = orc.estimate_frame_pose(k, init[i])
+                    if reference is None or oits == rits:
+                        assert_pose_close(S, poses[i], po, POSE_TOL, ("oracle",) + tag)
+                    else:
+                        print(f"{tag}: the oracle stopped after {oits} iterations, the reference and this path after {rits}")
                 # at_estimate: what bba_accumulate_pose_coeffs returns at the returned pose
                 pc = ba.AccumulatePoseEstimationCoeffs(k, poses[i])
                 got = coeffs[i]

@@ -121,9 +121,13 @@ def test_create_surfels_for_keyframe_three_way(mods, name, filt):
         else:
             runs = [c1] + [r.create_surfels_for_keyframe(k, filt) for r in more]
             mean = float(np.mean(runs))
-            print(name, filt, "keyframe", k, "created: ours", c0, "| reference runs", runs, f"relative offset {(c0 - mean) / mean:+.3f}")
-            assert max(runs) - min(runs) <= max(20, 0.06 * mean), (k, runs)          # the reference's own scatter (measured: <= 3 % range over five runs)
-            assert abs(c0 - mean) <= max(40, 0.16 * mean), (k, c0, runs)            # (different seed pixels: different coverage / filter outcome)
+            if max(runs) == 0:
+                # a keyframe the kept half of the map already covers: no cell to seed, whichever pixel the race would pick
+                assert c0 == 0, (k, c0, runs)
+            else:
+                print(name, filt, "keyframe", k, "created: ours", c0, "| reference runs", runs, f"relative offset {(c0 - mean) / mean:+.3f}")
+                assert max(runs) - min(runs) <= max(20, 0.06 * mean), (k, runs)          # the reference's own scatter (measured: <= 3 % range over five runs)
+                assert abs(c0 - mean) <= max(40, 0.16 * mean), (k, c0, runs)            # (different seed pixels: different coverage / filter outcome)
         assert ba.surfels_size() == orc.n
     n1 = ba.surfels_size()
     assert n1 > n0

@@ -10,7 +10,8 @@ import os
 import numpy as np
 import pytest
 
-from gpu_checks import POSE_R, POSE_T, REL, check_intrinsics_step, check_pcg_building_blocks, distorted_scene, rel
+from gpu_checks import (POSE_R, POSE_T, REL, check_intrinsics_step, check_pcg_building_blocks, check_pcg_inner_steps,
+                        distorted_scene, rel)
 
 pytestmark = pytest.mark.gpu
 
@@ -331,21 +332,7 @@ def test_pcg_bundle_adjustment_against_reference(mods, small_scene):
     sc = small_scene
     K = sc.cfg.num_keyframes
     # (1) 4 inner steps per outer iteration
-    ba, ref, ref2 = DirectBA.from_scene(sc), R.RefDirectBA(sc), R.RefDirectBA(sc)
-    ro = ba.BundleAdjustment(None, False, False, False, True, True, 2, 2, use_pcg=True, pcg_max_inner_iterations=4, pcg_gauge_keyframe=2)
-    rr = ref.bundle_adjust_pcg(min_iterations=2, max_iterations=2, max_inner_iterations=4, gauge_keyframe=2)
-    ref2.bundle_adjust_pcg(min_iterations=2, max_iterations=2, max_inner_iterations=4, gauge_keyframe=2)
-    assert ro.iterations_done == rr.iterations_done == 2 and ro.pcg_inner_iterations_total == rr.inner_iterations_total == 8
-    assert abs(ro.pcg_last_r_norm - rr.last_r_norm) < 1e-3 * rr.last_r_norm
-    noise = max(max(S.pose_error(ref.pose(k), ref2.pose(k))) for k in range(K))
-    pa = ba.GetKeyframeStates()[0]
-    assert np.array_equal(pa[2], sc.poses_init[2])     # the gauge keyframe does not move
-    for k in range(K):
-        dt, dr = S.pose_error(pa[k], ref.pose(k))
-        assert dt < 1e-5 + 3 * noise and dr < 1e-5 + 3 * noise, (k, dt, dr, noise)
-    a, b_ = ba.GetSurfelsHost(), ref.surfels()
-    assert np.abs(a[:3] - b_[:3]).max() < 1e-4 and np.abs(a[:3] - b_[:3]).mean() < 1e-6      # 8 fp32 CG steps
-    assert (a[3].view(np.uint32) != b_[3].view(np.uint32)).mean() < 1e-4   # second normals update sees 1e-6-different positions
+    check_pcg_inner_steps(S, R, DirectBA, sc)
     # (2) full solves: same quality as the reference
     ba, ref = DirectBA.from_scene(sc), R.RefDirectBA(sc)
     ro = ba.BundleAdjustment(None, False, False, False, True, True, 3, 3, use_pcg=True, pcg_gauge_keyframe=0)
