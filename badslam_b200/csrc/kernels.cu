@@ -579,7 +579,9 @@ static void LaunchPoseAccumulateS(const PoseAccumulateArgs& args, int sm_count, 
 
 LaunchResult LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
                                   int variant) {
-  if (args.n == 0) return {};
+  // (max_work = 0: a rank of a multi-GPU job whose share of the pose step's work list is empty -- no launch at all, a grid of
+  // zero blocks is an invalid configuration)
+  if (args.n == 0 || max_work <= 0) return {};
   PackWorkRecordsKernel<<<(max_work * 6 + 127) / 128, 128, 0, stream>>>(args.kfs, args.work_list, args.work_count, args.work_records);
   if (with_stats) LaunchPoseAccumulateS<true>(args, sm_count, variant, stream);
   else LaunchPoseAccumulateS<false>(args, sm_count, variant, stream);
