@@ -170,6 +170,7 @@ SYMBOLS = {
     "bba_cfactor_size": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "bba_accumulate_pose_coeffs": (C.c_int, [_P, C.c_int, _F7, C.POINTER(PoseCoeffs), _P]),
     "bba_debug_pose_coeffs_batch": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
+    "bba_debug_set_pose_group": (C.c_int, [_P, C.c_int]),
     "bba_estimate_frame_pose": (C.c_int, [_P, C.c_int, _F7, _F7, C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_estimate_frame_pose_for_frame": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _F7, _F7,
                                                     C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),

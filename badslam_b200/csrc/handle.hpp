@@ -235,6 +235,7 @@ struct bba_context {
     } order;
     uint32_t order_n = 0;
     bool order_stale = true;
+    int group = 0;   // keyframes per work item of the pose kernel (bba_debug_set_pose_group); 0: the launcher's choice
   } pose;
 
   // geometry step and intrinsics step (bundle_adjust.cu)

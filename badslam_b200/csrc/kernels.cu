@@ -90,7 +90,6 @@ constexpr int kPoseUnroll = 1;       // surfels of a chunk evaluated concurrentl
 constexpr int kPoseStagedRows = 7;   // x y z normal radius^2 d1 d2
 constexpr int kPoseStagedRowsPre = 14;   // x y z d1 d2 + the 9 frame rows (normal, tangent point 1, tangent point 2)
 static_assert(kPoseStagedRowsPre == kPoseStreamRows, "the PRE instantiations stage every row of the pose stream");
-constexpr int kPoseGroup = 8;        // keyframes per work item
 
 // Does the axis-aligned box {min x y z, -, max x y z, -} lie surely outside the view of the keyframe with frame_T_global T, i.e.
 // would ProjectIntoImage reject every position in it?  The box is culled when its 8 corners all lie beyond one plane: z = 0 or one
@@ -206,11 +205,12 @@ __device__ __forceinline__ void StorePoseTotal(const PoseAccumulateArgs& args, i
   else atomicAdd(args.acc + static_cast<size_t>(kf) * kPoseAccSize + lane, static_cast<double>(total));
 }
 
-// Work decomposition.  A work ITEM is (group of <= 8 keyframes from the work list) x (tile of TILE surfels); items are
+// Work decomposition.  A work ITEM is (group of <= args.group keyframes from the work list) x (tile of TILE surfels); items are
 // handed out through a global counter in GROUP-MAJOR order, so at any moment all resident CTAs read the images of the
-// same 8-16 keyframes (~12-24 MB: stays in the H100's 50 MB L2) while surfel tiles stream through shared memory via TMA.
-// Inside an item the 8 warps steal SUB-ITEMS (keyframe, 256- or 128-surfel chunk) from a shared-memory counter, which
-// evens out the very different cost of culled vs. associated chunks.
+// same one or two groups of keyframes while surfel tiles stream through shared memory via TMA (once per group: the larger the
+// group, the fewer passes over the surfels).  Inside an item the warps steal SUB-ITEMS (keyframe, 256- or 128-surfel chunk) from
+// a shared-memory counter, which evens out the very different cost of culled vs. associated chunks.  The group decides only
+// which sub-items share a staged tile, never what a sub-item computes.
 // STATS: also produce the residual costs and the stage counters of the byte model (the reference computes its
 // residual count / cost only in debug mode, kernel_opt_pose.cu:312-320,373-381).
 // PRE: the surfels are read from the pose stream in spatial order (LaunchPoseStream: positions, descriptors and the per-surfel
@@ -230,7 +230,8 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* stage_base = reinterpret_cast<float*>(smem_raw);   // [2][kRows][TILE]
   float* rings = stage_base + 2 * kRows * TILE;             // PRE: [producer][slot][kPoseBatchFloats]
-  __shared__ __align__(16) KfDevice s_kf[2][kPoseGroup];   // the work group's keyframe records, staged with the tile
+  // [2][G] the work group's keyframe records, staged with the tile
+  KfDevice* s_kf = reinterpret_cast<KfDevice*>(rings + (PRE ? kPoseRingBytes / sizeof(float) : 0));
   __shared__ __align__(16) float s_box[2][PRE ? TILE / kSpatialChunk : 1][8];   // PRE: the tile's chunk boxes, staged with it
   __shared__ __align__(8) uint64_t full_bar[2];
   __shared__ unsigned int s_item[2];
@@ -248,7 +249,8 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
   const int lane = tid & 31;
   const int warp = tid >> 5;
   const uint32_t n_tiles = (args.n + TILE - 1) / TILE;
-  const uint32_t n_groups = (n_work + kPoseGroup - 1) / kPoseGroup;
+  const int G = args.group;
+  const uint32_t n_groups = (n_work + G - 1) / G;
   const uint32_t n_items = n_groups * n_tiles;
   // 256-surfel chunks (one warp-level reduction per 8 steps); 128-surfel ones when the work list holds fewer than 4 keyframes,
   // so that every warp of the CTA still finds a sub-item (the tail of a Gauss-Newton loop)
@@ -262,11 +264,11 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
     const uint32_t base = tile * TILE;
     const uint32_t cnt = min(static_cast<uint32_t>(TILE), args.n - base);
     const uint32_t bytes = ((cnt * 4u + 15u) / 16u) * 16u;
-    const uint32_t kf_bytes = static_cast<uint32_t>(sizeof(KfDevice)) * min(kPoseGroup, n_work - static_cast<int>(group) * kPoseGroup);
+    const uint32_t kf_bytes = static_cast<uint32_t>(sizeof(KfDevice)) * min(G, n_work - static_cast<int>(group) * G);
     // PRE: the boxes of the tile's chunks come with it (32 bytes each)
     const uint32_t box_bytes = PRE ? (cnt + kSpatialChunk - 1) / kSpatialChunk * 8 * sizeof(float) : 0u;
     MbarArriveExpectTx(&full_bar[s], bytes * kRows + kf_bytes + box_bytes);
-    BulkCopyG2S(&s_kf[s][0], args.work_records + static_cast<size_t>(group) * kPoseGroup, kf_bytes, &full_bar[s]);
+    BulkCopyG2S(s_kf + s * G, args.work_records + static_cast<size_t>(group) * G, kf_bytes, &full_bar[s]);
     if (PRE) {
       BulkCopyG2S(&s_box[s][0][0], args.boxes + static_cast<size_t>(base / kSpatialChunk) * 8, box_bytes, &full_bar[s]);
 #pragma unroll
@@ -383,7 +385,7 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
     const uint32_t tile = item - group * n_tiles;
     const uint32_t base = tile * TILE;
     const uint32_t cnt = min(static_cast<uint32_t>(TILE), args.n - base);
-    const int kfs_in_group = min(kPoseGroup, n_work - static_cast<int>(group) * kPoseGroup);
+    const int kfs_in_group = min(G, n_work - static_cast<int>(group) * G);
     // One chunk size per launch: sizing per item from its group's keyframe count cost more in the extra warp reductions of the
     // smaller chunks than the idle warps of the few short groups save (on the project's first GPU, not on the H100).
     const int wanted_shift = n_work >= 4 ? kPoseChunkShift : 7;
@@ -402,7 +404,7 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
       if (j0 >= cnt) continue;
       const uint32_t j1 = min(cnt, j0 + chunk_len);
       KfRegs K;
-      const int kf = LoadKfShared(&s_kf[s][kf_local], &K);
+      const int kf = LoadKfShared(s_kf + s * G + kf_local, &K);
       if (PRE && BoxOutsideView(cam, K.T, s_box[s][PRE ? j0 / kSpatialChunk : 0], lane)) continue;   // no pair in the image
       K.tex = UniformTexture(K.tex);
 
@@ -528,13 +530,15 @@ __global__ void __launch_bounds__(128) PackWorkRecordsKernel(const KfDevice* __r
   }
 }
 
-static constexpr size_t PoseSmemBytes(int tile, bool pre) {
-  return static_cast<size_t>(2) * (pre ? kPoseStagedRowsPre : kPoseStagedRows) * tile * sizeof(float) + (pre ? kPoseRingBytes : 0);
+// Dynamic shared memory of the pose kernel: two stages of surfel rows, (PRE) the producers' rings, and the two stages' group records.
+static constexpr size_t PoseSmemBytes(int tile, bool pre, int group) {
+  return static_cast<size_t>(2) * (pre ? kPoseStagedRowsPre : kPoseStagedRows) * tile * sizeof(float) + (pre ? kPoseRingBytes : 0) +
+         static_cast<size_t>(2) * group * sizeof(KfDevice);
 }
 
 template <int TILE, bool PRE>
 static cudaError_t SetPoseSmemLimit() {
-  const int smem = static_cast<int>(PoseSmemBytes(TILE, PRE));
+  const int smem = static_cast<int>(PoseSmemBytes(TILE, PRE, kPoseMaxGroup));
   for (const void* k : {reinterpret_cast<const void*>(PoseAccumulateKernel<TILE, false, PRE, false>),
                         reinterpret_cast<const void*>(PoseAccumulateKernel<TILE, true, PRE, false>),
                         reinterpret_cast<const void*>(PoseAccumulateKernel<TILE, false, PRE, true>),
@@ -552,7 +556,7 @@ cudaError_t SetPoseAccumulateSmemLimits() {
 
 template <int TILE, bool STATS, bool PRE>
 static void LaunchPoseAccumulateT(const PoseAccumulateArgs& args, int sm_count, cudaStream_t stream) {
-  constexpr size_t smem = PoseSmemBytes(TILE, PRE);
+  const size_t smem = PoseSmemBytes(TILE, PRE, args.group);
   const dim3 grid(kPoseMinCtas * sm_count), block(PRE ? kPoseWsThreads : kPoseThreads);   // persistent
   if (args.exact) PoseAccumulateKernel<TILE, STATS, PRE, true><<<grid, block, smem, stream>>>(args);
   else PoseAccumulateKernel<TILE, STATS, PRE, false><<<grid, block, smem, stream>>>(args);
@@ -583,8 +587,15 @@ LaunchResult LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, 
   // zero blocks is an invalid configuration)
   if (args.n == 0 || max_work <= 0) return {};
   PackWorkRecordsKernel<<<(max_work * 6 + 127) / 128, 128, 0, stream>>>(args.kfs, args.work_list, args.work_count, args.work_records);
-  if (with_stats) LaunchPoseAccumulateS<true>(args, sm_count, variant, stream);
-  else LaunchPoseAccumulateS<false>(args, sm_count, variant, stream);
+  // Keyframes per work item.  Every item stages its tile's stream rows once for the whole group, so that one pass over the
+  // keyframes reads the stream n_work / group times.  In spatial order the tiles that the resident CTAs work on at one time are a
+  // compact region, a patch of each keyframe's image, so a group of 32 keyframes still gathers from a small part of L2: on cfg3 one
+  // 200-keyframe launch without stats took 6.90 ms at 32, 6.84 at 24, 7.14 at 16 and 7.48 at 8 (DESIGN §7.1).  In the caller's
+  // order a tile is a band across a whole image and larger groups did not pay (cfg2).
+  PoseAccumulateArgs a = args;
+  if (a.group == 0) a.group = a.stream && a.stream_sorted ? 32 : 8;
+  if (with_stats) LaunchPoseAccumulateS<true>(a, sm_count, variant, stream);
+  else LaunchPoseAccumulateS<false>(a, sm_count, variant, stream);
   return {2};
 }
 

@@ -28,13 +28,17 @@ struct PoseAccumulateArgs {
   const float* stream;       // kPoseStreamRows rows x stream_pitch, in spatial order (LaunchPoseStream); may be null
   uint32_t stream_pitch;     // floats per row
   const float* boxes;        // [n / kSpatialChunk rounded up][8] bounding box of every stream chunk (LaunchPoseStream)
+  bool stream_sorted;        // the stream is in spatial order (perm), not in the caller's
   KfDevice* work_records;   // [max_kf] scratch: the work list's KfDevice records in list order (pad = keyframe id), filled by
-                             // LaunchPoseAccumulate so that a work group's <= 8 records are ONE contiguous bulk copy
+                             // LaunchPoseAccumulate so that a work group's <= group records are ONE contiguous bulk copy
+  int group;                 // keyframes per work item, 1 .. kPoseMaxGroup; 0: LaunchPoseAccumulate picks it
   double* acc;               // [max_kf][32]
   ExactSum* exact;           // deterministic mode: [max_kf][32] exact sums that take the warp totals instead of acc; else null
   unsigned long long* stage_counts;  // [max_kf][2]
   unsigned int* queue;       // global work-item counter, must be 0 at launch
 };
+
+constexpr int kPoseMaxGroup = 64;
 
 // Persistent, TMA-staged pose residual/Jacobian/Hessian kernel (AccumulatePoseEstimationCoeffsCUDAKernel,
 // kernel_opt_pose.cu:251-383, for a whole list of keyframes in one launch).
@@ -73,7 +77,8 @@ inline bool PoseVariantPre(int v) { return v == kPoseVariant256Pre || v == kPose
 // variant = kPoseVariantAuto: the tile follows from args.n and the SM count, and args.stream != null selects the variant that
 // stages the sorted stream (and skips the chunks whose box lies outside a keyframe's view) instead of the caller's rows.  Any other
 // variant forces that instantiation; a PRE variant needs args.stream and args.boxes, the others ignore them.  args.exact != null
-// selects the deterministic instantiation of the same variant.
+// selects the deterministic instantiation of the same variant.  args.group = 0: 32 keyframes per work item on a stream in spatial
+// order, 8 otherwise.
 LaunchResult LaunchPoseAccumulate(const PoseAccumulateArgs& args, int sm_count, bool with_stats, int max_work, cudaStream_t stream,
                                   int variant = kPoseVariantAuto);
 // Sets the dynamic shared-memory limit of every instantiation of the pose kernel on the current device (once per handle).

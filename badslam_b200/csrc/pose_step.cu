@@ -61,28 +61,32 @@ bba_status PreparePoseAccumulate(bba_handle h, int n_work, int variant, cudaStre
   acc->exact = h->deterministic ? p.d_exact.get() : nullptr;
   acc->stage_counts = p.d_stage_counts;
   acc->queue = p.d_queue;
+  acc->group = p.group;
   acc->stream = nullptr;
   acc->stream_pitch = 0;
   acc->boxes = nullptr;
+  acc->stream_sorted = false;
   const bool pre = variant == kPoseVariantAuto ? h->cfg.use_descriptor_residuals && n_work >= 4 : PoseVariantPre(variant);
+  // The rebuild (bounds, keys, radix sort) has a fixed cost of ~0.1 ms, most of it launch overhead at the start of a pose step
+  // whose stream has just drained: measured on cfg2 (20 keyframes x 200 k surfels) it cost more than the culling it buys, on
+  // cfg3_rank8 (200 x 375 k) it paid for itself many times over.  Below kSpatialOrderMinPairs (surfel, keyframe) pairs per
+  // launch the stream keeps the caller's order; its chunk boxes are culled all the same.  A forced variant always sorts.  (In a
+  // BA iteration the geometry step has usually made the order current already.)
+  const bool sort = variant != kPoseVariantAuto ||
+                    static_cast<uint64_t>(h->surfels_size) * static_cast<uint64_t>(n_work) >= kSpatialOrderMinPairs;
   if (pre && h->surfels_size > 0 && stream_current) {
     acc->stream = p.order.stream;
     acc->stream_pitch = p.order.capacity;
     acc->boxes = p.order.boxes;
+    acc->stream_sorted = sort;
   } else if (pre && h->surfels_size > 0) {
-    // The rebuild (bounds, keys, radix sort) has a fixed cost of ~0.1 ms, most of it launch overhead at the start of a pose step
-    // whose stream has just drained: measured on cfg2 (20 keyframes x 200 k surfels) it cost more than the culling it buys, on
-    // cfg3_rank8 (200 x 375 k) it paid for itself many times over.  Below kSpatialOrderMinPairs (surfel, keyframe) pairs per
-    // launch the stream keeps the caller's order; its chunk boxes are culled all the same.  A forced variant always sorts.  (In a
-    // BA iteration the geometry step has usually made the order current already.)
-    const bool sort = variant != kPoseVariantAuto ||
-                      static_cast<uint64_t>(h->surfels_size) * static_cast<uint64_t>(n_work) >= kSpatialOrderMinPairs;
     if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/false, s)) return st;
     BBA_LAUNCH(h, h->launches, LaunchPoseStream, h->surfels, acc->pitch, h->surfels_size, sort ? p.order.view.perm : nullptr, p.order.stream,
                p.order.capacity, p.order.boxes, s);
     acc->stream = p.order.stream;
     acc->stream_pitch = p.order.capacity;
     acc->boxes = p.order.boxes;
+    acc->stream_sorted = sort;
   }
   return BBA_OK;
 }
@@ -419,6 +423,14 @@ bba_status bba_debug_pose_coeffs_batch(bba_handle h, int count, const int* ids, 
     c[3] = static_cast<uint64_t>(r[28] + 0.5);
     if (with_stats) std::memcpy(costs + 3 * static_cast<size_t>(k), r + 29, sizeof(double) * 3);
   }
+  return BBA_OK;
+}
+
+bba_status bba_debug_set_pose_group(bba_handle h, int keyframes) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (keyframes < 0 || keyframes > kPoseMaxGroup)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_set_pose_group: keyframes out of range (0 .. " + std::to_string(kPoseMaxGroup) + ")");
+  h->pose.group = keyframes;
   return BBA_OK;
 }
 

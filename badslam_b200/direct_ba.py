@@ -571,6 +571,10 @@ class DirectBA:
                                                           costs.ctypes.data, self._stream_ptr(stream)))
         return H, b, counts, costs
 
+    def DebugSetPoseGroup(self, keyframes: int):
+        """bba_debug_set_pose_group: keyframes per staged surfel tile in every later pose-kernel launch (0: the library's choice)."""
+        self._check(self._lib.bba_debug_set_pose_group(self._h, int(keyframes)))
+
     def EstimateFramePose(self, stream, global_T_frame_initial_estimate, keyframe_id: int):
         """direct_ba.h:122-129; returns (global_T_frame_estimate, iterations, converged)."""
         p = np.ascontiguousarray(global_T_frame_initial_estimate, np.float32)

@@ -246,6 +246,10 @@ typedef enum {
 } bba_pose_variant;
 bba_status bba_debug_pose_coeffs_batch(bba_handle h, int count, const int* keyframe_ids, const float* global_T_frame, int variant,
                                        int with_stats, double* H, double* b, uint64_t* counts, double* costs, void* stream);
+/* Forces the number of keyframes that share one staged surfel tile in every later launch of the pose kernel (1 .. 64; 0, the
+ * default: the library's choice).  The results do not depend on it beyond the order of the default mode's floating-point
+ * sums; in the deterministic mode they are the same bits.  For tests and timing. */
+bba_status bba_debug_set_pose_group(bba_handle h, int keyframes);
 /* DirectBA::EstimateFramePose (direct_ba.h:122-129, direct_ba_alternating.cc:42-283) against a stored keyframe's
  * images.  iterations/converged may be NULL. */
 bba_status bba_estimate_frame_pose(bba_handle h, int keyframe_id, const float global_T_frame_initial[7],
