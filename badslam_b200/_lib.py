@@ -210,6 +210,11 @@ SYMBOLS = {
     "bba_peer_unmap": (C.c_int, [_P]),
     "bba_mark_replica_rewritten": (C.c_int, [_P]),
     "bba_set_collective": (C.c_int, [_P, COLLECTIVE_FN, _P]),
+    "bba_local_group_create": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int, C.POINTER(_P)]),
+    "bba_local_group_reset": (C.c_int, [_P]),
+    "bba_local_group_poison": (C.c_int, [_P]),
+    "bba_local_group_destroy": (None, [_P]),
+    "bba_debug_collective": (C.c_int, [_P, C.c_int, _P, C.c_size_t, _P]),
     "bba_shard_surfel_owner": (C.c_int, [C.c_uint32, C.c_int]),
     "bba_shard_surfel_local_index": (C.c_uint32, [C.c_uint32, C.c_int]),
     "bba_shard_slice_length": (C.c_uint32, [C.c_uint32, C.c_int]),

@@ -32,9 +32,10 @@ UNITS = [
     ("pose_step.cu", []),
     ("bundle_adjust.cu", []),
     ("multi_gpu.cu", []),
+    ("local_group.cu", ["-Xptxas", "-v"]),   # (the all-reduce sums keep denormals: no -use_fast_math)
     ("frames.cu", []),
 ]
-HEADERS = ["device_math.cuh", "exact_sum.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", os.path.join("..", "..", "include", "badba.h")]
+HEADERS = ["device_math.cuh", "exact_sum.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", "rendezvous.hpp", os.path.join("..", "..", "include", "badba.h")]
 
 
 def _newer(src, dst):

@@ -19,8 +19,11 @@ void SetError(bba_handle h, const std::string& msg) {
   h->errors[std::this_thread::get_id()] = msg;
 }
 
+thread_local int FrontEndScope::depth_ = 0;
+
 bba_status Fail(bba_handle h, bba_status s, const std::string& msg) {
   if (h) SetError(h, msg);
+  if (h && h->xchg.group && !FrontEndScope::active()) PoisonLocalGroup(h->xchg.group);
   return s;
 }
 
@@ -719,6 +722,7 @@ bba_status bba_set_keyframe_pose(bba_handle h, int id, const float p[7]) {
   return Publish(h, nullptr, false);
 }
 bba_status bba_get_keyframe_pose(bba_handle h, int id, float p[7]) {
+  FrontEndScope front_end;
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   std::unique_lock<std::mutex> lock(h->fe.mu);
   if (id < 0 || id >= static_cast<int>(h->fe.kfs.size())) {
@@ -735,6 +739,7 @@ bba_status bba_set_keyframe_activation(bba_handle h, int id, int activation) {
   return Publish(h, nullptr, false);
 }
 bba_status bba_get_keyframe_activation(bba_handle h, int id, int* activation) {
+  FrontEndScope front_end;
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   std::unique_lock<std::mutex> lock(h->fe.mu);
   if (id < 0 || id >= static_cast<int>(h->fe.kfs.size())) {
@@ -819,6 +824,7 @@ bba_status bba_set_cfactor_host(bba_handle h, const float* host, void* stream) {
   return BBA_OK;
 }
 bba_status bba_get_cfactor_host(bba_handle h, float* host, void* stream) {
+  FrontEndScope front_end;
   if (!h || !host) return BBA_ERR_INVALID_ARGUMENT;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   FrontEndCall view(h);

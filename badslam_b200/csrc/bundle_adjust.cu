@@ -126,7 +126,7 @@ bba_status AccumulateIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cu
   if (h->cfg.world_size > 1) {
     // every rank accumulated its surfel shard: one sum all-reduce over [34 global sums | B | D | b2 | obs]
     BBA_LAUNCH(h, h->launches, LaunchIntrinsicsConvertSums, h->geo.d_intr_sums, h->geo.d_intr, true, s);
-    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->geo.d_intr, 64 + static_cast<size_t>(8) * P, s);
+    if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->geo.d_intr, 64 + static_cast<size_t>(8) * P, s)) return st;
     BBA_LAUNCH(h, h->launches, LaunchIntrinsicsConvertSums, h->geo.d_intr_sums, h->geo.d_intr, false, s);
   }
   *eq = IntrinsicsEquations{P, cell_B, cell_D, cell_b2, cell_obs, d_x1, a.cam};
@@ -386,7 +386,7 @@ bba_status PerformEndTasks(bba_handle h, cudaStream_t s, uint32_t* deleted_out, 
     h->xchg.h_count_xchg[0] = static_cast<float>(*h->life.h_count & 0xfffu);
     h->xchg.h_count_xchg[1] = static_cast<float>(*h->life.h_count >> 12);
     BBA_CUDA(h, cudaMemcpyAsync(h->xchg.d_count_xchg, h->xchg.h_count_xchg, sizeof(float) * 2, cudaMemcpyHostToDevice, s));
-    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->xchg.d_count_xchg, 2, s);
+    if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->xchg.d_count_xchg, 2, s)) return st;
     BBA_CUDA(h, cudaMemcpyAsync(h->xchg.h_count_xchg, h->xchg.d_count_xchg, sizeof(float) * 2, cudaMemcpyDeviceToHost, s));
     BBA_CUDA(h, cudaStreamSynchronize(s));
     deleted_total = static_cast<uint32_t>(h->xchg.h_count_xchg[0] + 0.5f) + (static_cast<uint32_t>(h->xchg.h_count_xchg[1] + 0.5f) << 12);
@@ -515,8 +515,8 @@ bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int 
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars, 0, sizeof(double) * 4, s));
   BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
   if (h->cfg.world_size > 1) {
-    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[0], U, s);
-    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[1], U, s);
+    if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[0], U, s)) return st;
+    if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[1], U, s)) return st;
     h->xchg.replicated_pass_pending = false;
   }
   BBA_LAUNCH(h, h->launches, LaunchPcgInit2, U, L.a_index, h->depth_a, a.kf_count, h->pcg.d_vec[0], h->pcg.d_vec[1], h->pcg.d_vec[2],
@@ -530,7 +530,7 @@ bba_status PcgStep1(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, cud
   if (h->cfg.world_size > 1) {   // g and this rank's part of alpha_d: one all-reduce
     float* g = h->pcg.d_vec[3];
     BBA_LAUNCH(h, h->launches, LaunchPcgPackAlphaD, h->pcg.d_scalars, g + L.unknown_count, s);
-    h->xchg.collective(h->xchg.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, g, static_cast<size_t>(L.unknown_count) + 2, s);
+    if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, g, static_cast<size_t>(L.unknown_count) + 2, s)) return st;
     BBA_LAUNCH(h, h->launches, LaunchPcgUnpackAlphaD, h->pcg.d_scalars, g + L.unknown_count, s);
   }
   return BBA_OK;

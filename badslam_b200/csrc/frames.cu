@@ -459,6 +459,7 @@ bba_status bba_track_frame_pairwise(bba_handle h, const bba_odometry_options* o,
                                     const uint16_t* device_depth, size_t depth_pitch, const uint16_t* device_normals, size_t normals_pitch,
                                     const uint8_t* device_color_rgba, size_t color_pitch, const float init1[7], const float init2[7],
                                     float out[7], bba_odometry_result* result, void* stream) {
+  FrontEndScope front_end;
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   // (-1 would mean a frame base in an entry)
   if (base_keyframe_id < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_track_frame_pairwise: no such keyframe");
@@ -474,6 +475,7 @@ bba_status bba_track_frame_pairwise_to_frame(bba_handle h, const bba_odometry_op
                                              size_t normals_pitch, const uint8_t* device_color_rgba, size_t color_pitch,
                                              const float init1[7], const float init2[7], float out[7], bba_odometry_result* result,
                                              void* stream) {
+  FrontEndScope front_end;
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   const bba_frame_buffers frames[2] = {{base_depth, base_depth_pitch, base_normals, base_normals_pitch, base_color_rgba, base_color_pitch},
                                        {device_depth, depth_pitch, device_normals, normals_pitch, device_color_rgba, color_pitch}};
@@ -483,6 +485,7 @@ bba_status bba_track_frame_pairwise_to_frame(bba_handle h, const bba_odometry_op
 bba_status bba_track_frames_pairwise(bba_handle h, const bba_odometry_options* o, int frame_count, const bba_frame_buffers* frames,
                                      int count, const bba_odometry_entry* entries, float* base_T_frame_estimate,
                                      bba_odometry_result* results, uint32_t* kernel_launches, void* stream) {
+  FrontEndScope front_end;
   const char* fn = "bba_track_frames_pairwise";
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   if (bba_status st = CheckOdometryCall(h, fn, o, frame_count, frames, count, entries, base_T_frame_estimate)) return st;
@@ -492,6 +495,7 @@ bba_status bba_track_frames_pairwise(bba_handle h, const bba_odometry_options* o
 
 bba_status bba_odometry_get_level(bba_handle h, int which, int scale, float* host_depth, uint16_t* host_normals, uint8_t* host_color,
                                   int* width, int* height, void* stream) {
+  FrontEndScope front_end;
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> call(h->fe.call);
   auto& st = h->odo;
@@ -511,6 +515,7 @@ bba_status bba_odometry_get_level(bba_handle h, int which, int scale, float* hos
 
 bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, const float pose_a[7], const float pose_b[7], float H[21],
                                      float b[6], uint32_t* residual_count, float* residual_sum, uint32_t counts[2], float costs[2], void* stream) {
+  FrontEndScope front_end;
   if (!h || !pose_a) return BBA_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> call(h->fe.call);
   auto& st = h->odo;
@@ -543,6 +548,7 @@ bba_status bba_preprocess_frame(bba_handle h, const bba_preprocess_options* o,
                                 uint16_t* device_radius, size_t radius_pitch,
                                 uint8_t* device_color_rgba, size_t color_pitch,
                                 float* min_depth, float* max_depth, void* stream) {
+  FrontEndScope front_end;
   return PreprocessFrame(h, "bba_preprocess_frame", o, device_raw_depth, raw_depth_pitch, device_rgb, rgb_pitch, device_depth,
                          depth_pitch, device_normals, normals_pitch, device_radius, radius_pitch, device_color_rgba, color_pitch,
                          min_depth, max_depth, stream, nullptr);
@@ -557,6 +563,7 @@ bba_status bba_preprocess_raw_frame(bba_handle h, const bba_raw_frame_options* o
                                     uint16_t* device_radius, size_t radius_pitch,
                                     uint8_t* device_color_rgba, size_t color_pitch,
                                     float* min_depth, float* max_depth, void* stream) {
+  FrontEndScope front_end;
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   if (!o) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_preprocess_raw_frame: null argument");
   const int n = o->median_filter_and_densify_iterations, ld = o->pyramid_level_for_depth, lc = o->pyramid_level_for_color;

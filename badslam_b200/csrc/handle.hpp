@@ -282,6 +282,10 @@ struct bba_context {
   struct Exchange {
     bba_collective_fn collective = nullptr;
     void* collective_user = nullptr;
+    // The local group this handle is a member of (local_group.cu), and the reason its last exchange failed: a local group's
+    // collective returns nothing, so it leaves the reason here for Collective.
+    bba_local_group group = nullptr;
+    std::string exchange_error;
     bba::DeviceBuffer<float> d_exchange;    // [world][rows][shard_len] floats, rows <= kShardRows (ExchangeShards)
     bba::DeviceBuffer<float> d_pose_pack;   // [max_kf][kPoseSlot] floats
     bba::PinnedBuffer<float> h_pose_pack;
@@ -377,9 +381,28 @@ struct bba_context {
 
 namespace bba {
 
+// Sets the calling thread's bba_last_error message and returns s.  A failure of a BA-side call on a member of a local group
+// poisons the group, so that the other ranks' exchanges return instead of waiting for this rank (FrontEndScope).
 bba_status Fail(bba_handle h, bba_status s, const std::string& msg);
 // Sets the calling thread's bba_last_error message.
 void SetError(bba_handle h, const std::string& msg);
+
+// Marks the calling thread as inside a front-end call (badba.h "Conventions") while it lives: its failures concern that call
+// only and leave the handle's local group in service.
+class FrontEndScope {
+ public:
+  FrontEndScope() { ++depth_; }
+  ~FrontEndScope() { --depth_; }
+  FrontEndScope(const FrontEndScope&) = delete;
+  FrontEndScope& operator=(const FrontEndScope&) = delete;
+  static bool active() { return depth_ > 0; }
+
+ private:
+  static thread_local int depth_;
+};
+
+// local_group.cu
+void PoisonLocalGroup(bba_local_group g);
 
 #define BBA_CUDA(h, expr)                                                                                  \
   do {                                                                                                      \
@@ -481,6 +504,9 @@ void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t
 uint32_t LocalCountBelow(uint32_t global_end, int rank, int world);
 void AssignKeyframes(bba_handle h, const std::vector<int>& ids, std::vector<int>* owner);
 bba_status CheckCollective(bba_handle h);
+// Runs the registered exchange (bba_set_collective or a local group) on `buffer`; fails with BBA_ERR_STATE when a local
+// group's exchange did not complete (its group is poisoned).
+bba_status Collective(bba_handle h, int op, void* buffer, size_t count, cudaStream_t s);
 bba_status PeerFence(bba_handle h, cudaStream_t s);
 bba_status ExchangeShards(bba_handle h, const ShardRows& rows, const uint32_t* perm, cudaStream_t s);
 bba_status ExchangeGeometry(bba_handle h, cudaStream_t s);

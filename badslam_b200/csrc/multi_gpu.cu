@@ -38,25 +38,34 @@ bba_status Barrier(bba_handle h, cudaStream_t s) {
   auto& x = h->xchg;
   BBA_CUDA(h, x.d_barrier.Reserve(1));
   BBA_CUDA(h, cudaMemsetAsync(x.d_barrier, 0, sizeof(float), s));
-  x.collective(x.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, x.d_barrier, 1, s);
-  return BBA_OK;
+  return Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, x.d_barrier, 1, s);
 }
 
 bba_status AllocationBase(bba_handle h, const void* ptr, void** base) {
   typedef int (*GetRangeFn)(unsigned long long*, size_t*, unsigned long long);
-  static GetRangeFn fn = nullptr;
-  if (!fn) {
+  // (looked up once per process; the initialisation of a local static is thread-safe, so handles of several threads may race here)
+  static const GetRangeFn fn = [] {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
-    BBA_CUDA(h, cudaGetDriverEntryPoint("cuMemGetAddressRange", &p, cudaEnableDefault, &q));
-    if (!p) return Fail(h, BBA_ERR_CUDA, "cuMemGetAddressRange is not available");
-    fn = reinterpret_cast<GetRangeFn>(p);
-  }
+    if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &p, cudaEnableDefault, &q) != cudaSuccess) {
+      cudaGetLastError();
+      p = nullptr;
+    }
+    return reinterpret_cast<GetRangeFn>(p);
+  }();
+  if (!fn) return Fail(h, BBA_ERR_CUDA, "cuMemGetAddressRange is not available");
   unsigned long long b = 0;
   size_t size = 0;
   if (fn(&b, &size, reinterpret_cast<unsigned long long>(ptr)) != 0) return Fail(h, BBA_ERR_CUDA, "cuMemGetAddressRange failed");
   *base = reinterpret_cast<void*>(b);
   return BBA_OK;
+}
+
+// A member of a local group exchanges through its group: the calls that would replace that are refused, and leave the group
+// in service (nothing changed).
+bba_status RefuseMember(bba_handle h, const char* fn) {
+  SetError(h, std::string(fn) + ": the handle is a member of a local group (bba_local_group_destroy first)");
+  return BBA_ERR_STATE;
 }
 
 }  // namespace
@@ -95,6 +104,14 @@ bba_status CheckCollective(bba_handle h) {
   return BBA_OK;
 }
 
+bba_status Collective(bba_handle h, int op, void* buffer, size_t count, cudaStream_t s) {
+  auto& x = h->xchg;
+  x.exchange_error.clear();
+  x.collective(x.collective_user, op, buffer, count, s);
+  if (!x.exchange_error.empty()) return Fail(h, BBA_ERR_STATE, x.exchange_error);
+  return BBA_OK;
+}
+
 // Every rank has updated `rows` of its own surfel shard only (granules of stream positions, surfel perm[s] at position s; perm
 // null: the caller's order): each rank packs them into its slice of the exchange buffer, one all-gather, and every rank unpacks
 // the other ranks' slices.  The buffer grows to room for kShardRows rows of max_surfel_count surfels (or more).
@@ -109,7 +126,7 @@ bba_status ExchangeShards(bba_handle h, const ShardRows& rows, const uint32_t* p
   const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
   BBA_LAUNCH(h, h->launches, LaunchPackShard, h->surfels, pitch, h->active, h->surfels_size, rows, perm, rank, world, shard_len,
              x.d_exchange + slice_floats * rank, s);
-  x.collective(x.collective_user, BBA_COLLECTIVE_ALLGATHER, x.d_exchange, slice_floats * sizeof(float), s);
+  if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLGATHER, x.d_exchange, slice_floats * sizeof(float), s)) return st;
   BBA_LAUNCH(h, h->launches, LaunchUnpackShards, h->surfels, pitch, h->active, h->surfels_size, rows, perm, shard_len, world, rank,
              x.d_exchange, s);
   return BBA_OK;
@@ -171,6 +188,7 @@ bba_status bba_peer_import(bba_handle h, const bba_peer_handle* all, int count) 
   if (!h || !all) return BBA_ERR_INVALID_ARGUMENT;
   if (count != h->cfg.world_size) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_peer_import: need one handle per rank");
   if (count - 1 > kMaxPeers) return Fail(h, BBA_ERR_UNSUPPORTED, "bba_peer_import: more than 8 ranks");
+  if (h->xchg.group) return RefuseMember(h, "bba_peer_import");
   if (bba_status st = CheckSurfels(h)) return st;
   UnmapPeers(h);
   auto& x = h->xchg;
@@ -225,6 +243,7 @@ bba_status bba_peer_unmap(bba_handle h) {
 
 bba_status bba_set_collective(bba_handle h, bba_collective_fn fn, void* user) {
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (h->xchg.group) return RefuseMember(h, "bba_set_collective");
   h->xchg.collective = fn;
   h->xchg.collective_user = user;
   return BBA_OK;

@@ -324,7 +324,7 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
     BBA_CUDA(h, cudaMemsetAsync(x.d_pose_pack, 0, sizeof(float) * kPoseSlot * K, s));
     BBA_LAUNCH(h, h->launches, LaunchPackPoseResults, x.d_local_ids, n_local, p.d_pose_est, p.d_iterations, p.d_converged, p.d_first_stats,
                x.d_pose_pack, s);
-    x.collective(x.collective_user, BBA_COLLECTIVE_ALLREDUCE_SUM, x.d_pose_pack, static_cast<size_t>(kPoseSlot) * K, s);
+    if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, x.d_pose_pack, static_cast<size_t>(kPoseSlot) * K, s)) return st;
     x.replicated_pass_pending = false;   // (every rank's earlier work on this stream precedes its contribution)
     BBA_CUDA(h, cudaMemcpyAsync(x.h_pose_pack, x.d_pose_pack, sizeof(float) * kPoseSlot * K, cudaMemcpyDeviceToHost, s));
   } else {

@@ -896,6 +896,22 @@ class DirectBA:
         self._collective_cb = lib_defs.COLLECTIVE_FN(cb)   # keep alive
         self._check(self._lib.bba_set_collective(self._h, self._collective_cb, None))
 
+    def DebugCollective(self, op: int, buffer: torch.Tensor, count: int, stream=None):
+        """bba_debug_collective: runs the registered exchange (a LocalGroup's or SetCollective's) once on `buffer`, as the BA
+        code does (op _lib.COLLECTIVE_ALLREDUCE_SUM: `count` fp32 values; _lib.COLLECTIVE_ALLGATHER: world slices of `count`
+        bytes).  Every rank makes the same call."""
+        self._check(self._lib.bba_debug_collective(self._h, int(op), C.c_void_p(buffer.data_ptr()), int(count),
+                                                   self._stream_ptr(stream)))
+
+    @classmethod
+    def create_local_ranks(cls, scene, world: int, devices=None, **kw) -> List["DirectBA"]:
+        """The `world` ranks of a multi-GPU job on `scene` as handles of this process (rank r on devices[r], default cuda:0),
+        ready for LocalGroup.  Keyword arguments go to from_scene."""
+        devices = devices or ["cuda:0"] * world
+        if len(devices) != world:
+            raise ValueError("one device per rank")
+        return [cls.from_scene(scene, device=devices[r], rank=r, world_size=world, **kw) for r in range(world)]
+
     def kernel_launch_count(self) -> int:
         return int(self._lib.bba_kernel_launch_count(self._h))
 
@@ -973,3 +989,84 @@ class DirectBA:
         if np.any(scene.cfactor != 0):
             ba.SetCFactorBuffer(scene.cfactor)
         return ba
+
+
+class LocalGroup:
+    """The ranks of a multi-GPU job as DirectBA handles of this process (bba_local_group_create): the library exchanges between
+    them itself, through device memory and CUDA events, without a host collective.  handles[r] must have been created with
+    rank r and world_size len(handles) (DirectBA.create_local_ranks); peer_stores maps every surfel replica into every rank.
+
+        with LocalGroup(DirectBA.create_local_ranks(scene, 2)) as group:
+            results = group.run(lambda rank, ba: ba.BundleAdjustment(None, False, False, False, True, True, 3, 3))
+
+    run() is the way to drive the members: every BA-side call of a member belongs on its own thread, and all members make the
+    same calls.  Close the group (or leave the with-block) before closing its members."""
+
+    def __init__(self, handles, peer_stores: bool = False):
+        self._lib = _lib.load()
+        self.handles = list(handles)
+        self._g = C.c_void_p()
+        arr = (C.c_void_p * len(self.handles))(*[ba._h.value for ba in self.handles])
+        st = self._lib.bba_local_group_create(arr, len(self.handles), int(peer_stores), C.byref(self._g))
+        if st != _lib.OK:
+            msg = self._lib.bba_last_error(self.handles[0]._h).decode() if self.handles else ""
+            for ba in self.handles:   # (the message is on the handle the check refused)
+                m = self._lib.bba_last_error(ba._h).decode()
+                if m.startswith("bba_local_group_create"):
+                    msg = m
+            raise BadBAError(st, msg)
+        # one stream per rank: two ranks on one device then queue their work side by side
+        self._streams = [torch.cuda.Stream(device=ba.device) for ba in self.handles]
+
+    def run(self, fn):
+        """Calls fn(rank, ba) on one thread per rank, inside torch.cuda.device(ba.device) and on a stream of the rank's own,
+        joins the threads and returns the list of their results.  Re-raises the first error.  Any error on a rank's thread
+        poisons the group, also one that fn raises outside the library, so that the other ranks' exchanges return instead of
+        waiting for that rank; reset() restores service."""
+        import threading
+        n = len(self.handles)
+        results, errors = [None] * n, []
+        lock = threading.Lock()
+
+        def body(rank):
+            ba = self.handles[rank]
+            try:
+                with torch.cuda.device(ba.device), torch.cuda.stream(self._streams[rank]):
+                    results[rank] = fn(rank, ba)
+                    self._streams[rank].synchronize()
+            except BaseException as e:  # noqa: B036 -- handed to the calling thread
+                self._lib.bba_local_group_poison(self._g)
+                with lock:
+                    errors.append(e)
+
+        threads = [threading.Thread(target=body, args=(r,), name=f"bba-rank-{r}") for r in range(n)]
+        for t in threads:
+            t.start()
+        for t in threads:
+            t.join()
+        if errors:
+            raise errors[0]
+        return results
+
+    def reset(self):
+        """bba_local_group_reset: clears the poisoned state after a failed run."""
+        st = self._lib.bba_local_group_reset(self._g)
+        if st != _lib.OK:
+            raise BadBAError(st, "bba_local_group_reset")
+
+    def close(self):
+        if getattr(self, "_g", None) is not None and self._g.value:
+            self._lib.bba_local_group_destroy(self._g)
+            self._g = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

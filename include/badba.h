@@ -36,6 +36,9 @@
  *    one thread a front-end call therefore sees exactly the handle's current state.  The front end
  *    does not get a view in the middle of a BA iteration, nor any share of the SMs: its kernels
  *    queue behind the BA kernels that occupy them (INTEGRATION.md section 2);
+ *  - several handles may be driven concurrently from different threads of one process (one BA side
+ *    each); the members of a local group (bba_local_group_create) are such handles, with the
+ *    threading contract given there;
  *  - errors are status codes + bba_last_error(), per calling thread; nothing aborts (the reference
  *    LOG(FATAL)s, libvis/src/libvis/cuda/cuda_util.h:35-49) and nothing falls back to a CPU path.
  */
@@ -418,6 +421,34 @@ int  bba_shard_keyframe_owner(int list_index, int world_size);
 /* The assignment rule itself (host-only, no device needed): cost[i] > 0 = measured work of work-list entry i, 0 = unknown
  * (mean of the known ones); all unknown or world_size 1 -> round-robin. */
 void bba_balance_keyframes(const float* cost, int count, int world_size, int* owner);
+
+/* ---- local groups: the ranks of a multi-GPU job as handles of ONE process (DESIGN.md "Local groups") ----
+ * Each member is driven by its own host thread; the library exchanges between them itself, through device memory and CUDA
+ * events (no callback, NCCL, MPI or IPC), across the GPUs of one node or with several ranks on one GPU.  The all-reduce sums
+ * the ranks' buffers in rank order 0..N-1 on every rank, so the replicas stay equal bit for bit.
+ * Threading contract:
+ *  - each member's BA-side calls run on its own thread, with that thread's current device set to the member's device;
+ *  - all members make the same sequence of BA-side calls (as the ranks of a multi-process job do);
+ *  - front-end calls stay per handle, as above.
+ * A BA-side call on a member that returns an error poisons the group: every exchange of every member waiting in it, and every
+ * later one, fails at once with BBA_ERR_STATE, so no rank waits for one that returned early.  bba_local_group_reset clears the
+ * poison, once every member's thread has returned. */
+typedef struct bba_local_group_s* bba_local_group;
+/* ranks[i] is the handle of rank i (created with world_size == count, rank == i), all in this process, <= 9 ranks.  Devices must be
+ * equal or peer-capable (else BBA_ERR_UNSUPPORTED).  peer_stores: map every replica into every rank (needs equal surfels_size and
+ * pitch): the geometry kernels then store into every replica and the geometry exchange is a barrier, as after bba_peer_import;
+ * replacing a member's surfel buffer or flags (bba_set_surfels*, bba_set_active_flags) then needs a new group.  Replaces each
+ * member's collective; arguments are checked before anything changes.  bba_set_collective and bba_peer_import on a member
+ * return BBA_ERR_STATE.  Enables peer access between the members' distinct devices (left enabled by destroy). */
+bba_status bba_local_group_create(const bba_handle* ranks, int count, int peer_stores, bba_local_group* out);
+bba_status bba_local_group_reset(bba_local_group g);   /* clears the poisoned state */
+/* Poisons the group from outside the library: for a member's thread that gives up between calls (an exception of the caller's
+ * own code), so that the other members' exchanges return instead of waiting for it. */
+bba_status bba_local_group_poison(bba_local_group g);
+void       bba_local_group_destroy(bba_local_group g); /* before bba_destroy of any member; restores "no collective" */
+/* Parity hook: runs the handle's registered exchange (group or bba_set_collective) once on a caller device buffer, on every rank
+ * (op: bba_collective_op; count as for bba_collective_fn).  Stream-ordered, does not synchronise. */
+bba_status bba_debug_collective(bba_handle h, int op, void* device_buffer, size_t count, void* stream);
 
 /* Re-uploads the images of an existing keyframe from host memory (same sizes as at creation) -- the per-step
  * host->device input path of a live system, where a keyframe's RGB-D data arrives from the sensor thread

@@ -19,9 +19,12 @@
 #include <cstdint>
 #include <cstddef>
 #include <cstring>
+#include <exception>
 #include <fstream>
 #include <functional>
+#include <memory>
 #include <mutex>
+#include <thread>
 #include <vector>
 #include <stdexcept>
 #include <string>
@@ -406,6 +409,64 @@ class DirectBA {
   int pcg_gauge_keyframe_ = -1;
   int min_observation_counts_[3] = {1, 2, 3};
   mutable std::mutex mutex_;
+};
+
+// The ranks of a multi-GPU bundle adjustment as DirectBA members of one process (bba_local_group_create): the library exchanges
+// between them itself, so a BA thread can drive several GPUs without NCCL, MPI or IPC.  members[r] must have been constructed
+// with rank r, world_size members.size() and device devices[r].  The group is destroyed before its members.
+//
+//   group.RunOnRanks([&](int rank, DA& ba) { ba.BundleAdjustment(streams[rank], ...); });
+//
+// RunOnRanks runs fn on one thread per rank with that thread's current device set to the rank's device, joins them and rethrows
+// the first exception; any exception poisons the group first, so that no other rank waits for one that gave up.  Reset()
+// restores service afterwards.
+template <typename DA>
+class LocalGroup {
+ public:
+  LocalGroup(std::vector<std::unique_ptr<DA>> members, std::vector<int> devices, bool peer_stores = false)
+      : members_(std::move(members)), devices_(std::move(devices)) {
+    if (devices_.size() != members_.size()) throw Error(BBA_ERR_INVALID_ARGUMENT, "LocalGroup: one device per member");
+    std::vector<bba_handle> handles;
+    for (const auto& m : members_) handles.push_back(m->handle());
+    const bba_status s = bba_local_group_create(handles.data(), static_cast<int>(handles.size()), peer_stores ? 1 : 0, &g_);
+    if (s != BBA_OK) {
+      std::string msg = "bba_local_group_create";
+      for (bba_handle h : handles)
+        if (h && std::strncmp(bba_last_error(h), "bba_local_group_create", 22) == 0) msg = bba_last_error(h);
+      throw Error(s, msg);
+    }
+  }
+  ~LocalGroup() { bba_local_group_destroy(g_); }   // (members_ go after the group)
+  LocalGroup(const LocalGroup&) = delete;
+  LocalGroup& operator=(const LocalGroup&) = delete;
+
+  void RunOnRanks(const std::function<void(int, DA&)>& fn) {
+    std::vector<std::exception_ptr> errors(members_.size());
+    std::vector<std::thread> threads;
+    for (size_t r = 0; r < members_.size(); ++r)
+      threads.emplace_back([&, r] {
+        try {
+          if (cudaSetDevice(devices_[r]) != cudaSuccess) throw Error(BBA_ERR_CUDA, "LocalGroup: cudaSetDevice");
+          fn(static_cast<int>(r), *members_[r]);
+        } catch (...) {
+          errors[r] = std::current_exception();
+          bba_local_group_poison(g_);
+        }
+      });
+    for (auto& t : threads) t.join();
+    for (auto& e : errors)
+      if (e) std::rethrow_exception(e);
+  }
+  void Reset() {
+    if (bba_local_group_reset(g_) != BBA_OK) throw Error(BBA_ERR_INVALID_ARGUMENT, "bba_local_group_reset");
+  }
+  int size() const { return static_cast<int>(members_.size()); }
+  DA& member(int rank) { return *members_.at(rank); }
+
+ private:
+  std::vector<std::unique_ptr<DA>> members_;
+  std::vector<int> devices_;
+  bba_local_group g_ = nullptr;
 };
 
 // SaveCalibration / LoadCalibration (io.h:60-72, io.cc:570-700), same three text files: <base>.depth_intrinsics.txt and
