@@ -34,10 +34,11 @@ __device__ __forceinline__ void FenceBarrierInit() { asm volatile("fence.mbarrie
 __device__ __forceinline__ void MbarArriveExpectTx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(SmemAddr(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void MbarArrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(SmemAddr(bar)) : "memory");
+// (MbarArrive / MbarWait / MbarTest take the barrier's shared-memory address, SmemAddr, so that a loop can keep it in a register.)
+__device__ __forceinline__ void MbarArrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void MbarWait(uint64_t* bar, uint32_t parity) {
+__device__ __forceinline__ void MbarWait(uint32_t bar, uint32_t parity) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
@@ -46,12 +47,12 @@ __device__ __forceinline__ void MbarWait(uint64_t* bar, uint32_t parity) {
       "@p bra.uni WAIT_DONE;\n"
       "bra.uni WAIT_LOOP;\n"
       "WAIT_DONE:\n"
-      "}\n" ::"r"(SmemAddr(bar)),
+      "}\n" ::"r"(bar),
       "r"(parity)
       : "memory");
 }
 // Non-blocking form of MbarWait: has the phase of the given parity completed?
-__device__ __forceinline__ bool MbarTest(uint64_t* bar, uint32_t parity) {
+__device__ __forceinline__ bool MbarTest(uint32_t bar, uint32_t parity) {
   uint32_t done;
   asm volatile(
       "{\n"
@@ -60,7 +61,7 @@ __device__ __forceinline__ bool MbarTest(uint64_t* bar, uint32_t parity) {
       "selp.u32 %0, 1, 0, p;\n"
       "}\n"
       : "=r"(done)
-      : "r"(SmemAddr(bar)), "r"(parity)
+      : "r"(bar), "r"(parity)
       : "memory");
   return done != 0;
 }
@@ -149,13 +150,14 @@ constexpr int kPoseProducerRegs = 72;
 constexpr int kPoseConsumerRegs = 96;
 static_assert(kPoseProducerWarps * kPoseProducerRegs + kPoseConsumerWarps * kPoseConsumerRegs ==
                   (kPoseProducerWarps + kPoseConsumerWarps) * 80, "register split");
-// One record per associated pair, as 32-pair batches in shared memory, field-major (field f of pair i at [f][i]):
-// lp (3) ln (3) d nx ny r1 r2 gx1 gy1 gx2 gy2 photo.  Each producer owns a ring of two batch slots with a full / empty mbarrier pair
-// per slot.
-constexpr int kPoseRecFields = 16;
+// A slot holds one 32-surfel step of a producer: lane L's record at position L, whether or not lane L associated.  A record is 15
+// floats in four float4 chunks -- {lp.x lp.y lp.z ln.x} {ln.y ln.z d nx} {ny r1 r2 gx1} {gy1 gx2 gy2 -} -- stored chunk-major
+// ([chunk][lane]) so that each of the four 16-byte stores and loads of a warp covers 512 contiguous bytes without a bank conflict.
+// Each producer owns a ring of two slots with a full / empty mbarrier pair per slot.
+constexpr int kPoseRecChunks = 4;
 constexpr int kPoseRingSlots = 2;
-constexpr int kPoseBatchFloats = kPoseRecFields * 32;
-constexpr size_t kPoseRingBytes = sizeof(float) * kPoseBatchFloats * kPoseRingSlots * kPoseProducerWarps;
+constexpr int kPoseSlotChunks = kPoseRecChunks * 32;
+constexpr size_t kPoseRingBytes = sizeof(float4) * kPoseSlotChunks * kPoseRingSlots * kPoseProducerWarps;
 
 template <int N>
 __device__ __forceinline__ void SetMaxRegsDec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
@@ -190,23 +192,24 @@ __device__ __forceinline__ void AccumulatePair(const CameraParams& cam, const As
   }
 }
 
-// The same from a pair's record (kPoseRecFields, one every 32 floats).
+// The same from a pair's record (the four chunks of a slot position, kPoseRecChunks).
 template <bool STATS>
-__device__ __forceinline__ void AccumulateRecord(const CameraParams& cam, const float* rec, float (&acc)[kPoseAccSize]) {
+__device__ __forceinline__ void AccumulateRecord(const CameraParams& cam, const float4 (&q)[kPoseRecChunks], bool photo,
+                                                 float (&acc)[kPoseAccSize]) {
   Assoc r;
-  r.lp = V3(rec[0 * 32], rec[1 * 32], rec[2 * 32]);
-  r.ln = V3(rec[3 * 32], rec[4 * 32], rec[5 * 32]);
-  r.d = rec[6 * 32];
-  r.nx = rec[7 * 32];
-  r.ny = rec[8 * 32];
+  r.lp = V3(q[0].x, q[0].y, q[0].z);
+  r.ln = V3(q[0].w, q[1].x, q[1].y);
+  r.d = q[1].z;
+  r.nx = q[1].w;
+  r.ny = q[2].x;
   DescEval e;
-  e.r1 = rec[9 * 32];
-  e.r2 = rec[10 * 32];
-  e.gx1 = rec[11 * 32];
-  e.gy1 = rec[12 * 32];
-  e.gx2 = rec[13 * 32];
-  e.gy2 = rec[14 * 32];
-  AccumulatePair<STATS>(cam, r, e, rec[15 * 32] != 0.f, acc);
+  e.r1 = q[2].y;
+  e.r2 = q[2].z;
+  e.gx1 = q[2].w;
+  e.gy1 = q[3].x;
+  e.gx2 = q[3].y;
+  e.gy2 = q[3].z;
+  AccumulatePair<STATS>(cam, r, e, photo, acc);
 }
 
 // Where a sub-item's warp total of slot `lane` goes: one fp64 atomic into acc, or (DET, the deterministic mode) a deposit into the
@@ -232,9 +235,10 @@ __device__ __forceinline__ void StorePoseTotal(const PoseAccumulateArgs& args, i
 // its keyframe's view (BoxOutsideView) is skipped without projecting a surfel, and the CTA is warp-specialised: the producer warps run the item loop below up to the association and hand each associated pair to
 // their consumer warp as a record.  Without PRE every warp accumulates its own pairs (26 of 32 lanes busy on average) and
 // holds the 32 sums in registers throughout.
-// A sub-item's records are packed densely in surfel order into 32-pair batches; lane L of the consumer sums pair L of every
-// batch of the sub-item, with fresh sums, and reduces once at its last batch.  The fp32 partials therefore depend on the
-// sub-item alone, never on timing, and are the same with and without STATS.
+// Every 32-surfel step with an associated lane fills one slot, lane L's record at position L (no packing: on the sorted stream
+// ~94 % of a visible chunk's lanes are in the image); lane L of the consumer sums the record of every slot of the sub-item whose
+// associated-lane mask has bit L, i.e. its surfels j = L (mod 32), with fresh sums, and reduces once at the sub-item's last slot.
+// The fp32 partials therefore depend on the sub-item alone, never on timing, and are the same with and without STATS.
 // DET: the warp totals go to exact sums (StorePoseTotal); with the partials fixed by the sub-item, the result is then the same bits
 // in every run.
 template <int TILE, bool STATS, bool PRE, bool DET>
@@ -243,18 +247,19 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
   constexpr int kRows = PRE ? kPoseStagedRowsPre : kPoseStagedRows;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* stage_base = reinterpret_cast<float*>(smem_raw);   // [2][kRows][TILE]
-  float* rings = stage_base + 2 * kRows * TILE;             // PRE: [producer][slot][kPoseBatchFloats]
+  float4* rings = reinterpret_cast<float4*>(stage_base + 2 * kRows * TILE);   // PRE: [producer][slot][kPoseSlotChunks]
   // [2][G] the work group's keyframe records, staged with the tile
-  KfDevice* s_kf = reinterpret_cast<KfDevice*>(rings + (PRE ? kPoseRingBytes / sizeof(float) : 0));
+  KfDevice* s_kf = reinterpret_cast<KfDevice*>(rings + (PRE ? kPoseRingBytes / sizeof(float4) : 0));
   __shared__ __align__(16) float s_box[2][PRE ? TILE / kSpatialChunk : 1][8];   // PRE: the tile's chunk boxes, staged with it
   __shared__ __align__(8) uint64_t full_bar[2];
   __shared__ unsigned int s_item[2];
   __shared__ int s_sub[2];
-  // PRE: batch handoff, per producer and slot: full / empty barriers (32 arrivals each: every lane releases its own accesses) and
-  // the batch header {pairs, last batch of its sub-item, keyframe id; keyframe id -1: the producer has finished}
+  // PRE: step handoff, per producer and slot: full / empty barriers (32 arrivals each: every lane releases its own accesses) and
+  // the slot header {associated-lane mask, photometric-lane mask, last step of its sub-item, keyframe id; keyframe id -1: the
+  // producer has finished}
   __shared__ __align__(8) uint64_t batch_full[PRE ? kPoseProducerWarps : 1][kPoseRingSlots];
   __shared__ __align__(8) uint64_t batch_empty[PRE ? kPoseProducerWarps : 1][kPoseRingSlots];
-  __shared__ int3 batch_hdr[PRE ? kPoseProducerWarps : 1][kPoseRingSlots];
+  __shared__ int4 batch_hdr[PRE ? kPoseProducerWarps : 1][kPoseRingSlots];
 
   const int n_work = __ldg(args.work_count);
   if (n_work <= 0) return;
@@ -310,7 +315,7 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
     const unsigned int item = atomicAdd(args.queue, 1u);
     s_item[s] = item;
     if (item < n_items) issue_tile(item, s);
-    else MbarArrive(&full_bar[s]);
+    else MbarArrive(SmemAddr(&full_bar[s]));
   };
   if (tid == 0) {
     MbarInit(&full_bar[0], 1);
@@ -328,10 +333,9 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
   }
   __syncthreads();
 
-  // Batch handoff.  Use number u of a producer's ring is slot u & 1 in phase (u >> 1) & 1; a slot starts out empty.
-  uint32_t batch_seq = 0;     // producer: the ring use that the pairs of the current batch go to
-  bool batch_owned = false;   // producer: slot batch_seq has been waited for (empty)
-  int batch_fill = 0;         // producer: pairs in slot batch_seq
+  // Step handoff.  Use number u of a producer's ring is slot u & 1 in phase (u >> 1) & 1; a slot starts out empty.
+  uint32_t batch_seq = 0;   // producer: the ring use that the next step goes to
+  bool pending = false;     // producer: use batch_seq - 1 holds the sub-item's latest step and is not yet handed over
   if constexpr (PRE) {
     if (warp >= kPoseProducerWarps) {
       SetMaxRegsInc<kPoseConsumerRegs>();
@@ -341,20 +345,26 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
       for (int i = 0; i < kPoseAccSize; ++i) acc0[i] = acc1[i] = 0.f;
       uint32_t seq0 = 0, seq1 = 0;
       bool done0 = false, done1 = false;
-      // Takes the next batch of producer p if it is ready; false if not.
+      // Takes the next step of producer p if it is ready; false if not.  The slot is released as soon as its records are in
+      // registers.
       auto consume = [&](int p, uint32_t& seq, bool& done, float (&acc)[kPoseAccSize]) {
         const int b = seq & 1;
-        if (!__all_sync(0xffffffffu, MbarTest(&batch_full[p][b], (seq >> 1) & 1))) return false;
-        const int3 h = batch_hdr[p][b];
-        if (h.z < 0) {
+        if (!__all_sync(0xffffffffu, MbarTest(SmemAddr(&batch_full[p][b]), (seq >> 1) & 1))) return false;
+        const int4 h = batch_hdr[p][b];
+        if (h.w < 0) {
           done = true;
           return true;
         }
-        if (lane < h.x) AccumulateRecord<STATS>(args.cam, rings + (p * kPoseRingSlots + b) * kPoseBatchFloats + lane, acc);
-        MbarArrive(&batch_empty[p][b]);
+        const float4* rec = rings + (p * kPoseRingSlots + b) * kPoseSlotChunks + lane;
+        float4 q[kPoseRecChunks];
+#pragma unroll
+        for (int c = 0; c < kPoseRecChunks; ++c) q[c] = rec[c * 32];
+        MbarArrive(SmemAddr(&batch_empty[p][b]));
         ++seq;
-        if (h.y) {
-          StorePoseTotal<DET>(args, h.z, lane, WarpTransposeReduce(acc, lane));
+        const unsigned bit = 1u << lane;
+        if (static_cast<unsigned>(h.x) & bit) AccumulateRecord<STATS>(args.cam, q, (static_cast<unsigned>(h.y) & bit) != 0u, acc);
+        if (h.z) {
+          StorePoseTotal<DET>(args, h.w, lane, WarpTransposeReduce(acc, lane));
 #pragma unroll
           for (int i = 0; i < kPoseAccSize; ++i) acc[i] = 0.f;
         }
@@ -370,19 +380,15 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
     }
     SetMaxRegsDec<kPoseProducerRegs>();
   }
-  float* my_ring = rings + warp * kPoseRingSlots * kPoseBatchFloats;   // PRE producers
-  auto acquire_slot = [&](uint32_t u) {
-    MbarWait(&batch_empty[warp][u & 1], ((u >> 1) & 1) ^ 1);
-  };
-  // last: the sub-item's final batch; kf < 0: no more batches from this producer
-  auto commit_slot = [&](uint32_t u, int pairs, bool last, int kf) {
-    if (lane == 0) batch_hdr[warp][u & 1] = make_int3(pairs, last ? 1 : 0, kf);
-    MbarArrive(&batch_full[warp][u & 1]);
-  };
+  // PRE producers: the ring, and the barriers of its slot 0 (slot 1's follow at + 8 bytes)
+  float4* my_ring = rings + warp * kPoseRingSlots * kPoseSlotChunks;
+  const uint32_t my_full = SmemAddr(&batch_full[PRE ? warp : 0][0]), my_empty = SmemAddr(&batch_empty[PRE ? warp : 0][0]);
+  auto acquire_slot = [&](uint32_t u) { MbarWait(my_empty + 8 * (u & 1), ((u >> 1) & 1) ^ 1); };
+  auto commit_slot = [&](uint32_t u) { MbarArrive(my_full + 8 * (u & 1)); };
 
   for (uint32_t it = 0;; ++it) {
     const int s = it & 1;
-    MbarWait(&full_bar[s], (it >> 1) & 1);
+    MbarWait(SmemAddr(&full_bar[s]), (it >> 1) & 1);
     const unsigned int item = *reinterpret_cast<volatile unsigned int*>(&s_item[s]);
     if (item >= n_items) break;
 
@@ -466,44 +472,33 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
         }
         const unsigned assoc_mask = __ballot_sync(0xffffffffu, st == 3);
         if (assoc_mask == 0) continue;
-        touched |= assoc_mask;
         if constexpr (PRE) {
-          // Pack the associated lanes densely behind the batch_fill pairs already in the current slot; the pairs that do not fit
-          // go to the next slot, and the full one is handed over.  A slot that is exactly full is handed over only once it is
-          // known whether more pairs follow in this sub-item (its header says whether it is the last batch).
-          const int m = __popc(assoc_mask);
-          const int pos = batch_fill + __popc(assoc_mask & ((1u << lane) - 1u));
-          const bool spill = batch_fill + m > 32;
-          if (!batch_owned) acquire_slot(batch_seq);
-          batch_owned = true;
-          if (spill) acquire_slot(batch_seq + 1);
+          // The step goes to a slot of its own.  The previous one is handed over only now that it is known not to be the
+          // sub-item's last (its header says whether it is).
+          const unsigned photo_mask = __ballot_sync(0xffffffffu, st == 3 && photo);
+          if (pending) commit_slot(batch_seq - 1);
+          acquire_slot(batch_seq);
+          float4* rec = my_ring + (batch_seq & 1) * kPoseSlotChunks + lane;
           if (st == 3) {
-            float* rec = my_ring + ((batch_seq + (pos >> 5)) & 1) * kPoseBatchFloats + (pos & 31);
-            rec[0 * 32] = r.lp.x; rec[1 * 32] = r.lp.y; rec[2 * 32] = r.lp.z;
-            rec[3 * 32] = r.ln.x; rec[4 * 32] = r.ln.y; rec[5 * 32] = r.ln.z;
-            rec[6 * 32] = r.d; rec[7 * 32] = r.nx; rec[8 * 32] = r.ny;
-            rec[9 * 32] = e.r1; rec[10 * 32] = e.r2;
-            rec[11 * 32] = e.gx1; rec[12 * 32] = e.gy1; rec[13 * 32] = e.gx2; rec[14 * 32] = e.gy2;
-            rec[15 * 32] = photo ? 1.f : 0.f;
+            rec[0 * 32] = make_float4(r.lp.x, r.lp.y, r.lp.z, r.ln.x);
+            rec[1 * 32] = make_float4(r.ln.y, r.ln.z, r.d, r.nx);
+            rec[2 * 32] = make_float4(r.ny, e.r1, e.r2, e.gx1);
+            rec[3 * 32] = make_float4(e.gy1, e.gx2, e.gy2, 0.f);
           }
-          if (spill) {
-            commit_slot(batch_seq, 32, false, kf);
-            ++batch_seq;
-            batch_fill += m - 32;
-          } else {
-            batch_fill += m;
-          }
-        } else if (st == 3) {
-          AccumulatePair<STATS>(cam, r, e, photo, acc);
+          if (lane == 0) batch_hdr[warp][batch_seq & 1] = make_int4(static_cast<int>(assoc_mask), static_cast<int>(photo_mask), 0, kf);
+          ++batch_seq;
+          pending = true;
+        } else {
+          touched |= assoc_mask;
+          if (st == 3) AccumulatePair<STATS>(cam, r, e, photo, acc);
         }
       }
 
-      if (PRE && touched) {
-        commit_slot(batch_seq, batch_fill, true, kf);
-        ++batch_seq;
-        batch_owned = false;
-        batch_fill = 0;
-      } else if (touched) {
+      if (PRE && pending) {   // the sub-item's last slot, also when its last steps had no associated lane
+        if (lane == 0) batch_hdr[warp][(batch_seq - 1) & 1].z = 1;
+        commit_slot(batch_seq - 1);
+        pending = false;
+      } else if (!PRE && touched) {
         StorePoseTotal<DET>(args, kf, lane, WarpTransposeReduce(acc, lane));
       }
       if (STATS) {
@@ -524,9 +519,10 @@ __global__ void __launch_bounds__(PRE ? kPoseWsThreads : kPoseThreads, kPoseMinC
       }
     }
   }
-  if (PRE) {
-    if (!batch_owned) acquire_slot(batch_seq);
-    commit_slot(batch_seq, 0, false, -1);
+  if (PRE) {   // no more slots from this producer
+    acquire_slot(batch_seq);
+    if (lane == 0) batch_hdr[warp][batch_seq & 1] = make_int4(0, 0, 0, -1);
+    commit_slot(batch_seq);
   }
 }
 

@@ -32,7 +32,7 @@ def main():
     txt = subprocess.run(["nvdisasm", "--print-line-info", cub], capture_output=True, text=True).stdout.splitlines()
     rows, cur, on = [], ("?", 0), False
     for ln in txt:
-        if ln.lstrip().startswith(".section"):
+        if ln.split()[:1] == [".section"]:   # (not .sectionflags, which follows it)
             on = ".text." in ln and kern in ln
             continue
         if not on:
