@@ -149,6 +149,9 @@ SYMBOLS = {
     "bba_set_keyframe_states": (C.c_int, [_P, C.c_int, _P, _P]),
     "bba_get_keyframe_states": (C.c_int, [_P, C.c_int, _P, _P]),
     "bba_get_covisibility": (C.c_int, [_P, C.c_int, _P]),
+    "bba_set_keyframe_pose_priors": (C.c_int, [_P, C.c_int, _P, _P, _P]),
+    "bba_clear_keyframe_pose_priors": (C.c_int, [_P, C.c_int, _P]),
+    "bba_get_keyframe_pose_prior": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
     "bba_set_intrinsics": (C.c_int, [_P, _F7, _F7, C.c_float]),
     "bba_get_intrinsics": (C.c_int, [_P, _F7, _F7, C.POINTER(C.c_float)]),
     "bba_host_se3_exp": (None, [_P, _P]),
@@ -157,6 +160,7 @@ SYMBOLS = {
     "bba_host_se3_inverse": (None, [_P, _P]),
     "bba_host_pose_update_converged": (C.c_int, [_P]),
     "bba_host_solve_ldlt": (C.c_int, [C.c_int, _P, _P, _P]),
+    "bba_host_pose_prior_terms": (None, [_P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_frusta_intersect": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, C.c_float, _P, C.c_float, C.c_float]),
     "bba_host_motion_model_clear": (None, [C.POINTER(MotionModelRecord), _P, _P]),
     "bba_host_motion_model_predict": (C.c_int, [C.POINTER(MotionModelRecord), C.c_int, _P, _P]),

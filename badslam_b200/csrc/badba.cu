@@ -8,6 +8,7 @@
 //     <=30 x 2   pose accumulate + solve for ALL keyframes at once (reference: K x n_GN x {2 clears, kernel,
 //                2 D2H copies, stream sync}, kernel_opt_pose.cc:67-96)
 // and the host synchronises ONCE per outer iteration to read back the poses.
+#include <cmath>
 #include <cstring>
 
 #include "handle.hpp"
@@ -103,6 +104,7 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
     v.pose = kf.pose;
     v.min_depth = kf.min_depth; v.max_depth = kf.max_depth;
     v.activation = kf.activation;
+    v.prior = h->pose_priors[k];
   }
   const CameraView cams = LiveCameraView(h);
   std::lock_guard<std::mutex> lock(f.mu);
@@ -349,6 +351,9 @@ bba_status bba_create(const bba_config* cfg, bba_handle* out) {
   CREATE_TRY(h->d_cfactor.Reserve(static_cast<size_t>(h->cf_w) * h->cf_h));
   CREATE_TRY(cudaMemset(h->d_cfactor, 0, sizeof(float) * h->cf_w * h->cf_h));
   CREATE_TRY(h->d_kfs.Reserve(K));
+  CREATE_TRY(h->d_pose_priors.Reserve(K));
+  CREATE_TRY(cudaMemset(h->d_pose_priors, 0, sizeof(bba::PosePrior) * K));
+  h->pose_priors.assign(K, bba::PosePrior{});
   CREATE_TRY(p.d_work_records.Reserve(K));
   CREATE_TRY(p.d_pose_est.Reserve(7 * K));
   CREATE_TRY(p.d_acc.Reserve(bba::kPoseAccSize * K));
@@ -564,6 +569,10 @@ int bba_host_solve_ldlt(int n, const double* upper, const double* b, double* x) 
   else return 0;
   return 1;
 }
+void bba_host_pose_prior_terms(const float prior[7], const float pose[7], const float info[21], double H[21], double b[6], double* cost) {
+  if (!prior || !pose || !info || !H || !b || !cost) return;
+  bba::PosePriorTerms(prior, pose, info, H, b, cost);
+}
 int bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height, const float global_T_frame_a[7], float min_depth_a,
                               float max_depth_a, const float global_T_frame_b[7], float min_depth_b, float max_depth_b) {
   Frustum a, b;
@@ -772,6 +781,108 @@ bba_status bba_get_keyframe_states(bba_handle h, int count, float* poses, int* a
   }
   return BBA_OK;
 }
+// ---- soft pose priors ----
+namespace {
+// Whether the symmetric 6x6 matrix with upper triangle info is positive semi-definite up to fp32 rounding: the pivoted LDLT of
+// SolveLDLT (largest |diagonal| first) has no negative pivot, and a zero pivot leaves nothing in its column.
+bool InformationPsd(const float info[21]) {
+  double M[36];
+  double scale = 0.0;
+  int idx = 0;
+  for (int r = 0; r < 6; ++r)
+    for (int c = r; c < 6; ++c) {
+      M[r * 6 + c] = M[c * 6 + r] = info[idx++];
+      scale = std::max(scale, std::fabs(static_cast<double>(info[idx - 1])));
+    }
+  if (scale == 0.0) return true;
+  const double pivot_tol = 1e-6 * scale, column_tol = 1e-3 * scale;
+  bool done[6] = {};
+  for (int k = 0; k < 6; ++k) {
+    int p = -1;
+    for (int i = 0; i < 6; ++i)
+      if (!done[i] && (p < 0 || std::fabs(M[i * 6 + i]) > std::fabs(M[p * 6 + p]))) p = i;
+    done[p] = true;
+    const double d = M[p * 6 + p];
+    if (d < -pivot_tol) return false;
+    if (d <= pivot_tol) {
+      for (int i = 0; i < 6; ++i)
+        if (!done[i] && std::fabs(M[i * 6 + p]) > column_tol) return false;
+      continue;
+    }
+    for (int i = 0; i < 6; ++i)
+      for (int j = 0; j < 6; ++j)
+        if (!done[i] && !done[j]) M[i * 6 + j] -= M[i * 6 + p] * M[p * 6 + j] / d;
+  }
+  return true;
+}
+
+// Uploads the prior table for the pose solve and publishes the records.
+bba_status CommitPosePriors(bba_handle h) {
+  int count = 0;
+  for (const PosePrior& p : h->pose_priors) count += p.has ? 1 : 0;
+  h->pose_prior_count = count;
+  BBA_CUDA(h, cudaMemcpy(h->d_pose_priors, h->pose_priors.data(), sizeof(PosePrior) * h->pose_priors.size(), cudaMemcpyHostToDevice));
+  return Publish(h, nullptr, false);
+}
+}  // namespace
+
+bba_status bba_set_keyframe_pose_priors(bba_handle h, int count, const int* ids, const float* poses, const float* information) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_set_keyframe_pose_priors: ";
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
+  if (count > 0 && (!ids || !poses || !information)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  const int K = static_cast<int>(h->keyframes.size());
+  for (int i = 0; i < count; ++i) {
+    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
+    const float* p = poses + 7 * static_cast<size_t>(i);
+    const float* info = information + 21 * static_cast<size_t>(i);
+    bool finite = true;
+    for (int j = 0; j < 7; ++j) finite = finite && std::isfinite(p[j]);
+    for (int j = 0; j < 21; ++j) finite = finite && std::isfinite(info[j]);
+    if (!finite) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose or information");
+    if (p[0] * p[0] + p[1] * p[1] + p[2] * p[2] + p[3] * p[3] < 1e-12f) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "zero quaternion");
+    if (!InformationPsd(info)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information matrix is not positive semi-definite");
+  }
+  for (int i = 0; i < count; ++i) {
+    PosePrior& r = h->pose_priors[ids[i]];
+    std::memcpy(r.pose, poses + 7 * static_cast<size_t>(i), sizeof(r.pose));
+    std::memcpy(r.info, information + 21 * static_cast<size_t>(i), sizeof(r.info));
+    r.has = 1;
+  }
+  return CommitPosePriors(h);
+}
+
+bba_status bba_clear_keyframe_pose_priors(bba_handle h, int count, const int* ids) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_clear_keyframe_pose_priors: ";
+  const int K = static_cast<int>(h->keyframes.size());
+  if (count == -1) {
+    std::fill(h->pose_priors.begin(), h->pose_priors.end(), PosePrior{});
+    return CommitPosePriors(h);
+  }
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < -1");
+  if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  for (int i = 0; i < count; ++i)
+    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
+  for (int i = 0; i < count; ++i) h->pose_priors[ids[i]] = PosePrior{};
+  return CommitPosePriors(h);
+}
+
+bba_status bba_get_keyframe_pose_prior(bba_handle h, int id, float pose[7], float information[21], int* has_prior) {
+  FrontEndScope front_end;
+  if (!h || !has_prior) return BBA_ERR_INVALID_ARGUMENT;
+  std::unique_lock<std::mutex> lock(h->fe.mu);
+  if (id < 0 || id >= static_cast<int>(h->fe.kfs.size())) {
+    lock.unlock();
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bad keyframe id");
+  }
+  const PosePrior& p = h->fe.kfs[id].prior;
+  *has_prior = p.has;
+  if (pose) std::memcpy(pose, p.pose, sizeof(p.pose));
+  if (information) std::memcpy(information, p.info, sizeof(p.info));
+  return BBA_OK;
+}
+
 bba_status bba_get_covisibility(bba_handle h, int id, uint8_t* out_row) {
   CHECK_KF(h, id);
   std::memset(out_row, 0, h->keyframes.size());

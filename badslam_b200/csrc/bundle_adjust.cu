@@ -505,6 +505,33 @@ bba::PcgArgs MakePcgArgs(bba_handle h, const PcgLayout& L, int gauge) {
   return a;
 }
 
+// The soft pose priors' terms of the pose unknowns (every keyframe with a prior but the gauge) at the poses the init pass sees,
+// staged for LaunchPcgPosePrior.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.
+bba_status StagePcgPriors(bba_handle h, const PcgLayout& L, int gauge, cudaStream_t s) {
+  auto& pc = h->pcg;
+  pc.prior_terms = 0;
+  if (!L.opt_poses || h->pose_prior_count == 0 || h->cfg.rank != 0) return BBA_OK;
+  const int K = static_cast<int>(h->keyframes.size());
+  BBA_CUDA(h, pc.h_prior_terms.Reserve(h->cfg.max_keyframes));
+  BBA_CUDA(h, pc.d_prior_terms.Reserve(h->cfg.max_keyframes));
+  int n = 0;
+  for (int k = 0; k < K; ++k) {
+    const PosePrior& prior = h->pose_priors[k];
+    if (k == gauge || !prior.has) continue;
+    bba::PcgPriorTerm& t = pc.h_prior_terms[n++];
+    t.u = 6u * static_cast<uint32_t>(k < gauge ? k : k - 1);
+    float pose[7];
+    PoseToArray(h->keyframes[k].pose, pose);
+    double H[21], b[6], cost;
+    bba::PosePriorTerms(prior.pose, pose, prior.info, H, b, &cost);
+    for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(H[j]);
+    for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(b[j]);
+  }
+  if (n) BBA_CUDA(h, cudaMemcpyAsync(pc.d_prior_terms, pc.h_prior_terms, sizeof(bba::PcgPriorTerm) * n, cudaMemcpyHostToDevice, s));
+  pc.prior_terms = n;
+  return BBA_OK;
+}
+
 // The PCG solver's phases, shared by BundleAdjustPCG and the parity hook bba_pcg_debug.  Vectors: d_pcg = {r, M, delta, g, p};
 // scalars = {alpha_n or beta_n (slot an), alpha_d (1), beta_n or alpha_n (slot bn), this rank's alpha_d (3, multi-GPU)}.
 // Init: r = -J^T W F and M = diag(J^T W J) over every keyframe (:312-361), then PCGInit2 (:363-373) into slot `an`.
@@ -514,6 +541,8 @@ bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int 
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_vec[1], 0, sizeof(float) * U, s));
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars, 0, sizeof(double) * 4, s));
   BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
+  if (bba_status st = StagePcgPriors(h, L, a.gauge_kf, s)) return st;
+  BBA_LAUNCH(h, h->launches, LaunchPcgPosePrior, h->pcg.d_prior_terms, h->pcg.prior_terms, true, a.r, a.M, nullptr, nullptr, nullptr, s);
   if (h->cfg.world_size > 1) {
     if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[0], U, s)) return st;
     if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[1], U, s)) return st;
@@ -527,6 +556,8 @@ bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int 
 // Inner step, first half: g += J^T W J p and alpha_d += p^T J^T W J p over every keyframe (PCGStep1CUDA, :392-419).
 bba_status PcgStep1(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, cudaStream_t s) {
   BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, false, s);
+  BBA_LAUNCH(h, h->launches, LaunchPcgPosePrior, h->pcg.d_prior_terms, h->pcg.prior_terms, false, nullptr, nullptr, a.p, a.g,
+             a.scalars + a.alpha_d_slot, s);
   if (h->cfg.world_size > 1) {   // g and this rank's part of alpha_d: one all-reduce
     float* g = h->pcg.d_vec[3];
     BBA_LAUNCH(h, h->launches, LaunchPcgPackAlphaD, h->pcg.d_scalars, g + L.unknown_count, s);

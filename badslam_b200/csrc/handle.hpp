@@ -139,6 +139,7 @@ struct KeyframeView {
   Pose pose;
   float min_depth = 0.f, max_depth = 0.f;
   int activation = BBA_KF_ACTIVE;
+  PosePrior prior{};
 };
 
 // The cameras, the depth deformation parameter a, the residual types and the deterministic mode as the BA side published them last.
@@ -183,6 +184,11 @@ struct bba_context {
   bba::DeviceBuffer<float> d_cfactor;
   std::vector<bba::Keyframe> keyframes;
   bba::DeviceBuffer<bba::KfDevice> d_kfs;   // [max_kf] the keyframes' parameters as the kernels read them
+  // soft pose priors by keyframe id (bba_set_keyframe_pose_priors): the host records, their device copy that the pose solve
+  // reads, and how many keyframes have one (0: the pose solve and the PCG solver run without the table)
+  std::vector<bba::PosePrior> pose_priors;   // [max_kf]
+  bba::DeviceBuffer<bba::PosePrior> d_pose_priors;
+  int pose_prior_count = 0;
 
   // staging: pinned records and the shared planes of the keyframe / frame uploads
   struct Staging {
@@ -276,6 +282,10 @@ struct bba_context {
     bba::DeviceBuffer<double> d_scalars;   // [0] / [2] alpha_n, beta_n (roles swap), [1] alpha_d
     bba::PinnedBuffer<double> h_scalars;
     bba::PinnedBuffer<float> h_delta;      // pose part (6 * max_keyframes) + 16
+    // the soft pose priors' terms at the poses of the current outer iteration (StagePcgPriors)
+    bba::PinnedBuffer<bba::PcgPriorTerm> h_prior_terms;
+    bba::DeviceBuffer<bba::PcgPriorTerm> d_prior_terms;
+    int prior_terms = 0;
   } pcg;
 
   // multi-GPU exchange (multi_gpu.cu)

@@ -254,6 +254,170 @@ BBA_HD void SolveLDLT(const double* upper, const double* b, double* x) {
   for (int i = 0; i < N; ++i) x[perm[i]] = y[i];
 }
 
+// ---- soft pose prior on a keyframe (bba_set_keyframe_pose_priors) ----
+// One keyframe's prior as the pose solve reads it: the prior global_T_frame P and the upper triangle of its 6x6 information
+// matrix L (row-major, the tangent order of H: translation, then rotation).
+struct PosePrior {
+  float pose[7];
+  float info[21];
+  int has;   // 0: no prior on this keyframe
+};
+
+// 3x3 helpers in fp64 (row-major).
+BBA_HD void HatD(const double w[3], double O[9]) {
+  O[0] = 0.0; O[1] = -w[2]; O[2] = w[1];
+  O[3] = w[2]; O[4] = 0.0; O[5] = -w[0];
+  O[6] = -w[1]; O[7] = w[0]; O[8] = 0.0;
+}
+BBA_HD void Mat3MulD(const double A[9], const double B[9], double C[9]) {
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) C[r * 3 + c] = A[r * 3] * B[c] + A[r * 3 + 1] * B[3 + c] + A[r * 3 + 2] * B[6 + c];
+}
+
+// The inverse left Jacobian of SO(3) at the rotation vector w with angle theta = |w|: I - W/2 + c W^2.
+BBA_HD void So3LeftJacobianInverse(const double w[3], double theta, double A[9]) {
+  const double t2 = theta * theta;
+  double c;
+  if (theta < 0.05) {
+    c = 1.0 / 12.0 + t2 / 720.0 + t2 * t2 / 30240.0;
+  } else {
+    const double h = 0.5 * theta;
+    c = (1.0 - h * cos(h) / sin(h)) / t2;
+  }
+  double W[9], W2[9];
+  HatD(w, W);
+  Mat3MulD(W, W, W2);
+  for (int i = 0; i < 9; ++i) A[i] = -0.5 * W[i] + c * W2[i];
+  A[0] += 1.0; A[4] += 1.0; A[8] += 1.0;
+}
+
+// r = log(P^-1 T) in the tangent order (translation, rotation), fp64, the rotation angle in [0, pi].  The quaternions are
+// normalised first.
+BBA_HD void PosePriorResidual(const float prior[7], const float pose[7], double r[6], double* theta_out) {
+  double qp[4], qt[4];
+  double np = 0.0, nt = 0.0;
+  for (int i = 0; i < 4; ++i) {
+    qp[i] = prior[i];
+    qt[i] = pose[i];
+    np += qp[i] * qp[i];
+    nt += qt[i] * qt[i];
+  }
+  np = 1.0 / sqrt(np);
+  nt = 1.0 / sqrt(nt);
+  for (int i = 0; i < 4; ++i) {
+    qp[i] *= np;
+    qt[i] *= nt;
+  }
+  // q = conj(qp) * qt,  t = R(qp)^T (t_T - t_P)
+  const double ax = -qp[0], ay = -qp[1], az = -qp[2], aw = qp[3];
+  const double bx = qt[0], by = qt[1], bz = qt[2], bw = qt[3];
+  double q[4];
+  q[3] = aw * bw - ax * bx - ay * by - az * bz;
+  q[0] = aw * bx + ax * bw + ay * bz - az * by;
+  q[1] = aw * by + ay * bw + az * bx - ax * bz;
+  q[2] = aw * bz + az * bw + ax * by - ay * bx;
+  const double d[3] = {static_cast<double>(pose[4]) - prior[4], static_cast<double>(pose[5]) - prior[5],
+                       static_cast<double>(pose[6]) - prior[6]};
+  // rotate d by conj(qp): v + w u + v x u with u = 2 (qv x d), qv = -qp.xyz
+  const double ux = 2.0 * (ay * d[2] - az * d[1]), uy = 2.0 * (az * d[0] - ax * d[2]), uz = 2.0 * (ax * d[1] - ay * d[0]);
+  const double t[3] = {d[0] + aw * ux + (ay * uz - az * uy), d[1] + aw * uy + (az * ux - ax * uz), d[2] + aw * uz + (ax * uy - ay * ux)};
+  if (q[3] < 0.0)
+    for (int i = 0; i < 4; ++i) q[i] = -q[i];
+  const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+  const double theta = 2.0 * atan2(n, q[3]);
+  const double f = (n > 1e-10) ? theta / n : 2.0 / q[3] * (1.0 - n * n / (3.0 * q[3] * q[3]));
+  const double w[3] = {f * q[0], f * q[1], f * q[2]};
+  double A[9];
+  So3LeftJacobianInverse(w, theta, A);
+  for (int i = 0; i < 3; ++i) {
+    r[i] = A[i * 3] * t[0] + A[i * 3 + 1] * t[1] + A[i * 3 + 2] * t[2];
+    r[3 + i] = w[i];
+  }
+  *theta_out = theta;
+}
+
+// J = Jr^-1(r), the inverse right Jacobian of SE(3) in the tangent order (rho, phi): d log(exp(r) exp(delta)) / d delta at 0.
+// Jr^-1(r) = Jl^-1(-r) = [[A, -A Q A], [0, A]] with A = Jl^-1_SO3(-phi) and Q = Q(-rho, -phi) (Barfoot, eq. 7.86).
+BBA_HD void Se3RightJacobianInverse(const double r[6], double theta, double J[36]) {
+  const double rho[3] = {-r[0], -r[1], -r[2]}, phi[3] = {-r[3], -r[4], -r[5]};
+  double A[9];
+  So3LeftJacobianInverse(phi, theta, A);
+  const double t2 = theta * theta;
+  double c1, c2, c3;
+  if (theta < 0.05) {
+    c1 = 1.0 / 6.0 - t2 / 120.0 + t2 * t2 / 5040.0;
+    c2 = 1.0 / 24.0 - t2 / 720.0 + t2 * t2 / 40320.0;
+    c3 = 1.0 / 120.0 - t2 / 2520.0 + t2 * t2 / 120960.0;
+  } else {
+    const double s = sin(theta), c = cos(theta);
+    c1 = (theta - s) / (t2 * theta);
+    c2 = (t2 + 2.0 * c - 2.0) / (2.0 * t2 * t2);
+    c3 = (2.0 * theta - 3.0 * s + theta * c) / (2.0 * t2 * t2 * theta);
+  }
+  double P[9], R[9], PR[9], RP[9], PRP[9], PP[9], PPR[9], RPP[9], PRPP[9], PPRP[9];
+  HatD(phi, P);
+  HatD(rho, R);
+  Mat3MulD(P, R, PR);
+  Mat3MulD(R, P, RP);
+  Mat3MulD(PR, P, PRP);
+  Mat3MulD(P, P, PP);
+  Mat3MulD(PP, R, PPR);
+  Mat3MulD(RP, P, RPP);
+  Mat3MulD(PRP, P, PRPP);
+  Mat3MulD(PP, RP, PPRP);
+  double Q[9];
+  for (int i = 0; i < 9; ++i)
+    Q[i] = 0.5 * R[i] + c1 * (PR[i] + RP[i] + PRP[i]) + c2 * (PPR[i] + RPP[i] - 3.0 * PRP[i]) + c3 * (PRPP[i] + PPRP[i]);
+  double AQ[9], AQA[9];
+  Mat3MulD(A, Q, AQ);
+  Mat3MulD(AQ, A, AQA);
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      J[i * 6 + j] = A[i * 3 + j];
+      J[i * 6 + 3 + j] = -AQA[i * 3 + j];
+      J[(3 + i) * 6 + j] = 0.0;
+      J[(3 + i) * 6 + 3 + j] = A[i * 3 + j];
+    }
+}
+
+// The prior's terms at global_T_frame = pose, for an update pose <- pose * exp(delta): with r = log(P^-1 pose) and J = Jr^-1(r),
+// H = J^T L J (upper triangle, 21), b = J^T L r (6), cost = r^T L r / 2.  fp64 throughout.
+BBA_HD void PosePriorTerms(const float prior[7], const float pose[7], const float info[21], double H[21], double b[6], double* cost) {
+  double r[6], theta, J[36], L[36];
+  PosePriorResidual(prior, pose, r, &theta);
+  Se3RightJacobianInverse(r, theta, J);
+  int idx = 0;
+  for (int i = 0; i < 6; ++i)
+    for (int j = i; j < 6; ++j) {
+      L[i * 6 + j] = L[j * 6 + i] = info[idx];
+      ++idx;
+    }
+  double LJ[36], Lr[6];
+  for (int i = 0; i < 6; ++i) {
+    Lr[i] = 0.0;
+    for (int k = 0; k < 6; ++k) Lr[i] += L[i * 6 + k] * r[k];
+    for (int j = 0; j < 6; ++j) {
+      double s = 0.0;
+      for (int k = 0; k < 6; ++k) s += L[i * 6 + k] * J[k * 6 + j];
+      LJ[i * 6 + j] = s;
+    }
+  }
+  idx = 0;
+  double c = 0.0;
+  for (int i = 0; i < 6; ++i) {
+    double s = 0.0;
+    for (int k = 0; k < 6; ++k) s += J[k * 6 + i] * Lr[k];
+    b[i] = s;
+    c += r[i] * Lr[i];
+    for (int j = i; j < 6; ++j) {
+      double h = 0.0;
+      for (int k = 0; k < 6; ++k) h += J[k * 6 + i] * LJ[k * 6 + j];
+      H[idx++] = h;
+    }
+  }
+  *cost = 0.5 * c;
+}
+
 // Camera frusta and their intersection test (co-visibility of keyframes), host only.
 struct Frustum {   // libvis/src/libvis/camera_frustum.h:43-250
   float p[8][3];

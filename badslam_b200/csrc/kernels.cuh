@@ -11,6 +11,8 @@
 
 namespace bba {
 
+struct PosePrior;   // host_math.hpp
+
 // Accumulator record per keyframe written by the pose kernel: 32 fp64 sums
 //   [0..20] H upper triangle row-major, [21..26] b, [27] n_assoc, [28] n_photo,
 //   [29] cost_depth, [30] cost_desc1, [31] cost_desc2
@@ -102,6 +104,7 @@ struct PoseSolveArgs {
   unsigned int* queue;         // PoseAccumulateKernel's work-item counter, re-armed here
   int iteration;
   int max_iterations;
+  const PosePrior* priors;     // [max_kf] soft pose priors by keyframe id, or null when no keyframe has one
 };
 // Device-side Gauss-Newton step for every keyframe in the list (direct_ba_alternating.cc:173-233).
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
@@ -248,6 +251,15 @@ LaunchResult LaunchPcgStep3(uint32_t n, uint32_t a_index, int kf_count, float* g
 LaunchResult LaunchPcgUpdateSurfels(float* surfels, uint32_t pitch, uint32_t n, bool use_desc, uint32_t surfel_start, const float* delta,
                                     cudaStream_t stream);
 LaunchResult LaunchPcgUpdateCfactor(float* cfactor, uint32_t cells, const float* delta, cudaStream_t stream);
+// The soft pose prior of one pose unknown block of the PCG solver: first unknown u, J^T L J (upper triangle) and J^T L r.
+struct PcgPriorTerm {
+  uint32_t u;
+  float H[21];
+  float b[6];
+};
+// init: r -= J^T L r, M += diag(J^T L J); else g += J^T L J p, *alpha_d += p^T J^T L J p (a fixed-order fp64 sum).
+LaunchResult LaunchPcgPosePrior(const PcgPriorTerm* terms, int count, bool init, float* r, float* M, const float* p, float* g,
+                                double* alpha_d, cudaStream_t stream);
 
 // End-of-BA surfel maintenance (lifecycle.cu; PerformBASchemeEndTasks, direct_ba.cc:566-653).
 struct KfRadius {

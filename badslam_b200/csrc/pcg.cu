@@ -437,6 +437,55 @@ LaunchResult LaunchPcgUnpackAlphaD(double* scalars, const float* tail, cudaStrea
   return {1};
 }
 
+// The soft pose priors' part of the products, one thread per prior-carrying pose block after PcgAccumulateKernel (one block: a
+// few thousand keyframes at most, and alpha_d's share is summed in a fixed order).
+template <bool INIT>
+__global__ void __launch_bounds__(256) PcgPosePriorKernel(const PcgPriorTerm* __restrict__ terms, int count, float* __restrict__ r,
+                                                          float* __restrict__ M, const float* __restrict__ p, float* __restrict__ g,
+                                                          double* __restrict__ alpha_d) {
+  double pap = 0.0;
+  for (int i = threadIdx.x; i < count; i += blockDim.x) {
+    const PcgPriorTerm& t = terms[i];
+    if constexpr (INIT) {
+      int d = 0;
+      for (int c = 0; c < 6; ++c) {
+        r[t.u + c] -= t.b[c];
+        M[t.u + c] += t.H[d];
+        d += 6 - c;
+      }
+    } else {
+      float pv[6], hp[6];
+      for (int c = 0; c < 6; ++c) {
+        pv[c] = p[t.u + c];
+        hp[c] = 0.f;
+      }
+      int idx = 0;
+      for (int row = 0; row < 6; ++row)
+        for (int col = row; col < 6; ++col) {
+          const float h = t.H[idx++];
+          hp[row] += h * pv[col];
+          if (col != row) hp[col] += h * pv[row];
+        }
+      for (int c = 0; c < 6; ++c) {
+        g[t.u + c] += hp[c];
+        pap += static_cast<double>(pv[c] * hp[c]);
+      }
+    }
+  }
+  if constexpr (!INIT) {
+    pap = BlockSum(pap);
+    if (threadIdx.x == 0) *alpha_d += pap;
+  }
+}
+
+LaunchResult LaunchPcgPosePrior(const PcgPriorTerm* terms, int count, bool init, float* r, float* M, const float* p, float* g,
+                                double* alpha_d, cudaStream_t stream) {
+  if (count <= 0) return {};
+  if (init) PcgPosePriorKernel<true><<<1, 256, 0, stream>>>(terms, count, r, M, p, g, alpha_d);
+  else PcgPosePriorKernel<false><<<1, 256, 0, stream>>>(terms, count, r, M, p, g, alpha_d);
+  return {1};
+}
+
 LaunchResult LaunchPcgAccumulate(const PcgArgs& a, int sm_count, bool init, cudaStream_t stream) {
   if (a.end <= a.begin || a.kf_count <= 0) return {};
   LaunchResult r{1, cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream)};

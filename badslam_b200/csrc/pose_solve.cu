@@ -54,6 +54,15 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
     a.stage_counts[2 * kf] = 0ull;
     a.stage_counts[2 * kf + 1] = 0ull;
 
+    float* pe = a.pose_est + static_cast<size_t>(kf) * 7;
+    if (a.priors && a.priors[kf].has) {
+      // the soft pose prior (bba_set_keyframe_pose_priors), added to the rounded sums in fp64 at the current estimate
+      const PosePrior& prior = a.priors[kf];
+      double Hp[21], bp[6], cost;
+      PosePriorTerms(prior.pose, pe, prior.info, Hp, bp, &cost);
+      for (int j = 0; j < 21; ++j) H[j] += Hp[j];
+      for (int j = 0; j < 6; ++j) b[j] += bp[j];
+    }
     SolveLDLT<6>(H, b, x);
     float xf[6], neg[6];
     for (int j = 0; j < 6; ++j) {
@@ -61,7 +70,6 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
       neg[j] = -xf[j];
     }
     Pose est;
-    float* pe = a.pose_est + static_cast<size_t>(kf) * 7;
     est.q[0] = pe[0]; est.q[1] = pe[1]; est.q[2] = pe[2]; est.q[3] = pe[3];
     est.t[0] = pe[4]; est.t[1] = pe[5]; est.t[2] = pe[6];
     est = Compose(est, Exp(neg));   // direct_ba_alternating.cc:214 (kDamping = 1)

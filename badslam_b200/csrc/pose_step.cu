@@ -280,6 +280,7 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
   sol.totals = p.d_totals;
   sol.host_flag = p.d_flag;
   sol.queue = p.d_queue;
+  sol.priors = h->pose_prior_count ? h->d_pose_priors.get() : nullptr;
   p.h_flag[0] = 0;
   p.h_flag[1] = n_local;
   if (h->profiling) BBA_CUDA(h, cudaMemsetAsync(p.d_totals, 0, sizeof(unsigned long long) * 8, s));

@@ -500,6 +500,35 @@ class DirectBA:
         self._check(self._lib.bba_get_keyframe_states(self._h, K, p.ctypes.data, a.ctypes.data))
         return p, a
 
+    # -- soft pose priors (not in the reference; include/badba.h "Soft pose priors") ----------------------------------------
+    def SetKeyframePosePriors(self, ids, poses, information):
+        """Anchors keyframes `ids` to prior global_T_frame poses ([n, 7]) with the cost 1/2 r^T L r, r = log(prior^-1 *
+        global_T_frame) (translation, then rotation).  information: [n, 21] upper triangles of L, or [n, 6, 6] / [6, 6]
+        matrices (one matrix for all).  Refused as a whole (nothing changes) for an unknown id, a non-finite value or an L that
+        is not positive semi-definite."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), np.int32)
+        n = len(ids)
+        p = np.ascontiguousarray(np.asarray(poses, np.float32).reshape(n, 7))
+        L = np.asarray(information, np.float32)
+        if L.shape[-2:] == (6, 6):
+            L = np.broadcast_to(L, (n, 6, 6))[:, np.triu_indices(6)[0], np.triu_indices(6)[1]]
+        L = np.ascontiguousarray(np.broadcast_to(L.reshape(-1, 21), (n, 21)), np.float32)
+        self._check(self._lib.bba_set_keyframe_pose_priors(self._h, n, ids.ctypes.data, p.ctypes.data, L.ctypes.data))
+
+    def ClearKeyframePosePriors(self, ids=None):
+        """Removes the priors of keyframes `ids`, or every prior with ids=None."""
+        if ids is None:
+            self._check(self._lib.bba_clear_keyframe_pose_priors(self._h, -1, None))
+            return
+        ids = np.ascontiguousarray(np.atleast_1d(ids), np.int32)
+        self._check(self._lib.bba_clear_keyframe_pose_priors(self._h, len(ids), ids.ctypes.data))
+
+    def KeyframePosePrior(self, keyframe_id: int):
+        """(prior global_T_frame [7], L upper triangle [21]) of a keyframe as last published, or None without a prior."""
+        p, L, has = np.zeros(7, np.float32), np.zeros(21, np.float32), C.c_int()
+        self._check(self._lib.bba_get_keyframe_pose_prior(self._h, keyframe_id, p.ctypes.data, L.ctypes.data, C.byref(has)))
+        return (p, L) if has.value else None
+
     # -- trajectory deformation around a BA call (trajectory_deformation.h:43-58) ----------------------------------------
     def RememberKeyframePoses(self) -> np.ndarray:
         """RememberKeyframePoses (trajectory_deformation.cc:33-42): frame_T_global of every keyframe, [K, 7], all from one

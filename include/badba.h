@@ -208,6 +208,26 @@ bba_status bba_get_keyframe_activation(bba_handle h, int keyframe_id, int* activ
 bba_status bba_set_keyframe_states(bba_handle h, int count, const float* global_T_frame, const int* activation);
 bba_status bba_get_keyframe_states(bba_handle h, int count, float* global_T_frame, int* activation);
 bba_status bba_get_covisibility(bba_handle h, int keyframe_id, uint8_t* out_row /* [keyframe_count] */);
+/* Soft pose priors (not in the reference; g2o / Ceres / GTSAM offer the same term): a keyframe with a prior adds
+ * 1/2 r^T L r to the cost, r = log(prior^-1 * global_T_frame) in the tangent order of the pose solve (translation, then
+ * rotation, Sophus), L a 6x6 information matrix given as its upper triangle, row-major, in the layout of H (21 floats).  The
+ * term enters only where the keyframe's pose is optimised: the pose step of the alternating scheme and bba_estimate_frame_pose
+ * (a keyframe that is inactive in a BA iteration keeps its pose), and the pose unknowns of the PCG scheme (not the gauge
+ * keyframe).  A handle without priors runs exactly the code it ran before they existed.  With several ranks every rank sets the
+ * same priors, as it adds the same keyframes.
+ *  bba_set_keyframe_pose_priors: ids [count], prior_global_T_frame [count][7], information [count][21]; replaces the prior of
+ *    each listed keyframe.  BBA_ERR_INVALID_ARGUMENT for an unknown id, a non-finite value, a zero quaternion or an L that is not
+ *    positive semi-definite (the pivoted LDLT of L has a negative pivot, or a zero pivot with a non-zero column); the arguments
+ *    are checked before anything changes, and a failed call leaves the handle unchanged.
+ *  bba_clear_keyframe_pose_priors: removes the priors of ids [count]; count = -1 removes every prior (ids is not read).
+ *  bba_get_keyframe_pose_prior: front-end call (the published priors); *has_prior = 0 and zeros without a prior (pose /
+ *    information may be NULL).
+ * The setters are BA-side calls and publish. */
+bba_status bba_set_keyframe_pose_priors(bba_handle h, int count, const int* keyframe_ids, const float* prior_global_T_frame,
+                                        const float* information);
+bba_status bba_clear_keyframe_pose_priors(bba_handle h, int count, const int* keyframe_ids);
+bba_status bba_get_keyframe_pose_prior(bba_handle h, int keyframe_id, float prior_global_T_frame[7], float information[21],
+                                       int* has_prior);
 
 /* depth_params_ / cameras (direct_ba.h:243-297; SetColorCamera etc.).  The getters bba_get_intrinsics, bba_get_residual_types,
  * bba_get_cfactor_host and bba_cfactor_size are front-end calls (the published cameras, a, residual types and cfactor; the
@@ -645,6 +665,11 @@ void bba_host_se3_compose(const float a[7], const float b[7], float out_pose[7])
 void bba_host_se3_inverse(const float a[7], float out_pose[7]);
 int  bba_host_pose_update_converged(const float x[6]);
 int  bba_host_solve_ldlt(int n, const double* upper, const double* b, double* x);
+/* The terms a soft pose prior adds to a keyframe's pose solve at global_T_frame = pose, for the update pose * exp(delta): with
+ * r = log(prior^-1 * pose) and J = Jr^-1(r), the inverse right Jacobian of SE(3), H = J^T L J (upper triangle, 21), b = J^T L r
+ * (6) and cost = r^T L r / 2, all in fp64.  information: L's upper triangle (21).  Writes nothing if a pointer is NULL. */
+void bba_host_pose_prior_terms(const float prior_global_T_frame[7], const float global_T_frame[7], const float information[21],
+                               double H[21], double b[6], double* cost);
 int  bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height,
                                const float global_T_frame_a[7], float min_depth_a, float max_depth_a,
                                const float global_T_frame_b[7], float min_depth_b, float max_depth_b);

@@ -347,6 +347,16 @@ class DirectBA {
   void SetKeyframePose(int keyframe_id, const SE3f& global_T_frame) {
     Check(bba_set_keyframe_pose(h_, keyframe_id, global_T_frame.data()), "bba_set_keyframe_pose");
   }
+  // Soft pose priors (not in the reference; badba.h): anchors keyframe_id to `prior` with the cost 1/2 r^T L r,
+  // r = log(prior^-1 global_T_frame), L given as its upper triangle (translation, then rotation).
+  void SetKeyframePosePrior(int keyframe_id, const SE3f& prior, const float (&information)[21]) {
+    Check(bba_set_keyframe_pose_priors(h_, 1, &keyframe_id, prior.data(), information), "bba_set_keyframe_pose_priors");
+  }
+  // Removes the priors of keyframe_ids, or every prior when the list is empty.
+  void ClearKeyframePosePriors(const std::vector<int>& keyframe_ids = {}) {
+    Check(bba_clear_keyframe_pose_priors(h_, keyframe_ids.empty() ? -1 : static_cast<int>(keyframe_ids.size()), keyframe_ids.data()),
+          "bba_clear_keyframe_pose_priors");
+  }
   uint32_t surfels_size() const { return bba_surfels_size(h_); }   // direct_ba.h:265
   void GetIntrinsics(float depth[4], float color[4], float* a) const { Check(bba_get_intrinsics(h_, depth, color, a), "bba_get_intrinsics"); }
   void SetPCGGaugeKeyframe(int keyframe_id) { pcg_gauge_keyframe_ = keyframe_id; }

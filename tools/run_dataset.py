@@ -26,6 +26,11 @@ surfel map in one call (DirectBA.EstimateFramePosesFromBuffers, bba_estimate_fra
 free slots), starting from its deformed pose; the JSON line then also gives the refined frame-pose error and the seconds the
 refinement took.  That keeps every frame's buffers resident: about 2.5 MB per 640x480 frame.
 
+With --pose-prior-sigma T,R every keyframe gets a soft pose prior at its trajectory pose (DirectBA.SetKeyframePosePriors) with
+the information diag(1/T^2 x3, 1/R^2 x3), T in metres and R in radians, which holds the map in the trajectory's frame.  The JSON
+line always gives the keyframes' absolute error against the trajectory ("max_abs_keyframe_error_m_rad"); with the flag it also
+repeats the run without priors on the same noisy poses and gives that error as "max_abs_keyframe_error_without_priors_m_rad".
+
 The views of --make-synthetic lie metres apart (a BA test scene, not a video), so odometry between them fails and only the
 keyframe poses of that sequence are meaningful; on a recorded sequence every frame is tracked from its neighbour.
 """
@@ -73,12 +78,35 @@ def main():
     ap.add_argument("--refine-frames", action="store_true",
                     help="after the last BA, refine every non-keyframe pose against the final map in one call (needs --export-poses)")
     ap.add_argument("--refine-headroom", type=int, default=64, help="free keyframe slots the handle keeps for --refine-frames")
+    ap.add_argument("--pose-prior-sigma", metavar="T,R", default=None,
+                    help="anchor every keyframe to its trajectory pose with a soft prior of these sigmas (metres, radians)")
     a = ap.parse_args()
     if a.refine_frames and a.export_poses is None:
         ap.error("--refine-frames needs --export-poses")
     if a.make_synthetic:
         make_synthetic(a.make_synthetic)
         return 0
+    if a.pose_prior_sigma is not None:
+        try:
+            a.pose_prior_sigma = [float(x) for x in a.pose_prior_sigma.split(",")]
+            assert len(a.pose_prior_sigma) == 2 and min(a.pose_prior_sigma) > 0
+        except (ValueError, AssertionError):
+            ap.error("--pose-prior-sigma takes two positive numbers T,R")
+        line = run(a, a.pose_prior_sigma)
+        without = run(a, None) if line is not None else None
+        if without is None:
+            return 1
+        line["max_abs_keyframe_error_without_priors_m_rad"] = without["max_abs_keyframe_error_m_rad"]
+    else:
+        line = run(a, None)
+    if line is None:
+        return 1
+    print(json.dumps(line))
+    return 0
+
+
+def run(a, prior_sigma):
+    """One pass over the sequence; returns the JSON line's fields (None if the poses could not be written)."""
     import torch
     from badslam_b200 import rgbd_dataset as D
     from badslam_b200 import scene as S
@@ -131,6 +159,8 @@ def main():
         torch.cuda.synchronize()
         t = time.perf_counter()
         kf = ba.CreateKeyframeFromFrame(i, raw, rgb, noisy, max_depth=a.max_depth, **raw_options)
+        if prior_sigma is not None:
+            ba.SetKeyframePosePriors([kf.id], [pose], np.diag([prior_sigma[0] ** -2] * 3 + [prior_sigma[1] ** -2] * 3))
         created += ba.CreateSurfelsForKeyframe(None, True, kf.id)
         torch.cuda.synchronize()
         t_pre += time.perf_counter() - t
@@ -156,6 +186,10 @@ def main():
             "surfels": ba.surfels_size(), "ba_calls": results, "seconds_preprocess_and_creation": round(t_pre, 3),
             "seconds_bundle_adjustment": round(t_ba, 3),
             "max_relative_pose_error_m_rad": [max(e[0] for e in err), max(e[1] for e in err)] if err else None}
+    abs_err = [S.pose_error(poses[k], true_poses[k]) for k in range(len(idx))]
+    line["max_abs_keyframe_error_m_rad"] = [max(e[0] for e in abs_err), max(e[1] for e in abs_err)]
+    if prior_sigma is not None:
+        line["pose_prior_sigma_m_rad"] = prior_sigma
     if export:
         frame_poses[idx] = poses
         all_true = [f.depth_global_T_frame for f in ds.frames]
@@ -175,9 +209,8 @@ def main():
                          "max_relative_frame_pose_error_refined_m_rad": max_err(frame_poses)})
         if not D.save_poses(a.export_poses, [f.depth_time_string for f in ds.frames], frame_poses):
             print(f"cannot write {a.export_poses}", file=sys.stderr)
-            return 1
-    print(json.dumps(line))
-    return 0
+            return None
+    return line
 
 
 if __name__ == "__main__":
