@@ -300,7 +300,7 @@ struct bba_context {
     bba::DeviceBuffer<float> d_pose_pack;   // [max_kf][kPoseSlot] floats
     bba::PinnedBuffer<float> h_pose_pack;
     bba::DeviceBuffer<int> d_local_ids;     // [max_kf]
-    bba::DeviceBuffer<float> d_count_xchg;  // [2] deleted count of this rank's shard for the sum all-reduce
+    bba::DeviceBuffer<float> d_count_xchg;  // [2] this rank's count for the sum all-reduce (SumOverRanks)
     bba::PinnedBuffer<float> h_count_xchg;
     bba::DeviceBuffer<float> d_barrier;
     // NVLink peer replicas (bba_peer_import)
@@ -486,11 +486,13 @@ bool FramePitchesOk(bba_handle h, size_t depth_pitch, size_t normals_pitch, size
 // Clamp addressing, linear filtering, normalised float reads and unnormalised coordinates (keyframe.cc:67-73, and
 // CUDABuffer::CreateTextureObject as pairwise_frame_tracking.cc:57-79 calls it).
 cudaTextureDesc LinearTextureDesc();
+// The surfel buffer's pitch in floats, as the kernels take it.
+inline uint32_t SurfelPitch(bba_handle h) { return static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)); }
 // The camera, the surfel buffer, its pitch in floats and the surfel count in kernel arguments.
 template <class Args> void SetSurfelFields(bba_handle h, Args* a) {
   a->cam = MakeCamera(h);
   a->surfels = h->surfels;
-  a->pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
+  a->pitch = SurfelPitch(h);
   a->n = h->surfels_size;
 }
 // The luma textures of n >= 1 colour images in device memory (sources[i] -> *out[i]): one extraction launch and one copy per
@@ -517,6 +519,12 @@ bba_status CheckCollective(bba_handle h);
 // Runs the registered exchange (bba_set_collective or a local group) on `buffer`; fails with BBA_ERR_STATE when a local
 // group's exchange did not complete (its group is poisoned).
 bba_status Collective(bba_handle h, int op, void* buffer, size_t count, cudaStream_t s);
+// The sum of every rank's `count` in *total, through one sum all-reduce (a barrier) and a synchronise of s.
+bba_status SumOverRanks(bba_handle h, uint32_t count, cudaStream_t s, uint32_t* total);
+// Whether the kernels store their shard's surfel rows into every rank's replica (bba_peer_import) instead of an exchange.
+bool PeerStores(bba_handle h);
+// The peer replicas kernel arguments get: empty unless PeerStores.
+PeerSet KernelPeers(bba_handle h);
 bba_status PeerFence(bba_handle h, cudaStream_t s);
 bba_status ExchangeShards(bba_handle h, const ShardRows& rows, const uint32_t* perm, cudaStream_t s);
 bba_status ExchangeGeometry(bba_handle h, cudaStream_t s);

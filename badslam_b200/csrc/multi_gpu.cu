@@ -112,6 +112,24 @@ bba_status Collective(bba_handle h, int op, void* buffer, size_t count, cudaStre
   return BBA_OK;
 }
 
+// The count travels as two exactly representable floats (its low 12 bits, the rest), so that the float sum stays exact.
+bba_status SumOverRanks(bba_handle h, uint32_t count, cudaStream_t s, uint32_t* total) {
+  auto& x = h->xchg;
+  BBA_CUDA(h, x.d_count_xchg.Reserve(2));
+  BBA_CUDA(h, x.h_count_xchg.Reserve(2));
+  x.h_count_xchg[0] = static_cast<float>(count & 0xfffu);
+  x.h_count_xchg[1] = static_cast<float>(count >> 12);
+  BBA_CUDA(h, cudaMemcpyAsync(x.d_count_xchg, x.h_count_xchg, sizeof(float) * 2, cudaMemcpyHostToDevice, s));
+  if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, x.d_count_xchg, 2, s)) return st;
+  BBA_CUDA(h, cudaMemcpyAsync(x.h_count_xchg, x.d_count_xchg, sizeof(float) * 2, cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  *total = static_cast<uint32_t>(x.h_count_xchg[0] + 0.5f) + (static_cast<uint32_t>(x.h_count_xchg[1] + 0.5f) << 12);
+  return BBA_OK;
+}
+
+bool PeerStores(bba_handle h) { return h->cfg.world_size > 1 && h->xchg.peers.count == h->cfg.world_size - 1; }
+PeerSet KernelPeers(bba_handle h) { return PeerStores(h) ? h->xchg.peers : PeerSet{}; }
+
 // Every rank has updated `rows` of its own surfel shard only (granules of stream positions, surfel perm[s] at position s; perm
 // null: the caller's order): each rank packs them into its slice of the exchange buffer, one all-gather, and every rank unpacks
 // the other ranks' slices.  The buffer grows to room for kShardRows rows of max_surfel_count surfels (or more).
@@ -123,12 +141,11 @@ bba_status ExchangeShards(bba_handle h, const ShardRows& rows, const uint32_t* p
   ShardSurfels(std::max(h->cfg.max_surfel_count, h->surfels_size), 0, world, nullptr, &max_len);
   const size_t slice_floats = static_cast<size_t>(rows.count + rows.active) * shard_len;
   BBA_CUDA(h, x.d_exchange.Reserve(world * slice_floats, static_cast<size_t>(world) * kShardRows * max_len));
-  const uint32_t pitch = static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float));
-  BBA_LAUNCH(h, h->launches, LaunchPackShard, h->surfels, pitch, h->active, h->surfels_size, rows, perm, rank, world, shard_len,
-             x.d_exchange + slice_floats * rank, s);
+  BBA_LAUNCH(h, h->launches, LaunchPackShard, h->surfels, SurfelPitch(h), h->active, h->surfels_size, rows, perm, rank, world,
+             shard_len, x.d_exchange + slice_floats * rank, s);
   if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLGATHER, x.d_exchange, slice_floats * sizeof(float), s)) return st;
-  BBA_LAUNCH(h, h->launches, LaunchUnpackShards, h->surfels, pitch, h->active, h->surfels_size, rows, perm, shard_len, world, rank,
-             x.d_exchange, s);
+  BBA_LAUNCH(h, h->launches, LaunchUnpackShards, h->surfels, SurfelPitch(h), h->active, h->surfels_size, rows, perm, shard_len,
+             world, rank, x.d_exchange, s);
   return BBA_OK;
 }
 
@@ -136,7 +153,7 @@ bba_status ExchangeShards(bba_handle h, const ShardRows& rows, const uint32_t* p
 bba_status ExchangeGeometry(bba_handle h, cudaStream_t s) {
   if (h->cfg.world_size <= 1 || h->surfels_size == 0) return BBA_OK;
   // the geometry kernels already stored the updated rows into every replica over NVLink: only a barrier is left
-  if (h->xchg.peers.count == h->cfg.world_size - 1) return Barrier(h, s);
+  if (PeerStores(h)) return Barrier(h, s);
   return ExchangeShards(h, ShardRows{{kRowX, kRowY, kRowZ, kRowNormal, kRowD1, kRowD2}, 6, 1}, h->geo.perm, s);
 }
 
@@ -145,7 +162,7 @@ bba_status ExchangeGeometry(bba_handle h, cudaStream_t s) {
 bba_status PeerFence(bba_handle h, cudaStream_t s) {
   if (h->cfg.world_size <= 1 || !h->xchg.replicated_pass_pending) return BBA_OK;
   h->xchg.replicated_pass_pending = false;
-  if (h->xchg.peers.count != h->cfg.world_size - 1) return BBA_OK;   // exchange through the host's collective: no remote stores
+  if (!PeerStores(h)) return BBA_OK;   // exchange through the host's collective: no remote stores
   if (bba_status st = CheckCollective(h)) return st;
   return Barrier(h, s);
 }

@@ -32,8 +32,7 @@ bba_status EnsureSpatialOrder(bba_handle h, bool sort, bool rebuild, cudaStream_
     p.order.capacity = cap;
   }
   if (sort && (rebuild || p.order_stale || p.order_n != n)) {
-    BBA_LAUNCH(h, h->launches, LaunchSpatialOrder, h->surfels, static_cast<uint32_t>(h->surfel_pitch_bytes / sizeof(float)), n,
-               p.order.view, s);
+    BBA_LAUNCH(h, h->launches, LaunchSpatialOrder, h->surfels, SurfelPitch(h), n, p.order.view, s);
     p.order_n = n;
     p.order_stale = false;
   }
