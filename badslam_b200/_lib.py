@@ -88,6 +88,10 @@ class MotionModelRecord(C.Structure):
     _fields_ = [("count", C.c_int), ("base_kf_tr_frame", (C.c_float * 7) * 3), ("frame_tr_base_kf", (C.c_float * 7) * 3)]
 
 
+class PoseConstraint(C.Structure):   # bba_pose_constraint
+    _fields_ = [("keyframe_a", C.c_int), ("keyframe_b", C.c_int), ("a_T_b", C.c_float * 7), ("information", C.c_float * 21)]
+
+
 class PeerHandle(C.Structure):
     _fields_ = [("surfels_ipc", C.c_ubyte * 64), ("surfels_offset", C.c_uint64), ("active_ipc", C.c_ubyte * 64),
                 ("active_offset", C.c_uint64), ("pitch_bytes", C.c_uint64), ("surfels_size", C.c_uint32), ("rank", C.c_int32)]
@@ -152,6 +156,9 @@ SYMBOLS = {
     "bba_set_keyframe_pose_priors": (C.c_int, [_P, C.c_int, _P, _P, _P]),
     "bba_clear_keyframe_pose_priors": (C.c_int, [_P, C.c_int, _P]),
     "bba_get_keyframe_pose_prior": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
+    "bba_add_keyframe_pose_constraints": (C.c_int, [_P, C.c_int, _P, _P]),
+    "bba_remove_keyframe_pose_constraints": (C.c_int, [_P, C.c_int, _P]),
+    "bba_get_keyframe_pose_constraints": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
     "bba_set_intrinsics": (C.c_int, [_P, _F7, _F7, C.c_float]),
     "bba_get_intrinsics": (C.c_int, [_P, _F7, _F7, C.POINTER(C.c_float)]),
     "bba_host_se3_exp": (None, [_P, _P]),
@@ -161,6 +168,7 @@ SYMBOLS = {
     "bba_host_pose_update_converged": (C.c_int, [_P]),
     "bba_host_solve_ldlt": (C.c_int, [C.c_int, _P, _P, _P]),
     "bba_host_pose_prior_terms": (None, [_P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
+    "bba_host_pose_constraint_terms": (None, [_P, _P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_frusta_intersect": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, C.c_float, _P, C.c_float, C.c_float]),
     "bba_host_motion_model_clear": (None, [C.POINTER(MotionModelRecord), _P, _P]),
     "bba_host_motion_model_predict": (C.c_int, [C.POINTER(MotionModelRecord), C.c_int, _P, _P]),

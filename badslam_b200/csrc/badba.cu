@@ -107,9 +107,11 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
     v.prior = h->pose_priors[k];
   }
   const CameraView cams = LiveCameraView(h);
+  std::vector<PoseConstraint> constraints = h->pose_constraints;
   std::lock_guard<std::mutex> lock(f.mu);
   f.cams = cams;
   f.kfs.swap(kfs);
+  f.constraints.swap(constraints);
   if (cfactor) f.current = next;
   return BBA_OK;
 }
@@ -351,8 +353,6 @@ bba_status bba_create(const bba_config* cfg, bba_handle* out) {
   CREATE_TRY(h->d_cfactor.Reserve(static_cast<size_t>(h->cf_w) * h->cf_h));
   CREATE_TRY(cudaMemset(h->d_cfactor, 0, sizeof(float) * h->cf_w * h->cf_h));
   CREATE_TRY(h->d_kfs.Reserve(K));
-  CREATE_TRY(h->d_pose_priors.Reserve(K));
-  CREATE_TRY(cudaMemset(h->d_pose_priors, 0, sizeof(bba::PosePrior) * K));
   h->pose_priors.assign(K, bba::PosePrior{});
   CREATE_TRY(p.d_work_records.Reserve(K));
   CREATE_TRY(p.d_pose_est.Reserve(7 * K));
@@ -572,6 +572,12 @@ int bba_host_solve_ldlt(int n, const double* upper, const double* b, double* x) 
 void bba_host_pose_prior_terms(const float prior[7], const float pose[7], const float info[21], double H[21], double b[6], double* cost) {
   if (!prior || !pose || !info || !H || !b || !cost) return;
   bba::PosePriorTerms(prior, pose, info, H, b, cost);
+}
+void bba_host_pose_constraint_terms(const float a_T_b[7], const float pose_a[7], const float pose_b[7], const float info[21], double H[78],
+                                    double b[12], double* cost) {
+  if (!a_T_b || !pose_a || !pose_b || !info || !H || !b || !cost) return;
+  double r[6];
+  bba::PoseConstraintTerms(a_T_b, pose_a, pose_b, info, r, H, b, cost);
 }
 int bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height, const float global_T_frame_a[7], float min_depth_a,
                               float max_depth_a, const float global_T_frame_b[7], float min_depth_b, float max_depth_b) {
@@ -816,13 +822,19 @@ bool InformationPsd(const float info[21]) {
   return true;
 }
 
-// Uploads the prior table for the pose solve and publishes the records.
+// Counts the priors and publishes the records.
 bba_status CommitPosePriors(bba_handle h) {
   int count = 0;
   for (const PosePrior& p : h->pose_priors) count += p.has ? 1 : 0;
   h->pose_prior_count = count;
-  BBA_CUDA(h, cudaMemcpy(h->d_pose_priors, h->pose_priors.data(), sizeof(PosePrior) * h->pose_priors.size(), cudaMemcpyHostToDevice));
   return Publish(h, nullptr, false);
+}
+
+bool PoseRecordFinite(const float* pose, const float* info) {
+  bool finite = true;
+  for (int j = 0; j < 7; ++j) finite = finite && std::isfinite(pose[j]);
+  for (int j = 0; j < 21; ++j) finite = finite && std::isfinite(info[j]);
+  return finite;
 }
 }  // namespace
 
@@ -836,13 +848,12 @@ bba_status bba_set_keyframe_pose_priors(bba_handle h, int count, const int* ids,
     if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
     const float* p = poses + 7 * static_cast<size_t>(i);
     const float* info = information + 21 * static_cast<size_t>(i);
-    bool finite = true;
-    for (int j = 0; j < 7; ++j) finite = finite && std::isfinite(p[j]);
-    for (int j = 0; j < 21; ++j) finite = finite && std::isfinite(info[j]);
-    if (!finite) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose or information");
+    if (!PoseRecordFinite(p, info)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose or information");
     if (p[0] * p[0] + p[1] * p[1] + p[2] * p[2] + p[3] * p[3] < 1e-12f) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "zero quaternion");
     if (!InformationPsd(info)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information matrix is not positive semi-definite");
   }
+  if (count > 0)
+    if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size())) return st;
   for (int i = 0; i < count; ++i) {
     PosePrior& r = h->pose_priors[ids[i]];
     std::memcpy(r.pose, poses + 7 * static_cast<size_t>(i), sizeof(r.pose));
@@ -880,6 +891,77 @@ bba_status bba_get_keyframe_pose_prior(bba_handle h, int id, float pose[7], floa
   *has_prior = p.has;
   if (pose) std::memcpy(pose, p.pose, sizeof(p.pose));
   if (information) std::memcpy(information, p.info, sizeof(p.info));
+  return BBA_OK;
+}
+
+// ---- soft relative pose constraints ----
+bba_status bba_add_keyframe_pose_constraints(bba_handle h, int count, const bba_pose_constraint* constraints, int* out_ids) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_add_keyframe_pose_constraints: ";
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
+  if (count > 0 && !constraints) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  const int K = static_cast<int>(h->keyframes.size());
+  for (int i = 0; i < count; ++i) {
+    const bba_pose_constraint& c = constraints[i];
+    if (c.keyframe_a < 0 || c.keyframe_a >= K || c.keyframe_b < 0 || c.keyframe_b >= K)
+      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
+    if (c.keyframe_a == c.keyframe_b) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "keyframe_a == keyframe_b");
+    if (!PoseRecordFinite(c.a_T_b, c.information)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose or information");
+    const float* q = c.a_T_b;
+    if (q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] < 1e-12f) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "zero quaternion");
+    if (!InformationPsd(c.information)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information matrix is not positive semi-definite");
+  }
+  if (count == 0) return BBA_OK;
+  if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size() + count)) return st;
+  for (int i = 0; i < count; ++i) {
+    PoseConstraint r{};
+    r.id = h->next_pose_constraint_id++;
+    r.c = constraints[i];
+    double info_a[21];
+    PoseConstraintInformationA(r.c.a_T_b, r.c.information, info_a);
+    for (int j = 0; j < 21; ++j) r.info_a[j] = static_cast<float>(info_a[j]);
+    h->pose_constraints.push_back(r);
+    if (out_ids) out_ids[i] = r.id;
+  }
+  return Publish(h, nullptr, false);
+}
+
+bba_status bba_remove_keyframe_pose_constraints(bba_handle h, int count, const int* ids) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_remove_keyframe_pose_constraints: ";
+  auto& cons = h->pose_constraints;
+  if (count == -1) {
+    cons.clear();
+    return Publish(h, nullptr, false);
+  }
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < -1");
+  if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  std::vector<char> drop(cons.size(), 0);
+  for (int i = 0; i < count; ++i) {
+    // ids increase along the list
+    auto it = std::lower_bound(cons.begin(), cons.end(), ids[i], [](const PoseConstraint& c, int id) { return c.id < id; });
+    if (it == cons.end() || it->id != ids[i]) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown constraint id");
+    drop[it - cons.begin()] = 1;
+  }
+  size_t n = 0;
+  for (size_t i = 0; i < cons.size(); ++i)
+    if (!drop[i]) cons[n++] = cons[i];
+  cons.resize(n);
+  return Publish(h, nullptr, false);
+}
+
+bba_status bba_get_keyframe_pose_constraints(bba_handle h, int capacity, int* ids, bba_pose_constraint* out, int* count) {
+  FrontEndScope front_end;
+  if (!h || !count) return BBA_ERR_INVALID_ARGUMENT;
+  if (capacity < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_get_keyframe_pose_constraints: capacity < 0");
+  std::lock_guard<std::mutex> lock(h->fe.mu);
+  const std::vector<PoseConstraint>& cons = h->fe.constraints;
+  *count = static_cast<int>(cons.size());
+  const int n = std::min(capacity, *count);
+  for (int i = 0; i < n; ++i) {
+    if (ids) ids[i] = cons[i].id;
+    if (out) out[i] = cons[i].c;
+  }
   return BBA_OK;
 }
 

@@ -526,30 +526,72 @@ bba::PcgArgs MakePcgArgs(bba_handle h, const PcgLayout& L, int gauge) {
   return a;
 }
 
-// The soft pose priors' terms of the pose unknowns (every keyframe with a prior but the gauge) at the poses the init pass sees,
-// staged for LaunchPcgPosePrior.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.
-bba_status StagePcgPriors(bba_handle h, const PcgLayout& L, int gauge, cudaStream_t s) {
+// The pose-block terms of the products at the poses the init pass sees, staged for LaunchPcgPoseTerms: a keyframe's prior and,
+// per constraint, H_aa / H_bb, H_ab and b_a / b_b of PoseConstraintTerms, gathered per pose block (every keyframe but the
+// gauge) in the order prior, then constraints by id.  An edge to the gauge keeps only its other end's diagonal terms (p_gauge = 0).
+// fp64, rounded to fp32.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.
+bba_status StagePcgPoseTerms(bba_handle h, const PcgLayout& L, int gauge, cudaStream_t s) {
   auto& pc = h->pcg;
-  pc.prior_terms = 0;
-  if (!L.opt_poses || h->pose_prior_count == 0 || h->cfg.rank != 0) return BBA_OK;
+  pc.pose_blocks = 0;
+  if (!L.opt_poses || (h->pose_prior_count == 0 && h->pose_constraints.empty()) || h->cfg.rank != 0) return BBA_OK;
   const int K = static_cast<int>(h->keyframes.size());
-  BBA_CUDA(h, pc.h_prior_terms.Reserve(h->cfg.max_keyframes));
-  BBA_CUDA(h, pc.d_prior_terms.Reserve(h->cfg.max_keyframes));
-  int n = 0;
-  for (int k = 0; k < K; ++k) {
-    const PosePrior& prior = h->pose_priors[k];
-    if (k == gauge || !prior.has) continue;
-    bba::PcgPriorTerm& t = pc.h_prior_terms[n++];
-    t.u = 6u * static_cast<uint32_t>(k < gauge ? k : k - 1);
-    float pose[7];
-    PoseToArray(h->keyframes[k].pose, pose);
-    double H[21], b[6], cost;
-    bba::PosePriorTerms(prior.pose, pose, prior.info, H, b, &cost);
-    for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(H[j]);
-    for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(b[j]);
+  const size_t C = h->pose_constraints.size();
+  if (bba_status st = ReservePoseTerms(h, C)) return st;
+  auto unknown = [&](int k) { return k == gauge ? -1 : 6 * (k < gauge ? k : k - 1); };
+  std::vector<float> poses(7 * static_cast<size_t>(K));
+  for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses.data() + 7 * k);
+  // every constraint's terms at the current poses: [a's term, b's term]
+  std::vector<bba::PcgPoseTerm> edge(2 * C);
+  for (size_t i = 0; i < C; ++i) {
+    const bba_pose_constraint& c = h->pose_constraints[i].c;
+    double r[6], H[78], b[12], cost;
+    PoseConstraintTerms(c.a_T_b, poses.data() + 7 * c.keyframe_a, poses.data() + 7 * c.keyframe_b, c.information, r, H, b, &cost);
+    auto upper = [&](int row, int col) { return H[row * 12 - row * (row - 1) / 2 + (col - row)]; };
+    bba::PcgPoseTerm& ta = edge[2 * i];
+    bba::PcgPoseTerm& tb = edge[2 * i + 1];
+    ta.other = unknown(c.keyframe_b);
+    tb.other = unknown(c.keyframe_a);
+    int idx = 0;
+    for (int row = 0; row < 6; ++row) {
+      ta.b[row] = static_cast<float>(b[row]);
+      tb.b[row] = static_cast<float>(b[6 + row]);
+      for (int col = row; col < 6; ++col, ++idx) {
+        ta.H[idx] = static_cast<float>(upper(row, col));
+        tb.H[idx] = static_cast<float>(upper(6 + row, 6 + col));
+      }
+      for (int col = 0; col < 6; ++col) {
+        const float x = static_cast<float>(upper(row, 6 + col));   // H_ab[row][col]
+        ta.X[row * 6 + col] = x;
+        tb.X[col * 6 + row] = x;                                  // H_ba = H_ab^T
+      }
+    }
   }
-  if (n) BBA_CUDA(h, cudaMemcpyAsync(pc.d_prior_terms, pc.h_prior_terms, sizeof(bba::PcgPriorTerm) * n, cudaMemcpyHostToDevice, s));
-  pc.prior_terms = n;
+  std::vector<int> off, adj;
+  ConstraintAdjacency(h, K, &off, &adj);
+  int nb = 0, nt = 0;
+  for (int k = 0; k < K; ++k) {
+    if (k == gauge) continue;
+    const int begin = nt;
+    const PosePrior& prior = h->pose_priors[k];
+    if (prior.has) {
+      bba::PcgPoseTerm& t = pc.h_pose_terms[nt++];
+      t.other = -1;
+      double H[21], b[6], cost;
+      bba::PosePriorTerms(prior.pose, poses.data() + 7 * k, prior.info, H, b, &cost);
+      for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(H[j]);
+      for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(b[j]);
+    }
+    for (int e = off[k]; e < off[k + 1]; ++e) {
+      const int i = adj[e];
+      pc.h_pose_terms[nt++] = edge[2 * i + (h->pose_constraints[i].c.keyframe_a == k ? 0 : 1)];
+    }
+    if (nt > begin) pc.h_pose_blocks[nb++] = bba::PcgPoseBlock{static_cast<uint32_t>(unknown(k)), begin, nt};
+  }
+  if (nb) {
+    BBA_CUDA(h, cudaMemcpyAsync(pc.d_pose_blocks, pc.h_pose_blocks, sizeof(bba::PcgPoseBlock) * nb, cudaMemcpyHostToDevice, s));
+    BBA_CUDA(h, cudaMemcpyAsync(pc.d_pose_terms, pc.h_pose_terms, sizeof(bba::PcgPoseTerm) * nt, cudaMemcpyHostToDevice, s));
+  }
+  pc.pose_blocks = nb;
   return BBA_OK;
 }
 
@@ -562,8 +604,9 @@ bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int 
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_vec[1], 0, sizeof(float) * U, s));
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars, 0, sizeof(double) * 4, s));
   BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
-  if (bba_status st = StagePcgPriors(h, L, a.gauge_kf, s)) return st;
-  BBA_LAUNCH(h, h->launches, LaunchPcgPosePrior, h->pcg.d_prior_terms, h->pcg.prior_terms, true, a.r, a.M, nullptr, nullptr, nullptr, s);
+  if (bba_status st = StagePcgPoseTerms(h, L, a.gauge_kf, s)) return st;
+  BBA_LAUNCH(h, h->launches, LaunchPcgPoseTerms, h->pcg.d_pose_blocks, h->pcg.pose_blocks, h->pcg.d_pose_terms, true, a.r, a.M, nullptr,
+             nullptr, nullptr, s);
   if (h->cfg.world_size > 1) {
     if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[0], U, s)) return st;
     if (bba_status st = Collective(h, BBA_COLLECTIVE_ALLREDUCE_SUM, h->pcg.d_vec[1], U, s)) return st;
@@ -577,8 +620,8 @@ bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int 
 // Inner step, first half: g += J^T W J p and alpha_d += p^T J^T W J p over every keyframe (PCGStep1CUDA, :392-419).
 bba_status PcgStep1(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, cudaStream_t s) {
   BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, false, s);
-  BBA_LAUNCH(h, h->launches, LaunchPcgPosePrior, h->pcg.d_prior_terms, h->pcg.prior_terms, false, nullptr, nullptr, a.p, a.g,
-             a.scalars + a.alpha_d_slot, s);
+  BBA_LAUNCH(h, h->launches, LaunchPcgPoseTerms, h->pcg.d_pose_blocks, h->pcg.pose_blocks, h->pcg.d_pose_terms, false, nullptr, nullptr,
+             a.p, a.g, a.scalars + a.alpha_d_slot, s);
   if (h->cfg.world_size > 1) {   // g and this rank's part of alpha_d: one all-reduce
     float* g = h->pcg.d_vec[3];
     BBA_LAUNCH(h, h->launches, LaunchPcgPackAlphaD, h->pcg.d_scalars, g + L.unknown_count, s);

@@ -142,6 +142,14 @@ struct KeyframeView {
   PosePrior prior{};
 };
 
+// A soft relative pose constraint as the handle keeps it: its id, the caller's record, and the information of the equivalent
+// prior on keyframe_a (host_math.hpp PoseConstraintInformationA).
+struct PoseConstraint {
+  int id;
+  bba_pose_constraint c;
+  float info_a[21];
+};
+
 // The cameras, the depth deformation parameter a, the residual types and the deterministic mode as the BA side published them last.
 struct CameraView {
   float depth_K[4] = {}, color_K[4] = {};
@@ -184,11 +192,13 @@ struct bba_context {
   bba::DeviceBuffer<float> d_cfactor;
   std::vector<bba::Keyframe> keyframes;
   bba::DeviceBuffer<bba::KfDevice> d_kfs;   // [max_kf] the keyframes' parameters as the kernels read them
-  // soft pose priors by keyframe id (bba_set_keyframe_pose_priors): the host records, their device copy that the pose solve
-  // reads, and how many keyframes have one (0: the pose solve and the PCG solver run without the table)
+  // soft pose priors by keyframe id (bba_set_keyframe_pose_priors) and how many keyframes have one; with no prior and no
+  // constraint the pose solve and the PCG solver run without pose terms
   std::vector<bba::PosePrior> pose_priors;   // [max_kf]
-  bba::DeviceBuffer<bba::PosePrior> d_pose_priors;
   int pose_prior_count = 0;
+  // soft relative pose constraints (bba_add_keyframe_pose_constraints) in id order, and the id the next one gets
+  std::vector<bba::PoseConstraint> pose_constraints;
+  int next_pose_constraint_id = 0;
 
   // staging: pinned records and the shared planes of the keyframe / frame uploads
   struct Staging {
@@ -226,6 +236,12 @@ struct bba_context {
     bba::PinnedBuffer<int> h_converged;
     bba::PinnedBuffer<double> h_first_stats;
     bba::PinnedBuffer<unsigned long long> h_totals;
+    // the soft pose terms of the keyframes in the step (StagePoseTerms): CSR offsets [max_kf + 1] and records, staged at the
+    // start of every pose step; reserved by the calls that add priors or constraints
+    bba::PinnedBuffer<int> h_term_offsets;
+    bba::DeviceBuffer<int> d_term_offsets;
+    bba::PinnedBuffer<bba::PoseTerm> h_terms;
+    bba::DeviceBuffer<bba::PoseTerm> d_terms;
     // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream); the
     // geometry step's stream (bba::LaunchGeometryStream) shares the buffer.
     // The order is rebuilt at the start of every BA call, after an in-loop change of the surfel set, and whenever the surfel
@@ -282,10 +298,12 @@ struct bba_context {
     bba::DeviceBuffer<double> d_scalars;   // [0] / [2] alpha_n, beta_n (roles swap), [1] alpha_d
     bba::PinnedBuffer<double> h_scalars;
     bba::PinnedBuffer<float> h_delta;      // pose part (6 * max_keyframes) + 16
-    // the soft pose priors' terms at the poses of the current outer iteration (StagePcgPriors)
-    bba::PinnedBuffer<bba::PcgPriorTerm> h_prior_terms;
-    bba::DeviceBuffer<bba::PcgPriorTerm> d_prior_terms;
-    int prior_terms = 0;
+    // the pose-block terms (priors, constraints) at the poses of the current outer iteration (StagePcgPoseTerms)
+    bba::PinnedBuffer<bba::PcgPoseBlock> h_pose_blocks;
+    bba::DeviceBuffer<bba::PcgPoseBlock> d_pose_blocks;
+    bba::PinnedBuffer<bba::PcgPoseTerm> h_pose_terms;
+    bba::DeviceBuffer<bba::PcgPoseTerm> d_pose_terms;
+    int pose_blocks = 0;
   } pcg;
 
   // multi-GPU exchange (multi_gpu.cu)
@@ -357,6 +375,7 @@ struct bba_context {
     std::condition_variable slot_free;   // a cfactor slot lost its last reader
     bba::CameraView cams;
     std::vector<bba::KeyframeView> kfs;
+    std::vector<bba::PoseConstraint> constraints;   // the soft relative pose constraints, in id order
     // Two device copies of the cfactor.  Publish copies d_cfactor into the slot that is not current, on the BA side's stream,
     // after that slot's readers are done, records `published` and makes the slot current; a front-end call claims the
     // current slot, makes its stream wait on `published` and records `readers_done` after its last read.
@@ -510,6 +529,13 @@ bba_status MakeFrameLumaTextures(bba_handle h, bool front_end, const bba_frame_b
 constexpr uint64_t kSpatialOrderMinPairs = 16u << 20;   // (surfel, keyframe) pairs per launch
 bba_status EnsureSpatialOrder(bba_handle h, bool sort, bool rebuild, cudaStream_t s);
 bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, int max_iterations, cudaStream_t s);
+// Reserves the staging buffers of the soft pose terms (pose step and PCG) for a prior on every keyframe and `constraints`
+// constraints, with room to double the constraints before the next allocation.  The calls that add priors or constraints make
+// it before they change anything; the staging repeats it, a no-op unless an earlier reservation failed.
+bba_status ReservePoseTerms(bba_handle h, size_t constraints);
+// The soft relative pose constraints that touch each of the first K keyframes, in id order: indices into
+// h->pose_constraints, adj[off[k] .. off[k + 1]).
+void ConstraintAdjacency(bba_handle h, int K, std::vector<int>* off, std::vector<int>* adj);
 
 // multi_gpu.cu
 void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t* shard_len);

@@ -291,36 +291,68 @@ BBA_HD void So3LeftJacobianInverse(const double w[3], double theta, double A[9])
   A[0] += 1.0; A[4] += 1.0; A[8] += 1.0;
 }
 
-// r = log(P^-1 T) in the tangent order (translation, rotation), fp64, the rotation angle in [0, pi].  The quaternions are
-// normalised first.
-BBA_HD void PosePriorResidual(const float prior[7], const float pose[7], double r[6], double* theta_out) {
-  double qp[4], qt[4];
-  double np = 0.0, nt = 0.0;
+// A pose in fp64 with its quaternion normalised: q (x, y, z, w) and t.
+BBA_HD void LoadPoseD(const float p[7], double q[4], double t[3]) {
+  double n = 0.0;
   for (int i = 0; i < 4; ++i) {
-    qp[i] = prior[i];
-    qt[i] = pose[i];
-    np += qp[i] * qp[i];
-    nt += qt[i] * qt[i];
+    q[i] = p[i];
+    n += q[i] * q[i];
   }
-  np = 1.0 / sqrt(np);
-  nt = 1.0 / sqrt(nt);
-  for (int i = 0; i < 4; ++i) {
-    qp[i] *= np;
-    qt[i] *= nt;
-  }
-  // q = conj(qp) * qt,  t = R(qp)^T (t_T - t_P)
+  n = 1.0 / sqrt(n);
+  for (int i = 0; i < 4; ++i) q[i] *= n;
+  for (int i = 0; i < 3; ++i) t[i] = p[4 + i];
+}
+
+// P^-1 T of two poses in fp64: q = conj(qp) * qt, t = R(qp)^T (t_T - t_P).
+BBA_HD void Se3BetweenD(const double qp[4], const double tp[3], const double qt[4], const double tt[3], double q[4], double t[3]) {
   const double ax = -qp[0], ay = -qp[1], az = -qp[2], aw = qp[3];
   const double bx = qt[0], by = qt[1], bz = qt[2], bw = qt[3];
-  double q[4];
   q[3] = aw * bw - ax * bx - ay * by - az * bz;
   q[0] = aw * bx + ax * bw + ay * bz - az * by;
   q[1] = aw * by + ay * bw + az * bx - ax * bz;
   q[2] = aw * bz + az * bw + ax * by - ay * bx;
-  const double d[3] = {static_cast<double>(pose[4]) - prior[4], static_cast<double>(pose[5]) - prior[5],
-                       static_cast<double>(pose[6]) - prior[6]};
+  const double d[3] = {tt[0] - tp[0], tt[1] - tp[1], tt[2] - tp[2]};
   // rotate d by conj(qp): v + w u + v x u with u = 2 (qv x d), qv = -qp.xyz
   const double ux = 2.0 * (ay * d[2] - az * d[1]), uy = 2.0 * (az * d[0] - ax * d[2]), uz = 2.0 * (ax * d[1] - ay * d[0]);
-  const double t[3] = {d[0] + aw * ux + (ay * uz - az * uy), d[1] + aw * uy + (az * ux - ax * uz), d[2] + aw * uz + (ax * uy - ay * ux)};
+  t[0] = d[0] + aw * ux + (ay * uz - az * uy);
+  t[1] = d[1] + aw * uy + (az * ux - ax * uz);
+  t[2] = d[2] + aw * uz + (ax * uy - ay * ux);
+}
+
+// A * B of two poses in fp64: q = qa * qb, t = R(qa) t_B + t_A.
+BBA_HD void Se3ComposeD(const double qa[4], const double ta[3], const double qb[4], const double tb[3], double q[4], double t[3]) {
+  const double ax = qa[0], ay = qa[1], az = qa[2], aw = qa[3];
+  q[3] = aw * qb[3] - ax * qb[0] - ay * qb[1] - az * qb[2];
+  q[0] = aw * qb[0] + ax * qb[3] + ay * qb[2] - az * qb[1];
+  q[1] = aw * qb[1] + ay * qb[3] + az * qb[0] - ax * qb[2];
+  q[2] = aw * qb[2] + az * qb[3] + ax * qb[1] - ay * qb[0];
+  const double ux = 2.0 * (ay * tb[2] - az * tb[1]), uy = 2.0 * (az * tb[0] - ax * tb[2]), uz = 2.0 * (ax * tb[1] - ay * tb[0]);
+  t[0] = ta[0] + tb[0] + aw * ux + (ay * uz - az * uy);
+  t[1] = ta[1] + tb[1] + aw * uy + (az * ux - ax * uz);
+  t[2] = ta[2] + tb[2] + aw * uz + (ax * uy - ay * ux);
+}
+
+// Ad(T) of a pose in the tangent order (translation, rotation): [[R, [t]x R], [0, R]], so that T exp(x) T^-1 = exp(Ad(T) x).
+BBA_HD void Se3AdjointD(const double q[4], const double t[3], double Ad[36]) {
+  const double x = q[0], y = q[1], z = q[2], w = q[3];
+  const double R[9] = {1.0 - 2.0 * (y * y + z * z), 2.0 * (x * y - z * w), 2.0 * (x * z + y * w),
+                       2.0 * (x * y + z * w), 1.0 - 2.0 * (x * x + z * z), 2.0 * (y * z - x * w),
+                       2.0 * (x * z - y * w), 2.0 * (y * z + x * w), 1.0 - 2.0 * (x * x + y * y)};
+  double T[9], TR[9];
+  HatD(t, T);
+  Mat3MulD(T, R, TR);
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      Ad[i * 6 + j] = R[i * 3 + j];
+      Ad[i * 6 + 3 + j] = TR[i * 3 + j];
+      Ad[(3 + i) * 6 + j] = 0.0;
+      Ad[(3 + i) * 6 + 3 + j] = R[i * 3 + j];
+    }
+}
+
+// log of a pose with a unit quaternion, in the tangent order (translation, rotation), fp64, the rotation angle in [0, pi].
+BBA_HD void Se3LogD(const double q_in[4], const double t[3], double r[6], double* theta_out) {
+  double q[4] = {q_in[0], q_in[1], q_in[2], q_in[3]};
   if (q[3] < 0.0)
     for (int i = 0; i < 4; ++i) q[i] = -q[i];
   const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
@@ -334,6 +366,16 @@ BBA_HD void PosePriorResidual(const float prior[7], const float pose[7], double 
     r[3 + i] = w[i];
   }
   *theta_out = theta;
+}
+
+// r = log(P^-1 T) in the tangent order (translation, rotation), fp64, the rotation angle in [0, pi].  The quaternions are
+// normalised first.
+BBA_HD void PosePriorResidual(const float prior[7], const float pose[7], double r[6], double* theta_out) {
+  double qp[4], tp[3], qt[4], tt[3], q[4], t[3];
+  LoadPoseD(prior, qp, tp);
+  LoadPoseD(pose, qt, tt);
+  Se3BetweenD(qp, tp, qt, tt, q, t);
+  Se3LogD(q, t, r, theta_out);
 }
 
 // J = Jr^-1(r), the inverse right Jacobian of SE(3) in the tangent order (rho, phi): d log(exp(r) exp(delta)) / d delta at 0.
@@ -380,42 +422,102 @@ BBA_HD void Se3RightJacobianInverse(const double r[6], double theta, double J[36
     }
 }
 
-// The prior's terms at global_T_frame = pose, for an update pose <- pose * exp(delta): with r = log(P^-1 pose) and J = Jr^-1(r),
-// H = J^T L J (upper triangle, 21), b = J^T L r (6), cost = r^T L r / 2.  fp64 throughout.
-BBA_HD void PosePriorTerms(const float prior[7], const float pose[7], const float info[21], double H[21], double b[6], double* cost) {
-  double r[6], theta, J[36], L[36];
-  PosePriorResidual(prior, pose, r, &theta);
-  Se3RightJacobianInverse(r, theta, J);
+// The terms of 1/2 r^T L r with the 6 x N Jacobian J (row-major): H = J^T L J (upper triangle, N (N + 1) / 2), b = J^T L r (N),
+// cost = r^T L r / 2.  info: L's upper triangle (21).  fp64 throughout.
+template <int N>
+BBA_HD void InformationTerms(const double r[6], const double* J, const float info[21], double* H, double* b, double* cost) {
+  double L[36];
   int idx = 0;
   for (int i = 0; i < 6; ++i)
     for (int j = i; j < 6; ++j) {
       L[i * 6 + j] = L[j * 6 + i] = info[idx];
       ++idx;
     }
-  double LJ[36], Lr[6];
+  double LJ[6 * N], Lr[6];
   for (int i = 0; i < 6; ++i) {
     Lr[i] = 0.0;
     for (int k = 0; k < 6; ++k) Lr[i] += L[i * 6 + k] * r[k];
-    for (int j = 0; j < 6; ++j) {
+    for (int j = 0; j < N; ++j) {
       double s = 0.0;
-      for (int k = 0; k < 6; ++k) s += L[i * 6 + k] * J[k * 6 + j];
-      LJ[i * 6 + j] = s;
+      for (int k = 0; k < 6; ++k) s += L[i * 6 + k] * J[k * N + j];
+      LJ[i * N + j] = s;
     }
   }
   idx = 0;
   double c = 0.0;
-  for (int i = 0; i < 6; ++i) {
+  for (int i = 0; i < N; ++i) {
     double s = 0.0;
-    for (int k = 0; k < 6; ++k) s += J[k * 6 + i] * Lr[k];
+    for (int k = 0; k < 6; ++k) s += J[k * N + i] * Lr[k];
     b[i] = s;
-    c += r[i] * Lr[i];
-    for (int j = i; j < 6; ++j) {
+    if (i < 6) c += r[i] * Lr[i];
+    for (int j = i; j < N; ++j) {
       double h = 0.0;
-      for (int k = 0; k < 6; ++k) h += J[k * 6 + i] * LJ[k * 6 + j];
+      for (int k = 0; k < 6; ++k) h += J[k * N + i] * LJ[k * N + j];
       H[idx++] = h;
     }
   }
   *cost = 0.5 * c;
+}
+
+// The prior's terms at global_T_frame = pose, for an update pose <- pose * exp(delta): with r = log(P^-1 pose) and J = Jr^-1(r),
+// H = J^T L J (upper triangle, 21), b = J^T L r (6), cost = r^T L r / 2.  fp64 throughout.
+BBA_HD void PosePriorTerms(const float prior[7], const float pose[7], const float info[21], double H[21], double b[6], double* cost) {
+  double r[6], theta, J[36];
+  PosePriorResidual(prior, pose, r, &theta);
+  Se3RightJacobianInverse(r, theta, J);
+  InformationTerms<6>(r, J, info, H, b, cost);
+}
+
+// ---- soft relative pose constraint between two keyframes (bba_add_keyframe_pose_constraints) ----
+// The constraint's terms at global_T_frame = pose_a, pose_b, for the updates pose_a * exp(delta_a), pose_b * exp(delta_b): with
+// r = log(Z^-1 pose_a^-1 pose_b), Z = a_T_b, J_b = Jr^-1(r) and J_a = -Jr^-1(r) Ad(pose_b^-1 pose_a), and J = [J_a | J_b]:
+// H = J^T L J over (delta_a, delta_b) (12 x 12 upper triangle, 78), b = J^T L r (12), cost = r^T L r / 2.  fp64 throughout.
+BBA_HD void PoseConstraintTerms(const float a_T_b[7], const float pose_a[7], const float pose_b[7], const float info[21], double r[6],
+                                double H[78], double b[12], double* cost) {
+  double qz[4], tz[3], qa[4], ta[3], qb[4], tb[3], qe[4], te[3], qx[4], tx[3];
+  LoadPoseD(a_T_b, qz, tz);
+  LoadPoseD(pose_a, qa, ta);
+  LoadPoseD(pose_b, qb, tb);
+  Se3BetweenD(qa, ta, qb, tb, qe, te);   // pose_a^-1 pose_b
+  Se3BetweenD(qz, tz, qe, te, qx, tx);   // Z^-1 pose_a^-1 pose_b
+  double theta, Jr[36], Ad[36], J[72];
+  Se3LogD(qx, tx, r, &theta);
+  Se3RightJacobianInverse(r, theta, Jr);
+  Se3BetweenD(qb, tb, qa, ta, qe, te);   // pose_b^-1 pose_a
+  Se3AdjointD(qe, te, Ad);
+  for (int i = 0; i < 6; ++i)
+    for (int j = 0; j < 6; ++j) {
+      double s = 0.0;
+      for (int k = 0; k < 6; ++k) s += Jr[i * 6 + k] * Ad[k * 6 + j];
+      J[i * 12 + j] = -s;
+      J[i * 12 + 6 + j] = Jr[i * 6 + j];
+    }
+  InformationTerms<12>(r, J, info, H, b, cost);
+}
+
+// The information of the prior that stands for a constraint's term in pose_a while pose_b stays fixed.  That prior sits at
+// P = pose_b Z^-1, and its residual log(P^-1 pose_a) = log(Z (Z^-1 pose_a^-1 pose_b)^-1 Z^-1) = -Ad(Z) r, so with
+// L_a = Ad(Z^-1)^T L Ad(Z^-1) its cost equals the constraint's.  info_a: L_a's upper triangle (21).
+BBA_HD void PoseConstraintInformationA(const float a_T_b[7], const float info[21], double info_a[21]) {
+  double qz[4], tz[3], qi[4], ti[3], Ad[36], L[36];
+  LoadPoseD(a_T_b, qz, tz);
+  const double q_id[4] = {0.0, 0.0, 0.0, 1.0}, t_id[3] = {0.0, 0.0, 0.0};
+  Se3BetweenD(qz, tz, q_id, t_id, qi, ti);   // Z^-1
+  Se3AdjointD(qi, ti, Ad);
+  int idx = 0;
+  for (int i = 0; i < 6; ++i)
+    for (int j = i; j < 6; ++j) {
+      L[i * 6 + j] = L[j * 6 + i] = info[idx];
+      ++idx;
+    }
+  idx = 0;
+  for (int i = 0; i < 6; ++i)
+    for (int j = i; j < 6; ++j) {
+      double s = 0.0;
+      for (int k = 0; k < 6; ++k)
+        for (int l = 0; l < 6; ++l) s += Ad[k * 6 + i] * L[k * 6 + l] * Ad[l * 6 + j];
+      info_a[idx++] = s;
+    }
 }
 
 // Camera frusta and their intersection test (co-visibility of keyframes), host only.

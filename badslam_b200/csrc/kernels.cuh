@@ -11,7 +11,13 @@
 
 namespace bba {
 
-struct PosePrior;   // host_math.hpp
+// One term of a keyframe's pose solve in the form of a soft pose prior (host_math.hpp PosePriorTerms): the prior global_T_frame
+// and the upper triangle of its 6x6 information matrix.  The pose step stages a keyframe's prior, the equivalent priors of its
+// relative pose constraints and their damping anchors as such terms (pose_step.cu StagePoseTerms).
+struct PoseTerm {
+  float pose[7];
+  float info[21];
+};
 
 // Accumulator record per keyframe written by the pose kernel: 32 fp64 sums
 //   [0..20] H upper triangle row-major, [21..26] b, [27] n_assoc, [28] n_photo,
@@ -104,7 +110,10 @@ struct PoseSolveArgs {
   unsigned int* queue;         // PoseAccumulateKernel's work-item counter, re-armed here
   int iteration;
   int max_iterations;
-  const PosePrior* priors;     // [max_kf] soft pose priors by keyframe id, or null when no keyframe has one
+  // the soft pose terms by keyframe id: keyframe k's are terms[term_offsets[k] .. term_offsets[k + 1]), added in list order;
+  // both null when no keyframe has one
+  const int* term_offsets;     // [keyframes + 1]
+  const PoseTerm* terms;
 };
 // Device-side Gauss-Newton step for every keyframe in the list (direct_ba_alternating.cc:173-233).
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
@@ -251,15 +260,24 @@ LaunchResult LaunchPcgStep3(uint32_t n, uint32_t a_index, int kf_count, float* g
 LaunchResult LaunchPcgUpdateSurfels(float* surfels, uint32_t pitch, uint32_t n, bool use_desc, uint32_t surfel_start, const float* delta,
                                     cudaStream_t stream);
 LaunchResult LaunchPcgUpdateCfactor(float* cfactor, uint32_t cells, const float* delta, cudaStream_t stream);
-// The soft pose prior of one pose unknown block of the PCG solver: first unknown u, J^T L J (upper triangle) and J^T L r.
-struct PcgPriorTerm {
-  uint32_t u;
+// The pose-block terms of the PCG products (soft pose priors and relative pose constraints).  One term of pose block i: H_ii
+// (upper triangle), b_i (J^T L r), and for a constraint whose other end j is a pose unknown, j's first unknown and H_ij
+// (row-major, rows i); other = -1 for a prior or an edge to the gauge keyframe (p_gauge = 0).
+struct PcgPoseTerm {
+  int other;
   float H[21];
   float b[6];
+  float X[36];
 };
-// init: r -= J^T L r, M += diag(J^T L J); else g += J^T L J p, *alpha_d += p^T J^T L J p (a fixed-order fp64 sum).
-LaunchResult LaunchPcgPosePrior(const PcgPriorTerm* terms, int count, bool init, float* r, float* M, const float* p, float* g,
-                                double* alpha_d, cudaStream_t stream);
+// A pose block with terms: its first unknown u and its terms [begin, end) in a fixed order.
+struct PcgPoseBlock {
+  uint32_t u;
+  int begin, end;
+};
+// init: r_i -= sum b_i, M_i += sum diag(H_ii); else g_i += sum (H_ii p_i + H_ij p_j) and *alpha_d += sum_i p_i . (that
+// contribution) = p^T A p over the terms, a fixed-order fp64 sum without atomics.
+LaunchResult LaunchPcgPoseTerms(const PcgPoseBlock* blocks, int block_count, const PcgPoseTerm* terms, bool init, float* r, float* M,
+                                const float* p, float* g, double* alpha_d, cudaStream_t stream);
 
 // End-of-BA surfel maintenance (lifecycle.cu; PerformBASchemeEndTasks, direct_ba.cc:566-653).
 struct KfRadius {

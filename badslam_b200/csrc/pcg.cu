@@ -437,37 +437,51 @@ LaunchResult LaunchPcgUnpackAlphaD(double* scalars, const float* tail, cudaStrea
   return {1};
 }
 
-// The soft pose priors' part of the products, one thread per prior-carrying pose block after PcgAccumulateKernel (one block: a
-// few thousand keyframes at most, and alpha_d's share is summed in a fixed order).
+// The pose-block terms' part of the products (soft pose priors, relative pose constraints), one thread per pose block with terms,
+// after PcgAccumulateKernel.  A thread gathers its block's terms in list order and writes only its own block; the one block
+// sums alpha_d's share in a fixed order (a few thousand keyframes at most).
 template <bool INIT>
-__global__ void __launch_bounds__(256) PcgPosePriorKernel(const PcgPriorTerm* __restrict__ terms, int count, float* __restrict__ r,
+__global__ void __launch_bounds__(256) PcgPoseTermsKernel(const PcgPoseBlock* __restrict__ blocks, int block_count,
+                                                          const PcgPoseTerm* __restrict__ terms, float* __restrict__ r,
                                                           float* __restrict__ M, const float* __restrict__ p, float* __restrict__ g,
                                                           double* __restrict__ alpha_d) {
   double pap = 0.0;
-  for (int i = threadIdx.x; i < count; i += blockDim.x) {
-    const PcgPriorTerm& t = terms[i];
+  for (int i = threadIdx.x; i < block_count; i += blockDim.x) {
+    const PcgPoseBlock blk = blocks[i];
     if constexpr (INIT) {
-      int d = 0;
-      for (int c = 0; c < 6; ++c) {
-        r[t.u + c] -= t.b[c];
-        M[t.u + c] += t.H[d];
-        d += 6 - c;
+      for (int e = blk.begin; e < blk.end; ++e) {
+        const PcgPoseTerm& t = terms[e];
+        int d = 0;
+        for (int c = 0; c < 6; ++c) {
+          r[blk.u + c] -= t.b[c];
+          M[blk.u + c] += t.H[d];
+          d += 6 - c;
+        }
       }
     } else {
       float pv[6], hp[6];
       for (int c = 0; c < 6; ++c) {
-        pv[c] = p[t.u + c];
+        pv[c] = p[blk.u + c];
         hp[c] = 0.f;
       }
-      int idx = 0;
-      for (int row = 0; row < 6; ++row)
-        for (int col = row; col < 6; ++col) {
-          const float h = t.H[idx++];
-          hp[row] += h * pv[col];
-          if (col != row) hp[col] += h * pv[row];
+      for (int e = blk.begin; e < blk.end; ++e) {
+        const PcgPoseTerm& t = terms[e];
+        int idx = 0;
+        for (int row = 0; row < 6; ++row)
+          for (int col = row; col < 6; ++col) {
+            const float h = t.H[idx++];
+            hp[row] += h * pv[col];
+            if (col != row) hp[col] += h * pv[row];
+          }
+        if (t.other >= 0) {
+          float pj[6];
+          for (int c = 0; c < 6; ++c) pj[c] = p[t.other + c];
+          for (int row = 0; row < 6; ++row)
+            for (int col = 0; col < 6; ++col) hp[row] += t.X[row * 6 + col] * pj[col];
         }
+      }
       for (int c = 0; c < 6; ++c) {
-        g[t.u + c] += hp[c];
+        g[blk.u + c] += hp[c];
         pap += static_cast<double>(pv[c] * hp[c]);
       }
     }
@@ -478,11 +492,11 @@ __global__ void __launch_bounds__(256) PcgPosePriorKernel(const PcgPriorTerm* __
   }
 }
 
-LaunchResult LaunchPcgPosePrior(const PcgPriorTerm* terms, int count, bool init, float* r, float* M, const float* p, float* g,
-                                double* alpha_d, cudaStream_t stream) {
-  if (count <= 0) return {};
-  if (init) PcgPosePriorKernel<true><<<1, 256, 0, stream>>>(terms, count, r, M, p, g, alpha_d);
-  else PcgPosePriorKernel<false><<<1, 256, 0, stream>>>(terms, count, r, M, p, g, alpha_d);
+LaunchResult LaunchPcgPoseTerms(const PcgPoseBlock* blocks, int block_count, const PcgPoseTerm* terms, bool init, float* r, float* M,
+                                const float* p, float* g, double* alpha_d, cudaStream_t stream) {
+  if (block_count <= 0) return {};
+  if (init) PcgPoseTermsKernel<true><<<1, 256, 0, stream>>>(blocks, block_count, terms, r, M, p, g, alpha_d);
+  else PcgPoseTermsKernel<false><<<1, 256, 0, stream>>>(blocks, block_count, terms, r, M, p, g, alpha_d);
   return {1};
 }
 

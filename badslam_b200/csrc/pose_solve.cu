@@ -55,13 +55,17 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
     a.stage_counts[2 * kf + 1] = 0ull;
 
     float* pe = a.pose_est + static_cast<size_t>(kf) * 7;
-    if (a.priors && a.priors[kf].has) {
-      // the soft pose prior (bba_set_keyframe_pose_priors), added to the rounded sums in fp64 at the current estimate
-      const PosePrior& prior = a.priors[kf];
-      double Hp[21], bp[6], cost;
-      PosePriorTerms(prior.pose, pe, prior.info, Hp, bp, &cost);
-      for (int j = 0; j < 21; ++j) H[j] += Hp[j];
-      for (int j = 0; j < 6; ++j) b[j] += bp[j];
+    if (a.term_offsets) {
+      // the soft pose terms (a prior, the equivalent priors of relative pose constraints and their damping anchors), added to
+      // the rounded sums in fp64 at the current estimate, in list order
+      const int end = a.term_offsets[kf + 1];
+      for (int t = a.term_offsets[kf]; t < end; ++t) {
+        const PoseTerm& term = a.terms[t];
+        double Hp[21], bp[6], cost;
+        PosePriorTerms(term.pose, pe, term.info, Hp, bp, &cost);
+        for (int j = 0; j < 21; ++j) H[j] += Hp[j];
+        for (int j = 0; j < 6; ++j) b[j] += bp[j];
+      }
     }
     SolveLDLT<6>(H, b, x);
     float xf[6], neg[6];

@@ -529,6 +529,54 @@ class DirectBA:
         self._check(self._lib.bba_get_keyframe_pose_prior(self._h, keyframe_id, p.ctypes.data, L.ctypes.data, C.byref(has)))
         return (p, L) if has.value else None
 
+    # -- soft relative pose constraints (not in the reference; include/badba.h "Soft relative pose constraints") -------------
+    def AddKeyframePoseConstraints(self, a_ids, b_ids, a_T_b, information) -> np.ndarray:
+        """Adds constraints (a, b, Z = a_T_b, L) with the cost 1/2 r^T L r, r = log(Z^-1 global_T_a^-1 global_T_b) (translation,
+        then rotation), and returns their ids ([n] int32).  a_T_b: [n, 7]; information: [n, 21] upper triangles of L, or
+        [n, 6, 6] / [6, 6] matrices (one matrix for all).  Refused as a whole (nothing changes) for an unknown keyframe, a == b,
+        a non-finite value, a zero quaternion or an L that is not positive semi-definite."""
+        a = np.atleast_1d(np.asarray(a_ids, np.int64))
+        b = np.atleast_1d(np.asarray(b_ids, np.int64))
+        n = len(a)
+        if len(b) != n:
+            raise ValueError("a_ids and b_ids differ in length")
+        Z = np.asarray(a_T_b, np.float32).reshape(n, 7)
+        L = np.asarray(information, np.float32)
+        if L.shape[-2:] == (6, 6):
+            L = np.broadcast_to(L, (n, 6, 6))[:, np.triu_indices(6)[0], np.triu_indices(6)[1]]
+        L = np.broadcast_to(L.reshape(-1, 21), (n, 21))
+        recs = (_lib.PoseConstraint * max(n, 1))()
+        for i in range(n):
+            recs[i].keyframe_a, recs[i].keyframe_b = int(a[i]), int(b[i])
+            recs[i].a_T_b[:] = [float(v) for v in Z[i]]
+            recs[i].information[:] = [float(v) for v in L[i]]
+        ids = np.zeros(max(n, 1), np.int32)
+        self._check(self._lib.bba_add_keyframe_pose_constraints(self._h, n, recs, ids.ctypes.data))
+        return ids[:n]
+
+    def RemoveKeyframePoseConstraints(self, ids=None):
+        """Removes the constraints `ids`, or every constraint with ids=None."""
+        if ids is None:
+            self._check(self._lib.bba_remove_keyframe_pose_constraints(self._h, -1, None))
+            return
+        ids = np.ascontiguousarray(np.atleast_1d(ids), np.int32)
+        self._check(self._lib.bba_remove_keyframe_pose_constraints(self._h, len(ids), ids.ctypes.data))
+
+    def KeyframePoseConstraints(self):
+        """The constraints as last published, in id order: (ids [n], a [n], b [n], a_T_b [n, 7], L upper triangles [n, 21])."""
+        count = C.c_int()
+        self._check(self._lib.bba_get_keyframe_pose_constraints(self._h, 0, None, None, C.byref(count)))
+        n = count.value
+        ids = np.zeros(max(n, 1), np.int32)
+        recs = (_lib.PoseConstraint * max(n, 1))()
+        self._check(self._lib.bba_get_keyframe_pose_constraints(self._h, n, ids.ctypes.data, recs, C.byref(count)))
+        n = min(n, count.value)
+        a = np.array([recs[i].keyframe_a for i in range(n)], np.int32)
+        b = np.array([recs[i].keyframe_b for i in range(n)], np.int32)
+        Z = np.array([list(recs[i].a_T_b) for i in range(n)], np.float32).reshape(n, 7)
+        L = np.array([list(recs[i].information) for i in range(n)], np.float32).reshape(n, 21)
+        return ids[:n], a, b, Z, L
+
     # -- trajectory deformation around a BA call (trajectory_deformation.h:43-58) ----------------------------------------
     def RememberKeyframePoses(self) -> np.ndarray:
         """RememberKeyframePoses (trajectory_deformation.cc:33-42): frame_T_global of every keyframe, [K, 7], all from one

@@ -228,6 +228,37 @@ bba_status bba_set_keyframe_pose_priors(bba_handle h, int count, const int* keyf
 bba_status bba_clear_keyframe_pose_priors(bba_handle h, int count, const int* keyframe_ids);
 bba_status bba_get_keyframe_pose_prior(bba_handle h, int keyframe_id, float prior_global_T_frame[7], float information[21],
                                        int* has_prior);
+/* Soft relative pose constraints between two keyframes (not in the reference; the binary counterpart of the priors, as the edges
+ * of a pose graph): a loop closure's relative pose (bba_track_frames_pairwise), wheel odometry or integrated IMU motion between
+ * two keyframes, the fixed extrinsics of a camera rig.  A constraint (a, b, Z = a_T_b, L), a != b, adds 1/2 r^T L r to the cost,
+ * r = log(Z^-1 * global_T_a^-1 * global_T_b) in the tangent order of the pose solve (translation, then rotation), L a 6x6
+ * information matrix given as its upper triangle, row-major, in the layout of H (21 floats).  Unlike a prior it fixes no gauge.
+ * Where it enters:
+ *  - the pose step of the alternating scheme and bba_estimate_frame_pose: each end that is in the step's keyframe list sees the
+ *    term as a prior, with the other end held at its pose at the start of the step; when both ends are in the list each also
+ *    gets a damping anchor at its own start pose (DESIGN.md 3.12).  An end outside the list (inactive, or every keyframe but
+ *    the one of bba_estimate_frame_pose) keeps its pose.  The frames of bba_estimate_frame_poses_for_frames get no terms.
+ *  - the PCG scheme: the exact 12x12 terms of both pose unknowns, with the gauge keyframe fixed.
+ * A handle without constraints runs exactly the code it ran before they existed.  With several ranks every rank makes the same
+ * calls, as it adds the same keyframes, and so gets the same ids.
+ *  bba_add_keyframe_pose_constraints: constraints [count]; writes the ids they get to out_ids [count] (may be NULL).  Ids come
+ *    from a counter of the handle and are never reused.  BBA_ERR_INVALID_ARGUMENT for an unknown keyframe, a == b, a non-finite
+ *    value, a zero quaternion or an L that is not positive semi-definite (the test of bba_set_keyframe_pose_priors); the
+ *    arguments are checked before anything changes, and a failed call leaves the handle unchanged.  The call reserves what the
+ *    bundle adjustment needs for the new count.
+ *  bba_remove_keyframe_pose_constraints: removes ids [count]; count = -1 removes every constraint (ids is not read).  An
+ *    unknown id refuses the whole call.
+ *  bba_get_keyframe_pose_constraints: front-end call (the published constraints, in id order): *count = their number; at most
+ *    capacity of them are written to ids / out (either may be NULL).
+ * The add and remove calls are BA-side calls and publish. */
+typedef struct {
+  int keyframe_a, keyframe_b;
+  float a_T_b[7];        /* Z = global_T_a^-1 * global_T_b at the constraint's optimum (qx qy qz qw tx ty tz) */
+  float information[21]; /* L's upper triangle, row-major */
+} bba_pose_constraint;
+bba_status bba_add_keyframe_pose_constraints(bba_handle h, int count, const bba_pose_constraint* constraints, int* out_ids);
+bba_status bba_remove_keyframe_pose_constraints(bba_handle h, int count, const int* ids);
+bba_status bba_get_keyframe_pose_constraints(bba_handle h, int capacity, int* ids, bba_pose_constraint* out, int* count);
 
 /* depth_params_ / cameras (direct_ba.h:243-297; SetColorCamera etc.).  The getters bba_get_intrinsics, bba_get_residual_types,
  * bba_get_cfactor_host and bba_cfactor_size are front-end calls (the published cameras, a, residual types and cfactor; the
@@ -670,6 +701,12 @@ int  bba_host_solve_ldlt(int n, const double* upper, const double* b, double* x)
  * (6) and cost = r^T L r / 2, all in fp64.  information: L's upper triangle (21).  Writes nothing if a pointer is NULL. */
 void bba_host_pose_prior_terms(const float prior_global_T_frame[7], const float global_T_frame[7], const float information[21],
                                double H[21], double b[6], double* cost);
+/* The terms of a soft relative pose constraint at global_T_a = pose_a, global_T_b = pose_b, for the updates pose_a * exp(delta_a)
+ * and pose_b * exp(delta_b): with r = log(a_T_b^-1 * pose_a^-1 * pose_b), J_b = Jr^-1(r) and J_a = -Jr^-1(r) Ad(pose_b^-1 pose_a),
+ * H = J^T L J over (delta_a, delta_b) (12 x 12 upper triangle, 78), b = J^T L r (12) and cost = r^T L r / 2, all in fp64.
+ * Writes nothing if a pointer is NULL. */
+void bba_host_pose_constraint_terms(const float a_T_b[7], const float global_T_a[7], const float global_T_b[7],
+                                    const float information[21], double H[78], double b[12], double* cost);
 int  bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height,
                                const float global_T_frame_a[7], float min_depth_a, float max_depth_a,
                                const float global_T_frame_b[7], float min_depth_b, float max_depth_b);

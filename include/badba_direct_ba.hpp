@@ -357,6 +357,23 @@ class DirectBA {
     Check(bba_clear_keyframe_pose_priors(h_, keyframe_ids.empty() ? -1 : static_cast<int>(keyframe_ids.size()), keyframe_ids.data()),
           "bba_clear_keyframe_pose_priors");
   }
+  // Soft relative pose constraints (not in the reference; badba.h): the cost 1/2 r^T L r, r = log(a_T_b^-1 global_T_a^-1
+  // global_T_b), L given as its upper triangle (translation, then rotation).  Returns the constraint's id.
+  int AddKeyframePoseConstraint(int keyframe_a, int keyframe_b, const SE3f& a_T_b, const float (&information)[21]) {
+    bba_pose_constraint c;
+    c.keyframe_a = keyframe_a;
+    c.keyframe_b = keyframe_b;
+    std::memcpy(c.a_T_b, a_T_b.data(), sizeof(c.a_T_b));
+    std::memcpy(c.information, information, sizeof(c.information));
+    int id = -1;
+    Check(bba_add_keyframe_pose_constraints(h_, 1, &c, &id), "bba_add_keyframe_pose_constraints");
+    return id;
+  }
+  // Removes the constraints `ids`, or every constraint when the list is empty.
+  void RemoveKeyframePoseConstraints(const std::vector<int>& ids = {}) {
+    Check(bba_remove_keyframe_pose_constraints(h_, ids.empty() ? -1 : static_cast<int>(ids.size()), ids.data()),
+          "bba_remove_keyframe_pose_constraints");
+  }
   uint32_t surfels_size() const { return bba_surfels_size(h_); }   // direct_ba.h:265
   void GetIntrinsics(float depth[4], float color[4], float* a) const { Check(bba_get_intrinsics(h_, depth, color, a), "bba_get_intrinsics"); }
   void SetPCGGaugeKeyframe(int keyframe_id) { pcg_gauge_keyframe_ = keyframe_id; }
