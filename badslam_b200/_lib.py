@@ -200,6 +200,7 @@ SYMBOLS = {
                                             _P, _P, _P]),
     "bba_update_surfel_activation": (C.c_int, [_P, _P]),
     "bba_optimize_geometry_iteration": (C.c_int, [_P, _P]),
+    "bba_deform_surfels": (C.c_int, [_P, C.c_int, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P]),
     "bba_optimize_intrinsics": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "bba_debug_intrinsics_coeffs": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P]),
     "bba_perform_end_tasks": (C.c_int, [_P, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P]),

@@ -68,6 +68,18 @@ bba_status BuildGeometryArgs(bba_handle h, bba::GeometryArgs* g, cudaStream_t s,
   return BBA_OK;
 }
 
+// geo.d_all_list, the keyframe list 0 .. max_keyframes - 1, made on first use.
+bba_status MakeAllKeyframeList(bba_handle h) {
+  if (h->geo.d_all_list) return BBA_OK;   // (set only once it is filled)
+  DeviceBuffer<int> all;
+  BBA_CUDA(h, all.Reserve(h->cfg.max_keyframes));
+  std::vector<int> iota(h->cfg.max_keyframes);
+  for (int i = 0; i < h->cfg.max_keyframes; ++i) iota[i] = i;
+  BBA_CUDA(h, cudaMemcpy(all, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice));
+  h->geo.d_all_list = std::move(all);
+  return BBA_OK;
+}
+
 // The normal equations of the intrinsics step as AccumulateIntrinsics leaves them on the device: the kIntrinsicsSums global sums
 // in geo.d_intr_sums and the cell rows, P floats each, in geo.d_intr.
 struct IntrinsicsEquations {
@@ -84,14 +96,7 @@ bba_status AccumulateIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cu
   const size_t intr_floats = 64 + static_cast<size_t>(8) * P + 8;
   BBA_CUDA(h, h->geo.d_intr.Reserve(intr_floats));
   BBA_CUDA(h, h->geo.d_intr_sums.Reserve(bba::kIntrinsicsSums));
-  if (!h->geo.d_all_list) {   // (set only once it is filled)
-    DeviceBuffer<int> all;
-    BBA_CUDA(h, all.Reserve(h->cfg.max_keyframes));
-    std::vector<int> iota(h->cfg.max_keyframes);
-    for (int i = 0; i < h->cfg.max_keyframes; ++i) iota[i] = i;
-    BBA_CUDA(h, cudaMemcpy(all, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice));
-    h->geo.d_all_list = std::move(all);
-  }
+  if (bba_status st = MakeAllKeyframeList(h)) return st;
   BBA_CUDA(h, h->geo.h_intr_sums.Reserve(bba::kIntrinsicsSums));
   BBA_CUDA(h, h->geo.h_intr_x1.Reserve(8));
   if (bba_status st = UploadKeyframes(h, s)) return st;
@@ -815,6 +820,97 @@ bba_status GeometryPass(bba_handle h, bool activation, cudaStream_t s) {
   return MarkStaging(h, s);
 }
 
+// Rotation matrix of a quaternion (x y z w), normalised in fp64.
+void QuatToMatrix64(const float q[4], double R[9]) {
+  const double n = std::sqrt(static_cast<double>(q[0]) * q[0] + static_cast<double>(q[1]) * q[1] + static_cast<double>(q[2]) * q[2] +
+                             static_cast<double>(q[3]) * q[3]);
+  const double x = q[0] / n, y = q[1] / n, z = q[2] / n, w = q[3] / n;
+  R[0] = 1 - 2 * (y * y + z * z); R[1] = 2 * (x * y - z * w); R[2] = 2 * (x * z + y * w);
+  R[3] = 2 * (x * y + z * w); R[4] = 1 - 2 * (x * x + z * z); R[5] = 2 * (y * z - x * w);
+  R[6] = 2 * (x * z - y * w); R[7] = 2 * (y * z + x * w); R[8] = 1 - 2 * (x * x + y * y);
+}
+
+// Keyframe k's change for the surfel deformation (DESIGN §3.13): D = global_T_frame (now) * original frame_T_global and the
+// original camera centre, in fp64 and rounded; a keyframe whose current pose inverts to the original bit for bit is unmoved.
+KfChange KeyframeChange(const Pose& global_T_frame, const float original[7]) {
+  KfChange c{};
+  float inv[7];
+  PoseToArray(Inverse(global_T_frame), inv);
+  c.unmoved = std::memcmp(inv, original, sizeof(inv)) == 0;
+  double Rc[9], Ro[9];
+  QuatToMatrix64(global_T_frame.q, Rc);
+  QuatToMatrix64(original, Ro);
+  for (int r = 0; r < 3; ++r) {
+    for (int col = 0; col < 3; ++col)
+      c.D[4 * r + col] = static_cast<float>(Rc[3 * r] * Ro[col] + Rc[3 * r + 1] * Ro[3 + col] + Rc[3 * r + 2] * Ro[6 + col]);
+    c.D[4 * r + 3] = static_cast<float>(Rc[3 * r] * original[4] + Rc[3 * r + 1] * original[5] + Rc[3 * r + 2] * original[6] +
+                                        global_T_frame.t[r]);
+    c.centre[r] = static_cast<float>(-(Ro[r] * original[4] + Ro[3 + r] * original[5] + Ro[6 + r] * original[6]));
+  }
+  if (c.unmoved)
+    for (int i = 0; i < 12; ++i) c.D[i] = (i % 5 == 0) ? 1.f : 0.f;
+  return c;
+}
+
+// bba_deform_surfels.  Every argument is checked before anything is enqueued.
+bba_status DeformSurfels(bba_handle h, int count, const float* original, uint32_t* moved, uint32_t* unobserved, cudaStream_t s) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_deform_surfels: ";
+  if (count < 0 || count > static_cast<int>(h->keyframes.size())) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad count");
+  if (count > 0 && !original) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  for (int k = 0; k < count; ++k) {
+    const float* p = original + 7 * static_cast<size_t>(k);
+    for (int j = 0; j < 7; ++j)
+      if (!std::isfinite(p[j])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose");
+    if (p[0] * p[0] + p[1] * p[1] + p[2] * p[2] + p[3] * p[3] < 1e-12f) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "zero quaternion");
+  }
+  if (moved) *moved = 0;
+  if (unobserved) *unobserved = 0;
+  if (count == 0 || h->surfels_size == 0) return BBA_OK;
+  if (bba_status st = CheckSurfels(h)) return st;
+  if (bba_status st = CheckCollective(h)) return st;
+  auto& d = h->deform;
+  BBA_CUDA(h, d.h_kfs.Reserve(count, h->cfg.max_keyframes));
+  BBA_CUDA(h, d.d_kfs.Reserve(count, h->cfg.max_keyframes));
+  BBA_CUDA(h, d.h_changes.Reserve(count, h->cfg.max_keyframes));
+  BBA_CUDA(h, d.d_changes.Reserve(count, h->cfg.max_keyframes));
+  BBA_CUDA(h, d.d_counts.Reserve(2));
+  BBA_CUDA(h, d.h_counts.Reserve(2));
+  if (bba_status st = MakeAllKeyframeList(h)) return st;
+  if (bba_status st = WaitStaging(h)) return st;
+  for (int k = 0; k < count; ++k) {
+    const Keyframe& kf = h->keyframes[k];
+    const float* p = original + 7 * static_cast<size_t>(k);
+    FillKfDevice(kf, kf.pose, d.h_kfs + k);
+    ToMatrix3x4(PoseFromArray(p), d.h_kfs[k].T);   // the association runs at the original pose
+    d.h_changes[k] = KeyframeChange(kf.pose, p);
+  }
+  BBA_CUDA(h, cudaMemcpyAsync(d.d_kfs, d.h_kfs, sizeof(KfDevice) * count, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemcpyAsync(d.d_changes, d.h_changes, sizeof(KfChange) * count, cudaMemcpyHostToDevice, s));
+  if (bba_status st = MarkStaging(h, s)) return st;
+  BBA_CUDA(h, cudaMemsetAsync(d.d_counts, 0, sizeof(unsigned int) * 2, s));
+  bba::DeformArgs a;
+  if (bba_status st = BuildGeometryArgs(h, &a.geo, s, GeoOrder::kSpatial)) return st;
+  a.geo.kfs = d.d_kfs;
+  a.geo.kf_list = h->geo.d_all_list;
+  a.geo.kf_count = count;
+  a.changes = d.d_changes;
+  a.counts = d.d_counts;
+  BBA_LAUNCH(h, h->launches, LaunchDeformSurfels, a, h->sm_count, s);
+  if (bba_status st = ExchangeGeometry(h, s)) return st;
+  h->pose.order_stale = true;   // the positions moved
+  if (!moved && !unobserved) return BBA_OK;
+  BBA_CUDA(h, cudaMemcpyAsync(d.h_counts, d.d_counts, sizeof(unsigned int) * 2, cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  uint32_t counts[2] = {d.h_counts[0], d.h_counts[1]};
+  if (h->cfg.world_size > 1)   // every rank counted its own shard
+    for (uint32_t& c : counts)
+      if (bba_status st = SumOverRanks(h, c, s, &c)) return st;
+  if (moved) *moved = counts[0];
+  if (unobserved) *unobserved = counts[1];
+  return BBA_OK;
+}
+
 }  // namespace
 }  // namespace bba
 
@@ -828,6 +924,11 @@ bba_status bba_update_surfel_activation(bba_handle h, void* stream) {
 
 bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream) {
   return GeometryPass(h, /*activation=*/false, static_cast<cudaStream_t>(stream));
+}
+
+bba_status bba_deform_surfels(bba_handle h, int count, const float* original_keyframe_T_global, uint32_t* moved, uint32_t* unobserved,
+                              void* stream) {
+  return DeformSurfels(h, count, original_keyframe_T_global, moved, unobserved, static_cast<cudaStream_t>(stream));
 }
 
 bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth, int optimize_color, void* stream) {

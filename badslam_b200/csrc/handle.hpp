@@ -276,6 +276,17 @@ struct bba_context {
     bba::PinnedBuffer<float> h_intr_x1;   // 8 floats
   } geo;
 
+  // surfel deformation (bba_deform_surfels): the keyframe records at the caller's original poses, the keyframes' pose changes and
+  // the two counters
+  struct Deform {
+    bba::PinnedBuffer<bba::KfDevice> h_kfs;
+    bba::DeviceBuffer<bba::KfDevice> d_kfs;
+    bba::PinnedBuffer<bba::KfChange> h_changes;
+    bba::DeviceBuffer<bba::KfChange> d_changes;
+    bba::DeviceBuffer<unsigned int> d_counts;   // [2] moved, unobserved
+    bba::PinnedBuffer<unsigned int> h_counts;
+  } deform;
+
   // in-loop surfel lifecycle (creation / merge / compaction) and the end tasks
   struct Lifecycle {
     bba::DeviceBuffer<unsigned int> d_sup;         // [3][cells]

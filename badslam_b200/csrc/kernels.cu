@@ -690,6 +690,26 @@ __device__ __forceinline__ void StoreSurfelRow(const GeometryArgs& a, int row, u
   StoreReplicas(a.surfels, a.peers.surfels, a.peers.count, static_cast<size_t>(row) * a.pitch + i, v);
 }
 
+// The stream position s of the lane's surfel in sub-step `sub` of a work item's tile, and whether it is one of the launch's surfels.
+__device__ __forceinline__ bool GeoStreamPosition(const GeometryArgs& a, uint32_t tile, uint32_t sub, int lane, uint32_t* s) {
+  const uint32_t li = a.begin + (tile << a.tile_shift) + sub * 32 + lane;
+  *s = SurfelShardToGlobal(li, a.shard_rank, a.shard_world);
+  return li < a.end && *s < a.n;
+}
+// The caller index of the surfel at stream position s.
+__device__ __forceinline__ uint32_t GeoResultIndex(const GeometryArgs& a, uint32_t s) { return a.perm ? __ldg(a.perm + s) : s; }
+// The N partial sums a surfel parks in the scratch rows 8 .. 8 + N - 1 between keyframe groups, at its stream position.
+template <int N>
+__device__ __forceinline__ void LoadParkedSums(const GeometryArgs& a, uint32_t s, float (&v)[N]) {
+#pragma unroll
+  for (int r = 0; r < N; ++r) v[r] = __ldcg(a.surfels + (kRowAccum0 + r) * static_cast<size_t>(a.pitch) + s);
+}
+template <int N>
+__device__ __forceinline__ void StoreParkedSums(const GeometryArgs& a, uint32_t s, const float (&v)[N]) {
+#pragma unroll
+  for (int r = 0; r < N; ++r) __stcg(a.surfels + (kRowAccum0 + r) * static_cast<size_t>(a.pitch) + s, v[r]);
+}
+
 // Both geometry kernels walk a work item's tile in sub-steps of 32 stream positions, one surfel per lane, with the keyframe loop
 // executed by the whole warp.  In spatial order a sub-step's surfels are a compact cluster: the box of the lanes that still have
 // pairs to evaluate is tested against the views of all keyframes of the group at once, one keyframe per lane (VisibleKeyframes,
@@ -713,9 +733,8 @@ __global__ void __launch_bounds__(kGeoThreads) ActivationNormalsKernel(const __g
     KfDevice* recs = s_kfs + (threadIdx.x >> 5) * kGeoGroup;
     StageGroupRecords(a.kfs, a.kf_list + j_begin, n_kf, recs, lane);
     for (uint32_t sub = 0; sub < tile_len / 32; ++sub) {
-      const uint32_t li = a.begin + (tile << a.tile_shift) + sub * 32 + lane;
-      const uint32_t s = SurfelShardToGlobal(li, a.shard_rank, a.shard_world);
-      const bool in_range = li < a.end && s < a.n;
+      uint32_t s;
+      const bool in_range = GeoStreamPosition(a, tile, sub, lane, &s);
       const uint32_t flags = in_range ? __float_as_uint(a.stream[(kGeoStreamRows - 1) * F + s]) : 0u;
       const bool live = in_range && (DETERMINE || (flags & kSurfelActiveFlag));   // normals are updated for active surfels only
       if (__ballot_sync(0xffffffffu, live) == 0) continue;
@@ -777,7 +796,7 @@ __global__ void __launch_bounds__(kGeoThreads) ActivationNormalsKernel(const __g
         }
         if (DETERMINE) __stcg(a.surfels + (kRowAccum0 + 4) * P + s, act ? 1.f : 0.f);
       } else {
-        const uint32_t i = a.perm ? __ldg(a.perm + s) : s;
+        const uint32_t i = GeoResultIndex(a, s);
         // SetSurfelInactive + DetermineActiveSurfels (kernel_surfel_activation.cu:38-79)
         if (DETERMINE) StoreReplicas(a.active, a.peers.active, a.peers.count, i, act ? kSurfelActiveFlag : static_cast<uint8_t>(flags & ~kSurfelActiveFlag));
         if (NORMALS && act && s3 >= 1.f) {
@@ -947,19 +966,134 @@ __global__ void __launch_bounds__(kGeoThreads, 3) PositionDescriptorKernel(const
   }
 }
 
+// The surfel deformation (DESIGN §3.13).  The walk is ActivationNormalsKernel's: the keyframe groups of a tile in ascending order,
+// the warp's box culled against the group's views, the sums parked between groups in the scratch rows.  The records carry the
+// ORIGINAL poses, so the voters of a surfel are the keyframes it is associated with at those poses, in ascending id; each adds
+// D_k p - p and R_k n.  A surfel without a voter takes the keyframe whose original camera centre is nearest.  The per-surfel sums
+// run in keyframe order without atomics, so a surfel's result does not depend on the order, the warp, the grouping or the culling.
+constexpr int kDeformSums = 8;   // displacement x y z, normal x y z, voters, moved voters
+__global__ void __launch_bounds__(kGeoThreads) DeformSurfelsKernel(const __grid_constant__ DeformArgs d) {
+  extern __shared__ __align__(16) unsigned char geo_smem[];
+  const GeometryArgs& a = d.geo;
+  KfDevice* s_kfs = reinterpret_cast<KfDevice*>(geo_smem);
+  const uint32_t tile_len = 1u << a.tile_shift;
+  const uint32_t n_tiles = (a.end - a.begin + tile_len - 1) >> a.tile_shift;
+  const uint32_t n_groups = (a.kf_count + kGeoGroup - 1) / kGeoGroup;
+  const uint32_t n_items = n_groups * n_tiles;
+  const size_t F = a.stream_pitch;
+  const int lane = threadIdx.x & 31;
+  // One voter's terms: D p - p and R n.
+  auto vote = [&](const KfChange* __restrict__ c, const Vec3& p, const Vec3& n, float (&v)[kDeformSums]) {
+    const float* D = c->D;
+    const Vec3 q = Transform(D, p);
+    v[0] += q.x - p.x;
+    v[1] += q.y - p.y;
+    v[2] += q.z - p.z;
+    const Vec3 rn = Rotate(D, n);
+    v[3] += rn.x;
+    v[4] += rn.y;
+    v[5] += rn.z;
+    v[6] += 1.f;
+    if (!__ldg(&c->unmoved)) v[7] += 1.f;
+  };
+  uint32_t group, tile;
+  while (ClaimItem(a.queue, n_tiles, n_items, a.tile_epoch, &group, &tile)) {
+    const bool first = group == 0, last = group + 1 == n_groups;
+    const int j_begin = group * kGeoGroup, j_end = min(a.kf_count, static_cast<int>(group + 1) * kGeoGroup);
+    const int n_kf = j_end - j_begin;
+    KfDevice* recs = s_kfs + (threadIdx.x >> 5) * kGeoGroup;
+    StageGroupRecords(a.kfs, a.kf_list + j_begin, n_kf, recs, lane);
+    for (uint32_t sub = 0; sub < tile_len / 32; ++sub) {
+      uint32_t s;
+      const bool in_range = GeoStreamPosition(a, tile, sub, lane, &s);
+      Vec3 gp = V3(0.f, 0.f, 0.f), nrm = V3(0.f, 0.f, 1.f);
+      if (in_range) gp = V3(a.stream[0 * F + s], a.stream[1 * F + s], a.stream[2 * F + s]);
+      const bool live = in_range && !isnan(gp.x);   // deleted surfels: x = NaN
+      if (__ballot_sync(0xffffffffu, live) == 0) continue;
+      if (live) nrm = UnpackNormal(__float_as_uint(a.stream[3 * F + s]));
+      float v[kDeformSums] = {};
+      if (!first && live) LoadParkedSums(a, s, v);
+      float lo[3], hi[3];
+      WarpBox(gp, live, lo, hi);
+      unsigned vis = VisibleKeyframes<false>(a.cam, recs, n_kf, lo, hi, lane);
+      for (int j = PopLowest(&vis); j >= 0; j = PopLowest(&vis)) {
+        KfRegs K;
+        LoadKfShared(recs + j, &K);
+        Assoc r;
+        if (live && ProjectIntoImage(a.cam, K.T, gp, &r) &&
+            Associate(a.cam, K.T, nrm, LoadPixel(a.cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r), &r) == 3)
+          vote(d.changes + j_begin + j, gp, nrm, v);
+      }
+      if (live && !last) StoreParkedSums(a, s, v);
+      bool unobserved = false, moved = false;
+      if (live && last) {
+        // Fallback: the keyframe whose original camera centre is nearest, the smaller id on a tie.
+        unobserved = v[6] == 0.f;
+        if (unobserved) {
+          int best = 0;
+          float best_d = INFINITY;
+          for (int k = 0; k < a.kf_count; ++k) {
+            const Vec3 e = gp - V3(__ldg(&d.changes[k].centre[0]), __ldg(&d.changes[k].centre[1]), __ldg(&d.changes[k].centre[2]));
+            const float dist = Dot(e, e);
+            if (dist < best_d) {
+              best_d = dist;
+              best = k;
+            }
+          }
+          vote(d.changes + best, gp, nrm, v);
+        }
+        // A surfel whose voters are all unmoved keeps its bits.
+        moved = v[7] != 0.f;
+        if (moved) {
+          const uint32_t i = GeoResultIndex(a, s);
+          StoreSurfelRow(a, kRowX, i, gp.x + __fdiv_rn(v[0], v[6]));
+          StoreSurfelRow(a, kRowY, i, gp.y + __fdiv_rn(v[1], v[6]));
+          StoreSurfelRow(a, kRowZ, i, gp.z + __fdiv_rn(v[2], v[6]));
+          const float len = __fsqrt_rn(v[3] * v[3] + v[4] * v[4] + v[5] * v[5]);
+          // (normals that cancel out keep the old one)
+          if (len > 0.f)
+            StoreSurfelRow(a, kRowNormal, i, __uint_as_float(PackNormal(V3(__fdiv_rn(v[3], len), __fdiv_rn(v[4], len), __fdiv_rn(v[5], len)))));
+        }
+      }
+      if (last) {
+        const unsigned moved_lanes = __ballot_sync(0xffffffffu, moved), unobserved_lanes = __ballot_sync(0xffffffffu, unobserved);
+        if (lane == 0 && moved_lanes) atomicAdd(d.counts, __popc(moved_lanes));
+        if (lane == 0 && unobserved_lanes) atomicAdd(d.counts + 1, __popc(unobserved_lanes));
+      }
+    }
+    RetireItem(a.tile_epoch, group, tile);
+  }
+}
+
 constexpr size_t kGeoSmemBytes = sizeof(KfDevice) * (kGeoThreads / 32) * kGeoGroup;   // the per-warp record slices
+
+// Everything a geometry launch does before its kernel: the grid (with *a's tile), the counters and the stream gather.
+template <typename Kernel>
+static LaunchResult PrepareGeo(Kernel kernel, GeometryArgs* a, int sm_count, bool desc_rows, cudaStream_t stream, uint32_t* grid) {
+  int per_sm = 0;
+  LaunchResult r{1, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGeoThreads, kGeoSmemBytes)};
+  *grid = EpochOrderedGrid(per_sm, sm_count, kGeoThreads, a->end - a->begin, (a->kf_count + kGeoGroup - 1) / kGeoGroup, &a->tile_shift);
+  const uint32_t n_tiles = (a->end - a->begin + (1u << a->tile_shift) - 1) >> a->tile_shift;
+  r += cudaMemsetAsync(a->queue, 0, sizeof(unsigned int), stream);
+  r += cudaMemsetAsync(a->tile_epoch, 0, sizeof(unsigned int) * n_tiles, stream);
+  r += LaunchGeometryStream(*a, desc_rows, stream);
+  return r;
+}
 
 template <typename Kernel>
 static LaunchResult LaunchGeo(Kernel kernel, GeometryArgs a, int sm_count, bool desc_rows, cudaStream_t stream) {
-  int per_sm = 0;
-  LaunchResult r{1, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGeoThreads, kGeoSmemBytes)};
-  const uint32_t grid =
-      EpochOrderedGrid(per_sm, sm_count, kGeoThreads, a.end - a.begin, (a.kf_count + kGeoGroup - 1) / kGeoGroup, &a.tile_shift);
-  const uint32_t n_tiles = (a.end - a.begin + (1u << a.tile_shift) - 1) >> a.tile_shift;
-  r += cudaMemsetAsync(a.queue, 0, sizeof(unsigned int), stream);
-  r += cudaMemsetAsync(a.tile_epoch, 0, sizeof(unsigned int) * n_tiles, stream);
-  r += LaunchGeometryStream(a, desc_rows, stream);
+  uint32_t grid;
+  const LaunchResult r = PrepareGeo(kernel, &a, sm_count, desc_rows, stream, &grid);
   kernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
+  return r;
+}
+
+LaunchResult LaunchDeformSurfels(const DeformArgs& args, int sm_count, cudaStream_t stream) {
+  if (args.geo.end <= args.geo.begin || args.geo.kf_count <= 0) return {};
+  DeformArgs a = args;
+  uint32_t grid;
+  const LaunchResult r = PrepareGeo(DeformSurfelsKernel, &a.geo, sm_count, false, stream, &grid);
+  DeformSurfelsKernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
   return r;
 }
 

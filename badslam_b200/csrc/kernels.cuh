@@ -165,6 +165,21 @@ LaunchResult LaunchActivationAndNormals(const GeometryArgs& args, int sm_count, 
 // Position (+ descriptor) accumulation and per-surfel solve (kernel_opt_geometry.cu:118-231,273-361 or :417-507).
 LaunchResult LaunchPositionAndDescriptor(const GeometryArgs& args, int sm_count, cudaStream_t stream);
 
+// Surfel deformation after an outside pose correction (bba_deform_surfels, DESIGN §3.13).  Per keyframe: D = global_T_frame (now)
+// * original frame_T_global, row-major 3x4 from old global coordinates to new ones, and the original camera centre.
+struct KfChange {
+  float D[12];
+  float centre[3];
+  int unmoved;               // 1: D is the exact identity
+};
+struct DeformArgs {
+  GeometryArgs geo;          // kfs: the keyframe records at their ORIGINAL poses; kf_list: 0 .. kf_count - 1
+  const KfChange* changes;   // [kf_count] by keyframe id
+  unsigned int* counts;      // [2] += surfels whose rows changed, surfels without an associated keyframe (zero at launch)
+};
+// The stream gather and the kernel, or nothing when there is nothing to do.  Deleted surfels (x = NaN) are skipped.
+LaunchResult LaunchDeformSurfels(const DeformArgs& a, int sm_count, cudaStream_t stream);
+
 // Multi-GPU surfel sharding: 256-surfel granules are dealt round-robin to the ranks (granule g belongs to rank g % world), so
 // that every rank sees the same mix of well- and poorly-observed surfels (surfels are stored in creation order, and the
 // cost of a surfel is the number of keyframes that see it).  A rank addresses its surfels through a dense local index.

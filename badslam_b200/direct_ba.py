@@ -601,6 +601,17 @@ class DirectBA:
         self._check(self._lib.bba_get_keyframe_states(self._h, K, current.ctypes.data, None))
         return deform_trajectory(start_frame, end_frame, keyframe_frame_indices, original_keyframe_T_global, current, frame_poses)
 
+    def DeformSurfelsWithKeyframePoseChanges(self, original_keyframe_T_global, stream=None):
+        """bba_deform_surfels (not in the reference): after an outside correction of the keyframe poses, moves every surfel
+        with the keyframes it is associated with at the remembered poses.  original_keyframe_T_global: what RememberKeyframePoses
+        returned ([count, 7], keyframes 0 .. count-1).  Returns (moved, unobserved): surfels whose rows changed, and surfels that
+        no keyframe observed (they follow the keyframe with the nearest original camera centre).  Synchronises the stream."""
+        original = np.ascontiguousarray(original_keyframe_T_global, np.float32).reshape(-1, 7)
+        moved, unobserved = C.c_uint32(), C.c_uint32()
+        self._check(self._lib.bba_deform_surfels(self._h, len(original), original.ctypes.data, C.byref(moved), C.byref(unobserved),
+                                                 self._stream_ptr(stream)))
+        return moved.value, unobserved.value
+
     def SurfelsDeviceView(self) -> torch.Tensor:
         """The 17-row surfel buffer as a torch tensor, whoever owns it (zero-copy)."""
         if self._surfels is not None:

@@ -348,6 +348,24 @@ bba_status bba_estimate_frame_poses_for_frames(bba_handle h, int frame_count, co
 bba_status bba_update_surfel_activation(bba_handle h, void* stream);
 /* OptimizeGeometryIterationCUDA (kernels.h:234-244, kernel_opt_geometry.cc:80-201) */
 bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream);
+/* Carries the keyframes' pose changes since original_keyframe_T_global over to the surfel map (not in the reference; DESIGN.md
+ * §3.13), after an outside pose correction written with bba_set_keyframe_states: a caller's pose graph after a loop closure, a
+ * re-anchoring to GNSS or motion-capture priors, a relocalisation.
+ * original_keyframe_T_global [count][7]: frame_T_global of keyframes 0 .. count-1 before the correction (RememberKeyframePoses).
+ * Keyframe k's change is D_k = global_T_frame[k] * original_keyframe_T_global[k]; a keyframe whose current pose inverts
+ * (bba_host_se3_inverse) to its original bit for bit is unmoved.  The voters of a surfel are the keyframes k < count it is
+ * associated with at their original poses (the association test of the geometry passes, with the current cameras, a and
+ * cfactor); without one, the keyframe whose original camera centre is nearest (the smaller id on a tie).  A surfel whose voters
+ * are all unmoved keeps its bits; any other gets p + sum_k (D_k p - p) / |voters| and the packed normalised sum of R_k n.
+ * Radius, colour, descriptors and active flags are not touched; deleted surfels (x = NaN) are skipped.  The result of a surfel
+ * depends on nothing but its own row and the keyframes, bit for bit, with any number of ranks.
+ * *moved: surfels whose rows changed; *unobserved: surfels without an associated keyframe.  Either may be NULL; a non-NULL one
+ * synchronises the stream (with several ranks, every rank must pass the same NULL-ness: the counts are summed over the ranks).
+ * BBA_ERR_INVALID_ARGUMENT: count < 0 or > the keyframe count, a NULL original_keyframe_T_global with count > 0, a non-finite
+ * value or a zero quaternion; arguments are checked before anything is enqueued, and a failed check changes nothing.  count = 0
+ * or an empty map: nothing to do.  A BA-side call. */
+bba_status bba_deform_surfels(bba_handle h, int count, const float* original_keyframe_T_global, uint32_t* moved, uint32_t* unobserved,
+                              void* stream);
 /* DirectBA::PerformBASchemeEndTasks (direct_ba.cc:566-653): DeleteSurfelsAndUpdateRadiiCUDA over every keyframe (surfels
  * with fewer than GetMinObservationCount() observations, or more free-space violations than observations, are deleted; the
  * others get the smallest observed radius) + CompactSurfelsCUDA.  bba_bundle_adjust runs it like the reference does: at

@@ -639,4 +639,17 @@ void ExtrapolateAndInterpolateKeyframePoseChanges(uint32_t start_frame, uint32_t
   ExtrapolateAndInterpolateKeyframePoseChanges(start_frame, end_frame, frame_index, original_keyframe_T_global, current, rgbd_video);
 }
 
+// The same pose changes carried over to the surfel map (bba_deform_surfels, not in the reference): after an outside correction of
+// the keyframe poses (a pose graph after a loop closure, written with bba_set_keyframe_states), the surfels move with the
+// keyframes they are associated with at the remembered poses.  A BA-side call; does not synchronise the stream.
+template <typename SE3f, typename PinholeCamera4f>
+void DeformSurfelsWithKeyframePoseChanges(DirectBA<SE3f, PinholeCamera4f>& dense_ba, const std::vector<SE3f>& original_keyframe_T_global,
+                                          cudaStream_t stream) {
+  const int K = static_cast<int>(original_keyframe_T_global.size());
+  std::vector<float> original(7 * static_cast<size_t>(K));
+  for (int k = 0; k < K; ++k) std::memcpy(&original[7 * k], original_keyframe_T_global[k].data(), 7 * sizeof(float));
+  if (bba_status s = bba_deform_surfels(dense_ba.handle(), K, original.data(), nullptr, nullptr, stream))
+    throw Error(s, std::string("DeformSurfelsWithKeyframePoseChanges: ") + bba_last_error(dense_ba.handle()));
+}
+
 }  // namespace badba
