@@ -92,6 +92,16 @@ class PoseConstraint(C.Structure):   # bba_pose_constraint
     _fields_ = [("keyframe_a", C.c_int), ("keyframe_b", C.c_int), ("a_T_b", C.c_float * 7), ("information", C.c_float * 21)]
 
 
+class PoseGraphOptions(C.Structure):   # bba_pose_graph_options
+    _fields_ = [("gauge_keyframe", C.c_int), ("max_iterations", C.c_int), ("use_odometry_chain", C.c_int),
+                ("odometry_information", C.c_float * 21)]
+
+
+class PoseGraphResult(C.Structure):   # bba_pose_graph_result
+    _fields_ = [("iterations", C.c_int), ("converged", C.c_int), ("linear_iterations", C.c_int), ("held_keyframes", C.c_int),
+                ("initial_cost", C.c_double), ("final_cost", C.c_double)]
+
+
 class PeerHandle(C.Structure):
     _fields_ = [("surfels_ipc", C.c_ubyte * 64), ("surfels_offset", C.c_uint64), ("active_ipc", C.c_ubyte * 64),
                 ("active_offset", C.c_uint64), ("pitch_bytes", C.c_uint64), ("surfels_size", C.c_uint32), ("rank", C.c_int32)]
@@ -201,6 +211,7 @@ SYMBOLS = {
     "bba_update_surfel_activation": (C.c_int, [_P, _P]),
     "bba_optimize_geometry_iteration": (C.c_int, [_P, _P]),
     "bba_deform_surfels": (C.c_int, [_P, C.c_int, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P]),
+    "bba_optimize_pose_graph": (C.c_int, [_P, C.POINTER(PoseGraphOptions), C.POINTER(PoseGraphResult), _P]),
     "bba_optimize_intrinsics": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "bba_debug_intrinsics_coeffs": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P]),
     "bba_perform_end_tasks": (C.c_int, [_P, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P]),

@@ -27,6 +27,7 @@ UNITS = [
     ("preprocess.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("odometry.cu", ["-use_fast_math", "-Xptxas", "-v"]),
     ("pose_solve.cu", []),
+    ("pose_graph.cu", ["-Xptxas", "-v"]),
     ("exact_sum.cu", ["-Xptxas", "-v"]),
     ("badba.cu", []),
     ("pose_step.cu", []),

@@ -789,39 +789,6 @@ bba_status bba_get_keyframe_states(bba_handle h, int count, float* poses, int* a
 }
 // ---- soft pose priors ----
 namespace {
-// Whether the symmetric 6x6 matrix with upper triangle info is positive semi-definite up to fp32 rounding: the pivoted LDLT of
-// SolveLDLT (largest |diagonal| first) has no negative pivot, and a zero pivot leaves nothing in its column.
-bool InformationPsd(const float info[21]) {
-  double M[36];
-  double scale = 0.0;
-  int idx = 0;
-  for (int r = 0; r < 6; ++r)
-    for (int c = r; c < 6; ++c) {
-      M[r * 6 + c] = M[c * 6 + r] = info[idx++];
-      scale = std::max(scale, std::fabs(static_cast<double>(info[idx - 1])));
-    }
-  if (scale == 0.0) return true;
-  const double pivot_tol = 1e-6 * scale, column_tol = 1e-3 * scale;
-  bool done[6] = {};
-  for (int k = 0; k < 6; ++k) {
-    int p = -1;
-    for (int i = 0; i < 6; ++i)
-      if (!done[i] && (p < 0 || std::fabs(M[i * 6 + i]) > std::fabs(M[p * 6 + p]))) p = i;
-    done[p] = true;
-    const double d = M[p * 6 + p];
-    if (d < -pivot_tol) return false;
-    if (d <= pivot_tol) {
-      for (int i = 0; i < 6; ++i)
-        if (!done[i] && std::fabs(M[i * 6 + p]) > column_tol) return false;
-      continue;
-    }
-    for (int i = 0; i < 6; ++i)
-      for (int j = 0; j < 6; ++j)
-        if (!done[i] && !done[j]) M[i * 6 + j] -= M[i * 6 + p] * M[p * 6 + j] / d;
-  }
-  return true;
-}
-
 // Counts the priors and publishes the records.
 bba_status CommitPosePriors(bba_handle h) {
   int count = 0;

@@ -911,6 +911,205 @@ bba_status DeformSurfels(bba_handle h, int count, const float* original, uint32_
   return BBA_OK;
 }
 
+// ---- keyframe pose graph (bba_optimize_pose_graph, DESIGN §3.14) ----
+// What the pose graph stages for K keyframes and C constraints: terms (a prior per keyframe, the constraints, the chain), ints
+// (held flags, row offsets, two ints per row entry, CSR offsets and columns) and doubles (the terms' blocks, the CSR blocks, b, the
+// couplings and the solver's work).  A row holds its prior and one entry per end of a constraint or chain edge.
+struct PoseGraphSizes {
+  size_t terms, ints, doubles;
+};
+PoseGraphSizes PoseGraphCapacity(size_t K, size_t C) {
+  const size_t terms = 2 * K + C, entries = 3 * K + 2 * C, nnz = 3 * K + 2 * C;
+  const size_t block_doubles = sizeof(PoseGraphTermBlocks) / sizeof(double);
+  return {terms, K + 2 * (K + 1) + 2 * entries + nnz, terms * block_doubles + 36 * nnz + 42 * K + PoseGraphWorkDoubles(K)};
+}
+
+// Sizes the pose graph's buffers for max_keyframes and `constraints` constraints, with room to double the constraints.
+bba_status ReservePoseGraph(bba_handle h, size_t constraints) {
+  const size_t M = static_cast<size_t>(h->cfg.max_keyframes);
+  const PoseGraphSizes need = PoseGraphCapacity(M, constraints), alloc = PoseGraphCapacity(M, 2 * constraints);
+  auto& g = h->graph;
+  BBA_CUDA(h, g.h_terms.Reserve(need.terms, alloc.terms));
+  BBA_CUDA(h, g.d_terms.Reserve(need.terms, alloc.terms));
+  BBA_CUDA(h, g.h_ints.Reserve(need.ints, alloc.ints));
+  BBA_CUDA(h, g.d_ints.Reserve(need.ints, alloc.ints));
+  BBA_CUDA(h, g.d_doubles.Reserve(need.doubles, alloc.doubles));
+  BBA_CUDA(h, g.h_poses.Reserve(7 * M));
+  BBA_CUDA(h, g.d_poses.Reserve(14 * M));
+  BBA_CUDA(h, g.d_state.Reserve(1));
+  BBA_CUDA(h, g.h_state.Reserve(1));
+  return BBA_OK;
+}
+
+int FindRoot(std::vector<int>& parent, int k) {
+  while (parent[k] != k) k = parent[k] = parent[parent[k]];
+  return k;
+}
+
+bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_pose_graph_result* result, cudaStream_t s) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_optimize_pose_graph: ";
+  if (!o) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null options");
+  const int K = static_cast<int>(h->keyframes.size());
+  const int gauge = o->gauge_keyframe;
+  if (gauge < -1 || gauge >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "gauge_keyframe out of range");
+  if (o->use_odometry_chain) {
+    for (int j = 0; j < 21; ++j)
+      if (!std::isfinite(o->odometry_information[j])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite odometry_information");
+    if (!InformationPsd(o->odometry_information))
+      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "odometry_information is not positive semi-definite");
+  }
+  bba_pose_graph_result r{};
+  if (result) *result = r;
+  if (K < 2 && h->pose_prior_count == 0) return BBA_OK;
+  const std::vector<PoseConstraint>& cons = h->pose_constraints;
+  if (bba_status st = ReservePoseGraph(h, cons.size())) return st;
+  auto& g = h->graph;
+  const bool chain = o->use_odometry_chain != 0;
+  const int max_iterations = o->max_iterations > 0 ? o->max_iterations : 20;   // pose_graph_optimizer.cc kMaxIterations
+
+  // the terms: priors, constraints by id, then the chain at the poses the call starts from
+  float* poses = g.h_poses;
+  for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses + 7 * k);
+  std::vector<int> prior_term(K, -1);
+  int T = 0;
+  auto add = [&](int a, int b, const float* z, const float* info) {
+    PoseGraphTerm& t = g.h_terms[T++];
+    t.a = a;
+    t.b = b;
+    std::memcpy(t.z, z, sizeof(t.z));
+    std::memcpy(t.info, info, sizeof(t.info));
+  };
+  for (int k = 0; k < K; ++k) {
+    const PosePrior& p = h->pose_priors[k];
+    if (!p.has) continue;
+    prior_term[k] = T;
+    add(k, -1, p.pose, p.info);
+  }
+  const int first_constraint = T;
+  for (const PoseConstraint& c : cons) add(c.c.keyframe_a, c.c.keyframe_b, c.c.a_T_b, c.c.information);
+  const int first_chain = T;
+  if (chain)
+    for (int k = 0; k + 1 < K; ++k) {
+      double qa[4], ta[3], qb[4], tb[3], q[4], t[3];
+      LoadPoseD(poses + 7 * k, qa, ta);
+      LoadPoseD(poses + 7 * (k + 1), qb, tb);
+      Se3BetweenD(qa, ta, qb, tb, q, t);   // T_k^-1 T_{k+1}
+      float z[7];
+      for (int j = 0; j < 4; ++j) z[j] = static_cast<float>(q[j]);
+      for (int j = 0; j < 3; ++j) z[4 + j] = static_cast<float>(t[j]);
+      add(k, k + 1, z, o->odometry_information);
+    }
+
+  // the held keyframes: the gauge, the untouched ones, and the lowest id of every component without the gauge or a prior
+  std::vector<int> parent(K), lowest(K, -1);
+  std::vector<char> touched(K, 0), anchored(K, 0);
+  for (int k = 0; k < K; ++k) parent[k] = k;
+  for (int i = first_constraint; i < T; ++i) {
+    const PoseGraphTerm& t = g.h_terms[i];
+    touched[t.a] = touched[t.b] = 1;
+    const int ra = FindRoot(parent, t.a), rb = FindRoot(parent, t.b);
+    if (ra != rb) parent[std::max(ra, rb)] = std::min(ra, rb);
+  }
+  for (int k = 0; k < K; ++k) {
+    const int root = FindRoot(parent, k);
+    if (lowest[root] < 0) lowest[root] = k;
+    if (prior_term[k] >= 0) touched[k] = 1;
+    if (prior_term[k] >= 0 || k == gauge) anchored[root] = 1;
+  }
+  int* held = g.h_ints;
+  int held_count = 0;
+  for (int k = 0; k < K; ++k) {
+    const int root = FindRoot(parent, k);
+    held[k] = (k == gauge || !touched[k] || (!anchored[root] && lowest[root] == k)) ? 1 : 0;
+    held_count += held[k];
+  }
+
+  // row k: its prior, its constraints by id, the chain edges (k - 1, k) and (k, k + 1); the CSR row: the diagonal, then the other
+  // end of every constraint and chain edge in the same order
+  std::vector<int> off, adj;
+  ConstraintAdjacency(h, K, &off, &adj);
+  int* row_off = held + K;
+  int entries = 0, nnz = 0;
+  for (int k = 0; k < K; ++k) {
+    row_off[k] = entries;
+    const int binary = (off[k + 1] - off[k]) + (chain ? (k > 0) + (k + 1 < K) : 0);
+    entries += (prior_term[k] >= 0) + binary;
+    nnz += 1 + binary;
+  }
+  row_off[K] = entries;
+  int* row_terms = row_off + K + 1;
+  int* csr_off = row_terms + 2 * entries;
+  int* csr_col = csr_off + K + 1;
+  int e = 0, c = 0;
+  auto entry = [&](int term, int side, int col) {
+    row_terms[2 * e] = term;
+    row_terms[2 * e + 1] = side;
+    ++e;
+    if (col >= 0) csr_col[c++] = col;
+  };
+  for (int k = 0; k < K; ++k) {
+    csr_off[k] = c;
+    csr_col[c++] = k;
+    if (prior_term[k] >= 0) entry(prior_term[k], 0, -1);
+    for (int j = off[k]; j < off[k + 1]; ++j) {
+      const bba_pose_constraint& pc = cons[adj[j]].c;
+      const bool is_a = pc.keyframe_a == k;
+      entry(first_constraint + adj[j], is_a ? 0 : 1, is_a ? pc.keyframe_b : pc.keyframe_a);
+    }
+    if (chain && k > 0) entry(first_chain + k - 1, 1, k - 1);
+    if (chain && k + 1 < K) entry(first_chain + k, 0, k + 1);
+  }
+  csr_off[K] = c;
+  const size_t ints = static_cast<size_t>(csr_col + nnz - held);
+
+  const size_t M = static_cast<size_t>(h->cfg.max_keyframes);
+  if (T) BBA_CUDA(h, cudaMemcpyAsync(g.d_terms, g.h_terms, sizeof(PoseGraphTerm) * T, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemcpyAsync(g.d_ints, g.h_ints, sizeof(int) * ints, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemcpyAsync(g.d_poses, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemcpyAsync(g.d_poses + 7 * M, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemsetAsync(g.d_state, 0, sizeof(PoseGraphState), s));
+  PoseGraphArgs a{};
+  a.K = K;
+  a.term_count = T;
+  a.terms = g.d_terms;
+  a.blocks = reinterpret_cast<PoseGraphTermBlocks*>(g.d_doubles.get());
+  a.poses = g.d_poses;
+  a.prev = g.d_poses + 7 * M;
+  const int* d_ints = g.d_ints;
+  a.held = d_ints;
+  a.row_off = d_ints + (row_off - held);
+  a.row_terms = d_ints + (row_terms - held);
+  a.csr_off = d_ints + (csr_off - held);
+  a.csr_col = d_ints + (csr_col - held);
+  double* d = g.d_doubles.get() + static_cast<size_t>(T) * (sizeof(PoseGraphTermBlocks) / sizeof(double));
+  a.csr_val = d;
+  a.rhs = a.csr_val + 36 * static_cast<size_t>(nnz);
+  a.tri = a.rhs + 6 * static_cast<size_t>(K);
+  a.work = a.tri + 36 * static_cast<size_t>(K);
+  a.state = g.d_state;
+  a.max_iterations = max_iterations;
+  a.max_linear = 6 * (K - held_count);
+  for (int round = 0; round <= max_iterations; ++round) {
+    a.round = round;
+    BBA_LAUNCH(h, h->launches, LaunchPoseGraphRound, a, s);
+  }
+  BBA_CUDA(h, cudaMemcpyAsync(g.h_state, g.d_state, sizeof(PoseGraphState), cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaMemcpyAsync(poses, g.d_poses, sizeof(float) * 7 * K, cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  for (int k = 0; k < K; ++k)
+    if (!held[k]) h->keyframes[k].pose = PoseFromArray(poses + 7 * k);
+  const PoseGraphState& st = *g.h_state.get();
+  r.iterations = st.iterations;
+  r.converged = st.converged;
+  r.linear_iterations = st.linear_iterations;
+  r.held_keyframes = held_count;
+  r.initial_cost = st.initial_cost;
+  r.final_cost = st.cost;
+  if (result) *result = r;
+  return Publish(h, s, false);
+}
+
 }  // namespace
 }  // namespace bba
 
@@ -929,6 +1128,10 @@ bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream) {
 bba_status bba_deform_surfels(bba_handle h, int count, const float* original_keyframe_T_global, uint32_t* moved, uint32_t* unobserved,
                               void* stream) {
   return DeformSurfels(h, count, original_keyframe_T_global, moved, unobserved, static_cast<cudaStream_t>(stream));
+}
+
+bba_status bba_optimize_pose_graph(bba_handle h, const bba_pose_graph_options* options, bba_pose_graph_result* result, void* stream) {
+  return OptimizePoseGraph(h, options, result, static_cast<cudaStream_t>(stream));
 }
 
 bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth, int optimize_color, void* stream) {

@@ -2,7 +2,7 @@
 // memory, events and textures, the keyframe record, error reporting and the helpers that more than one unit calls.
 //
 // Host units: badba.cu (handle, setters / getters, keyframes, textures, bba_host_*), pose_step.cu (spatial order, pose step),
-// bundle_adjust.cu (BA schemes, intrinsics, PCG, surfel lifecycle), multi_gpu.cu (sharding, exchange, peer replicas),
+// bundle_adjust.cu (BA schemes, intrinsics, PCG, surfel lifecycle, pose graph), multi_gpu.cu (sharding, exchange, peer replicas),
 // frames.cu (odometry, preprocessing).  None of them contains a kernel.
 #pragma once
 
@@ -286,6 +286,21 @@ struct bba_context {
     bba::DeviceBuffer<unsigned int> d_counts;   // [2] moved, unobserved
     bba::PinnedBuffer<unsigned int> h_counts;
   } deform;
+
+  // keyframe pose graph (bba_optimize_pose_graph): the terms, the held flags, the row lists and the block-CSR structure (one pinned
+  // staging buffer of ints and its device copy), the fp32 poses and the state; the terms' blocks, H, b, M and the solver's work in
+  // one fp64 buffer.  Sized for max_keyframes and the constraints, with room to double the constraints (ReservePoseGraph).
+  struct PoseGraph {
+    bba::PinnedBuffer<bba::PoseGraphTerm> h_terms;
+    bba::DeviceBuffer<bba::PoseGraphTerm> d_terms;
+    bba::PinnedBuffer<int> h_ints;
+    bba::DeviceBuffer<int> d_ints;
+    bba::PinnedBuffer<float> h_poses;        // [max_kf][7]
+    bba::DeviceBuffer<float> d_poses;        // [2][max_kf][7]: the poses, then the poses before the last step
+    bba::DeviceBuffer<double> d_doubles;
+    bba::DeviceBuffer<bba::PoseGraphState> d_state;
+    bba::PinnedBuffer<bba::PoseGraphState> h_state;
+  } graph;
 
   // in-loop surfel lifecycle (creation / merge / compaction) and the end tasks
   struct Lifecycle {

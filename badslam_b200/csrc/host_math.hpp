@@ -468,6 +468,40 @@ BBA_HD void PosePriorTerms(const float prior[7], const float pose[7], const floa
   InformationTerms<6>(r, J, info, H, b, cost);
 }
 
+// Whether the symmetric 6x6 matrix with upper triangle info is positive semi-definite up to fp32 rounding: the pivoted LDLT of
+// SolveLDLT (largest |diagonal| first) has no negative pivot, and a zero pivot leaves nothing in its column.  Host only: the test of
+// every information matrix a caller passes (priors, constraints, the pose graph's odometry chain).
+inline bool InformationPsd(const float info[21]) {
+  double M[36];
+  double scale = 0.0;
+  int idx = 0;
+  for (int r = 0; r < 6; ++r)
+    for (int c = r; c < 6; ++c) {
+      M[r * 6 + c] = M[c * 6 + r] = info[idx++];
+      scale = fmax(scale, fabs(static_cast<double>(info[idx - 1])));
+    }
+  if (scale == 0.0) return true;
+  const double pivot_tol = 1e-6 * scale, column_tol = 1e-3 * scale;
+  bool done[6] = {};
+  for (int k = 0; k < 6; ++k) {
+    int p = -1;
+    for (int i = 0; i < 6; ++i)
+      if (!done[i] && (p < 0 || fabs(M[i * 6 + i]) > fabs(M[p * 6 + p]))) p = i;
+    done[p] = true;
+    const double d = M[p * 6 + p];
+    if (d < -pivot_tol) return false;
+    if (d <= pivot_tol) {
+      for (int i = 0; i < 6; ++i)
+        if (!done[i] && fabs(M[i * 6 + p]) > column_tol) return false;
+      continue;
+    }
+    for (int i = 0; i < 6; ++i)
+      for (int j = 0; j < 6; ++j)
+        if (!done[i] && !done[j]) M[i * 6 + j] -= M[i * 6 + p] * M[p * 6 + j] / d;
+  }
+  return true;
+}
+
 // ---- soft relative pose constraint between two keyframes (bba_add_keyframe_pose_constraints) ----
 // The constraint's terms at global_T_frame = pose_a, pose_b, for the updates pose_a * exp(delta_a), pose_b * exp(delta_b): with
 // r = log(Z^-1 pose_a^-1 pose_b), Z = a_T_b, J_b = Jr^-1(r) and J_a = -Jr^-1(r) Ad(pose_b^-1 pose_a), and J = [J_a | J_b]:

@@ -118,6 +118,59 @@ struct PoseSolveArgs {
 // Device-side Gauss-Newton step for every keyframe in the list (direct_ba_alternating.cc:173-233).
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
 
+// Keyframe pose graph (pose_graph.cu; bba_optimize_pose_graph, DESIGN §3.14).  One term of the cost: a soft pose prior on
+// keyframe a (b = -1, z = the prior's global_T_frame), or a relative pose constraint (a, b, z = a_T_b): a handle constraint
+// or an odometry-chain edge of the call.  info: the upper triangle of L.
+struct PoseGraphTerm {
+  int a, b;
+  float z[7];
+  float info[21];
+};
+// A term's linearisation at the current poses (host_math.hpp PosePriorTerms / PoseConstraintTerms): H's upper triangle (21 of
+// a prior, 78 of a constraint over (delta_a, delta_b)), b = J^T L r (6 or 12) and the cost.
+struct PoseGraphTermBlocks {
+  double H[78];
+  double b[12];
+  double cost;
+};
+// The Gauss-Newton loop's state on the device.  Every kernel returns at once when done is set.
+struct PoseGraphState {
+  double initial_cost;   // at the poses the call starts from
+  double cost;           // at the poses of the last accepted step
+  int done;
+  int iterations;        // Gauss-Newton iterations that solved a linear system
+  int converged;
+  int linear_iterations; // PCG iterations, summed
+};
+struct PoseGraphArgs {
+  int K;                         // keyframes (row blocks)
+  int term_count;
+  const PoseGraphTerm* terms;    // [term_count]: priors, constraints by id, then the odometry chain
+  PoseGraphTermBlocks* blocks;   // [term_count]
+  float* poses;                  // [K][7] global_T_frame, updated in place
+  float* prev;                   // [K][7] the poses before the last step (a rejected step reverts to them)
+  const int* held;               // [K] 1: the keyframe keeps its pose (an identity row of H)
+  const int* row_off;            // [K + 1] into row_terms
+  const int* row_terms;          // [2 per entry] (term, side 0 = a / 1 = b): the terms of row block k in term order
+  const int* csr_off;            // [K + 1] block-CSR of H: row k's blocks [csr_off[k], csr_off[k + 1]), the diagonal first,
+  const int* csr_col;            //   then one block per constraint term of the row in term order
+  double* csr_val;               // [nnz][36] row-major
+  double* rhs;                   // [K][6] b
+  double* tri;                   // [K][36] H_{k,k+1}: the upper coupling of the block-tridiagonal preconditioner M
+  double* work;                  // the cyclic reduction's levels and the PCG vectors (PoseGraphWorkDoubles)
+  PoseGraphState* state;
+  int max_iterations;            // Gauss-Newton iterations
+  int max_linear;                // PCG iterations per linear solve
+  int round;                     // 0 .. max_iterations: the round of this launch
+};
+// The doubles of PoseGraphArgs::work for K keyframes: the reduction's levels (at most 2K + 32 blocks of six 6x6 matrices and
+// three 6-vectors) and five PCG vectors of K blocks.
+inline size_t PoseGraphWorkDoubles(size_t K) { return (2 * K + 32) * (6 * 36 + 3 * 6) + 5 * 6 * K; }
+// One round of a Gauss-Newton iteration, four launches: linearise every term, assemble H / b / M per row block, solve (the cost
+// test of the last step, then PCG with the block-tridiagonal preconditioner factorised by cyclic reduction, one CTA), and
+// T <- T exp(delta).  round == max_iterations launches the first three only (the test of the last step).
+LaunchResult LaunchPoseGraphRound(const PoseGraphArgs& a, cudaStream_t stream);
+
 // Replicas of the surfel buffer / active flags on the OTHER ranks of a one-process-per-GPU job, mapped into this process
 // (CUDA IPC) and written directly over NVLink by the geometry kernels: the owner of a surfel stores its updated rows into
 // every replica, so the "all-gather" of the geometry step is fused into the kernels' own final stores.

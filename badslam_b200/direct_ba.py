@@ -577,6 +577,26 @@ class DirectBA:
         L = np.array([list(recs[i].information) for i in range(n)], np.float32).reshape(n, 21)
         return ids[:n], a, b, Z, L
 
+    def OptimizePoseGraph(self, add_current_state_odometry_constraints=True, gauge_keyframe=0, max_iterations=20,
+                          odometry_information=None, stream=None) -> dict:
+        """bba_optimize_pose_graph (the reference's PoseGraphOptimizer, here on the device): Gauss-Newton over the keyframe poses
+        with the priors, the constraints and -- with add_current_state_odometry_constraints -- one edge per consecutive pair of
+        keyframes at their current relative pose, information odometry_information ([21] upper triangle or [6, 6]; None:
+        identity).  gauge_keyframe (-1: none) keeps its pose, as do untouched keyframes and the lowest id of every component
+        without the gauge or a prior.  Returns the result as a dict (iterations, converged, linear_iterations, held_keyframes,
+        initial_cost, final_cost).  Synchronises the stream."""
+        o = _lib.PoseGraphOptions()
+        o.gauge_keyframe = int(gauge_keyframe)
+        o.max_iterations = int(max_iterations)
+        o.use_odometry_chain = int(bool(add_current_state_odometry_constraints))
+        L = np.eye(6, dtype=np.float32) if odometry_information is None else np.asarray(odometry_information, np.float32)
+        if L.shape == (6, 6):
+            L = L[np.triu_indices(6)]
+        o.odometry_information[:] = [float(v) for v in L.reshape(21)]
+        r = _lib.PoseGraphResult()
+        self._check(self._lib.bba_optimize_pose_graph(self._h, C.byref(o), C.byref(r), self._stream_ptr(stream)))
+        return {name: getattr(r, name) for name, _ in _lib.PoseGraphResult._fields_}
+
     # -- trajectory deformation around a BA call (trajectory_deformation.h:43-58) ----------------------------------------
     def RememberKeyframePoses(self) -> np.ndarray:
         """RememberKeyframePoses (trajectory_deformation.cc:33-42): frame_T_global of every keyframe, [K, 7], all from one

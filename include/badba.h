@@ -366,6 +366,44 @@ bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream);
  * or an empty map: nothing to do.  A BA-side call. */
 bba_status bba_deform_surfels(bba_handle h, int count, const float* original_keyframe_T_global, uint32_t* moved, uint32_t* unobserved,
                               void* stream);
+/* Optimises the keyframe pose graph on the device (DESIGN.md §3.14): what the reference's PoseGraphOptimizer
+ * (pose_graph_optimizer.cc, g2o + CSparse, called from loop_detector.cc after a loop closure) does, over the handle's own pose
+ * terms.  It minimises over the keyframe poses
+ *   sum_priors 1/2 r^T L r + sum_constraints 1/2 r^T L r + sum_chain 1/2 r^T L_o r
+ * with the priors and constraints of bba_set_keyframe_pose_priors / bba_add_keyframe_pose_constraints (the pose-only terms of the
+ * BA cost) and, with use_odometry_chain, one edge (k, k + 1) per consecutive pair of keyframe ids whose Z = T_k^-1 T_{k+1} is taken
+ * at the poses the call starts from (fp64, rounded to fp32) and whose L is odometry_information (the reference's
+ * add_current_state_odometry_constraints).  The chain lives for the call only.  A loop edge is a constraint added first; it stays
+ * on the handle for the BA that follows (remove it afterwards for the reference's throw-away edge).
+ * Held keyframes keep their poses bit for bit: gauge_keyframe (-1: none; 0 in a zero-initialised struct, the reference's "vertex
+ * 0 fixed"), every keyframe that no term touches, and in every connected component of the edges (constraints and chain) with
+ * neither the gauge nor a prior, its lowest id.  Every other keyframe is an unknown, whatever its activation.
+ * Gauss-Newton as in the reference: at the current poses H delta = -b (the PCG scheme's update T <- T exp(delta)) is solved by
+ * PCG to a relative residual of 1e-10 (at most 6 x unknowns iterations), with the block-tridiagonal part of H in keyframe order
+ * as its preconditioner; a step that raises the cost is taken back and ends the call; the call stops after max_iterations (<= 0:
+ * 20, the reference's kMaxIterations) or when every component of a step is at most 1e-7, or 2^-19 of its pose's scale (1 for a
+ * rotation, max(1, |t|_inf) for a translation) when that is larger: the resolution of fp32 poses (converged; that step is not
+ * applied).
+ * Poses stay fp32 between iterations; linearisation and solve run in fp64.  No float atomics: the result is bit-identical from
+ * run to run, in the deterministic mode or not, and on every rank (each rank solves the whole graph; there is no exchange).
+ * The free keyframes' poses are written back and published once; activations, priors, constraints, surfels, co-visibility and
+ * the spatial order are not touched.  Synchronises the stream once.  result (may be NULL): Gauss-Newton iterations that solved a
+ * system, converged, the PCG iterations summed, the held keyframes, and the cost at the start and at the end (never above it).
+ * BBA_ERR_INVALID_ARGUMENT: a NULL options, a gauge outside [-1, keyframe count), or use_odometry_chain with a non-finite
+ * odometry_information or one that is not positive semi-definite (the test of bba_set_keyframe_pose_priors); checked before
+ * anything is enqueued, and a refused call changes nothing.  Fewer than two keyframes and no prior: nothing to do, a zero
+ * result.  A BA-side call. */
+typedef struct {
+  int gauge_keyframe;              /* -1: none */
+  int max_iterations;              /* <= 0: 20 */
+  int use_odometry_chain;
+  float odometry_information[21];  /* L_o's upper triangle, row-major (translation, then rotation) */
+} bba_pose_graph_options;
+typedef struct {
+  int iterations, converged, linear_iterations, held_keyframes;
+  double initial_cost, final_cost;
+} bba_pose_graph_result;
+bba_status bba_optimize_pose_graph(bba_handle h, const bba_pose_graph_options* options, bba_pose_graph_result* result, void* stream);
 /* DirectBA::PerformBASchemeEndTasks (direct_ba.cc:566-653): DeleteSurfelsAndUpdateRadiiCUDA over every keyframe (surfels
  * with fewer than GetMinObservationCount() observations, or more free-space violations than observations, are deleted; the
  * others get the smallest observed radius) + CompactSurfelsCUDA.  bba_bundle_adjust runs it like the reference does: at

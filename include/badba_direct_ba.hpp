@@ -374,6 +374,22 @@ class DirectBA {
     Check(bba_remove_keyframe_pose_constraints(h_, ids.empty() ? -1 : static_cast<int>(ids.size()), ids.data()),
           "bba_remove_keyframe_pose_constraints");
   }
+  // The keyframe pose graph (bba_optimize_pose_graph; the reference's PoseGraphOptimizer, here on the device): Gauss-Newton over
+  // the priors, the constraints and, with add_current_state_odometry_constraints, one edge per consecutive pair of keyframes at
+  // their current relative pose with `information` (identity when null).  The defaults are the reference's: vertex 0 fixed, 20
+  // iterations.  Synchronises the stream.
+  bba_pose_graph_result OptimizePoseGraph(cudaStream_t stream, bool add_current_state_odometry_constraints = true, int gauge_keyframe = 0,
+                                          int max_iterations = 20, const float (*information)[21] = nullptr) {
+    bba_pose_graph_options o{};
+    o.gauge_keyframe = gauge_keyframe;
+    o.max_iterations = max_iterations;
+    o.use_odometry_chain = add_current_state_odometry_constraints ? 1 : 0;
+    for (int i = 0, idx = 0; i < 6; ++i)
+      for (int j = i; j < 6; ++j, ++idx) o.odometry_information[idx] = information ? (*information)[idx] : (i == j ? 1.f : 0.f);
+    bba_pose_graph_result r{};
+    Check(bba_optimize_pose_graph(h_, &o, &r, stream), "bba_optimize_pose_graph");
+    return r;
+  }
   uint32_t surfels_size() const { return bba_surfels_size(h_); }   // direct_ba.h:265
   void GetIntrinsics(float depth[4], float color[4], float* a) const { Check(bba_get_intrinsics(h_, depth, color, a), "bba_get_intrinsics"); }
   void SetPCGGaugeKeyframe(int keyframe_id) { pcg_gauge_keyframe_ = keyframe_id; }
