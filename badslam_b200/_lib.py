@@ -15,6 +15,7 @@ ABI_VERSION = 10   # BBA_ABI_VERSION of the include/badba.h this binding types
 
 # bba_pose_variant: the pose kernel's instantiations (surfel tile, precomputed per-surfel frames)
 POSE_VARIANT_AUTO, POSE_VARIANT_256_PRE, POSE_VARIANT_512_PRE, POSE_VARIANT_256, POSE_VARIANT_512, POSE_VARIANT_1024 = range(6)
+GEOMETRY_PASS_AUTO, GEOMETRY_PASS_SPLIT, GEOMETRY_PASS_ONE = range(3)
 
 OK, ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_STATE, ERR_UNSUPPORTED, ERR_NO_DEVICE = range(6)
 STATUS_NAMES = {0: "BBA_OK", 1: "BBA_ERR_INVALID_ARGUMENT", 2: "BBA_ERR_CUDA", 3: "BBA_ERR_STATE",
@@ -193,6 +194,7 @@ SYMBOLS = {
     "bba_accumulate_pose_coeffs": (C.c_int, [_P, C.c_int, _F7, C.POINTER(PoseCoeffs), _P]),
     "bba_debug_pose_coeffs_batch": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "bba_debug_set_pose_group": (C.c_int, [_P, C.c_int]),
+    "bba_debug_set_geometry_pass": (C.c_int, [_P, C.c_int, C.c_int]),
     "bba_estimate_frame_pose": (C.c_int, [_P, C.c_int, _F7, _F7, C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_estimate_frame_pose_for_frame": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _F7, _F7,
                                                     C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),

@@ -804,6 +804,12 @@ bba_status BundleAdjustPCG(bba_handle h, const bba_ba_options* o, bba_ba_result*
   return EndBundleAdjust(h, o, launches_before, res, s);
 }
 
+// Whether the normals and the position / descriptor update of g run as one tile-major launch (bba::LaunchGeometryPass) rather than
+// the two group-major ones: whenever the keyframe records fit, unless bba_debug_set_geometry_pass asks for the two launches.
+bool OneGeometryPass(bba_handle h, const bba::GeometryArgs& g) {
+  return h->geo.pass != BBA_GEOMETRY_PASS_SPLIT && bba::GeometryPassFits(g);
+}
+
 // The standalone geometry passes over every keyframe that is not inactive, in spatial order: the surfel activation
 // (bba_update_surfel_activation), or the normals and then the positions and descriptors (bba_optimize_geometry_iteration).
 bba_status GeometryPass(bba_handle h, bool activation, cudaStream_t s) {
@@ -814,8 +820,13 @@ bba_status GeometryPass(bba_handle h, bool activation, cudaStream_t s) {
   bba::GeometryArgs g;
   if (bba_status st = BuildGeometryArgs(h, &g, s, GeoOrder::kSpatial)) return st;
   if (bba_status st = CheckCollective(h)) return st;
-  BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g, h->sm_count, activation, !activation, s);
-  if (!activation) BBA_LAUNCH(h, h->launches, LaunchPositionAndDescriptor, g, h->sm_count, s);
+  if (!activation && OneGeometryPass(h, g)) {
+    BBA_LAUNCH(h, h->launches, LaunchGeometryStream, g, g.cam.use_desc, s);
+    BBA_LAUNCH(h, h->launches, LaunchGeometryPass, g, h->sm_count, false, h->geo.pass_tile_shift, s);
+  } else {
+    BBA_LAUNCH(h, h->launches, LaunchActivationAndNormals, g, h->sm_count, activation, !activation, s);
+    if (!activation) BBA_LAUNCH(h, h->launches, LaunchPositionAndDescriptor, g, h->sm_count, s);
+  }
   if (bba_status st = ExchangeGeometry(h, s)) return st;
   return MarkStaging(h, s);
 }
@@ -1142,6 +1153,17 @@ bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth, int optimiz
   return OptimizeIntrinsics(h, optimize_depth != 0, optimize_color != 0, static_cast<cudaStream_t>(stream));
 }
 
+bba_status bba_debug_set_geometry_pass(bba_handle h, int pass, int tile_shift) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (pass < BBA_GEOMETRY_PASS_AUTO || pass > BBA_GEOMETRY_PASS_ONE)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_set_geometry_pass: unknown pass");
+  if (tile_shift != 0 && (tile_shift < 5 || tile_shift > 8))
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_set_geometry_pass: tile_shift out of range (0, 5 .. 8)");
+  h->geo.pass = pass;
+  h->geo.pass_tile_shift = tile_shift;
+  return BBA_OK;
+}
+
 bba_status bba_debug_intrinsics_coeffs(bba_handle h, int optimize_depth, int optimize_color, double* sums, float* cells, void* stream) {
   if (!h) return BBA_ERR_INVALID_ARGUMENT;
   if (!sums || !cells) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_debug_intrinsics_coeffs: null argument");
@@ -1219,13 +1241,18 @@ bba_status BundleAdjust(bba_handle h, const bba_ba_options* o, bba_ba_result* re
     if (bba_status st = BuildGeometryArgs(h, &g, s, has_new ? GeoOrder::kCaller : GeoOrder::kByPairs)) return st;
 
     BBA_TRACE("after creation + upload");
-    // --- surfel activation (:432-456) fused with the normal update of the geometry step (:466-485)
+    // --- surfel activation (:432-456) fused with the normal update of the geometry step (:466-485), and the position /
+    // descriptor update (:487-489).  Without new surfels all of it is one launch after the stream gather (OneGeometryPass); the
+    // events then split the gather (ms_surfel_activation) from that launch (ms_geometry_optimization).
+    const bool one_pass = o->optimize_geometry && !has_new && h->surfels_size > 0 && OneGeometryPass(h, g);
     BBA_CUDA(h, cudaEventRecord(h->ev[0], s));
     if (has_new)   // new surfels are active (:435-441); only the old ones are re-evaluated below
       BBA_CUDA(h, cudaMemsetAsync(h->active + old_surfels_size, bba::kSurfelActiveFlag, h->surfels_size - old_surfels_size, s));
     if (!whole_window) BBA_CUDA(h, cudaMemsetAsync(h->active, bba::kSurfelActiveFlag, old_surfels_size, s));
     if (h->surfels_size > 0) {
-      if (whole_window && has_new) {
+      if (one_pass) {
+        BBA_LAUNCH(h, h->launches, LaunchGeometryStream, g, g.cam.use_desc, s);
+      } else if (whole_window && has_new) {
         bba::GeometryArgs g_old = g, g_new = g;   // (begin / end are LOCAL indices of this rank's shard)
         g_old.end = LocalCountBelow(old_surfels_size, h->cfg.rank, h->cfg.world_size);
         g_new.begin = g_old.end;
@@ -1238,7 +1265,8 @@ bba_status BundleAdjust(bba_handle h, const bba_ba_options* o, bba_ba_result* re
       }
     }
     BBA_CUDA(h, cudaEventRecord(h->ev[1], s));
-    if (o->optimize_geometry && h->surfels_size > 0) BBA_LAUNCH(h, h->launches, LaunchPositionAndDescriptor, g, h->sm_count, s);
+    if (one_pass) BBA_LAUNCH(h, h->launches, LaunchGeometryPass, g, h->sm_count, whole_window, h->geo.pass_tile_shift, s);
+    else if (o->optimize_geometry && h->surfels_size > 0) BBA_LAUNCH(h, h->launches, LaunchPositionAndDescriptor, g, h->sm_count, s);
     if (bba_status st = ExchangeGeometry(h, s)) return st;   // multi-GPU: all-gather of the updated surfel shards
     BBA_CUDA(h, cudaEventRecord(h->ev[2], s));
     if (bba_status st = MarkStaging(h, s)) return st;
@@ -1308,7 +1336,7 @@ bba_status BundleAdjust(bba_handle h, const bba_ba_options* o, bba_ba_result* re
     if (h->profiling) {
       h->profile.activation_normals_ms += res->ms_surfel_activation;
       h->profile.position_descriptor_ms += res->ms_geometry_optimization;
-      h->profile.geometry_launches += (o->optimize_geometry ? 2 : 1);
+      h->profile.geometry_launches += one_pass ? 1 : (o->optimize_geometry ? 2 : 1);
     }
 
     if (StopIterating(o, iteration, num_converged, K, t_start, res)) break;   // :693-709

@@ -266,6 +266,8 @@ struct bba_context {
     bba::PinnedBuffer<int> h_list;
     bba::DeviceBuffer<unsigned int> d_queue;        // work-item counter of the geometry kernels
     bba::DeviceBuffer<unsigned int> d_tile_epoch;   // per-tile group epochs of the geometry kernels
+    int pass = BBA_GEOMETRY_PASS_AUTO;   // bba_debug_set_geometry_pass
+    int pass_tile_shift = 0;             // 0: the launcher's choice
     const uint32_t* perm = nullptr;   // the order of the last geometry launches (pose.order's perm or null), for ExchangeGeometry
     // intrinsics step: [head 64 | B 5P | D P | b2 P | obs P | x1 8] floats + 34 fp64 sums
     bba::DeviceBuffer<float> d_intr;

@@ -217,6 +217,13 @@ LaunchResult LaunchActivationAndNormals(const GeometryArgs& args, int sm_count, 
                                         cudaStream_t stream);
 // Position (+ descriptor) accumulation and per-surfel solve (kernel_opt_geometry.cu:118-231,273-361 or :417-507).
 LaunchResult LaunchPositionAndDescriptor(const GeometryArgs& args, int sm_count, cudaStream_t stream);
+// The two launches above in one tile-major pass (GeometryPassKernel): activation (determine_activation) and normals, then position
+// and descriptors, with the same results bit for bit.  Every keyframe record of the launch is staged in each CTA's shared memory,
+// so it takes at most kGeoPassMaxKeyframes keyframes (GeometryPassFits).  The caller gathers the geometry stream first
+// (LaunchGeometryStream, desc_rows = cam.use_desc).  tile_shift: log2 of the surfels per work item, 5..8; 0: the launcher's choice.
+constexpr int kGeoPassMaxKeyframes = 512;   // 48 KB of records, and one visibility word per lane
+inline bool GeometryPassFits(const GeometryArgs& args) { return args.kf_count > 0 && args.kf_count <= kGeoPassMaxKeyframes; }
+LaunchResult LaunchGeometryPass(const GeometryArgs& args, int sm_count, bool determine_activation, int tile_shift, cudaStream_t stream);
 
 // Surfel deformation after an outside pose correction (bba_deform_surfels, DESIGN §3.13).  Per keyframe: D = global_T_frame (now)
 // * original frame_T_global, row-major 3x4 from old global coordinates to new ones, and the original camera centre.

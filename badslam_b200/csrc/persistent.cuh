@@ -187,5 +187,15 @@ inline uint32_t EpochOrderedGrid(int per_sm, int sm_count, int threads, uint32_t
 inline uint32_t ItemGrid(int per_sm, int sm_count, uint64_t n_items) {
   return static_cast<uint32_t>(std::min<uint64_t>((n_items + 7) / 8, static_cast<uint64_t>(std::max(per_sm, 1)) * sm_count));
 }
+// Tile-major kernels (one item per tile, every keyframe inside it): 32-surfel tiles, one warp sub-step each, unless a tile of
+// 2^forced_shift surfels (5..8) is asked for; the shift goes to *tile_shift.  The cost of a tile varies with how many keyframes
+// see it, and the smallest tiles even that out best in the tail: on cfg3 GeometryPassKernel took 5.22 ms at 32 surfels, 5.47 at
+// 64, 6.24 at 128 and 7.45 at 256 (DESIGN §7.1).
+constexpr int kTileMajorShift = 5;
+inline uint32_t TileGrid(int per_sm, int sm_count, uint32_t n, int forced_shift, int* tile_shift) {
+  const int shift = forced_shift >= 5 && forced_shift <= 8 ? forced_shift : kTileMajorShift;
+  *tile_shift = shift;
+  return ItemGrid(per_sm, sm_count, (static_cast<uint64_t>(n) + (1u << shift) - 1) >> shift);
+}
 
 }  // namespace bba

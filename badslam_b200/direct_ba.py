@@ -683,6 +683,11 @@ class DirectBA:
         """bba_debug_set_pose_group: keyframes per staged surfel tile in every later pose-kernel launch (0: the library's choice)."""
         self._check(self._lib.bba_debug_set_pose_group(self._h, int(keyframes)))
 
+    def DebugSetGeometryPass(self, pass_: int, tile_shift: int = 0):
+        """bba_debug_set_geometry_pass: 0 (auto) / 2 (one tile-major launch when the keyframes fit) or 1 (the two group-major launches)
+        for the normal and position / descriptor updates of every later geometry step; tile_shift 5..8 (0: the library's choice)."""
+        self._check(self._lib.bba_debug_set_geometry_pass(self._h, int(pass_), int(tile_shift)))
+
     def EstimateFramePose(self, stream, global_T_frame_initial_estimate, keyframe_id: int):
         """direct_ba.h:122-129; returns (global_T_frame_estimate, iterations, converged)."""
         p = np.ascontiguousarray(global_T_frame_initial_estimate, np.float32)

@@ -304,6 +304,13 @@ bba_status bba_debug_pose_coeffs_batch(bba_handle h, int count, const int* keyfr
  * default: the library's choice).  The results do not depend on it beyond the order of the default mode's floating-point
  * sums; in the deterministic mode they are the same bits.  For tests and timing. */
 bba_status bba_debug_set_pose_group(bba_handle h, int keyframes);
+/* Chooses how every later geometry step without new surfels (bba_bundle_adjust's alternating iterations,
+ * bba_optimize_geometry_iteration) runs its normal and position / descriptor updates: AUTO (the default) and ONE run them in one
+ * tile-major launch whenever the non-inactive keyframes number 1 .. 512, SPLIT always in the two group-major launches.  tile_shift:
+ * log2 of the surfels per work item of the one launch, 5 .. 8; 0: the library's choice.  The results are the same bits in every
+ * mode.  For tests and timing. */
+typedef enum { BBA_GEOMETRY_PASS_AUTO = 0, BBA_GEOMETRY_PASS_SPLIT = 1, BBA_GEOMETRY_PASS_ONE = 2 } bba_geometry_pass;
+bba_status bba_debug_set_geometry_pass(bba_handle h, int pass, int tile_shift);
 /* DirectBA::EstimateFramePose (direct_ba.h:122-129, direct_ba_alternating.cc:42-283) against a stored keyframe's
  * images.  iterations/converged may be NULL. */
 bba_status bba_estimate_frame_pose(bba_handle h, int keyframe_id, const float global_T_frame_initial[7],
