@@ -93,6 +93,10 @@ class PoseConstraint(C.Structure):   # bba_pose_constraint
     _fields_ = [("keyframe_a", C.c_int), ("keyframe_b", C.c_int), ("a_T_b", C.c_float * 7), ("information", C.c_float * 21)]
 
 
+class RobustLoss(C.Structure):   # bba_robust_loss
+    _fields_ = [("type", C.c_int), ("scale", C.c_float)]
+
+
 class PoseGraphOptions(C.Structure):   # bba_pose_graph_options
     _fields_ = [("gauge_keyframe", C.c_int), ("max_iterations", C.c_int), ("use_odometry_chain", C.c_int),
                 ("odometry_information", C.c_float * 21)]
@@ -170,6 +174,11 @@ SYMBOLS = {
     "bba_add_keyframe_pose_constraints": (C.c_int, [_P, C.c_int, _P, _P]),
     "bba_remove_keyframe_pose_constraints": (C.c_int, [_P, C.c_int, _P]),
     "bba_get_keyframe_pose_constraints": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
+    "bba_set_keyframe_pose_prior_losses": (C.c_int, [_P, C.c_int, _P, _P]),
+    "bba_set_keyframe_pose_constraint_losses": (C.c_int, [_P, C.c_int, _P, _P]),
+    "bba_get_keyframe_pose_prior_loss": (C.c_int, [_P, C.c_int, C.POINTER(RobustLoss)]),
+    "bba_get_keyframe_pose_constraint_losses": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
+    "bba_evaluate_keyframe_pose_terms": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, _P, _P, _P]),
     "bba_set_intrinsics": (C.c_int, [_P, _F7, _F7, C.c_float]),
     "bba_get_intrinsics": (C.c_int, [_P, _F7, _F7, C.POINTER(C.c_float)]),
     "bba_host_se3_exp": (None, [_P, _P]),
@@ -180,6 +189,7 @@ SYMBOLS = {
     "bba_host_solve_ldlt": (C.c_int, [C.c_int, _P, _P, _P]),
     "bba_host_pose_prior_terms": (None, [_P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_pose_constraint_terms": (None, [_P, _P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
+    "bba_host_robust_loss": (None, [C.c_int, C.c_float, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "bba_host_frusta_intersect": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, C.c_float, _P, C.c_float, C.c_float]),
     "bba_host_motion_model_clear": (None, [C.POINTER(MotionModelRecord), _P, _P]),
     "bba_host_motion_model_predict": (C.c_int, [C.POINTER(MotionModelRecord), C.c_int, _P, _P]),

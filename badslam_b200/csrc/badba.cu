@@ -105,6 +105,7 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
     v.min_depth = kf.min_depth; v.max_depth = kf.max_depth;
     v.activation = kf.activation;
     v.prior = h->pose_priors[k];
+    v.prior_loss = h->pose_prior_losses[k];
   }
   const CameraView cams = LiveCameraView(h);
   std::vector<PoseConstraint> constraints = h->pose_constraints;
@@ -354,6 +355,7 @@ bba_status bba_create(const bba_config* cfg, bba_handle* out) {
   CREATE_TRY(cudaMemset(h->d_cfactor, 0, sizeof(float) * h->cf_w * h->cf_h));
   CREATE_TRY(h->d_kfs.Reserve(K));
   h->pose_priors.assign(K, bba::PosePrior{});
+  h->pose_prior_losses.assign(K, bba_robust_loss{});
   CREATE_TRY(p.d_work_records.Reserve(K));
   CREATE_TRY(p.d_pose_est.Reserve(7 * K));
   CREATE_TRY(p.d_acc.Reserve(bba::kPoseAccSize * K));
@@ -579,6 +581,10 @@ void bba_host_pose_constraint_terms(const float a_T_b[7], const float pose_a[7],
   double r[6];
   bba::PoseConstraintTerms(a_T_b, pose_a, pose_b, info, r, H, b, cost);
 }
+void bba_host_robust_loss(int type, float scale, double s, double* rho, double* weight) {
+  if (!rho || !weight) return;
+  bba::RobustLoss(type, scale, s, rho, weight);
+}
 int bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height, const float global_T_frame_a[7], float min_depth_a,
                               float max_depth_a, const float global_T_frame_b[7], float min_depth_b, float max_depth_b) {
   Frustum a, b;
@@ -797,6 +803,12 @@ bba_status CommitPosePriors(bba_handle h) {
   return Publish(h, nullptr, false);
 }
 
+// The test of a robust loss a caller passes: a known type, and for HUBER / CAUCHY a finite scale > 0.
+bool RobustLossValid(const bba_robust_loss& l) {
+  if (l.type == BBA_LOSS_TRIVIAL) return true;
+  return (l.type == BBA_LOSS_HUBER || l.type == BBA_LOSS_CAUCHY) && std::isfinite(l.scale) && l.scale > 0.f;
+}
+
 bool PoseRecordFinite(const float* pose, const float* info) {
   bool finite = true;
   for (int j = 0; j < 7; ++j) finite = finite && std::isfinite(pose[j]);
@@ -836,13 +848,17 @@ bba_status bba_clear_keyframe_pose_priors(bba_handle h, int count, const int* id
   const int K = static_cast<int>(h->keyframes.size());
   if (count == -1) {
     std::fill(h->pose_priors.begin(), h->pose_priors.end(), PosePrior{});
+    std::fill(h->pose_prior_losses.begin(), h->pose_prior_losses.end(), bba_robust_loss{});
     return CommitPosePriors(h);
   }
   if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < -1");
   if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
   for (int i = 0; i < count; ++i)
     if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
-  for (int i = 0; i < count; ++i) h->pose_priors[ids[i]] = PosePrior{};
+  for (int i = 0; i < count; ++i) {
+    h->pose_priors[ids[i]] = PosePrior{};
+    h->pose_prior_losses[ids[i]] = bba_robust_loss{};
+  }
   return CommitPosePriors(h);
 }
 
@@ -858,6 +874,33 @@ bba_status bba_get_keyframe_pose_prior(bba_handle h, int id, float pose[7], floa
   *has_prior = p.has;
   if (pose) std::memcpy(pose, p.pose, sizeof(p.pose));
   if (information) std::memcpy(information, p.info, sizeof(p.info));
+  return BBA_OK;
+}
+
+bba_status bba_set_keyframe_pose_prior_losses(bba_handle h, int count, const int* ids, const bba_robust_loss* losses) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_set_keyframe_pose_prior_losses: ";
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
+  if (count > 0 && (!ids || !losses)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  const int K = static_cast<int>(h->keyframes.size());
+  for (int i = 0; i < count; ++i) {
+    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
+    if (!h->pose_priors[ids[i]].has) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "keyframe has no prior");
+    if (!RobustLossValid(losses[i])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown loss type or bad scale");
+  }
+  for (int i = 0; i < count; ++i) h->pose_prior_losses[ids[i]] = losses[i];
+  return Publish(h, nullptr, false);
+}
+
+bba_status bba_get_keyframe_pose_prior_loss(bba_handle h, int id, bba_robust_loss* out) {
+  FrontEndScope front_end;
+  if (!h || !out) return BBA_ERR_INVALID_ARGUMENT;
+  std::unique_lock<std::mutex> lock(h->fe.mu);
+  if (id < 0 || id >= static_cast<int>(h->fe.kfs.size())) {
+    lock.unlock();
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bad keyframe id");
+  }
+  *out = h->fe.kfs[id].prior_loss;
   return BBA_OK;
 }
 
@@ -928,6 +971,38 @@ bba_status bba_get_keyframe_pose_constraints(bba_handle h, int capacity, int* id
   for (int i = 0; i < n; ++i) {
     if (ids) ids[i] = cons[i].id;
     if (out) out[i] = cons[i].c;
+  }
+  return BBA_OK;
+}
+
+bba_status bba_set_keyframe_pose_constraint_losses(bba_handle h, int count, const int* ids, const bba_robust_loss* losses) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_set_keyframe_pose_constraint_losses: ";
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
+  if (count > 0 && (!ids || !losses)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  auto& cons = h->pose_constraints;
+  std::vector<size_t> at(count);
+  for (int i = 0; i < count; ++i) {
+    auto it = std::lower_bound(cons.begin(), cons.end(), ids[i], [](const PoseConstraint& c, int id) { return c.id < id; });
+    if (it == cons.end() || it->id != ids[i]) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown constraint id");
+    if (!RobustLossValid(losses[i])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown loss type or bad scale");
+    at[i] = static_cast<size_t>(it - cons.begin());
+  }
+  for (int i = 0; i < count; ++i) cons[at[i]].loss = losses[i];
+  return Publish(h, nullptr, false);
+}
+
+bba_status bba_get_keyframe_pose_constraint_losses(bba_handle h, int capacity, int* ids, bba_robust_loss* out, int* count) {
+  FrontEndScope front_end;
+  if (!h || !count) return BBA_ERR_INVALID_ARGUMENT;
+  if (capacity < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_get_keyframe_pose_constraint_losses: capacity < 0");
+  std::lock_guard<std::mutex> lock(h->fe.mu);
+  const std::vector<PoseConstraint>& cons = h->fe.constraints;
+  *count = static_cast<int>(cons.size());
+  const int n = std::min(capacity, *count);
+  for (int i = 0; i < n; ++i) {
+    if (ids) ids[i] = cons[i].id;
+    if (out) out[i] = cons[i].loss;
   }
   return BBA_OK;
 }

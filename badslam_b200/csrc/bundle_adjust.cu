@@ -534,7 +534,8 @@ bba::PcgArgs MakePcgArgs(bba_handle h, const PcgLayout& L, int gauge) {
 // The pose-block terms of the products at the poses the init pass sees, staged for LaunchPcgPoseTerms: a keyframe's prior and,
 // per constraint, H_aa / H_bb, H_ab and b_a / b_b of PoseConstraintTerms, gathered per pose block (every keyframe but the
 // gauge) in the order prior, then constraints by id.  An edge to the gauge keeps only its other end's diagonal terms (p_gauge = 0).
-// fp64, rounded to fp32.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.
+// Every term's H and b are scaled by its robust weight at these poses (one IRLS step per outer iteration; w = 1 exactly for a
+// trivial loss).  fp64, rounded to fp32.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.
 bba_status StagePcgPoseTerms(bba_handle h, const PcgLayout& L, int gauge, cudaStream_t s) {
   auto& pc = h->pcg;
   pc.pose_blocks = 0;
@@ -551,6 +552,11 @@ bba_status StagePcgPoseTerms(bba_handle h, const PcgLayout& L, int gauge, cudaSt
     const bba_pose_constraint& c = h->pose_constraints[i].c;
     double r[6], H[78], b[12], cost;
     PoseConstraintTerms(c.a_T_b, poses.data() + 7 * c.keyframe_a, poses.data() + 7 * c.keyframe_b, c.information, r, H, b, &cost);
+    const bba_robust_loss& loss = h->pose_constraints[i].loss;
+    double rho, w;
+    RobustLoss(loss.type, loss.scale, 2.0 * cost, &rho, &w);
+    for (double& v : H) v *= w;
+    for (double& v : b) v *= w;
     auto upper = [&](int row, int col) { return H[row * 12 - row * (row - 1) / 2 + (col - row)]; };
     bba::PcgPoseTerm& ta = edge[2 * i];
     bba::PcgPoseTerm& tb = edge[2 * i + 1];
@@ -583,8 +589,11 @@ bba_status StagePcgPoseTerms(bba_handle h, const PcgLayout& L, int gauge, cudaSt
       t.other = -1;
       double H[21], b[6], cost;
       bba::PosePriorTerms(prior.pose, poses.data() + 7 * k, prior.info, H, b, &cost);
-      for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(H[j]);
-      for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(b[j]);
+      const bba_robust_loss& loss = h->pose_prior_losses[k];
+      double rho, w;
+      RobustLoss(loss.type, loss.scale, 2.0 * cost, &rho, &w);
+      for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(w * H[j]);
+      for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(w * b[j]);
     }
     for (int e = off[k]; e < off[k + 1]; ++e) {
       const int i = adj[e];
@@ -944,6 +953,10 @@ bba_status ReservePoseGraph(bba_handle h, size_t constraints) {
   BBA_CUDA(h, g.d_terms.Reserve(need.terms, alloc.terms));
   BBA_CUDA(h, g.h_ints.Reserve(need.ints, alloc.ints));
   BBA_CUDA(h, g.d_ints.Reserve(need.ints, alloc.ints));
+  BBA_CUDA(h, g.h_losses.Reserve(need.terms, alloc.terms));
+  BBA_CUDA(h, g.d_losses.Reserve(need.terms, alloc.terms));
+  BBA_CUDA(h, g.h_eval.Reserve(2 * need.terms, 2 * alloc.terms));
+  BBA_CUDA(h, g.d_eval.Reserve(2 * need.terms, 2 * alloc.terms));
   BBA_CUDA(h, g.d_doubles.Reserve(need.doubles, alloc.doubles));
   BBA_CUDA(h, g.h_poses.Reserve(7 * M));
   BBA_CUDA(h, g.d_poses.Reserve(14 * M));
@@ -955,6 +968,46 @@ bba_status ReservePoseGraph(bba_handle h, size_t constraints) {
 int FindRoot(std::vector<int>& parent, int k) {
   while (parent[k] != k) k = parent[k] = parent[parent[k]];
   return k;
+}
+
+// The pose graph's terms in h->graph.h_terms at the keyframe poses `poses`: the priors (prior_term[k]: keyframe k's term, or -1),
+// the constraints by id from *first_constraint, then with odometry_information the odometry chain from *first_chain, whose Z are
+// taken at `poses`.  With losses, every term's loss goes to h_losses (the chain's TRIVIAL).  Returns the number of terms.
+int StagePoseGraphTerms(bba_handle h, const float* poses, const float* odometry_information, bool losses, std::vector<int>* prior_term,
+                        int* first_constraint, int* first_chain) {
+  auto& g = h->graph;
+  const int K = static_cast<int>(h->keyframes.size());
+  prior_term->assign(K, -1);
+  int T = 0;
+  auto add = [&](int a, int b, const float* z, const float* info, const bba_robust_loss& loss) {
+    if (losses) g.h_losses[T] = loss;
+    PoseGraphTerm& t = g.h_terms[T++];
+    t.a = a;
+    t.b = b;
+    std::memcpy(t.z, z, sizeof(t.z));
+    std::memcpy(t.info, info, sizeof(t.info));
+  };
+  for (int k = 0; k < K; ++k) {
+    const PosePrior& p = h->pose_priors[k];
+    if (!p.has) continue;
+    (*prior_term)[k] = T;
+    add(k, -1, p.pose, p.info, h->pose_prior_losses[k]);
+  }
+  *first_constraint = T;
+  for (const PoseConstraint& c : h->pose_constraints) add(c.c.keyframe_a, c.c.keyframe_b, c.c.a_T_b, c.c.information, c.loss);
+  *first_chain = T;
+  if (odometry_information)
+    for (int k = 0; k + 1 < K; ++k) {
+      double qa[4], ta[3], qb[4], tb[3], q[4], t[3];
+      LoadPoseD(poses + 7 * k, qa, ta);
+      LoadPoseD(poses + 7 * (k + 1), qb, tb);
+      Se3BetweenD(qa, ta, qb, tb, q, t);   // T_k^-1 T_{k+1}
+      float z[7];
+      for (int j = 0; j < 4; ++j) z[j] = static_cast<float>(q[j]);
+      for (int j = 0; j < 3; ++j) z[4 + j] = static_cast<float>(t[j]);
+      add(k, k + 1, z, odometry_information, bba_robust_loss{BBA_LOSS_TRIVIAL, 0.f});
+    }
+  return T;
 }
 
 bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_pose_graph_result* result, cudaStream_t s) {
@@ -982,35 +1035,11 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   // the terms: priors, constraints by id, then the chain at the poses the call starts from
   float* poses = g.h_poses;
   for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses + 7 * k);
-  std::vector<int> prior_term(K, -1);
-  int T = 0;
-  auto add = [&](int a, int b, const float* z, const float* info) {
-    PoseGraphTerm& t = g.h_terms[T++];
-    t.a = a;
-    t.b = b;
-    std::memcpy(t.z, z, sizeof(t.z));
-    std::memcpy(t.info, info, sizeof(t.info));
-  };
-  for (int k = 0; k < K; ++k) {
-    const PosePrior& p = h->pose_priors[k];
-    if (!p.has) continue;
-    prior_term[k] = T;
-    add(k, -1, p.pose, p.info);
-  }
-  const int first_constraint = T;
-  for (const PoseConstraint& c : cons) add(c.c.keyframe_a, c.c.keyframe_b, c.c.a_T_b, c.c.information);
-  const int first_chain = T;
-  if (chain)
-    for (int k = 0; k + 1 < K; ++k) {
-      double qa[4], ta[3], qb[4], tb[3], q[4], t[3];
-      LoadPoseD(poses + 7 * k, qa, ta);
-      LoadPoseD(poses + 7 * (k + 1), qb, tb);
-      Se3BetweenD(qa, ta, qb, tb, q, t);   // T_k^-1 T_{k+1}
-      float z[7];
-      for (int j = 0; j < 4; ++j) z[j] = static_cast<float>(q[j]);
-      for (int j = 0; j < 3; ++j) z[4 + j] = static_cast<float>(t[j]);
-      add(k, k + 1, z, o->odometry_information);
-    }
+  const bool robust = PoseLossesNonTrivial(h);
+  std::vector<int> prior_term;
+  int first_constraint = 0, first_chain = 0;
+  const int T = StagePoseGraphTerms(h, poses, chain ? o->odometry_information : nullptr, robust, &prior_term, &first_constraint,
+                                    &first_chain);
 
   // the held keyframes: the gauge, the untouched ones, and the lowest id of every component without the gauge or a prior
   std::vector<int> parent(K), lowest(K, -1);
@@ -1076,6 +1105,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
 
   const size_t M = static_cast<size_t>(h->cfg.max_keyframes);
   if (T) BBA_CUDA(h, cudaMemcpyAsync(g.d_terms, g.h_terms, sizeof(PoseGraphTerm) * T, cudaMemcpyHostToDevice, s));
+  if (T && robust) BBA_CUDA(h, cudaMemcpyAsync(g.d_losses, g.h_losses, sizeof(bba_robust_loss) * T, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemcpyAsync(g.d_ints, g.h_ints, sizeof(int) * ints, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemcpyAsync(g.d_poses, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemcpyAsync(g.d_poses + 7 * M, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
@@ -1101,6 +1131,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   a.state = g.d_state;
   a.max_iterations = max_iterations;
   a.max_linear = 6 * (K - held_count);
+  a.losses = robust ? g.d_losses.get() : nullptr;
   for (int round = 0; round <= max_iterations; ++round) {
     a.round = round;
     BBA_LAUNCH(h, h->launches, LaunchPoseGraphRound, a, s);
@@ -1119,6 +1150,54 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   r.final_cost = st.cost;
   if (result) *result = r;
   return Publish(h, s, false);
+}
+
+// bba_evaluate_keyframe_pose_terms: the pose graph's terms without the chain, linearised once by the robust instantiation at the
+// current poses, which writes every term's {s, w}.
+bba_status EvaluatePoseTerms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight, int constraint_capacity,
+                             double* constraint_s, double* constraint_weight, cudaStream_t s) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (keyframe_capacity < 0 || constraint_capacity < 0)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_evaluate_keyframe_pose_terms: negative capacity");
+  const int K = static_cast<int>(h->keyframes.size());
+  const std::vector<PoseConstraint>& cons = h->pose_constraints;
+  if (bba_status st = ReservePoseGraph(h, cons.size())) return st;
+  auto& g = h->graph;
+  float* poses = g.h_poses;
+  for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses + 7 * k);
+  std::vector<int> prior_term;
+  int first_constraint = 0, first_chain = 0;
+  const int T = StagePoseGraphTerms(h, poses, nullptr, /*losses=*/true, &prior_term, &first_constraint, &first_chain);
+  if (T) {
+    BBA_CUDA(h, cudaMemcpyAsync(g.d_terms, g.h_terms, sizeof(PoseGraphTerm) * T, cudaMemcpyHostToDevice, s));
+    BBA_CUDA(h, cudaMemcpyAsync(g.d_losses, g.h_losses, sizeof(bba_robust_loss) * T, cudaMemcpyHostToDevice, s));
+    BBA_CUDA(h, cudaMemcpyAsync(g.d_poses, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
+    BBA_CUDA(h, cudaMemsetAsync(g.d_state, 0, sizeof(PoseGraphState), s));
+    PoseGraphArgs a{};
+    a.K = K;
+    a.term_count = T;
+    a.terms = g.d_terms;
+    a.blocks = reinterpret_cast<PoseGraphTermBlocks*>(g.d_doubles.get());
+    a.poses = g.d_poses;
+    a.state = g.d_state;
+    a.losses = g.d_losses;
+    a.eval = g.d_eval;
+    BBA_LAUNCH(h, h->launches, LaunchPoseGraphEvaluate, a, s);
+    BBA_CUDA(h, cudaMemcpyAsync(g.h_eval, g.d_eval, sizeof(double) * 2 * T, cudaMemcpyDeviceToHost, s));
+    BBA_CUDA(h, cudaStreamSynchronize(s));
+  }
+  const double* ev = g.h_eval;
+  for (int k = 0; k < std::min(keyframe_capacity, K); ++k) {
+    const int t = prior_term[k];
+    if (prior_s) prior_s[k] = t >= 0 ? ev[2 * t] : std::nan("");
+    if (prior_weight) prior_weight[k] = t >= 0 ? ev[2 * t + 1] : std::nan("");
+  }
+  for (int i = 0; i < std::min(constraint_capacity, static_cast<int>(cons.size())); ++i) {
+    const int t = first_constraint + i;
+    if (constraint_s) constraint_s[i] = ev[2 * t];
+    if (constraint_weight) constraint_weight[i] = ev[2 * t + 1];
+  }
+  return BBA_OK;
 }
 
 }  // namespace
@@ -1143,6 +1222,12 @@ bba_status bba_deform_surfels(bba_handle h, int count, const float* original_key
 
 bba_status bba_optimize_pose_graph(bba_handle h, const bba_pose_graph_options* options, bba_pose_graph_result* result, void* stream) {
   return OptimizePoseGraph(h, options, result, static_cast<cudaStream_t>(stream));
+}
+
+bba_status bba_evaluate_keyframe_pose_terms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight,
+                                            int constraint_capacity, double* constraint_s, double* constraint_weight, void* stream) {
+  return EvaluatePoseTerms(h, keyframe_capacity, prior_s, prior_weight, constraint_capacity, constraint_s, constraint_weight,
+                           static_cast<cudaStream_t>(stream));
 }
 
 bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth, int optimize_color, void* stream) {

@@ -140,6 +140,7 @@ struct KeyframeView {
   float min_depth = 0.f, max_depth = 0.f;
   int activation = BBA_KF_ACTIVE;
   PosePrior prior{};
+  bba_robust_loss prior_loss{};
 };
 
 // A soft relative pose constraint as the handle keeps it: its id, the caller's record, and the information of the equivalent
@@ -148,6 +149,7 @@ struct PoseConstraint {
   int id;
   bba_pose_constraint c;
   float info_a[21];
+  bba_robust_loss loss;   // bba_set_keyframe_pose_constraint_losses; TRIVIAL when added
 };
 
 // The cameras, the depth deformation parameter a, the residual types and the deterministic mode as the BA side published them last.
@@ -196,6 +198,9 @@ struct bba_context {
   // constraint the pose solve and the PCG solver run without pose terms
   std::vector<bba::PosePrior> pose_priors;   // [max_kf]
   int pose_prior_count = 0;
+  // the priors' robust losses by keyframe id (bba_set_keyframe_pose_prior_losses): TRIVIAL until set, kept when a prior is
+  // replaced, reset when it is cleared.  A constraint's loss is PoseConstraint::loss.
+  std::vector<bba_robust_loss> pose_prior_losses;   // [max_kf]
   // soft relative pose constraints (bba_add_keyframe_pose_constraints) in id order, and the id the next one gets
   std::vector<bba::PoseConstraint> pose_constraints;
   int next_pose_constraint_id = 0;
@@ -242,6 +247,9 @@ struct bba_context {
     bba::DeviceBuffer<int> d_term_offsets;
     bba::PinnedBuffer<bba::PoseTerm> h_terms;
     bba::DeviceBuffer<bba::PoseTerm> d_terms;
+    // the terms' robust losses, parallel to h_terms; staged only when a prior or constraint has a non-trivial loss
+    bba::PinnedBuffer<bba_robust_loss> h_term_losses;
+    bba::DeviceBuffer<bba_robust_loss> d_term_losses;
     // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream); the
     // geometry step's stream (bba::LaunchGeometryStream) shares the buffer.
     // The order is rebuilt at the start of every BA call, after an in-loop change of the surfel set, and whenever the surfel
@@ -295,6 +303,11 @@ struct bba_context {
   struct PoseGraph {
     bba::PinnedBuffer<bba::PoseGraphTerm> h_terms;
     bba::DeviceBuffer<bba::PoseGraphTerm> d_terms;
+    // the terms' robust losses (the chain's trivial) and, for bba_evaluate_keyframe_pose_terms, every term's {s, w}
+    bba::PinnedBuffer<bba_robust_loss> h_losses;
+    bba::DeviceBuffer<bba_robust_loss> d_losses;
+    bba::PinnedBuffer<double> h_eval;
+    bba::DeviceBuffer<double> d_eval;
     bba::PinnedBuffer<int> h_ints;
     bba::DeviceBuffer<int> d_ints;
     bba::PinnedBuffer<float> h_poses;        // [max_kf][7]
@@ -564,6 +577,8 @@ bba_status ReservePoseTerms(bba_handle h, size_t constraints);
 // The soft relative pose constraints that touch each of the first K keyframes, in id order: indices into
 // h->pose_constraints, adj[off[k] .. off[k + 1]).
 void ConstraintAdjacency(bba_handle h, int K, std::vector<int>* off, std::vector<int>* adj);
+// Whether a prior or a constraint has a loss other than TRIVIAL: only then do the solvers run their robust instantiations.
+bool PoseLossesNonTrivial(bba_handle h);
 
 // multi_gpu.cu
 void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t* shard_len);

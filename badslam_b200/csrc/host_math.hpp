@@ -468,6 +468,24 @@ BBA_HD void PosePriorTerms(const float prior[7], const float pose[7], const floa
   InformationTerms<6>(r, J, info, H, b, cost);
 }
 
+// The robust loss of a pose term (bba_robust_loss, Ceres' conventions): a term whose squared Mahalanobis norm is s = r^T L r costs
+// rho(s) / 2 instead of s / 2, and IRLS scales its H and b by w = rho'(s).  type: 0 trivial (rho = s), 1 Huber, 2 Cauchy; scale =
+// delta in units of sqrt(s).  An inlier under Huber (s <= delta^2) gets rho = s and w = 1.0 exactly, as the trivial loss does.
+BBA_HD void RobustLoss(int type, float scale, double s, double* rho, double* w) {
+  const double d = scale, d2 = d * d;
+  if (type == 1 && s > d2) {
+    const double root = sqrt(s);
+    *rho = 2.0 * d * root - d2;
+    *w = d / root;
+  } else if (type == 2) {
+    *rho = d2 * log1p(s / d2);
+    *w = 1.0 / (1.0 + s / d2);
+  } else {
+    *rho = s;
+    *w = 1.0;
+  }
+}
+
 // Whether the symmetric 6x6 matrix with upper triangle info is positive semi-definite up to fp32 rounding: the pivoted LDLT of
 // SolveLDLT (largest |diagonal| first) has no negative pivot, and a zero pivot leaves nothing in its column.  Host only: the test of
 // every information matrix a caller passes (priors, constraints, the pose graph's odometry chain).

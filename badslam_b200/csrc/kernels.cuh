@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/badba.h"
 #include "device_math.cuh"
 #include "exact_sum.cuh"
 #include "launch.hpp"
@@ -114,6 +115,9 @@ struct PoseSolveArgs {
   // both null when no keyframe has one
   const int* term_offsets;     // [keyframes + 1]
   const PoseTerm* terms;
+  // the terms' robust losses, parallel to terms (host_math.hpp RobustLoss: a term's H and b are scaled by w at the current
+  // estimate); null when every loss is trivial, which runs the instantiation without them
+  const bba_robust_loss* term_losses;
 };
 // Device-side Gauss-Newton step for every keyframe in the list (direct_ba_alternating.cc:173-233).
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
@@ -162,6 +166,10 @@ struct PoseGraphArgs {
   int max_iterations;            // Gauss-Newton iterations
   int max_linear;                // PCG iterations per linear solve
   int round;                     // 0 .. max_iterations: the round of this launch
+  // the terms' robust losses (host_math.hpp RobustLoss: H and b scaled by w, the cost rho(s) / 2); null when every loss is
+  // trivial, which runs the linearisation without them
+  const bba_robust_loss* losses;   // [term_count]
+  double* eval;                    // null, or [term_count][2]: every term's {s, w} (bba_evaluate_keyframe_pose_terms)
 };
 // The doubles of PoseGraphArgs::work for K keyframes: the reduction's levels (at most 2K + 32 blocks of six 6x6 matrices and
 // three 6-vectors) and five PCG vectors of K blocks.
@@ -170,6 +178,8 @@ inline size_t PoseGraphWorkDoubles(size_t K) { return (2 * K + 32) * (6 * 36 + 3
 // test of the last step, then PCG with the block-tridiagonal preconditioner factorised by cyclic reduction, one CTA), and
 // T <- T exp(delta).  round == max_iterations launches the first three only (the test of the last step).
 LaunchResult LaunchPoseGraphRound(const PoseGraphArgs& a, cudaStream_t stream);
+// One launch of the robust linearisation with a.eval set: every term's {s, w} at a.poses (a.state->done must be 0).
+LaunchResult LaunchPoseGraphEvaluate(const PoseGraphArgs& a, cudaStream_t stream);
 
 // Replicas of the surfel buffer / active flags on the OTHER ranks of a one-process-per-GPU job, mapped into this process
 // (CUDA IPC) and written directly over NVLink by the geometry kernels: the owner of a surfel stores its updated rows into

@@ -3,7 +3,8 @@
 //
 // One Gauss-Newton iteration is one round of four kernels, and the host enqueues every round without synchronising: the state
 // (PoseGraphState) decides on the device whether the last step is kept, and once it is done every later kernel returns at once.
-//   PoseGraphLinearizeKernel  one thread per term: PosePriorTerms / PoseConstraintTerms at the fp32 poses, in fp64.
+//   PoseGraphLinearizeKernel  one thread per term: PosePriorTerms / PoseConstraintTerms at the fp32 poses, in fp64; with robust
+//                             losses (the ROBUST instantiation) scaled by the IRLS weight, the cost rho(s) / 2.
 //   PoseGraphAssembleKernel   one thread per row block: H_kk, b_k, the block-CSR row and the coupling H_{k,k+1}, summed over the
 //                             row's terms in term order.  A held keyframe's row is the identity with a zero right-hand side.
 //   PoseGraphSolveKernel      one CTA: the cost at the current poses (a fixed-order sum) and the test of the last step, then
@@ -175,6 +176,9 @@ __device__ double Dot(const double* a, const double* b, int n, double* sh) {
   return BlockSum(s, sh);
 }
 
+// ROBUST: the term's blocks are scaled by the weight of its loss (a.losses) at the current poses and its cost is rho(s) / 2; with
+// a.eval, {s, w} is written too.
+template <bool ROBUST>
 __global__ void __launch_bounds__(64) PoseGraphLinearizeKernel(const PoseGraphArgs a) {
   if (a.state->done) return;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -186,6 +190,20 @@ __global__ void __launch_bounds__(64) PoseGraphLinearizeKernel(const PoseGraphAr
   } else {
     double r[6];
     PoseConstraintTerms(term.z, a.poses + 7 * term.a, a.poses + 7 * term.b, term.info, r, blk.H, blk.b, &blk.cost);
+  }
+  if constexpr (ROBUST) {
+    const bba_robust_loss loss = a.losses[t];
+    const double s = 2.0 * blk.cost;
+    double rho, w;
+    RobustLoss(loss.type, loss.scale, s, &rho, &w);
+    const int nh = term.b < 0 ? 21 : 78, nb = term.b < 0 ? 6 : 12;
+    for (int i = 0; i < nh; ++i) blk.H[i] *= w;
+    for (int i = 0; i < nb; ++i) blk.b[i] *= w;
+    blk.cost = 0.5 * rho;
+    if (a.eval) {
+      a.eval[2 * t] = s;
+      a.eval[2 * t + 1] = w;
+    }
   }
 }
 
@@ -485,12 +503,19 @@ __global__ void __launch_bounds__(128) PoseGraphUpdateKernel(const PoseGraphArgs
 }  // namespace
 
 LaunchResult LaunchPoseGraphRound(const PoseGraphArgs& a, cudaStream_t stream) {
-  PoseGraphLinearizeKernel<<<(a.term_count + 63) / 64 > 0 ? (a.term_count + 63) / 64 : 1, 64, 0, stream>>>(a);
+  const int blocks = (a.term_count + 63) / 64 > 0 ? (a.term_count + 63) / 64 : 1;
+  if (a.losses) PoseGraphLinearizeKernel<true><<<blocks, 64, 0, stream>>>(a);
+  else PoseGraphLinearizeKernel<false><<<blocks, 64, 0, stream>>>(a);
   PoseGraphAssembleKernel<<<(a.K + 127) / 128, 128, 0, stream>>>(a);
   PoseGraphSolveKernel<<<1, kSolveThreads, 0, stream>>>(a);
   if (a.round >= a.max_iterations) return {3};
   PoseGraphUpdateKernel<<<(a.K + 127) / 128, 128, 0, stream>>>(a);
   return {4};
+}
+
+LaunchResult LaunchPoseGraphEvaluate(const PoseGraphArgs& a, cudaStream_t stream) {
+  PoseGraphLinearizeKernel<true><<<(a.term_count + 63) / 64 > 0 ? (a.term_count + 63) / 64 : 1, 64, 0, stream>>>(a);
+  return {1};
 }
 
 }  // namespace bba

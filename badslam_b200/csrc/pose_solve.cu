@@ -13,7 +13,8 @@
 namespace bba {
 
 // DET (the deterministic mode): the accumulator record is read from the keyframe's exact sums, rounded to fp64, instead of acc.
-template <bool DET>
+// ROBUST: every pose term's H and b are scaled by the weight of its loss (term_losses) at the current estimate.
+template <bool DET, bool ROBUST>
 __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
   __shared__ int next_count;
   __shared__ unsigned long long tot[5];
@@ -63,8 +64,16 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
         const PoseTerm& term = a.terms[t];
         double Hp[21], bp[6], cost;
         PosePriorTerms(term.pose, pe, term.info, Hp, bp, &cost);
-        for (int j = 0; j < 21; ++j) H[j] += Hp[j];
-        for (int j = 0; j < 6; ++j) b[j] += bp[j];
+        if constexpr (ROBUST) {
+          const bba_robust_loss loss = a.term_losses[t];
+          double rho, w;
+          RobustLoss(loss.type, loss.scale, 2.0 * cost, &rho, &w);
+          for (int j = 0; j < 21; ++j) H[j] += w * Hp[j];
+          for (int j = 0; j < 6; ++j) b[j] += w * bp[j];
+        } else {
+          for (int j = 0; j < 21; ++j) H[j] += Hp[j];
+          for (int j = 0; j < 6; ++j) b[j] += bp[j];
+        }
       }
     }
     SolveLDLT<6>(H, b, x);
@@ -105,8 +114,13 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
 }
 
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream) {
-  if (args.exact) PoseSolveKernel<true><<<1, 256, 0, stream>>>(args);
-  else PoseSolveKernel<false><<<1, 256, 0, stream>>>(args);
+  if (args.term_losses) {
+    if (args.exact) PoseSolveKernel<true, true><<<1, 256, 0, stream>>>(args);
+    else PoseSolveKernel<false, true><<<1, 256, 0, stream>>>(args);
+  } else {
+    if (args.exact) PoseSolveKernel<true, false><<<1, 256, 0, stream>>>(args);
+    else PoseSolveKernel<false, false><<<1, 256, 0, stream>>>(args);
+  }
   return {1};
 }
 

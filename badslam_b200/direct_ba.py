@@ -577,6 +577,64 @@ class DirectBA:
         L = np.array([list(recs[i].information) for i in range(n)], np.float32).reshape(n, 21)
         return ids[:n], a, b, Z, L
 
+    # -- robust losses on the priors and constraints (not in the reference; include/badba.h "Robust losses") ----------------
+    LOSS_TYPES = {"trivial": 0, "huber": 1, "cauchy": 2}
+
+    @classmethod
+    def _losses(cls, n, loss, scale):
+        """n bba_robust_loss records from a type name or number (one for all, or [n]) and scale(s)."""
+        types = [cls.LOSS_TYPES.get(t, t) if isinstance(t, str) else t for t in (loss if isinstance(loss, (list, tuple, np.ndarray)) else [loss] * n)]
+        scales = np.broadcast_to(np.asarray(scale, np.float32), (n,))
+        if len(types) != n:
+            raise ValueError("one loss per id")
+        recs = (_lib.RobustLoss * max(n, 1))()
+        for i in range(n):
+            recs[i].type, recs[i].scale = int(types[i]), float(scales[i])
+        return recs
+
+    def SetKeyframePosePriorLosses(self, ids, loss, scale=1.0):
+        """Gives the priors of keyframes `ids` a robust loss: "trivial", "huber" or "cauchy" (or BBA_LOSS_* numbers; one for all,
+        or one per id) with scale delta in units of sqrt(r^T L r).  Refused as a whole (nothing changes) for an unknown type, a
+        scale that is not finite and > 0, or a keyframe without a prior."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), np.int32)
+        self._check(self._lib.bba_set_keyframe_pose_prior_losses(self._h, len(ids), ids.ctypes.data, self._losses(len(ids), loss, scale)))
+
+    def KeyframePosePriorLoss(self, keyframe_id: int):
+        """(type, scale) of a keyframe's prior loss as last published."""
+        r = _lib.RobustLoss()
+        self._check(self._lib.bba_get_keyframe_pose_prior_loss(self._h, keyframe_id, C.byref(r)))
+        return r.type, r.scale
+
+    def SetKeyframePoseConstraintLosses(self, ids, loss, scale=1.0):
+        """Gives the constraints `ids` a robust loss (as SetKeyframePosePriorLosses); refused as a whole for an unknown id."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), np.int32)
+        self._check(self._lib.bba_set_keyframe_pose_constraint_losses(self._h, len(ids), ids.ctypes.data,
+                                                                      self._losses(len(ids), loss, scale)))
+
+    def GetKeyframePoseConstraintLosses(self):
+        """The constraints' losses as last published, in id order: (ids [n], types [n] int32, scales [n] float32)."""
+        count = C.c_int()
+        self._check(self._lib.bba_get_keyframe_pose_constraint_losses(self._h, 0, None, None, C.byref(count)))
+        n = count.value
+        ids = np.zeros(max(n, 1), np.int32)
+        recs = (_lib.RobustLoss * max(n, 1))()
+        self._check(self._lib.bba_get_keyframe_pose_constraint_losses(self._h, n, ids.ctypes.data, recs, C.byref(count)))
+        n = min(n, count.value)
+        return ids[:n], np.array([recs[i].type for i in range(n)], np.int32), np.array([recs[i].scale for i in range(n)], np.float32)
+
+    def EvaluateKeyframePoseTerms(self, stream=None) -> dict:
+        """s = r^T L r and the robust weight w of every term at the current poses, evaluated on the device: prior_s /
+        prior_weight [keyframes] (NaN without a prior), constraint_ids / constraint_s / constraint_weight [constraints] in id
+        order.  A constraint that a robust pose graph rejected has w near 0.  Synchronises the stream."""
+        K = self._lib.bba_keyframe_count(self._h)
+        ids = self.GetKeyframePoseConstraintLosses()[0]
+        n = len(ids)
+        ps, pw = np.zeros(max(K, 1)), np.zeros(max(K, 1))
+        cs, cw = np.zeros(max(n, 1)), np.zeros(max(n, 1))
+        self._check(self._lib.bba_evaluate_keyframe_pose_terms(self._h, K, ps.ctypes.data, pw.ctypes.data, n, cs.ctypes.data,
+                                                               cw.ctypes.data, self._stream_ptr(stream)))
+        return {"prior_s": ps[:K], "prior_weight": pw[:K], "constraint_ids": ids, "constraint_s": cs[:n], "constraint_weight": cw[:n]}
+
     def OptimizePoseGraph(self, add_current_state_odometry_constraints=True, gauge_keyframe=0, max_iterations=20,
                           odometry_information=None, stream=None) -> dict:
         """bba_optimize_pose_graph (the reference's PoseGraphOptimizer, here on the device): Gauss-Newton over the keyframe poses

@@ -259,6 +259,47 @@ typedef struct {
 bba_status bba_add_keyframe_pose_constraints(bba_handle h, int count, const bba_pose_constraint* constraints, int* out_ids);
 bba_status bba_remove_keyframe_pose_constraints(bba_handle h, int count, const int* ids);
 bba_status bba_get_keyframe_pose_constraints(bba_handle h, int capacity, int* ids, bba_pose_constraint* out, int* count);
+/* Robust losses on the pose terms (not in the reference; the robust kernels of g2o / Ceres / GTSAM edges): a prior or constraint
+ * whose squared Mahalanobis norm is s = r^T L r costs 1/2 rho(s) instead of 1/2 s, with Ceres' rho (scipy's least_squares with
+ * f_scale = scale):
+ *   TRIVIAL  rho = s                                             w = 1            (the default)
+ *   HUBER    rho = s for s <= scale^2, else 2 scale sqrt(s) - scale^2   w = 1, else scale / sqrt(s)
+ *   CAUCHY   rho = scale^2 ln(1 + s / scale^2)                   w = 1 / (1 + s / scale^2)
+ * The solvers linearise it by IRLS (g2o's first-order robustification, no second-order correction): a term's H and b are scaled by
+ * w = rho'(s) at the poses where it is linearised -- every Gauss-Newton iteration of the pose step of the alternating scheme and
+ * bba_estimate_frame_pose (a constraint's equivalent prior by its own s, which is the constraint's with the other end at its start
+ * pose; a damping anchor by its constraint's w at the start poses), once per outer iteration of the PCG scheme, and every iteration
+ * of bba_optimize_pose_graph, whose costs (initial_cost, final_cost and the test of a step) become the robust cost.  The odometry
+ * chain of the pose graph stays trivial.  A handle whose losses are all trivial runs exactly the code it ran before losses existed;
+ * an inlier under Huber (s <= scale^2) has w = 1 exactly.  With several ranks every rank makes the same calls.
+ *  bba_set_keyframe_pose_prior_losses: the losses of the priors of keyframe_ids [count].  A prior keeps its loss when
+ *    bba_set_keyframe_pose_priors replaces it; bba_clear_keyframe_pose_priors resets it to TRIVIAL.
+ *  bba_set_keyframe_pose_constraint_losses: the losses of constraint_ids [count].  A new constraint starts TRIVIAL; removing it
+ *    drops its loss.
+ *  Both are BA-side calls and publish.  BBA_ERR_INVALID_ARGUMENT for an unknown type, a scale that is not finite and > 0 for HUBER
+ *  or CAUCHY (scale is ignored for TRIVIAL), a keyframe without a prior, or an unknown constraint id; the arguments are checked
+ *  before anything changes, and a refused call changes nothing.
+ *  bba_get_keyframe_pose_prior_loss: front-end call (the published loss; TRIVIAL without a prior).
+ *  bba_get_keyframe_pose_constraint_losses: front-end call (the published constraints in id order, as
+ *    bba_get_keyframe_pose_constraints): *count = their number; at most capacity of them are written to ids / out (either may be
+ *    NULL). */
+typedef enum { BBA_LOSS_TRIVIAL = 0, BBA_LOSS_HUBER = 1, BBA_LOSS_CAUCHY = 2 } bba_loss_type;
+typedef struct {
+  int type;      /* bba_loss_type */
+  float scale;   /* delta, in units of sqrt(r^T L r); ignored for TRIVIAL */
+} bba_robust_loss;
+bba_status bba_set_keyframe_pose_prior_losses(bba_handle h, int count, const int* keyframe_ids, const bba_robust_loss* losses);
+bba_status bba_set_keyframe_pose_constraint_losses(bba_handle h, int count, const int* constraint_ids, const bba_robust_loss* losses);
+bba_status bba_get_keyframe_pose_prior_loss(bba_handle h, int keyframe_id, bba_robust_loss* out);
+bba_status bba_get_keyframe_pose_constraint_losses(bba_handle h, int capacity, int* ids, bba_robust_loss* out, int* count);
+/* s and w of every prior and constraint at the current keyframe poses, evaluated on the device with the pose graph's term
+ * evaluation (one launch, no odometry chain): how a caller finds the constraints a robust bba_optimize_pose_graph rejected
+ * (w near 0) and removes them before the BA.  Prior arrays are indexed by keyframe id over min(keyframe_capacity, keyframe count)
+ * entries (NaN where a keyframe has no prior); constraint arrays follow the id order of bba_get_keyframe_pose_constraints over
+ * min(constraint_capacity, constraint count) entries.  Any array may be NULL.  BBA_ERR_INVALID_ARGUMENT: a negative capacity.  A
+ * BA-side call; changes nothing on the handle; synchronises the stream. */
+bba_status bba_evaluate_keyframe_pose_terms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight,
+                                            int constraint_capacity, double* constraint_s, double* constraint_weight, void* stream);
 
 /* depth_params_ / cameras (direct_ba.h:243-297; SetColorCamera etc.).  The getters bba_get_intrinsics, bba_get_residual_types,
  * bba_get_cfactor_host and bba_cfactor_size are front-end calls (the published cameras, a, residual types and cfactor; the
@@ -770,6 +811,9 @@ void bba_host_pose_prior_terms(const float prior_global_T_frame[7], const float 
  * Writes nothing if a pointer is NULL. */
 void bba_host_pose_constraint_terms(const float a_T_b[7], const float global_T_a[7], const float global_T_b[7],
                                     const float information[21], double H[78], double b[12], double* cost);
+/* The robust loss of a pose term (bba_robust_loss) at s = r^T L r: *rho = rho(s) and *weight = rho'(s), in fp64, as the solvers
+ * evaluate them.  An unknown type counts as TRIVIAL.  Writes nothing if a pointer is NULL. */
+void bba_host_robust_loss(int type, float scale, double s, double* rho, double* weight);
 int  bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height,
                                const float global_T_frame_a[7], float min_depth_a, float max_depth_a,
                                const float global_T_frame_b[7], float min_depth_b, float max_depth_b);

@@ -374,6 +374,31 @@ class DirectBA {
     Check(bba_remove_keyframe_pose_constraints(h_, ids.empty() ? -1 : static_cast<int>(ids.size()), ids.data()),
           "bba_remove_keyframe_pose_constraints");
   }
+  // Robust losses (not in the reference; badba.h): the prior of keyframe_id, or constraint `id`, costs 1/2 rho(r^T L r) with
+  // rho of type (BBA_LOSS_TRIVIAL / HUBER / CAUCHY) and scale delta in units of sqrt(r^T L r).
+  void SetKeyframePosePriorLoss(int keyframe_id, int type, float scale) {
+    const bba_robust_loss loss{type, scale};
+    Check(bba_set_keyframe_pose_prior_losses(h_, 1, &keyframe_id, &loss), "bba_set_keyframe_pose_prior_losses");
+  }
+  void SetKeyframePoseConstraintLoss(int id, int type, float scale) {
+    const bba_robust_loss loss{type, scale};
+    Check(bba_set_keyframe_pose_constraint_losses(h_, 1, &id, &loss), "bba_set_keyframe_pose_constraint_losses");
+  }
+  // s = r^T L r and the robust weight of every prior (indexed by keyframe id, NaN without a prior) and constraint (in id order)
+  // at the current poses; a loop closure that a robust pose graph rejected has a weight near 0.  Synchronises the stream.
+  void EvaluateKeyframePoseTerms(cudaStream_t stream, std::vector<double>* prior_s, std::vector<double>* prior_weight,
+                                 std::vector<double>* constraint_s, std::vector<double>* constraint_weight) {
+    int constraints = 0;
+    Check(bba_get_keyframe_pose_constraints(h_, 0, nullptr, nullptr, &constraints), "bba_get_keyframe_pose_constraints");
+    const int K = bba_keyframe_count(h_);
+    prior_s->resize(K);
+    prior_weight->resize(K);
+    constraint_s->resize(constraints);
+    constraint_weight->resize(constraints);
+    Check(bba_evaluate_keyframe_pose_terms(h_, K, prior_s->data(), prior_weight->data(), constraints, constraint_s->data(),
+                                           constraint_weight->data(), stream),
+          "bba_evaluate_keyframe_pose_terms");
+  }
   // The keyframe pose graph (bba_optimize_pose_graph; the reference's PoseGraphOptimizer, here on the device): Gauss-Newton over
   // the priors, the constraints and, with add_current_state_odometry_constraints, one edge per consecutive pair of keyframes at
   // their current relative pose with `information` (identity when null).  The defaults are the reference's: vertex 0 fixed, 20
