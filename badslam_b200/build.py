@@ -31,6 +31,7 @@ UNITS = [
     ("exact_sum.cu", ["-Xptxas", "-v"]),
     ("badba.cu", []),
     ("pose_step.cu", []),
+    ("pose_terms.cu", []),
     ("bundle_adjust.cu", []),
     ("multi_gpu.cu", []),
     ("local_group.cu", ["-Xptxas", "-v"]),   # (the all-reduce sums keep denormals: no -use_fast_math)

@@ -105,7 +105,6 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
     v.min_depth = kf.min_depth; v.max_depth = kf.max_depth;
     v.activation = kf.activation;
     v.prior = h->pose_priors[k];
-    v.prior_loss = h->pose_prior_losses[k];
   }
   const CameraView cams = LiveCameraView(h);
   std::vector<PoseConstraint> constraints = h->pose_constraints;
@@ -355,7 +354,6 @@ bba_status bba_create(const bba_config* cfg, bba_handle* out) {
   CREATE_TRY(cudaMemset(h->d_cfactor, 0, sizeof(float) * h->cf_w * h->cf_h));
   CREATE_TRY(h->d_kfs.Reserve(K));
   h->pose_priors.assign(K, bba::PosePrior{});
-  h->pose_prior_losses.assign(K, bba_robust_loss{});
   CREATE_TRY(p.d_work_records.Reserve(K));
   CREATE_TRY(p.d_pose_est.Reserve(7 * K));
   CREATE_TRY(p.d_acc.Reserve(bba::kPoseAccSize * K));
@@ -793,220 +791,6 @@ bba_status bba_get_keyframe_states(bba_handle h, int count, float* poses, int* a
   }
   return BBA_OK;
 }
-// ---- soft pose priors ----
-namespace {
-// Counts the priors and publishes the records.
-bba_status CommitPosePriors(bba_handle h) {
-  int count = 0;
-  for (const PosePrior& p : h->pose_priors) count += p.has ? 1 : 0;
-  h->pose_prior_count = count;
-  return Publish(h, nullptr, false);
-}
-
-// The test of a robust loss a caller passes: a known type, and for HUBER / CAUCHY a finite scale > 0.
-bool RobustLossValid(const bba_robust_loss& l) {
-  if (l.type == BBA_LOSS_TRIVIAL) return true;
-  return (l.type == BBA_LOSS_HUBER || l.type == BBA_LOSS_CAUCHY) && std::isfinite(l.scale) && l.scale > 0.f;
-}
-
-bool PoseRecordFinite(const float* pose, const float* info) {
-  bool finite = true;
-  for (int j = 0; j < 7; ++j) finite = finite && std::isfinite(pose[j]);
-  for (int j = 0; j < 21; ++j) finite = finite && std::isfinite(info[j]);
-  return finite;
-}
-}  // namespace
-
-bba_status bba_set_keyframe_pose_priors(bba_handle h, int count, const int* ids, const float* poses, const float* information) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_set_keyframe_pose_priors: ";
-  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
-  if (count > 0 && (!ids || !poses || !information)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  const int K = static_cast<int>(h->keyframes.size());
-  for (int i = 0; i < count; ++i) {
-    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
-    const float* p = poses + 7 * static_cast<size_t>(i);
-    const float* info = information + 21 * static_cast<size_t>(i);
-    if (!PoseRecordFinite(p, info)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose or information");
-    if (p[0] * p[0] + p[1] * p[1] + p[2] * p[2] + p[3] * p[3] < 1e-12f) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "zero quaternion");
-    if (!InformationPsd(info)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information matrix is not positive semi-definite");
-  }
-  if (count > 0)
-    if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size())) return st;
-  for (int i = 0; i < count; ++i) {
-    PosePrior& r = h->pose_priors[ids[i]];
-    std::memcpy(r.pose, poses + 7 * static_cast<size_t>(i), sizeof(r.pose));
-    std::memcpy(r.info, information + 21 * static_cast<size_t>(i), sizeof(r.info));
-    r.has = 1;
-  }
-  return CommitPosePriors(h);
-}
-
-bba_status bba_clear_keyframe_pose_priors(bba_handle h, int count, const int* ids) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_clear_keyframe_pose_priors: ";
-  const int K = static_cast<int>(h->keyframes.size());
-  if (count == -1) {
-    std::fill(h->pose_priors.begin(), h->pose_priors.end(), PosePrior{});
-    std::fill(h->pose_prior_losses.begin(), h->pose_prior_losses.end(), bba_robust_loss{});
-    return CommitPosePriors(h);
-  }
-  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < -1");
-  if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  for (int i = 0; i < count; ++i)
-    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
-  for (int i = 0; i < count; ++i) {
-    h->pose_priors[ids[i]] = PosePrior{};
-    h->pose_prior_losses[ids[i]] = bba_robust_loss{};
-  }
-  return CommitPosePriors(h);
-}
-
-bba_status bba_get_keyframe_pose_prior(bba_handle h, int id, float pose[7], float information[21], int* has_prior) {
-  FrontEndScope front_end;
-  if (!h || !has_prior) return BBA_ERR_INVALID_ARGUMENT;
-  std::unique_lock<std::mutex> lock(h->fe.mu);
-  if (id < 0 || id >= static_cast<int>(h->fe.kfs.size())) {
-    lock.unlock();
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bad keyframe id");
-  }
-  const PosePrior& p = h->fe.kfs[id].prior;
-  *has_prior = p.has;
-  if (pose) std::memcpy(pose, p.pose, sizeof(p.pose));
-  if (information) std::memcpy(information, p.info, sizeof(p.info));
-  return BBA_OK;
-}
-
-bba_status bba_set_keyframe_pose_prior_losses(bba_handle h, int count, const int* ids, const bba_robust_loss* losses) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_set_keyframe_pose_prior_losses: ";
-  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
-  if (count > 0 && (!ids || !losses)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  const int K = static_cast<int>(h->keyframes.size());
-  for (int i = 0; i < count; ++i) {
-    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
-    if (!h->pose_priors[ids[i]].has) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "keyframe has no prior");
-    if (!RobustLossValid(losses[i])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown loss type or bad scale");
-  }
-  for (int i = 0; i < count; ++i) h->pose_prior_losses[ids[i]] = losses[i];
-  return Publish(h, nullptr, false);
-}
-
-bba_status bba_get_keyframe_pose_prior_loss(bba_handle h, int id, bba_robust_loss* out) {
-  FrontEndScope front_end;
-  if (!h || !out) return BBA_ERR_INVALID_ARGUMENT;
-  std::unique_lock<std::mutex> lock(h->fe.mu);
-  if (id < 0 || id >= static_cast<int>(h->fe.kfs.size())) {
-    lock.unlock();
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bad keyframe id");
-  }
-  *out = h->fe.kfs[id].prior_loss;
-  return BBA_OK;
-}
-
-// ---- soft relative pose constraints ----
-bba_status bba_add_keyframe_pose_constraints(bba_handle h, int count, const bba_pose_constraint* constraints, int* out_ids) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_add_keyframe_pose_constraints: ";
-  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
-  if (count > 0 && !constraints) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  const int K = static_cast<int>(h->keyframes.size());
-  for (int i = 0; i < count; ++i) {
-    const bba_pose_constraint& c = constraints[i];
-    if (c.keyframe_a < 0 || c.keyframe_a >= K || c.keyframe_b < 0 || c.keyframe_b >= K)
-      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
-    if (c.keyframe_a == c.keyframe_b) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "keyframe_a == keyframe_b");
-    if (!PoseRecordFinite(c.a_T_b, c.information)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose or information");
-    const float* q = c.a_T_b;
-    if (q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] < 1e-12f) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "zero quaternion");
-    if (!InformationPsd(c.information)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information matrix is not positive semi-definite");
-  }
-  if (count == 0) return BBA_OK;
-  if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size() + count)) return st;
-  for (int i = 0; i < count; ++i) {
-    PoseConstraint r{};
-    r.id = h->next_pose_constraint_id++;
-    r.c = constraints[i];
-    double info_a[21];
-    PoseConstraintInformationA(r.c.a_T_b, r.c.information, info_a);
-    for (int j = 0; j < 21; ++j) r.info_a[j] = static_cast<float>(info_a[j]);
-    h->pose_constraints.push_back(r);
-    if (out_ids) out_ids[i] = r.id;
-  }
-  return Publish(h, nullptr, false);
-}
-
-bba_status bba_remove_keyframe_pose_constraints(bba_handle h, int count, const int* ids) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_remove_keyframe_pose_constraints: ";
-  auto& cons = h->pose_constraints;
-  if (count == -1) {
-    cons.clear();
-    return Publish(h, nullptr, false);
-  }
-  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < -1");
-  if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  std::vector<char> drop(cons.size(), 0);
-  for (int i = 0; i < count; ++i) {
-    // ids increase along the list
-    auto it = std::lower_bound(cons.begin(), cons.end(), ids[i], [](const PoseConstraint& c, int id) { return c.id < id; });
-    if (it == cons.end() || it->id != ids[i]) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown constraint id");
-    drop[it - cons.begin()] = 1;
-  }
-  size_t n = 0;
-  for (size_t i = 0; i < cons.size(); ++i)
-    if (!drop[i]) cons[n++] = cons[i];
-  cons.resize(n);
-  return Publish(h, nullptr, false);
-}
-
-bba_status bba_get_keyframe_pose_constraints(bba_handle h, int capacity, int* ids, bba_pose_constraint* out, int* count) {
-  FrontEndScope front_end;
-  if (!h || !count) return BBA_ERR_INVALID_ARGUMENT;
-  if (capacity < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_get_keyframe_pose_constraints: capacity < 0");
-  std::lock_guard<std::mutex> lock(h->fe.mu);
-  const std::vector<PoseConstraint>& cons = h->fe.constraints;
-  *count = static_cast<int>(cons.size());
-  const int n = std::min(capacity, *count);
-  for (int i = 0; i < n; ++i) {
-    if (ids) ids[i] = cons[i].id;
-    if (out) out[i] = cons[i].c;
-  }
-  return BBA_OK;
-}
-
-bba_status bba_set_keyframe_pose_constraint_losses(bba_handle h, int count, const int* ids, const bba_robust_loss* losses) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_set_keyframe_pose_constraint_losses: ";
-  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
-  if (count > 0 && (!ids || !losses)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  auto& cons = h->pose_constraints;
-  std::vector<size_t> at(count);
-  for (int i = 0; i < count; ++i) {
-    auto it = std::lower_bound(cons.begin(), cons.end(), ids[i], [](const PoseConstraint& c, int id) { return c.id < id; });
-    if (it == cons.end() || it->id != ids[i]) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown constraint id");
-    if (!RobustLossValid(losses[i])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown loss type or bad scale");
-    at[i] = static_cast<size_t>(it - cons.begin());
-  }
-  for (int i = 0; i < count; ++i) cons[at[i]].loss = losses[i];
-  return Publish(h, nullptr, false);
-}
-
-bba_status bba_get_keyframe_pose_constraint_losses(bba_handle h, int capacity, int* ids, bba_robust_loss* out, int* count) {
-  FrontEndScope front_end;
-  if (!h || !count) return BBA_ERR_INVALID_ARGUMENT;
-  if (capacity < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_get_keyframe_pose_constraint_losses: capacity < 0");
-  std::lock_guard<std::mutex> lock(h->fe.mu);
-  const std::vector<PoseConstraint>& cons = h->fe.constraints;
-  *count = static_cast<int>(cons.size());
-  const int n = std::min(capacity, *count);
-  for (int i = 0; i < n; ++i) {
-    if (ids) ids[i] = cons[i].id;
-    if (out) out[i] = cons[i].loss;
-  }
-  return BBA_OK;
-}
-
 bba_status bba_get_covisibility(bba_handle h, int id, uint8_t* out_row) {
   CHECK_KF(h, id);
   std::memset(out_row, 0, h->keyframes.size());

@@ -531,84 +531,6 @@ bba::PcgArgs MakePcgArgs(bba_handle h, const PcgLayout& L, int gauge) {
   return a;
 }
 
-// The pose-block terms of the products at the poses the init pass sees, staged for LaunchPcgPoseTerms: a keyframe's prior and,
-// per constraint, H_aa / H_bb, H_ab and b_a / b_b of PoseConstraintTerms, gathered per pose block (every keyframe but the
-// gauge) in the order prior, then constraints by id.  An edge to the gauge keeps only its other end's diagonal terms (p_gauge = 0).
-// Every term's H and b are scaled by its robust weight at these poses (one IRLS step per outer iteration; w = 1 exactly for a
-// trivial loss).  fp64, rounded to fp32.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.
-bba_status StagePcgPoseTerms(bba_handle h, const PcgLayout& L, int gauge, cudaStream_t s) {
-  auto& pc = h->pcg;
-  pc.pose_blocks = 0;
-  if (!L.opt_poses || (h->pose_prior_count == 0 && h->pose_constraints.empty()) || h->cfg.rank != 0) return BBA_OK;
-  const int K = static_cast<int>(h->keyframes.size());
-  const size_t C = h->pose_constraints.size();
-  if (bba_status st = ReservePoseTerms(h, C)) return st;
-  auto unknown = [&](int k) { return k == gauge ? -1 : 6 * (k < gauge ? k : k - 1); };
-  std::vector<float> poses(7 * static_cast<size_t>(K));
-  for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses.data() + 7 * k);
-  // every constraint's terms at the current poses: [a's term, b's term]
-  std::vector<bba::PcgPoseTerm> edge(2 * C);
-  for (size_t i = 0; i < C; ++i) {
-    const bba_pose_constraint& c = h->pose_constraints[i].c;
-    double r[6], H[78], b[12], cost;
-    PoseConstraintTerms(c.a_T_b, poses.data() + 7 * c.keyframe_a, poses.data() + 7 * c.keyframe_b, c.information, r, H, b, &cost);
-    const bba_robust_loss& loss = h->pose_constraints[i].loss;
-    double rho, w;
-    RobustLoss(loss.type, loss.scale, 2.0 * cost, &rho, &w);
-    for (double& v : H) v *= w;
-    for (double& v : b) v *= w;
-    auto upper = [&](int row, int col) { return H[row * 12 - row * (row - 1) / 2 + (col - row)]; };
-    bba::PcgPoseTerm& ta = edge[2 * i];
-    bba::PcgPoseTerm& tb = edge[2 * i + 1];
-    ta.other = unknown(c.keyframe_b);
-    tb.other = unknown(c.keyframe_a);
-    int idx = 0;
-    for (int row = 0; row < 6; ++row) {
-      ta.b[row] = static_cast<float>(b[row]);
-      tb.b[row] = static_cast<float>(b[6 + row]);
-      for (int col = row; col < 6; ++col, ++idx) {
-        ta.H[idx] = static_cast<float>(upper(row, col));
-        tb.H[idx] = static_cast<float>(upper(6 + row, 6 + col));
-      }
-      for (int col = 0; col < 6; ++col) {
-        const float x = static_cast<float>(upper(row, 6 + col));   // H_ab[row][col]
-        ta.X[row * 6 + col] = x;
-        tb.X[col * 6 + row] = x;                                  // H_ba = H_ab^T
-      }
-    }
-  }
-  std::vector<int> off, adj;
-  ConstraintAdjacency(h, K, &off, &adj);
-  int nb = 0, nt = 0;
-  for (int k = 0; k < K; ++k) {
-    if (k == gauge) continue;
-    const int begin = nt;
-    const PosePrior& prior = h->pose_priors[k];
-    if (prior.has) {
-      bba::PcgPoseTerm& t = pc.h_pose_terms[nt++];
-      t.other = -1;
-      double H[21], b[6], cost;
-      bba::PosePriorTerms(prior.pose, poses.data() + 7 * k, prior.info, H, b, &cost);
-      const bba_robust_loss& loss = h->pose_prior_losses[k];
-      double rho, w;
-      RobustLoss(loss.type, loss.scale, 2.0 * cost, &rho, &w);
-      for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(w * H[j]);
-      for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(w * b[j]);
-    }
-    for (int e = off[k]; e < off[k + 1]; ++e) {
-      const int i = adj[e];
-      pc.h_pose_terms[nt++] = edge[2 * i + (h->pose_constraints[i].c.keyframe_a == k ? 0 : 1)];
-    }
-    if (nt > begin) pc.h_pose_blocks[nb++] = bba::PcgPoseBlock{static_cast<uint32_t>(unknown(k)), begin, nt};
-  }
-  if (nb) {
-    BBA_CUDA(h, cudaMemcpyAsync(pc.d_pose_blocks, pc.h_pose_blocks, sizeof(bba::PcgPoseBlock) * nb, cudaMemcpyHostToDevice, s));
-    BBA_CUDA(h, cudaMemcpyAsync(pc.d_pose_terms, pc.h_pose_terms, sizeof(bba::PcgPoseTerm) * nt, cudaMemcpyHostToDevice, s));
-  }
-  pc.pose_blocks = nb;
-  return BBA_OK;
-}
-
 // The PCG solver's phases, shared by BundleAdjustPCG and the parity hook bba_pcg_debug.  Vectors: d_pcg = {r, M, delta, g, p};
 // scalars = {alpha_n or beta_n (slot an), alpha_d (1), beta_n or alpha_n (slot bn), this rank's alpha_d (3, multi-GPU)}.
 // Init: r = -J^T W F and M = diag(J^T W J) over every keyframe (:312-361), then PCGInit2 (:363-373) into slot `an`.
@@ -618,7 +540,7 @@ bba_status PcgInit(bba_handle h, const PcgLayout& L, const bba::PcgArgs& a, int 
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_vec[1], 0, sizeof(float) * U, s));
   BBA_CUDA(h, cudaMemsetAsync(h->pcg.d_scalars, 0, sizeof(double) * 4, s));
   BBA_LAUNCH(h, h->launches, LaunchPcgAccumulate, a, h->sm_count, true, s);   // PCGInitCUDA for every keyframe
-  if (bba_status st = StagePcgPoseTerms(h, L, a.gauge_kf, s)) return st;
+  if (bba_status st = StagePcgPoseTerms(h, L.opt_poses, a.gauge_kf, s)) return st;
   BBA_LAUNCH(h, h->launches, LaunchPcgPoseTerms, h->pcg.d_pose_blocks, h->pcg.pose_blocks, h->pcg.d_pose_terms, true, a.r, a.M, nullptr,
              nullptr, nullptr, s);
   if (h->cfg.world_size > 1) {
@@ -931,275 +853,6 @@ bba_status DeformSurfels(bba_handle h, int count, const float* original, uint32_
   return BBA_OK;
 }
 
-// ---- keyframe pose graph (bba_optimize_pose_graph, DESIGN §3.14) ----
-// What the pose graph stages for K keyframes and C constraints: terms (a prior per keyframe, the constraints, the chain), ints
-// (held flags, row offsets, two ints per row entry, CSR offsets and columns) and doubles (the terms' blocks, the CSR blocks, b, the
-// couplings and the solver's work).  A row holds its prior and one entry per end of a constraint or chain edge.
-struct PoseGraphSizes {
-  size_t terms, ints, doubles;
-};
-PoseGraphSizes PoseGraphCapacity(size_t K, size_t C) {
-  const size_t terms = 2 * K + C, entries = 3 * K + 2 * C, nnz = 3 * K + 2 * C;
-  const size_t block_doubles = sizeof(PoseGraphTermBlocks) / sizeof(double);
-  return {terms, K + 2 * (K + 1) + 2 * entries + nnz, terms * block_doubles + 36 * nnz + 42 * K + PoseGraphWorkDoubles(K)};
-}
-
-// Sizes the pose graph's buffers for max_keyframes and `constraints` constraints, with room to double the constraints.
-bba_status ReservePoseGraph(bba_handle h, size_t constraints) {
-  const size_t M = static_cast<size_t>(h->cfg.max_keyframes);
-  const PoseGraphSizes need = PoseGraphCapacity(M, constraints), alloc = PoseGraphCapacity(M, 2 * constraints);
-  auto& g = h->graph;
-  BBA_CUDA(h, g.h_terms.Reserve(need.terms, alloc.terms));
-  BBA_CUDA(h, g.d_terms.Reserve(need.terms, alloc.terms));
-  BBA_CUDA(h, g.h_ints.Reserve(need.ints, alloc.ints));
-  BBA_CUDA(h, g.d_ints.Reserve(need.ints, alloc.ints));
-  BBA_CUDA(h, g.h_losses.Reserve(need.terms, alloc.terms));
-  BBA_CUDA(h, g.d_losses.Reserve(need.terms, alloc.terms));
-  BBA_CUDA(h, g.h_eval.Reserve(2 * need.terms, 2 * alloc.terms));
-  BBA_CUDA(h, g.d_eval.Reserve(2 * need.terms, 2 * alloc.terms));
-  BBA_CUDA(h, g.d_doubles.Reserve(need.doubles, alloc.doubles));
-  BBA_CUDA(h, g.h_poses.Reserve(7 * M));
-  BBA_CUDA(h, g.d_poses.Reserve(14 * M));
-  BBA_CUDA(h, g.d_state.Reserve(1));
-  BBA_CUDA(h, g.h_state.Reserve(1));
-  return BBA_OK;
-}
-
-int FindRoot(std::vector<int>& parent, int k) {
-  while (parent[k] != k) k = parent[k] = parent[parent[k]];
-  return k;
-}
-
-// The pose graph's terms in h->graph.h_terms at the keyframe poses `poses`: the priors (prior_term[k]: keyframe k's term, or -1),
-// the constraints by id from *first_constraint, then with odometry_information the odometry chain from *first_chain, whose Z are
-// taken at `poses`.  With losses, every term's loss goes to h_losses (the chain's TRIVIAL).  Returns the number of terms.
-int StagePoseGraphTerms(bba_handle h, const float* poses, const float* odometry_information, bool losses, std::vector<int>* prior_term,
-                        int* first_constraint, int* first_chain) {
-  auto& g = h->graph;
-  const int K = static_cast<int>(h->keyframes.size());
-  prior_term->assign(K, -1);
-  int T = 0;
-  auto add = [&](int a, int b, const float* z, const float* info, const bba_robust_loss& loss) {
-    if (losses) g.h_losses[T] = loss;
-    PoseGraphTerm& t = g.h_terms[T++];
-    t.a = a;
-    t.b = b;
-    std::memcpy(t.z, z, sizeof(t.z));
-    std::memcpy(t.info, info, sizeof(t.info));
-  };
-  for (int k = 0; k < K; ++k) {
-    const PosePrior& p = h->pose_priors[k];
-    if (!p.has) continue;
-    (*prior_term)[k] = T;
-    add(k, -1, p.pose, p.info, h->pose_prior_losses[k]);
-  }
-  *first_constraint = T;
-  for (const PoseConstraint& c : h->pose_constraints) add(c.c.keyframe_a, c.c.keyframe_b, c.c.a_T_b, c.c.information, c.loss);
-  *first_chain = T;
-  if (odometry_information)
-    for (int k = 0; k + 1 < K; ++k) {
-      double qa[4], ta[3], qb[4], tb[3], q[4], t[3];
-      LoadPoseD(poses + 7 * k, qa, ta);
-      LoadPoseD(poses + 7 * (k + 1), qb, tb);
-      Se3BetweenD(qa, ta, qb, tb, q, t);   // T_k^-1 T_{k+1}
-      float z[7];
-      for (int j = 0; j < 4; ++j) z[j] = static_cast<float>(q[j]);
-      for (int j = 0; j < 3; ++j) z[4 + j] = static_cast<float>(t[j]);
-      add(k, k + 1, z, odometry_information, bba_robust_loss{BBA_LOSS_TRIVIAL, 0.f});
-    }
-  return T;
-}
-
-bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_pose_graph_result* result, cudaStream_t s) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_optimize_pose_graph: ";
-  if (!o) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null options");
-  const int K = static_cast<int>(h->keyframes.size());
-  const int gauge = o->gauge_keyframe;
-  if (gauge < -1 || gauge >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "gauge_keyframe out of range");
-  if (o->use_odometry_chain) {
-    for (int j = 0; j < 21; ++j)
-      if (!std::isfinite(o->odometry_information[j])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite odometry_information");
-    if (!InformationPsd(o->odometry_information))
-      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "odometry_information is not positive semi-definite");
-  }
-  bba_pose_graph_result r{};
-  if (result) *result = r;
-  if (K < 2 && h->pose_prior_count == 0) return BBA_OK;
-  const std::vector<PoseConstraint>& cons = h->pose_constraints;
-  if (bba_status st = ReservePoseGraph(h, cons.size())) return st;
-  auto& g = h->graph;
-  const bool chain = o->use_odometry_chain != 0;
-  const int max_iterations = o->max_iterations > 0 ? o->max_iterations : 20;   // pose_graph_optimizer.cc kMaxIterations
-
-  // the terms: priors, constraints by id, then the chain at the poses the call starts from
-  float* poses = g.h_poses;
-  for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses + 7 * k);
-  const bool robust = PoseLossesNonTrivial(h);
-  std::vector<int> prior_term;
-  int first_constraint = 0, first_chain = 0;
-  const int T = StagePoseGraphTerms(h, poses, chain ? o->odometry_information : nullptr, robust, &prior_term, &first_constraint,
-                                    &first_chain);
-
-  // the held keyframes: the gauge, the untouched ones, and the lowest id of every component without the gauge or a prior
-  std::vector<int> parent(K), lowest(K, -1);
-  std::vector<char> touched(K, 0), anchored(K, 0);
-  for (int k = 0; k < K; ++k) parent[k] = k;
-  for (int i = first_constraint; i < T; ++i) {
-    const PoseGraphTerm& t = g.h_terms[i];
-    touched[t.a] = touched[t.b] = 1;
-    const int ra = FindRoot(parent, t.a), rb = FindRoot(parent, t.b);
-    if (ra != rb) parent[std::max(ra, rb)] = std::min(ra, rb);
-  }
-  for (int k = 0; k < K; ++k) {
-    const int root = FindRoot(parent, k);
-    if (lowest[root] < 0) lowest[root] = k;
-    if (prior_term[k] >= 0) touched[k] = 1;
-    if (prior_term[k] >= 0 || k == gauge) anchored[root] = 1;
-  }
-  int* held = g.h_ints;
-  int held_count = 0;
-  for (int k = 0; k < K; ++k) {
-    const int root = FindRoot(parent, k);
-    held[k] = (k == gauge || !touched[k] || (!anchored[root] && lowest[root] == k)) ? 1 : 0;
-    held_count += held[k];
-  }
-
-  // row k: its prior, its constraints by id, the chain edges (k - 1, k) and (k, k + 1); the CSR row: the diagonal, then the other
-  // end of every constraint and chain edge in the same order
-  std::vector<int> off, adj;
-  ConstraintAdjacency(h, K, &off, &adj);
-  int* row_off = held + K;
-  int entries = 0, nnz = 0;
-  for (int k = 0; k < K; ++k) {
-    row_off[k] = entries;
-    const int binary = (off[k + 1] - off[k]) + (chain ? (k > 0) + (k + 1 < K) : 0);
-    entries += (prior_term[k] >= 0) + binary;
-    nnz += 1 + binary;
-  }
-  row_off[K] = entries;
-  int* row_terms = row_off + K + 1;
-  int* csr_off = row_terms + 2 * entries;
-  int* csr_col = csr_off + K + 1;
-  int e = 0, c = 0;
-  auto entry = [&](int term, int side, int col) {
-    row_terms[2 * e] = term;
-    row_terms[2 * e + 1] = side;
-    ++e;
-    if (col >= 0) csr_col[c++] = col;
-  };
-  for (int k = 0; k < K; ++k) {
-    csr_off[k] = c;
-    csr_col[c++] = k;
-    if (prior_term[k] >= 0) entry(prior_term[k], 0, -1);
-    for (int j = off[k]; j < off[k + 1]; ++j) {
-      const bba_pose_constraint& pc = cons[adj[j]].c;
-      const bool is_a = pc.keyframe_a == k;
-      entry(first_constraint + adj[j], is_a ? 0 : 1, is_a ? pc.keyframe_b : pc.keyframe_a);
-    }
-    if (chain && k > 0) entry(first_chain + k - 1, 1, k - 1);
-    if (chain && k + 1 < K) entry(first_chain + k, 0, k + 1);
-  }
-  csr_off[K] = c;
-  const size_t ints = static_cast<size_t>(csr_col + nnz - held);
-
-  const size_t M = static_cast<size_t>(h->cfg.max_keyframes);
-  if (T) BBA_CUDA(h, cudaMemcpyAsync(g.d_terms, g.h_terms, sizeof(PoseGraphTerm) * T, cudaMemcpyHostToDevice, s));
-  if (T && robust) BBA_CUDA(h, cudaMemcpyAsync(g.d_losses, g.h_losses, sizeof(bba_robust_loss) * T, cudaMemcpyHostToDevice, s));
-  BBA_CUDA(h, cudaMemcpyAsync(g.d_ints, g.h_ints, sizeof(int) * ints, cudaMemcpyHostToDevice, s));
-  BBA_CUDA(h, cudaMemcpyAsync(g.d_poses, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
-  BBA_CUDA(h, cudaMemcpyAsync(g.d_poses + 7 * M, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
-  BBA_CUDA(h, cudaMemsetAsync(g.d_state, 0, sizeof(PoseGraphState), s));
-  PoseGraphArgs a{};
-  a.K = K;
-  a.term_count = T;
-  a.terms = g.d_terms;
-  a.blocks = reinterpret_cast<PoseGraphTermBlocks*>(g.d_doubles.get());
-  a.poses = g.d_poses;
-  a.prev = g.d_poses + 7 * M;
-  const int* d_ints = g.d_ints;
-  a.held = d_ints;
-  a.row_off = d_ints + (row_off - held);
-  a.row_terms = d_ints + (row_terms - held);
-  a.csr_off = d_ints + (csr_off - held);
-  a.csr_col = d_ints + (csr_col - held);
-  double* d = g.d_doubles.get() + static_cast<size_t>(T) * (sizeof(PoseGraphTermBlocks) / sizeof(double));
-  a.csr_val = d;
-  a.rhs = a.csr_val + 36 * static_cast<size_t>(nnz);
-  a.tri = a.rhs + 6 * static_cast<size_t>(K);
-  a.work = a.tri + 36 * static_cast<size_t>(K);
-  a.state = g.d_state;
-  a.max_iterations = max_iterations;
-  a.max_linear = 6 * (K - held_count);
-  a.losses = robust ? g.d_losses.get() : nullptr;
-  for (int round = 0; round <= max_iterations; ++round) {
-    a.round = round;
-    BBA_LAUNCH(h, h->launches, LaunchPoseGraphRound, a, s);
-  }
-  BBA_CUDA(h, cudaMemcpyAsync(g.h_state, g.d_state, sizeof(PoseGraphState), cudaMemcpyDeviceToHost, s));
-  BBA_CUDA(h, cudaMemcpyAsync(poses, g.d_poses, sizeof(float) * 7 * K, cudaMemcpyDeviceToHost, s));
-  BBA_CUDA(h, cudaStreamSynchronize(s));
-  for (int k = 0; k < K; ++k)
-    if (!held[k]) h->keyframes[k].pose = PoseFromArray(poses + 7 * k);
-  const PoseGraphState& st = *g.h_state.get();
-  r.iterations = st.iterations;
-  r.converged = st.converged;
-  r.linear_iterations = st.linear_iterations;
-  r.held_keyframes = held_count;
-  r.initial_cost = st.initial_cost;
-  r.final_cost = st.cost;
-  if (result) *result = r;
-  return Publish(h, s, false);
-}
-
-// bba_evaluate_keyframe_pose_terms: the pose graph's terms without the chain, linearised once by the robust instantiation at the
-// current poses, which writes every term's {s, w}.
-bba_status EvaluatePoseTerms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight, int constraint_capacity,
-                             double* constraint_s, double* constraint_weight, cudaStream_t s) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  if (keyframe_capacity < 0 || constraint_capacity < 0)
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_evaluate_keyframe_pose_terms: negative capacity");
-  const int K = static_cast<int>(h->keyframes.size());
-  const std::vector<PoseConstraint>& cons = h->pose_constraints;
-  if (bba_status st = ReservePoseGraph(h, cons.size())) return st;
-  auto& g = h->graph;
-  float* poses = g.h_poses;
-  for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses + 7 * k);
-  std::vector<int> prior_term;
-  int first_constraint = 0, first_chain = 0;
-  const int T = StagePoseGraphTerms(h, poses, nullptr, /*losses=*/true, &prior_term, &first_constraint, &first_chain);
-  if (T) {
-    BBA_CUDA(h, cudaMemcpyAsync(g.d_terms, g.h_terms, sizeof(PoseGraphTerm) * T, cudaMemcpyHostToDevice, s));
-    BBA_CUDA(h, cudaMemcpyAsync(g.d_losses, g.h_losses, sizeof(bba_robust_loss) * T, cudaMemcpyHostToDevice, s));
-    BBA_CUDA(h, cudaMemcpyAsync(g.d_poses, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
-    BBA_CUDA(h, cudaMemsetAsync(g.d_state, 0, sizeof(PoseGraphState), s));
-    PoseGraphArgs a{};
-    a.K = K;
-    a.term_count = T;
-    a.terms = g.d_terms;
-    a.blocks = reinterpret_cast<PoseGraphTermBlocks*>(g.d_doubles.get());
-    a.poses = g.d_poses;
-    a.state = g.d_state;
-    a.losses = g.d_losses;
-    a.eval = g.d_eval;
-    BBA_LAUNCH(h, h->launches, LaunchPoseGraphEvaluate, a, s);
-    BBA_CUDA(h, cudaMemcpyAsync(g.h_eval, g.d_eval, sizeof(double) * 2 * T, cudaMemcpyDeviceToHost, s));
-    BBA_CUDA(h, cudaStreamSynchronize(s));
-  }
-  const double* ev = g.h_eval;
-  for (int k = 0; k < std::min(keyframe_capacity, K); ++k) {
-    const int t = prior_term[k];
-    if (prior_s) prior_s[k] = t >= 0 ? ev[2 * t] : std::nan("");
-    if (prior_weight) prior_weight[k] = t >= 0 ? ev[2 * t + 1] : std::nan("");
-  }
-  for (int i = 0; i < std::min(constraint_capacity, static_cast<int>(cons.size())); ++i) {
-    const int t = first_constraint + i;
-    if (constraint_s) constraint_s[i] = ev[2 * t];
-    if (constraint_weight) constraint_weight[i] = ev[2 * t + 1];
-  }
-  return BBA_OK;
-}
-
 }  // namespace
 }  // namespace bba
 
@@ -1218,16 +871,6 @@ bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream) {
 bba_status bba_deform_surfels(bba_handle h, int count, const float* original_keyframe_T_global, uint32_t* moved, uint32_t* unobserved,
                               void* stream) {
   return DeformSurfels(h, count, original_keyframe_T_global, moved, unobserved, static_cast<cudaStream_t>(stream));
-}
-
-bba_status bba_optimize_pose_graph(bba_handle h, const bba_pose_graph_options* options, bba_pose_graph_result* result, void* stream) {
-  return OptimizePoseGraph(h, options, result, static_cast<cudaStream_t>(stream));
-}
-
-bba_status bba_evaluate_keyframe_pose_terms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight,
-                                            int constraint_capacity, double* constraint_s, double* constraint_weight, void* stream) {
-  return EvaluatePoseTerms(h, keyframe_capacity, prior_s, prior_weight, constraint_capacity, constraint_s, constraint_weight,
-                           static_cast<cudaStream_t>(stream));
 }
 
 bba_status bba_optimize_intrinsics(bba_handle h, int optimize_depth, int optimize_color, void* stream) {

@@ -2,8 +2,9 @@
 // memory, events and textures, the keyframe record, error reporting and the helpers that more than one unit calls.
 //
 // Host units: badba.cu (handle, setters / getters, keyframes, textures, bba_host_*), pose_step.cu (spatial order, pose step),
-// bundle_adjust.cu (BA schemes, intrinsics, PCG, surfel lifecycle, pose graph), multi_gpu.cu (sharding, exchange, peer replicas),
-// frames.cu (odometry, preprocessing).  None of them contains a kernel.
+// pose_terms.cu (soft pose priors and constraints, their losses and staging, pose graph), bundle_adjust.cu (BA schemes,
+// intrinsics, PCG, surfel lifecycle), multi_gpu.cu (sharding, exchange, peer replicas), frames.cu (odometry, preprocessing).  None
+// of them contains a kernel.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -129,6 +130,16 @@ struct Keyframe {
   std::vector<int> covis;
 };
 
+// One keyframe's soft pose prior (bba_set_keyframe_pose_priors): the prior global_T_frame P, the upper triangle of its 6x6
+// information matrix L (row-major, the tangent order of H: translation, then rotation) and its robust loss
+// (bba_set_keyframe_pose_prior_losses).  Setting a prior keeps the loss; clearing it resets the whole record.
+struct PosePrior {
+  float pose[7];
+  float info[21];
+  int has;   // 0: no prior on this keyframe
+  bba_robust_loss loss;
+};
+
 // ---- the front end's view (badba.h "Conventions"; DESIGN.md "Front end beside a running BA") -----------------------------------
 // What front-end calls read of a keyframe: copied from its Keyframe record whenever the BA side publishes.
 struct KeyframeView {
@@ -140,7 +151,6 @@ struct KeyframeView {
   float min_depth = 0.f, max_depth = 0.f;
   int activation = BBA_KF_ACTIVE;
   PosePrior prior{};
-  bba_robust_loss prior_loss{};
 };
 
 // A soft relative pose constraint as the handle keeps it: its id, the caller's record, and the information of the equivalent
@@ -198,9 +208,6 @@ struct bba_context {
   // constraint the pose solve and the PCG solver run without pose terms
   std::vector<bba::PosePrior> pose_priors;   // [max_kf]
   int pose_prior_count = 0;
-  // the priors' robust losses by keyframe id (bba_set_keyframe_pose_prior_losses): TRIVIAL until set, kept when a prior is
-  // replaced, reset when it is cleared.  A constraint's loss is PoseConstraint::loss.
-  std::vector<bba_robust_loss> pose_prior_losses;   // [max_kf]
   // soft relative pose constraints (bba_add_keyframe_pose_constraints) in id order, and the id the next one gets
   std::vector<bba::PoseConstraint> pose_constraints;
   int next_pose_constraint_id = 0;
@@ -247,9 +254,6 @@ struct bba_context {
     bba::DeviceBuffer<int> d_term_offsets;
     bba::PinnedBuffer<bba::PoseTerm> h_terms;
     bba::DeviceBuffer<bba::PoseTerm> d_terms;
-    // the terms' robust losses, parallel to h_terms; staged only when a prior or constraint has a non-trivial loss
-    bba::PinnedBuffer<bba_robust_loss> h_term_losses;
-    bba::DeviceBuffer<bba_robust_loss> d_term_losses;
     // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream); the
     // geometry step's stream (bba::LaunchGeometryStream) shares the buffer.
     // The order is rebuilt at the start of every BA call, after an in-loop change of the surfel set, and whenever the surfel
@@ -303,9 +307,7 @@ struct bba_context {
   struct PoseGraph {
     bba::PinnedBuffer<bba::PoseGraphTerm> h_terms;
     bba::DeviceBuffer<bba::PoseGraphTerm> d_terms;
-    // the terms' robust losses (the chain's trivial) and, for bba_evaluate_keyframe_pose_terms, every term's {s, w}
-    bba::PinnedBuffer<bba_robust_loss> h_losses;
-    bba::DeviceBuffer<bba_robust_loss> d_losses;
+    // every term's {s, w} (bba_evaluate_keyframe_pose_terms)
     bba::PinnedBuffer<double> h_eval;
     bba::DeviceBuffer<double> d_eval;
     bba::PinnedBuffer<int> h_ints;
@@ -339,7 +341,7 @@ struct bba_context {
     bba::DeviceBuffer<double> d_scalars;   // [0] / [2] alpha_n, beta_n (roles swap), [1] alpha_d
     bba::PinnedBuffer<double> h_scalars;
     bba::PinnedBuffer<float> h_delta;      // pose part (6 * max_keyframes) + 16
-    // the pose-block terms (priors, constraints) at the poses of the current outer iteration (StagePcgPoseTerms)
+    // the pose-block terms (priors, constraints) at the poses of the current outer iteration (pose_terms.cu StagePcgPoseTerms)
     bba::PinnedBuffer<bba::PcgPoseBlock> h_pose_blocks;
     bba::DeviceBuffer<bba::PcgPoseBlock> d_pose_blocks;
     bba::PinnedBuffer<bba::PcgPoseTerm> h_pose_terms;
@@ -570,15 +572,14 @@ bba_status MakeFrameLumaTextures(bba_handle h, bool front_end, const bba_frame_b
 constexpr uint64_t kSpatialOrderMinPairs = 16u << 20;   // (surfel, keyframe) pairs per launch
 bba_status EnsureSpatialOrder(bba_handle h, bool sort, bool rebuild, cudaStream_t s);
 bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, int max_iterations, cudaStream_t s);
-// Reserves the staging buffers of the soft pose terms (pose step and PCG) for a prior on every keyframe and `constraints`
-// constraints, with room to double the constraints before the next allocation.  The calls that add priors or constraints make
-// it before they change anything; the staging repeats it, a no-op unless an earlier reservation failed.
-bba_status ReservePoseTerms(bba_handle h, size_t constraints);
-// The soft relative pose constraints that touch each of the first K keyframes, in id order: indices into
-// h->pose_constraints, adj[off[k] .. off[k + 1]).
-void ConstraintAdjacency(bba_handle h, int K, std::vector<int>* off, std::vector<int>* adj);
-// Whether a prior or a constraint has a loss other than TRIVIAL: only then do the solvers run their robust instantiations.
-bool PoseLossesNonTrivial(bba_handle h);
+
+// pose_terms.cu
+// Stages the soft pose terms of the keyframes in `ids` (start poses init) for PoseSolveKernel into h->pose and uploads them on s.
+// *staged: false when the handle has no prior and no constraint (then nothing is staged).
+bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, cudaStream_t s, bool* staged);
+// Stages the pose-block terms of the PCG products at the current keyframe poses for LaunchPcgPoseTerms into h->pcg and uploads
+// them on s; none unless opt_poses.  gauge: the keyframe without pose unknowns.
+bba_status StagePcgPoseTerms(bba_handle h, bool opt_poses, int gauge, cudaStream_t s);
 
 // multi_gpu.cu
 void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t* shard_len);

@@ -255,14 +255,6 @@ BBA_HD void SolveLDLT(const double* upper, const double* b, double* x) {
 }
 
 // ---- soft pose prior on a keyframe (bba_set_keyframe_pose_priors) ----
-// One keyframe's prior as the pose solve reads it: the prior global_T_frame P and the upper triangle of its 6x6 information
-// matrix L (row-major, the tangent order of H: translation, then rotation).
-struct PosePrior {
-  float pose[7];
-  float info[21];
-  int has;   // 0: no prior on this keyframe
-};
-
 // 3x3 helpers in fp64 (row-major).
 BBA_HD void HatD(const double w[3], double O[9]) {
   O[0] = 0.0; O[1] = -w[2]; O[2] = w[1];
@@ -521,6 +513,9 @@ inline bool InformationPsd(const float info[21]) {
 }
 
 // ---- soft relative pose constraint between two keyframes (bba_add_keyframe_pose_constraints) ----
+// The index of (r, c), r <= c, in the row-major upper triangle of a 12 x 12 matrix (78 entries).
+BBA_HD int Upper12(int r, int c) { return r * 12 - r * (r - 1) / 2 + (c - r); }
+
 // The constraint's terms at global_T_frame = pose_a, pose_b, for the updates pose_a * exp(delta_a), pose_b * exp(delta_b): with
 // r = log(Z^-1 pose_a^-1 pose_b), Z = a_T_b, J_b = Jr^-1(r) and J_a = -Jr^-1(r) Ad(pose_b^-1 pose_a), and J = [J_a | J_b]:
 // H = J^T L J over (delta_a, delta_b) (12 x 12 upper triangle, 78), b = J^T L r (12), cost = r^T L r / 2.  fp64 throughout.

@@ -12,12 +12,14 @@
 
 namespace bba {
 
-// One term of a keyframe's pose solve in the form of a soft pose prior (host_math.hpp PosePriorTerms): the prior global_T_frame
-// and the upper triangle of its 6x6 information matrix.  The pose step stages a keyframe's prior, the equivalent priors of its
-// relative pose constraints and their damping anchors as such terms (pose_step.cu StagePoseTerms).
+// One term of a keyframe's pose solve in the form of a soft pose prior (host_math.hpp PosePriorTerms): the prior global_T_frame,
+// the upper triangle of its 6x6 information matrix and its robust loss (host_math.hpp RobustLoss: H and b are scaled by w at the
+// current estimate).  The pose step stages a keyframe's prior, the equivalent priors of its relative pose constraints and their
+// damping anchors as such terms (pose_terms.cu StagePoseTerms).
 struct PoseTerm {
   float pose[7];
   float info[21];
+  bba_robust_loss loss;
 };
 
 // Accumulator record per keyframe written by the pose kernel: 32 fp64 sums
@@ -115,20 +117,19 @@ struct PoseSolveArgs {
   // both null when no keyframe has one
   const int* term_offsets;     // [keyframes + 1]
   const PoseTerm* terms;
-  // the terms' robust losses, parallel to terms (host_math.hpp RobustLoss: a term's H and b are scaled by w at the current
-  // estimate); null when every loss is trivial, which runs the instantiation without them
-  const bba_robust_loss* term_losses;
 };
 // Device-side Gauss-Newton step for every keyframe in the list (direct_ba_alternating.cc:173-233).
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
 
 // Keyframe pose graph (pose_graph.cu; bba_optimize_pose_graph, DESIGN §3.14).  One term of the cost: a soft pose prior on
 // keyframe a (b = -1, z = the prior's global_T_frame), or a relative pose constraint (a, b, z = a_T_b): a handle constraint
-// or an odometry-chain edge of the call.  info: the upper triangle of L.
+// or an odometry-chain edge of the call.  info: the upper triangle of L.  loss: the term's robust loss (host_math.hpp RobustLoss:
+// its blocks are scaled by w at the current poses and it costs rho(s) / 2); TRIVIAL for a chain edge.
 struct PoseGraphTerm {
   int a, b;
   float z[7];
   float info[21];
+  bba_robust_loss loss;
 };
 // A term's linearisation at the current poses (host_math.hpp PosePriorTerms / PoseConstraintTerms): H's upper triangle (21 of
 // a prior, 78 of a constraint over (delta_a, delta_b)), b = J^T L r (6 or 12) and the cost.
@@ -166,10 +167,7 @@ struct PoseGraphArgs {
   int max_iterations;            // Gauss-Newton iterations
   int max_linear;                // PCG iterations per linear solve
   int round;                     // 0 .. max_iterations: the round of this launch
-  // the terms' robust losses (host_math.hpp RobustLoss: H and b scaled by w, the cost rho(s) / 2); null when every loss is
-  // trivial, which runs the linearisation without them
-  const bba_robust_loss* losses;   // [term_count]
-  double* eval;                    // null, or [term_count][2]: every term's {s, w} (bba_evaluate_keyframe_pose_terms)
+  double* eval;                  // null, or [term_count][2]: every term's {s, w} (bba_evaluate_keyframe_pose_terms)
 };
 // The doubles of PoseGraphArgs::work for K keyframes: the reduction's levels (at most 2K + 32 blocks of six 6x6 matrices and
 // three 6-vectors) and five PCG vectors of K blocks.
@@ -178,7 +176,7 @@ inline size_t PoseGraphWorkDoubles(size_t K) { return (2 * K + 32) * (6 * 36 + 3
 // test of the last step, then PCG with the block-tridiagonal preconditioner factorised by cyclic reduction, one CTA), and
 // T <- T exp(delta).  round == max_iterations launches the first three only (the test of the last step).
 LaunchResult LaunchPoseGraphRound(const PoseGraphArgs& a, cudaStream_t stream);
-// One launch of the robust linearisation with a.eval set: every term's {s, w} at a.poses (a.state->done must be 0).
+// One launch of the linearisation with a.eval set: every term's {s, w} at a.poses (a.state->done must be 0).
 LaunchResult LaunchPoseGraphEvaluate(const PoseGraphArgs& a, cudaStream_t stream);
 
 // Replicas of the surfel buffer / active flags on the OTHER ranks of a one-process-per-GPU job, mapped into this process

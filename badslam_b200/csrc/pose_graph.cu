@@ -3,8 +3,9 @@
 //
 // One Gauss-Newton iteration is one round of four kernels, and the host enqueues every round without synchronising: the state
 // (PoseGraphState) decides on the device whether the last step is kept, and once it is done every later kernel returns at once.
-//   PoseGraphLinearizeKernel  one thread per term: PosePriorTerms / PoseConstraintTerms at the fp32 poses, in fp64; with robust
-//                             losses (the ROBUST instantiation) scaled by the IRLS weight, the cost rho(s) / 2.
+//   PoseGraphLinearizeKernel  one thread per term: PosePriorTerms / PoseConstraintTerms at the fp32 poses, in fp64, scaled by the
+//                             IRLS weight of the term's loss, the cost rho(s) / 2 (w = 1 and rho(s) / 2 = cost exactly for a
+//                             trivial loss).
 //   PoseGraphAssembleKernel   one thread per row block: H_kk, b_k, the block-CSR row and the coupling H_{k,k+1}, summed over the
 //                             row's terms in term order.  A held keyframe's row is the identity with a zero right-hand side.
 //   PoseGraphSolveKernel      one CTA: the cost at the current poses (a fixed-order sum) and the test of the last step, then
@@ -176,9 +177,8 @@ __device__ double Dot(const double* a, const double* b, int n, double* sh) {
   return BlockSum(s, sh);
 }
 
-// ROBUST: the term's blocks are scaled by the weight of its loss (a.losses) at the current poses and its cost is rho(s) / 2; with
-// a.eval, {s, w} is written too.
-template <bool ROBUST>
+// The term's blocks are scaled by the weight of its loss at the current poses and its cost is rho(s) / 2; with a.eval, {s, w} is
+// written too.
 __global__ void __launch_bounds__(64) PoseGraphLinearizeKernel(const PoseGraphArgs a) {
   if (a.state->done) return;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -191,19 +191,16 @@ __global__ void __launch_bounds__(64) PoseGraphLinearizeKernel(const PoseGraphAr
     double r[6];
     PoseConstraintTerms(term.z, a.poses + 7 * term.a, a.poses + 7 * term.b, term.info, r, blk.H, blk.b, &blk.cost);
   }
-  if constexpr (ROBUST) {
-    const bba_robust_loss loss = a.losses[t];
-    const double s = 2.0 * blk.cost;
-    double rho, w;
-    RobustLoss(loss.type, loss.scale, s, &rho, &w);
-    const int nh = term.b < 0 ? 21 : 78, nb = term.b < 0 ? 6 : 12;
-    for (int i = 0; i < nh; ++i) blk.H[i] *= w;
-    for (int i = 0; i < nb; ++i) blk.b[i] *= w;
-    blk.cost = 0.5 * rho;
-    if (a.eval) {
-      a.eval[2 * t] = s;
-      a.eval[2 * t + 1] = w;
-    }
+  const double s = 2.0 * blk.cost;
+  double rho, w;
+  RobustLoss(term.loss.type, term.loss.scale, s, &rho, &w);
+  const int nh = term.b < 0 ? 21 : 78, nb = term.b < 0 ? 6 : 12;
+  for (int i = 0; i < nh; ++i) blk.H[i] *= w;
+  for (int i = 0; i < nb; ++i) blk.b[i] *= w;
+  blk.cost = 0.5 * rho;
+  if (a.eval) {
+    a.eval[2 * t] = s;
+    a.eval[2 * t + 1] = w;
   }
 }
 
@@ -243,7 +240,7 @@ __global__ void __launch_bounds__(128) PoseGraphAssembleKernel(const PoseGraphAr
       continue;
     }
     // the 12x12 upper triangle over (delta_a, delta_b)
-    auto h12 = [&](int r, int c) { return blk.H[r * 12 - r * (r - 1) / 2 + (c - r)]; };
+    auto h12 = [&](int r, int c) { return blk.H[Upper12(r, c)]; };
     const int o = side ? 6 : 0, other = side ? term.a : term.b;
     for (int r = 0; r < 6; ++r) {
       bk[r] += blk.b[o + r];
@@ -504,8 +501,7 @@ __global__ void __launch_bounds__(128) PoseGraphUpdateKernel(const PoseGraphArgs
 
 LaunchResult LaunchPoseGraphRound(const PoseGraphArgs& a, cudaStream_t stream) {
   const int blocks = (a.term_count + 63) / 64 > 0 ? (a.term_count + 63) / 64 : 1;
-  if (a.losses) PoseGraphLinearizeKernel<true><<<blocks, 64, 0, stream>>>(a);
-  else PoseGraphLinearizeKernel<false><<<blocks, 64, 0, stream>>>(a);
+  PoseGraphLinearizeKernel<<<blocks, 64, 0, stream>>>(a);
   PoseGraphAssembleKernel<<<(a.K + 127) / 128, 128, 0, stream>>>(a);
   PoseGraphSolveKernel<<<1, kSolveThreads, 0, stream>>>(a);
   if (a.round >= a.max_iterations) return {3};
@@ -514,7 +510,7 @@ LaunchResult LaunchPoseGraphRound(const PoseGraphArgs& a, cudaStream_t stream) {
 }
 
 LaunchResult LaunchPoseGraphEvaluate(const PoseGraphArgs& a, cudaStream_t stream) {
-  PoseGraphLinearizeKernel<true><<<(a.term_count + 63) / 64 > 0 ? (a.term_count + 63) / 64 : 1, 64, 0, stream>>>(a);
+  PoseGraphLinearizeKernel<<<(a.term_count + 63) / 64 > 0 ? (a.term_count + 63) / 64 : 1, 64, 0, stream>>>(a);
   return {1};
 }
 

@@ -13,8 +13,7 @@
 namespace bba {
 
 // DET (the deterministic mode): the accumulator record is read from the keyframe's exact sums, rounded to fp64, instead of acc.
-// ROBUST: every pose term's H and b are scaled by the weight of its loss (term_losses) at the current estimate.
-template <bool DET, bool ROBUST>
+template <bool DET>
 __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
   __shared__ int next_count;
   __shared__ unsigned long long tot[5];
@@ -58,22 +57,16 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
     float* pe = a.pose_est + static_cast<size_t>(kf) * 7;
     if (a.term_offsets) {
       // the soft pose terms (a prior, the equivalent priors of relative pose constraints and their damping anchors), added to
-      // the rounded sums in fp64 at the current estimate, in list order
+      // the rounded sums in fp64 at the current estimate, in list order, each scaled by the weight of its loss there (w = 1.0
+      // exactly for a trivial loss, so H + 1.0 * Hp = H + Hp)
       const int end = a.term_offsets[kf + 1];
       for (int t = a.term_offsets[kf]; t < end; ++t) {
         const PoseTerm& term = a.terms[t];
-        double Hp[21], bp[6], cost;
+        double Hp[21], bp[6], cost, rho, w;
         PosePriorTerms(term.pose, pe, term.info, Hp, bp, &cost);
-        if constexpr (ROBUST) {
-          const bba_robust_loss loss = a.term_losses[t];
-          double rho, w;
-          RobustLoss(loss.type, loss.scale, 2.0 * cost, &rho, &w);
-          for (int j = 0; j < 21; ++j) H[j] += w * Hp[j];
-          for (int j = 0; j < 6; ++j) b[j] += w * bp[j];
-        } else {
-          for (int j = 0; j < 21; ++j) H[j] += Hp[j];
-          for (int j = 0; j < 6; ++j) b[j] += bp[j];
-        }
+        RobustLoss(term.loss.type, term.loss.scale, 2.0 * cost, &rho, &w);
+        for (int j = 0; j < 21; ++j) H[j] += w * Hp[j];
+        for (int j = 0; j < 6; ++j) b[j] += w * bp[j];
       }
     }
     SolveLDLT<6>(H, b, x);
@@ -114,13 +107,8 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
 }
 
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream) {
-  if (args.term_losses) {
-    if (args.exact) PoseSolveKernel<true, true><<<1, 256, 0, stream>>>(args);
-    else PoseSolveKernel<false, true><<<1, 256, 0, stream>>>(args);
-  } else {
-    if (args.exact) PoseSolveKernel<true, false><<<1, 256, 0, stream>>>(args);
-    else PoseSolveKernel<false, false><<<1, 256, 0, stream>>>(args);
-  }
+  if (args.exact) PoseSolveKernel<true><<<1, 256, 0, stream>>>(args);
+  else PoseSolveKernel<false><<<1, 256, 0, stream>>>(args);
   return {1};
 }
 

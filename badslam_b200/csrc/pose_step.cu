@@ -238,143 +238,7 @@ bba_status EstimateFramePoses(bba_handle h, int frame_count, const bba_frame_buf
   return BBA_OK;
 }
 
-// Stages the soft pose terms of the keyframes in `ids` (start poses init) for PoseSolveKernel and uploads them on s: keyframe k's
-// list holds its prior, then for every constraint that touches it (in id order) the equivalent prior with the other end held at
-// its start pose (T_b Z^-1 with the information of PoseConstraintInformationA, or T_a Z with L), then for every such constraint
-// whose other end is in the step too a damping anchor, a prior at k's own start pose with the constraint's diagonal block for k
-// at the start poses, scaled by the constraint's robust weight there, as its information (DESIGN.md 3.12, 3.15).  With a non-trivial
-// loss the terms' losses are staged beside them: a prior's own, an equivalent prior's its constraint's, an anchor's TRIVIAL.  Every
-// rank stages the same lists: they depend only on the start of the step.  *staged: false when the handle has no prior and no
-// constraint (then nothing is staged); *robust: the losses were staged.
-bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, cudaStream_t s, bool* staged,
-                          bool* robust) {
-  auto& p = h->pose;
-  *staged = false;
-  *robust = false;
-  if (h->pose_prior_count == 0 && h->pose_constraints.empty()) return BBA_OK;
-  const bool losses = PoseLossesNonTrivial(h);
-  const std::vector<PoseConstraint>& cons = h->pose_constraints;
-  if (bba_status st = ReservePoseTerms(h, cons.size())) return st;
-  const int K = static_cast<int>(h->keyframes.size());
-  std::vector<int> pos(K, -1);   // index in ids
-  for (size_t i = 0; i < ids.size(); ++i) pos[ids[i]] = static_cast<int>(i);
-  auto start = [&](int k, float out[7]) { PoseToArray(pos[k] >= 0 ? init[pos[k]] : h->keyframes[k].pose, out); };
-  std::vector<int> off, adj;
-  ConstraintAdjacency(h, K, &off, &adj);
-  // the anchors' information, once per constraint with both ends in the step: [a's diagonal block, b's] (upper triangles)
-  std::vector<float> anchor_info;
-  std::vector<int> anchor_of(cons.size(), -1);
-  for (size_t i = 0; i < cons.size(); ++i) {
-    const bba_pose_constraint& c = cons[i].c;
-    if (pos[c.keyframe_a] < 0 || pos[c.keyframe_b] < 0) continue;
-    float pa[7], pb[7];
-    start(c.keyframe_a, pa);
-    start(c.keyframe_b, pb);
-    double r[6], H[78], b[12], cost;
-    PoseConstraintTerms(c.a_T_b, pa, pb, c.information, r, H, b, &cost);
-    double rho, w;
-    RobustLoss(cons[i].loss.type, cons[i].loss.scale, 2.0 * cost, &rho, &w);
-    anchor_of[i] = static_cast<int>(anchor_info.size());
-    for (int o = 0; o < 12; o += 6)   // the diagonal blocks in the 12 x 12 upper triangle
-      for (int row = o; row < o + 6; ++row)
-        for (int col = row; col < o + 6; ++col)
-          anchor_info.push_back(static_cast<float>(w * H[row * 12 - row * (row - 1) / 2 + (col - row)]));
-  }
-  int n = 0;
-  for (int k = 0; k < K; ++k) {
-    p.h_term_offsets[k] = n;
-    if (pos[k] < 0) continue;
-    const PosePrior& prior = h->pose_priors[k];
-    if (prior.has) {
-      if (losses) p.h_term_losses[n] = h->pose_prior_losses[k];
-      PoseTerm& r = p.h_terms[n++];
-      std::memcpy(r.pose, prior.pose, sizeof(r.pose));
-      std::memcpy(r.info, prior.info, sizeof(r.info));
-    }
-    for (int e = off[k]; e < off[k + 1]; ++e) {   // the equivalent priors
-      const PoseConstraint& c = cons[adj[e]];
-      const bool is_a = c.c.keyframe_a == k;
-      float other[7];
-      start(is_a ? c.c.keyframe_b : c.c.keyframe_a, other);
-      double qz[4], tz[3], qo[4], to[3], q[4], t[3];
-      LoadPoseD(c.c.a_T_b, qz, tz);
-      LoadPoseD(other, qo, to);
-      if (is_a) {   // T_b Z^-1
-        double qi[4], ti[3];
-        const double q_id[4] = {0.0, 0.0, 0.0, 1.0}, t_id[3] = {0.0, 0.0, 0.0};
-        Se3BetweenD(qz, tz, q_id, t_id, qi, ti);
-        Se3ComposeD(qo, to, qi, ti, q, t);
-      } else {      // T_a Z
-        Se3ComposeD(qo, to, qz, tz, q, t);
-      }
-      if (losses) p.h_term_losses[n] = c.loss;
-      PoseTerm& r = p.h_terms[n++];
-      for (int j = 0; j < 4; ++j) r.pose[j] = static_cast<float>(q[j]);
-      for (int j = 0; j < 3; ++j) r.pose[4 + j] = static_cast<float>(t[j]);
-      std::memcpy(r.info, is_a ? c.info_a : c.c.information, sizeof(r.info));
-    }
-    for (int e = off[k]; e < off[k + 1]; ++e) {   // the damping anchors
-      const int a = anchor_of[adj[e]];
-      if (a < 0) continue;
-      if (losses) p.h_term_losses[n] = bba_robust_loss{BBA_LOSS_TRIVIAL, 0.f};
-      PoseTerm& anchor = p.h_terms[n++];
-      PoseToArray(init[pos[k]], anchor.pose);
-      std::memcpy(anchor.info, anchor_info.data() + a + (cons[adj[e]].c.keyframe_a == k ? 0 : 21), sizeof(anchor.info));
-    }
-  }
-  p.h_term_offsets[K] = n;
-  BBA_CUDA(h, cudaMemcpyAsync(p.d_term_offsets, p.h_term_offsets, sizeof(int) * (K + 1), cudaMemcpyHostToDevice, s));
-  if (n) BBA_CUDA(h, cudaMemcpyAsync(p.d_terms, p.h_terms, sizeof(PoseTerm) * n, cudaMemcpyHostToDevice, s));
-  if (n && losses) BBA_CUDA(h, cudaMemcpyAsync(p.d_term_losses, p.h_term_losses, sizeof(bba_robust_loss) * n, cudaMemcpyHostToDevice, s));
-  *staged = true;
-  *robust = n && losses;
-  return BBA_OK;
-}
-
 }  // namespace
-
-bba_status ReservePoseTerms(bba_handle h, size_t constraints) {
-  // pose step: a prior per keyframe, and per constraint an equivalent prior and a damping anchor at each end; PCG: a prior per
-  // pose block and one term at each end of a constraint
-  const size_t M = static_cast<size_t>(h->cfg.max_keyframes), grow = 2 * constraints;
-  auto& p = h->pose;
-  BBA_CUDA(h, p.h_term_offsets.Reserve(M + 1));
-  BBA_CUDA(h, p.d_term_offsets.Reserve(M + 1));
-  BBA_CUDA(h, p.h_terms.Reserve(M + 4 * constraints, M + 4 * grow));
-  BBA_CUDA(h, p.d_terms.Reserve(M + 4 * constraints, M + 4 * grow));
-  BBA_CUDA(h, p.h_term_losses.Reserve(M + 4 * constraints, M + 4 * grow));
-  BBA_CUDA(h, p.d_term_losses.Reserve(M + 4 * constraints, M + 4 * grow));
-  auto& pc = h->pcg;
-  BBA_CUDA(h, pc.h_pose_blocks.Reserve(M));
-  BBA_CUDA(h, pc.d_pose_blocks.Reserve(M));
-  BBA_CUDA(h, pc.h_pose_terms.Reserve(M + 2 * constraints, M + 2 * grow));
-  BBA_CUDA(h, pc.d_pose_terms.Reserve(M + 2 * constraints, M + 2 * grow));
-  return BBA_OK;
-}
-
-bool PoseLossesNonTrivial(bba_handle h) {
-  for (size_t k = 0; k < h->pose_priors.size(); ++k)
-    if (h->pose_priors[k].has && h->pose_prior_losses[k].type != BBA_LOSS_TRIVIAL) return true;
-  for (const PoseConstraint& c : h->pose_constraints)
-    if (c.loss.type != BBA_LOSS_TRIVIAL) return true;
-  return false;
-}
-
-void ConstraintAdjacency(bba_handle h, int K, std::vector<int>* off, std::vector<int>* adj) {
-  const std::vector<PoseConstraint>& cons = h->pose_constraints;
-  off->assign(K + 1, 0);
-  for (const PoseConstraint& c : cons) {
-    ++(*off)[c.c.keyframe_a + 1];
-    ++(*off)[c.c.keyframe_b + 1];
-  }
-  for (int k = 0; k < K; ++k) (*off)[k + 1] += (*off)[k];
-  adj->resize(2 * cons.size());
-  std::vector<int> fill(off->begin(), off->end() - 1);
-  for (size_t i = 0; i < cons.size(); ++i) {   // in id order: cons is sorted by id
-    (*adj)[fill[cons[i].c.keyframe_a]++] = static_cast<int>(i);
-    (*adj)[fill[cons[i].c.keyframe_b]++] = static_cast<int>(i);
-  }
-}
 
 // Runs the Gauss-Newton loop of EstimateFramePose for the keyframes in `ids`, all at once, starting from
 // `init` poses.  On return (stream synchronised) h_pose_est / h_iterations / h_converged / h_first_stats hold the results.
@@ -396,8 +260,8 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
   for (int i = 0; i < n; ++i) PoseToArray(init[i], p.h_pose_est + 7 * ids[i]);
   BBA_CUDA(h, cudaMemcpyAsync(p.d_pose_est, p.h_pose_est, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
   if (world > 1 && n_local) BBA_CUDA(h, cudaMemcpyAsync(x.d_local_ids, p.h_work, sizeof(int) * n_local, cudaMemcpyHostToDevice, s));
-  bool terms = false, robust = false;
-  if (bba_status st = StagePoseTerms(h, ids, init, s, &terms, &robust)) return st;
+  bool terms = false;
+  if (bba_status st = StagePoseTerms(h, ids, init, s, &terms)) return st;
   BBA_CUDA(h, cudaMemsetAsync(p.d_iterations, 0, sizeof(int) * K, s));
   BBA_CUDA(h, cudaMemsetAsync(p.d_converged, 0, sizeof(int) * K, s));
   if (bba_status st = MarkStaging(h, s)) return st;
@@ -419,7 +283,6 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
   sol.queue = p.d_queue;
   sol.term_offsets = terms ? p.d_term_offsets.get() : nullptr;
   sol.terms = terms ? p.d_terms.get() : nullptr;
-  sol.term_losses = robust ? p.d_term_losses.get() : nullptr;
   p.h_flag[0] = 0;
   p.h_flag[1] = n_local;
   if (h->profiling) BBA_CUDA(h, cudaMemsetAsync(p.d_totals, 0, sizeof(unsigned long long) * 8, s));
