@@ -131,6 +131,25 @@ class OdometryEntry(C.Structure):   # bba_odometry_entry
 
 ODOMETRY_CHUNK_ENTRIES = 64   # BBA_ODOMETRY_CHUNK_ENTRIES
 
+# bba_loop_status
+LOOP_ACCEPTED, LOOP_NO_NEIGHBOUR, LOOP_ROTATION_DISAGREES, LOOP_TRANSLATION_DISAGREES, LOOP_CORRECTION_TOO_SMALL = range(5)
+LOOP_STATUS_NAMES = {0: "ACCEPTED", 1: "NO_NEIGHBOUR", 2: "ROTATION_DISAGREES", 3: "TRANSLATION_DISAGREES", 4: "CORRECTION_TOO_SMALL"}
+
+
+class LoopCandidate(C.Structure):   # bba_loop_candidate
+    _fields_ = [("current_keyframe_id", C.c_int), ("matched_keyframe_id", C.c_int), ("old_T_cur_initial", C.c_float * 7)]
+
+
+class LoopVerificationOptions(C.Structure):   # bba_loop_verification_options
+    _fields_ = [("odometry", OdometryOptions), ("max_angle_difference", C.c_float), ("max_translation_difference", C.c_float),
+                ("max_pixel_distance", C.c_float)]
+
+
+class LoopVerification(C.Structure):   # bba_loop_verification
+    _fields_ = [("status", C.c_int), ("tracked_keyframe_ids", C.c_int * 3), ("cur_T_old_refined", (C.c_float * 7) * 3),
+                ("cur_T_old", C.c_float * 7), ("angle_difference", C.c_float), ("translation_difference", C.c_float),
+                ("average_pixel_distance", C.c_float), ("pixel_count", C.c_uint32), ("tracking", OdometryResult * 3)]
+
 
 class Profile(C.Structure):
     _fields_ = [("pose_launches", C.c_uint64), ("pose_ms", C.c_double), ("kf_evals", C.c_uint64),
@@ -190,6 +209,8 @@ SYMBOLS = {
     "bba_host_pose_prior_terms": (None, [_P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_pose_constraint_terms": (None, [_P, _P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_robust_loss": (None, [C.c_int, C.c_float, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "bba_host_average_pose": (None, [C.c_int, _P, _P]),
+    "bba_host_loop_agreement": (C.c_int, [_P, C.c_float, C.c_float, _P, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     "bba_host_frusta_intersect": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, C.c_float, _P, C.c_float, C.c_float]),
     "bba_host_motion_model_clear": (None, [C.POINTER(MotionModelRecord), _P, _P]),
     "bba_host_motion_model_predict": (C.c_int, [C.POINTER(MotionModelRecord), C.c_int, _P, _P]),
@@ -217,6 +238,8 @@ SYMBOLS = {
     "bba_track_frame_pairwise_to_frame": (C.c_int, [_P, C.POINTER(OdometryOptions), _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t,
                                                     _P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, _F7, _F7, _F7,
                                                     C.POINTER(OdometryResult), _P]),
+    "bba_verify_loop_closures": (C.c_int, [_P, C.POINTER(LoopVerificationOptions), C.c_int, C.POINTER(LoopCandidate),
+                                           C.POINTER(LoopVerification), _P]),
     "bba_odometry_get_level": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_odometry_debug_coeffs": (C.c_int, [_P, C.c_int, C.c_int, _F7, _F7, _P, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_float),
                                             _P, _P, _P]),

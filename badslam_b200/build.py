@@ -36,6 +36,7 @@ UNITS = [
     ("multi_gpu.cu", []),
     ("local_group.cu", ["-Xptxas", "-v"]),   # (the all-reduce sums keep denormals: no -use_fast_math)
     ("frames.cu", []),
+    ("loop_verification.cu", ["-Xptxas", "-v"]),
 ]
 HEADERS = ["device_math.cuh", "exact_sum.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", "rendezvous.hpp", os.path.join("..", "..", "include", "badba.h")]
 

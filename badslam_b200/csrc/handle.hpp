@@ -4,7 +4,7 @@
 // Host units: badba.cu (handle, setters / getters, keyframes, textures, bba_host_*), pose_step.cu (spatial order, pose step),
 // pose_terms.cu (soft pose priors and constraints, their losses and staging, pose graph), bundle_adjust.cu (BA schemes,
 // intrinsics, PCG, surfel lifecycle), multi_gpu.cu (sharding, exchange, peer replicas), frames.cu (odometry, preprocessing).  None
-// of them contains a kernel.
+// of them contains a kernel.  loop_verification.cu (bba_verify_loop_closures) holds its host orchestration and its one kernel.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -106,6 +106,15 @@ using Event = Owned<cudaEvent_t, cudaEventDestroy>;
 struct Texture {
   Owned<cudaArray_t, cudaFreeArray> array;
   Owned<cudaTextureObject_t, cudaDestroyTextureObject> tex;
+};
+
+// One candidate of the necessity test of bba_verify_loop_closures (loop_verification.cu): its move cur_estimate_TR_cur_actual
+// (row-major 3x4) and its current keyframe's depth.
+struct LoopNecessityCandidate {
+  float T[12];
+  const uint16_t* depth;
+  uint32_t depth_pitch;   // bytes
+  uint32_t pad;
 };
 
 // ---- keyframes ---------------------------------------------------------------------------------------------------------------
@@ -430,6 +439,15 @@ struct bba_context {
     std::mutex call;           // serialises the front-end calls that use the buffers below and odo / pre
     bba::LumaStaging luma;
     std::vector<bba::Texture> frames;   // luma of the distinct frames of an odometry chunk, grown on demand
+    // bba_verify_loop_closures: the necessity test's candidates and its per-CTA partials (loop_verification.cu)
+    struct Loop {
+      bba::PinnedBuffer<bba::LoopNecessityCandidate> h_candidates;
+      bba::DeviceBuffer<bba::LoopNecessityCandidate> d_candidates;
+      bba::DeviceBuffer<double> d_sum;
+      bba::PinnedBuffer<double> h_sum;
+      bba::DeviceBuffer<unsigned int> d_count;
+      bba::PinnedBuffer<unsigned int> h_count;
+    } loop;
   } fe;
 
   // kernels launched by BA-side calls and by front-end calls (bba_kernel_launch_count: the sum); two counters so that the
@@ -580,6 +598,18 @@ bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::
 // Stages the pose-block terms of the PCG products at the current keyframe poses for LaunchPcgPoseTerms into h->pcg and uploads
 // them on s; none unless opt_poses.  gauge: the keyframe without pose unknowns.
 bba_status StagePcgPoseTerms(bba_handle h, bool opt_poses, int gauge, cudaStream_t s);
+
+// frames.cu
+// The option checks of every odometry call (num_scales, the depth / colour pyramid combination, the level sizes).
+bba_status CheckOdometryOptions(bba_handle h, const char* fn, const bba_odometry_options& o);
+// The odometry chunks of bba_track_frames_pairwise on a snapshot the caller took under fe.call, whose keyframe records kfs hold
+// every keyframe an entry names.  tracked_keyframe_ids: NULL, or per entry the stored keyframe that is its tracked image (-1: the
+// frame frames[tracked_frame] is).  release_slot: drop the snapshot's cfactor claim after the last chunk's pyramids (otherwise the
+// caller still reads it).  Writes out [count][7] and results (may be NULL); synchronises s once per chunk.
+bba_status TrackPairsOnSnapshot(bba_handle h, const bba_odometry_options& o, FrontEndCall& view, const std::vector<KeyframeView>& kfs,
+                                int frame_count, const bba_frame_buffers* frames, int count, const bba_odometry_entry* entries,
+                                const int* tracked_keyframe_ids, bool release_slot, float* out, bba_odometry_result* results,
+                                cudaStream_t s);
 
 // multi_gpu.cu
 void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t* shard_len);

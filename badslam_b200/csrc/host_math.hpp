@@ -567,6 +567,156 @@ BBA_HD void PoseConstraintInformationA(const float a_T_b[7], const float info[21
     }
 }
 
+// ---- loop-closure verification (bba_verify_loop_closures), host only ----
+// Eigen's Quaternion(Matrix3f) (Quaternion.h quaternionbase_assign_impl) on a row-major 3x3 matrix, fp32.
+inline void QuatFromMatrix(const float R[9], float q[4]) {
+  const auto m = [&](int r, int c) { return R[r * 3 + c]; };
+  float t = m(0, 0) + m(1, 1) + m(2, 2);
+  if (t > 0.f) {
+    t = sqrtf(t + 1.0f);
+    q[3] = 0.5f * t;
+    t = 0.5f / t;
+    q[0] = (m(2, 1) - m(1, 2)) * t;
+    q[1] = (m(0, 2) - m(2, 0)) * t;
+    q[2] = (m(1, 0) - m(0, 1)) * t;
+  } else {
+    int i = 0;
+    if (m(1, 1) > m(0, 0)) i = 1;
+    if (m(2, 2) > m(i, i)) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    t = sqrtf(m(i, i) - m(j, j) - m(k, k) + 1.0f);
+    q[i] = 0.5f * t;
+    t = 0.5f / t;
+    q[3] = (m(k, j) - m(j, k)) * t;
+    q[j] = (m(j, i) + m(i, j)) * t;
+    q[k] = (m(k, i) + m(i, k)) * t;
+  }
+}
+
+// The eigen-decomposition A = V diag(w) V^T of a symmetric 3x3 matrix (row-major) by cyclic Jacobi rotations in fp64, the
+// eigenvalues in descending order and V's columns the unit eigenvectors.
+inline void SymmetricEigen3(const double A_in[9], double w[3], double V[9]) {
+  double A[9];
+  for (int i = 0; i < 9; ++i) {
+    A[i] = A_in[i];
+    V[i] = (i % 4 == 0) ? 1.0 : 0.0;
+  }
+  for (int sweep = 0; sweep < 50; ++sweep) {
+    const double off = A[1] * A[1] + A[2] * A[2] + A[5] * A[5];
+    const double diag = A[0] * A[0] + A[4] * A[4] + A[8] * A[8];
+    if (off <= 1e-30 * diag || off == 0.0) break;
+    for (int p = 0; p < 2; ++p)
+      for (int q = p + 1; q < 3; ++q) {
+        const double apq = A[p * 3 + q];
+        if (apq == 0.0) continue;
+        const double theta = (A[q * 3 + q] - A[p * 3 + p]) / (2.0 * apq);
+        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < 3; ++k) {   // A <- A G (columns p, q), then G^T A (rows p, q)
+          const double akp = A[k * 3 + p], akq = A[k * 3 + q];
+          A[k * 3 + p] = c * akp - s * akq;
+          A[k * 3 + q] = s * akp + c * akq;
+        }
+        for (int k = 0; k < 3; ++k) {
+          const double apk = A[p * 3 + k], aqk = A[q * 3 + k];
+          A[p * 3 + k] = c * apk - s * aqk;
+          A[q * 3 + k] = s * apk + c * aqk;
+        }
+        for (int k = 0; k < 3; ++k) {
+          const double vkp = V[k * 3 + p], vkq = V[k * 3 + q];
+          V[k * 3 + p] = c * vkp - s * vkq;
+          V[k * 3 + q] = s * vkp + c * vkq;
+        }
+      }
+  }
+  int order[3] = {0, 1, 2};
+  for (int i = 0; i < 3; ++i)
+    for (int j = i + 1; j < 3; ++j)
+      if (A[order[j] * 4] > A[order[i] * 4]) { const int t = order[i]; order[i] = order[j]; order[j] = t; }
+  double Vs[9];
+  for (int c = 0; c < 3; ++c) {
+    w[c] = A[order[c] * 4];
+    for (int r = 0; r < 3; ++r) Vs[r * 3 + c] = V[r * 3 + order[c]];
+  }
+  for (int i = 0; i < 9; ++i) V[i] = Vs[i];
+}
+
+// AveragePose (util.cc:110-128): the rotation matrices and the translations of `count` poses summed in fp64; the rotation is U V^T
+// of the SVD M = U S V^T of the rotation sum, rounded to fp32 and set as Sophus' setRotationMatrix does (Eigen's matrix-to-
+// quaternion conversion, then normalised); the translation is the fp64 mean rounded to fp32.  The SVD comes from the
+// eigen-decomposition M^T M = V S^2 V^T: u_i = M v_i / s_i.  U V^T is the orthogonal polar factor of M, the same matrix whatever
+// signs an SVD routine picks for its singular vectors when M has full rank.  Like the reference, a sum with det < 0 is not
+// corrected: U V^T is then a reflection.  (A sum of rank < 3 -- rotations that cancel -- completes U by cross products.)
+inline Pose AveragePose(int count, const Pose* poses) {
+  double M[9] = {}, t[3] = {};
+  for (int i = 0; i < count; ++i) {
+    float R[9];
+    QuatToMatrix(poses[i].q, R);
+    for (int j = 0; j < 9; ++j) M[j] += static_cast<double>(R[j]);
+    for (int j = 0; j < 3; ++j) t[j] += static_cast<double>(poses[i].t[j]);
+  }
+  double MtM[9], s2[3], V[9];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) MtM[r * 3 + c] = M[r] * M[c] + M[3 + r] * M[3 + c] + M[6 + r] * M[6 + c];
+  SymmetricEigen3(MtM, s2, V);
+  double U[9] = {};
+  int rank = 0;
+  for (int c = 0; c < 3; ++c) {
+    const double s = sqrt(fmax(s2[c], 0.0));
+    if (!(s > 1e-12 * sqrt(fmax(s2[0], 0.0)))) break;
+    for (int r = 0; r < 3; ++r) U[r * 3 + c] = (M[r * 3] * V[c] + M[r * 3 + 1] * V[3 + c] + M[r * 3 + 2] * V[6 + c]) / s;
+    ++rank;
+  }
+  if (rank < 3) {   // complete U to an orthonormal basis
+    if (rank == 0) { U[0] = 1.0; rank = 1; }
+    if (rank == 1) {
+      const double a = fabs(U[0]) < 0.9 ? 1.0 : 0.0, b = 1.0 - a;   // any vector not parallel to u_1
+      double u[3] = {a - U[0] * (a * U[0] + b * U[3]), b - U[3] * (a * U[0] + b * U[3]), -U[6] * (a * U[0] + b * U[3])};
+      const double n = sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);
+      for (int r = 0; r < 3; ++r) U[r * 3 + 1] = u[r] / n;
+    }
+    U[2] = U[3] * U[7] - U[6] * U[4];
+    U[5] = U[6] * U[1] - U[0] * U[7];
+    U[8] = U[0] * U[4] - U[3] * U[1];
+  }
+  float Rf[9];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c)
+      Rf[r * 3 + c] = static_cast<float>(U[r * 3] * V[c * 3] + U[r * 3 + 1] * V[c * 3 + 1] + U[r * 3 + 2] * V[c * 3 + 2]);
+  Pose out;
+  QuatFromMatrix(Rf, out.q);
+  QuatNormalize(out.q);
+  for (int j = 0; j < 3; ++j) out.t[j] = static_cast<float>(t[j] / (1.0 * count));
+  return out;
+}
+
+// The agreement test of three refined cur_T_old estimates (loop_detector.cc:575-609), in fp32 like Sophus: for the pairs (0, 1),
+// (0, 2), (1, 2) in this order, the rotational distance acos(clamp(dot of the third columns of the two rotation matrices)) --
+// blind to a roll about the optical axis, as in the reference -- is tested first, then the Euclidean distance of the translations.
+// The 3-vector dot product and squared norm reduce as Eigen's unrolled redux does, a0 + (a1 + a2).  Returns 0 when every pair
+// agrees, 2 (BBA_LOOP_ROTATION_DISAGREES) or 3 (BBA_LOOP_TRANSLATION_DISAGREES) for the first failed test; *angle and
+// *translation receive the largest distances over all three pairs.
+inline int LoopAgreement(const Pose refined[3], float max_angle, float max_translation, float* angle, float* translation) {
+  int status = 0;
+  *angle = 0.f;
+  *translation = 0.f;
+  for (int i = 0; i < 2; ++i)
+    for (int k = i + 1; k < 3; ++k) {
+      float Ri[9], Rk[9];
+      QuatToMatrix(refined[i].q, Ri);
+      QuatToMatrix(refined[k].q, Rk);
+      const float dot = Ri[2] * Rk[2] + (Ri[5] * Rk[5] + Ri[8] * Rk[8]);
+      const float rotational = acosf(fminf(1.f, fmaxf(-1.f, dot)));
+      const float d[3] = {refined[i].t[0] - refined[k].t[0], refined[i].t[1] - refined[k].t[1], refined[i].t[2] - refined[k].t[2]};
+      const float translational = sqrtf(d[0] * d[0] + (d[1] * d[1] + d[2] * d[2]));
+      if (status == 0 && rotational > max_angle) status = 2;
+      if (status == 0 && translational > max_translation) status = 3;
+      *angle = fmaxf(*angle, rotational);
+      *translation = fmaxf(*translation, translational);
+    }
+  return status;
+}
+
 // Camera frusta and their intersection test (co-visibility of keyframes), host only.
 struct Frustum {   // libvis/src/libvis/camera_frustum.h:43-250
   float p[8][3];

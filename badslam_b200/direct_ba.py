@@ -857,6 +857,24 @@ class DirectBA:
                                                         C.byref(launches), self._stream_ptr(stream)))
         return out, list(results), launches.value
 
+    def VerifyLoopClosures(self, stream, candidates, num_scales: int = 5, use_pyramid_level_0: bool = True,
+                           use_gradmag: bool = False, max_iterations_per_scale: int = 30, max_angle_difference: float = 0.0,
+                           max_translation_difference: float = 0.0, max_pixel_distance: float = 0.0):
+        """LoopDetector's verification of loop-closure candidates (loop_detector.cc:436-668, bba_verify_loop_closures): each
+        (current_keyframe_id, matched_keyframe_id, old_T_cur_initial[7]) is refined against the matched keyframe and its two
+        neighbours, the three estimates are tested for agreement and averaged, and the correction is tested for necessity.
+        Thresholds <= 0 select the reference's (10 deg, 0.02 m, 1 px).  Returns a list of the count LoopVerification records;
+        `status` is one of _lib.LOOP_*, and cur_T_old is the loop edge a_T_b for AddKeyframePoseConstraints(current, matched)."""
+        cands = (_lib.LoopCandidate * len(candidates))()
+        for c, spec in zip(cands, candidates):
+            c.current_keyframe_id, c.matched_keyframe_id = int(spec[0]), int(spec[1])
+            c.old_T_cur_initial[:] = np.ascontiguousarray(spec[2], np.float32).reshape(7).tolist()
+        o = _lib.LoopVerificationOptions(_odometry_options(num_scales, use_pyramid_level_0, use_gradmag, False, max_iterations_per_scale),
+                                         float(max_angle_difference), float(max_translation_difference), float(max_pixel_distance))
+        out = (_lib.LoopVerification * max(1, len(candidates)))()
+        self._check(self._lib.bba_verify_loop_closures(self._h, C.byref(o), len(candidates), cands, out, self._stream_ptr(stream)))
+        return list(out)[:len(candidates)]
+
     def OdometryLevel(self, which: int, scale: int, stream=None):
         """Parity hook: (depth f32, normals u16, colour u8) of one pyramid level of the last TrackFramePairwise call
         (which: 0 = base keyframe, 1 = tracked frame)."""

@@ -24,8 +24,8 @@
  *      front-end side: one further thread may make one call at a time, on its own stream, while a
  *        BA-side call is in flight -- also from inside progress_function.  The front-end calls are
  *        bba_preprocess_frame, bba_preprocess_raw_frame, bba_track_frame_pairwise,
- *        bba_track_frame_pairwise_to_frame, bba_track_frames_pairwise, bba_odometry_get_level,
- *        bba_odometry_debug_coeffs, the
+ *        bba_track_frame_pairwise_to_frame, bba_track_frames_pairwise, bba_verify_loop_closures,
+ *        bba_odometry_get_level, bba_odometry_debug_coeffs, the
  *        bba_host_* functions (no handle) and the readers bba_keyframe_count, bba_get_keyframe_pose,
  *        bba_get_keyframe_states, bba_get_keyframe_activation, bba_get_intrinsics,
  *        bba_get_cfactor_host, bba_cfactor_size and bba_get_residual_types.
@@ -766,13 +766,76 @@ bba_status bba_odometry_debug_coeffs(bba_handle h, int scale, int use_gradmag, c
                                      float H[21], float b[6], uint32_t* residual_count, float* residual_sum,
                                      uint32_t counts[2], float costs[2], void* stream);
 
+/* ---- loop-closure verification (DESIGN.md §3.16) ----
+ * LoopDetector's check of a loop-closure candidate before the pose graph sees it (loop_detector.cc:436-668): the step of a loop
+ * closure between the caller's place recognition (DBoW2, features and RANSAC, which give old_T_cur_initial) and
+ * AddKeyframePoseConstraint + bba_optimize_pose_graph + bba_deform_surfels.  For every candidate, with K the published keyframe
+ * count:
+ *  - neighbours (:455-496): next = matched + 1 (none unless < K: NO_NEIGHBOUR); previous = matched - 1, or next + 1 when matched is
+ *    0 (none unless < K: NO_NEIGHBOUR).  The current keyframe is not excluded, as in the reference;
+ *  - tracking (:498-548): for old_i in (matched, next, previous) with matched_T_this = matched.frame_T_global * old_i.global_T_frame
+ *    (identity for i = 0), keyframe old_i is tracked against the current keyframe as the base by the image-pair odometry of
+ *    bba_track_frames_pairwise, from old_T_cur_initial^-1 * matched_T_this as both initial estimates; cur_T_old_refined[i] =
+ *    (matched_T_this * cur_T_tracked^-1)^-1.  All 3 x count pairs run through its chunks (one tracking launch per 64 pairs);
+ *  - agreement (:575-599): the pairs (0, 1), (0, 2), (1, 2) in this order, the rotation first: acos of the dot product of the two
+ *    rotation matrices' third columns (blind to a roll about the optical axis, as in the reference) above max_angle_difference
+ *    gives ROTATION_DISAGREES, the distance of the translations above max_translation_difference TRANSLATION_DISAGREES;
+ *  - average (:609, AveragePose util.cc:110-128): cur_T_old = U V^T of the SVD of the summed rotation matrices (fp64; a reflection
+ *    is not corrected, as in the reference) and the mean translation; it is written whenever the tracking ran;
+ *  - necessity (:630-666): every valid depth pixel of the current keyframe, unprojected at its centre with the calibrated depth
+ *    (a, cfactor) and moved by (cur_T_old * matched.frame_T_global) * current.global_T_frame, is projected with and without the
+ *    move by the colour camera (pixel-corner convention, no border); the mean distance over the pixels whose both projections
+ *    are in the image is average_pixel_distance (NaN without such a pixel), and with at least 5 such pixels and a mean at most
+ *    max_pixel_distance the candidate gets CORRECTION_TOO_SMALL: BA can close it alone.  The reference measures its matched
+ *    keypoints instead; one launch serves every candidate that passed the agreement test, with fp64 per-CTA partials summed in a
+ *    fixed order on the host.
+ * The call reads the published snapshot (cameras, a, cfactor, residual types, keyframe poses and images) and changes nothing on
+ * the handle: the caller decides what to do with the result, e.g. add cur_T_old as the constraint a_T_b of (current, matched).
+ * In the deterministic mode the results are bit-identical from call to call and to the same candidate verified alone, and
+ * tracking[i] / cur_T_old_refined[i] equal bba_track_frames_pairwise on the same pair with old_i's buffers given as a frame.
+ * BBA_ERR_INVALID_ARGUMENT: a NULL options, candidates or out, count < 1, a keyframe id outside the published keyframes, current ==
+ * matched, a non-finite old_T_cur_initial or one with a zero quaternion, a non-finite threshold, test_different_initial_estimates
+ * set or odometry options bba_track_frames_pairwise refuses (BBA_ERR_UNSUPPORTED for its unsupported pyramid combination).
+ * Arguments are checked before anything is enqueued, and a failed check leaves the handle and the launch counter unchanged.
+ * A front-end call; synchronises the stream once per 64 tracked pairs and once for the necessity test. */
+typedef enum {
+  BBA_LOOP_ACCEPTED = 0,
+  BBA_LOOP_NO_NEIGHBOUR = 1,           /* loop_detector.cc:464-496 */
+  BBA_LOOP_ROTATION_DISAGREES = 2,     /* :582-590 */
+  BBA_LOOP_TRANSLATION_DISAGREES = 3,  /* :592-599 */
+  BBA_LOOP_CORRECTION_TOO_SMALL = 4    /* :656-666: BA can close it; the caller may still use cur_T_old */
+} bba_loop_status;
+typedef struct {
+  int current_keyframe_id;     /* the new keyframe (the reference's current_keyframe) */
+  int matched_keyframe_id;     /* the place recogniser's match (result.match) */
+  float old_T_cur_initial[7];  /* the caller's initial estimate, e.g. its RANSAC (loop_detector.cc:358-360) */
+} bba_loop_candidate;
+typedef struct {
+  bba_odometry_options odometry;     /* as for bba_track_frames_pairwise; test_different_initial_estimates must be 0 (:541) */
+  float max_angle_difference;        /* rad, <= 0: 10 deg (kMaxAngleDifference, :577) */
+  float max_translation_difference;  /* m,   <= 0: 0.02   (kMaxEuclideanDistance, :578) */
+  float max_pixel_distance;          /* px,  <= 0: 1.0    (kAveragePixelDistanceThreshold, :656) */
+} bba_loop_verification_options;
+typedef struct {
+  int status;                        /* bba_loop_status */
+  int tracked_keyframe_ids[3];       /* matched, next, previous (or the second next); -1 where none */
+  float cur_T_old_refined[3][7];     /* the three refined estimates (:546-547); zero with NO_NEIGHBOUR */
+  float cur_T_old[7];                /* their AveragePose: the loop edge a_T_b for (current, matched); zero with NO_NEIGHBOUR */
+  float angle_difference, translation_difference;   /* the largest over the three pairs */
+  float average_pixel_distance;      /* the necessity test; NaN where it did not run or counted no pixel */
+  uint32_t pixel_count;
+  bba_odometry_result tracking[3];
+} bba_loop_verification;
+bba_status bba_verify_loop_closures(bba_handle h, const bba_loop_verification_options* options, int count,
+                                    const bba_loop_candidate* candidates, bba_loop_verification* out, void* stream);
+
 /* ---- deterministic mode ----
  * Off by default.  When on, every floating-point sum whose order depends on the scheduling of the GPU goes through an exact,
  * order-independent accumulator (or, in the odometry kernel, a fixed-order sum of per-CTA totals), so that the same inputs on the
  * same GPU model give the same results bit for bit in every run, whatever else runs beside them on other streams.  Covered:
  * bba_bundle_adjust (pose, geometry and intrinsics steps, surfel lifecycle), bba_estimate_frame_pose (both forms),
  * bba_estimate_frame_poses_for_frames, bba_accumulate_pose_coeffs, bba_debug_pose_coeffs_batch, bba_optimize_intrinsics, bba_track_frame_pairwise(_to_frame),
- * bba_track_frames_pairwise,
+ * bba_track_frames_pairwise, bba_verify_loop_closures,
  * bba_odometry_debug_coeffs and the preprocessing.  The results differ from those of the default mode only by the rounding of
  * those sums.  Not covered: the PCG solver -- bba_bundle_adjust with use_pcg and bba_pcg_debug return BBA_ERR_UNSUPPORTED while
  * the mode is on -- and more than one rank (the setter returns BBA_ERR_UNSUPPORTED for world_size > 1).  A call with
@@ -814,6 +877,14 @@ void bba_host_pose_constraint_terms(const float a_T_b[7], const float global_T_a
 /* The robust loss of a pose term (bba_robust_loss) at s = r^T L r: *rho = rho(s) and *weight = rho'(s), in fp64, as the solvers
  * evaluate them.  An unknown type counts as TRIVIAL.  Writes nothing if a pointer is NULL. */
 void bba_host_robust_loss(int type, float scale, double s, double* rho, double* weight);
+/* The host steps of bba_verify_loop_closures.  bba_host_average_pose: AveragePose (util.cc:110-128) of count >= 1 poses [count][7]
+ * (writes nothing for count < 1 or a NULL pointer).  bba_host_loop_agreement: the agreement test of the three refined cur_T_old
+ * estimates [3][7] (thresholds <= 0 select 10 deg and 0.02 m); returns BBA_LOOP_ACCEPTED, BBA_LOOP_ROTATION_DISAGREES or
+ * BBA_LOOP_TRANSLATION_DISAGREES, writes their AveragePose to out_average and the largest distances over the three pairs (each
+ * output may be NULL); -1 for a NULL cur_T_old_refined. */
+void bba_host_average_pose(int count, const float* poses, float out[7]);
+int  bba_host_loop_agreement(const float cur_T_old_refined[21], float max_angle, float max_translation, float out_average[7],
+                             float* angle_difference, float* translation_difference);
 int  bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height,
                                const float global_T_frame_a[7], float min_depth_a, float max_depth_a,
                                const float global_T_frame_b[7], float min_depth_b, float max_depth_b);

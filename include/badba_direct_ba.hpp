@@ -235,6 +235,23 @@ class DirectBA {
     for (size_t i = 0; i < count; ++i) std::memcpy((*out_base_T_frame_estimates)[i].data(), out.data() + 7 * i, sizeof(float) * 7);
   }
 
+  // LoopDetector's verification of loop-closure candidates (loop_detector.cc:436-668, bba_verify_loop_closures): each candidate's
+  // initial old_T_cur is refined against the matched keyframe and its two neighbours, the three estimates are tested for agreement
+  // and averaged, and the correction is tested for necessity.  Thresholds <= 0 select the reference's.  out->at(i).status is a
+  // bba_loop_status; on BBA_LOOP_ACCEPTED, cur_T_old is the loop edge for AddKeyframePoseConstraint(current, matched, ...).
+  void VerifyLoopClosures(cudaStream_t stream, const std::vector<bba_loop_candidate>& candidates, bool use_pyramid_level_0,
+                          bool use_gradmag, std::vector<bba_loop_verification>* out, int num_scales = 5,
+                          float max_angle_difference = 0, float max_translation_difference = 0, float max_pixel_distance = 0) {
+    bba_loop_verification_options o{};
+    o.odometry = MakeOdometryOptions(num_scales, use_pyramid_level_0, use_gradmag, /*test_different_initial_estimates=*/false);
+    o.max_angle_difference = max_angle_difference;
+    o.max_translation_difference = max_translation_difference;
+    o.max_pixel_distance = max_pixel_distance;
+    out->resize(candidates.size());
+    Check(bba_verify_loop_closures(h_, &o, static_cast<int>(candidates.size()), candidates.data(), out->data(), stream),
+          "bba_verify_loop_closures");
+  }
+
   // direct_ba.h:143-162, same argument order and defaults (Timer* is any type with GetTimeSinceStart()).
   template <typename TimerT = NoTimer>
   void BundleAdjustment(cudaStream_t stream, bool optimize_depth_intrinsics, bool optimize_color_intrinsics, bool do_surfel_updates,
