@@ -97,6 +97,11 @@ class RobustLoss(C.Structure):   # bba_robust_loss
     _fields_ = [("type", C.c_int), ("scale", C.c_float)]
 
 
+class AttitudePrior(C.Structure):   # bba_attitude_prior
+    _fields_ = [("reference_direction", C.c_float * 3), ("measured_direction", C.c_float * 3), ("information", C.c_float),
+                ("loss", RobustLoss)]
+
+
 class PoseGraphOptions(C.Structure):   # bba_pose_graph_options
     _fields_ = [("gauge_keyframe", C.c_int), ("max_iterations", C.c_int), ("use_odometry_chain", C.c_int),
                 ("odometry_information", C.c_float * 21)]
@@ -198,6 +203,10 @@ SYMBOLS = {
     "bba_get_keyframe_pose_prior_loss": (C.c_int, [_P, C.c_int, C.POINTER(RobustLoss)]),
     "bba_get_keyframe_pose_constraint_losses": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
     "bba_evaluate_keyframe_pose_terms": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, _P, _P, _P]),
+    "bba_set_keyframe_attitude_priors": (C.c_int, [_P, C.c_int, _P, _P]),
+    "bba_clear_keyframe_attitude_priors": (C.c_int, [_P, C.c_int, _P]),
+    "bba_get_keyframe_attitude_prior": (C.c_int, [_P, C.c_int, C.POINTER(AttitudePrior), C.POINTER(C.c_int)]),
+    "bba_evaluate_keyframe_attitude_priors": (C.c_int, [_P, C.c_int, _P, _P, _P]),
     "bba_set_intrinsics": (C.c_int, [_P, _F7, _F7, C.c_float]),
     "bba_get_intrinsics": (C.c_int, [_P, _F7, _F7, C.POINTER(C.c_float)]),
     "bba_host_se3_exp": (None, [_P, _P]),
@@ -209,6 +218,7 @@ SYMBOLS = {
     "bba_host_pose_prior_terms": (None, [_P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_pose_constraint_terms": (None, [_P, _P, _P, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_robust_loss": (None, [C.c_int, C.c_float, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "bba_host_attitude_prior_terms": (None, [_P, _P, C.c_float, _P, _P, _P, C.POINTER(C.c_double)]),
     "bba_host_average_pose": (None, [C.c_int, _P, _P]),
     "bba_host_loop_agreement": (C.c_int, [_P, C.c_float, C.c_float, _P, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     "bba_host_frusta_intersect": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, C.c_float, _P, C.c_float, C.c_float]),

@@ -105,6 +105,7 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
     v.min_depth = kf.min_depth; v.max_depth = kf.max_depth;
     v.activation = kf.activation;
     v.prior = h->pose_priors[k];
+    v.attitude = h->attitude_priors[k];
   }
   const CameraView cams = LiveCameraView(h);
   std::vector<PoseConstraint> constraints = h->pose_constraints;
@@ -354,6 +355,7 @@ bba_status bba_create(const bba_config* cfg, bba_handle* out) {
   CREATE_TRY(cudaMemset(h->d_cfactor, 0, sizeof(float) * h->cf_w * h->cf_h));
   CREATE_TRY(h->d_kfs.Reserve(K));
   h->pose_priors.assign(K, bba::PosePrior{});
+  h->attitude_priors.assign(K, bba::AttitudePrior{});
   CREATE_TRY(p.d_work_records.Reserve(K));
   CREATE_TRY(p.d_pose_est.Reserve(7 * K));
   CREATE_TRY(p.d_acc.Reserve(bba::kPoseAccSize * K));
@@ -582,6 +584,11 @@ void bba_host_pose_constraint_terms(const float a_T_b[7], const float pose_a[7],
 void bba_host_robust_loss(int type, float scale, double s, double* rho, double* weight) {
   if (!rho || !weight) return;
   bba::RobustLoss(type, scale, s, rho, weight);
+}
+void bba_host_attitude_prior_terms(const float d_ref[3], const float d_meas[3], float information, const float pose[7], double H[21],
+                                   double b[6], double* cost) {
+  if (!d_ref || !d_meas || !pose || !H || !b || !cost) return;
+  bba::AttitudePriorTerms(d_ref, d_meas, information, pose, H, b, cost);
 }
 int bba_host_frusta_intersect(const float depth_intrinsics[4], int width, int height, const float global_T_frame_a[7], float min_depth_a,
                               float max_depth_a, const float global_T_frame_b[7], float min_depth_b, float max_depth_b) {

@@ -160,6 +160,7 @@ struct KeyframeView {
   float min_depth = 0.f, max_depth = 0.f;
   int activation = BBA_KF_ACTIVE;
   PosePrior prior{};
+  AttitudePrior attitude{};
 };
 
 // A soft relative pose constraint as the handle keeps it: its id, the caller's record, and the information of the equivalent
@@ -217,6 +218,10 @@ struct bba_context {
   // constraint the pose solve and the PCG solver run without pose terms
   std::vector<bba::PosePrior> pose_priors;   // [max_kf]
   int pose_prior_count = 0;
+  // attitude priors by keyframe id (bba_set_keyframe_attitude_priors) and how many keyframes have one; with none every solver
+  // runs without them
+  std::vector<bba::AttitudePrior> attitude_priors;   // [max_kf]
+  int attitude_prior_count = 0;
   // soft relative pose constraints (bba_add_keyframe_pose_constraints) in id order, and the id the next one gets
   std::vector<bba::PoseConstraint> pose_constraints;
   int next_pose_constraint_id = 0;
@@ -263,6 +268,9 @@ struct bba_context {
     bba::DeviceBuffer<int> d_term_offsets;
     bba::PinnedBuffer<bba::PoseTerm> h_terms;
     bba::DeviceBuffer<bba::PoseTerm> d_terms;
+    // the attitude priors [max_kf], staged with the terms when a keyframe has one
+    bba::PinnedBuffer<bba::AttitudePrior> h_attitude;
+    bba::DeviceBuffer<bba::AttitudePrior> d_attitude;
     // Spatial order of the surfels (bba::LaunchSpatialOrder) and the pose step's stream in that order (bba::LaunchPoseStream); the
     // geometry step's stream (bba::LaunchGeometryStream) shares the buffer.
     // The order is rebuilt at the start of every BA call, after an in-loop change of the surfel set, and whenever the surfel
@@ -323,6 +331,8 @@ struct bba_context {
     bba::DeviceBuffer<int> d_ints;
     bba::PinnedBuffer<float> h_poses;        // [max_kf][7]
     bba::DeviceBuffer<float> d_poses;        // [2][max_kf][7]: the poses, then the poses before the last step
+    bba::PinnedBuffer<float> h_hold_axes;    // [max_kf][3] PoseGraphArgs::hold_axis
+    bba::DeviceBuffer<float> d_hold_axes;
     bba::DeviceBuffer<double> d_doubles;
     bba::DeviceBuffer<bba::PoseGraphState> d_state;
     bba::PinnedBuffer<bba::PoseGraphState> h_state;
@@ -593,8 +603,10 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
 
 // pose_terms.cu
 // Stages the soft pose terms of the keyframes in `ids` (start poses init) for PoseSolveKernel into h->pose and uploads them on s.
-// *staged: false when the handle has no prior and no constraint (then nothing is staged).
-bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, cudaStream_t s, bool* staged);
+// *staged: false when the handle has no prior and no constraint (then no term is staged); *attitude: whether the attitude
+// priors were staged (h->pose.d_attitude), false when no keyframe has one.
+bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, cudaStream_t s, bool* staged,
+                          bool* attitude);
 // Stages the pose-block terms of the PCG products at the current keyframe poses for LaunchPcgPoseTerms into h->pcg and uploads
 // them on s; none unless opt_poses.  gauge: the keyframe without pose unknowns.
 bba_status StagePcgPoseTerms(bba_handle h, bool opt_poses, int gauge, cudaStream_t s);

@@ -460,6 +460,50 @@ BBA_HD void PosePriorTerms(const float prior[7], const float pose[7], const floa
   InformationTerms<6>(r, J, info, H, b, cost);
 }
 
+// ---- attitude prior on a keyframe (bba_set_keyframe_attitude_priors, DESIGN §3.17) ----
+// The attitude prior's terms at global_T_frame = pose, for an update pose <- pose * exp(delta).  p = R^-1 d_ref is the predicted
+// direction in the camera frame and m = d_meas the measured one (both normalised here); theta in [0, pi] is their angle and the
+// term costs L theta^2 / 2.  The residual is r = theta n with n = (p x m) / |p x m|, the rotation vector that turns p into m.
+//   b = L theta n: the exact gradient (d theta = n . omega for the rotation part omega of delta; at theta = pi exactly, p x m = 0
+//       and b = 0).
+//   H = L (I - p p^T) in the rotation block: r's Gauss-Newton matrix at theta = 0, which stays finite at every angle (the exact one
+//       grows as (theta / sin theta)^2 across the great circle through p and m).
+// The translation rows of H and b are zero and p, the yaw axis about d_ref, is H's null direction.  H: upper triangle (21) in the
+// tangent order (translation, rotation); cost = L theta^2 / 2.  fp64 throughout.
+BBA_HD void AttitudePriorTerms(const float d_ref[3], const float d_meas[3], float information, const float pose[7], double H[21],
+                               double b[6], double* cost) {
+  double q[4], t[3], d[3], m[3], nd = 0.0, nm = 0.0;
+  LoadPoseD(pose, q, t);
+  for (int i = 0; i < 3; ++i) {
+    d[i] = d_ref[i];
+    m[i] = d_meas[i];
+    nd += d[i] * d[i];
+    nm += m[i] * m[i];
+  }
+  nd = 1.0 / sqrt(nd);
+  nm = 1.0 / sqrt(nm);
+  for (int i = 0; i < 3; ++i) {
+    d[i] *= nd;
+    m[i] *= nm;
+  }
+  // p = R^T d: rotate d by conj(q), as Se3BetweenD
+  const double ax = -q[0], ay = -q[1], az = -q[2], aw = q[3];
+  const double ux = 2.0 * (ay * d[2] - az * d[1]), uy = 2.0 * (az * d[0] - ax * d[2]), uz = 2.0 * (ax * d[1] - ay * d[0]);
+  const double p[3] = {d[0] + aw * ux + (ay * uz - az * uy), d[1] + aw * uy + (az * ux - ax * uz), d[2] + aw * uz + (ax * uy - ay * ux)};
+  const double x[3] = {p[1] * m[2] - p[2] * m[1], p[2] * m[0] - p[0] * m[2], p[0] * m[1] - p[1] * m[0]};   // p x m
+  const double s = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]), c = p[0] * m[0] + p[1] * m[1] + p[2] * m[2];
+  const double theta = atan2(s, c);
+  const double f = s > 0.0 ? theta / s : 1.0;   // |x| = sin theta; p x m = 0 at 0 and pi, where b = 0
+  const double L = information;
+  int idx = 0;
+  for (int r = 0; r < 6; ++r) {
+    b[r] = r < 3 ? 0.0 : L * f * x[r - 3];
+    for (int col = r; col < 6; ++col, ++idx)
+      H[idx] = r < 3 ? 0.0 : L * ((r == col ? 1.0 : 0.0) - p[r - 3] * p[col - 3]);
+  }
+  *cost = 0.5 * L * theta * theta;
+}
+
 // The robust loss of a pose term (bba_robust_loss, Ceres' conventions): a term whose squared Mahalanobis norm is s = r^T L r costs
 // rho(s) / 2 instead of s / 2, and IRLS scales its H and b by w = rho'(s).  type: 0 trivial (rho = s), 1 Huber, 2 Cauchy; scale =
 // delta in units of sqrt(s).  An inlier under Huber (s <= delta^2) gets rho = s and w = 1.0 exactly, as the trivial loss does.

@@ -22,6 +22,13 @@ struct PoseTerm {
   bba_robust_loss loss;
 };
 
+// A keyframe's attitude prior (bba_set_keyframe_attitude_priors, host_math.hpp AttitudePriorTerms): the caller's record with both
+// directions normalised, its loss inside; has = 0: the keyframe has none.
+struct AttitudePrior {
+  bba_attitude_prior p;
+  int has;
+};
+
 // Accumulator record per keyframe written by the pose kernel: 32 fp64 sums
 //   [0..20] H upper triangle row-major, [21..26] b, [27] n_assoc, [28] n_photo,
 //   [29] cost_depth, [30] cost_desc1, [31] cost_desc2
@@ -117,14 +124,19 @@ struct PoseSolveArgs {
   // both null when no keyframe has one
   const int* term_offsets;     // [keyframes + 1]
   const PoseTerm* terms;
+  // the attitude priors by keyframe id, added after the terms; null when no keyframe has one
+  const AttitudePrior* attitude;   // [keyframes]
 };
 // Device-side Gauss-Newton step for every keyframe in the list (direct_ba_alternating.cc:173-233).
 LaunchResult LaunchPoseSolve(const PoseSolveArgs& args, cudaStream_t stream);
 
 // Keyframe pose graph (pose_graph.cu; bba_optimize_pose_graph, DESIGN §3.14).  One term of the cost: a soft pose prior on
-// keyframe a (b = -1, z = the prior's global_T_frame), or a relative pose constraint (a, b, z = a_T_b): a handle constraint
-// or an odometry-chain edge of the call.  info: the upper triangle of L.  loss: the term's robust loss (host_math.hpp RobustLoss:
-// its blocks are scaled by w at the current poses and it costs rho(s) / 2); TRIVIAL for a chain edge.
+// keyframe a (b = -1, z = the prior's global_T_frame), an attitude prior on keyframe a (b = kPoseGraphAttitude, z[0..3) = d_ref,
+// z[3..6) = d_meas, info[0] = L; DESIGN §3.17), or a relative pose constraint (a, b, z = a_T_b): a handle constraint or an
+// odometry-chain edge of the call.  info: the upper triangle of L.  loss: the term's robust loss (host_math.hpp RobustLoss:
+// its blocks are scaled by w at the current poses and it costs rho(s) / 2); TRIVIAL for a chain edge.  Every unary term (b < 0)
+// has the 21 + 6 blocks of a prior.
+constexpr int kPoseGraphAttitude = -2;
 struct PoseGraphTerm {
   int a, b;
   float z[7];
@@ -154,7 +166,9 @@ struct PoseGraphArgs {
   PoseGraphTermBlocks* blocks;   // [term_count]
   float* poses;                  // [K][7] global_T_frame, updated in place
   float* prev;                   // [K][7] the poses before the last step (a rejected step reverts to them)
-  const int* held;               // [K] 1: the keyframe keeps its pose (an identity row of H)
+  const int* held;               // [K] 1: the keyframe keeps its pose (an identity row of H); 2: it keeps its translation and
+                                 //   its rotation about hold_axis (the update is projected, DESIGN §3.17)
+  const float* hold_axis;        // [K][3] for held = 2: a unit direction in the map frame, or 0 (translation only); else null
   const int* row_off;            // [K + 1] into row_terms
   const int* row_terms;          // [2 per entry] (term, side 0 = a / 1 = b): the terms of row block k in term order
   const int* csr_off;            // [K + 1] block-CSR of H: row k's blocks [csr_off[k], csr_off[k + 1]), the diagonal first,

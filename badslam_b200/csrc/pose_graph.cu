@@ -3,11 +3,12 @@
 //
 // One Gauss-Newton iteration is one round of four kernels, and the host enqueues every round without synchronising: the state
 // (PoseGraphState) decides on the device whether the last step is kept, and once it is done every later kernel returns at once.
-//   PoseGraphLinearizeKernel  one thread per term: PosePriorTerms / PoseConstraintTerms at the fp32 poses, in fp64, scaled by the
-//                             IRLS weight of the term's loss, the cost rho(s) / 2 (w = 1 and rho(s) / 2 = cost exactly for a
-//                             trivial loss).
+//   PoseGraphLinearizeKernel  one thread per term: PosePriorTerms / AttitudePriorTerms / PoseConstraintTerms at the fp32 poses,
+//                             in fp64, scaled by the IRLS weight of the term's loss, the cost rho(s) / 2 (w = 1 and rho(s) / 2 =
+//                             cost exactly for a trivial loss).
 //   PoseGraphAssembleKernel   one thread per row block: H_kk, b_k, the block-CSR row and the coupling H_{k,k+1}, summed over the
-//                             row's terms in term order.  A held keyframe's row is the identity with a zero right-hand side.
+//                             row's terms in term order.  A held keyframe's row is the identity with a zero right-hand side; a
+//                             partially held one's is projected (DESIGN §3.17).
 //   PoseGraphSolveKernel      one CTA: the cost at the current poses (a fixed-order sum) and the test of the last step, then
 //                             H delta = -b by PCG.  The preconditioner M is the block-tridiagonal part of H in keyframe order,
 //                             factorised by odd-even (cyclic) reduction; every 6x6 pivot is an LDLT in SolveLDLT's convention,
@@ -185,7 +186,9 @@ __global__ void __launch_bounds__(64) PoseGraphLinearizeKernel(const PoseGraphAr
   if (t >= a.term_count) return;
   const PoseGraphTerm& term = a.terms[t];
   PoseGraphTermBlocks& blk = a.blocks[t];
-  if (term.b < 0) {
+  if (term.b == kPoseGraphAttitude) {
+    AttitudePriorTerms(term.z, term.z + 3, term.info[0], a.poses + 7 * term.a, blk.H, blk.b, &blk.cost);
+  } else if (term.b < 0) {
     PosePriorTerms(term.z, a.poses + 7 * term.a, term.info, blk.H, blk.b, &blk.cost);
   } else {
     double r[6];
@@ -204,6 +207,41 @@ __global__ void __launch_bounds__(64) PoseGraphLinearizeKernel(const PoseGraphAr
   }
 }
 
+// Q = I - u u^T for a partially held keyframe (held = 2), u = R^-1 hold_axis its held rotation axis in the camera frame, or Q = I
+// when hold_axis is 0 (translation only): the keyframe's update is P delta with P = diag(0, 0, 0, Q).
+__device__ void HoldProjection(const PoseGraphArgs& a, int k, double Q[9]) {
+  double q[4], t[3];
+  LoadPoseD(a.poses + 7 * k, q, t);
+  const float* d = a.hold_axis + 3 * k;
+  const double ax = -q[0], ay = -q[1], az = -q[2], aw = q[3];   // u = R^T d (rotation by conj(q), as Se3BetweenD)
+  const double ux = 2.0 * (ay * d[2] - az * d[1]), uy = 2.0 * (az * d[0] - ax * d[2]), uz = 2.0 * (ax * d[1] - ay * d[0]);
+  const double u[3] = {d[0] + aw * ux + (ay * uz - az * uy), d[1] + aw * uy + (az * ux - ax * uz), d[2] + aw * uz + (ax * uy - ay * ux)};
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) Q[r * 3 + c] = (r == c ? 1.0 : 0.0) - u[r] * u[c];
+}
+
+// X <- P_l X P_r for a 6x6 row-major block, P = diag(0, 0, 0, Q); a null Q leaves that side as it is.
+__device__ void ProjectBlock(const double* Ql, double* X, const double* Qr) {
+  if (Ql)
+    for (int c = 0; c < 6; ++c) {
+      const double v[3] = {X[18 + c], X[24 + c], X[30 + c]};
+      for (int r = 0; r < 3; ++r) {
+        X[r * 6 + c] = 0.0;
+        X[(3 + r) * 6 + c] = Ql[r * 3] * v[0] + Ql[r * 3 + 1] * v[1] + Ql[r * 3 + 2] * v[2];
+      }
+    }
+  if (Qr)
+    for (int r = 0; r < 6; ++r) {
+      const double v[3] = {X[r * 6 + 3], X[r * 6 + 4], X[r * 6 + 5]};
+      for (int c = 0; c < 3; ++c) {
+        X[r * 6 + c] = 0.0;
+        X[r * 6 + 3 + c] = v[0] * Qr[c] + v[1] * Qr[3 + c] + v[2] * Qr[6 + c];
+      }
+    }
+}
+
+// A partially held keyframe's row (held = 2) is P H P + (I - P) with P b as its right-hand side, and every coupling to it is
+// projected on its side too: the held directions get an identity with nothing to solve for, so the update keeps them at 0.
 __global__ void __launch_bounds__(128) PoseGraphAssembleKernel(const PoseGraphArgs a) {
   if (a.state->done) return;
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -217,12 +255,15 @@ __global__ void __launch_bounds__(128) PoseGraphAssembleKernel(const PoseGraphAr
   }
   for (int i = 0; i < 6; ++i) bk[i] = 0.0;
   const int first = a.csr_off[k] + 1, last = a.csr_off[k + 1];
-  if (a.held[k]) {
+  if (a.held[k] == 1) {
     for (int i = 0; i < 6; ++i) D[i * 7] = 1.0;
     for (int e = first; e < last; ++e)
       for (int i = 0; i < 36; ++i) a.csr_val[36 * static_cast<size_t>(e) + i] = 0.0;
     return;
   }
+  double Qk[9];
+  const bool partial = a.held[k] == 2;
+  if (partial) HoldProjection(a, k, Qk);
   int e = first;
   for (int j = a.row_off[k]; j < a.row_off[k + 1]; ++j) {
     const int t = a.row_terms[2 * j], side = a.row_terms[2 * j + 1];
@@ -251,13 +292,33 @@ __global__ void __launch_bounds__(128) PoseGraphAssembleKernel(const PoseGraphAr
       }
     }
     double* X = a.csr_val + 36 * static_cast<size_t>(e++);
-    const bool coupled = !a.held[other];
+    const bool coupled = a.held[other] != 1;
+    if (partial || a.held[other] == 2) {
+      double Qo[9];
+      if (a.held[other] == 2) HoldProjection(a, other, Qo);
+      for (int r = 0; r < 6; ++r)
+        for (int c = 0; c < 6; ++c) X[r * 6 + c] = coupled ? (side ? h12(c, 6 + r) : h12(r, 6 + c)) : 0.0;
+      ProjectBlock(partial ? Qk : nullptr, X, a.held[other] == 2 ? Qo : nullptr);
+      if (other == k + 1)
+        for (int i = 0; i < 36; ++i) U[i] += X[i];
+      continue;
+    }
     for (int r = 0; r < 6; ++r)
       for (int c = 0; c < 6; ++c) {
         const double v = coupled ? (side ? h12(c, 6 + r) : h12(r, 6 + c)) : 0.0;   // H_kb = H_ab (side a), H_ba = H_ab^T
         X[r * 6 + c] = v;
         if (other == k + 1) U[r * 6 + c] += v;
       }
+  }
+  if (partial) {
+    ProjectBlock(Qk, D, Qk);
+    for (int i = 0; i < 3; ++i) {
+      D[i * 7] = 1.0;
+      bk[i] = 0.0;
+      for (int j = 0; j < 3; ++j) D[(3 + i) * 6 + 3 + j] += (i == j ? 1.0 : 0.0) - Qk[i * 3 + j];
+    }
+    const double v[3] = {bk[3], bk[4], bk[5]};
+    for (int i = 0; i < 3; ++i) bk[3 + i] = Qk[i * 3] * v[0] + Qk[i * 3 + 1] * v[1] + Qk[i * 3 + 2] * v[2];
   }
 }
 
@@ -482,12 +543,13 @@ __global__ void __launch_bounds__(kSolveThreads) PoseGraphSolveKernel(const Pose
 __global__ void __launch_bounds__(128) PoseGraphUpdateKernel(const PoseGraphArgs a) {
   if (a.state->done) return;
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= a.K || a.held[k]) return;
+  if (k >= a.K || a.held[k] == 1) return;
   float* pe = a.poses + 7 * k;
   float* pv = a.prev + 7 * k;
   const double* x = a.work + 6 * static_cast<size_t>(k);   // Work::x
   float d[6];
   for (int i = 0; i < 6; ++i) d[i] = static_cast<float>(x[i]);
+  if (a.held[k] == 2) d[0] = d[1] = d[2] = 0.f;   // (the projected system leaves them 0 up to rounding)
   for (int i = 0; i < 7; ++i) pv[i] = pe[i];
   Pose T;
   T.q[0] = pe[0]; T.q[1] = pe[1]; T.q[2] = pe[2]; T.q[3] = pe[3];

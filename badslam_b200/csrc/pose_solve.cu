@@ -69,6 +69,15 @@ __global__ void __launch_bounds__(256) PoseSolveKernel(const PoseSolveArgs a) {
         for (int j = 0; j < 6; ++j) b[j] += w * bp[j];
       }
     }
+    if (a.attitude && a.attitude[kf].has) {
+      // the attitude prior (DESIGN §3.17), after the terms, weighted as they are
+      const bba_attitude_prior& ap = a.attitude[kf].p;
+      double Hp[21], bp[6], cost, rho, w;
+      AttitudePriorTerms(ap.reference_direction, ap.measured_direction, ap.information, pe, Hp, bp, &cost);
+      RobustLoss(ap.loss.type, ap.loss.scale, 2.0 * cost, &rho, &w);
+      for (int j = 0; j < 21; ++j) H[j] += w * Hp[j];
+      for (int j = 0; j < 6; ++j) b[j] += w * bp[j];
+    }
     SolveLDLT<6>(H, b, x);
     float xf[6], neg[6];
     for (int j = 0; j < 6; ++j) {

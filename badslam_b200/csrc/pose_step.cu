@@ -260,8 +260,8 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
   for (int i = 0; i < n; ++i) PoseToArray(init[i], p.h_pose_est + 7 * ids[i]);
   BBA_CUDA(h, cudaMemcpyAsync(p.d_pose_est, p.h_pose_est, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
   if (world > 1 && n_local) BBA_CUDA(h, cudaMemcpyAsync(x.d_local_ids, p.h_work, sizeof(int) * n_local, cudaMemcpyHostToDevice, s));
-  bool terms = false;
-  if (bba_status st = StagePoseTerms(h, ids, init, s, &terms)) return st;
+  bool terms = false, attitude = false;
+  if (bba_status st = StagePoseTerms(h, ids, init, s, &terms, &attitude)) return st;
   BBA_CUDA(h, cudaMemsetAsync(p.d_iterations, 0, sizeof(int) * K, s));
   BBA_CUDA(h, cudaMemsetAsync(p.d_converged, 0, sizeof(int) * K, s));
   if (bba_status st = MarkStaging(h, s)) return st;
@@ -283,6 +283,7 @@ bba_status RunPoseStep(bba_handle h, const std::vector<int>& ids, const std::vec
   sol.queue = p.d_queue;
   sol.term_offsets = terms ? p.d_term_offsets.get() : nullptr;
   sol.terms = terms ? p.d_terms.get() : nullptr;
+  sol.attitude = attitude ? p.d_attitude.get() : nullptr;
   p.h_flag[0] = 0;
   p.h_flag[1] = n_local;
   if (h->profiling) BBA_CUDA(h, cudaMemsetAsync(p.d_totals, 0, sizeof(unsigned long long) * 8, s));

@@ -1,5 +1,5 @@
-// pose_terms.cu -- the soft keyframe pose terms of libbadba_b200 (host side): the pose priors and relative pose constraints with
-// their robust losses and entry points, their staging for the pose step (PoseSolveKernel) and the PCG products
+// pose_terms.cu -- the soft keyframe pose terms of libbadba_b200 (host side): the pose priors, attitude priors and relative pose
+// constraints with their robust losses and entry points, their staging for the pose step (PoseSolveKernel) and the PCG products
 // (LaunchPcgPoseTerms), and the keyframe pose graph (bba_optimize_pose_graph, bba_evaluate_keyframe_pose_terms, DESIGN §3.14).
 #include <cmath>
 #include <cstring>
@@ -31,13 +31,19 @@ bool PoseRecordFinite(const float* pose, const float* info) {
 }
 
 // Reserves the staging buffers of the soft pose terms (pose step and PCG) for a prior on every keyframe and `constraints`
-// constraints, with room to double the constraints before the next allocation.  The calls that add priors or constraints make
-// it before they change anything; the staging repeats it, a no-op unless an earlier reservation failed.
-bba_status ReservePoseTerms(bba_handle h, size_t constraints) {
-  // pose step: a prior per keyframe, and per constraint an equivalent prior and a damping anchor at each end; PCG: a prior per
-  // pose block and one term at each end of a constraint
+// constraints, with room to double the constraints before the next allocation, and with `attitude` for an attitude prior on every
+// keyframe too.  The calls that add priors or constraints make it before they change anything; the staging repeats it, a no-op
+// unless an earlier reservation failed.
+bba_status ReservePoseTerms(bba_handle h, size_t constraints, bool attitude) {
+  // pose step: a prior per keyframe, and per constraint an equivalent prior and a damping anchor at each end, the attitude priors
+  // apart; PCG: a prior and an attitude prior per pose block and one term at each end of a constraint
   const size_t M = static_cast<size_t>(h->cfg.max_keyframes), grow = 2 * constraints;
   auto& p = h->pose;
+  if (attitude) {
+    BBA_CUDA(h, p.h_attitude.Reserve(M));
+    BBA_CUDA(h, p.d_attitude.Reserve(M));
+  }
+  const size_t unary = attitude ? 2 * M : M;
   BBA_CUDA(h, p.h_term_offsets.Reserve(M + 1));
   BBA_CUDA(h, p.d_term_offsets.Reserve(M + 1));
   BBA_CUDA(h, p.h_terms.Reserve(M + 4 * constraints, M + 4 * grow));
@@ -45,9 +51,28 @@ bba_status ReservePoseTerms(bba_handle h, size_t constraints) {
   auto& pc = h->pcg;
   BBA_CUDA(h, pc.h_pose_blocks.Reserve(M));
   BBA_CUDA(h, pc.d_pose_blocks.Reserve(M));
-  BBA_CUDA(h, pc.h_pose_terms.Reserve(M + 2 * constraints, M + 2 * grow));
-  BBA_CUDA(h, pc.d_pose_terms.Reserve(M + 2 * constraints, M + 2 * grow));
+  BBA_CUDA(h, pc.h_pose_terms.Reserve(unary + 2 * constraints, unary + 2 * grow));
+  BBA_CUDA(h, pc.d_pose_terms.Reserve(unary + 2 * constraints, unary + 2 * grow));
   return BBA_OK;
+}
+
+bool HasAttitude(bba_handle h) { return h->attitude_prior_count > 0; }
+
+// Counts the attitude priors and publishes the records.
+bba_status CommitAttitudePriors(bba_handle h) {
+  int count = 0;
+  for (const AttitudePrior& p : h->attitude_priors) count += p.has ? 1 : 0;
+  h->attitude_prior_count = count;
+  return Publish(h, nullptr, false);
+}
+
+// An attitude prior's terms at global_T_frame = pose (AttitudePriorTerms), scaled by the robust weight of its loss there.
+void WeightedAttitudeTerms(const AttitudePrior& a, const float pose[7], double H[21], double b[6]) {
+  double cost, rho, w;
+  AttitudePriorTerms(a.p.reference_direction, a.p.measured_direction, a.p.information, pose, H, b, &cost);
+  RobustLoss(a.p.loss.type, a.p.loss.scale, 2.0 * cost, &rho, &w);
+  for (int i = 0; i < 21; ++i) H[i] *= w;
+  for (int i = 0; i < 6; ++i) b[i] *= w;
 }
 
 // The soft relative pose constraints that touch each of the first K keyframes, in id order: indices into h->pose_constraints,
@@ -79,14 +104,15 @@ void WeightedConstraintTerms(const PoseConstraint& c, const float pa[7], const f
 }
 
 // ---- keyframe pose graph (bba_optimize_pose_graph, DESIGN §3.14) ----
-// What the pose graph stages for K keyframes and C constraints: terms (a prior per keyframe, the constraints, the chain), ints
-// (held flags, row offsets, two ints per row entry, CSR offsets and columns) and doubles (the terms' blocks, the CSR blocks, b, the
-// couplings and the solver's work).  A row holds its prior and one entry per end of a constraint or chain edge.
+// What the pose graph stages for K keyframes and C constraints: terms (a prior and an attitude prior per keyframe, the
+// constraints, the chain), ints (held flags, row offsets, two ints per row entry, CSR offsets and columns) and doubles (the terms'
+// blocks, the CSR blocks, b, the couplings and the solver's work).  A row holds its priors and one entry per end of a constraint or
+// chain edge.
 struct PoseGraphSizes {
   size_t terms, ints, doubles;
 };
 PoseGraphSizes PoseGraphCapacity(size_t K, size_t C) {
-  const size_t terms = 2 * K + C, entries = 3 * K + 2 * C, nnz = 3 * K + 2 * C;
+  const size_t terms = 3 * K + C, entries = 4 * K + 2 * C, nnz = 3 * K + 2 * C;
   const size_t block_doubles = sizeof(PoseGraphTermBlocks) / sizeof(double);
   return {terms, K + 2 * (K + 1) + 2 * entries + nnz, terms * block_doubles + 36 * nnz + 42 * K + PoseGraphWorkDoubles(K)};
 }
@@ -105,6 +131,8 @@ bba_status ReservePoseGraph(bba_handle h, size_t constraints) {
   BBA_CUDA(h, g.d_doubles.Reserve(need.doubles, alloc.doubles));
   BBA_CUDA(h, g.h_poses.Reserve(7 * M));
   BBA_CUDA(h, g.d_poses.Reserve(14 * M));
+  BBA_CUDA(h, g.h_hold_axes.Reserve(3 * M));
+  BBA_CUDA(h, g.d_hold_axes.Reserve(3 * M));
   BBA_CUDA(h, g.d_state.Reserve(1));
   BBA_CUDA(h, g.h_state.Reserve(1));
   return BBA_OK;
@@ -115,14 +143,20 @@ int FindRoot(std::vector<int>& parent, int k) {
   return k;
 }
 
-// The pose graph's terms in h->graph.h_terms at the keyframe poses `poses`: the priors (prior_term[k]: keyframe k's term, or -1),
-// the constraints by id from *first_constraint, then with odometry_information the odometry chain from *first_chain, whose Z are
-// taken at `poses` and whose losses are TRIVIAL.  Returns the number of terms.
-int StagePoseGraphTerms(bba_handle h, const float* poses, const float* odometry_information, std::vector<int>* prior_term,
-                        int* first_constraint, int* first_chain) {
+// Where StagePoseGraphTerms put the terms: keyframe k's prior and attitude prior (or -1), the first constraint and chain edge.
+struct PoseGraphLayout {
+  std::vector<int> prior_term, attitude_term;
+  int first_constraint = 0, first_chain = 0;
+};
+
+// The pose graph's terms in h->graph.h_terms at the keyframe poses `poses`: the priors, the attitude priors, the constraints by
+// id, then with odometry_information the odometry chain, whose Z are taken at `poses` and whose losses are TRIVIAL.  Returns the
+// number of terms.
+int StagePoseGraphTerms(bba_handle h, const float* poses, const float* odometry_information, PoseGraphLayout* layout) {
   auto& g = h->graph;
   const int K = static_cast<int>(h->keyframes.size());
-  prior_term->assign(K, -1);
+  layout->prior_term.assign(K, -1);
+  layout->attitude_term.assign(K, -1);
   int T = 0;
   auto add = [&](int a, int b, const float* z, const float* info, const bba_robust_loss& loss) {
     PoseGraphTerm& t = g.h_terms[T++];
@@ -135,12 +169,22 @@ int StagePoseGraphTerms(bba_handle h, const float* poses, const float* odometry_
   for (int k = 0; k < K; ++k) {
     const PosePrior& p = h->pose_priors[k];
     if (!p.has) continue;
-    (*prior_term)[k] = T;
+    layout->prior_term[k] = T;
     add(k, -1, p.pose, p.info, p.loss);
   }
-  *first_constraint = T;
+  for (int k = 0; k < K && HasAttitude(h); ++k) {
+    const AttitudePrior& p = h->attitude_priors[k];
+    if (!p.has) continue;
+    layout->attitude_term[k] = T;
+    float z[7] = {}, info[21] = {};
+    std::memcpy(z, p.p.reference_direction, sizeof(float) * 3);
+    std::memcpy(z + 3, p.p.measured_direction, sizeof(float) * 3);
+    info[0] = p.p.information;
+    add(k, kPoseGraphAttitude, z, info, p.p.loss);
+  }
+  layout->first_constraint = T;
   for (const PoseConstraint& c : h->pose_constraints) add(c.c.keyframe_a, c.c.keyframe_b, c.c.a_T_b, c.c.information, c.loss);
-  *first_chain = T;
+  layout->first_chain = T;
   if (odometry_information)
     for (int k = 0; k + 1 < K; ++k) {
       double qa[4], ta[3], qb[4], tb[3], q[4], t[3];
@@ -170,7 +214,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   }
   bba_pose_graph_result r{};
   if (result) *result = r;
-  if (K < 2 && h->pose_prior_count == 0) return BBA_OK;
+  if (K < 2 && h->pose_prior_count == 0 && !HasAttitude(h)) return BBA_OK;
   const std::vector<PoseConstraint>& cons = h->pose_constraints;
   if (bba_status st = ReservePoseGraph(h, cons.size())) return st;
   auto& g = h->graph;
@@ -180,13 +224,18 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   // the terms: priors, constraints by id, then the chain at the poses the call starts from
   float* poses = g.h_poses;
   for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses + 7 * k);
-  std::vector<int> prior_term;
-  int first_constraint = 0, first_chain = 0;
-  const int T = StagePoseGraphTerms(h, poses, chain ? o->odometry_information : nullptr, &prior_term, &first_constraint, &first_chain);
+  PoseGraphLayout layout;
+  const int T = StagePoseGraphTerms(h, poses, chain ? o->odometry_information : nullptr, &layout);
+  const std::vector<int>& prior_term = layout.prior_term;
+  const std::vector<int>& attitude_term = layout.attitude_term;
+  const int first_constraint = layout.first_constraint, first_chain = layout.first_chain;
 
-  // the held keyframes: the gauge, the untouched ones, and the lowest id of every component without the gauge or a prior
-  std::vector<int> parent(K), lowest(K, -1);
-  std::vector<char> touched(K, 0), anchored(K, 0);
+  // the held keyframes: the gauge, the untouched ones, and the lowest id of every component without the gauge or a prior.  In
+  // such a component with attitude priors the lowest id is held only in translation and, when the component's reference
+  // directions are parallel, in rotation about them (held = 2, DESIGN §3.17): the priors fix the component's tilt, and holding
+  // that keyframe's tilt too would bias every other keyframe toward it.
+  std::vector<int> parent(K), lowest(K, -1), axis_of(K, -1);
+  std::vector<char> touched(K, 0), anchored(K, 0), parallel(K, 1);
   for (int k = 0; k < K; ++k) parent[k] = k;
   for (int i = first_constraint; i < T; ++i) {
     const PoseGraphTerm& t = g.h_terms[i];
@@ -197,15 +246,37 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   for (int k = 0; k < K; ++k) {
     const int root = FindRoot(parent, k);
     if (lowest[root] < 0) lowest[root] = k;
-    if (prior_term[k] >= 0) touched[k] = 1;
+    if (prior_term[k] >= 0 || attitude_term[k] >= 0) touched[k] = 1;
     if (prior_term[k] >= 0 || k == gauge) anchored[root] = 1;
+    if (attitude_term[k] < 0) continue;
+    const float* d = h->attitude_priors[k].p.reference_direction;   // (unit)
+    if (axis_of[root] < 0) {
+      axis_of[root] = k;
+    } else {
+      const float* d0 = h->attitude_priors[axis_of[root]].p.reference_direction;
+      const double cx = d[1] * d0[2] - d[2] * d0[1], cy = d[2] * d0[0] - d[0] * d0[2], cz = d[0] * d0[1] - d[1] * d0[0];
+      if (cx * cx + cy * cy + cz * cz > 1e-12) parallel[root] = 0;
+    }
   }
   int* held = g.h_ints;
-  int held_count = 0;
+  float* hold_axes = g.h_hold_axes;
+  int held_count = 0, free_directions = 0;
+  bool partial = false;
   for (int k = 0; k < K; ++k) {
     const int root = FindRoot(parent, k);
-    held[k] = (k == gauge || !touched[k] || (!anchored[root] && lowest[root] == k)) ? 1 : 0;
-    held_count += held[k];
+    const bool lowest_unanchored = !anchored[root] && lowest[root] == k;
+    if (k == gauge || !touched[k] || (lowest_unanchored && axis_of[root] < 0)) {
+      held[k] = 1;
+      ++held_count;
+    } else if (lowest_unanchored) {
+      held[k] = 2;
+      partial = true;
+      for (int j = 0; j < 3; ++j) hold_axes[3 * k + j] = parallel[root] ? h->attitude_priors[axis_of[root]].p.reference_direction[j] : 0.f;
+      free_directions += parallel[root] ? 2 : 3;
+    } else {
+      held[k] = 0;
+      free_directions += 6;
+    }
   }
 
   // row k: its prior, its constraints by id, the chain edges (k - 1, k) and (k, k + 1); the CSR row: the diagonal, then the other
@@ -217,7 +288,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   for (int k = 0; k < K; ++k) {
     row_off[k] = entries;
     const int binary = (off[k + 1] - off[k]) + (chain ? (k > 0) + (k + 1 < K) : 0);
-    entries += (prior_term[k] >= 0) + binary;
+    entries += (prior_term[k] >= 0) + (attitude_term[k] >= 0) + binary;
     nnz += 1 + binary;
   }
   row_off[K] = entries;
@@ -235,6 +306,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
     csr_off[k] = c;
     csr_col[c++] = k;
     if (prior_term[k] >= 0) entry(prior_term[k], 0, -1);
+    if (attitude_term[k] >= 0) entry(attitude_term[k], 0, -1);
     for (int j = off[k]; j < off[k + 1]; ++j) {
       const bba_pose_constraint& pc = cons[adj[j]].c;
       const bool is_a = pc.keyframe_a == k;
@@ -251,6 +323,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   BBA_CUDA(h, cudaMemcpyAsync(g.d_ints, g.h_ints, sizeof(int) * ints, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemcpyAsync(g.d_poses, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemcpyAsync(g.d_poses + 7 * M, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
+  if (partial) BBA_CUDA(h, cudaMemcpyAsync(g.d_hold_axes, hold_axes, sizeof(float) * 3 * K, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemsetAsync(g.d_state, 0, sizeof(PoseGraphState), s));
   PoseGraphArgs a{};
   a.K = K;
@@ -261,6 +334,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   a.prev = g.d_poses + 7 * M;
   const int* d_ints = g.d_ints;
   a.held = d_ints;
+  a.hold_axis = partial ? g.d_hold_axes.get() : nullptr;
   a.row_off = d_ints + (row_off - held);
   a.row_terms = d_ints + (row_terms - held);
   a.csr_off = d_ints + (csr_off - held);
@@ -272,7 +346,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   a.work = a.tri + 36 * static_cast<size_t>(K);
   a.state = g.d_state;
   a.max_iterations = max_iterations;
-  a.max_linear = 6 * (K - held_count);
+  a.max_linear = free_directions;   // 6 (K - held_count) without partial holds
   for (int round = 0; round <= max_iterations; ++round) {
     a.round = round;
     BBA_LAUNCH(h, h->launches, LaunchPoseGraphRound, a, s);
@@ -281,7 +355,7 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   BBA_CUDA(h, cudaMemcpyAsync(poses, g.d_poses, sizeof(float) * 7 * K, cudaMemcpyDeviceToHost, s));
   BBA_CUDA(h, cudaStreamSynchronize(s));
   for (int k = 0; k < K; ++k)
-    if (!held[k]) h->keyframes[k].pose = PoseFromArray(poses + 7 * k);
+    if (held[k] != 1) h->keyframes[k].pose = PoseFromArray(poses + 7 * k);
   const PoseGraphState& st = *g.h_state.get();
   r.iterations = st.iterations;
   r.converged = st.converged;
@@ -293,22 +367,15 @@ bba_status OptimizePoseGraph(bba_handle h, const bba_pose_graph_options* o, bba_
   return Publish(h, s, false);
 }
 
-// bba_evaluate_keyframe_pose_terms: the pose graph's terms without the chain, linearised once at the current poses with a.eval
-// set, which writes every term's {s, w}.
-bba_status EvaluatePoseTerms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight, int constraint_capacity,
-                             double* constraint_s, double* constraint_weight, cudaStream_t s) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  if (keyframe_capacity < 0 || constraint_capacity < 0)
-    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_evaluate_keyframe_pose_terms: negative capacity");
+// The pose graph's terms without the chain, linearised once at the current poses with a.eval set, which writes every term's
+// {s, w} to h->graph.h_eval (bba_evaluate_keyframe_pose_terms, bba_evaluate_keyframe_attitude_priors).
+bba_status EvaluateTerms(bba_handle h, PoseGraphLayout* layout, cudaStream_t s) {
   const int K = static_cast<int>(h->keyframes.size());
-  const std::vector<PoseConstraint>& cons = h->pose_constraints;
-  if (bba_status st = ReservePoseGraph(h, cons.size())) return st;
+  if (bba_status st = ReservePoseGraph(h, h->pose_constraints.size())) return st;
   auto& g = h->graph;
   float* poses = g.h_poses;
   for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses + 7 * k);
-  std::vector<int> prior_term;
-  int first_constraint = 0, first_chain = 0;
-  const int T = StagePoseGraphTerms(h, poses, nullptr, &prior_term, &first_constraint, &first_chain);
+  const int T = StagePoseGraphTerms(h, poses, nullptr, layout);
   if (T) {
     BBA_CUDA(h, cudaMemcpyAsync(g.d_terms, g.h_terms, sizeof(PoseGraphTerm) * T, cudaMemcpyHostToDevice, s));
     BBA_CUDA(h, cudaMemcpyAsync(g.d_poses, poses, sizeof(float) * 7 * K, cudaMemcpyHostToDevice, s));
@@ -325,16 +392,43 @@ bba_status EvaluatePoseTerms(bba_handle h, int keyframe_capacity, double* prior_
     BBA_CUDA(h, cudaMemcpyAsync(g.h_eval, g.d_eval, sizeof(double) * 2 * T, cudaMemcpyDeviceToHost, s));
     BBA_CUDA(h, cudaStreamSynchronize(s));
   }
-  const double* ev = g.h_eval;
+  return BBA_OK;
+}
+
+bba_status EvaluatePoseTerms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight, int constraint_capacity,
+                             double* constraint_s, double* constraint_weight, cudaStream_t s) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (keyframe_capacity < 0 || constraint_capacity < 0)
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_evaluate_keyframe_pose_terms: negative capacity");
+  PoseGraphLayout layout;
+  if (bba_status st = EvaluateTerms(h, &layout, s)) return st;
+  const int K = static_cast<int>(h->keyframes.size());
+  const std::vector<PoseConstraint>& cons = h->pose_constraints;
+  const double* ev = h->graph.h_eval;
   for (int k = 0; k < std::min(keyframe_capacity, K); ++k) {
-    const int t = prior_term[k];
+    const int t = layout.prior_term[k];
     if (prior_s) prior_s[k] = t >= 0 ? ev[2 * t] : std::nan("");
     if (prior_weight) prior_weight[k] = t >= 0 ? ev[2 * t + 1] : std::nan("");
   }
   for (int i = 0; i < std::min(constraint_capacity, static_cast<int>(cons.size())); ++i) {
-    const int t = first_constraint + i;
+    const int t = layout.first_constraint + i;
     if (constraint_s) constraint_s[i] = ev[2 * t];
     if (constraint_weight) constraint_weight[i] = ev[2 * t + 1];
+  }
+  return BBA_OK;
+}
+
+bba_status EvaluateAttitudePriors(bba_handle h, int keyframe_capacity, double* s_out, double* weight, cudaStream_t s) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  if (keyframe_capacity < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bba_evaluate_keyframe_attitude_priors: negative capacity");
+  PoseGraphLayout layout;
+  if (bba_status st = EvaluateTerms(h, &layout, s)) return st;
+  const int K = static_cast<int>(h->keyframes.size());
+  const double* ev = h->graph.h_eval;
+  for (int k = 0; k < std::min(keyframe_capacity, K); ++k) {
+    const int t = layout.attitude_term[k];
+    if (s_out) s_out[k] = t >= 0 ? ev[2 * t] : std::nan("");
+    if (weight) weight[k] = t >= 0 ? ev[2 * t + 1] : std::nan("");
   }
   return BBA_OK;
 }
@@ -346,14 +440,21 @@ bba_status EvaluatePoseTerms(bba_handle h, int keyframe_capacity, double* prior_
 // constraint whose other end is in the step too a damping anchor, a prior at k's own start pose with the constraint's diagonal
 // block for k at the start poses, scaled by the constraint's robust weight there, as its information (DESIGN.md 3.12, 3.15).  A
 // term's loss is the prior's own, an equivalent prior's its constraint's, an anchor's TRIVIAL.  Every rank stages the same lists:
-// they depend only on the start of the step.
-bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, cudaStream_t s, bool* staged) {
+// they depend only on the start of the step.  The attitude priors go apart, as the per-keyframe array h->pose.d_attitude.
+bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::vector<Pose>& init, cudaStream_t s, bool* staged,
+                          bool* attitude) {
   auto& p = h->pose;
-  *staged = false;
+  *staged = *attitude = false;
+  const int K = static_cast<int>(h->keyframes.size());
+  if (HasAttitude(h)) {
+    if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size(), true)) return st;
+    std::copy(h->attitude_priors.begin(), h->attitude_priors.begin() + K, p.h_attitude.get());
+    BBA_CUDA(h, cudaMemcpyAsync(p.d_attitude, p.h_attitude, sizeof(AttitudePrior) * K, cudaMemcpyHostToDevice, s));
+    *attitude = true;
+  }
   if (h->pose_prior_count == 0 && h->pose_constraints.empty()) return BBA_OK;
   const std::vector<PoseConstraint>& cons = h->pose_constraints;
-  if (bba_status st = ReservePoseTerms(h, cons.size())) return st;
-  const int K = static_cast<int>(h->keyframes.size());
+  if (bba_status st = ReservePoseTerms(h, cons.size(), HasAttitude(h))) return st;
   std::vector<int> pos(K, -1);   // index in ids
   for (size_t i = 0; i < ids.size(); ++i) pos[ids[i]] = static_cast<int>(i);
   auto start = [&](int k, float out[7]) { PoseToArray(pos[k] >= 0 ? init[pos[k]] : h->keyframes[k].pose, out); };
@@ -427,14 +528,15 @@ bba_status StagePoseTerms(bba_handle h, const std::vector<int>& ids, const std::
 // A keyframe's prior and, per constraint, H_aa / H_bb, H_ab and b_a / b_b of PoseConstraintTerms, gathered per pose block (every
 // keyframe but the gauge) in the order prior, then constraints by id.  An edge to the gauge keeps only its other end's diagonal
 // terms (p_gauge = 0).  Every term's H and b are scaled by its robust weight at these poses (one IRLS step per outer iteration).
-// fp64, rounded to fp32.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.
+// fp64, rounded to fp32.  Only rank 0 adds them: the sum all-reduce of r / M / g then counts each once.  A keyframe's attitude
+// prior follows its prior.
 bba_status StagePcgPoseTerms(bba_handle h, bool opt_poses, int gauge, cudaStream_t s) {
   auto& pc = h->pcg;
   pc.pose_blocks = 0;
-  if (!opt_poses || (h->pose_prior_count == 0 && h->pose_constraints.empty()) || h->cfg.rank != 0) return BBA_OK;
+  if (!opt_poses || (h->pose_prior_count == 0 && h->pose_constraints.empty() && !HasAttitude(h)) || h->cfg.rank != 0) return BBA_OK;
   const int K = static_cast<int>(h->keyframes.size());
   const size_t C = h->pose_constraints.size();
-  if (bba_status st = ReservePoseTerms(h, C)) return st;
+  if (bba_status st = ReservePoseTerms(h, C, HasAttitude(h))) return st;
   auto unknown = [&](int k) { return k == gauge ? -1 : 6 * (k < gauge ? k : k - 1); };
   std::vector<float> poses(7 * static_cast<size_t>(K));
   for (int k = 0; k < K; ++k) PoseToArray(h->keyframes[k].pose, poses.data() + 7 * k);
@@ -479,6 +581,14 @@ bba_status StagePcgPoseTerms(bba_handle h, bool opt_poses, int gauge, cudaStream
       for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(w * H[j]);
       for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(w * b[j]);
     }
+    if (h->attitude_priors[k].has) {
+      PcgPoseTerm& t = pc.h_pose_terms[nt++];
+      t.other = -1;
+      double H[21], b[6];
+      WeightedAttitudeTerms(h->attitude_priors[k], poses.data() + 7 * k, H, b);
+      for (int j = 0; j < 21; ++j) t.H[j] = static_cast<float>(H[j]);
+      for (int j = 0; j < 6; ++j) t.b[j] = static_cast<float>(b[j]);
+    }
     for (int e = off[k]; e < off[k + 1]; ++e) {
       const int i = adj[e];
       pc.h_pose_terms[nt++] = edge[2 * i + (h->pose_constraints[i].c.keyframe_a == k ? 0 : 1)];
@@ -515,7 +625,7 @@ bba_status bba_set_keyframe_pose_priors(bba_handle h, int count, const int* ids,
     if (!InformationPsd(info)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information matrix is not positive semi-definite");
   }
   if (count > 0)
-    if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size())) return st;
+    if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size(), HasAttitude(h))) return st;
   for (int i = 0; i < count; ++i) {
     PosePrior& r = h->pose_priors[ids[i]];
     std::memcpy(r.pose, poses + 7 * static_cast<size_t>(i), sizeof(r.pose));
@@ -601,7 +711,7 @@ bba_status bba_add_keyframe_pose_constraints(bba_handle h, int count, const bba_
     if (!InformationPsd(c.information)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information matrix is not positive semi-definite");
   }
   if (count == 0) return BBA_OK;
-  if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size() + count)) return st;
+  if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size() + count, HasAttitude(h))) return st;
   for (int i = 0; i < count; ++i) {
     PoseConstraint r{};
     r.id = h->next_pose_constraint_id++;
@@ -684,6 +794,73 @@ bba_status bba_get_keyframe_pose_constraint_losses(bba_handle h, int capacity, i
     if (out) out[i] = cons[i].loss;
   }
   return BBA_OK;
+}
+
+// ---- attitude priors ----
+bba_status bba_set_keyframe_attitude_priors(bba_handle h, int count, const int* ids, const bba_attitude_prior* priors) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_set_keyframe_attitude_priors: ";
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < 0");
+  if (count > 0 && (!ids || !priors)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  const int K = static_cast<int>(h->keyframes.size());
+  for (int i = 0; i < count; ++i) {
+    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
+    const bba_attitude_prior& p = priors[i];
+    bool finite = std::isfinite(p.information);
+    for (int j = 0; j < 3; ++j) finite = finite && std::isfinite(p.reference_direction[j]) && std::isfinite(p.measured_direction[j]);
+    if (!finite) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite direction or information");
+    for (const float* d : {p.reference_direction, p.measured_direction})
+      if (std::sqrt(static_cast<double>(d[0]) * d[0] + static_cast<double>(d[1]) * d[1] + static_cast<double>(d[2]) * d[2]) < 1e-6)
+        return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "direction of norm < 1e-6");
+    if (!(p.information > 0.f)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "information is not > 0");
+    if (!RobustLossValid(p.loss)) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown loss type or bad scale");
+  }
+  if (count > 0)
+    if (bba_status st = ReservePoseTerms(h, h->pose_constraints.size(), true)) return st;
+  for (int i = 0; i < count; ++i) {
+    AttitudePrior& r = h->attitude_priors[ids[i]];
+    r.p = priors[i];
+    for (float* d : {r.p.reference_direction, r.p.measured_direction}) {
+      const double n = std::sqrt(static_cast<double>(d[0]) * d[0] + static_cast<double>(d[1]) * d[1] + static_cast<double>(d[2]) * d[2]);
+      for (int j = 0; j < 3; ++j) d[j] = static_cast<float>(d[j] / n);
+    }
+    r.has = 1;
+  }
+  return CommitAttitudePriors(h);
+}
+
+bba_status bba_clear_keyframe_attitude_priors(bba_handle h, int count, const int* ids) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_clear_keyframe_attitude_priors: ";
+  const int K = static_cast<int>(h->keyframes.size());
+  if (count == -1) {
+    std::fill(h->attitude_priors.begin(), h->attitude_priors.end(), AttitudePrior{});
+    return CommitAttitudePriors(h);
+  }
+  if (count < 0) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count < -1");
+  if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
+  for (int i = 0; i < count; ++i)
+    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad keyframe id");
+  for (int i = 0; i < count; ++i) h->attitude_priors[ids[i]] = AttitudePrior{};
+  return CommitAttitudePriors(h);
+}
+
+bba_status bba_get_keyframe_attitude_prior(bba_handle h, int id, bba_attitude_prior* out, int* has) {
+  FrontEndScope front_end;
+  if (!h || !has) return BBA_ERR_INVALID_ARGUMENT;
+  std::unique_lock<std::mutex> lock(h->fe.mu);
+  if (id < 0 || id >= static_cast<int>(h->fe.kfs.size())) {
+    lock.unlock();
+    return Fail(h, BBA_ERR_INVALID_ARGUMENT, "bad keyframe id");
+  }
+  const AttitudePrior& p = h->fe.kfs[id].attitude;
+  *has = p.has;
+  if (out) *out = p.p;
+  return BBA_OK;
+}
+
+bba_status bba_evaluate_keyframe_attitude_priors(bba_handle h, int keyframe_capacity, double* s, double* weight, void* stream) {
+  return EvaluateAttitudePriors(h, keyframe_capacity, s, weight, static_cast<cudaStream_t>(stream));
 }
 
 // ---- keyframe pose graph ----

@@ -635,6 +635,54 @@ class DirectBA:
                                                                cw.ctypes.data, self._stream_ptr(stream)))
         return {"prior_s": ps[:K], "prior_weight": pw[:K], "constraint_ids": ids, "constraint_s": cs[:n], "constraint_weight": cw[:n]}
 
+    # -- attitude priors (not in the reference; include/badba.h "Attitude priors") ----------------------------------------------
+    def SetKeyframeAttitudePriors(self, ids, reference_directions, measured_directions, information, loss="trivial", scale=1.0):
+        """Gives keyframes `ids` an attitude prior: the angle theta between R^-1 d_ref (R: the rotation of global_T_frame) and
+        d_meas costs 1/2 rho(L theta^2).  reference_directions: d_ref in the map frame ([n, 3] or one [3] for all, e.g. gravity);
+        measured_directions: d_meas in each keyframe's camera frame ([n, 3]); information: L in rad^-2 (one for all, or [n]);
+        loss / scale as SetKeyframePosePriorLosses.  The directions are normalised.  Refused as a whole (nothing changes) for an
+        unknown id, a non-finite value, a direction of norm < 1e-6, L not finite and > 0, or a bad loss."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), np.int32)
+        n = len(ids)
+        d_ref = np.broadcast_to(np.asarray(reference_directions, np.float32).reshape(-1, 3), (n, 3))
+        d_meas = np.broadcast_to(np.asarray(measured_directions, np.float32).reshape(-1, 3), (n, 3))
+        L = np.broadcast_to(np.asarray(information, np.float32).reshape(-1), (n,))
+        losses = self._losses(n, loss, scale)
+        recs = (_lib.AttitudePrior * max(n, 1))()
+        for i in range(n):
+            recs[i].reference_direction[:] = [float(v) for v in d_ref[i]]
+            recs[i].measured_direction[:] = [float(v) for v in d_meas[i]]
+            recs[i].information = float(L[i])
+            recs[i].loss = losses[i]
+        self._check(self._lib.bba_set_keyframe_attitude_priors(self._h, n, ids.ctypes.data, recs))
+
+    def ClearKeyframeAttitudePriors(self, ids=None):
+        """Removes the attitude priors of keyframes `ids`, or every one with ids=None."""
+        if ids is None:
+            self._check(self._lib.bba_clear_keyframe_attitude_priors(self._h, -1, None))
+            return
+        ids = np.ascontiguousarray(np.atleast_1d(ids), np.int32)
+        self._check(self._lib.bba_clear_keyframe_attitude_priors(self._h, len(ids), ids.ctypes.data))
+
+    def GetKeyframeAttitudePrior(self, keyframe_id: int):
+        """A keyframe's attitude prior as last published, as a dict (reference_direction [3], measured_direction [3],
+        information, loss_type, loss_scale), or None without one."""
+        r, has = _lib.AttitudePrior(), C.c_int()
+        self._check(self._lib.bba_get_keyframe_attitude_prior(self._h, keyframe_id, C.byref(r), C.byref(has)))
+        if not has.value:
+            return None
+        return {"reference_direction": np.array(r.reference_direction[:], np.float32),
+                "measured_direction": np.array(r.measured_direction[:], np.float32), "information": r.information,
+                "loss_type": r.loss.type, "loss_scale": r.loss.scale}
+
+    def EvaluateKeyframeAttitudePriors(self, stream=None):
+        """(s = L theta^2 [keyframes], w [keyframes]) of every attitude prior at the current poses, evaluated on the device (NaN
+        where a keyframe has none).  Synchronises the stream."""
+        K = self._lib.bba_keyframe_count(self._h)
+        s, w = np.zeros(max(K, 1)), np.zeros(max(K, 1))
+        self._check(self._lib.bba_evaluate_keyframe_attitude_priors(self._h, K, s.ctypes.data, w.ctypes.data, self._stream_ptr(stream)))
+        return s[:K], w[:K]
+
     def OptimizePoseGraph(self, add_current_state_odometry_constraints=True, gauge_keyframe=0, max_iterations=20,
                           odometry_information=None, stream=None) -> dict:
         """bba_optimize_pose_graph (the reference's PoseGraphOptimizer, here on the device): Gauss-Newton over the keyframe poses

@@ -300,6 +300,39 @@ bba_status bba_get_keyframe_pose_constraint_losses(bba_handle h, int capacity, i
  * BA-side call; changes nothing on the handle; synchronises the stream. */
 bba_status bba_evaluate_keyframe_pose_terms(bba_handle h, int keyframe_capacity, double* prior_s, double* prior_weight,
                                             int constraint_capacity, double* constraint_s, double* constraint_weight, void* stream);
+/* Attitude priors (not in the reference; GTSAM's Pose3AttitudeFactor): a measured direction, typically gravity from an
+ * accelerometer at rest, fixes a keyframe's roll and pitch but not its yaw or translation, which direct BA cannot observe and so
+ * lets drift.  A record (d_ref, d_meas, L, loss) on a keyframe adds 1/2 rho(s) to the cost, s = L theta^2, where theta in [0, pi]
+ * is the angle between the predicted direction R^-1 d_ref (R: the rotation of global_T_frame) and d_meas.  d_ref is in the map
+ * frame (e.g. gravity in map coordinates), d_meas in the keyframe's camera frame (e.g. the negated accelerometer reading at rest,
+ * rotated into the camera frame by the caller), L in rad^-2, loss as in "Robust losses".  The term is invariant to yaw about d_ref
+ * and to translation.  It enters where a prior does (the pose step of the alternating scheme and bba_estimate_frame_pose, the
+ * pose unknowns of the PCG scheme but the gauge keyframe, bba_optimize_pose_graph), with IRLS weights as a prior's; the frames of
+ * bba_estimate_frame_poses_for_frames get no terms.  In bba_optimize_pose_graph an attitude prior does not anchor a component: in
+ * a component with neither the gauge nor a pose prior the lowest id is held in translation and, when the component's reference
+ * directions are parallel, in rotation about them (not counted in held_keyframes); it is optimised in the other directions.  A
+ * handle without attitude priors runs exactly the code it ran before they existed.  At most one record per keyframe.
+ *  bba_set_keyframe_attitude_priors: ids [count], priors [count]; replaces the record of each listed keyframe, with both
+ *    directions normalised.  BBA_ERR_INVALID_ARGUMENT for an unknown id, a non-finite value, a direction of norm < 1e-6, an
+ *    information that is not finite and > 0, or a loss bba_set_keyframe_pose_prior_losses refuses; the arguments are checked
+ *    before anything changes, and a refused call changes nothing.
+ *  bba_clear_keyframe_attitude_priors: removes the records of ids [count]; count = -1 removes every record (ids is not read).
+ *  bba_get_keyframe_attitude_prior: front-end call (the published records); *has = 0 and zeros without one (out may be NULL).
+ *  The setters are BA-side calls and publish.  With several ranks every rank makes the same calls.
+ *  bba_evaluate_keyframe_attitude_priors: s and w of every attitude prior at the current keyframe poses, by keyframe id over
+ *    min(keyframe_capacity, keyframe count) entries (NaN where a keyframe has none), from the launch of
+ *    bba_evaluate_keyframe_pose_terms.  Either array may be NULL.  BBA_ERR_INVALID_ARGUMENT: a negative capacity.  A BA-side
+ *    call; changes nothing on the handle; synchronises the stream. */
+typedef struct {
+  float reference_direction[3];   /* d_ref, map frame */
+  float measured_direction[3];    /* d_meas, the keyframe's camera frame */
+  float information;              /* L, rad^-2 */
+  bba_robust_loss loss;
+} bba_attitude_prior;
+bba_status bba_set_keyframe_attitude_priors(bba_handle h, int count, const int* keyframe_ids, const bba_attitude_prior* priors);
+bba_status bba_clear_keyframe_attitude_priors(bba_handle h, int count, const int* keyframe_ids);
+bba_status bba_get_keyframe_attitude_prior(bba_handle h, int keyframe_id, bba_attitude_prior* out, int* has);
+bba_status bba_evaluate_keyframe_attitude_priors(bba_handle h, int keyframe_capacity, double* s, double* weight, void* stream);
 
 /* depth_params_ / cameras (direct_ba.h:243-297; SetColorCamera etc.).  The getters bba_get_intrinsics, bba_get_residual_types,
  * bba_get_cfactor_host and bba_cfactor_size are front-end calls (the published cameras, a, residual types and cfactor; the
@@ -877,6 +910,12 @@ void bba_host_pose_constraint_terms(const float a_T_b[7], const float global_T_a
 /* The robust loss of a pose term (bba_robust_loss) at s = r^T L r: *rho = rho(s) and *weight = rho'(s), in fp64, as the solvers
  * evaluate them.  An unknown type counts as TRIVIAL.  Writes nothing if a pointer is NULL. */
 void bba_host_robust_loss(int type, float scale, double s, double* rho, double* weight);
+/* The terms an attitude prior (d_ref, d_meas, L) adds to a keyframe's pose solve at global_T_frame = pose, for the update
+ * pose * exp(delta), in fp64 (the directions are normalised first): with p = R^-1 d_ref, m = d_meas and theta their angle,
+ * b = L theta (p x m) / |p x m| in the rotation rows (0 where p x m = 0), H = L (I - p p^T) in the rotation block (upper triangle,
+ * 21), zero translation rows, and cost = L theta^2 / 2 (DESIGN §3.17).  Writes nothing if a pointer is NULL. */
+void bba_host_attitude_prior_terms(const float reference_direction[3], const float measured_direction[3], float information,
+                                   const float global_T_frame[7], double H[21], double b[6], double* cost);
 /* The host steps of bba_verify_loop_closures.  bba_host_average_pose: AveragePose (util.cc:110-128) of count >= 1 poses [count][7]
  * (writes nothing for count < 1 or a NULL pointer).  bba_host_loop_agreement: the agreement test of the three refined cur_T_old
  * estimates [3][7] (thresholds <= 0 select 10 deg and 0.02 m); returns BBA_LOOP_ACCEPTED, BBA_LOOP_ROTATION_DISAGREES or

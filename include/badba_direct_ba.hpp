@@ -416,6 +416,31 @@ class DirectBA {
                                            constraint_weight->data(), stream),
           "bba_evaluate_keyframe_pose_terms");
   }
+  // Attitude priors (not in the reference; badba.h): the angle theta between R^-1 d_ref and d_meas costs 1/2 rho(L theta^2), with
+  // d_ref in the map frame (e.g. gravity), d_meas in the keyframe's camera frame (e.g. the negated accelerometer reading at rest).
+  void SetKeyframeAttitudePriors(const std::vector<int>& ids, const std::vector<bba_attitude_prior>& priors) {
+    if (ids.size() != priors.size()) throw Error(BBA_ERR_INVALID_ARGUMENT, "SetKeyframeAttitudePriors: one prior per id");
+    Check(bba_set_keyframe_attitude_priors(h_, static_cast<int>(ids.size()), ids.data(), priors.data()), "bba_set_keyframe_attitude_priors");
+  }
+  // Removes the attitude priors of `ids`, or every one when the list is empty.
+  void ClearKeyframeAttitudePriors(const std::vector<int>& ids = {}) {
+    Check(bba_clear_keyframe_attitude_priors(h_, ids.empty() ? -1 : static_cast<int>(ids.size()), ids.data()),
+          "bba_clear_keyframe_attitude_priors");
+  }
+  // A keyframe's attitude prior as last published; false without one.
+  bool GetKeyframeAttitudePrior(int keyframe_id, bba_attitude_prior* out) {
+    int has = 0;
+    Check(bba_get_keyframe_attitude_prior(h_, keyframe_id, out, &has), "bba_get_keyframe_attitude_prior");
+    return has != 0;
+  }
+  // s = L theta^2 and the robust weight of every attitude prior (indexed by keyframe id, NaN without one) at the current poses.
+  // Synchronises the stream.
+  void EvaluateKeyframeAttitudePriors(cudaStream_t stream, std::vector<double>* s, std::vector<double>* weight) {
+    const int K = bba_keyframe_count(h_);
+    s->resize(K);
+    weight->resize(K);
+    Check(bba_evaluate_keyframe_attitude_priors(h_, K, s->data(), weight->data(), stream), "bba_evaluate_keyframe_attitude_priors");
+  }
   // The keyframe pose graph (bba_optimize_pose_graph; the reference's PoseGraphOptimizer, here on the device): Gauss-Newton over
   // the priors, the constraints and, with add_current_state_odometry_constraints, one edge per consecutive pair of keyframes at
   // their current relative pose with `information` (identity when null).  The defaults are the reference's: vertex 0 fixed, 20

@@ -31,6 +31,13 @@ the information diag(1/T^2 x3, 1/R^2 x3), T in metres and R in radians, which ho
 line always gives the keyframes' absolute error against the trajectory ("max_abs_keyframe_error_m_rad"); with the flag it also
 repeats the run without priors on the same noisy poses and gives that error as "max_abs_keyframe_error_without_priors_m_rad".
 
+With --attitude-prior-sigma R every keyframe gets an attitude prior (DirectBA.SetKeyframeAttitudePriors): the map-frame direction
+d_ref = (0, 0, -1) as measured in the keyframe's camera frame at its trajectory pose, turned by seeded noise of R radians about a
+random axis, with the information 1/R^2.  That is what an accelerometer at rest reports as gravity, and it holds the map's roll and
+pitch.  The JSON line always gives the keyframes' mean tilt error against the trajectory ("mean_tilt_error_rad"); with the flag it
+also repeats the run without attitude priors and gives that error as "mean_tilt_error_without_attitude_priors_rad".  Both flags
+together repeat the run without either.
+
 The views of --make-synthetic lie metres apart (a BA test scene, not a video), so odometry between them fails and only the
 keyframe poses of that sequence are meaningful; on a recorded sequence every frame is tracked from its neighbour.
 """
@@ -80,6 +87,8 @@ def main():
     ap.add_argument("--refine-headroom", type=int, default=64, help="free keyframe slots the handle keeps for --refine-frames")
     ap.add_argument("--pose-prior-sigma", metavar="T,R", default=None,
                     help="anchor every keyframe to its trajectory pose with a soft prior of these sigmas (metres, radians)")
+    ap.add_argument("--attitude-prior-sigma", metavar="RAD", type=float, default=None,
+                    help="give every keyframe an attitude prior from its trajectory pose with this sigma (radians)")
     a = ap.parse_args()
     if a.refine_frames and a.export_poses is None:
         ap.error("--refine-frames needs --export-poses")
@@ -92,20 +101,34 @@ def main():
             assert len(a.pose_prior_sigma) == 2 and min(a.pose_prior_sigma) > 0
         except (ValueError, AssertionError):
             ap.error("--pose-prior-sigma takes two positive numbers T,R")
-        line = run(a, a.pose_prior_sigma)
-        without = run(a, None) if line is not None else None
+    if a.attitude_prior_sigma is not None and not a.attitude_prior_sigma > 0:
+        ap.error("--attitude-prior-sigma takes a positive number RAD")
+    if a.pose_prior_sigma is not None or a.attitude_prior_sigma is not None:
+        line = run(a, a.pose_prior_sigma, a.attitude_prior_sigma)
+        without = run(a, None, None) if line is not None else None
         if without is None:
             return 1
-        line["max_abs_keyframe_error_without_priors_m_rad"] = without["max_abs_keyframe_error_m_rad"]
+        if a.pose_prior_sigma is not None:
+            line["max_abs_keyframe_error_without_priors_m_rad"] = without["max_abs_keyframe_error_m_rad"]
+        if a.attitude_prior_sigma is not None:
+            line["mean_tilt_error_without_attitude_priors_rad"] = without["mean_tilt_error_rad"]
     else:
-        line = run(a, None)
+        line = run(a, None, None)
     if line is None:
         return 1
     print(json.dumps(line))
     return 0
 
 
-def run(a, prior_sigma):
+DOWN = np.array([0.0, 0.0, -1.0])   # d_ref of --attitude-prior-sigma, map frame
+
+
+def tilt(pose, S):
+    """DOWN in the camera frame of global_T_frame `pose`."""
+    return S.quat_to_R(np.asarray(pose[:4], np.float64)).T @ DOWN
+
+
+def run(a, prior_sigma, attitude_sigma):
     """One pass over the sequence; returns the JSON line's fields (None if the poses could not be written)."""
     import torch
     from badslam_b200 import rgbd_dataset as D
@@ -124,6 +147,7 @@ def run(a, prior_sigma):
     surfels = torch.zeros((17, a.max_surfels), dtype=torch.float32, device="cuda")
     ba.SetSurfels(surfels, 0)
     rng = np.random.default_rng(0)
+    rng_attitude = np.random.default_rng(1)   # (a stream of its own: the pose noise stays that of a run without the flag)
     true_poses, t_pre, t_ba, created, results = [], 0.0, 0.0, 0, []
     export = a.export_poses is not None
     keyframe_frames = set(idx)
@@ -161,6 +185,11 @@ def run(a, prior_sigma):
         kf = ba.CreateKeyframeFromFrame(i, raw, rgb, noisy, max_depth=a.max_depth, **raw_options)
         if prior_sigma is not None:
             ba.SetKeyframePosePriors([kf.id], [pose], np.diag([prior_sigma[0] ** -2] * 3 + [prior_sigma[1] ** -2] * 3))
+        if attitude_sigma is not None:
+            axis = rng_attitude.normal(size=3)
+            noise = S.se3_exp(np.r_[0.0, 0.0, 0.0, rng_attitude.normal(0, attitude_sigma) * axis / np.linalg.norm(axis)])
+            measured = tilt(S.se3_mul(pose, noise), S)
+            ba.SetKeyframeAttitudePriors([kf.id], DOWN, measured[None], attitude_sigma ** -2)
         created += ba.CreateSurfelsForKeyframe(None, True, kf.id)
         torch.cuda.synchronize()
         t_pre += time.perf_counter() - t
@@ -188,8 +217,12 @@ def run(a, prior_sigma):
             "max_relative_pose_error_m_rad": [max(e[0] for e in err), max(e[1] for e in err)] if err else None}
     abs_err = [S.pose_error(poses[k], true_poses[k]) for k in range(len(idx))]
     line["max_abs_keyframe_error_m_rad"] = [max(e[0] for e in abs_err), max(e[1] for e in abs_err)]
+    tilts = [np.arccos(np.clip(tilt(poses[k], S) @ tilt(true_poses[k], S), -1.0, 1.0)) for k in range(len(idx))]
+    line["mean_tilt_error_rad"] = float(np.mean(tilts))
     if prior_sigma is not None:
         line["pose_prior_sigma_m_rad"] = prior_sigma
+    if attitude_sigma is not None:
+        line["attitude_prior_sigma_rad"] = attitude_sigma
     if export:
         frame_poses[idx] = poses
         all_true = [f.depth_global_T_frame for f in ds.frames]
