@@ -156,6 +156,17 @@ class LoopVerification(C.Structure):   # bba_loop_verification
                 ("average_pixel_distance", C.c_float), ("pixel_count", C.c_uint32), ("tracking", OdometryResult * 3)]
 
 
+class PlaceIndexOptions(C.Structure):   # bba_place_index_options
+    _fields_ = [("num_ferns", C.c_int), ("min_depth", C.c_float), ("max_depth", C.c_float)]
+
+
+class PlaceQuery(C.Structure):   # bba_place_query
+    _fields_ = [("keyframe_id", C.c_int), ("frame", C.c_int), ("first_keyframe", C.c_int), ("last_keyframe", C.c_int)]
+
+
+PLACE_MAX_MATCHES = 64   # the largest max_matches of bba_query_place_index
+
+
 class Profile(C.Structure):
     _fields_ = [("pose_launches", C.c_uint64), ("pose_ms", C.c_double), ("kf_evals", C.c_uint64),
                 ("n_pair", C.c_uint64), ("n_inimg", C.c_uint64), ("n_depthok", C.c_uint64),
@@ -250,6 +261,11 @@ SYMBOLS = {
                                                     C.POINTER(OdometryResult), _P]),
     "bba_verify_loop_closures": (C.c_int, [_P, C.POINTER(LoopVerificationOptions), C.c_int, C.POINTER(LoopCandidate),
                                            C.POINTER(LoopVerification), _P]),
+    "bba_index_keyframes": (C.c_int, [_P, C.POINTER(PlaceIndexOptions), C.c_int, _P, _P]),
+    "bba_query_place_index": (C.c_int, [_P, C.c_int, C.POINTER(FrameBuffers), C.c_int, C.POINTER(PlaceQuery), C.c_int, _P, _P, _P, _P]),
+    "bba_get_place_index_codes": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "bba_get_place_index_options": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "bba_host_place_ferns": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, _P]),
     "bba_odometry_get_level": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.POINTER(C.c_int), C.POINTER(C.c_int), _P]),
     "bba_odometry_debug_coeffs": (C.c_int, [_P, C.c_int, C.c_int, _F7, _F7, _P, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_float),
                                             _P, _P, _P]),

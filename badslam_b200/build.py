@@ -37,6 +37,7 @@ UNITS = [
     ("local_group.cu", ["-Xptxas", "-v"]),   # (the all-reduce sums keep denormals: no -use_fast_math)
     ("frames.cu", []),
     ("loop_verification.cu", ["-Xptxas", "-v"]),
+    ("place_index.cu", ["-Xptxas", "-v"]),
 ]
 HEADERS = ["device_math.cuh", "exact_sum.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", "rendezvous.hpp", os.path.join("..", "..", "include", "badba.h")]
 

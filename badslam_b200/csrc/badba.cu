@@ -92,8 +92,15 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
     }
     BBA_CUDA(h, cudaStreamWaitEvent(s, f.readers_done[next], 0));
     BBA_CUDA(h, cudaMemcpyAsync(f.cfactor[next], h->d_cfactor, sizeof(float) * h->cf_w * h->cf_h, cudaMemcpyDeviceToDevice, s));
+    if (h->place.state.num_ferns > 0 && !h->keyframes.empty()) {   // the place index's rows of every keyframe
+      const size_t row = sizeof(uint32_t) * kPlaceRowWords;
+      BBA_CUDA(h, cudaMemcpy2DAsync(f.place_codes[next], row, h->place.codes, row, sizeof(uint32_t) * (h->place.state.num_ferns / 8),
+                                    h->keyframes.size(), cudaMemcpyDeviceToDevice, s));
+    }
     BBA_CUDA(h, cudaEventRecord(f.published[next], s));
   }
+  PlaceIndexState place;
+  if (cfactor) place = h->place.state;
   std::vector<KeyframeView> kfs(h->keyframes.size());
   for (size_t k = 0; k < kfs.size(); ++k) {
     const Keyframe& kf = h->keyframes[k];
@@ -113,19 +120,35 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
   f.cams = cams;
   f.kfs.swap(kfs);
   f.constraints.swap(constraints);
-  if (cfactor) f.current = next;
+  if (cfactor) {
+    f.current = next;
+    f.place.num_ferns = place.num_ferns;
+    f.place.min_raw = place.min_raw;
+    f.place.max_raw = place.max_raw;
+    f.place.indexed.swap(place.indexed);
+  }
   return BBA_OK;
 }
 
-bba_status FrontEndCall::Snapshot(cudaStream_t s, int kf_id, const char* fn, int max_kf_id, std::vector<KeyframeView>* all_kfs) {
+bba_status FrontEndCall::Snapshot(cudaStream_t s, int kf_id, const char* fn, int max_kf_id, std::vector<KeyframeView>* all_kfs,
+                                  PlaceIndexState* place, const std::vector<int>* place_ids) {
   auto& f = h_->fe;
   {
     std::lock_guard<std::mutex> lock(f.mu);
     if (std::max(kf_id, max_kf_id) >= static_cast<int>(f.kfs.size())) return Fail(h_, BBA_ERR_INVALID_ARGUMENT, std::string(fn) + ": no such keyframe");
     if (kf_id >= 0) base = f.kfs[kf_id];
     if (all_kfs) *all_kfs = f.kfs;
+    if (place) {
+      if (f.place.num_ferns == 0) return Fail(h_, BBA_ERR_STATE, std::string(fn) + ": no place index yet (bba_index_keyframes)");
+      if (place_ids)
+        for (int id : *place_ids)
+          if (!f.place.indexed[id]) return Fail(h_, BBA_ERR_INVALID_ARGUMENT, std::string(fn) + ": keyframe " + std::to_string(id) + " is not indexed");
+      *place = f.place;
+    }
     cams = f.cams;
+    keyframe_count = static_cast<int>(f.kfs.size());
     slot_ = f.current;
+    place_codes = f.place.num_ferns > 0 ? f.place_codes[slot_].get() : nullptr;
     ++f.readers[slot_];
   }
   s_ = s;

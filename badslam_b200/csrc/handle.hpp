@@ -4,7 +4,8 @@
 // Host units: badba.cu (handle, setters / getters, keyframes, textures, bba_host_*), pose_step.cu (spatial order, pose step),
 // pose_terms.cu (soft pose priors and constraints, their losses and staging, pose graph), bundle_adjust.cu (BA schemes,
 // intrinsics, PCG, surfel lifecycle), multi_gpu.cu (sharding, exchange, peer replicas), frames.cu (odometry, preprocessing).  None
-// of them contains a kernel.  loop_verification.cu (bba_verify_loop_closures) holds its host orchestration and its one kernel.
+// of them contains a kernel.  loop_verification.cu (bba_verify_loop_closures) holds its host orchestration and its one kernel, and
+// place_index.cu (the fern place index) its entry points and its two kernels.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -115,6 +116,29 @@ struct LoopNecessityCandidate {
   const uint16_t* depth;
   uint32_t depth_pitch;   // bytes
   uint32_t pad;
+};
+
+// The place index (place_index.cu, DESIGN.md §3.18): its resolved options and which keyframes hold a code.  The code table has
+// kPlaceRowWords words per keyframe row whatever the fern count, so that it is allocated once, for max_keyframes rows.
+constexpr int kPlaceRowWords = 2048 / 8;
+struct PlaceIndexState {
+  int num_ferns = 0;   // 0: no index yet
+  int min_raw = 0, max_raw = 0;
+  std::vector<uint8_t> indexed;   // [max_keyframes] once an index exists
+};
+
+// What the place index's kernels read of one image (place_index.cu): the depth and colour images and the code row it writes.
+struct PlaceImage {
+  const uint16_t* depth;
+  const uint8_t* rgba;   // uchar4
+  uint32_t depth_pitch, rgba_pitch;   // bytes
+  uint32_t* code;
+};
+// One query of the matching kernel: the code row it compares, its clipped keyframe range [first, last] (empty when first > last)
+// and the keyframe it excludes (-1: none).
+struct PlaceQueryRecord {
+  const uint32_t* code;
+  int first, last, exclude, pad;
 };
 
 // ---- keyframes ---------------------------------------------------------------------------------------------------------------
@@ -338,6 +362,15 @@ struct bba_context {
     bba::PinnedBuffer<bba::PoseGraphState> h_state;
   } graph;
 
+  // place index (bba_index_keyframes): the live state and code table [max_kf][kPlaceRowWords], allocated by the first call, and
+  // the encoder's image records.  Publish copies the table into the front end's slots with the cfactor.
+  struct Place {
+    bba::PlaceIndexState state;
+    bba::DeviceBuffer<uint32_t> codes;
+    bba::PinnedBuffer<bba::PlaceImage> h_images;
+    bba::DeviceBuffer<bba::PlaceImage> d_images;
+  } place;
+
   // in-loop surfel lifecycle (creation / merge / compaction) and the end tasks
   struct Lifecycle {
     bba::DeviceBuffer<unsigned int> d_sup;         // [3][cells]
@@ -438,10 +471,13 @@ struct bba_context {
     bba::CameraView cams;
     std::vector<bba::KeyframeView> kfs;
     std::vector<bba::PoseConstraint> constraints;   // the soft relative pose constraints, in id order
-    // Two device copies of the cfactor.  Publish copies d_cfactor into the slot that is not current, on the BA side's stream,
-    // after that slot's readers are done, records `published` and makes the slot current; a front-end call claims the
-    // current slot, makes its stream wait on `published` and records `readers_done` after its last read.
+    // Two device copies of the cfactor and of the place index's code table.  Publish copies d_cfactor (and, once an index
+    // exists, place.codes) into the slot that is not current, on the BA side's stream, after that slot's readers are done,
+    // records `published` and makes the slot current together with `place`; a front-end call claims the current slot, makes
+    // its stream wait on `published` and records `readers_done` after its last read.
     bba::DeviceBuffer<float> cfactor[2];
+    bba::DeviceBuffer<uint32_t> place_codes[2];
+    bba::PlaceIndexState place;   // the index state of the current slot
     bba::Event published[2];
     bba::Event readers_done[2];
     int current = 0;
@@ -458,6 +494,18 @@ struct bba_context {
       bba::DeviceBuffer<unsigned int> d_count;
       bba::PinnedBuffer<unsigned int> h_count;
     } loop;
+    // bba_query_place_index: the queries, the frames' image records and codes, the indexed flags and the matches (place_index.cu)
+    struct PlaceQuery {
+      bba::PinnedBuffer<bba::PlaceQueryRecord> h_queries;
+      bba::DeviceBuffer<bba::PlaceQueryRecord> d_queries;
+      bba::PinnedBuffer<bba::PlaceImage> h_images;
+      bba::DeviceBuffer<bba::PlaceImage> d_images;
+      bba::DeviceBuffer<uint32_t> d_frame_codes;   // [frames][kPlaceRowWords]
+      bba::PinnedBuffer<uint8_t> h_indexed;
+      bba::DeviceBuffer<uint8_t> d_indexed;
+      bba::DeviceBuffer<int> d_matches;            // [queries][2 * max_matches + 1]: ids, differences, count
+      bba::PinnedBuffer<int> h_matches;
+    } place_query;
   } fe;
 
   // kernels launched by BA-side calls and by front-end calls (bba_kernel_launch_count: the sum); two counters so that the
@@ -554,11 +602,16 @@ class FrontEndCall {
   FrontEndCall(const FrontEndCall&) = delete;
   FrontEndCall& operator=(const FrontEndCall&) = delete;
   // (max_kf_id: fails unless every keyframe id up to it is published; all_kfs: receives every published keyframe record)
-  bba_status Snapshot(cudaStream_t s, int kf_id, const char* fn, int max_kf_id = -1, std::vector<KeyframeView>* all_kfs = nullptr);
+  // (place: receives the place index state of the claimed slot; the call then fails with BBA_ERR_STATE before claiming anything
+  // when there is no index, and with BBA_ERR_INVALID_ARGUMENT when a keyframe of place_ids (may be null) is not indexed)
+  bba_status Snapshot(cudaStream_t s, int kf_id, const char* fn, int max_kf_id = -1, std::vector<KeyframeView>* all_kfs = nullptr,
+                      PlaceIndexState* place = nullptr, const std::vector<int>* place_ids = nullptr);
   bba_status ReleaseSlot(bool record = true);
   CameraView cams;
   KeyframeView base;
   const float* cfactor = nullptr;
+  const uint32_t* place_codes = nullptr;   // the claimed slot's code table (null before the first index)
+  int keyframe_count = 0;                  // published keyframes
 
  private:
   bba_handle h_;

@@ -923,6 +923,56 @@ class DirectBA:
         self._check(self._lib.bba_verify_loop_closures(self._h, C.byref(o), len(candidates), cands, out, self._stream_ptr(stream)))
         return list(out)[:len(candidates)]
 
+    def IndexKeyframes(self, ids=None, num_ferns: int = 512, min_depth: float = 0.5, max_depth: float = 3.0, stream=None):
+        """Encodes keyframes into the randomized-fern place index (bba_index_keyframes, DESIGN §3.18) from their current images;
+        ids None: every keyframe.  Options that differ from the current ones reset the index first.  Index a keyframe again
+        after changing its images."""
+        ids = np.arange(self.KeyframeCount(), dtype=np.int32) if ids is None else np.ascontiguousarray(ids, np.int32).reshape(-1)
+        o = _lib.PlaceIndexOptions(int(num_ferns), float(min_depth), float(max_depth))
+        self._check(self._lib.bba_index_keyframes(self._h, C.byref(o), len(ids), ids.ctypes.data if len(ids) else None,
+                                                  self._stream_ptr(stream)))
+
+    def KeyframeCount(self) -> int:
+        """The published keyframe count (bba_keyframe_count)."""
+        return int(self._lib.bba_keyframe_count(self._h))
+
+    def PlaceIndexOptions(self):
+        """The published place index's (num_ferns, min_raw, max_raw) (bba_get_place_index_options); zeros before the first index."""
+        v = [C.c_int(), C.c_int(), C.c_int()]
+        self._check(self._lib.bba_get_place_index_options(self._h, *(C.byref(x) for x in v)))
+        return tuple(x.value for x in v)
+
+    def QueryPlaceIndex(self, queries, frames=(), max_matches: int = 8, stream=None):
+        """Place-index queries in one call (bba_query_place_index).  queries: a sequence of (keyframe_id, frame, first_keyframe,
+        last_keyframe), keyframe_id -1 meaning the frame frames[frame] (a (depth, normals or None, colour) tuple of device
+        tensors) is encoded in this call.  Returns per query (ids, differences): the indexed keyframes of the range, the query
+        keyframe excluded, ordered by (difference, id), at most max_matches of them."""
+        bufs = (_lib.FrameBuffers * max(1, len(frames)))()
+        for b, (depth, normals, color) in zip(bufs, frames):
+            b.depth, b.depth_pitch = depth.data_ptr(), depth.stride(0) * 2
+            if normals is not None:
+                b.normals, b.normals_pitch = normals.data_ptr(), normals.stride(0) * 2
+            b.color_rgba, b.color_pitch = color.data_ptr(), color.stride(0)
+        qs = (_lib.PlaceQuery * max(1, len(queries)))()
+        for q, spec in zip(qs, queries):
+            q.keyframe_id, q.frame, q.first_keyframe, q.last_keyframe = (int(v) for v in spec)
+        n = len(queries)
+        ids = np.zeros((max(1, n), max_matches), np.int32)
+        diffs = np.zeros((max(1, n), max_matches), np.int32)
+        counts = np.zeros(max(1, n), np.int32)
+        self._check(self._lib.bba_query_place_index(self._h, len(frames), bufs if frames else None, n, qs, int(max_matches),
+                                                    ids.ctypes.data, diffs.ctypes.data, counts.ctypes.data, self._stream_ptr(stream)))
+        return [(ids[i, :counts[i]].copy(), diffs[i, :counts[i]].copy()) for i in range(n)]
+
+    def PlaceIndexCodes(self, ids, stream=None):
+        """The published place-index codes of indexed keyframes (bba_get_place_index_codes): uint32 [len(ids), num_ferns / 8]."""
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        words = self.PlaceIndexOptions()[0] // 8
+        out = np.zeros((len(ids), max(1, words)), np.uint32)
+        self._check(self._lib.bba_get_place_index_codes(self._h, len(ids), ids.ctypes.data if len(ids) else None, words,
+                                                        out.ctypes.data, self._stream_ptr(stream)))
+        return out
+
     def OdometryLevel(self, which: int, scale: int, stream=None):
         """Parity hook: (depth f32, normals u16, colour u8) of one pyramid level of the last TrackFramePairwise call
         (which: 0 = base keyframe, 1 = tracked frame)."""

@@ -25,12 +25,13 @@
  *        BA-side call is in flight -- also from inside progress_function.  The front-end calls are
  *        bba_preprocess_frame, bba_preprocess_raw_frame, bba_track_frame_pairwise,
  *        bba_track_frame_pairwise_to_frame, bba_track_frames_pairwise, bba_verify_loop_closures,
+ *        bba_query_place_index, bba_get_place_index_codes, bba_get_place_index_options,
  *        bba_odometry_get_level, bba_odometry_debug_coeffs, the
  *        bba_host_* functions (no handle) and the readers bba_keyframe_count, bba_get_keyframe_pose,
  *        bba_get_keyframe_states, bba_get_keyframe_activation, bba_get_intrinsics,
  *        bba_get_cfactor_host, bba_cfactor_size and bba_get_residual_types.
  *    Front-end calls read a snapshot of the state the BA side published last (cameras, a, cfactor,
- *    residual types, keyframe records and poses), never the state a running BA call is changing.
+ *    residual types, keyframe records and poses, place index), never the state a running BA call is changing.
  *    The BA side publishes in every setter, bba_add_keyframe*, bba_update_keyframe_host, at the end
  *    of every pose step (all poses together), of every intrinsics step and of every BA call.  With
  *    one thread a front-end call therefore sees exactly the handle's current state.  The front end
@@ -861,6 +862,70 @@ typedef struct {
 } bba_loop_verification;
 bba_status bba_verify_loop_closures(bba_handle h, const bba_loop_verification_options* options, int count,
                                     const bba_loop_candidate* candidates, bba_loop_verification* out, void* stream);
+
+/* ---- place recognition: the randomized-fern keyframe index (DESIGN.md §3.18; not in the reference) ----
+ * Finds loop-closure and relocalisation candidates on the device without a vocabulary or features (Glocker et al., TVCG 2015, as
+ * ElasticFusion uses it).  An image's code is F 4-bit fern values; fern f reads one cell of an 80 x 60 grid laid on the depth
+ * and on the colour image separately (cell (cx, cy) of a W x H image: x in [cx W / 80, (cx + 1) W / 80), y in [cy H / 60,
+ * (cy + 1) H / 60)).  Bit c (c = 0, 1, 2) is set when the sum of byte c of the uchar4 colour pixels exceeds t_c * n (n: the
+ * cell's pixels), bit 3 when the sum of the raw depth values without the invalid bit (0x8000) exceeds t_d * n_v (n_v: their
+ * count; no valid depth gives 0), all in exact integer arithmetic.  The raw values make a code depend on the images only, not on
+ * a or the cfactor.  The ferns come from splitmix64 with a fixed seed (bba_host_place_ferns).  A code is F / 8 words; fern f is
+ * the nibble at bit 4 (f % 8) of word f / 8.  The difference D(a, b) of two codes is the number of ferns whose nibbles differ.
+ * Everything is integer, so codes and matches are the same bits in every mode, on every rank and in every run.
+ * Depth and colour images must be at least 80 x 60 (BBA_ERR_UNSUPPORTED otherwise).
+ *
+ * bba_index_keyframes: a BA-side call.  Encodes the listed keyframes from their current depth and colour buffers in one launch
+ * (one CTA per keyframe) into a library-owned table of max_keyframes rows (1 KB each, with the front end's two published copies:
+ * 3 KB per keyframe, allocated by the first call), marks them indexed and publishes.  options NULL keeps the current options
+ * (the defaults on the first call); options that differ from the current ones reset the index first, so that only the listed
+ * keyframes are indexed afterwards.  Nothing is encoded by bba_add_keyframe* or bba_update_keyframe_host: after changing a
+ * keyframe's images, index it again.  Under several ranks every rank makes the same call; the codes are equal by construction.
+ * BBA_ERR_INVALID_ARGUMENT: NULL keyframe_ids, count < 1, an id that is not a keyframe, num_ferns not a multiple of 8 in
+ * [8, 2048], or a depth range outside 0 < min_raw <= max_raw <= 0x7fff with x_raw = llround(x / raw_to_float_depth) in fp64.
+ * Launches one kernel and does not synchronise.
+ *
+ * bba_query_place_index: a front-end call on the published index.  Query q compares the code of keyframe queries[q].keyframe_id
+ * (>= 0, which must be indexed), or of frames[queries[q].frame] encoded in this call (keyframe_id -1; the normals are not read),
+ * with the indexed keyframes whose ids lie in [first_keyframe, last_keyframe] clipped to the published keyframes, the query
+ * keyframe itself excluded.  The candidates are ordered by (D, id) ascending and the first min(max_matches, candidates) go to
+ * match_ids[q][.] / match_differences[q][.] ([count][max_matches], -1 after the last), their number to match_counts[q].  An empty
+ * range is valid and gives 0.  The range is the only policy: a loop detector asks for [0, current - gap], a relocaliser for
+ * everything; thresholds on D are the caller's.
+ * BBA_ERR_STATE: no index yet.  BBA_ERR_INVALID_ARGUMENT: a NULL queries or output array, count < 1, frame_count < 0, NULL frames
+ * with frame_count > 0, a frame index out of range, a NULL frame image, a pitch too small, a depth image or pitch that is not
+ * 2-byte aligned or a colour image or pitch that is not 4-byte aligned, keyframe_id < -1, a query keyframe
+ * that is not published or not indexed, or max_matches outside 1..64.  Arguments are checked before anything is enqueued, and a
+ * failed check leaves the handle and the launch counter unchanged.  Launches one matching kernel (one CTA per query), and one
+ * encoding kernel before it when a query names a frame; synchronises the stream once.
+ *
+ * bba_get_place_index_codes: a front-end call; the published codes of the listed indexed keyframes, [count][words_per_code] words.
+ * words_per_code must be the published index's num_ferns / 8 (bba_get_place_index_options gives num_ferns), so that out is never
+ * overrun when the options change between the two calls: BBA_ERR_INVALID_ARGUMENT otherwise.  Same errors as the query for the
+ * ids.  Synchronises the stream.
+ *
+ * bba_get_place_index_options: a front-end call; the published index's fern count and raw depth range (0 for each before the
+ * first bba_index_keyframes).  Any pointer may be NULL.
+ *
+ * bba_host_place_ferns: the fern table: cells [num_ferns][2] = (cx, cy) and thresholds [num_ferns][4] = (t_r, t_g, t_b, t_d).
+ * Returns BBA_ERR_INVALID_ARGUMENT (writing nothing) for the num_ferns or raw range the index refuses, or a NULL array. */
+typedef struct {
+  int num_ferns;      /* <= 0: 512 */
+  float min_depth;    /* m, <= 0: 0.5 */
+  float max_depth;    /* m, <= 0: 3.0 */
+} bba_place_index_options;
+typedef struct {
+  int keyframe_id;                    /* >= 0: that keyframe's stored code; -1: frames[frame] */
+  int frame;
+  int first_keyframe, last_keyframe;  /* the candidate range, inclusive */
+} bba_place_query;
+bba_status bba_index_keyframes(bba_handle h, const bba_place_index_options* options, int count, const int* keyframe_ids, void* stream);
+bba_status bba_query_place_index(bba_handle h, int frame_count, const bba_frame_buffers* frames, int count, const bba_place_query* queries,
+                                 int max_matches, int* match_ids, int* match_differences, int* match_counts, void* stream);
+bba_status bba_get_place_index_codes(bba_handle h, int count, const int* keyframe_ids, int words_per_code, uint32_t* out,
+                                     void* stream);
+bba_status bba_get_place_index_options(bba_handle h, int* num_ferns, int* min_raw, int* max_raw);
+int        bba_host_place_ferns(int num_ferns, int min_raw, int max_raw, int32_t* cells, int32_t* thresholds);
 
 /* ---- deterministic mode ----
  * Off by default.  When on, every floating-point sum whose order depends on the scheduling of the GPU goes through an exact,

@@ -252,6 +252,41 @@ class DirectBA {
           "bba_verify_loop_closures");
   }
 
+  // The randomized-fern place index (bba_index_keyframes, DESIGN.md §3.18; not in the reference): encodes the keyframes `ids`
+  // (every keyframe when empty) from their current images.  Options that differ from the current ones reset the index first.
+  void IndexKeyframes(cudaStream_t stream, const std::vector<int>& ids = {}, int num_ferns = 512, float min_depth = 0.5f,
+                      float max_depth = 3.0f) {
+    std::vector<int> all = ids;
+    if (all.empty())
+      for (int k = 0; k < bba_keyframe_count(h_); ++k) all.push_back(k);
+    const bba_place_index_options o{num_ferns, min_depth, max_depth};
+    Check(bba_index_keyframes(h_, &o, static_cast<int>(all.size()), all.data(), stream), "bba_index_keyframes");
+  }
+  // bba_query_place_index: per query, the ids and differences of at most max_matches candidates in (difference, id) order.
+  void QueryPlaceIndex(cudaStream_t stream, const std::vector<bba_place_query>& queries, const std::vector<bba_frame_buffers>& frames,
+                       int max_matches, std::vector<std::vector<int>>* ids, std::vector<std::vector<int>>* differences) {
+    const size_t n = queries.size();
+    std::vector<int> flat_ids(n * max_matches), flat_diffs(n * max_matches), counts(n);
+    Check(bba_query_place_index(h_, static_cast<int>(frames.size()), frames.empty() ? nullptr : frames.data(), static_cast<int>(n),
+                                queries.data(), max_matches, flat_ids.data(), flat_diffs.data(), counts.data(), stream),
+          "bba_query_place_index");
+    ids->assign(n, {});
+    differences->assign(n, {});
+    for (size_t q = 0; q < n; ++q) {
+      (*ids)[q].assign(flat_ids.begin() + q * max_matches, flat_ids.begin() + q * max_matches + counts[q]);
+      (*differences)[q].assign(flat_diffs.begin() + q * max_matches, flat_diffs.begin() + q * max_matches + counts[q]);
+    }
+  }
+  // bba_get_place_index_codes: num_ferns / 8 words per keyframe of `ids`, num_ferns of the published index.
+  std::vector<uint32_t> PlaceIndexCodes(cudaStream_t stream, const std::vector<int>& ids) {
+    int num_ferns = 0;
+    Check(bba_get_place_index_options(h_, &num_ferns, nullptr, nullptr), "bba_get_place_index_options");
+    std::vector<uint32_t> out(ids.size() * static_cast<size_t>(num_ferns / 8));
+    Check(bba_get_place_index_codes(h_, static_cast<int>(ids.size()), ids.data(), num_ferns / 8, out.data(), stream),
+          "bba_get_place_index_codes");
+    return out;
+  }
+
   // direct_ba.h:143-162, same argument order and defaults (Timer* is any type with GetTimeSinceStart()).
   template <typename TimerT = NoTimer>
   void BundleAdjustment(cudaStream_t stream, bool optimize_depth_intrinsics, bool optimize_color_intrinsics, bool do_surfel_updates,
