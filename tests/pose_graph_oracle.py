@@ -39,26 +39,26 @@ def so3_exp(w):
 
 
 def quat_from_matrix(R):
-    """Unit quaternions (x, y, z, w), w >= 0, of rotation matrices [..., 3, 3] (Shepperd's method, stable at any angle)."""
+    """Unit quaternions (x, y, z, w), w >= 0, of rotation matrices [..., 3, 3] (Shepperd's method, stable at any angle): each
+    matrix takes the branch of the largest of (trace, R00, R11, R22), the first one on a tie."""
     R = np.asarray(R, np.float64)
-    flat = R.reshape(-1, 3, 3)
-    q = np.zeros((len(flat), 4))
-    for i, M in enumerate(flat):
-        tr = np.trace(M)
-        k = int(np.argmax([tr, M[0, 0], M[1, 1], M[2, 2]]))
-        if k == 0:
-            s = 2.0 * np.sqrt(1.0 + tr)
-            q[i] = [(M[2, 1] - M[1, 2]) / s, (M[0, 2] - M[2, 0]) / s, (M[1, 0] - M[0, 1]) / s, s / 4]
-        else:
-            j, l = k % 3, (k + 1) % 3
-            m = k - 1
-            s = 2.0 * np.sqrt(1.0 + M[m, m] - M[j, j] - M[l, l])
-            v = np.zeros(4)
-            v[m] = s / 4
-            v[j] = (M[j, m] + M[m, j]) / s
-            v[l] = (M[l, m] + M[m, l]) / s
-            v[3] = (M[l, j] - M[j, l]) / s
-            q[i] = v
+    M = R.reshape(-1, 3, 3)
+    tr = M[:, 0, 0] + M[:, 1, 1] + M[:, 2, 2]
+    k = np.argmax(np.stack([tr, M[:, 0, 0], M[:, 1, 1], M[:, 2, 2]], -1), -1)
+    q = np.zeros((len(M), 4))
+    sel = k == 0
+    s = 2.0 * np.sqrt(1.0 + tr[sel])
+    Ms = M[sel]
+    q[sel] = np.stack([(Ms[:, 2, 1] - Ms[:, 1, 2]) / s, (Ms[:, 0, 2] - Ms[:, 2, 0]) / s, (Ms[:, 1, 0] - Ms[:, 0, 1]) / s, s / 4], -1)
+    for b in (1, 2, 3):   # the largest diagonal entry m = b - 1, then j and l in cyclic order
+        m, j, l = b - 1, b % 3, (b + 1) % 3
+        sel = k == b
+        Ms = M[sel]
+        s = 2.0 * np.sqrt(1.0 + Ms[:, m, m] - Ms[:, j, j] - Ms[:, l, l])
+        q[sel, m] = s / 4
+        q[sel, j] = (Ms[:, j, m] + Ms[:, m, j]) / s
+        q[sel, l] = (Ms[:, l, m] + Ms[:, m, l]) / s
+        q[sel, 3] = (Ms[:, l, j] - Ms[:, j, l]) / s
     q *= np.where(q[:, 3:] < 0, -1.0, 1.0)
     return q.reshape(R.shape[:-2] + (4,))
 
@@ -145,18 +145,59 @@ def residual(term, Ta, Tb=None, da=None, db=None):
     return se3_log(*mul(inv(term.Z), mul(inv(Ta), Tb)))
 
 
+def _residuals(Zi, Ta, Tb=None):
+    """residual over a batch: Zi = Z^-1, Ta, Tb (R [..., 3, 3], t [..., 3]) broadcast against each other; Tb None for priors."""
+    return se3_log(*mul(Zi, Ta if Tb is None else mul(inv(Ta), Tb)))
+
+
+def _batch_blocks(Zi, Ta, Tb=None, h=1e-6):
+    """(r [N, 6], J [N, 6, n]) of N terms of one kind (n = 6 for priors, 12 for constraints): r at (Ta, Tb), J by central
+    differences in every column of (da[, db]) at once, the columns of term_jacobian."""
+    n = 6 if Tb is None else 12
+    steps = np.concatenate([h * np.eye(n), -h * np.eye(n)])   # [2n, n]: +h e_i, then -h e_i
+    Zb = (Zi[0][:, None], Zi[1][:, None])
+    Xa = se3_exp(steps[:, :6])
+    Ta_p = mul((Ta[0][:, None], Ta[1][:, None]), Xa)
+    if Tb is None:
+        rp = _residuals(Zb, Ta_p)
+    else:
+        Tb_p = mul((Tb[0][:, None], Tb[1][:, None]), se3_exp(steps[:, 6:]))
+        rp = _residuals(Zb, Ta_p, Tb_p)
+    J = np.swapaxes(rp[:, :n] - rp[:, n:], -1, -2) / (2 * h)
+    return _residuals(Zi, Ta, Tb), J
+
+
+def _stack(terms):
+    """(a [N], b [N], Z^-1 (R [N, 3, 3], t [N, 3])) of a list of terms."""
+    a = np.array([t.a for t in terms], np.int64)
+    b = np.array([t.b for t in terms], np.int64)
+    Zi = inv((np.array([t.Z[0] for t in terms]).reshape(-1, 3, 3), np.array([t.Z[1] for t in terms]).reshape(-1, 3)))
+    return a, b, Zi
+
+
+def _linearise(terms, poses, jacobians=True):
+    """Every term's residual r [6] and, with `jacobians`, its term_jacobian J, in term order.  The terms of one kind are
+    evaluated together, each with term_blocks' own arithmetic, so the values are the per-term ones bit for bit."""
+    rs, Js = [None] * len(terms), [None] * len(terms)
+    if not terms:
+        return rs, Js
+    a, b, Zi = _stack(terms)
+    for sel in (np.nonzero(b < 0)[0], np.nonzero(b >= 0)[0]):
+        if len(sel) == 0:
+            continue
+        Z = (Zi[0][sel], Zi[1][sel])
+        Ta = (poses[0][a[sel]], poses[1][a[sel]])
+        Tb = None if b[sel[0]] < 0 else (poses[0][b[sel]], poses[1][b[sel]])
+        r, J = _batch_blocks(Z, Ta, Tb) if jacobians else (_residuals(Z, Ta, Tb), [None] * len(sel))
+        for i, n in enumerate(sel):
+            rs[n], Js[n] = r[i], J[i]
+    return rs, Js
+
+
 def term_jacobian(term, Ta, Tb=None, h=1e-6):
     """[6, 6] (prior) or [6, 12] (constraint): central differences of the residual in (da[, db])."""
-    n = 6 if term.b < 0 else 12
-    J = np.zeros((6, n))
-    for i in range(n):
-        e = np.zeros(n)
-        e[i] = h
-        if term.b < 0:
-            J[:, i] = (residual(term, Ta, da=e) - residual(term, Ta, da=-e)) / (2 * h)
-        else:
-            J[:, i] = (residual(term, Ta, Tb, e[:6], e[6:]) - residual(term, Ta, Tb, -e[:6], -e[6:])) / (2 * h)
-    return J
+    one = lambda T: None if T is None else (np.asarray(T[0], np.float64)[None], np.asarray(T[1], np.float64)[None])
+    return _batch_blocks(_stack([term])[2], one(Ta), None if term.b < 0 else one(Tb), h)[1][0]
 
 
 def term_blocks(term, Ta, Tb=None):
@@ -168,8 +209,7 @@ def term_blocks(term, Ta, Tb=None):
 
 def total_cost(terms, poses):
     c = 0.0
-    for t in terms:
-        r = residual(t, pose(poses, t.a), None if t.b < 0 else pose(poses, t.b))
+    for t, r in zip(terms, _linearise(terms, poses, jacobians=False)[0]):
         c += 0.5 * r @ t.L @ r
     return c
 
@@ -220,18 +260,16 @@ def normal_equations(terms, poses, held):
     K = len(poses[0])
     rows, cols, vals = [], [], []
     b = np.zeros(6 * K)
-    for t in terms:
+    for t, r, J in zip(terms, *_linearise(terms, poses)):   # term_blocks' H and b of every term, summed in term order
         if t.b < 0:
-            H, g, _ = term_blocks(t, pose(poses, t.a))
             idx = np.arange(6 * t.a, 6 * t.a + 6)
         else:
-            H, g, _ = term_blocks(t, pose(poses, t.a), pose(poses, t.b))
             idx = np.r_[6 * t.a:6 * t.a + 6, 6 * t.b:6 * t.b + 6]
         ii, jj = np.meshgrid(idx, idx, indexing="ij")
         rows.append(ii.ravel())
         cols.append(jj.ravel())
-        vals.append(H.ravel())
-        b[idx] += g
+        vals.append((J.T @ t.L @ J).ravel())
+        b[idx] += J.T @ t.L @ r
     H = sp.csr_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(6 * K, 6 * K))
     free = np.repeat(~held, 6)
     return H[free][:, free], b[free], np.nonzero(free)[0]

@@ -130,3 +130,60 @@ def test_held_rule():
     held = O.held_keyframes(9, t, gauge=5)
     # 0, 3, 8: untouched; 1: lowest of a component without gauge or prior; 5: the gauge; {6, 7} has a prior
     assert np.nonzero(held)[0].tolist() == [0, 1, 3, 5, 8]
+
+
+def _scalar_blocks(t, Ta, Tb=None, h=1e-6):
+    """One term's (H, b, cost) with its Jacobian column by column: the per-term statement the batched oracle must sum to."""
+    n = 6 if t.b < 0 else 12
+    J = np.zeros((6, n))
+    for i in range(n):
+        e = np.zeros(n)
+        e[i] = h
+        if t.b < 0:
+            J[:, i] = (O.residual(t, Ta, da=e) - O.residual(t, Ta, da=-e)) / (2 * h)
+        else:
+            J[:, i] = (O.residual(t, Ta, Tb, e[:6], e[6:]) - O.residual(t, Ta, Tb, -e[:6], -e[6:])) / (2 * h)
+    r = O.residual(t, Ta, Tb)
+    return J.T @ t.L @ J, J.T @ t.L @ r, 0.5 * r @ t.L @ r
+
+
+def test_batched_normal_equations_are_the_per_term_sum():
+    K = 40
+    rng = np.random.default_rng(12)
+
+    def info():
+        G = rng.normal(size=(6, 6))
+        return G @ G.T + 0.5 * np.eye(6)
+    # the chain, constraints with a < b and a > b, and priors, interleaved, each with its own information
+    truth, start, terms = _graph(K, [], seed=12)
+    for a, b in ((5, K - 3), (30, 12), (17, 2), (0, 39)):
+        Z = O.mul(O.mul(O.inv(O.pose(truth, a)), O.pose(truth, b)), O.se3_exp(rng.normal(0, 0.05, 6)))
+        terms.insert(int(rng.integers(len(terms))), O.Term(a, b, Z, info()))
+    for k in (0, 9, 21, 39):
+        terms.insert(int(rng.integers(len(terms))), O.Term(k, -1, O.mul(O.pose(truth, k), O.se3_exp(rng.normal(0, 0.05, 6))), info()))
+    Hs, bs, cost = np.zeros((6 * K, 6 * K)), np.zeros(6 * K), 0.0
+    for t in terms:
+        H, g, c = _scalar_blocks(t, O.pose(start, t.a), None if t.b < 0 else O.pose(start, t.b))
+        idx = np.r_[6 * t.a:6 * t.a + 6] if t.b < 0 else np.r_[6 * t.a:6 * t.a + 6, 6 * t.b:6 * t.b + 6]
+        Hs[np.ix_(idx, idx)] += H
+        bs[idx] += g
+        cost += c
+    for held in (np.zeros(K, bool), O.held_keyframes(K, terms, 7)):
+        H, b, free = O.normal_equations(terms, start, held)
+        assert np.array_equal(free, np.nonzero(np.repeat(~held, 6))[0])
+        want = Hs[np.ix_(free, free)]
+        assert np.abs(H.toarray() - want).max() <= 1e-12 * np.abs(want).max()
+        assert np.abs(b - bs[free]).max() <= 1e-12 * np.abs(bs).max()
+    assert abs(O.total_cost(terms, start) - cost) <= 1e-12 * cost
+
+
+def test_reduction_levels_fit_the_solver_workspace():
+    """The odd-even reduction over K blocks keeps levels of n_0 = K, n_(l+1) = ceil(n_l / 2) blocks down to one; the solver's
+    workspace (PoseGraphWorkDoubles, MakeWork) gives them 2 K + 32 slots.  Every K up to 2^20."""
+    K = np.arange(1, 2 ** 20 + 1)
+    n, total = K.copy(), K.copy()
+    while (n > 1).any():
+        step = n > 1
+        n = np.where(step, (n + 1) // 2, n)
+        total += np.where(step, n, 0)
+    assert (total <= 2 * K + 32).all(), int(np.max(total - 2 * K))
