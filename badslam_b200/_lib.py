@@ -272,6 +272,8 @@ SYMBOLS = {
     "bba_update_surfel_activation": (C.c_int, [_P, _P]),
     "bba_optimize_geometry_iteration": (C.c_int, [_P, _P]),
     "bba_deform_surfels": (C.c_int, [_P, C.c_int, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P]),
+    "bba_measure_keyframe_covisibility": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "bba_debug_set_covisibility_chunk": (C.c_int, [_P, C.c_uint32]),
     "bba_optimize_pose_graph": (C.c_int, [_P, C.POINTER(PoseGraphOptions), C.POINTER(PoseGraphResult), _P]),
     "bba_optimize_intrinsics": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "bba_debug_intrinsics_coeffs": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P]),

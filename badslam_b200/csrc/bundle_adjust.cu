@@ -853,12 +853,98 @@ bba_status DeformSurfels(bba_handle h, int count, const float* original, uint32_
   return BBA_OK;
 }
 
+// The bit rows of one chunk of the stream take K x chunk / 32 words: chunks of at most this many bytes of them (DESIGN §3.19).
+constexpr uint64_t kCovisibilityBitsBudget = 128ull << 20;
+
+// bba_measure_keyframe_covisibility.  Every argument is checked before anything is enqueued; nothing on the handle changes but the
+// spatial order, which is rebuilt when stale (a function of the positions alone).
+bba_status MeasureKeyframeCovisibility(bba_handle h, int count, const int* ids, int keyframe_count, uint32_t* out, cudaStream_t s) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  const std::string fn = "bba_measure_keyframe_covisibility: ";
+  const int K = static_cast<int>(h->keyframes.size());
+  if (!out) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null out_counts");
+  if (count == 0 || count < -1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad count");
+  if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null keyframe_ids");
+  if (keyframe_count != K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "keyframe_count is not the handle's keyframe count");
+  for (int i = 0; i < count; ++i)
+    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown keyframe id");
+  const int rows = count < 0 ? K : count;
+  const uint32_t n = h->surfels_size;
+  if (K == 0 || n == 0) {
+    std::fill(out, out + static_cast<size_t>(rows) * K, 0u);
+    return BBA_OK;
+  }
+  if (bba_status st = CheckSurfels(h)) return st;
+  auto& c = h->covis;
+  uint32_t chunk = c.chunk;
+  if (chunk == 0) {   // whole 256-surfel geometry tiles
+    const uint64_t fit = kCovisibilityBitsBudget * 8 / static_cast<uint64_t>(K);
+    chunk = static_cast<uint32_t>(std::max<uint64_t>(256, std::min<uint64_t>(fit, 0xffffff00ull) / 256 * 256));
+  }
+  chunk = std::min(chunk, n);
+  const uint32_t words = (chunk + 31u) / 32u;
+  BBA_CUDA(h, c.d_bits.Reserve(static_cast<size_t>(K) * words));
+  BBA_CUDA(h, c.d_counts.Reserve(static_cast<size_t>(rows) * K));
+  if (count > 0) BBA_CUDA(h, c.d_rows.Reserve(count));
+  if (bba_status st = MakeAllKeyframeList(h)) return st;
+  if (bba_status st = UploadKeyframes(h, s)) return st;   // the current poses
+  if (count > 0) BBA_CUDA(h, cudaMemcpyAsync(c.d_rows, ids, sizeof(int) * count, cudaMemcpyHostToDevice, s));
+  BBA_CUDA(h, cudaMemsetAsync(c.d_counts, 0, sizeof(uint32_t) * rows * K, s));
+  // Every rank measures its whole replica (begin 0, end n, one shard), in the spatial order unless the geometry launches keep the
+  // caller's (peer stores): the counts do not depend on the order.
+  const bool sort = !PeerStores(h);
+  if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/false, s)) return st;
+  bba::CovisibilityBitsArgs a;
+  bba::GeometryArgs& g = a.geo;
+  SetSurfelFields(h, &g);
+  g.shard_rank = 0;
+  g.shard_world = 1;
+  g.perm = sort ? h->pose.order.view.perm : nullptr;
+  g.stream = h->pose.order.stream;
+  g.stream_pitch = h->pose.order.capacity;
+  g.active = h->active;
+  g.kfs = h->d_kfs;
+  g.kf_list = h->geo.d_all_list;
+  g.kf_count = K;
+  g.queue = h->geo.d_queue;
+  g.peers = PeerSet{};
+  if (bba_status st = ReserveTileEpochs(h)) return st;
+  g.tile_epoch = h->geo.d_tile_epoch;
+  a.bits = c.d_bits;
+  const bba::CovisibilityGramArgs q{c.d_bits, 0, count > 0 ? c.d_rows.get() : h->geo.d_all_list.get(), rows, K, c.d_counts};
+  for (uint32_t begin = 0; begin < n; begin += chunk) {
+    g.begin = begin;
+    g.end = begin + std::min(chunk, n - begin);
+    g.tile_shift = 8;
+    a.words = (g.end - g.begin + 31u) / 32u;
+    BBA_CUDA(h, cudaMemsetAsync(c.d_bits, 0, sizeof(uint32_t) * K * a.words, s));
+    BBA_LAUNCH(h, h->launches, LaunchCovisibilityBits, a, h->sm_count, s);
+    bba::CovisibilityGramArgs qc = q;
+    qc.words = a.words;
+    BBA_LAUNCH(h, h->launches, LaunchCovisibilityGram, qc, h->sm_count, s);
+  }
+  BBA_CUDA(h, cudaMemcpyAsync(out, c.d_counts, sizeof(uint32_t) * rows * K, cudaMemcpyDeviceToHost, s));
+  BBA_CUDA(h, cudaStreamSynchronize(s));
+  return BBA_OK;
+}
+
 }  // namespace
 }  // namespace bba
 
 using namespace bba;
 
 extern "C" {
+
+bba_status bba_measure_keyframe_covisibility(bba_handle h, int count, const int* keyframe_ids, int keyframe_count, uint32_t* out_counts,
+                                             void* stream) {
+  return MeasureKeyframeCovisibility(h, count, keyframe_ids, keyframe_count, out_counts, static_cast<cudaStream_t>(stream));
+}
+
+bba_status bba_debug_set_covisibility_chunk(bba_handle h, uint32_t surfels) {
+  if (!h) return BBA_ERR_INVALID_ARGUMENT;
+  h->covis.chunk = surfels;
+  return BBA_OK;
+}
 
 bba_status bba_update_surfel_activation(bba_handle h, void* stream) {
   return GeometryPass(h, /*activation=*/true, static_cast<cudaStream_t>(stream));

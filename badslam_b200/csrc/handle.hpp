@@ -342,6 +342,15 @@ struct bba_context {
     bba::PinnedBuffer<unsigned int> h_counts;
   } deform;
 
+  // keyframe co-visibility (bba_measure_keyframe_covisibility): the bit rows of one chunk of the stream, the listed rows' ids and
+  // the counts, allocated by the first call
+  struct Covisibility {
+    bba::DeviceBuffer<uint32_t> d_bits;     // [K][words of a chunk]
+    bba::DeviceBuffer<int> d_rows;
+    bba::DeviceBuffer<uint32_t> d_counts;   // [rows][K]
+    uint32_t chunk = 0;   // surfels per chunk (bba_debug_set_covisibility_chunk); 0: the budget rule
+  } covis;
+
   // keyframe pose graph (bba_optimize_pose_graph): the terms, the held flags, the row lists and the block-CSR structure (one pinned
   // staging buffer of ints and its device copy), the fp32 poses and the state; the terms' blocks, H, b, M and the solver's work in
   // one fp64 buffer.  Sized for max_keyframes and the constraints, with room to double the constraints (ReservePoseGraph).

@@ -1179,6 +1179,113 @@ __global__ void __launch_bounds__(kGeoThreads) DeformSurfelsKernel(const __grid_
   }
 }
 
+// Keyframe co-visibility, bit rows (DESIGN §3.19).  The walk is DeformSurfelsKernel's at the current poses, without the sums: for
+// every 32-surfel sub-step and visible keyframe j the ballot of the association test is word w = sub-step of row j, stored when
+// it is not zero.  Nothing is parked between groups, so the items need no epoch order.
+__global__ void __launch_bounds__(kGeoThreads) CovisibilityBitsKernel(const __grid_constant__ CovisibilityBitsArgs c) {
+  extern __shared__ __align__(16) unsigned char geo_smem[];
+  const GeometryArgs& a = c.geo;
+  KfDevice* s_kfs = reinterpret_cast<KfDevice*>(geo_smem);
+  const uint32_t tile_len = 1u << a.tile_shift;
+  const uint32_t n_tiles = (a.end - a.begin + tile_len - 1) >> a.tile_shift;
+  const uint32_t n_groups = (a.kf_count + kGeoGroup - 1) / kGeoGroup;
+  const uint32_t n_items = n_groups * n_tiles;
+  const size_t F = a.stream_pitch;
+  const int lane = threadIdx.x & 31;
+  uint32_t group, tile;
+  while (ClaimItem(a.queue, n_tiles, n_items, nullptr, &group, &tile)) {
+    const int j_begin = group * kGeoGroup, j_end = min(a.kf_count, static_cast<int>(group + 1) * kGeoGroup);
+    const int n_kf = j_end - j_begin;
+    KfDevice* recs = s_kfs + (threadIdx.x >> 5) * kGeoGroup;
+    StageGroupRecords(a.kfs, a.kf_list + j_begin, n_kf, recs, lane);
+    for (uint32_t sub = 0; sub < tile_len / 32; ++sub) {
+      uint32_t s;
+      const bool in_range = GeoStreamPosition(a, tile, sub, lane, &s);
+      Vec3 gp = V3(0.f, 0.f, 0.f), nrm = V3(0.f, 0.f, 1.f);
+      if (in_range) gp = V3(a.stream[0 * F + s], a.stream[1 * F + s], a.stream[2 * F + s]);
+      const bool live = in_range && !isnan(gp.x);   // deleted surfels: x = NaN
+      if (__ballot_sync(0xffffffffu, live) == 0) continue;
+      if (live) nrm = UnpackNormal(__float_as_uint(a.stream[3 * F + s]));
+      float lo[3], hi[3];
+      WarpBox(gp, live, lo, hi);
+      unsigned vis = VisibleKeyframes<false>(a.cam, recs, n_kf, lo, hi, lane);
+      const uint32_t w = (tile << (a.tile_shift - 5)) + sub;
+      for (int j = PopLowest(&vis); j >= 0; j = PopLowest(&vis)) {
+        KfRegs K;
+        LoadKfShared(recs + j, &K);
+        Assoc r;
+        const bool assoc = live && ProjectIntoImage(a.cam, K.T, gp, &r) &&
+                           Associate(a.cam, K.T, nrm, LoadPixel(a.cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r), &r) == 3;
+        const unsigned word = __ballot_sync(0xffffffffu, assoc);
+        if (lane == 0 && word) c.bits[static_cast<size_t>(j_begin + j) * c.words + w] = word;
+      }
+    }
+  }
+}
+
+// Keyframe co-visibility, the counts: counts[i][b] += sum_w popc(bits[rows[i]][w] & bits[b][w]).  A CTA owns a 64 x 64 tile of
+// counts and the word range blockIdx.z of every row; it stages 32-word slices of its 64 listed rows and 64 columns in shared
+// memory, and thread (tx, ty) sums rows ty + 16 i and columns tx + 16 j (i, j < 4) in registers.  A slice pair in which either side
+// is all zero -- most of them: a keyframe sees a compact part of the spatially ordered stream -- is skipped.  The sums go to the
+// counts with integer atomics, so the result does not depend on the order in which the CTAs finish.
+constexpr int kGramTile = 64, kGramSlice = 32, kGramThreads = 256;
+__global__ void __launch_bounds__(kGramThreads) CovisibilityGramKernel(const __grid_constant__ CovisibilityGramArgs a) {
+  __shared__ uint32_t s_a[kGramTile][kGramSlice + 1], s_b[kGramTile][kGramSlice + 1];   // (+1: conflict-free column reads)
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int row0 = blockIdx.y * kGramTile, col0 = blockIdx.x * kGramTile;
+  const uint32_t per = (a.words + gridDim.z - 1) / gridDim.z;
+  const uint32_t w0 = blockIdx.z * per, w1 = min(a.words, w0 + per);
+  // staging: thread t loads word t % 32 of tile rows t / 32 + 8 k
+  const int load_w = threadIdx.x & 31, load_r = threadIdx.x >> 5;
+  const uint32_t* a_row[kGramTile / 8];
+  const uint32_t* b_row[kGramTile / 8];
+#pragma unroll
+  for (int k = 0; k < kGramTile / 8; ++k) {
+    const int r = row0 + load_r + 8 * k, b = col0 + load_r + 8 * k;
+    a_row[k] = r < a.row_count ? a.bits + static_cast<size_t>(__ldg(a.rows + r)) * a.words : nullptr;
+    b_row[k] = b < a.col_count ? a.bits + static_cast<size_t>(b) * a.words : nullptr;
+  }
+  uint32_t acc[4][4] = {};
+  for (uint32_t base = w0; base < w1; base += kGramSlice) {
+    const uint32_t w = base + load_w;
+    uint32_t any_a = 0u, any_b = 0u;
+#pragma unroll
+    for (int k = 0; k < kGramTile / 8; ++k) {
+      const uint32_t va = w < w1 && a_row[k] ? __ldg(a_row[k] + w) : 0u;
+      const uint32_t vb = w < w1 && b_row[k] ? __ldg(b_row[k] + w) : 0u;
+      s_a[load_r + 8 * k][load_w] = va;
+      s_b[load_r + 8 * k][load_w] = vb;
+      any_a |= va;
+      any_b |= vb;
+    }
+    const bool nonzero_a = __syncthreads_or(any_a != 0u);
+    const bool nonzero_b = __syncthreads_or(any_b != 0u);
+    if (nonzero_a && nonzero_b) {
+#pragma unroll 4
+      for (int kk = 0; kk < kGramSlice; ++kk) {
+        uint32_t x[4], y[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          x[i] = s_a[ty + 16 * i][kk];
+          y[i] = s_b[tx + 16 * i][kk];
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) acc[i][j] += __popc(x[i] & y[j]);
+      }
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int r = row0 + ty + 16 * i, b = col0 + tx + 16 * j;
+      if (acc[i][j] && r < a.row_count && b < a.col_count) atomicAdd(a.counts + static_cast<size_t>(r) * a.col_count + b, acc[i][j]);
+    }
+}
+
 constexpr size_t kGeoSmemBytes = sizeof(KfDevice) * (kGeoThreads / 32) * kGeoGroup;   // the per-warp record slices
 
 // Everything a geometry launch does before its kernel: the grid (with *a's tile), the counters and the stream gather.
@@ -1209,6 +1316,26 @@ LaunchResult LaunchDeformSurfels(const DeformArgs& args, int sm_count, cudaStrea
   const LaunchResult r = PrepareGeo(DeformSurfelsKernel, &a.geo, sm_count, false, stream, &grid);
   DeformSurfelsKernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
   return r;
+}
+
+LaunchResult LaunchCovisibilityBits(const CovisibilityBitsArgs& args, int sm_count, cudaStream_t stream) {
+  if (args.geo.end <= args.geo.begin || args.geo.kf_count <= 0) return {};
+  CovisibilityBitsArgs a = args;
+  uint32_t grid;
+  const LaunchResult r = PrepareGeo(CovisibilityBitsKernel, &a.geo, sm_count, false, stream, &grid);
+  CovisibilityBitsKernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
+  return r;
+}
+
+// grid.z splits the words so that the grid holds about four CTAs per SM (one slice at least per CTA).
+LaunchResult LaunchCovisibilityGram(const CovisibilityGramArgs& a, int sm_count, cudaStream_t stream) {
+  if (a.words == 0 || a.row_count <= 0 || a.col_count <= 0) return {};
+  const uint32_t gx = (a.col_count + kGramTile - 1) / kGramTile, gy = (a.row_count + kGramTile - 1) / kGramTile;
+  if (gy > 65535) return {0, cudaErrorInvalidValue};
+  const uint64_t tiles = static_cast<uint64_t>(gx) * gy, slices = (a.words + kGramSlice - 1) / kGramSlice;
+  const uint64_t gz = std::min<uint64_t>({std::max<uint64_t>(1, (4 * static_cast<uint64_t>(sm_count) + tiles - 1) / tiles), slices, 65535});
+  CovisibilityGramKernel<<<dim3(gx, gy, static_cast<uint32_t>(gz)), kGramThreads, 0, stream>>>(a);
+  return {1};
 }
 
 LaunchResult LaunchActivationAndNormals(const GeometryArgs& a, int sm_count, bool determine_activation, bool update_normals,

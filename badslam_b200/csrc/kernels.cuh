@@ -262,6 +262,25 @@ struct DeformArgs {
 // The stream gather and the kernel, or nothing when there is nothing to do.  Deleted surfels (x = NaN) are skipped.
 LaunchResult LaunchDeformSurfels(const DeformArgs& a, int sm_count, cudaStream_t stream);
 
+// Keyframe co-visibility (bba_measure_keyframe_covisibility, DESIGN §3.19): which keyframes each surfel is associated with at the
+// current poses, as bit rows over one chunk [geo.begin, geo.end) of the stream, then the shared counts of keyframe pairs.
+struct CovisibilityBitsArgs {
+  GeometryArgs geo;   // kfs: every keyframe's record at its current pose; kf_list: 0 .. kf_count - 1
+  uint32_t* bits;     // [kf_count][words], zero at launch: bit L of word w of row k <=> stream position begin + 32 w + L is
+                      //   associated with keyframe k
+  uint32_t words;     // ceil((end - begin) / 32)
+};
+// The stream gather and the kernel.  Deleted surfels (x = NaN) are skipped.
+LaunchResult LaunchCovisibilityBits(const CovisibilityBitsArgs& a, int sm_count, cudaStream_t stream);
+struct CovisibilityGramArgs {
+  const uint32_t* bits;   // [col_count][words]
+  uint32_t words;
+  const int* rows;        // [row_count] bit rows (keyframe ids)
+  int row_count, col_count;
+  uint32_t* counts;       // [row_count][col_count] += sum_w popc(bits[rows[i]][w] & bits[b][w])
+};
+LaunchResult LaunchCovisibilityGram(const CovisibilityGramArgs& a, int sm_count, cudaStream_t stream);
+
 // Multi-GPU surfel sharding: 256-surfel granules are dealt round-robin to the ranks (granule g belongs to rank g % world), so
 // that every rank sees the same mix of well- and poorly-observed surfels (surfels are stored in creation order, and the
 // cost of a surfel is the number of keyframes that see it).  A rank addresses its surfels through a dense local index.

@@ -738,6 +738,25 @@ class DirectBA:
                                                  self._stream_ptr(stream)))
         return moved.value, unobserved.value
 
+    def MeasureKeyframeCovisibility(self, ids=None, stream=None) -> np.ndarray:
+        """bba_measure_keyframe_covisibility (not in the reference): uint32 [len(ids), K], entry [i, b] the number of surfels
+        associated with both keyframe ids[i] and keyframe b at their current poses ([i, ids[i]]: the surfels ids[i] observes).
+        ids=None: every keyframe in id order.  Synchronises the stream."""
+        K = self.KeyframeCount()
+        if ids is None:
+            out = np.zeros((K, K), np.uint32)
+            self._check(self._lib.bba_measure_keyframe_covisibility(self._h, -1, None, K, out.ctypes.data, self._stream_ptr(stream)))
+            return out
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        out = np.zeros((len(ids), K), np.uint32)
+        self._check(self._lib.bba_measure_keyframe_covisibility(self._h, len(ids), ids.ctypes.data if len(ids) else None, K,
+                                                                out.ctypes.data, self._stream_ptr(stream)))
+        return out
+
+    def DebugSetCovisibilityChunk(self, surfels: int):
+        """bba_debug_set_covisibility_chunk: surfels per chunk of MeasureKeyframeCovisibility (0: the 128 MiB budget rule)."""
+        self._check(self._lib.bba_debug_set_covisibility_chunk(self._h, int(surfels)))
+
     def SurfelsDeviceView(self) -> torch.Tensor:
         """The 17-row surfel buffer as a torch tensor, whoever owns it (zero-copy)."""
         if self._surfels is not None:

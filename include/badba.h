@@ -448,6 +448,26 @@ bba_status bba_optimize_geometry_iteration(bba_handle h, void* stream);
  * or an empty map: nothing to do.  A BA-side call. */
 bba_status bba_deform_surfels(bba_handle h, int count, const float* original_keyframe_T_global, uint32_t* moved, uint32_t* unobserved,
                               void* stream);
+/* Measures keyframe co-visibility on the device (not in the reference; DESIGN.md §3.19): out_counts[i][b] is the number of surfels
+ * associated with both keyframe ids[i] and keyframe b, and out_counts[i][ids[i]] the number keyframe ids[i] observes.  "Associated"
+ * is the association test of the geometry passes and of bba_deform_surfels (its voters) at the keyframes' CURRENT poses, with the
+ * current cameras, a and cfactor, for every keyframe whatever its activation and every surfel in [0, surfels_size); deleted
+ * surfels (x = NaN) count nowhere.  Unlike bba_get_covisibility (the reference's frustum intersection) it sees occlusion, depth
+ * and normals and gives a strength: the graph that loop-candidate filters, local BA windows and essential-graph edges are built
+ * from (INTEGRATION.md).
+ * count = -1: every keyframe in id order (keyframe_ids is not read); otherwise the rows of keyframe_ids [count], repeats allowed.
+ * out_counts [rows][keyframe_count]; keyframe_count must be the handle's keyframe count, so that out_counts is never overrun.  The
+ * counts are exact integers, the same bits with any surfel order, chunking, deterministic mode or number of ranks (every rank
+ * measures its whole replica; no exchange).  An empty map or no keyframes gives zeros without a launch.
+ * BBA_ERR_INVALID_ARGUMENT: a NULL out_counts, a NULL keyframe_ids with count > 0, count = 0 or < -1, an unknown id or a
+ * keyframe_count mismatch; arguments are checked before anything is enqueued, and a failed check changes nothing.  A BA-side call:
+ * it changes no surfel row, flag, pose, activation or published state (it may rebuild a stale spatial order of the surfels),
+ * launches three kernels per chunk of the surfel stream (128 MiB of bit rows each) and synchronises the stream once. */
+bba_status bba_measure_keyframe_covisibility(bba_handle h, int count, const int* keyframe_ids, int keyframe_count, uint32_t* out_counts,
+                                             void* stream);
+/* Sets the surfels per chunk of every later bba_measure_keyframe_covisibility (0: the 128 MiB budget rule), so that tests can force
+ * many chunks.  The counts are the same bits for every chunk size.  For tests and timing. */
+bba_status bba_debug_set_covisibility_chunk(bba_handle h, uint32_t surfels);
 /* Optimises the keyframe pose graph on the device (DESIGN.md §3.14): what the reference's PoseGraphOptimizer
  * (pose_graph_optimizer.cc, g2o + CSparse, called from loop_detector.cc after a loop closure) does, over the handle's own pose
  * terms.  It minimises over the keyframe poses

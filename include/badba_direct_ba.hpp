@@ -287,6 +287,19 @@ class DirectBA {
     return out;
   }
 
+  // bba_measure_keyframe_covisibility (not in the reference): counts [ids.size()][K], entry (i, b) the surfels associated with both
+  // keyframe ids[i] and keyframe b at their current poses; an empty ids: every keyframe in id order.  A BA-side call; synchronises
+  // the stream.
+  void MeasureKeyframeCovisibility(cudaStream_t stream, const std::vector<int>& ids, std::vector<uint32_t>* counts) {
+    const int K = bba_keyframe_count(h_);
+    const int rows = ids.empty() ? K : static_cast<int>(ids.size());
+    counts->assign(static_cast<size_t>(rows) * K, 0u);
+    if (rows == 0) return;
+    Check(bba_measure_keyframe_covisibility(h_, ids.empty() ? -1 : static_cast<int>(ids.size()), ids.empty() ? nullptr : ids.data(), K,
+                                            counts->data(), stream),
+          "bba_measure_keyframe_covisibility");
+  }
+
   // direct_ba.h:143-162, same argument order and defaults (Timer* is any type with GetTimeSinceStart()).
   template <typename TimerT = NoTimer>
   void BundleAdjustment(cudaStream_t stream, bool optimize_depth_intrinsics, bool optimize_color_intrinsics, bool do_surfel_updates,
