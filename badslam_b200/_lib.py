@@ -129,6 +129,15 @@ class FrameBuffers(C.Structure):   # bba_frame_buffers
                 ("color_rgba", C.c_void_p), ("color_pitch", C.c_size_t)]
 
 
+class FrameOverlapQuery(C.Structure):   # bba_frame_overlap_query
+    _fields_ = [("frame", C.c_int), ("global_T_frame", C.c_float * 7), ("min_depth", C.c_float), ("max_depth", C.c_float)]
+
+
+class FrameOverlap(C.Structure):   # bba_frame_overlap
+    _fields_ = [("observed_surfels", C.c_uint32), ("valid_cells", C.c_uint32), ("uncovered_cells", C.c_uint32),
+                ("new_surfels", C.c_uint32)]
+
+
 class OdometryEntry(C.Structure):   # bba_odometry_entry
     _fields_ = [("base_keyframe_id", C.c_int), ("base_frame", C.c_int), ("tracked_frame", C.c_int),
                 ("base_T_frame_initial_1", C.c_float * 7), ("base_T_frame_initial_2", C.c_float * 7)]
@@ -274,6 +283,8 @@ SYMBOLS = {
     "bba_deform_surfels": (C.c_int, [_P, C.c_int, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P]),
     "bba_measure_keyframe_covisibility": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
     "bba_debug_set_covisibility_chunk": (C.c_int, [_P, C.c_uint32]),
+    "bba_measure_frame_overlap": (C.c_int, [_P, C.c_int, C.POINTER(FrameBuffers), C.c_int, C.POINTER(FrameOverlapQuery), C.c_int, _P,
+                                            C.POINTER(FrameOverlap), _P]),
     "bba_optimize_pose_graph": (C.c_int, [_P, C.POINTER(PoseGraphOptions), C.POINTER(PoseGraphResult), _P]),
     "bba_optimize_intrinsics": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "bba_debug_intrinsics_coeffs": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P]),

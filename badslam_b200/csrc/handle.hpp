@@ -351,6 +351,21 @@ struct bba_context {
     uint32_t chunk = 0;   // surfels per chunk (bba_debug_set_covisibility_chunk); 0: the budget rule
   } covis;
 
+  // frame overlap (bba_measure_frame_overlap): the query frames' records, the Gram's row list, the frames' co-visible keyframes
+  // (CSR), their cell bit rows and the counts ([n][3] seed counts, then the Gram); the bit rows live in covis.d_bits.  Grown on
+  // demand by the calls; the host side is staging for one call, which synchronises before it returns.
+  struct FrameOverlap {
+    bba::DeviceBuffer<bba::KfDevice> d_frames;
+    bba::PinnedBuffer<bba::KfDevice> h_frames;
+    bba::DeviceBuffer<int> d_ints;        // [rows | covis offsets]
+    bba::PinnedBuffer<int> h_ints;
+    bba::DeviceBuffer<bba::CovisEntry> d_covis;
+    bba::PinnedBuffer<bba::CovisEntry> h_covis;
+    bba::DeviceBuffer<uint32_t> d_cells;  // [n][cell words]
+    bba::DeviceBuffer<uint32_t> d_counts;
+    bba::PinnedBuffer<uint32_t> h_counts;
+  } overlap;
+
   // keyframe pose graph (bba_optimize_pose_graph): the terms, the held flags, the row lists and the block-CSR structure (one pinned
   // staging buffer of ints and its device copy), the fp32 poses and the state; the terms' blocks, H, b, M and the solver's work in
   // one fp64 buffer.  Sized for max_keyframes and the constraints, with room to double the constraints (ReservePoseGraph).

@@ -1181,7 +1181,11 @@ __global__ void __launch_bounds__(kGeoThreads) DeformSurfelsKernel(const __grid_
 
 // Keyframe co-visibility, bit rows (DESIGN §3.19).  The walk is DeformSurfelsKernel's at the current poses, without the sums: for
 // every 32-surfel sub-step and visible keyframe j the ballot of the association test is word w = sub-step of row j, stored when
-// it is not zero.  Nothing is parked between groups, so the items need no epoch order.
+// it is not zero.  Nothing is parked between groups, so the items need no epoch order.  The association test is ProjectAssociate's
+// three steps (SupportLevel0Kernel's test), spelled out.  CELLS (the frames of bba_measure_frame_overlap, DESIGN §3.20): every
+// associated lane also sets the bit of its pixel's sparse cell in record j's cell row -- the cells surfel creation would find
+// supported.
+template <bool CELLS>
 __global__ void __launch_bounds__(kGeoThreads) CovisibilityBitsKernel(const __grid_constant__ CovisibilityBitsArgs c) {
   extern __shared__ __align__(16) unsigned char geo_smem[];
   const GeometryArgs& a = c.geo;
@@ -1218,6 +1222,10 @@ __global__ void __launch_bounds__(kGeoThreads) CovisibilityBitsKernel(const __gr
                            Associate(a.cam, K.T, nrm, LoadPixel(a.cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r), &r) == 3;
         const unsigned word = __ballot_sync(0xffffffffu, assoc);
         if (lane == 0 && word) c.bits[static_cast<size_t>(j_begin + j) * c.words + w] = word;
+        if (CELLS && assoc) {
+          const unsigned int cell = SparseCell(a.cam, r.px, r.py);
+          atomicOr(c.cells + static_cast<size_t>(j_begin + j) * c.cell_words + (cell >> 5), 1u << (cell & 31u));
+        }
       }
     }
   }
@@ -1322,8 +1330,13 @@ LaunchResult LaunchCovisibilityBits(const CovisibilityBitsArgs& args, int sm_cou
   if (args.geo.end <= args.geo.begin || args.geo.kf_count <= 0) return {};
   CovisibilityBitsArgs a = args;
   uint32_t grid;
-  const LaunchResult r = PrepareGeo(CovisibilityBitsKernel, &a.geo, sm_count, false, stream, &grid);
-  CovisibilityBitsKernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
+  if (a.cells) {
+    const LaunchResult r = PrepareGeo(CovisibilityBitsKernel<true>, &a.geo, sm_count, false, stream, &grid);
+    CovisibilityBitsKernel<true><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
+    return r;
+  }
+  const LaunchResult r = PrepareGeo(CovisibilityBitsKernel<false>, &a.geo, sm_count, false, stream, &grid);
+  CovisibilityBitsKernel<false><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
   return r;
 }
 

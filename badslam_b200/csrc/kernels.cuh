@@ -269,6 +269,10 @@ struct CovisibilityBitsArgs {
   uint32_t* bits;     // [kf_count][words], zero at launch: bit L of word w of row k <=> stream position begin + 32 w + L is
                       //   associated with keyframe k
   uint32_t words;     // ceil((end - begin) / 32)
+  uint32_t* cells = nullptr;   // null, or (the frame form of bba_measure_frame_overlap, DESIGN §3.20) [kf_count][cell_words]:
+                               //   bit c of row k <=> an associated surfel projects into sparse cell c of record k's image; zero
+                               //   before the first chunk
+  uint32_t cell_words = 0;     // ceil(cells / 32)
 };
 // The stream gather and the kernel.  Deleted surfels (x = NaN) are skipped.
 LaunchResult LaunchCovisibilityBits(const CovisibilityBitsArgs& a, int sm_count, cudaStream_t stream);
@@ -465,6 +469,23 @@ LaunchResult LaunchMergeSurfels(const LifecycleArgs& a, int sm_count, cudaStream
 LaunchResult LaunchSeedNewSurfels(const LifecycleArgs& a, bool filter, cudaStream_t stream);    // a.flags after LaunchSupportSurfels
 LaunchResult LaunchExclusiveScan(const unsigned int* in, uint32_t n, unsigned int* out, unsigned int* block_sums, cudaStream_t stream);
 LaunchResult LaunchCreateSurfels(const LifecycleArgs& a, const unsigned int* index, cudaStream_t stream);
+
+// The seed count of bba_measure_frame_overlap (DESIGN §3.20): for every sparse cell of every frame, SeedKernel's seed pixel, whether
+// the frame's cell bit row (LaunchCovisibilityBits' cells) leaves the cell uncovered, and FilterSeedsKernel's test of the seed
+// against the frame's co-visible keyframes.
+struct FrameSeedArgs {
+  CameraParams cam;
+  const KfDevice* frames;        // [frame_count]: depth, normals and their pitches
+  int frame_count;
+  uint32_t cells;
+  const uint32_t* covered;       // [frame_count][cell_words]
+  uint32_t cell_words;
+  const CovisEntry* covis;       // frame f's entries: [covis_offsets[f], covis_offsets[f + 1])
+  const int* covis_offsets;      // [frame_count + 1]
+  int min_observation_count;
+  uint32_t* counts;              // [frame_count][3] += valid, uncovered, surviving cells; zero at launch
+};
+LaunchResult LaunchFrameSeedCount(const FrameSeedArgs& a, cudaStream_t stream);
 
 // bba_debug_exact_sum: deposits the n values into *sum (zero at launch) from many CTAs, each visiting the values in a scrambled
 // order, and rounds the result into *out.

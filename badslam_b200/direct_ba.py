@@ -52,6 +52,18 @@ def _frame_buffers(frames):
     return bufs
 
 
+@dataclass
+class FrameOverlap:
+    """DirectBA.MeasureFrameOverlap's result: per query, the surfels associated with the frame, the sparse cells with a valid
+    depth pixel, those no associated surfel falls into, and those whose new surfel would survive the filter (uint32 [n]);
+    shared [n, K] uint32 (surfels shared with each keyframe) or None."""
+    observed_surfels: np.ndarray
+    valid_cells: np.ndarray
+    uncovered_cells: np.ndarray
+    new_surfels: np.ndarray
+    shared: Optional[np.ndarray]
+
+
 def _odometry_options(num_scales, use_pyramid_level_0, use_gradmag, test_different_initial_estimates, max_iterations_per_scale):
     return _lib.OdometryOptions(int(num_scales), int(use_pyramid_level_0), int(use_gradmag), int(test_different_initial_estimates),
                                 int(max_iterations_per_scale))
@@ -752,6 +764,31 @@ class DirectBA:
         self._check(self._lib.bba_measure_keyframe_covisibility(self._h, len(ids), ids.ctypes.data if len(ids) else None, K,
                                                                 out.ctypes.data, self._stream_ptr(stream)))
         return out
+
+    def MeasureFrameOverlap(self, frames, queries, with_shared: bool = True, stream=None) -> FrameOverlap:
+        """bba_measure_frame_overlap (not in the reference, DESIGN §3.20): what the surfel map already explains of frames that are
+        not keyframes.  frames: a sequence of (depth, normals[, colour]) [h, w] u16 device tensors (colour is not read); queries: a
+        sequence of (frame index, global_T_frame [7], min_depth, max_depth).  With the same buffers, pose and depth range,
+        AddKeyframe + CreateSurfelsForKeyframe would create uncovered_cells surfels unfiltered and new_surfels filtered.
+        with_shared=False skips the keyframes' side (shared is None then, as it is without keyframes).  Synchronises the stream."""
+        bufs = (_lib.FrameBuffers * len(frames))()
+        for b, fr in zip(bufs, frames):
+            depth, normals = fr[0], fr[1]
+            b.depth, b.depth_pitch = depth.data_ptr(), depth.stride(0) * 2
+            b.normals, b.normals_pitch = normals.data_ptr(), normals.stride(0) * 2
+        qs = (_lib.FrameOverlapQuery * max(1, len(queries)))()
+        for q, (f, pose, lo, hi) in zip(qs, queries):
+            q.frame = int(f)
+            q.global_T_frame[:] = np.ascontiguousarray(pose, np.float32).reshape(7).tolist()
+            q.min_depth, q.max_depth = float(lo), float(hi)
+        n, K = len(queries), self.KeyframeCount()
+        out = (_lib.FrameOverlap * max(1, n))()
+        shared = np.zeros((n, K), np.uint32) if with_shared and K > 0 else None
+        self._check(self._lib.bba_measure_frame_overlap(self._h, len(frames), bufs if len(frames) else None, n, qs if n else None, K,
+                                                        None if shared is None else shared.ctypes.data, out if n else None,
+                                                        self._stream_ptr(stream)))
+        col = lambda name: np.array([getattr(o, name) for o in list(out)[:n]], np.uint32)
+        return FrameOverlap(col("observed_surfels"), col("valid_cells"), col("uncovered_cells"), col("new_surfels"), shared)
 
     def DebugSetCovisibilityChunk(self, surfels: int):
         """bba_debug_set_covisibility_chunk: surfels per chunk of MeasureKeyframeCovisibility (0: the 128 MiB budget rule)."""

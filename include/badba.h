@@ -466,8 +466,43 @@ bba_status bba_deform_surfels(bba_handle h, int count, const float* original_key
 bba_status bba_measure_keyframe_covisibility(bba_handle h, int count, const int* keyframe_ids, int keyframe_count, uint32_t* out_counts,
                                              void* stream);
 /* Sets the surfels per chunk of every later bba_measure_keyframe_covisibility (0: the 128 MiB budget rule), so that tests can force
- * many chunks.  The counts are the same bits for every chunk size.  For tests and timing. */
+ * many chunks.  The counts are the same bits for every chunk size (of bba_measure_frame_overlap's too).  For tests and timing. */
 bba_status bba_debug_set_covisibility_chunk(bba_handle h, uint32_t surfels);
+/* One query of bba_measure_frame_overlap: a frame at a pose. */
+typedef struct {
+  int frame;                   /* index into frames */
+  float global_T_frame[7];     /* the pose to measure at, e.g. the tracked pose */
+  float min_depth, max_depth;  /* the depth range bba_add_keyframe would get (bba_preprocess_frame returns it): the frustum */
+} bba_frame_overlap_query;
+typedef struct {
+  uint32_t observed_surfels;   /* surfels associated with the frame at the pose */
+  uint32_t valid_cells;        /* sparse cells holding a valid depth pixel inside the one-pixel border (surfel creation's seed rule) */
+  uint32_t uncovered_cells;    /* of those, cells no associated surfel falls into */
+  uint32_t new_surfels;        /* uncovered cells whose seed survives the new-surfel filter */
+} bba_frame_overlap;
+/* Measures what the surfel map already explains of tracked frames that are not keyframes (not in the reference; DESIGN.md §3.20):
+ * the input of a keyframe decision (make frame i a keyframe when out[i].new_surfels / out[i].valid_cells is large) and of the choice
+ * of a reference keyframe (the argmax of shared[i]).  For each query i, frames[queries[i].frame] at queries[i].global_T_frame:
+ * - a surfel is associated with the frame when the association test of surfel creation's support pass (and of
+ *   bba_measure_keyframe_covisibility) passes at the query pose, with the current cameras, a and cfactor; deleted surfels
+ *   (x = NaN) count nowhere; an associated surfel covers the sparse cell of the pixel it projects to;
+ * - valid_cells and the seed pixel of a cell follow surfel creation's seed rule; new_surfels applies its filter to the seed of
+ *   every uncovered cell, against the keyframes whose frusta intersect the query's (the keyframes bba_add_keyframe would make
+ *   co-visible with it), with the minimum observation count the handle would use with one keyframe more.
+ * So if the frame is then added with bba_add_keyframe (same buffers, pose and depth range) and bba_create_surfels_for_keyframe runs
+ * on it while the surfel capacity suffices, `created` equals uncovered_cells with filter_new_surfels = 0 and new_surfels with 1.
+ * shared [count][keyframe_count] (may be NULL): shared[i][b] is the number of surfels associated with both query i and keyframe b
+ * at b's current pose; NULL skips the keyframes' side of the measurement.  Frames have the depth resolution; only depth and
+ * normals are read (color_rgba may be NULL).  keyframe_count must be the handle's keyframe count.  Every output is an exact
+ * integer, the same bits with any surfel order, chunking, deterministic mode or number of ranks (every rank measures its whole
+ * replica; no exchange).  An empty map still counts the cells; with no keyframes shared is not written.
+ * BBA_ERR_INVALID_ARGUMENT: a NULL frames, queries or out, count or frame_count < 1, a frame index out of range, a NULL depth or
+ * normals buffer, a pitch too small or odd, a non-finite pose or a zero quaternion, a depth range that is not 0 < min <= max, or
+ * a keyframe_count mismatch; arguments are checked before anything is enqueued, and a failed check changes nothing.  A BA-side
+ * call: it changes nothing on the handle (it may rebuild a stale spatial order of the surfels) and synchronises the stream once. */
+bba_status bba_measure_frame_overlap(bba_handle h, int frame_count, const bba_frame_buffers* frames, int count,
+                                     const bba_frame_overlap_query* queries, int keyframe_count, uint32_t* shared,
+                                     bba_frame_overlap* out, void* stream);
 /* Optimises the keyframe pose graph on the device (DESIGN.md §3.14): what the reference's PoseGraphOptimizer
  * (pose_graph_optimizer.cc, g2o + CSparse, called from loop_detector.cc after a loop closure) does, over the handle's own pose
  * terms.  It minimises over the keyframe poses

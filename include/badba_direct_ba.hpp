@@ -300,6 +300,20 @@ class DirectBA {
           "bba_measure_keyframe_covisibility");
   }
 
+  // bba_measure_frame_overlap (not in the reference): per query, what the surfel map already explains of a frame that is not a
+  // keyframe (*out, one record per query) and, with a non-null shared, the surfels it shares with every keyframe ([queries][K]).
+  // A BA-side call; synchronises the stream.
+  void MeasureFrameOverlap(cudaStream_t stream, const std::vector<bba_frame_buffers>& frames,
+                           const std::vector<bba_frame_overlap_query>& queries, std::vector<bba_frame_overlap>* out,
+                           std::vector<uint32_t>* shared = nullptr) {
+    const int K = bba_keyframe_count(h_);
+    out->assign(queries.size(), bba_frame_overlap{});
+    if (shared) shared->assign(queries.size() * static_cast<size_t>(K), 0u);
+    Check(bba_measure_frame_overlap(h_, static_cast<int>(frames.size()), frames.data(), static_cast<int>(queries.size()), queries.data(), K,
+                                    shared && K > 0 ? shared->data() : nullptr, out->data(), stream),
+          "bba_measure_frame_overlap");
+  }
+
   // direct_ba.h:143-162, same argument order and defaults (Timer* is any type with GetTimeSinceStart()).
   template <typename TimerT = NoTimer>
   void BundleAdjustment(cudaStream_t stream, bool optimize_depth_intrinsics, bool optimize_color_intrinsics, bool do_surfel_updates,
