@@ -112,6 +112,11 @@ class PoseGraphResult(C.Structure):   # bba_pose_graph_result
                 ("initial_cost", C.c_double), ("final_cost", C.c_double)]
 
 
+class ExposureOptions(C.Structure):   # bba_exposure_options
+    _fields_ = [("gauge_keyframe", C.c_int), ("min_luma", C.c_int), ("max_luma", C.c_int), ("inlier_threshold", C.c_float),
+                ("outer_iterations", C.c_int)]
+
+
 class PeerHandle(C.Structure):
     _fields_ = [("surfels_ipc", C.c_ubyte * 64), ("surfels_offset", C.c_uint64), ("active_ipc", C.c_ubyte * 64),
                 ("active_offset", C.c_uint64), ("pitch_bytes", C.c_uint64), ("surfels_size", C.c_uint32), ("rank", C.c_int32)]
@@ -283,6 +288,10 @@ SYMBOLS = {
     "bba_deform_surfels": (C.c_int, [_P, C.c_int, _P, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P]),
     "bba_measure_keyframe_covisibility": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
     "bba_debug_set_covisibility_chunk": (C.c_int, [_P, C.c_uint32]),
+    "bba_estimate_keyframe_exposures": (C.c_int, [_P, C.POINTER(ExposureOptions), C.c_int, _P, _P, _P, _P, _P]),
+    "bba_set_keyframe_exposures": (C.c_int, [_P, C.c_int, _P, _P, _P]),
+    "bba_get_keyframe_exposures": (C.c_int, [_P, C.c_int, _P, _P]),
+    "bba_debug_get_exposure_system": (C.c_int, [_P, C.c_int, _P, _P]),
     "bba_measure_frame_overlap": (C.c_int, [_P, C.c_int, C.POINTER(FrameBuffers), C.c_int, C.POINTER(FrameOverlapQuery), C.c_int, _P,
                                             C.POINTER(FrameOverlap), _P]),
     "bba_optimize_pose_graph": (C.c_int, [_P, C.POINTER(PoseGraphOptions), C.POINTER(PoseGraphResult), _P]),

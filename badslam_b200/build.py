@@ -38,6 +38,7 @@ UNITS = [
     ("frames.cu", []),
     ("loop_verification.cu", ["-Xptxas", "-v"]),
     ("place_index.cu", ["-Xptxas", "-v"]),
+    ("exposure.cu", ["-Xptxas", "-v"]),   # (the fp64 solve: no -use_fast_math)
 ]
 HEADERS = ["device_math.cuh", "exact_sum.cuh", "kernels.cuh", "launch.hpp", "persistent.cuh", "odometry.cuh", "preprocess_tile.cuh", "host_math.hpp", "handle.hpp", "rendezvous.hpp", os.path.join("..", "..", "include", "badba.h")]
 

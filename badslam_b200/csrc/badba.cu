@@ -113,6 +113,7 @@ bba_status Publish(bba_handle h, cudaStream_t s, bool cfactor) {
     v.activation = kf.activation;
     v.prior = h->pose_priors[k];
     v.attitude = h->attitude_priors[k];
+    v.gain = kf.gain;
   }
   const CameraView cams = LiveCameraView(h);
   std::vector<PoseConstraint> constraints = h->pose_constraints;
@@ -573,9 +574,10 @@ bba_status bba_update_keyframe_host(bba_handle h, int id, const uint16_t* host_d
     }
     BBA_CUDA(h, cudaMemcpy2DAsync(dst->get(), dst->pitch(), host_color_rgba, static_cast<size_t>(cw) * 4,
                                   static_cast<size_t>(cw) * 4, ch, cudaMemcpyHostToDevice, s));
-    const LumaSource source{dst->get(), dst->pitch()};
+    const LumaSource source{dst->get(), dst->pitch(), kf.gain};   // (the keyframe's exposure, DESIGN §3.21)
     Texture* const luma = &kf.luma;
     if (bba_status st = MakeLumaTextures(h, /*front_end=*/false, 1, &source, &luma, s)) return st;
+    kf.color_staged = dst == &h->staging.color;   // no colour image left to re-extract a gain from
   }
   return Publish(h, s, false);
 }

@@ -21,12 +21,28 @@ void DetermineCovisibleActiveKeyframes(bba_handle h) {
   }
 }
 
+}  // namespace
+
 // The per-tile group epochs of the geometry kernels for surfels_size surfels, with room for max_surfel_count when they grow.
 bba_status ReserveTileEpochs(bba_handle h) {
   const uint32_t need = (h->surfels_size + 31u) / 32u;
   BBA_CUDA(h, h->geo.d_tile_epoch.Reserve(need, std::max<uint32_t>((h->cfg.max_surfel_count + 31u) / 32u, need) + 1));
   return BBA_OK;
 }
+
+// geo.d_all_list, the keyframe list 0 .. max_keyframes - 1, made on first use.
+bba_status MakeAllKeyframeList(bba_handle h) {
+  if (h->geo.d_all_list) return BBA_OK;   // (set only once it is filled)
+  DeviceBuffer<int> all;
+  BBA_CUDA(h, all.Reserve(h->cfg.max_keyframes));
+  std::vector<int> iota(h->cfg.max_keyframes);
+  for (int i = 0; i < h->cfg.max_keyframes; ++i) iota[i] = i;
+  BBA_CUDA(h, cudaMemcpy(all, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice));
+  h->geo.d_all_list = std::move(all);
+  return BBA_OK;
+}
+
+namespace {
 
 // In which order the geometry launches visit the surfels.  kCaller: the caller's (the in-loop creation's two launches address the
 // old and the new surfels by caller index, the PCG scheme's shards are the caller's granules).  kByPairs: the spatial order from
@@ -65,18 +81,6 @@ bba_status BuildGeometryArgs(bba_handle h, bba::GeometryArgs* g, cudaStream_t s,
   g->peers = KernelPeers(h);
   if (bba_status st = ReserveTileEpochs(h)) return st;
   g->tile_epoch = h->geo.d_tile_epoch;
-  return BBA_OK;
-}
-
-// geo.d_all_list, the keyframe list 0 .. max_keyframes - 1, made on first use.
-bba_status MakeAllKeyframeList(bba_handle h) {
-  if (h->geo.d_all_list) return BBA_OK;   // (set only once it is filled)
-  DeviceBuffer<int> all;
-  BBA_CUDA(h, all.Reserve(h->cfg.max_keyframes));
-  std::vector<int> iota(h->cfg.max_keyframes);
-  for (int i = 0; i < h->cfg.max_keyframes; ++i) iota[i] = i;
-  BBA_CUDA(h, cudaMemcpy(all, iota.data(), sizeof(int) * iota.size(), cudaMemcpyHostToDevice));
-  h->geo.d_all_list = std::move(all);
   return BBA_OK;
 }
 
@@ -852,9 +856,6 @@ bba_status DeformSurfels(bba_handle h, int count, const float* original, uint32_
   if (unobserved) *unobserved = counts[1];
   return BBA_OK;
 }
-
-// The bit rows of one chunk of the stream take K x chunk / 32 words: chunks of at most this many bytes of them (DESIGN §3.19).
-constexpr uint64_t kCovisibilityBitsBudget = 128ull << 20;
 
 // bba_measure_keyframe_covisibility.  Every argument is checked before anything is enqueued; nothing on the handle changes but the
 // spatial order, which is rebuilt when stale (a function of the positions alone).

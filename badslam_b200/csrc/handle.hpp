@@ -154,6 +154,8 @@ struct Keyframe {
   PitchedBuffer owned[3];          // depth / normals / radius copies made by bba_add_keyframe_host
   PitchedBuffer owned_rgba;
   Texture luma;                    // library-owned u8 CUDA array (the .w channel of the colour image) + its texture
+  float gain = 1.f;                // exposure (bba_set_keyframe_exposures): luma = min(255, rint(colour .w / gain))
+  bool color_staged = false;       // the luma came last from the shared staging image (caller-owned colour updated from the host)
   int last_active_in_ba_iteration = -1;   // keyframe.cc:47-48
   int last_covis_in_ba_iteration = -1;
   Pose pose;                 // global_T_frame
@@ -185,6 +187,7 @@ struct KeyframeView {
   int activation = BBA_KF_ACTIVE;
   PosePrior prior{};
   AttitudePrior attitude{};
+  float gain = 1.f;
 };
 
 // A soft relative pose constraint as the handle keeps it: its id, the caller's record, and the information of the equivalent
@@ -350,6 +353,23 @@ struct bba_context {
     bba::DeviceBuffer<uint32_t> d_counts;   // [rows][K]
     uint32_t chunk = 0;   // surfels per chunk (bba_debug_set_covisibility_chunk); 0: the budget rule
   } covis;
+
+  // keyframe exposures (bba_estimate_keyframe_exposures, exposure.cu): the listed ids and colour images, the per-surfel integer
+  // sums of one chunk (n / sum of the members, two test sets), C and r of the listed keyframes, the Q16 log gains of every round,
+  // the solve's work and results.  The bit rows live in covis.d_bits.  Grown on demand by the calls.
+  struct Exposure {
+    bba::DeviceBuffer<int> d_ids;
+    bba::DeviceBuffer<bba::ExposureImage> d_images;
+    bba::DeviceBuffer<uint32_t> d_n, d_test_n[2];
+    bba::DeviceBuffer<long long> d_sum, d_test_sum[2];
+    bba::DeviceBuffer<uint32_t> d_C;      // [count][count] of the last round
+    bba::DeviceBuffer<long long> d_r;     // [count]
+    bba::DeviceBuffer<int> d_xq;          // [rounds][count]
+    bba::DeviceBuffer<int> d_csr;         // solve: row starts [count + 1], reached [count], columns [count * count]
+    bba::DeviceBuffer<double> d_work;     // solve: x, r, z, p, q [count] each
+    bba::DeviceBuffer<uint32_t> d_diag;   // [2][count] C's diagonal after the first and the last round
+    int count = 0;                        // of the last estimate, 0 before the first
+  } exposure;
 
   // frame overlap (bba_measure_frame_overlap): the query frames' records, the Gram's row list, the frames' co-visible keyframes
   // (CSR), their cell bit rows and the counts ([n][3] seed counts, then the Gram); the bit rows live in covis.d_bits.  Grown on
@@ -699,6 +719,14 @@ bba_status TrackPairsOnSnapshot(bba_handle h, const bba_odometry_options& o, Fro
                                 int frame_count, const bba_frame_buffers* frames, int count, const bba_odometry_entry* entries,
                                 const int* tracked_keyframe_ids, bool release_slot, float* out, bba_odometry_result* results,
                                 cudaStream_t s);
+
+// bundle_adjust.cu
+// The per-tile group epochs of the geometry kernels for surfels_size surfels, with room for max_surfel_count when they grow.
+bba_status ReserveTileEpochs(bba_handle h);
+// geo.d_all_list, the keyframe list 0 .. max_keyframes - 1, made on first use.
+bba_status MakeAllKeyframeList(bba_handle h);
+// The bit rows of one chunk of the stream take K x chunk / 32 words: chunks of at most this many bytes of them (DESIGN §3.19).
+constexpr uint64_t kCovisibilityBitsBudget = 128ull << 20;
 
 // multi_gpu.cu
 void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t* shard_len);

@@ -1185,10 +1185,13 @@ __global__ void __launch_bounds__(kGeoThreads) DeformSurfelsKernel(const __grid_
 // three steps (SupportLevel0Kernel's test), spelled out.  CELLS (the frames of bba_measure_frame_overlap, DESIGN §3.20): every
 // associated lane also sets the bit of its pixel's sparse cell in record j's cell row -- the cells surfel creation would find
 // supported.
-template <bool CELLS>
-__global__ void __launch_bounds__(kGeoThreads) CovisibilityBitsKernel(const __grid_constant__ CovisibilityBitsArgs c) {
+//
+// The walk itself is CovisibilityWalk: for every sub-step it calls v.Begin(s, live), then v.Pair(row, w, s, assoc, r) for every
+// visible keyframe (row: its position in kf_list, assoc: the lane's association test), then v.End(s, live); the calls are
+// warp-uniform.  The exposure walk (ExposureWalkKernel, DESIGN §3.21) is the same walk with another visitor.
+template <class Visitor>
+__device__ __forceinline__ void CovisibilityWalk(const GeometryArgs& a, Visitor& v) {
   extern __shared__ __align__(16) unsigned char geo_smem[];
-  const GeometryArgs& a = c.geo;
   KfDevice* s_kfs = reinterpret_cast<KfDevice*>(geo_smem);
   const uint32_t tile_len = 1u << a.tile_shift;
   const uint32_t n_tiles = (a.end - a.begin + tile_len - 1) >> a.tile_shift;
@@ -1214,21 +1217,109 @@ __global__ void __launch_bounds__(kGeoThreads) CovisibilityBitsKernel(const __gr
       WarpBox(gp, live, lo, hi);
       unsigned vis = VisibleKeyframes<false>(a.cam, recs, n_kf, lo, hi, lane);
       const uint32_t w = (tile << (a.tile_shift - 5)) + sub;
+      v.Begin(s, live);
       for (int j = PopLowest(&vis); j >= 0; j = PopLowest(&vis)) {
         KfRegs K;
         LoadKfShared(recs + j, &K);
         Assoc r;
         const bool assoc = live && ProjectIntoImage(a.cam, K.T, gp, &r) &&
                            Associate(a.cam, K.T, nrm, LoadPixel(a.cam, K.depth, K.depth_pitch, K.normals, K.normals_pitch, r), &r) == 3;
-        const unsigned word = __ballot_sync(0xffffffffu, assoc);
-        if (lane == 0 && word) c.bits[static_cast<size_t>(j_begin + j) * c.words + w] = word;
-        if (CELLS && assoc) {
-          const unsigned int cell = SparseCell(a.cam, r.px, r.py);
-          atomicOr(c.cells + static_cast<size_t>(j_begin + j) * c.cell_words + (cell >> 5), 1u << (cell & 31u));
+        v.Pair(j_begin + j, w, s, assoc, r);
+      }
+      v.End(s, live);
+    }
+  }
+}
+
+template <bool CELLS>
+struct CovisibilityVisitor {
+  const CovisibilityBitsArgs& c;
+  __device__ __forceinline__ void Begin(uint32_t, bool) {}
+  __device__ __forceinline__ void End(uint32_t, bool) {}
+  __device__ __forceinline__ void Pair(int row, uint32_t w, uint32_t, bool assoc, const Assoc& r) {
+    const unsigned word = __ballot_sync(0xffffffffu, assoc);
+    if ((threadIdx.x & 31) == 0 && word) c.bits[static_cast<size_t>(row) * c.words + w] = word;
+    if (CELLS && assoc) {
+      const unsigned int cell = SparseCell(c.geo.cam, r.px, r.py);
+      atomicOr(c.cells + static_cast<size_t>(row) * c.cell_words + (cell >> 5), 1u << (cell & 31u));
+    }
+  }
+};
+
+template <bool CELLS>
+__global__ void __launch_bounds__(kGeoThreads) CovisibilityBitsKernel(const __grid_constant__ CovisibilityBitsArgs c) {
+  CovisibilityVisitor<CELLS> v{c};
+  CovisibilityWalk(c.geo, v);
+}
+
+// Keyframe exposures (DESIGN §3.21): the observation of a pair and its membership (ExposureWalkArgs), then per RHS
+//  false: n and sum of the members, summed over the keyframes of a sub-step in registers and added with one integer atomic
+//         per surfel; with bits, the members' ballot words;
+//  true:  rhs[row] += n y - sum, reduced over the warp and added with one integer atomic per keyframe and sub-step.
+template <bool RHS>
+struct ExposureVisitor {
+  const ExposureWalkArgs& e;
+  uint32_t cnt = 0, tn = 0;   // accumulate: members of the sub-step; the surfel's test count / rhs: n
+  long long acc = 0, tsum = 0;   // accumulate: their sum / rhs: sum; the surfel's test sum
+  __device__ __forceinline__ void Begin(uint32_t s, bool live) {
+    if (!live) return;
+    const uint32_t i = s - e.geo.begin;
+    if (e.test_n) {
+      tn = __ldg(e.test_n + i);
+      tsum = __ldg(e.test_sum + i);
+    }
+    if (RHS) {
+      cnt = __ldg(e.n + i);
+      acc = __ldg(e.sum + i);
+    }
+  }
+  __device__ __forceinline__ void Pair(int row, uint32_t w, uint32_t, bool assoc, const Assoc& r) {
+    int y = 0;
+    bool member = false;
+    float ccx, ccy;
+    if (assoc && DepthToColor(e.geo.cam, r.pxf, r.pyf, &ccx, &ccy)) {
+      const ExposureImage im = e.images[row];
+      const int v = __ldg(im.rgba + static_cast<size_t>(ccy) * im.pitch + 4 * static_cast<size_t>(ccx) + 3);
+      if (v >= e.min_luma && v <= e.max_luma) {
+        y = e.log_q16[v];
+        member = true;
+        if (e.test_n) {
+          const long long d = static_cast<long long>(tn) * (y - __ldg(e.test_x + row)) - tsum;
+          member = (d < 0 ? -d : d) <= static_cast<long long>(tn) * e.tau;
         }
       }
     }
+    if (RHS) {
+      long long t = member ? static_cast<long long>(cnt) * y - acc : 0;
+      if (__ballot_sync(0xffffffffu, member) == 0) return;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+      if ((threadIdx.x & 31) == 0 && t) atomicAdd(reinterpret_cast<unsigned long long*>(e.rhs + row), static_cast<unsigned long long>(t));
+    } else {
+      if (member) {
+        ++cnt;
+        acc += y - (e.sub_x ? __ldg(e.sub_x + row) : 0);
+      }
+      if (e.bits) {
+        const unsigned word = __ballot_sync(0xffffffffu, member);
+        if ((threadIdx.x & 31) == 0 && word) e.bits[static_cast<size_t>(row) * e.words + w] = word;
+      }
+    }
   }
+  __device__ __forceinline__ void End(uint32_t s, bool live) {
+    if (RHS || !live || cnt == 0) return;
+    const uint32_t i = s - e.geo.begin;
+    atomicAdd(e.n + i, cnt);
+    atomicAdd(reinterpret_cast<unsigned long long*>(e.sum + i), static_cast<unsigned long long>(acc));
+    cnt = 0;
+    acc = 0;
+  }
+};
+
+template <bool RHS>
+__global__ void __launch_bounds__(kGeoThreads) ExposureWalkKernel(const __grid_constant__ ExposureWalkArgs e) {
+  ExposureVisitor<RHS> v{e};
+  CovisibilityWalk(e.geo, v);
 }
 
 // Keyframe co-visibility, the counts: counts[i][b] += sum_w popc(bits[rows[i]][w] & bits[b][w]).  A CTA owns a 64 x 64 tile of
@@ -1337,6 +1428,20 @@ LaunchResult LaunchCovisibilityBits(const CovisibilityBitsArgs& args, int sm_cou
   }
   const LaunchResult r = PrepareGeo(CovisibilityBitsKernel<false>, &a.geo, sm_count, false, stream, &grid);
   CovisibilityBitsKernel<false><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
+  return r;
+}
+
+LaunchResult LaunchExposureWalk(const ExposureWalkArgs& args, int sm_count, cudaStream_t stream) {
+  if (args.geo.end <= args.geo.begin || args.geo.kf_count <= 0) return {};
+  ExposureWalkArgs a = args;
+  uint32_t grid;
+  if (a.rhs) {
+    const LaunchResult r = PrepareGeo(ExposureWalkKernel<true>, &a.geo, sm_count, false, stream, &grid);
+    ExposureWalkKernel<true><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
+    return r;
+  }
+  const LaunchResult r = PrepareGeo(ExposureWalkKernel<false>, &a.geo, sm_count, false, stream, &grid);
+  ExposureWalkKernel<false><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
   return r;
 }
 
@@ -1493,7 +1598,11 @@ __global__ void __launch_bounds__(256) ExtractLumaKernel(LumaSource first, const
   const LumaSource f = blockIdx.z == 0 ? first : rest[blockIdx.z - 1];
   const uint8_t* src = f.rgba + static_cast<size_t>(y) * f.pitch + static_cast<size_t>(x4) * 4;
   uint8_t* dst = luma + (static_cast<size_t>(blockIdx.z) * h + y) * luma_pitch + x4;
-  if (x4 + 3 < w && (reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
+  if (f.gain != 1.f) {   // exposure compensation (DESIGN §3.21); v / g correctly rounded, as the host and the tests compute it
+    for (int k = 0; k < 4 && x4 + k < w; ++k) dst[k] = static_cast<uint8_t>(fminf(255.f, rintf(__fdiv_rn(src[4 * k + 3], f.gain))));
+    return;
+  }
+  if (x4 + 3 < w &&(reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
     const uint4 v = __ldg(reinterpret_cast<const uint4*>(src));
     const uint32_t packed = (v.x >> 24) | ((v.y >> 24) << 8) | ((v.z >> 24) << 16) | ((v.w >> 24) << 24);
     *reinterpret_cast<uint32_t*>(dst) = packed;

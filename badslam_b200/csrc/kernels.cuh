@@ -285,6 +285,38 @@ struct CovisibilityGramArgs {
 };
 LaunchResult LaunchCovisibilityGram(const CovisibilityGramArgs& a, int sm_count, cudaStream_t stream);
 
+// Keyframe exposure estimation (bba_estimate_keyframe_exposures, DESIGN §3.21): the co-visibility walk over the listed keyframes
+// with one colour texel per associated pair.  An observation (s, row) is an associated pair whose colour pixel lies in the image
+// and whose raw luma v (the .w byte of images[row] at the floor of the colour coordinates) is in [min_luma, max_luma]; its value
+// is y = log_q16[v] = round(2^16 ln v).  Sums are integers, so every launch gives the same bits in any order.
+struct ExposureImage {
+  const uint8_t* rgba;   // uchar4 colour image of the listed keyframe
+  uint32_t pitch;        // bytes
+  uint32_t pad;
+};
+struct ExposureWalkArgs {
+  GeometryArgs geo;               // kfs: every keyframe's record at its current pose; kf_list: the listed keyframes (row = position)
+  const ExposureImage* images;    // [kf_count] by row
+  int log_q16[256];               // (kernel parameters: read through the constant bank)
+  int min_luma, max_luma;
+  // members: every observation (test_n null), or those with |test_n (y - test_x[row]) - test_sum| <= test_n * tau
+  const uint32_t* test_n;         // [end - begin] at s - begin
+  const long long* test_sum;
+  const int* test_x;              // [kf_count] Q16 log gains
+  long long tau;                  // Q16
+  // accumulate (rhs null): n[s - begin] += 1 and sum[s - begin] += y - sub_x[row] (sub_x null: y) over the members; with bits, the
+  // member ballot of every 32-surfel step is word w of row `row`, as in CovisibilityBitsArgs.
+  // rhs: rhs[row] += n[s - begin] * y - sum[s - begin] over the members (n, sum read).
+  uint32_t* n;
+  long long* sum;
+  const int* sub_x;
+  uint32_t* bits;                 // [kf_count][words] or null
+  uint32_t words;
+  long long* rhs;
+};
+// The stream gather and the kernel.  Deleted surfels (x = NaN) are skipped.
+LaunchResult LaunchExposureWalk(const ExposureWalkArgs& a, int sm_count, cudaStream_t stream);
+
 // Multi-GPU surfel sharding: 256-surfel granules are dealt round-robin to the ranks (granule g belongs to rank g % world), so
 // that every rank sees the same mix of well- and poorly-observed surfels (surfels are stored in creation order, and the
 // cost of a surfel is the number of keyframes that see it).  A rank addresses its surfels through a dense local index.
@@ -492,10 +524,12 @@ LaunchResult LaunchFrameSeedCount(const FrameSeedArgs& a, cudaStream_t stream);
 LaunchResult LaunchExactSumDebug(const float* values, uint64_t n, ExactSum* sum, double* out, int sm_count, cudaStream_t stream);
 
 // uchar4 (.w = luma) -> u8 planes, `images` images in one launch: image i (first, or rest[i - 1] in device memory) -> rows
-// [i * h, (i + 1) * h) of luma.  One image reads no table (rest may be null).
+// [i * h, (i + 1) * h) of luma.  One image reads no table (rest may be null).  A gain g != 1 (the keyframe's exposure, DESIGN
+// §3.21) writes min(255, rint(v / g)); g == 1 copies v.
 struct LumaSource {
   const uint8_t* rgba;
   size_t pitch;
+  float gain = 1.f;
 };
 LaunchResult LaunchExtractLuma(LumaSource first, const LumaSource* rest, int images, uint8_t* luma, size_t luma_pitch, int w, int h,
                                cudaStream_t stream);

@@ -765,6 +765,52 @@ class DirectBA:
                                                                 out.ctypes.data, self._stream_ptr(stream)))
         return out
 
+    def _exposure_ids(self, ids):
+        if ids is None:
+            ids = np.arange(self.KeyframeCount(), dtype=np.int32)
+        return np.ascontiguousarray(ids, np.int32).reshape(-1)
+
+    def EstimateKeyframeExposures(self, ids=None, gauge_keyframe: int = -1, min_luma: int = 0, max_luma: int = 0,
+                                  inlier_threshold: float = 0.0, outer_iterations: int = 0, stream=None):
+        """bba_estimate_keyframe_exposures (not in the reference, DESIGN §3.21): (gains float32, observations uint32, inliers
+        uint32), each [len(ids)], the gains relative to the gauge keyframe (NaN outside its component).  ids=None: every keyframe
+        in id order.  Changes nothing on the handle; synchronises the stream."""
+        ids = self._exposure_ids(ids)
+        o = _lib.ExposureOptions(int(gauge_keyframe), int(min_luma), int(max_luma), float(inlier_threshold), int(outer_iterations))
+        n = len(ids)
+        gains = np.zeros(n, np.float32)
+        obs = np.zeros(n, np.uint32)
+        inl = np.zeros(n, np.uint32)
+        self._check(self._lib.bba_estimate_keyframe_exposures(self._h, C.byref(o), n, ids.ctypes.data if n else None,
+                                                              gains.ctypes.data if n else None, obs.ctypes.data if n else None,
+                                                              inl.ctypes.data if n else None, self._stream_ptr(stream)))
+        return gains, obs, inl
+
+    def SetKeyframeExposures(self, gains, ids=None, stream=None):
+        """bba_set_keyframe_exposures: keyframe ids[i] gets gain gains[i] (ids=None: every keyframe in id order) and its luma is
+        re-extracted from its colour image."""
+        ids = self._exposure_ids(ids)
+        g = np.ascontiguousarray(gains, np.float32).reshape(-1)
+        if len(g) != len(ids):
+            raise ValueError("one gain per keyframe id")
+        self._check(self._lib.bba_set_keyframe_exposures(self._h, len(ids), ids.ctypes.data if len(ids) else None,
+                                                         g.ctypes.data if len(g) else None, self._stream_ptr(stream)))
+
+    def GetKeyframeExposures(self, ids=None) -> np.ndarray:
+        """bba_get_keyframe_exposures: the published gains of ids (ids=None: every keyframe), float32."""
+        ids = self._exposure_ids(ids)
+        out = np.zeros(len(ids), np.float32)
+        self._check(self._lib.bba_get_keyframe_exposures(self._h, len(ids), ids.ctypes.data if len(ids) else None,
+                                                         out.ctypes.data if len(ids) else None))
+        return out
+
+    def DebugExposureSystem(self, count: int):
+        """bba_debug_get_exposure_system: (C uint32 [count, count], r int64 [count]) of the last round of the last estimate."""
+        Cm = np.zeros((count, count), np.uint32)
+        r = np.zeros(count, np.int64)
+        self._check(self._lib.bba_debug_get_exposure_system(self._h, int(count), Cm.ctypes.data, r.ctypes.data))
+        return Cm, r
+
     def MeasureFrameOverlap(self, frames, queries, with_shared: bool = True, stream=None) -> FrameOverlap:
         """bba_measure_frame_overlap (not in the reference, DESIGN §3.20): what the surfel map already explains of frames that are
         not keyframes.  frames: a sequence of (depth, normals[, colour]) [h, w] u16 device tensors (colour is not read); queries: a

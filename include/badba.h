@@ -466,8 +466,51 @@ bba_status bba_deform_surfels(bba_handle h, int count, const float* original_key
 bba_status bba_measure_keyframe_covisibility(bba_handle h, int count, const int* keyframe_ids, int keyframe_count, uint32_t* out_counts,
                                              void* stream);
 /* Sets the surfels per chunk of every later bba_measure_keyframe_covisibility (0: the 128 MiB budget rule), so that tests can force
- * many chunks.  The counts are the same bits for every chunk size (of bba_measure_frame_overlap's too).  For tests and timing. */
+ * many chunks.  The counts are the same bits for every chunk size (of bba_measure_frame_overlap's and
+ * bba_estimate_keyframe_exposures' too).  For tests and timing. */
 bba_status bba_debug_set_covisibility_chunk(bba_handle h, uint32_t surfels);
+/* Keyframe exposure compensation (not in the reference; DESIGN.md §3.21).  Every appearance residual reads a keyframe's luma, and
+ * the descriptor residual 180 (I(t) - I(c)) - d cancels a brightness offset but not a gain: a camera with auto-exposure makes
+ * keyframes disagree with the surfel descriptors.  Each keyframe keeps a gain g (default 1); its luma is min(255, rint(v / g)) of
+ * its colour image's .w channel v, and both BA schemes, bba_estimate_frame_pose, the intrinsics step and surfel creation read that
+ * luma.  g = 1 is the uncompensated luma bit for bit.  Not compensated: the odometry pyramids and the luma of the frames of
+ * bba_estimate_frame_poses_for_frames that are not keyframes (they build their own luma from colour).  Surfel descriptors are not
+ * rescaled when a gain changes; the next BA's geometry step re-fits them.  Recipe: estimate -> set -> BA (INTEGRATION.md). */
+typedef struct {
+  int gauge_keyframe;     /* < 0: the first listed keyframe; its gain is 1 */
+  int min_luma, max_luma; /* observations with raw luma in [min_luma, max_luma]; 0 = defaults 8 and 247; 1 <= min <= max <= 255 */
+  float inlier_threshold; /* |log residual| of an observation against its surfel's mean; <= 0: 0.1; at most 16 */
+  int outer_iterations;   /* rounds, the first with every observation an inlier; <= 0: 2; at most 16 */
+} bba_exposure_options;
+/* Estimates the gains of the listed keyframes on the device from the surfels they share (DESIGN.md §3.21).  An observation is a
+ * (surfel, listed keyframe) pair that passes the association test of bba_measure_keyframe_covisibility at the current poses, whose
+ * colour pixel lies in the colour image and whose raw luma v (the .w byte of the keyframe's colour image at the floor of the colour
+ * coordinates) is in [min_luma, max_luma]; its value is round(2^16 ln v).  The model y = log gain(keyframe) + log radiance(surfel),
+ * with the surfel eliminated pairwise, gives a graph Laplacian over the keyframes with integer weights (the inlier observations two
+ * keyframes share) and an integer right-hand side, solved in fp64 on the device with the gauge keyframe's log gain 0.  Later rounds
+ * keep the observations within inlier_threshold of their surfel's mean under the previous round's gains.
+ * gains[count] = exp(log gain) relative to the gauge keyframe (a keyframe brighter than it has a gain above 1); keyframes that share
+ * no chain of inlier surfels with the gauge keyframe get NaN and inliers 0.  observations / inliers (may be NULL) [count]: each
+ * keyframe's observations and inlier observations of the last round.  The same inputs give the same bits on every run, in any
+ * surfel order or chunking, in the deterministic mode or not, and on every rank (with world_size > 1 every rank walks its whole
+ * replica; no exchange).
+ * BBA_ERR_INVALID_ARGUMENT: a NULL options, keyframe_ids or gains, count <= 0, an unknown or repeated id, a gauge keyframe that is
+ * not listed, bad options.  BBA_ERR_STATE: a listed keyframe's colour was last updated through the shared staging image
+ * (bba_update_keyframe_host with colour on a keyframe whose colour buffer is caller-owned), so no colour image is left to read.
+ * Arguments are checked before anything is enqueued.  A BA-side call: it changes nothing on the handle (it may rebuild a stale
+ * spatial order of the surfels) and synchronises the stream once. */
+bba_status bba_estimate_keyframe_exposures(bba_handle h, const bba_exposure_options* options, int count, const int* keyframe_ids,
+                                           float* gains, uint32_t* observations, uint32_t* inliers, void* stream);
+/* Sets the gains of keyframes keyframe_ids [count] and re-extracts their luma from their colour images, then publishes the gains.
+ * BBA_ERR_INVALID_ARGUMENT: count < 0, a NULL array with count > 0, an unknown or repeated id, a gain that is not finite and > 0.
+ * BBA_ERR_STATE: a keyframe whose colour was last updated through the staging image (see above).  Checked before anything changes.
+ * bba_update_keyframe_host re-applies the stored gain to new colour.  A BA-side call. */
+bba_status bba_set_keyframe_exposures(bba_handle h, int count, const int* keyframe_ids, const float* gains, void* stream);
+/* The published gains of keyframes keyframe_ids [count] (1 unless set).  BBA_ERR_INVALID_ARGUMENT: an unknown id.  Front end. */
+bba_status bba_get_keyframe_exposures(bba_handle h, int count, const int* keyframe_ids, float* gains);
+/* The Laplacian's inputs of the last round of the last bba_estimate_keyframe_exposures: C [count][count] (the inlier observations
+ * each pair of listed keyframes shares, by list position) and r [count] (Q16).  count must be that call's.  For tests. */
+bba_status bba_debug_get_exposure_system(bba_handle h, int count, uint32_t* C, int64_t* r);
 /* One query of bba_measure_frame_overlap: a frame at a pose. */
 typedef struct {
   int frame;                   /* index into frames */

@@ -300,6 +300,33 @@ class DirectBA {
           "bba_measure_keyframe_covisibility");
   }
 
+  // bba_estimate_keyframe_exposures (not in the reference): the gains of keyframes ids relative to the gauge keyframe (an empty
+  // ids: every keyframe in id order), and optionally each one's observations and inliers.  A BA-side call that changes nothing;
+  // synchronises the stream.
+  void EstimateKeyframeExposures(cudaStream_t stream, const bba_exposure_options& options, const std::vector<int>& ids,
+                                 std::vector<float>* gains, std::vector<uint32_t>* observations = nullptr,
+                                 std::vector<uint32_t>* inliers = nullptr) {
+    const std::vector<int> list = ids.empty() ? AllKeyframeIds() : ids;
+    gains->assign(list.size(), 0.f);
+    if (observations) observations->assign(list.size(), 0u);
+    if (inliers) inliers->assign(list.size(), 0u);
+    Check(bba_estimate_keyframe_exposures(h_, &options, static_cast<int>(list.size()), list.data(), gains->data(),
+                                          observations ? observations->data() : nullptr, inliers ? inliers->data() : nullptr, stream),
+          "bba_estimate_keyframe_exposures");
+  }
+  // bba_set_keyframe_exposures: keyframe ids[i] gets gains[i] (an empty ids: every keyframe in id order); its luma is re-extracted.
+  void SetKeyframeExposures(cudaStream_t stream, const std::vector<int>& ids, const std::vector<float>& gains) {
+    const std::vector<int> list = ids.empty() ? AllKeyframeIds() : ids;
+    if (gains.size() != list.size()) throw std::invalid_argument("SetKeyframeExposures: one gain per keyframe id");
+    Check(bba_set_keyframe_exposures(h_, static_cast<int>(list.size()), list.data(), gains.data(), stream), "bba_set_keyframe_exposures");
+  }
+  // bba_get_keyframe_exposures: the published gains (an empty ids: every keyframe).  Front end.
+  void GetKeyframeExposures(const std::vector<int>& ids, std::vector<float>* gains) const {
+    const std::vector<int> list = ids.empty() ? AllKeyframeIds() : ids;
+    gains->assign(list.size(), 1.f);
+    Check(bba_get_keyframe_exposures(h_, static_cast<int>(list.size()), list.data(), gains->data()), "bba_get_keyframe_exposures");
+  }
+
   // bba_measure_frame_overlap (not in the reference): per query, what the surfel map already explains of a frame that is not a
   // keyframe (*out, one record per query) and, with a non-null shared, the surfels it shares with every keyframe ([queries][K]).
   // A BA-side call; synchronises the stream.
@@ -556,6 +583,11 @@ class DirectBA {
  private:
   void Check(bba_status s, const char* where) const {
     if (s != BBA_OK) throw Error(s, std::string(where) + ": " + (h_ ? bba_last_error(h_) : "no handle"));
+  }
+  std::vector<int> AllKeyframeIds() const {
+    std::vector<int> ids(static_cast<size_t>(std::max(0, bba_keyframe_count(h_))));
+    for (size_t i = 0; i < ids.size(); ++i) ids[i] = static_cast<int>(i);
+    return ids;
   }
   // The odometry options of the TrackFramePairwise forms: the reference's 30 iterations per scale.
   static bba_odometry_options MakeOdometryOptions(int num_scales, bool use_pyramid_level_0, bool use_gradmag,

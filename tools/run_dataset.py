@@ -44,6 +44,11 @@ DirectBA.MeasureFrameOverlap, bba_measure_frame_overlap, at its tracked pose), o
 the last keyframe, up to --max-keyframes.  A slow camera then adds fewer keyframes and a fast one more.  The JSON line gives the
 keyframe count either way.
 
+With --exposure-compensation the gains of every keyframe are estimated from the surfels they share and set before every
+BundleAdjustment call (DirectBA.EstimateKeyframeExposures / SetKeyframeExposures, DESIGN §3.21), so that an auto-exposure camera's
+brightness changes do not bias the descriptor residuals; a keyframe that shares nothing with keyframe 0 keeps its gain.  The JSON
+line gives the smallest and largest gain set ("exposure_gain_min_max").
+
 The views of --make-synthetic lie metres apart (a BA test scene, not a video), so odometry between them fails and only the
 keyframe poses of that sequence are meaningful; on a recorded sequence every frame is tracked from its neighbour.
 """
@@ -98,6 +103,8 @@ def main():
                     help="anchor every keyframe to its trajectory pose with a soft prior of these sigmas (metres, radians)")
     ap.add_argument("--attitude-prior-sigma", metavar="RAD", type=float, default=None,
                     help="give every keyframe an attitude prior from its trajectory pose with this sigma (radians)")
+    ap.add_argument("--exposure-compensation", action="store_true",
+                    help="estimate and set every keyframe's exposure gain before every BundleAdjustment call")
     a = ap.parse_args()
     if a.refine_frames and a.export_poses is None:
         ap.error("--refine-frames needs --export-poses")
@@ -169,11 +176,17 @@ def run(a, prior_sigma, attitude_sigma):
     kept = {}   # --refine-frames: frame index -> its preprocessed (depth, normals, rgba)
     n = -1   # keyframes added so far - 1
     last_ba = -1   # n at the last BundleAdjustment
+    gain_range = [np.inf, -np.inf]   # --exposure-compensation: the smallest and largest gain set
 
     def bundle_adjust(i):
         nonlocal t_ba, last_ba
         original = ba.RememberKeyframePoses() if export else None
         t = time.perf_counter()
+        if a.exposure_compensation:
+            gains = ba.EstimateKeyframeExposures()[0]
+            gains = np.where(np.isnan(gains), ba.GetKeyframeExposures(), gains).astype(np.float32)
+            ba.SetKeyframeExposures(gains)
+            gain_range[0], gain_range[1] = min(gain_range[0], float(gains.min())), max(gain_range[1], float(gains.max()))
         r = ba.BundleAdjustment(None, False, False, True, True, True, 1, a.ba_iterations)
         torch.cuda.synchronize()
         t_ba += time.perf_counter() - t
@@ -252,6 +265,8 @@ def run(a, prior_sigma, attitude_sigma):
     line["max_abs_keyframe_error_m_rad"] = [max(e[0] for e in abs_err), max(e[1] for e in abs_err)]
     tilts = [np.arccos(np.clip(tilt(poses[k], S) @ tilt(true_poses[k], S), -1.0, 1.0)) for k in range(len(idx))]
     line["mean_tilt_error_rad"] = float(np.mean(tilts))
+    if a.exposure_compensation:
+        line["exposure_gain_min_max"] = gain_range if np.isfinite(gain_range[0]) else None
     if prior_sigma is not None:
         line["pose_prior_sigma_m_rad"] = prior_sigma
     if attitude_sigma is not None:
