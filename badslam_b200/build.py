@@ -33,6 +33,7 @@ UNITS = [
     ("pose_step.cu", []),
     ("pose_terms.cu", []),
     ("bundle_adjust.cu", []),
+    ("covisibility.cu", []),
     ("multi_gpu.cu", []),
     ("local_group.cu", ["-Xptxas", "-v"]),   # (the all-reduce sums keep denormals: no -use_fast_math)
     ("frames.cu", []),

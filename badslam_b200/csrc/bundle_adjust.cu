@@ -42,6 +42,22 @@ bba_status MakeAllKeyframeList(bba_handle h) {
   return BBA_OK;
 }
 
+bba_status SetGeometryFields(bba_handle h, bool sort, const KfDevice* kfs, const int* list, int count, GeometryArgs* g) {
+  SetSurfelFields(h, g);
+  g->perm = sort && h->surfels_size > 0 ? h->pose.order.view.perm : nullptr;
+  g->stream = h->pose.order.stream;
+  g->stream_pitch = h->pose.order.capacity;
+  g->active = h->active;
+  g->kfs = kfs;
+  g->kf_list = list;
+  g->kf_count = count;
+  g->queue = h->geo.d_queue;
+  g->tile_shift = 8;
+  if (bba_status st = ReserveTileEpochs(h)) return st;
+  g->tile_epoch = h->geo.d_tile_epoch;
+  return BBA_OK;
+}
+
 namespace {
 
 // In which order the geometry launches visit the surfels.  kCaller: the caller's (the in-loop creation's two launches address the
@@ -66,21 +82,10 @@ bba_status BuildGeometryArgs(bba_handle h, bba::GeometryArgs* g, cudaStream_t s,
                                         static_cast<uint64_t>(h->surfels_size) * static_cast<uint64_t>(cnt) >= kSpatialOrderMinPairs));
   if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/h->cfg.world_size > 1, s)) return st;
   if (bba_status st = PeerFence(h, s)) return st;
-  SetSurfelFields(h, g);
+  if (bba_status st = SetGeometryFields(h, sort, h->d_kfs, h->geo.d_list, cnt, g)) return st;
   SetShardFields(h, g);
-  g->perm = sort && h->surfels_size > 0 ? h->pose.order.view.perm : nullptr;
-  g->stream = h->pose.order.stream;
-  g->stream_pitch = h->pose.order.capacity;
-  h->geo.perm = g->perm;
-  g->active = h->active;
-  g->kfs = h->d_kfs;
-  g->kf_list = h->geo.d_list;
-  g->kf_count = cnt;
-  g->queue = h->geo.d_queue;
-  g->tile_shift = 8;
   g->peers = KernelPeers(h);
-  if (bba_status st = ReserveTileEpochs(h)) return st;
-  g->tile_epoch = h->geo.d_tile_epoch;
+  h->geo.perm = g->perm;
   return BBA_OK;
 }
 
@@ -186,12 +191,28 @@ bba_status OptimizeIntrinsics(bba_handle h, bool opt_depth, bool opt_color, cuda
   return Publish(h, s, opt_depth);   // cameras, a and (depth) the cfactor together
 }
 
+}  // namespace
+
 // ---- in-loop surfel lifecycle ---------------------------------------------------------------------------------------------
 // direct_ba.h:220-226, for a handle with K keyframes
 int MinObservationCount(bba_handle h, size_t K) {
   return (K < 10) ? ((K < 5) ? h->cfg.min_observation_count_while_bootstrapping_1 : h->cfg.min_observation_count_while_bootstrapping_2)
                   : h->cfg.min_observation_count;
 }
+
+CovisEntry MakeCovisEntry(const Keyframe& other, const Pose& global_T_frame) {
+  CovisEntry e;
+  ToMatrix3x4(Compose(Inverse(other.pose), global_T_frame), e.R);
+  e.depth = other.depth;
+  e.normals = other.normals;
+  e.depth_pitch = static_cast<uint32_t>(other.depth_pitch);
+  e.normals_pitch = static_cast<uint32_t>(other.normals_pitch);
+  e.pad[0] = e.pad[1] = 0;
+  return e;
+}
+
+namespace {
+
 int GetMinObservationCount(bba_handle h) { return MinObservationCount(h, h->keyframes.size()); }
 
 uint32_t SurfelCapacity(bba_handle h) {
@@ -264,16 +285,7 @@ bba_status CreateSurfelsForKeyframe(bba_handle h, int k, bool filter, cudaStream
   BBA_TRACE("create: args made");
   if (filter) {   // covis_T_frame for every co-visible keyframe (direct_ba.cc:365-370)
     int cnt = 0;
-    for (int c : kf.covis) {
-      const Keyframe& other = h->keyframes[c];
-      bba::CovisEntry& e = h->life.h_covis[cnt++];
-      bba::ToMatrix3x4(bba::Compose(bba::Inverse(other.pose), kf.pose), e.R);
-      e.depth = other.depth;
-      e.normals = other.normals;
-      e.depth_pitch = static_cast<uint32_t>(other.depth_pitch);
-      e.normals_pitch = static_cast<uint32_t>(other.normals_pitch);
-      e.pad[0] = e.pad[1] = 0;
-    }
+    for (int c : kf.covis) h->life.h_covis[cnt++] = MakeCovisEntry(h->keyframes[c], kf.pose);
     a.covis_count = cnt;
     if (cnt) BBA_CUDA(h, cudaMemcpyAsync(h->life.d_covis, h->life.h_covis, sizeof(bba::CovisEntry) * cnt, cudaMemcpyHostToDevice, s));
   }
@@ -857,301 +869,12 @@ bba_status DeformSurfels(bba_handle h, int count, const float* original, uint32_
   return BBA_OK;
 }
 
-// bba_measure_keyframe_covisibility.  Every argument is checked before anything is enqueued; nothing on the handle changes but the
-// spatial order, which is rebuilt when stale (a function of the positions alone).
-bba_status MeasureKeyframeCovisibility(bba_handle h, int count, const int* ids, int keyframe_count, uint32_t* out, cudaStream_t s) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_measure_keyframe_covisibility: ";
-  const int K = static_cast<int>(h->keyframes.size());
-  if (!out) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null out_counts");
-  if (count == 0 || count < -1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "bad count");
-  if (count > 0 && !ids) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null keyframe_ids");
-  if (keyframe_count != K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "keyframe_count is not the handle's keyframe count");
-  for (int i = 0; i < count; ++i)
-    if (ids[i] < 0 || ids[i] >= K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "unknown keyframe id");
-  const int rows = count < 0 ? K : count;
-  const uint32_t n = h->surfels_size;
-  if (K == 0 || n == 0) {
-    std::fill(out, out + static_cast<size_t>(rows) * K, 0u);
-    return BBA_OK;
-  }
-  if (bba_status st = CheckSurfels(h)) return st;
-  auto& c = h->covis;
-  uint32_t chunk = c.chunk;
-  if (chunk == 0) {   // whole 256-surfel geometry tiles
-    const uint64_t fit = kCovisibilityBitsBudget * 8 / static_cast<uint64_t>(K);
-    chunk = static_cast<uint32_t>(std::max<uint64_t>(256, std::min<uint64_t>(fit, 0xffffff00ull) / 256 * 256));
-  }
-  chunk = std::min(chunk, n);
-  const uint32_t words = (chunk + 31u) / 32u;
-  BBA_CUDA(h, c.d_bits.Reserve(static_cast<size_t>(K) * words));
-  BBA_CUDA(h, c.d_counts.Reserve(static_cast<size_t>(rows) * K));
-  if (count > 0) BBA_CUDA(h, c.d_rows.Reserve(count));
-  if (bba_status st = MakeAllKeyframeList(h)) return st;
-  if (bba_status st = UploadKeyframes(h, s)) return st;   // the current poses
-  if (count > 0) BBA_CUDA(h, cudaMemcpyAsync(c.d_rows, ids, sizeof(int) * count, cudaMemcpyHostToDevice, s));
-  BBA_CUDA(h, cudaMemsetAsync(c.d_counts, 0, sizeof(uint32_t) * rows * K, s));
-  // Every rank measures its whole replica (begin 0, end n, one shard), in the spatial order unless the geometry launches keep the
-  // caller's (peer stores): the counts do not depend on the order.
-  const bool sort = !PeerStores(h);
-  if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/false, s)) return st;
-  bba::CovisibilityBitsArgs a;
-  bba::GeometryArgs& g = a.geo;
-  SetSurfelFields(h, &g);
-  g.shard_rank = 0;
-  g.shard_world = 1;
-  g.perm = sort ? h->pose.order.view.perm : nullptr;
-  g.stream = h->pose.order.stream;
-  g.stream_pitch = h->pose.order.capacity;
-  g.active = h->active;
-  g.kfs = h->d_kfs;
-  g.kf_list = h->geo.d_all_list;
-  g.kf_count = K;
-  g.queue = h->geo.d_queue;
-  g.peers = PeerSet{};
-  if (bba_status st = ReserveTileEpochs(h)) return st;
-  g.tile_epoch = h->geo.d_tile_epoch;
-  a.bits = c.d_bits;
-  const bba::CovisibilityGramArgs q{c.d_bits, 0, count > 0 ? c.d_rows.get() : h->geo.d_all_list.get(), rows, K, c.d_counts};
-  for (uint32_t begin = 0; begin < n; begin += chunk) {
-    g.begin = begin;
-    g.end = begin + std::min(chunk, n - begin);
-    g.tile_shift = 8;
-    a.words = (g.end - g.begin + 31u) / 32u;
-    BBA_CUDA(h, cudaMemsetAsync(c.d_bits, 0, sizeof(uint32_t) * K * a.words, s));
-    BBA_LAUNCH(h, h->launches, LaunchCovisibilityBits, a, h->sm_count, s);
-    bba::CovisibilityGramArgs qc = q;
-    qc.words = a.words;
-    BBA_LAUNCH(h, h->launches, LaunchCovisibilityGram, qc, h->sm_count, s);
-  }
-  BBA_CUDA(h, cudaMemcpyAsync(out, c.d_counts, sizeof(uint32_t) * rows * K, cudaMemcpyDeviceToHost, s));
-  BBA_CUDA(h, cudaStreamSynchronize(s));
-  return BBA_OK;
-}
-
-
-// A frame of bba_measure_frame_overlap as the kernels read it: u16 depth and normals rows of the depth width, 2-byte aligned.
-bool OverlapFrameOk(bba_handle h, const bba_frame_buffers& f) {
-  const size_t row = static_cast<size_t>(h->cfg.depth_width) * 2;
-  return f.depth && f.normals && f.depth_pitch >= row && f.normals_pitch >= row && f.depth_pitch <= 0xffffffffull &&
-         f.normals_pitch <= 0xffffffffull && !(f.depth_pitch & 1u) && !(f.normals_pitch & 1u) &&
-         !(reinterpret_cast<uintptr_t>(f.depth) & 1u) && !(reinterpret_cast<uintptr_t>(f.normals) & 1u);
-}
-
-// bba_measure_frame_overlap (DESIGN §3.20).  Every argument is checked before anything is enqueued; nothing on the handle changes
-// but the spatial order, which is rebuilt when stale.  The frames' records get rows after the keyframes' in the covisibility bit
-// rows (rows K .. K + n - 1, or 0 .. n - 1 without the keyframes' side), so that the keyframe Gram gives shared and, on its
-// diagonal, observed_surfels; the frames' cell rows then feed the seed count.
-bba_status MeasureFrameOverlap(bba_handle h, int frame_count, const bba_frame_buffers* frames, int count, const bba_frame_overlap_query* queries,
-                               int keyframe_count, uint32_t* shared, bba_frame_overlap* out, cudaStream_t s) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  const std::string fn = "bba_measure_frame_overlap: ";
-  const int K = static_cast<int>(h->keyframes.size());
-  if (!frames || !queries || !out) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null argument");
-  if (count < 1 || frame_count < 1) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "count and frame_count must be at least 1");
-  if (keyframe_count != K) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "keyframe_count is not the handle's keyframe count");
-  for (int f = 0; f < frame_count; ++f)
-    if (!OverlapFrameOk(h, frames[f])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "null, misaligned or too narrow frame image");
-  for (int i = 0; i < count; ++i) {
-    const bba_frame_overlap_query& q = queries[i];
-    const std::string which = " in query " + std::to_string(i);
-    if (q.frame < 0 || q.frame >= frame_count) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "frame index out of range" + which);
-    for (int j = 0; j < 7; ++j)
-      if (!std::isfinite(q.global_T_frame[j])) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "non-finite pose" + which);
-    const float* p = q.global_T_frame;
-    if (p[0] * p[0] + p[1] * p[1] + p[2] * p[2] + p[3] * p[3] < 1e-12f) return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "zero quaternion" + which);
-    if (!(q.min_depth > 0.f && q.min_depth <= q.max_depth && std::isfinite(q.max_depth)))
-      return Fail(h, BBA_ERR_INVALID_ARGUMENT, fn + "depth range must be 0 < min_depth <= max_depth" + which);
-  }
-  const uint32_t n_surfels = h->surfels_size;
-  if (n_surfels > 0)
-    if (bba_status st = CheckSurfels(h)) return st;
-
-  const int n = count;
-  const bool with_kfs = shared && K > 0;           // the keyframes' bit rows and the full Gram
-  const int kf_rows = with_kfs ? K : 0;
-  const int cols = kf_rows + n;
-  const uint32_t cells = static_cast<uint32_t>(h->cf_w) * h->cf_h;
-  const uint32_t cell_words = (cells + 31u) / 32u;
-  auto& o = h->overlap;
-  // the frusta of the keyframes and queries (AddKeyframeCommon's) and the CSR of the queries' co-visible keyframes
-  std::vector<Frustum> kf_frusta(K);
-  for (int k = 0; k < K; ++k) {
-    const Keyframe& kf = h->keyframes[k];
-    MakeFrustum(&kf_frusta[k], h->depth_K, h->cfg.depth_width, h->cfg.depth_height, kf.min_depth, kf.max_depth, kf.pose);
-  }
-  std::vector<std::vector<int>> covis(n);
-  size_t covis_total = 0;
-  for (int i = 0; i < n; ++i) {
-    Frustum fq;
-    MakeFrustum(&fq, h->depth_K, h->cfg.depth_width, h->cfg.depth_height, queries[i].min_depth, queries[i].max_depth,
-                PoseFromArray(queries[i].global_T_frame));
-    for (int k = 0; k < K; ++k)
-      if (FrustaIntersect(fq, kf_frusta[k])) covis[i].push_back(k);
-    covis_total += covis[i].size();
-  }
-  const size_t ints = 2 * static_cast<size_t>(n) + n + 1;   // [frame list 0 .. n-1 | Gram rows | covis offsets]
-  const size_t count_words = 3 * static_cast<size_t>(n) + static_cast<size_t>(n) * cols;   // [n][3] seed counts, then [n][cols]
-  BBA_CUDA(h, o.d_frames.Reserve(n));
-  BBA_CUDA(h, o.h_frames.Reserve(n));
-  BBA_CUDA(h, o.d_ints.Reserve(ints));
-  BBA_CUDA(h, o.h_ints.Reserve(ints));
-  BBA_CUDA(h, o.d_covis.Reserve(std::max<size_t>(covis_total, 1)));
-  BBA_CUDA(h, o.h_covis.Reserve(std::max<size_t>(covis_total, 1)));
-  BBA_CUDA(h, o.d_cells.Reserve(static_cast<size_t>(n) * cell_words));
-  BBA_CUDA(h, o.d_counts.Reserve(count_words));
-  BBA_CUDA(h, o.h_counts.Reserve(count_words));
-  uint32_t chunk = 0, words = 0;
-  if (n_surfels > 0) {
-    chunk = h->covis.chunk;
-    if (chunk == 0) {   // whole 256-surfel geometry tiles; the budget counts every row held
-      const uint64_t fit = kCovisibilityBitsBudget * 8 / static_cast<uint64_t>(cols);
-      chunk = static_cast<uint32_t>(std::max<uint64_t>(256, std::min<uint64_t>(fit, 0xffffff00ull) / 256 * 256));
-    }
-    chunk = std::min(chunk, n_surfels);
-    words = (chunk + 31u) / 32u;
-    BBA_CUDA(h, h->covis.d_bits.Reserve(static_cast<size_t>(cols) * words));
-  }
-
-  // staging: the frame records (UploadKeyframes' records at the query poses), the int lists and the co-visible keyframes
-  int* list = o.h_ints;
-  int* rows = list + n;
-  int* offsets = rows + n;
-  size_t e = 0;
-  for (int i = 0; i < n; ++i) {
-    const bba_frame_overlap_query& q = queries[i];
-    const bba_frame_buffers& f = frames[q.frame];
-    const Pose pose = PoseFromArray(q.global_T_frame);
-    KfDevice& d = o.h_frames[i];
-    std::memset(&d, 0, sizeof(d));
-    ToMatrix3x4(Inverse(pose), d.T);
-    d.depth = f.depth;
-    d.normals = f.normals;
-    d.depth_pitch = static_cast<uint32_t>(f.depth_pitch);
-    d.normals_pitch = static_cast<uint32_t>(f.normals_pitch);
-    list[i] = i;
-    rows[i] = kf_rows + i;
-    offsets[i] = static_cast<int>(e);
-    for (int k : covis[i]) {   // covis_T_frame (CreateSurfelsForKeyframe's entries)
-      const Keyframe& other = h->keyframes[k];
-      CovisEntry& c = o.h_covis[e++];
-      ToMatrix3x4(Compose(Inverse(other.pose), pose), c.R);
-      c.depth = other.depth;
-      c.normals = other.normals;
-      c.depth_pitch = static_cast<uint32_t>(other.depth_pitch);
-      c.normals_pitch = static_cast<uint32_t>(other.normals_pitch);
-      c.pad[0] = c.pad[1] = 0;
-    }
-  }
-  offsets[n] = static_cast<int>(e);
-  BBA_CUDA(h, cudaMemcpyAsync(o.d_frames, o.h_frames, sizeof(KfDevice) * n, cudaMemcpyHostToDevice, s));
-  BBA_CUDA(h, cudaMemcpyAsync(o.d_ints, o.h_ints, sizeof(int) * ints, cudaMemcpyHostToDevice, s));
-  if (e) BBA_CUDA(h, cudaMemcpyAsync(o.d_covis, o.h_covis, sizeof(CovisEntry) * e, cudaMemcpyHostToDevice, s));
-  BBA_CUDA(h, cudaMemsetAsync(o.d_cells, 0, sizeof(uint32_t) * n * cell_words, s));
-  BBA_CUDA(h, cudaMemsetAsync(o.d_counts, 0, sizeof(uint32_t) * count_words, s));
-
-  // the walk: per chunk, the keyframes' bit rows (with shared), the frames' bit rows and cell rows, and the Gram
-  if (n_surfels > 0) {
-    if (bba_status st = MakeAllKeyframeList(h)) return st;
-    if (with_kfs)
-      if (bba_status st = UploadKeyframes(h, s)) return st;   // the current poses
-    const bool sort = !PeerStores(h);   // (the order does not change the counts; MeasureKeyframeCovisibility's rule)
-    if (bba_status st = EnsureSpatialOrder(h, sort, /*rebuild=*/false, s)) return st;
-    if (bba_status st = ReserveTileEpochs(h)) return st;
-    CovisibilityBitsArgs kb;
-    GeometryArgs& g = kb.geo;
-    SetSurfelFields(h, &g);
-    g.shard_rank = 0;
-    g.shard_world = 1;
-    g.perm = sort ? h->pose.order.view.perm : nullptr;
-    g.stream = h->pose.order.stream;
-    g.stream_pitch = h->pose.order.capacity;
-    g.active = h->active;
-    g.kfs = h->d_kfs;
-    g.kf_list = h->geo.d_all_list;
-    g.kf_count = K;
-    g.queue = h->geo.d_queue;
-    g.peers = PeerSet{};
-    g.tile_epoch = h->geo.d_tile_epoch;
-    kb.bits = h->covis.d_bits;
-    kb.cells = nullptr;
-    kb.cell_words = 0;
-    CovisibilityBitsArgs fb = kb;
-    fb.geo.kfs = o.d_frames;
-    fb.geo.kf_list = o.d_ints;
-    fb.geo.kf_count = n;
-    fb.cells = o.d_cells;
-    fb.cell_words = cell_words;
-    CovisibilityGramArgs q{h->covis.d_bits, 0, o.d_ints.get() + n, n, cols, o.d_counts.get() + 3 * static_cast<size_t>(n)};
-    for (uint32_t begin = 0; begin < n_surfels; begin += chunk) {
-      const uint32_t end = begin + std::min(chunk, n_surfels - begin);
-      const uint32_t w = (end - begin + 31u) / 32u;
-      BBA_CUDA(h, cudaMemsetAsync(h->covis.d_bits, 0, sizeof(uint32_t) * cols * w, s));
-      for (CovisibilityBitsArgs* a : {&kb, &fb}) {
-        a->geo.begin = begin;
-        a->geo.end = end;
-        a->geo.tile_shift = 8;
-        a->words = w;
-      }
-      fb.bits = h->covis.d_bits.get() + static_cast<size_t>(kf_rows) * w;
-      if (with_kfs) BBA_LAUNCH(h, h->launches, LaunchCovisibilityBits, kb, h->sm_count, s);
-      BBA_LAUNCH(h, h->launches, LaunchCovisibilityBits, fb, h->sm_count, s);
-      q.words = w;
-      BBA_LAUNCH(h, h->launches, LaunchCovisibilityGram, q, h->sm_count, s);
-    }
-  }
-
-  // the seed count, with the minimum observation count of the handle with the frame added
-  FrameSeedArgs sa;
-  sa.cam = MakeCamera(h);
-  sa.frames = o.d_frames;
-  sa.frame_count = n;
-  sa.cells = cells;
-  sa.covered = o.d_cells;
-  sa.cell_words = cell_words;
-  sa.covis = o.d_covis;
-  sa.covis_offsets = o.d_ints.get() + 2 * static_cast<size_t>(n);
-  sa.min_observation_count = MinObservationCount(h, h->keyframes.size() + 1);
-  sa.counts = o.d_counts;
-  BBA_LAUNCH(h, h->launches, LaunchFrameSeedCount, sa, s);
-  BBA_CUDA(h, cudaMemcpyAsync(o.h_counts, o.d_counts, sizeof(uint32_t) * count_words, cudaMemcpyDeviceToHost, s));
-  BBA_CUDA(h, cudaStreamSynchronize(s));
-  const uint32_t* seeds = o.h_counts;
-  const uint32_t* gram = seeds + 3 * static_cast<size_t>(n);
-  for (int i = 0; i < n; ++i) {
-    const uint32_t* row = gram + static_cast<size_t>(i) * cols;
-    out[i].observed_surfels = row[kf_rows + i];
-    out[i].valid_cells = seeds[3 * i];
-    out[i].uncovered_cells = seeds[3 * i + 1];
-    out[i].new_surfels = seeds[3 * i + 2];
-    if (with_kfs) std::copy(row, row + K, shared + static_cast<size_t>(i) * K);
-  }
-  return BBA_OK;
-}
-
 }  // namespace
 }  // namespace bba
 
 using namespace bba;
 
 extern "C" {
-
-bba_status bba_measure_keyframe_covisibility(bba_handle h, int count, const int* keyframe_ids, int keyframe_count, uint32_t* out_counts,
-                                             void* stream) {
-  return MeasureKeyframeCovisibility(h, count, keyframe_ids, keyframe_count, out_counts, static_cast<cudaStream_t>(stream));
-}
-
-bba_status bba_measure_frame_overlap(bba_handle h, int frame_count, const bba_frame_buffers* frames, int count,
-                                     const bba_frame_overlap_query* queries, int keyframe_count, uint32_t* shared,
-                                     bba_frame_overlap* out, void* stream) {
-  return MeasureFrameOverlap(h, frame_count, frames, count, queries, keyframe_count, shared, out, static_cast<cudaStream_t>(stream));
-}
-
-bba_status bba_debug_set_covisibility_chunk(bba_handle h, uint32_t surfels) {
-  if (!h) return BBA_ERR_INVALID_ARGUMENT;
-  h->covis.chunk = surfels;
-  return BBA_OK;
-}
 
 bba_status bba_update_surfel_activation(bba_handle h, void* stream) {
   return GeometryPass(h, /*activation=*/true, static_cast<cudaStream_t>(stream));

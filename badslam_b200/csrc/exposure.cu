@@ -229,15 +229,10 @@ bba_status EstimateKeyframeExposures(bba_handle h, const bba_exposure_options* o
   if (n > 0)
     if (bba_status st2 = CheckSurfels(h)) return st2;
   auto& e = h->exposure;
-  uint32_t chunk = h->covis.chunk;
-  if (chunk == 0) {   // whole 256-surfel geometry tiles, the co-visibility rule over the listed rows
-    const uint64_t fit = kCovisibilityBitsBudget * 8 / static_cast<uint64_t>(count);
-    chunk = static_cast<uint32_t>(std::max<uint64_t>(256, std::min<uint64_t>(fit, 0xffffff00ull) / 256 * 256));
-  }
-  chunk = std::max<uint32_t>(1, std::min(chunk, n));
-  const uint32_t words = (chunk + 31u) / 32u;
   const size_t N = static_cast<size_t>(count);
-  BBA_CUDA(h, h->covis.d_bits.Reserve(N * words));
+  ReplicaWalk walk;   // (the co-visibility chunk rule over the listed rows)
+  if (bba_status st2 = ReserveReplicaWalk(h, N, &walk)) return st2;
+  const uint32_t chunk = walk.chunk;
   BBA_CUDA(h, e.d_ids.Reserve(N));
   BBA_CUDA(h, e.d_images.Reserve(N));
   BBA_CUDA(h, e.d_n.Reserve(chunk));
@@ -252,7 +247,6 @@ bba_status EstimateKeyframeExposures(bba_handle h, const bba_exposure_options* o
   BBA_CUDA(h, e.d_csr.Reserve(2 * N + 2 + N * N));
   BBA_CUDA(h, e.d_work.Reserve(7 * N));
   BBA_CUDA(h, e.d_diag.Reserve(2 * N));
-  if (bba_status st2 = MakeAllKeyframeList(h)) return st2;
   if (bba_status st2 = UploadKeyframes(h, s)) return st2;   // the current poses
   std::vector<ExposureImage> images(count);
   for (int i = 0; i < count; ++i) {
@@ -261,29 +255,7 @@ bba_status EstimateKeyframeExposures(bba_handle h, const bba_exposure_options* o
   }
   BBA_CUDA(h, cudaMemcpyAsync(e.d_ids, ids, sizeof(int) * N, cudaMemcpyHostToDevice, s));
   BBA_CUDA(h, cudaMemcpyAsync(e.d_images, images.data(), sizeof(ExposureImage) * N, cudaMemcpyHostToDevice, s));
-  // Every rank walks its whole replica (begin 0, end n, one shard), in the spatial order unless the geometry launches keep the
-  // caller's (peer stores): the sums are integers, so the result does not depend on the order.
-  const bool sort = !PeerStores(h);
-  if (n > 0) {
-    if (bba_status st2 = EnsureSpatialOrder(h, sort, /*rebuild=*/false, s)) return st2;
-    if (bba_status st2 = ReserveTileEpochs(h)) return st2;
-  }
   ExposureWalkArgs w{};
-  GeometryArgs& g = w.geo;
-  SetSurfelFields(h, &g);
-  g.shard_rank = 0;
-  g.shard_world = 1;
-  g.perm = sort && n > 0 ? h->pose.order.view.perm : nullptr;
-  g.stream = h->pose.order.stream;
-  g.stream_pitch = h->pose.order.capacity;
-  g.active = h->active;
-  g.kfs = h->d_kfs;
-  g.kf_list = e.d_ids;
-  g.kf_count = count;
-  g.queue = h->geo.d_queue;
-  g.peers = PeerSet{};
-  g.tile_epoch = h->geo.d_tile_epoch;
-  g.tile_shift = 8;
   w.images = e.d_images;
   std::copy(LogQ16Table(), LogQ16Table() + 256, w.log_q16);
   w.min_luma = min_luma;
@@ -296,46 +268,47 @@ bba_status EstimateKeyframeExposures(bba_handle h, const bba_exposure_options* o
   for (int k = 1; k <= rounds; ++k) {
     BBA_CUDA(h, cudaMemsetAsync(e.d_C, 0, sizeof(uint32_t) * N * N, s));
     BBA_CUDA(h, cudaMemsetAsync(e.d_r, 0, sizeof(long long) * N, s));
-    for (uint32_t begin = 0; begin < n; begin += chunk) {
-      g.begin = begin;
-      g.end = begin + std::min(chunk, n - begin);
-      const uint32_t len = g.end - g.begin;
-      w.words = (len + 31u) / 32u;
-      // the test sums of rounds 2 .. k: stats_j = the members of round j - 1 with y - x_{j-1}, in d_test[j % 2]
-      for (int j = 2; j <= k; ++j) {
-        ExposureWalkArgs a = w;
-        if (j >= 3) {
-          a.test_n = e.d_test_n[(j - 1) % 2];
-          a.test_sum = e.d_test_sum[(j - 1) % 2];
-          a.test_x = xq(j - 2);
-        }
-        a.n = e.d_test_n[j % 2];
-        a.sum = e.d_test_sum[j % 2];
-        a.sub_x = xq(j - 1);
-        BBA_CUDA(h, cudaMemsetAsync(a.n, 0, sizeof(uint32_t) * len, s));
-        BBA_CUDA(h, cudaMemsetAsync(a.sum, 0, sizeof(long long) * len, s));
-        BBA_LAUNCH(h, h->launches, LaunchExposureWalk, a, h->sm_count, s);
-      }
-      // the members of round k: their n and sum of y with the bit rows, then r
-      ExposureWalkArgs a = w;
-      if (k >= 2) {
-        a.test_n = e.d_test_n[k % 2];
-        a.test_sum = e.d_test_sum[k % 2];
-        a.test_x = xq(k - 1);
-      }
-      a.n = e.d_n;
-      a.sum = e.d_sum;
-      a.bits = h->covis.d_bits;
-      BBA_CUDA(h, cudaMemsetAsync(a.n, 0, sizeof(uint32_t) * len, s));
-      BBA_CUDA(h, cudaMemsetAsync(a.sum, 0, sizeof(long long) * len, s));
-      BBA_CUDA(h, cudaMemsetAsync(a.bits, 0, sizeof(uint32_t) * N * w.words, s));
-      BBA_LAUNCH(h, h->launches, LaunchExposureWalk, a, h->sm_count, s);
-      a.bits = nullptr;
-      a.rhs = e.d_r;
-      BBA_LAUNCH(h, h->launches, LaunchExposureWalk, a, h->sm_count, s);
-      const CovisibilityGramArgs q{h->covis.d_bits, w.words, h->geo.d_all_list, count, count, e.d_C};
-      BBA_LAUNCH(h, h->launches, LaunchCovisibilityGram, q, h->sm_count, s);
-    }
+    // (the walk zeroes the bit rows at the start of a chunk; only the members' walk writes them)
+    if (bba_status st2 = WalkReplica(h, walk, h->d_kfs, e.d_ids, count, s, [&](const GeometryArgs& g, uint32_t words) {
+          const uint32_t len = g.end - g.begin;
+          w.geo = g;
+          w.words = words;
+          // the test sums of rounds 2 .. k: stats_j = the members of round j - 1 with y - x_{j-1}, in d_test[j % 2]
+          for (int j = 2; j <= k; ++j) {
+            ExposureWalkArgs a = w;
+            if (j >= 3) {
+              a.test_n = e.d_test_n[(j - 1) % 2];
+              a.test_sum = e.d_test_sum[(j - 1) % 2];
+              a.test_x = xq(j - 2);
+            }
+            a.n = e.d_test_n[j % 2];
+            a.sum = e.d_test_sum[j % 2];
+            a.sub_x = xq(j - 1);
+            BBA_CUDA(h, cudaMemsetAsync(a.n, 0, sizeof(uint32_t) * len, s));
+            BBA_CUDA(h, cudaMemsetAsync(a.sum, 0, sizeof(long long) * len, s));
+            BBA_LAUNCH(h, h->launches, LaunchExposureWalk, a, h->sm_count, s);
+          }
+          // the members of round k: their n and sum of y with the bit rows, then r
+          ExposureWalkArgs a = w;
+          if (k >= 2) {
+            a.test_n = e.d_test_n[k % 2];
+            a.test_sum = e.d_test_sum[k % 2];
+            a.test_x = xq(k - 1);
+          }
+          a.n = e.d_n;
+          a.sum = e.d_sum;
+          a.bits = h->covis.d_bits;
+          BBA_CUDA(h, cudaMemsetAsync(a.n, 0, sizeof(uint32_t) * len, s));
+          BBA_CUDA(h, cudaMemsetAsync(a.sum, 0, sizeof(long long) * len, s));
+          BBA_LAUNCH(h, h->launches, LaunchExposureWalk, a, h->sm_count, s);
+          a.bits = nullptr;
+          a.rhs = e.d_r;
+          BBA_LAUNCH(h, h->launches, LaunchExposureWalk, a, h->sm_count, s);
+          const CovisibilityGramArgs q{h->covis.d_bits, words, h->geo.d_all_list, count, count, e.d_C};
+          BBA_LAUNCH(h, h->launches, LaunchCovisibilityGram, q, h->sm_count, s);
+          return BBA_OK;
+        }))
+      return st2;
     sa.xq = xq(k);
     BBA_LAUNCH(h, h->launches, LaunchExposureSolve, sa, s);
     if (k == 1) BBA_CUDA(h, cudaMemcpyAsync(e.d_diag, e.d_diag.get() + N, sizeof(uint32_t) * N, cudaMemcpyDeviceToDevice, s));

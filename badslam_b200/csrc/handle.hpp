@@ -3,9 +3,10 @@
 //
 // Host units: badba.cu (handle, setters / getters, keyframes, textures, bba_host_*), pose_step.cu (spatial order, pose step),
 // pose_terms.cu (soft pose priors and constraints, their losses and staging, pose graph), bundle_adjust.cu (BA schemes,
-// intrinsics, PCG, surfel lifecycle), multi_gpu.cu (sharding, exchange, peer replicas), frames.cu (odometry, preprocessing).  None
-// of them contains a kernel.  loop_verification.cu (bba_verify_loop_closures) holds its host orchestration and its one kernel, and
-// place_index.cu (the fern place index) its entry points and its two kernels.
+// intrinsics, PCG, surfel lifecycle), covisibility.cu (the whole-replica walk, co-visibility and frame overlap), multi_gpu.cu
+// (sharding, exchange, peer replicas), frames.cu (odometry, preprocessing).  None of them contains a kernel.
+// loop_verification.cu (bba_verify_loop_closures) holds its host orchestration and its one kernel, and place_index.cu (the fern
+// place index) its entry points and its two kernels.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -15,6 +16,7 @@
 #include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -345,10 +347,10 @@ struct bba_context {
     bba::PinnedBuffer<unsigned int> h_counts;
   } deform;
 
-  // keyframe co-visibility (bba_measure_keyframe_covisibility): the bit rows of one chunk of the stream, the listed rows' ids and
-  // the counts, allocated by the first call
+  // keyframe co-visibility (bba_measure_keyframe_covisibility, covisibility.cu): the bit rows of one chunk of the stream (those of
+  // every whole-replica walk, WalkReplica), the listed rows' ids and the counts, allocated by the first call
   struct Covisibility {
-    bba::DeviceBuffer<uint32_t> d_bits;     // [K][words of a chunk]
+    bba::DeviceBuffer<uint32_t> d_bits;     // [rows][words of a chunk]
     bba::DeviceBuffer<int> d_rows;
     bba::DeviceBuffer<uint32_t> d_counts;   // [rows][K]
     uint32_t chunk = 0;   // surfels per chunk (bba_debug_set_covisibility_chunk); 0: the budget rule
@@ -371,9 +373,9 @@ struct bba_context {
     int count = 0;                        // of the last estimate, 0 before the first
   } exposure;
 
-  // frame overlap (bba_measure_frame_overlap): the query frames' records, the Gram's row list, the frames' co-visible keyframes
-  // (CSR), their cell bit rows and the counts ([n][3] seed counts, then the Gram); the bit rows live in covis.d_bits.  Grown on
-  // demand by the calls; the host side is staging for one call, which synchronises before it returns.
+  // frame overlap (bba_measure_frame_overlap, covisibility.cu): the query frames' records, the Gram's row list, the frames'
+  // co-visible keyframes (CSR), their cell bit rows and the counts ([n][3] seed counts, then the Gram); the bit rows live in
+  // covis.d_bits.  Grown on demand by the calls; the host side is staging for one call, which synchronises before it returns.
   struct FrameOverlap {
     bba::DeviceBuffer<bba::KfDevice> d_frames;
     bba::PinnedBuffer<bba::KfDevice> h_frames;
@@ -725,8 +727,32 @@ bba_status TrackPairsOnSnapshot(bba_handle h, const bba_odometry_options& o, Fro
 bba_status ReserveTileEpochs(bba_handle h);
 // geo.d_all_list, the keyframe list 0 .. max_keyframes - 1, made on first use.
 bba_status MakeAllKeyframeList(bba_handle h);
+// The fields of a geometry launch but for its shard and peers: the surfels, in the spatial order with `sort` (the caller has
+// made it current) or else the caller's, the stream, the flags, the records kfs through list[0 .. count), the work-item counter and
+// the tile epochs (reserved here), tile_shift 8.
+bba_status SetGeometryFields(bba_handle h, bool sort, const KfDevice* kfs, const int* list, int count, GeometryArgs* g);
+// The minimum observation count of a new surfel on a handle with K keyframes.
+int MinObservationCount(bba_handle h, size_t K);
+// The surfel-creation filter's record of keyframe `other` for a keyframe or frame at global_T_frame: covis_T_frame and other's
+// depth and normals.
+CovisEntry MakeCovisEntry(const Keyframe& other, const Pose& global_T_frame);
+
+// covisibility.cu
 // The bit rows of one chunk of the stream take K x chunk / 32 words: chunks of at most this many bytes of them (DESIGN §3.19).
 constexpr uint64_t kCovisibilityBitsBudget = 128ull << 20;
+// A walk over the whole surfel replica with `rows` bit rows in covis.d_bits, `chunk` surfels at a time: the forced covis.chunk, or
+// whole 256-surfel geometry tiles whose bit rows fit kCovisibilityBitsBudget; at least 1, at most surfels_size when there are any.
+struct ReplicaWalk {
+  size_t rows;
+  uint32_t chunk;
+};
+// Chooses the chunk of a walk with rows >= 1 bit rows, reserves covis.d_bits for them and makes geo.d_all_list.
+bba_status ReserveReplicaWalk(bba_handle h, size_t rows, ReplicaWalk* w);
+// Walks every surfel of the replica (one shard, no peers) over the records kfs through list[0 .. count): brings the spatial order
+// up to date unless peer stores keep the caller's order, then per chunk zeroes its `rows` bit rows of `words` words each and calls
+// launch with the chunk's geometry arguments (begin, end).  Nothing happens without surfels.
+bba_status WalkReplica(bba_handle h, const ReplicaWalk& w, const KfDevice* kfs, const int* list, int count, cudaStream_t s,
+                       const std::function<bba_status(const GeometryArgs& g, uint32_t words)>& launch);
 
 // multi_gpu.cu
 void ShardSurfels(uint32_t n, int rank, int world, uint32_t* local_cap, uint32_t* shard_len);

@@ -1400,49 +1400,33 @@ static LaunchResult PrepareGeo(Kernel kernel, GeometryArgs* a, int sm_count, boo
   return r;
 }
 
-template <typename Kernel>
-static LaunchResult LaunchGeo(Kernel kernel, GeometryArgs a, int sm_count, bool desc_rows, cudaStream_t stream) {
+static GeometryArgs& Geo(GeometryArgs& a) { return a; }
+template <typename Args> static GeometryArgs& Geo(Args& a) { return a.geo; }
+
+// PrepareGeo, then the kernel on its argument struct a (a GeometryArgs, or a struct with one in .geo).
+template <typename Kernel, typename Args>
+static LaunchResult LaunchGeo(Kernel kernel, Args a, int sm_count, bool desc_rows, cudaStream_t stream) {
   uint32_t grid;
-  const LaunchResult r = PrepareGeo(kernel, &a, sm_count, desc_rows, stream, &grid);
+  const LaunchResult r = PrepareGeo(kernel, &Geo(a), sm_count, desc_rows, stream, &grid);
   kernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
   return r;
 }
 
-LaunchResult LaunchDeformSurfels(const DeformArgs& args, int sm_count, cudaStream_t stream) {
-  if (args.geo.end <= args.geo.begin || args.geo.kf_count <= 0) return {};
-  DeformArgs a = args;
-  uint32_t grid;
-  const LaunchResult r = PrepareGeo(DeformSurfelsKernel, &a.geo, sm_count, false, stream, &grid);
-  DeformSurfelsKernel<<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
-  return r;
+LaunchResult LaunchDeformSurfels(const DeformArgs& a, int sm_count, cudaStream_t stream) {
+  if (a.geo.end <= a.geo.begin || a.geo.kf_count <= 0) return {};
+  return LaunchGeo(DeformSurfelsKernel, a, sm_count, false, stream);
 }
 
-LaunchResult LaunchCovisibilityBits(const CovisibilityBitsArgs& args, int sm_count, cudaStream_t stream) {
-  if (args.geo.end <= args.geo.begin || args.geo.kf_count <= 0) return {};
-  CovisibilityBitsArgs a = args;
-  uint32_t grid;
-  if (a.cells) {
-    const LaunchResult r = PrepareGeo(CovisibilityBitsKernel<true>, &a.geo, sm_count, false, stream, &grid);
-    CovisibilityBitsKernel<true><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
-    return r;
-  }
-  const LaunchResult r = PrepareGeo(CovisibilityBitsKernel<false>, &a.geo, sm_count, false, stream, &grid);
-  CovisibilityBitsKernel<false><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
-  return r;
+LaunchResult LaunchCovisibilityBits(const CovisibilityBitsArgs& a, int sm_count, cudaStream_t stream) {
+  if (a.geo.end <= a.geo.begin || a.geo.kf_count <= 0) return {};
+  if (a.cells) return LaunchGeo(CovisibilityBitsKernel<true>, a, sm_count, false, stream);
+  return LaunchGeo(CovisibilityBitsKernel<false>, a, sm_count, false, stream);
 }
 
-LaunchResult LaunchExposureWalk(const ExposureWalkArgs& args, int sm_count, cudaStream_t stream) {
-  if (args.geo.end <= args.geo.begin || args.geo.kf_count <= 0) return {};
-  ExposureWalkArgs a = args;
-  uint32_t grid;
-  if (a.rhs) {
-    const LaunchResult r = PrepareGeo(ExposureWalkKernel<true>, &a.geo, sm_count, false, stream, &grid);
-    ExposureWalkKernel<true><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
-    return r;
-  }
-  const LaunchResult r = PrepareGeo(ExposureWalkKernel<false>, &a.geo, sm_count, false, stream, &grid);
-  ExposureWalkKernel<false><<<grid, kGeoThreads, kGeoSmemBytes, stream>>>(a);
-  return r;
+LaunchResult LaunchExposureWalk(const ExposureWalkArgs& a, int sm_count, cudaStream_t stream) {
+  if (a.geo.end <= a.geo.begin || a.geo.kf_count <= 0) return {};
+  if (a.rhs) return LaunchGeo(ExposureWalkKernel<true>, a, sm_count, false, stream);
+  return LaunchGeo(ExposureWalkKernel<false>, a, sm_count, false, stream);
 }
 
 // grid.z splits the words so that the grid holds about four CTAs per SM (one slice at least per CTA).

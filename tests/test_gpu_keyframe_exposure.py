@@ -5,7 +5,7 @@ bba_get_keyframe_exposures; DESIGN.md §3.21) against the numpy oracle (tests/ex
    exp(x) rounded to float32 (within 2 ulp); sum(r) = 0.  The kernels project with fast maths, so the surfels with a pair near a
    pixel or texel edge or an association threshold are deleted from these maps first (a few per cent of them);
 2. the same bits for repeated calls, caller and spatial order, permuted surfels, forced chunks, the deterministic mode, and two and
-   three ranks on one device;
+   three ranks on one device; the launch counts;
 3. keyframe colours scaled by seeded gains in [0.7, 1.4] give estimates within 2 % of the true ratios to the gauge keyframe;
 4. setting every gain to 1 leaves a deterministic BA bit-identical to a handle that never made the call;
 5. estimate -> set -> BA on gain-perturbed colours ends closer to the truth, with a lower descriptor cost, than BA without
@@ -177,6 +177,27 @@ def test_same_bits_everywhere():
     shuffled.surfels = np.array(sc.surfels, np.float32, copy=True)
     shuffled.surfels[:, :n] = sc.surfels[:, np.random.default_rng(9).permutation(n)]
     assert _result(_make(shuffled)) == want
+
+
+def test_launch_counts():
+    """With the spatial order current, C chunks and R rounds launch C R (R + 4) + R kernels: per chunk and round k, k + 1 walks (a
+    stream gather and the walk each) and the Gram; per round one solve.  An empty map launches the solves alone."""
+    sc = _scene("small")
+    ba = _make(sc)
+    ba.EstimateKeyframeExposures()   # (may build the spatial order)
+    for rounds, chunk in ((2, 0), (1, 0), (3, 0), (2, 4096)):
+        ba.DebugSetCovisibilityChunk(chunk)
+        chunks = -(-sc.num_surfels // chunk) if chunk else 1
+        n = ba.kernel_launch_count()
+        ba.EstimateKeyframeExposures(outer_iterations=rounds)
+        assert ba.kernel_launch_count() - n == chunks * rounds * (rounds + 4) + rounds, (rounds, chunk)
+    empty = copy.copy(_scene("tiny"))
+    empty.num_surfels = 0
+    ba = _make(empty)
+    n = ba.kernel_launch_count()
+    gains, obs, _ = ba.EstimateKeyframeExposures()
+    assert ba.kernel_launch_count() - n == 2
+    assert gains[0] == 1.0 and np.isnan(gains[1:]).all() and not obs.any()
 
 
 @pytest.mark.parametrize("world", [2, 3])
